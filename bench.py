@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (one JSON line on rank 0)
     python bench.py --impl reference ...                     # the reference's CPU implementation on the host cores
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as DIR/<name>.npy
 
 A step = one pass of the hot path over one synthetic batch: rho = X.V (projection) followed by the workload's EM
 iterations (epsilon = -inf: the reference then never breaks, VBx/VBx.py:122).  `value` is measured with X / gamma0
@@ -51,6 +52,9 @@ WORKLOADS = {
     'tinystrong': dict(B=12, T=(300, 5000), S=6, iters=6, Fa=0.3, Fb=17.0, loopP=0.99, strong=True),
 }
 D_RAW, R_DIM = 256, 128
+L2_BYTES = 50e6             # H100 L2: inputs below twice this size are flushed from L2 between steps
+DUMP_ROWS = 32768           # --dump-outputs: per-frame arrays keep this many seeded rows (rho: 16 MB)
+DUMP_LIMIT = 64 << 20
 
 
 def workload_lengths(w, seed):
@@ -117,12 +121,12 @@ def make_device_shard(all_lengths, indices, S, seed, device):
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks sampling during the timed region (B200_PROFILING.md "clocks line")
+# clocks sampling during the timed region
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
-         'clocks_event_reasons.sw_power_cap')
+         'clocks_event_reasons.sw_power_cap,power.limit')
 
     def __init__(self, index):
         self.index, self.proc, self.lines = index, None, []
@@ -146,7 +150,7 @@ class ClockSampler:
             return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': ['nvidia-smi unavailable']}
         time.sleep(0.15)
         self.proc.terminate()
-        sm, smax, reasons = [], None, set()
+        sm, smax, reasons, power, plimit = [], None, set(), [], None
         for ts, line in self.lines:
             f = [x.strip() for x in line.split(',')]
             if len(f) < 9:
@@ -158,6 +162,11 @@ class ClockSampler:
             smax = mx
             if t0 - 0.05 <= ts <= t1 + 0.05:
                 sm.append(clk)
+                try:
+                    power.append(float(f[3]))
+                    plimit = float(f[9])
+                except (ValueError, IndexError):
+                    pass
                 for name, val in zip(('hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap'), f[5:9]):
                     if val.lower().startswith('active'):
                         reasons.add(name)
@@ -173,7 +182,8 @@ class ClockSampler:
                         reasons.add(name)
             except Exception:
                 sm = [float('nan')]
-        return {'sm_mhz': float(np.median(sm)), 'sm_max_mhz': smax, 'reasons': sorted(reasons), 'samples': len(sm)}
+        return {'sm_mhz': float(np.median(sm)), 'sm_max_mhz': smax, 'reasons': sorted(reasons), 'samples': len(sm),
+                'power_w': float(np.median(power)) if power else None, 'power_limit_w': plimit}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -329,6 +339,35 @@ def es2005a_call():
     return z, z['fea'], z['Phi'], q, kw
 
 
+def frame_rows(N):
+    """The fixed, seeded sample of frame rows --dump-outputs keeps of per-frame arrays (all of them when N is small)."""
+    if N <= DUMP_ROWS:
+        return None
+    return np.sort(np.random.default_rng(0).choice(N, size=DUMP_ROWS, replace=False))
+
+
+def collect_outputs(N, per_frame, per_recording):
+    """Host copies of what the timed path returned in its last step: per-frame arrays [N, ...] reduced to frame_rows(N),
+    per-recording arrays whole; integers as float64."""
+    import torch
+    rows = frame_rows(N)
+    idx = None if rows is None else torch.from_numpy(rows)
+    out = {} if rows is None else {'frame_rows': rows.astype(np.float64)}
+    for name, t in per_frame.items():
+        out[name] = (t if idx is None else t[idx.to(t.device)]).cpu().numpy()
+    for name, t in per_recording.items():
+        out[name] = t.cpu().numpy()
+    return {k: v if v.dtype in (np.float32, np.float64) else v.astype(np.float64) for k, v in out.items()}
+
+
+def dump_outputs(path, arrays):
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_LIMIT, f'--dump-outputs: {total} bytes over the {DUMP_LIMIT} byte limit'
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + '.npy'), np.ascontiguousarray(a))
+
+
 def dist_env():
     return int(os.environ.get('RANK', 0)), int(os.environ.get('LOCAL_RANK', 0)), int(os.environ.get('WORLD_SIZE', 1))
 
@@ -342,7 +381,7 @@ def workload_config(w, wname, n_gpus):
            'frames_per_recording': list(T) if isinstance(T, tuple) else T, 'D': D_RAW,
            'R': R_DIM, 'S': w['S'], 'em_iterations': w['iters'], 'Fa': w['Fa'], 'Fb': w['Fb'], 'loopProb': w['loopP'],
            'parallelism': f'recordings sharded over {n_gpus} GPU(s), one NCCL all-reduce of the ELBO trace',
-           'l2': 'inputs larger than L2 (rho alone exceeds 126 MB)' if w['B'] * (np.mean(T) if isinstance(T, tuple) else T) * R_DIM * 4 / (n_gpus if w.get('strong') else 1) > 2 * 126e6
+           'l2': 'inputs larger than L2 (rho alone exceeds 100 MB)' if w['B'] * (np.mean(T) if isinstance(T, tuple) else T) * R_DIM * 4 / (n_gpus if w.get('strong') else 1) > 2 * L2_BYTES
                  else 'L2 flushed between steps (256 MB scratch write)'}
     if w.get('dropin'):
         cfg['workload'] = (f'{wname}: ES2005a (T=1025 x-vectors, R=128, S=31 AHC clusters), the reference call VBx/vbhmm.py:154-158 '
@@ -421,7 +460,7 @@ def run_c1(args, w, wname):
         for _ in range(max(args.warmup, 3)):
             call()
         ts = []
-        for _ in range(max(args.steps, 10)):
+        for _ in range(args.steps):
             t0 = time.perf_counter()
             g, p, L = call()
             ts.append(time.perf_counter() - t0)
@@ -451,7 +490,7 @@ def run_c1(args, w, wname):
 
     evs = []
     l0 = None
-    for i in range(3 + max(args.steps, 10)):        # production configuration: no per-kernel events, the run replayed as a CUDA graph
+    for i in range(3 + args.steps):                 # production configuration: no per-kernel events, the run replayed as a CUDA graph
         if i == 3:
             torch.cuda.synchronize()
             l0 = vb.launches
@@ -462,6 +501,9 @@ def run_c1(args, w, wname):
         if i >= 3:
             evs.append((e0, e1))
     torch.cuda.synchronize()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, collect_outputs(T, {'gamma': g_d[:, :S], 'rho': rho_d}, {
+            'pi': p_d[:, :S], 'Li': out['Li'], 'n_iters': out['n_iters']}))
     res_ms = float(np.median([a.elapsed_time(b) for a, b in evs]))
     n_steps = len(evs)
     launches = (vb.launches - l0) / n_steps
@@ -513,7 +555,7 @@ def load_peaks():
             return float(peaks['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
     except Exception:
         pass
-    return 6650.0, 'fallback 6.65 TB/s (B200_PROFILING.md)'
+    return 3350.0, 'fallback 3.35 TB/s (H100 SXM data sheet)'
 
 
 # ------------------------------------------------------------------------------------------------
@@ -535,9 +577,14 @@ def main():
     ap.add_argument('--fb-split', type=int, default=0, help='0 = auto, 1 = always, 2 = never: forward / backward sweeps on separate warps')
     ap.add_argument('--front', default='project', choices=['project', 'xvectors'],
                     help="what feeds the EM loop: 'project' = rho = X.V (the headline definition, SURVEY 8d); 'xvectors' = the "
-                         "real-data chain vbx_prepare_xvectors (x-vector transform + PLDA projection, two tcgen05 passes)")
+                         "real-data chain vbx_prepare_xvectors (x-vector transform + PLDA projection, two wgmma passes)")
     ap.add_argument('--extra', default='', help='comma separated extra workloads to time (kernel-only) in the same run')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps write what the last one computed (gamma, pi, Li, n_iters, rho; per-frame '
+                         'arrays as a fixed seeded sample of rows) as DIR/<name>.npy, to compare two builds output for output')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     args.warmup = max(args.warmup, 3) if args.impl == 'b200' else args.warmup
     w, wname = WORKLOADS[args.workload], args.workload
     if args.impl == 'reference':
@@ -568,7 +615,7 @@ def main():
         if os.environ.get('VBX_BENCH_DEBUG'):
             print(f'[rank {rank}] {msg}', file=sys.stderr, flush=True)
 
-    def time_workload(w, wname, steps, warmup, with_clocks):
+    def time_workload(w, wname, steps, warmup, with_clocks, dump=False):
         strong = bool(w.get('strong'))
         if strong:          # one fixed job, LPT-partitioned over the ranks (vbx_b200/shard.py)
             all_lengths = workload_lengths(w, seed=1000)
@@ -606,7 +653,7 @@ def main():
         pi0[:w['S']] = 1.0 / w['S']
         trace = torch.zeros(2 * w['iters'], dtype=torch.float64, device=device)
         flush = None
-        if N * R_DIM * 4 <= 2 * 126e6:
+        if N * R_DIM * 4 <= 2 * L2_BYTES:
             flush = torch.empty(256 << 20, dtype=torch.uint8, device=device)
         vb.n_states = None if w['S'] == S else torch.full((len(lengths),), w['S'], dtype=torch.int32, device=device)
 
@@ -663,6 +710,10 @@ def main():
         torch.cuda.synchronize()
         barrier()
         t_wall1 = time.time()
+        dumped = None
+        if dump:
+            dumped = collect_outputs(N, {'gamma': gamma[:, :w['S']], 'rho': rho}, {
+                'pi': pi[:, :w['S']], 'Li': out['Li'], 'n_iters': out['n_iters']})
         clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
         per_step = [a.elapsed_time(b) for a, b in evs]
         if os.environ.get('VBX_BENCH_DEBUG'):
@@ -716,7 +767,7 @@ def main():
         return dict(ms=ms, N=N, N_total=N_total, timings=timings, launches=launches, clocks=clocks, lengths=lengths,
                     data=data, vb=vb, S=S, out=out, steps=steps, strong=strong, trace=tr, gamma=gamma, pi=pi,
                     in_library_collective=bool(in_library_collective), partitioned=partitioned, kernel_pass=kernel_pass,
-                    parts=len(vb.children) if partitioned else 1)
+                    parts=len(vb.children) if partitioned else 1, dumped=dumped)
 
     def parity_sample(res, w, n_rec=3):
         """Size-true check inside the bench: a few recordings of THIS batch against the float64 C oracle (the checker)."""
@@ -742,7 +793,9 @@ def main():
                 'ok': bool(worst['gamma'] <= 1e-4 and worst['pi'] <= 1e-4 and worst['elbo'] <= 1e-4),
                 'checker': 'oracle/vbx_oracle_c.c (float64) on the projected inputs of the sampled recordings, same iteration count'}
 
-    res = time_workload(w, wname, args.steps, args.warmup, with_clocks=True)
+    res = time_workload(w, wname, args.steps, args.warmup, with_clocks=True, dump=bool(args.dump_outputs) and rank == 0)
+    if res['dumped'] is not None:
+        dump_outputs(args.dump_outputs, res['dumped'])
     dbg(f'timed region done: {res["ms"]:.3f} ms/step')
     ms, N, N_total = res['ms'], res['N'], res['N_total']
     value = N_total / (ms / 1e3)

@@ -1,5 +1,5 @@
 /*
- * vbx_b200 -- C ABI of the B200-native VB-HMM EM loop (the hot path of BUTSpeechFIT/VBx).
+ * vbx_b200 -- C ABI of the H100-native VB-HMM EM loop (the hot path of BUTSpeechFIT/VBx).
  *
  * The reference has no FFI: its boundary for this path is the Python function
  *     VBx(X, Phi, loopProb, Fa, Fb, pi, gamma, maxIters, epsilon, alphaQInit, ref, plot,
@@ -39,7 +39,7 @@ enum vbx_status {
     VBX_ERR_ARG = -1,       /* bad argument (shape, null pointer, unsupported size)           */
     VBX_ERR_CUDA = -2,      /* a CUDA runtime call or kernel launch failed                    */
     VBX_ERR_STATE = -3,     /* call order violated (no plan / workspace not bound / too small) */
-    VBX_ERR_NO_DEVICE = -4  /* no usable sm_100 device                                        */
+    VBX_ERR_NO_DEVICE = -4  /* no usable sm_90 device                                         */
 };
 
 /* per-recording bits written to flags_out by vbx_run */
@@ -77,7 +77,7 @@ const char *vbx_last_error(vbx_handle_t h);
  * the bandwidth-bound kernels of ANOTHER handle working on the same device (vbx_b200/parts.py runs two halves of a batch).
  * Tuning knobs: "fb_states_per_lane" (0 = auto, 1, 2, 4), "fb_classic" (forward-backward sweep: 0 = one-step
  * look-ahead recurrences, 1 = normalise-every-frame), "projection" (0 = auto, 1 = FFMA tiles,
- * 2 = tcgen05 3xTF32), "gemm" (in-loop contractions: 0 = tensor cores in split-precision 3xTF32, 1 = FFMA),
+ * 2 = wgmma 3xTF32), "gemm" (in-loop contractions: 0 = tensor cores in split-precision 3xTF32, 1 = FFMA),
  * "timing" (0/1, see vbx_get_timings).  Unknown names return VBX_ERR_ARG. */
 int vbx_set_option(vbx_handle_t h, const char *name, int32_t value);
 
@@ -100,7 +100,7 @@ int vbx_prepare_project(vbx_handle_t h, const float *X, int32_t D, const float *
                         float *rho_out, void *stream);
 
 /* The real-data caller chain in front of VBx() (VBx/vbhmm.py:125-129 x-vector transform, :153 PLDA projection)
- * fused with the scale of VBx/VBx.py:88-89, as two tcgen05 passes (R must be 128, Dx a multiple of 32):
+ * fused with the scale of VBx/VBx.py:88-89, as two wgmma passes (R must be 128, Dx a multiple of 32):
  *   x_norm = l2norm(l2norm(x_raw - mean1) . lda - mean2)          x_raw [N,Dx], lda [Dx,128], x_norm [N,128]
  *   rho    = ((x_norm - plda_mu) . plda_tr^T) * sqrt(plda_psi)    plda_tr [128,128] and plda_psi [128] are the
  *            DIAGONALISED model (VBx/vbhmm.py:136-143; row n of plda_tr is output dimension n), Phi = plda_psi.

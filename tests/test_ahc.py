@@ -83,7 +83,7 @@ def test_device_ahc_matches_reference_goldens(gold):
 
 @pytest.mark.gpu
 def test_device_ahc_from_float32_xvectors(gold):
-    """float32 x-vectors (what the tcgen05 front end hands over): same flat clusters, threshold within 1e-6."""
+    """float32 x-vectors (what the tensor-core front end hands over): same flat clusters, threshold within 1e-6."""
     labels, thr, _ = _device_ahc([case_x(gold, n) for n in CASES], torch.float32)
     for b, name in enumerate(CASES):
         assert abs(thr[b] - float(gold[name + '/thr'])) <= 1e-6, name

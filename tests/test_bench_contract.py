@@ -1,5 +1,5 @@
-"""The bench line contract, checked on the committed final-build line (profiles/r2_bench_headline.json, written by
-`python bench.py` on a B200): every key the driver reads is there and the derived numbers are consistent with each
+"""The bench line contract, checked on the committed line of the current build (profiles/h100_bench_headline.json,
+written by `python bench.py` on an H100): every key the driver reads is there and the derived numbers are consistent with each
 other (value = frames / step time, roofline.frac = achieved / peak, achieved = algorithmic bytes / launch time).
 CPU only - it guards the format, the numbers themselves come from the GPU run."""
 import json
@@ -8,7 +8,7 @@ import os
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LINE = os.path.join(ROOT, 'profiles', 'r2_bench_headline.json')
+LINE = os.path.join(ROOT, 'profiles', 'h100_bench_headline.json')
 BASELINE = os.path.join(ROOT, 'BASELINE.json')
 
 
@@ -72,6 +72,8 @@ def test_e2e_cpu_baseline_and_clocks(line):
         assert k in b, k
     assert b['kind'] in ('reference', 'port') and b['cores'] >= 1 and b['value'] > 0
     k = line['clocks']
-    assert k['sm_mhz'] > 0.8 * k['sm_max_mhz']
+    # a clock below 0.8 of the maximum only counts when the card was held there by its own power limit
+    capped = 'sw_power_cap' in k['reasons'] and k['power_w'] >= 0.9 * k['power_limit_w']
+    assert k['sm_mhz'] > 0.8 * k['sm_max_mhz'] or capped
     assert not set(k['reasons']) & {'hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown'}
     assert line['parity']['ok'] is True

@@ -109,18 +109,6 @@ def test_transform_h5_rejects_other_files(tmp_path):
         formats.read_xvec_transform(str(path))
 
 
-def test_shipped_model_files_when_present():
-    ref_dir = '/root/reference/VBx/models/ResNet101_16kHz'
-    if not os.path.exists(ref_dir):
-        pytest.skip('reference model files only exist in the build container')
-    m = np.load(os.path.join(ROOT, 'tests', 'golden', 'es2005a_model.npz'))
-    mean1, mean2, lda = formats.read_xvec_transform(os.path.join(ref_dir, 'transform.h5'))
-    np.testing.assert_array_equal(mean1, m['mean1'])
-    np.testing.assert_array_equal(lda, m['lda'])
-    mu, tr, psi = formats.read_kaldi_plda(os.path.join(ref_dir, 'plda'))
-    np.testing.assert_array_equal(mu, m['plda_mu'])
-
-
 def test_text_plda_round_trip_and_ark_writer(tmp_path):
     """Text-format Kaldi PLDA (VBx/kaldi_utils.py:41-48) and the ark writer used to build CLI fixtures."""
     from vbx_b200 import formats

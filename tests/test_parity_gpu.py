@@ -483,7 +483,7 @@ def test_projection_matches_fp32_matmul():
 
 @pytest.mark.parametrize('n_rec,T', [(4, 119), (300, 1000)])
 def test_projection_tcgen05(n_rec, T):
-    """The tcgen05/TMEM 3xTF32 projection kernel against a float64 matmul (several tiles per persistent CTA)."""
+    """The tensor-core (wgmma) 3xTF32 projection kernel against a float64 matmul (several tiles per persistent CTA)."""
     from vbx_b200.batch import VbxBatch
     lens = [T] * n_rec
     rng = np.random.default_rng(7)
@@ -502,7 +502,7 @@ def test_projection_tcgen05(n_rec, T):
     rho2 = vb.prepare_project(cuda(X), cuda(V), cuda(synth.plda_phi(128)))
     torch.cuda.synchronize()
     err2 = np.abs(rho2.double().cpu().numpy() - want).max() / np.abs(want).max()
-    print("projection error: tcgen05 3xTF32 %.2e, FFMA %.2e" % (err, err2))
+    print("projection error: wgmma 3xTF32 %.2e, FFMA %.2e" % (err, err2))
     assert err <= 32 * err2 + 1e-7, (err, err2)       # split-precision tensor cores stay near FFMA-level accuracy
     vb.close()
 

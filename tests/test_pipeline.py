@@ -46,17 +46,14 @@ def test_soft_init_and_hard_labels_cpu(es):
 
 
 def test_xvector_transform_matches_reference_cpu(es):
-    """VBx/vbhmm.py:129 (float64, CPU tensors here; the same code runs on the device)."""
-    from vbx_b200 import formats
-    ref_dir = '/root/reference/VBx/models/ResNet101_16kHz'
-    if not os.path.exists(ref_dir):
-        pytest.skip('reference model files only exist in the build container')
-    mean1, mean2, lda = formats.read_xvec_transform(os.path.join(ref_dir, 'transform.h5'))
-    x = pipeline.xvector_transform(torch.from_numpy(es['x_raw'].astype(np.float64)), torch.from_numpy(mean1),
-                                   torch.from_numpy(mean2), torch.from_numpy(lda))
+    """VBx/vbhmm.py:129 (float64, CPU tensors here; the same code runs on the device), with the shipped model as stored in
+    tests/golden/es2005a_model.npz (x-vector transform and the diagonalised PLDA)."""
+    m = np.load(os.path.join(GOLD, 'es2005a_model.npz'))
+    assert str(m['sha_plda']) == str(es['sha_plda']) and str(m['sha_transform']) == str(es['sha_transform'])
+    x = pipeline.xvector_transform(torch.from_numpy(es['x_raw'].astype(np.float64)), torch.from_numpy(m['mean1']),
+                                   torch.from_numpy(m['mean2']), torch.from_numpy(m['lda']))
     np.testing.assert_allclose(x.numpy(), es['x_lda'], atol=1e-12)
-    mu, tr, psi = formats.read_kaldi_plda(os.path.join(ref_dir, 'plda'))
-    mu, tr, psi = pipeline.diagonalise_plda(mu, tr, psi)
+    mu, tr, psi = m['plda_mu'], m['plda_tr'], m['plda_psi']
     fea = pipeline.plda_project(x, torch.from_numpy(mu), torch.from_numpy(tr), 128)
     np.testing.assert_allclose(fea.numpy(), es['fea'], atol=1e-9)
     np.testing.assert_allclose(psi[:128], es['Phi'], rtol=1e-12)
@@ -64,7 +61,7 @@ def test_xvector_transform_matches_reference_cpu(es):
 
 @pytest.mark.gpu
 def test_es2005a_rttm_end_to_end_on_gpu(es):
-    """fea -> VB-HMM on the B200 -> labels -> merged segments == the reference's committed system output
+    """fea -> VB-HMM on the GPU -> labels -> merged segments == the reference's committed system output
     exp/ES2005a.rttm (50 segments, speaker ids up to renaming)."""
     from vbx_b200.batch import VbxBatch
     dev = torch.device('cuda:0')
@@ -91,7 +88,7 @@ def test_es2005a_rttm_end_to_end_on_gpu(es):
 
 @pytest.mark.gpu
 def test_es2005a_raw_xvectors_to_rttm_on_gpu(es):
-    """The whole real-data path on the device: raw x-vectors of exp/ES2005a.ark -> fused tcgen05 x-vector transform +
+    """The whole real-data path on the device: raw x-vectors of exp/ES2005a.ark -> fused wgmma x-vector transform +
     PLDA projection (vbx_prepare_xvectors, VBx/vbhmm.py:125-129,153) -> VB-HMM -> RTTM, against the features and
     the system output the reference produces (tests/golden/make_golden.py)."""
     from vbx_b200.batch import VbxBatch
@@ -132,7 +129,7 @@ def test_es2005a_raw_xvectors_to_rttm_on_gpu(es):
 @pytest.mark.parametrize('chain', ['tcgen05', 'float64'])
 def test_es2005a_everything_on_the_device(es, chain):
     """Raw x-vectors -> x-vector transform / PLDA projection -> AHC initialisation (vbx_ahc) -> VB-HMM -> labels, all
-    on the B200; only the linkage matrix and the labels come back.  Equals the reference's AHC labels, final labels
+    on the GPU; only the linkage matrix and the labels come back.  Equals the reference's AHC labels, final labels
     and RTTM segmentation."""
     m = np.load(os.path.join(GOLD, 'es2005a_model.npz'))
     dev = torch.device('cuda:0')

@@ -1,6 +1,6 @@
-"""Static evidence that the shipped library is the sm_100a code DESIGN.md describes: the SASS of libvbx_b200.so holds
-the Blackwell tensor-core / TMA / TMEM instructions of the projection kernels, the mma.sync contractions, and the
-order-pinned accesses of the forward-backward sweep (mnemonics: /opt/skills/guides/B200_PROFILING.md).  CPU-only."""
+"""Static evidence that the shipped library is the sm_90a code DESIGN.md describes: the SASS of libvbx_b200.so holds
+the Hopper warpgroup tensor-core (wgmma) / TMA / mbarrier instructions of the projection kernels, the mma.sync
+contractions, and the order-pinned accesses of the forward-backward sweep.  CPU-only."""
 import collections
 import re
 import shutil
@@ -31,7 +31,7 @@ def sass():
         if m and fn:
             per_fn[fn][m.group(1)] += 1
             per_fn[fn][m.group(1) + m.group(2)] += 1
-    assert 'sm_100a' in out.stdout or per_fn
+    assert 'sm_90a' in out.stdout or per_fn
     return per_fn
 
 
@@ -39,22 +39,22 @@ def functions(sass, needle):
     return {f: c for f, c in sass.items() if needle in f}
 
 
-def test_only_sm_100a_code_is_shipped():
+def test_only_sm_90a_code_is_shipped():
     tool = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
     try:
         out = subprocess.run([tool, '-lelf', _lib.LIB_PATH], capture_output=True, text=True, timeout=120).stdout
     except (FileNotFoundError, subprocess.TimeoutExpired):
         pytest.skip('cuobjdump not available')
     archs = set(re.findall(r'sm_\d+a?', out))
-    assert archs == {'sm_100a'}, archs
+    assert archs == {'sm_90a'}, archs
 
 
-def test_projection_runs_on_tcgen05_tmem_and_tma(sass):
-    proj = functions(sass, 'project_tcgen05_kernel')
+def test_projection_runs_on_wgmma_and_tma(sass):
+    proj = functions(sass, 'project_wgmma_kernel')
     assert len(proj) == 3                                   # plain projection + the two passes of the x-vector front end
     for f, c in proj.items():
-        assert c['UTCHMMA'] >= 24, (f, c['UTCHMMA'])        # tcgen05.mma kind::tf32, 2 M-tiles x 4 k-steps x 3 split terms
-        assert c['LDTM'] >= 1, f                            # tcgen05.ld: accumulators come out of TMEM
+        assert c['HGMMA'] >= 12, (f, c['HGMMA'])            # wgmma m64n128k8 tf32, 4 k-steps x 3 split terms per block
+        assert c['WARPGROUP'] >= 1, f                       # wgmma.fence / wait_group: accumulators stay in registers
         assert c['UBLKCP'] >= 1, f                          # cp.async.bulk of the pre-swizzled V images
         assert c['SYNCS'] >= 4, f                           # mbarrier pipeline
 
@@ -91,12 +91,14 @@ def test_split_sweeps_and_float64_finish(sass):
 
 
 def test_front_end_uses_the_three_way_split(sass):
-    """The two passes of the real-data front end issue six tcgen05.mma per k-step (x3 v1, x1 v3, x2 v2, x2 v1, x1 v2, x1 v1)
-    on one 128-row M-tile; the headline projection three on two M-tiles: 24 per 32-column block either way."""
-    proj = functions(sass, 'project_tcgen05_kernel')
+    """The two passes of the real-data front end issue six wgmma per k-step (x3 v1, x1 v3, x2 v2, x2 v1, x1 v2, x1 v1),
+    the headline projection three (lo hi, hi lo, hi hi)."""
+    proj = functions(sass, 'project_wgmma_kernel')
     three = [f for f in proj if 'ILi1ELi3E' in f or 'ILi2ELi3E' in f]
     two = [f for f in proj if 'ILi0ELi2E' in f]
     assert len(three) == 2 and len(two) == 1, list(proj)
+    for f in three:
+        assert proj[f]['HGMMA'] >= 24, (f, proj[f]['HGMMA'])
 
 
 def test_float64_ahc_kernels(sass):

@@ -1,10 +1,9 @@
-"""Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): tcgen05 projection and
+"""Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection and
 x-vector chain, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
 6..64, per-recording state masks, AHC, hard labels, the dense forward_backward() and the ELBO trace.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
-
-Logs of the last run on a B200 are committed under profiles/ (r2_sanitizer_*.txt)."""
+"""
 import os
 import sys
 

@@ -1,4 +1,4 @@
-"""vbx_b200: the VB-HMM EM loop of BUTSpeechFIT/VBx (VBx/VBx.py) as hand-written sm_100a CUDA kernels
+"""vbx_b200: the VB-HMM EM loop of BUTSpeechFIT/VBx (VBx/VBx.py) as hand-written sm_90a CUDA kernels
 behind a C ABI (include/vbx_b200.h), with a drop-in `VBx()` (+ `forward_backward`, `DER`), a batched `VbxBatch` /
 `make_batch`, whole-archive `diarize_batch` and the command line `python -m vbx_b200.cli`."""
 from ._lib import VbxError, LIB_PATH  # noqa: F401

@@ -1,6 +1,6 @@
 """ctypes binding of libvbx_b200.so (the C ABI declared in include/vbx_b200.h).
 
-There is deliberately NO fallback: if the CUDA library is missing or no sm_100 device is visible,
+There is deliberately NO fallback: if the CUDA library is missing or no sm_90 (H100) device is visible,
 every product entry point raises.  (The CPU oracle lives under oracle/ and is test infrastructure.)
 """
 import ctypes

@@ -1,4 +1,4 @@
-"""Drop-in replacement for the reference's `VBx()` (VBx/VBx.py:27-126) running on the B200.
+"""Drop-in replacement for the reference's `VBx()` (VBx/VBx.py:27-126) running on the H100.
 
 Same positional/keyword arguments, same `(gamma, pi, Li[, alpha, invL])` return with float64 numpy
 arrays, same exceptions for bad arguments; the work itself happens in the CUDA library.  The
@@ -65,7 +65,7 @@ def forward_backward(lls, tr, ip):
     lib = _lib.load()
     h = ctypes.c_void_p()
     if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
-        raise _lib.VbxError('vbx_create failed: no usable sm_100 device')
+        raise _lib.VbxError('vbx_create failed: no usable sm_90 device')
     try:
         d = lambda a: torch.from_numpy(a).to(dev)
         lls_d, tr_d, ip_d = d(lls), d(tr), d(ip)

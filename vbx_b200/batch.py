@@ -30,7 +30,7 @@ class VbxBatch:
         fb_split: 0 = auto, 1 = always, 2 = never run the forward / backward sweeps concurrently (include/vbx_b200.h).
         f64_only: plan for run_f64() only (vbx_plan_f64): any R and any number of states, no padding."""
         if not torch.cuda.is_available():
-            raise VbxError('vbx_b200 needs a CUDA device (B200, sm_100); there is no CPU path')
+            raise VbxError('vbx_b200 needs a CUDA device (H100, sm_90); there is no CPU path')
         self.lib = _lib.load()
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         if self.device.index is None:       # a bare 'cuda' means the CURRENT device, not device 0
@@ -57,7 +57,7 @@ class VbxBatch:
         self._h = ctypes.c_void_p()
         rc = self.lib.vbx_create(self.device.index, ctypes.byref(self._h))
         if rc != 0:
-            raise VbxError(f'vbx_create failed ({rc}): no usable sm_100 device')
+            raise VbxError(f'vbx_create failed ({rc}): no usable sm_90 device')
         self.exact_stop = bool(exact_stop)
         self._check(self.lib.vbx_set_option(self._h, b'exact_stop', int(self.exact_stop)))
         self._check(self.lib.vbx_set_option(self._h, b'fb_split', int(fb_split)))

@@ -1,4 +1,4 @@
-"""Builds libvbx_b200.so (hand-written sm_100a kernels + C ABI) in-tree with nvcc."""
+"""Builds libvbx_b200.so (hand-written sm_90a kernels + C ABI) in-tree with nvcc."""
 import os
 import subprocess
 
@@ -7,8 +7,8 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libvbx_b200.so')
 SOURCES = ['vbx_kernels.cu', 'vbx_mma_kernels.cu', 'vbx_long_kernels.cu', 'vbx_fb_split.cu', 'vbx_project_tc.cu', 'vbx_f64.cu', 'vbx_exact64.cu', 'vbx_fb_dense.cu', 'vbx_ahc.cu',
            'vbx_capi.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
-              '-Xcompiler', '-fPIC', '-Xptxas', '-v']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+NVCC_FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC', '-Xptxas', '-v']
 
 
 def _nvcc():
@@ -29,7 +29,7 @@ def needs_build():
 
 
 def build_library(force=False, verbose=False):
-    """Compile every .cu for sm_100a and link the shared library.  Returns the .so path."""
+    """Compile every .cu for sm_90a and link the shared library.  Returns the .so path."""
     if not force and not needs_build():
         return LIB
     nvcc = _nvcc()
@@ -43,7 +43,7 @@ def build_library(force=False, verbose=False):
         if r.returncode != 0:
             raise RuntimeError('nvcc failed for %s:\n%s\n%s' % (src, r.stdout, r.stderr))
         objs.append(obj)
-    cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-lcuda', '-ldl']
+    cmd = [nvcc, '-shared', '-o', LIB] + objs + ARCH + ['-lcuda', '-ldl']
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n%s\n%s' % (r.stdout, r.stderr))

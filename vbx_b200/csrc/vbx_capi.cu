@@ -14,6 +14,7 @@
 
 struct vbx_handle_s {
     int device = 0;
+    int sms = 0;                 // multiprocessors of the device
     std::string err;
     vbx::Plan plan;
     vbx::Workspace ws;
@@ -26,9 +27,9 @@ struct vbx_handle_s {
     int opt_projection = 0;
     int opt_timing = 0;
     int opt_gemm = 0;  // 0 = mma.sync 3xTF32, 1 = FFMA
-    int opt_fold_speaker = 0;    // 1 = speaker model inside the tensor-core M-step kernel (last CTA of a recording).  Measured on
-                                 // the headline batch: M-step 0.414 -> 0.646 ms against 0.086 ms for the separate kernel (the
-                                 // 128-thread tails hold SM slots through S dependent L2 round trips), so it is off by default
+    int opt_fold_speaker = 0;    // 1 = speaker model inside the tensor-core M-step kernel (last CTA of a recording).  Off by
+                                 // default: the 128-thread tails hold SM slots through S dependent L2 round trips, which makes
+                                 // the folded M-step slower than the separate speaker-model kernel on the headline batch
     int opt_debug_sync = 0;      // 1 = synchronise after every launch group and name it on stderr (debugging aid)
     int opt_fb_split = 0;        // 0 = auto (few recordings: sweeps on separate warps), 1 = always, 2 = never
     int opt_exact_stop = 1;      // 1 = finish recordings in float64 once the ELBO step nears epsilon (vbx_exact64.cu)
@@ -186,7 +187,7 @@ size_t carve(const vbx::Plan &pl, void *base, vbx::Workspace *ws) {
 
 extern "C" {
 
-const char *vbx_version(void) { return "vbx_b200 0.1 (sm_100a)"; }
+const char *vbx_version(void) { return "vbx_b200 0.1 (sm_90a)"; }
 
 int32_t vbx_padded_states(int32_t n) {
     if (n < 1 || n > vbx::kMaxS) return -1;
@@ -203,9 +204,10 @@ int vbx_create(int32_t device, vbx_handle_t *out) {
         return VBX_ERR_NO_DEVICE;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return VBX_ERR_CUDA;
-    if (prop.major != 10) return VBX_ERR_NO_DEVICE;  // kernels are built for sm_100a only
+    if (prop.major != 9 || prop.minor != 0) return VBX_ERR_NO_DEVICE;  // kernels are built for sm_90a only
     vbx_handle_t h = new vbx_handle_s();
     h->device = device;
+    h->sms = prop.multiProcessorCount;
     {
         DeviceGuard guard(device);
         int lo = 0, hi = 0;
@@ -355,7 +357,7 @@ int vbx_plan(vbx_handle_t h, const int64_t *offsets_host, int32_t n_rec, int32_t
     if (h->opt_fb_split == 0) {
         const int spl = S >= 16 ? 2 : 1, rpw = 32 / (S / spl);
         const int warps = (n_rec + rpw - 1) / rpw;
-        split = warps <= 2 * 148;
+        split = warps <= 2 * h->sms;
     }
     // long recordings -> chunk lists of the chunked-scan forward-backward (not needed by the split sweeps)
     std::vector<int32_t> lrec_list, lrec_first(std::max(n_rec, 1), 0), lrec_nchunks(std::max(n_rec, 1), 0), lchunk_rec, lchunk_idx;
@@ -566,17 +568,17 @@ int vbx_prepare_project(vbx_handle_t h, const float *X, int32_t D, const float *
     cudaStream_t st = (cudaStream_t)stream;
     bool done = false, fused_g = false;
     Timed *tp = new Timed(h, st, VBX_K_PROJECT);
-    if (h->opt_projection != 1) {   // auto: tcgen05 when the shape allows it (R == 128, D % 32 == 0), else FFMA tiles
+    if (h->opt_projection != 1) {   // auto: wgmma when the shape allows it (R == 128, D % 32 == 0), else FFMA tiles
         std::string why;
-        // the tcgen05 epilogue also emits G_t per frame into the (not yet used) rowmax scratch array
-        int n = vbx::launch_project_tcgen05(h->plan, h->ws.tc_scratch, X, D, V, Phi, rho_out, h->ws.rowmax, st, &why);
+        // the wgmma epilogue also emits G_t per frame into the (not yet used) rowmax scratch array
+        int n = vbx::launch_project_wgmma(h->plan, h->ws.tc_scratch, X, D, V, Phi, rho_out, h->ws.rowmax, st, &why);
         if (n >= 0) {
             h->launches += n;
             done = true;
             fused_g = true;
         } else if (h->opt_projection == 2) {
             delete tp;
-            return fail(h, VBX_ERR_ARG, "vbx_prepare_project: tcgen05 path unavailable: " + why);
+            return fail(h, VBX_ERR_ARG, "vbx_prepare_project: wgmma path unavailable: " + why);
         }
     }
     if (!done) rc = counted(h, vbx::launch_project_ffma(h->plan, X, D, V, rho_out, st), "project_ffma");
@@ -610,8 +612,8 @@ int vbx_prepare_xvectors(vbx_handle_t h, const float *x_raw, int32_t Dx, const f
     {
         Timed t(h, st, VBX_K_PROJECT);
         std::string why;
-        int n = vbx::launch_xvector_chain_tcgen05(h->plan, h->ws.tc_scratch, x_raw, Dx, mean1, lda, mean2, plda_mu, plda_tr, plda_psi,
-                                                  x_norm_out, rho_out, h->ws.rowmax, st, &why);
+        int n = vbx::launch_xvector_chain_wgmma(h->plan, h->ws.tc_scratch, x_raw, Dx, mean1, lda, mean2, plda_mu, plda_tr, plda_psi,
+                                                x_norm_out, rho_out, h->ws.rowmax, st, &why);
         if (n < 0) return fail(h, VBX_ERR_CUDA, "vbx_prepare_xvectors: " + why);
         h->launches += n;
     }

@@ -16,7 +16,7 @@ constexpr int kLongT = 4096;   // recordings at least this long take the chunked
 constexpr int kChunk = 256;    // frames per chunk of that scan
 constexpr int kMaxR = 128;
 constexpr int kMaxS = 64;
-constexpr int kTcMaxD = 2048;  // largest raw dimension of the tcgen05 front end (bounds its scratch in the workspace)
+constexpr int kTcMaxD = 2048;  // largest raw dimension of the tensor-core front end (bounds its scratch in the workspace)
 
 // Device-resident description of a planned batch (arrays owned by the handle).
 struct Plan {
@@ -80,7 +80,7 @@ struct Workspace {
     // split forward-backward (vbx_fb_split.cu); null unless the plan chose it
     float *ahat = nullptr, *bhat = nullptr;   // [N,S] normalised forward variables / self-scaled backward variables
     float *socc = nullptr, *sent = nullptr;   // [n_mtiles,S] per-tile sums of gamma / of the re-entry terms of eq. (24)
-    float *tc_scratch = nullptr; // operand images of the tcgen05 front end (vbx_project_tc.cu); null unless R == 128
+    float *tc_scratch = nullptr; // operand images of the tensor-core front end (vbx_project_tc.cu); null unless R == 128
     // chunked scan of long recordings: per (chunk, basis) operators and per-chunk boundary vectors / partial sums
     float *fa_u = nullptr, *fa_lam = nullptr, *fa_exp = nullptr, *astart = nullptr;   // [LC,S,S], [LC,S] mantissa, [LC,S] exponent, [LC,S]
     float *bb_v = nullptr, *bb_mu = nullptr, *bb_exp = nullptr, *beta = nullptr;      // same shapes, backward sweep
@@ -220,13 +220,13 @@ int launch_fb_dense(const double *lls, const double *tr, const double *ip, int T
 size_t ahc_workspace_bytes(const int64_t *offsets_host, int n_rec, std::vector<int64_t> *d_off_host);
 int launch_ahc(const Plan &pl, const std::vector<int64_t> &d_off, const void *x, int x_is_f64, int dim, void *workspace,
                size_t workspace_bytes, double *Z_out, double *thr_out, cudaStream_t st, std::string *err);
-// tcgen05 projection (vbx_project_tc.cu)
+// wgmma projection (vbx_project_tc.cu)
 size_t tc_scratch_floats();
-int launch_project_tcgen05(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,
-                           float *gframe, cudaStream_t st, std::string *err);
-int launch_xvector_chain_tcgen05(const Plan &pl, float *tc_scratch, const float *x_raw, int Dx, const float *mean1, const float *lda,
-                                 const float *mean2, const float *plda_mu, const float *plda_tr, const float *psi,
-                                 float *x_norm, float *rho, float *gframe, cudaStream_t st, std::string *err);
+int launch_project_wgmma(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,
+                         float *gframe, cudaStream_t st, std::string *err);
+int launch_xvector_chain_wgmma(const Plan &pl, float *tc_scratch, const float *x_raw, int Dx, const float *mean1, const float *lda,
+                               const float *mean2, const float *plda_mu, const float *plda_tr, const float *psi,
+                               float *x_norm, float *rho, float *gframe, cudaStream_t st, std::string *err);
 int launch_gsum_from_frames(const Plan &pl, const Workspace &ws, const float *gframe, cudaStream_t st);
 
 }  // namespace vbx

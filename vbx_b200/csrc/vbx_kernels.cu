@@ -1,4 +1,4 @@
-// Hand-written sm_100a kernels of the VB-HMM EM loop (reference: VBx/VBx.py:74-126,146-175).
+// Hand-written sm_90a kernels of the VB-HMM EM loop (reference: VBx/VBx.py:74-126,146-175).
 //
 // Data layout (all float32, row-major, packed ragged over the batch):
 //   rho    [N,R]   x-vectors scaled into the PLDA space           VBx/VBx.py:89
@@ -103,7 +103,7 @@ __global__ void gsum_kernel(Plan pl, Workspace ws) {
     ws.gsum[rec] = s;
 }
 
-// per-recording sum of the per-frame constants written by the tcgen05 projection epilogue (float64, fixed order)
+// per-recording sum of the per-frame constants written by the wgmma projection epilogue (float64, fixed order)
 __global__ void __launch_bounds__(128) gsum_frames_kernel(Plan pl, Workspace ws, const float *__restrict__ gframe) {
     const int rec = blockIdx.x * 4 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;

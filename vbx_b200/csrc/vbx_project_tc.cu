@@ -1,29 +1,25 @@
-// Projection  rho[N,128] = X[N,D] . V[D,128]  on the 5th-generation tensor cores (tcgen05 / UMMA, sm_100a),
-// in split-precision 3xTF32 (x_lo*v_hi + x_hi*v_lo + x_hi*v_hi, fp32 accumulation in TMEM) because plain TF32
-// breaks the 1e-4 parity bar of the EM loop (SURVEY.md section 7, hard part 4).
+// Projection  rho[N,128] = X[N,D] . V[D,128]  on the Hopper tensor cores (wgmma, sm_90a), in split-precision 3xTF32
+// (x_lo*v_hi + x_hi*v_lo + x_hi*v_hi, fp32 accumulation in registers) because plain TF32 breaks the 1e-4 parity bar of
+// the EM loop (SURVEY.md section 7, hard part 4).
 // Reference: the caller-side projection VBx/vbhmm.py:129,153 folded with the scale VBx/VBx.py:88-89 (SURVEY 8d).
 //
 // The same kernel, templated on MODE, also runs the real-data front end (x-vector transform and PLDA projection,
-// VBx/vbhmm.py:125-129,153; launch_xvector_chain_tcgen05 below).
+// VBx/vbhmm.py:125-129,153; launch_xvector_chain_wgmma below).
 //
-// One persistent CTA per SM, 17 warps:
-//   warps 0-7  producers: coalesced LDG of a 256-frame x 32-column block of X (prefetched one block ahead in
-//              registers), split into TF32 hi/lo, stored into the 128B-swizzled K-major UMMA layout;
-//              thread 0 also issues the bulk-async (TMA, cp.async.bulk) copies of the pre-split V block.
-//   warp  8    MMA issuer: one thread issues 24 tcgen05.mma (M128 x N128 x K8, kind::tf32) per 32-column block
-//              (2 M-tiles x 4 k-steps x 3 split terms); tcgen05.commit releases the smem stage / publishes the
-//              accumulator.
-//   warps 9-16 epilogue: tcgen05.ld the 2 x (128 x 128) fp32 accumulators out of TMEM (lane = row), accumulate the
-//              per-frame constant G_t, transpose through a swizzled shared-memory tile and store rho with full
-//              128-byte lines per row.
-// Shared memory: 2 stages x (A hi/lo for 2 M-tiles 64 KB + B hi/lo 32 KB) = 192 KB.  TMEM: 2 accumulator sets of
-// 256 columns (all 512), so the epilogue of tile i overlaps the MMAs of tile i+1.
+// One persistent CTA per SM, 16 warps, tiles of 128 frames:
+//   warps 0-7   producers: coalesced LDG of a 128-frame x 32-column block of X (prefetched one block ahead in
+//               registers), split into TF32 parts, stored into the 128B-swizzled K-major wgmma layout;
+//               thread 0 also issues the bulk-async (TMA, cp.async.bulk) copies of the pre-split V block.
+//   warps 8-15  two consumer warpgroups, 64 frames each: wgmma.mma_async m64n128k8 tf32 from shared memory into
+//               64 fp32 registers per thread (4 k-steps x NS(NS+1)/2 split terms per 32-column block); a stage is
+//               released to the producers one block later (wgmma.wait_group 1).  The epilogue works on the register
+//               accumulators: the per-frame constant G_t (quad shuffles) and float2 stores of rho.
+// Shared memory: NS = 2: 3 stages x (A hi/lo 32 KB + B hi/lo 32 KB) = 192 KB; NS = 3: 2 stages x (A 48 KB + B 48 KB).
 //
 // NS = 3 (the real-data front end): operands are split three ways, x = x1 + x2 + x3 exactly (3 x 11 mantissa bits), and
 // six products are accumulated (x3 v1, x1 v3, x2 v2, x2 v1, x1 v2, x1 v1): the dropped terms are below 2^-33, i.e. the
 // GEMM is at fp32-accumulate accuracy.  The shipped LDA matrix is badly conditioned (sum |a_k lda_kn| ~ 1e3 |sum|), so
-// the 2^-21 relative error per product of the two-way split is visible on real data.  Three images per operand fit the
-// same 192 KB with ONE M-tile (128 frames) per CTA tile: 2 stages x (A 48 KB + B 48 KB).
+// the 2^-21 relative error per product of the two-way split is visible on real data.
 #include <cuda.h>
 
 #include "vbx_internal.cuh"
@@ -32,16 +28,19 @@ namespace vbx {
 
 namespace {
 
-constexpr int kMaxTileM = 256;              // frames per CTA tile: two UMMA M=128 tiles (NS = 2) or one (NS = 3)
+constexpr int kTileM = 128;                 // frames per CTA tile: two wgmma M=64 tiles
 constexpr int kKB = 32;                     // columns of X per pipeline block (= one 128-byte swizzle row)
-constexpr int kStages = 2;
 constexpr int kABytes = 128 * 128;          // one 128-row x 128-byte operand image
-constexpr int kStageBytes = 4 * kABytes + 2 * kABytes;  // A: 2 mtiles x hi/lo, B: hi/lo  ==  A: 1 mtile x 3 parts, B: 3 parts
 constexpr int kProducerThreads = 256;
-constexpr int kEpiWarps = 8;                // two per TMEM lane quarter (one per M-tile)
-constexpr int kThreads = (9 + kEpiWarps) * 32;
-constexpr int kEpiStageBytes = 32 * 128;    // per epilogue warp: 32 rows x 32 columns, 16-byte-chunk XOR swizzle
-constexpr uint32_t kTmemCols = 512;
+constexpr int kConsumerThreads = 256;       // two warpgroups
+constexpr int kThreads = kProducerThreads + kConsumerThreads;
+
+template <int NS> struct Pipe {
+    static constexpr int kStages = NS == 2 ? 3 : 2;
+    static constexpr int kStageBytes = 2 * NS * kABytes;   // A: NS images of 128 frames, B: NS images of V^T
+    // 1 KB alignment slack, stages, barriers (128 B), 1/Phi or e_off (512 B), row norms [2][128] (1 KB)
+    static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + 128 + 512 + 2 * kTileM * 4;
+};
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
@@ -71,33 +70,42 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
                  : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, both K-major, kind::tf32.  The 64-bit shared-memory descriptors are passed as
-// (lo, hi) words: hi is a constant, lo = (address >> 4) | LBO, so the single issuing thread spends two integer adds
-// per MMA instead of rebuilding descriptors (a lone thread retires ~1 dependent instruction per 4-5 cycles).
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-        "mov.b64 da, {%1, %3};\n\t"
-        "mov.b64 db, {%2, %3};\n\t"
-        "setp.ne.b32 p, %5, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %4, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-constexpr uint32_t kDescHi = (1024u >> 4) | (1u << 14) | (2u << 29);   // SBO = 1024 B, version 1, SWIZZLE_128B
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr) { return ((smem_addr >> 4) & 0x3fffu) | (1u << 16); }
-// Shared-memory matrix descriptors: K-major, 128-byte swizzle, dense 8-row groups (SBO = 1024 B), version 1 (sm_100);
-// see kDescHi / desc_lo above.
-// instruction descriptor: D=f32, A=B=tf32, both K-major, N=128, M=128
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
 
-// streaming 16-byte load that does not allocate in L1: with 194 KB of shared memory only ~32 KB of L1 remain, and
+// wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, dense 8-row groups (SBO = 1024 B, LBO unused = 1).
+// Advancing along K inside the 128-byte swizzle row, or by whole 1024-byte row groups, only adds to the start address
+// (bits 0-13, in 16-byte units), so the consumers add small integers to one descriptor per stage.
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
+    const uint32_t lo = ((smem_addr >> 4) & 0x3fffu) | (1u << 16);
+    const uint32_t hi = (1024u >> 4) | (1u << 30);                 // SBO, layout type 1 = SWIZZLE_128B
+    return ((uint64_t)hi << 32) | lo;
+}
+// D[64 x 128] (+)= A[smem, 64 x 8] * B[smem, 128 x 8]^T, tf32, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from touching the accumulators across the asynchronous MMAs
+__device__ __forceinline__ void fence_operands(float (&d)[64]) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// streaming 16-byte load that does not allocate in L1: with ~195 KB of shared memory only ~30 KB of L1 remain, and
 // allocating loads would cap the bytes in flight at that size
 __device__ __forceinline__ float4 ldg_stream(const float4 *p) {
     float4 v;
@@ -106,25 +114,6 @@ __device__ __forceinline__ float4 ldg_stream(const float4 *p) {
 }
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, const float4 v) {
     asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-__device__ __forceinline__ float4 ld_shared_v4(uint32_t addr) {
-    float4 v;
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-    return v;
-}
-// 32 consecutive fp32 TMEM columns of this warp's 32 lanes (lane = accumulator row)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 __device__ __forceinline__ void split_rn(const float x, float &hi, float &lo) {
     const uint32_t h = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;
@@ -171,30 +160,22 @@ __global__ void build_v_images_kernel(const float *__restrict__ V, int D, float 
 //         the producers also accumulate ||x - a_off||^2 per row and hand it to the epilogue through shared memory
 template <int MODE, int NS>
 __global__ void __launch_bounds__(kThreads, 1)
-project_tcgen05_kernel(const float *__restrict__ X, const float *__restrict__ vimg, float *__restrict__ rho, int64_t N,
-                       int D, const float *__restrict__ Phi, float *__restrict__ gframe,
-                       const float *__restrict__ a_off, const float *__restrict__ e_off) {
-    constexpr int MT = NS == 2 ? 2 : 1;          // UMMA M-tiles (128 frames) per CTA tile
-    constexpr int kTileM = 128 * MT;
+project_wgmma_kernel(const float *__restrict__ X, const float *__restrict__ vimg, float *__restrict__ rho, int64_t N,
+                     int D, const float *__restrict__ Phi, float *__restrict__ gframe,
+                     const float *__restrict__ a_off, const float *__restrict__ e_off) {
+    constexpr int kStages = Pipe<NS>::kStages, kStageBytes = Pipe<NS>::kStageBytes;
     constexpr int ROWS_PT = kTileM / 32;         // rows per producer thread
-    static_assert((MT * NS + NS) * kABytes == kStageBytes, "stage layout");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // the stage buffers must be 1024-byte aligned (128-byte swizzle); the dynamic window starts at offset 0 of the
-    // CTA's shared memory (no static __shared__ in this kernel), which is checked rather than padded for
-    uint8_t *smem = smem_raw;
-    if ((smem_u32(smem_raw) & 1023u) != 0) __trap();
+    // the stage buffers must be 1024-byte aligned (128-byte swizzle)
+    uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + kStages * kStageBytes);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 16);
-    float *s_inv_phi = reinterpret_cast<float *>(bars + 18);   // 128 floats: 1/Phi (MODE 0, 2) or e_off (MODE 1)
-    float *s_n1 = reinterpret_cast<float *>(smem + kStages * kStageBytes + 1024 + kEpiWarps * kEpiStageBytes);   // [2][kTileM]
+    float *s_inv_phi = reinterpret_cast<float *>(bars + 16);   // 128 floats: 1/Phi (MODE 0, 2) or e_off (MODE 1)
+    float *s_n1 = s_inv_phi + 128;                             // [2][kTileM] row norms (MODE 1), by tile parity
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t bar_base = smem_u32(bars);
-    // barrier ids
-    auto full_a = [&](int s) { return bar_base + 8u * (0 + s); };
-    auto full_b = [&](int s) { return bar_base + 8u * (2 + s); };
-    auto empty = [&](int s) { return bar_base + 8u * (4 + s); };
-    auto tmem_full = [&](int a) { return bar_base + 8u * (6 + a); };
-    auto tmem_empty = [&](int a) { return bar_base + 8u * (8 + a); };
+    auto full_a = [&](int s) { return bar_base + 8u * s; };
+    auto full_b = [&](int s) { return bar_base + 8u * (kStages + s); };
+    auto empty = [&](int s) { return bar_base + 8u * (2 * kStages + s); };
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int n_kb = D / kKB;
@@ -205,30 +186,18 @@ project_tcgen05_kernel(const float *__restrict__ X, const float *__restrict__ vi
         for (int s = 0; s < kStages; ++s) {
             mbar_init(full_a(s), kProducerThreads);
             mbar_init(full_b(s), 1);
-            mbar_init(empty(s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tmem_full(a), 1);
-            mbar_init(tmem_empty(a), 4 * MT * 32);     // the epilogue warps that own an M-tile
+            mbar_init(empty(s), kConsumerThreads);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 8) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(kTmemCols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp < 8) {
         // ======================= producers =======================
         // Blocks of this CTA in order: b -> (tile = blockIdx.x + (b / n_kb) * gridDim.x, kb = b % n_kb).  Two
         // ping-pong register sets keep the loads of the next block in flight while one is split and stored.
         const int c = tid & 7;            // 16-byte chunk inside the 128-byte row
-        const int r0 = tid >> 3;          // rows r0 + 32 i, i = 0..7
+        const int r0 = tid >> 3;          // rows r0 + 32 i
         const int64_t my_tiles = blockIdx.x < n_tiles ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
         const int64_t n_blocks = my_tiles * n_kb;
         float4 bufA[ROWS_PT], bufB[ROWS_PT];
@@ -247,8 +216,8 @@ project_tcgen05_kernel(const float *__restrict__ X, const float *__restrict__ vi
             }
         };
         auto process = [&](const int64_t b, const float4(&buf)[ROWS_PT]) {
-            const int s = (int)(b & 1);
-            const uint32_t ph = (uint32_t)((b >> 1) & 1);
+            const int s = (int)(b % kStages);
+            const uint32_t ph = (uint32_t)((b / kStages) & 1);
             const int kb = (int)(b % n_kb);
             float4 aoff = make_float4(0.f, 0.f, 0.f, 0.f);
             if (MODE != 0) aoff = __ldg(reinterpret_cast<const float4 *>(a_off + kb * kKB) + c);
@@ -256,12 +225,11 @@ project_tcgen05_kernel(const float *__restrict__ X, const float *__restrict__ vi
             const uint32_t stage = smem_base + s * kStageBytes;
             if (tid == 0) {
                 mbar_expect_tx(full_b(s), NS * kABytes);
-                bulk_g2s(stage + MT * NS * kABytes, vimg + (int64_t)kb * NS * 4096, NS * kABytes, full_b(s));
+                bulk_g2s(stage + NS * kABytes, vimg + (int64_t)kb * NS * 4096, NS * kABytes, full_b(s));
             }
 #pragma unroll
             for (int i = 0; i < ROWS_PT; ++i) {
-                const int r = r0 + 32 * i;             // 0..kTileM-1
-                const int mt = r >> 7, m = r & 127;
+                const int m = r0 + 32 * i;             // 0..kTileM-1
                 float4 hi, lo, x = buf[i];
                 if (MODE != 0) {
                     x.x -= aoff.x;
@@ -276,8 +244,8 @@ project_tcgen05_kernel(const float *__restrict__ X, const float *__restrict__ vi
                     split_rn(x.y, hi.y, lo.y);
                     split_rn(x.z, hi.z, lo.z);
                     split_rn(x.w, hi.w, lo.w);
-                    st_shared_v4(stage + (mt * 2 + 0) * kABytes + off, hi);
-                    st_shared_v4(stage + (mt * 2 + 1) * kABytes + off, lo);
+                    st_shared_v4(stage + 0 * kABytes + off, hi);
+                    st_shared_v4(stage + 1 * kABytes + off, lo);
                 } else {
                     float4 lo2;
                     split3_rn(x.x, hi.x, lo.x, lo2.x);
@@ -314,158 +282,106 @@ project_tcgen05_kernel(const float *__restrict__ X, const float *__restrict__ vi
                 process(b + 1, bufB);
             }
         }
-    } else if (warp == 8) {
-        // ======================= MMA issuer =======================
-        if (lane == 0) {
-            int s = 0;
-            uint32_t ph = 0;
-            int acc = 0;
-            uint32_t acc_ph = 0;
-            for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                mbar_wait(tmem_empty(acc), acc_ph ^ 1);   // epilogue has drained this accumulator set
-                tc_fence_after();
-                for (int kb = 0; kb < n_kb; ++kb) {
-                    mbar_wait(full_a(s), ph);
-                    mbar_wait(full_b(s), ph);
-                    tc_fence_after();
-                    const uint32_t st_lo = desc_lo(smem_base + s * kStageBytes);   // descriptor word of the stage base
-                    constexpr uint32_t kImg = kABytes >> 4;                        // one operand image, in 16-byte units
-                    const uint32_t b0 = st_lo + MT * NS * kImg;                    // B parts: b0, b0 + kImg, (b0 + 2 kImg)
+    } else {
+        // ======================= consumers: MMA + epilogue =======================
+        const int ct = tid - kProducerThreads;
+        const int wg = ct >> 7;                        // warpgroup: frames 64 wg .. 64 wg + 63 of the tile
+        const int rq = 16 * ((ct >> 5) & 3) + (lane >> 2);   // accumulator rows rq and rq + 8 of the warpgroup
+        const int cq = 2 * (lane & 3);                 // accumulator columns 8 j + cq, + 1
+        constexpr uint64_t kImg = kABytes >> 4;        // one operand image, in 16-byte descriptor units
+        float d[64];
+        int s = 0, last = 0;
+        uint32_t ph = 0;
+        int it = 0;
+        for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+            for (int kb = 0; kb < n_kb; ++kb) {
+                mbar_wait(full_a(s), ph);
+                mbar_wait(full_b(s), ph);
+                const uint32_t stage = smem_base + s * kStageBytes;
+                const uint64_t a0 = make_desc(stage + wg * 64 * 128);     // this warpgroup's 64 rows of the A images
+                const uint64_t b0 = make_desc(stage + NS * kABytes);
+                wgmma_fence();
 #pragma unroll
-                    for (int mt = 0; mt < MT; ++mt) {
-                        const uint32_t a0 = st_lo + mt * NS * kImg;                // A parts of this M-tile
-                        const uint32_t d = tmem_base + (uint32_t)(acc * (128 * MT) + mt * 128);
-#pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) {
-                            const uint32_t koff = ks * 2;      // 8 tf32 = 32 bytes inside the swizzle row (16-byte units)
-                            const uint32_t first = (kb == 0 && ks == 0) ? 0u : 1u;
-                            if (NS == 2) {                      // lo*hi + hi*lo + hi*hi
-                                umma_tf32(d, a0 + kImg + koff, b0 + koff, kDescHi, kIdesc, first);
-                                umma_tf32(d, a0 + koff, b0 + kImg + koff, kDescHi, kIdesc, 1u);
-                                umma_tf32(d, a0 + koff, b0 + koff, kDescHi, kIdesc, 1u);
-                            } else {                            // smallest terms first: x3 v1, x1 v3, x2 v2, x2 v1, x1 v2, x1 v1
-                                umma_tf32(d, a0 + 2 * kImg + koff, b0 + koff, kDescHi, kIdesc, first);
-                                umma_tf32(d, a0 + koff, b0 + 2 * kImg + koff, kDescHi, kIdesc, 1u);
-                                umma_tf32(d, a0 + kImg + koff, b0 + kImg + koff, kDescHi, kIdesc, 1u);
-                                umma_tf32(d, a0 + kImg + koff, b0 + koff, kDescHi, kIdesc, 1u);
-                                umma_tf32(d, a0 + koff, b0 + kImg + koff, kDescHi, kIdesc, 1u);
-                                umma_tf32(d, a0 + koff, b0 + koff, kDescHi, kIdesc, 1u);
-                            }
-                        }
-                    }
-                    tc_commit(empty(s));                       // stage reusable once these MMAs retire
-                    if (kb == n_kb - 1) tc_commit(tmem_full(acc));
-                    if (++s == kStages) {
-                        s = 0;
-                        ph ^= 1;
+                for (int ks = 0; ks < 4; ++ks) {
+                    const uint64_t k = ks * 2;         // 8 tf32 = 32 bytes inside the swizzle row (16-byte units)
+                    const uint32_t first = (kb == 0 && ks == 0) ? 0u : 1u;
+                    if (NS == 2) {                      // lo*hi + hi*lo + hi*hi
+                        wgmma_tf32(d, a0 + kImg + k, b0 + k, first);
+                        wgmma_tf32(d, a0 + k, b0 + kImg + k, 1u);
+                        wgmma_tf32(d, a0 + k, b0 + k, 1u);
+                    } else {                            // smallest terms first: x3 v1, x1 v3, x2 v2, x2 v1, x1 v2, x1 v1
+                        wgmma_tf32(d, a0 + 2 * kImg + k, b0 + k, first);
+                        wgmma_tf32(d, a0 + k, b0 + 2 * kImg + k, 1u);
+                        wgmma_tf32(d, a0 + kImg + k, b0 + kImg + k, 1u);
+                        wgmma_tf32(d, a0 + kImg + k, b0 + k, 1u);
+                        wgmma_tf32(d, a0 + k, b0 + kImg + k, 1u);
+                        wgmma_tf32(d, a0 + k, b0 + k, 1u);
                     }
                 }
-                if (++acc == 2) {
-                    acc = 0;
-                    acc_ph ^= 1;
+                wgmma_commit();
+                if (kb > 0) {                          // the previous block's MMAs have retired: release its stage
+                    wgmma_wait<1>();
+                    mbar_arrive(empty(last));
+                }
+                last = s;
+                if (++s == kStages) {
+                    s = 0;
+                    ph ^= 1;
                 }
             }
-        }
-        __syncwarp();
-    } else {
-        // ======================= epilogue =======================
-        const int quarter = warp & 3;                  // TMEM lanes 32*quarter .. +31 are visible to this warp
-        const int mt = (warp - 9) >> 2;                // M-tile handled by this warp
-        if (mt < MT) {                                 // with one M-tile per CTA tile the second group of four warps idles
-        const uint32_t epi = smem_base + kStages * kStageBytes + 1024 + (warp - 9) * kEpiStageBytes;
-        const uint32_t inv_phi_s = smem_u32(s_inv_phi);
-        int acc = 0;
-        uint32_t acc_ph = 0;
-        for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            mbar_wait(tmem_full(acc), acc_ph);
-            tc_fence_after();
-            const int64_t row_base = tile * kTileM + mt * 128 + quarter * 32;
-            const uint32_t tbase = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * (128 * MT) + mt * 128);
-            // lane = row.  8 lanes then cover the 128 bytes of one row: every store instruction writes 4 full lines
-            auto store_block = [&](const int cb) {
-                __syncwarp();
-                const int cc = lane & 7, rr = lane >> 3;
-#pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    const int r = 4 * k + rr;
-                    float4 x;
-                    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x.x), "=f"(x.y), "=f"(x.z), "=f"(x.w)
-                                 : "r"(epi + (uint32_t)(r * 128 + ((cc ^ (r & 7)) << 4))));
-                    if (row_base + r < N) *reinterpret_cast<float4 *>(rho + (row_base + r) * 128 + cb * 32 + 4 * cc) = x;
-                }
-                __syncwarp();
-            };
+            wgmma_wait<0>();
+            fence_operands(d);
+            const int64_t ra = tile * kTileM + wg * 64 + rq, rb = ra + 8;
+            float n1a = 0.f, n1b = 0.f;
+            if (MODE == 1) {                           // read before the release: the producers reuse this slot two tiles on
+                n1a = s_n1[(it & 1) * kTileM + wg * 64 + rq];
+                n1b = s_n1[(it & 1) * kTileM + wg * 64 + rq + 8];
+            }
+            mbar_arrive(empty(last));
+            float na = 0.f, nb = 0.f;
             if (MODE == 1) {
-                // y = acc / ||x - mean1|| - mean2 ; out = y / ||y||   (two passes over the TMEM accumulator)
-                const float inv_n1 = 1.f / sqrtf(s_n1[acc * kTileM + mt * 128 + quarter * 32 + lane]);
-                float n2 = 0.f;
-#pragma unroll 1
-                for (int cb = 0; cb < 4; ++cb) {
-                    uint32_t v[32];
-                    tmem_ld32(tbase + (uint32_t)(cb * 32), v);
+                // y = acc / ||x - mean1|| - mean2 ; out = y / ||y||
+                const float ia = 1.f / sqrtf(n1a), ib = 1.f / sqrtf(n1b);
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float4 e = ld_shared_v4(inv_phi_s + (uint32_t)(cb * 32 + 4 * j) * 4);
-                        const float y0 = fmaf(__uint_as_float(v[4 * j]), inv_n1, -e.x);
-                        const float y1 = fmaf(__uint_as_float(v[4 * j + 1]), inv_n1, -e.y);
-                        const float y2 = fmaf(__uint_as_float(v[4 * j + 2]), inv_n1, -e.z);
-                        const float y3 = fmaf(__uint_as_float(v[4 * j + 3]), inv_n1, -e.w);
-                        n2 = fmaf(y0, y0, fmaf(y1, y1, fmaf(y2, y2, fmaf(y3, y3, n2))));
-                    }
+                for (int j = 0; j < 16; ++j) {
+                    const float2 e = *reinterpret_cast<const float2 *>(s_inv_phi + 8 * j + cq);
+                    d[4 * j] = fmaf(d[4 * j], ia, -e.x);
+                    d[4 * j + 1] = fmaf(d[4 * j + 1], ia, -e.y);
+                    d[4 * j + 2] = fmaf(d[4 * j + 2], ib, -e.x);
+                    d[4 * j + 3] = fmaf(d[4 * j + 3], ib, -e.y);
+                    na = fmaf(d[4 * j], d[4 * j], fmaf(d[4 * j + 1], d[4 * j + 1], na));
+                    nb = fmaf(d[4 * j + 2], d[4 * j + 2], fmaf(d[4 * j + 3], d[4 * j + 3], nb));
                 }
-                const float inv_n2 = 1.f / sqrtf(n2);
-#pragma unroll 1
-                for (int cb = 0; cb < 4; ++cb) {
-                    uint32_t v[32];
-                    tmem_ld32(tbase + (uint32_t)(cb * 32), v);
+                na += __shfl_xor_sync(0xffffffffu, na, 1);
+                na += __shfl_xor_sync(0xffffffffu, na, 2);
+                nb += __shfl_xor_sync(0xffffffffu, nb, 1);
+                nb += __shfl_xor_sync(0xffffffffu, nb, 2);
+                const float sa = 1.f / sqrtf(na), sb = 1.f / sqrtf(nb);
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float4 e = ld_shared_v4(inv_phi_s + (uint32_t)(cb * 32 + 4 * j) * 4);
-                        float4 x;
-                        x.x = fmaf(__uint_as_float(v[4 * j]), inv_n1, -e.x) * inv_n2;
-                        x.y = fmaf(__uint_as_float(v[4 * j + 1]), inv_n1, -e.y) * inv_n2;
-                        x.z = fmaf(__uint_as_float(v[4 * j + 2]), inv_n1, -e.z) * inv_n2;
-                        x.w = fmaf(__uint_as_float(v[4 * j + 3]), inv_n1, -e.w) * inv_n2;
-                        st_shared_v4(epi + (uint32_t)(lane * 128 + ((j ^ (lane & 7)) << 4)), x);
-                    }
-                    store_block(cb);
+                for (int j = 0; j < 16; ++j) {
+                    if (ra < N) *reinterpret_cast<float2 *>(rho + ra * 128 + 8 * j + cq) = make_float2(d[4 * j] * sa, d[4 * j + 1] * sa);
+                    if (rb < N) *reinterpret_cast<float2 *>(rho + rb * 128 + 8 * j + cq) = make_float2(d[4 * j + 2] * sb, d[4 * j + 3] * sb);
                 }
             } else {
-                float n2 = 0.f;                          // ||fea||^2 = sum_r rho^2 / Phi_r   (VBx/VBx.py:87)
-#pragma unroll 1
-                for (int cb = 0; cb < 4; ++cb) {
-                    uint32_t v[32];
-                    tmem_ld32(tbase + (uint32_t)(cb * 32), v);
-                    // G_t partial sum and the swizzled stage (chunk j of row r at position j ^ (r & 7))
+                // ||fea||^2 = sum_r rho^2 / Phi_r   (VBx/VBx.py:87); a row's 128 columns are spread over a quad of lanes
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float4 ip = ld_shared_v4(inv_phi_s + (uint32_t)(cb * 32 + 4 * j) * 4);
-                        const float4 x = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                                     __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                        n2 = fmaf(x.x * x.x, ip.x, n2);
-                        n2 = fmaf(x.y * x.y, ip.y, n2);
-                        n2 = fmaf(x.z * x.z, ip.z, n2);
-                        n2 = fmaf(x.w * x.w, ip.w, n2);
-                        st_shared_v4(epi + (uint32_t)(lane * 128 + ((j ^ (lane & 7)) << 4)), x);
-                    }
-                    store_block(cb);
+                for (int j = 0; j < 16; ++j) {
+                    const float2 ip = *reinterpret_cast<const float2 *>(s_inv_phi + 8 * j + cq);
+                    na = fmaf(d[4 * j] * d[4 * j], ip.x, fmaf(d[4 * j + 1] * d[4 * j + 1], ip.y, na));
+                    nb = fmaf(d[4 * j + 2] * d[4 * j + 2], ip.x, fmaf(d[4 * j + 3] * d[4 * j + 3], ip.y, nb));
+                    if (ra < N) *reinterpret_cast<float2 *>(rho + ra * 128 + 8 * j + cq) = make_float2(d[4 * j], d[4 * j + 1]);
+                    if (rb < N) *reinterpret_cast<float2 *>(rho + rb * 128 + 8 * j + cq) = make_float2(d[4 * j + 2], d[4 * j + 3]);
                 }
-                if (row_base + lane < N) gframe[row_base + lane] = -0.5f * (n2 + 128.f * 1.8378770664093453f);   // G_t, R = 128
-            }
-            tc_fence_before();
-            mbar_arrive(tmem_empty(acc));
-            if (++acc == 2) {
-                acc = 0;
-                acc_ph ^= 1;
+                na += __shfl_xor_sync(0xffffffffu, na, 1);
+                na += __shfl_xor_sync(0xffffffffu, na, 2);
+                nb += __shfl_xor_sync(0xffffffffu, nb, 1);
+                nb += __shfl_xor_sync(0xffffffffu, nb, 2);
+                if ((lane & 3) == 0) {                 // G_t, R = 128
+                    if (ra < N) gframe[ra] = -0.5f * (na + 128.f * 1.8378770664093453f);
+                    if (rb < N) gframe[rb] = -0.5f * (nb + 128.f * 1.8378770664093453f);
+                }
             }
         }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 8) {
-        tc_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols) : "memory");
     }
 }
 
@@ -482,8 +398,6 @@ __global__ void build_plda_v_kernel(const float *__restrict__ tr, const float *_
 // cudaFuncSetAttribute is per device; everything else the launches need comes from the caller's workspace
 bool g_configured[64][3][2] = {};
 
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 + kEpiWarps * kEpiStageBytes + 2 * kMaxTileM * 4;
-
 // one GEMM pass [N,D] x [D,128] of the given MODE; V is row-major [D,128] in device memory
 template <int MODE, int NS>
 int launch_gemm_tc(float *vimg, int64_t N, const float *X, int D, const float *V, const float *Phi, float *out, float *gframe,
@@ -495,22 +409,24 @@ int launch_gemm_tc(float *vimg, int64_t N, const float *X, int D, const float *V
         return -1;
     }
     if (!g_configured[dev][MODE][NS - 2]) {
-        if (cudaFuncSetAttribute(project_tcgen05_kernel<MODE, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) !=
+        if (cudaFuncSetAttribute(project_wgmma_kernel<MODE, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Pipe<NS>::kSmemBytes) !=
             cudaSuccess) {
             if (err) *err = "cudaFuncSetAttribute(smem) failed";
             return -1;
         }
         g_configured[dev][MODE][NS - 2] = true;
     }
-    constexpr int kTileM = NS == 2 ? 256 : 128;
-    int sms = 148;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int sms = 0;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) {
+        if (err) *err = "cudaDeviceGetAttribute(multiprocessor count) failed";
+        return -1;
+    }
     build_v_images_kernel<NS><<<D / kKB, 256, 0, st>>>(V, D, vimg);
     const int64_t n_tiles = (N + kTileM - 1) / kTileM;
     const int grid = (int)std::min<int64_t>(n_tiles, sms);
-    project_tcgen05_kernel<MODE, NS><<<grid, kThreads, kSmemBytes, st>>>(X, vimg, out, N, D, Phi, gframe, a_off, e_off);
+    project_wgmma_kernel<MODE, NS><<<grid, kThreads, Pipe<NS>::kSmemBytes, st>>>(X, vimg, out, N, D, Phi, gframe, a_off, e_off);
     if (cudaGetLastError() != cudaSuccess) {
-        if (err) *err = "tcgen05 projection launch failed";
+        if (err) *err = "wgmma projection launch failed";
         return -1;
     }
     return 2;
@@ -522,18 +438,18 @@ int launch_gemm_tc(float *vimg, int64_t N, const float *X, int D, const float *V
 // 32 rows of V) for D up to kTcMaxD, and the folded PLDA matrix of the x-vector chain.
 size_t tc_scratch_floats() { return (size_t)(kTcMaxD / kKB) * 3 * 4096 + 128 * 128; }
 
-int launch_project_tcgen05(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,
-                           float *gframe, cudaStream_t st, std::string *err) {
+int launch_project_wgmma(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,
+                         float *gframe, cudaStream_t st, std::string *err) {
     if (pl.R != 128) {
-        if (err) *err = "tcgen05 projection needs R == 128";
+        if (err) *err = "the tensor-core projection needs R == 128";
         return -1;
     }
     if (D % kKB != 0 || D < kKB) {
-        if (err) *err = "tcgen05 projection needs D to be a multiple of 32";
+        if (err) *err = "the tensor-core projection needs D to be a multiple of 32";
         return -1;
     }
     if (D > kTcMaxD || !tc_scratch) {
-        if (err) *err = "tcgen05 projection needs D <= 2048 and a plan with R == 128";
+        if (err) *err = "the tensor-core projection needs D <= 2048 and a plan with R == 128";
         return -1;
     }
     if (pl.n_frames == 0) return 0;
@@ -543,9 +459,9 @@ int launch_project_tcgen05(const Plan &pl, float *tc_scratch, const float *X, in
 // The caller-side chain of VBx/vbhmm.py:125-129,153 plus the scale of VBx/VBx.py:88-89 as two tensor-core passes:
 //   x_norm = l2norm(l2norm(x_raw - mean1) . lda - mean2)             [N,128]
 //   rho    = (x_norm - plda_mu) . (plda_tr^T * sqrt(psi))            [N,128], with G_t per frame
-int launch_xvector_chain_tcgen05(const Plan &pl, float *tc_scratch, const float *x_raw, int Dx, const float *mean1, const float *lda,
-                                 const float *mean2, const float *plda_mu, const float *plda_tr, const float *psi,
-                                 float *x_norm, float *rho, float *gframe, cudaStream_t st, std::string *err) {
+int launch_xvector_chain_wgmma(const Plan &pl, float *tc_scratch, const float *x_raw, int Dx, const float *mean1, const float *lda,
+                               const float *mean2, const float *plda_mu, const float *plda_tr, const float *psi,
+                               float *x_norm, float *rho, float *gframe, cudaStream_t st, std::string *err) {
     if (pl.R != 128) {
         if (err) *err = "the x-vector chain needs R == 128";
         return -1;

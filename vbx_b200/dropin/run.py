@@ -1,4 +1,4 @@
-"""Run an UNCHANGED reference script (VBx/vbhmm.py) with `VBx` bound to the B200 implementation:
+"""Run an UNCHANGED reference script (VBx/vbhmm.py) with `VBx` bound to the H100 implementation:
 
     python -m vbx_b200.dropin.run /path/to/VBx/vbhmm.py --init AHC+VB --out-rttm-dir exp ...
 
