@@ -120,7 +120,9 @@ int vbx_prepare_xvectors(vbx_handle_t h, const float *x_raw, int32_t Dx, const f
  *             (VBx/VBx.py:94), written with the last M-step's values (return_model, VBx/VBx.py:126)
  *   Li_out    [n_rec,max_iters] float64 ELBO trace, NaN after the last executed iteration (VBx/VBx.py:105)
  *   n_iters_out [n_rec] iterations executed (the epsilon stop of VBx/VBx.py:122-125 is per recording)
- *   flags_out [n_rec] vbx_flag bits */
+ *   flags_out [n_rec] vbx_flag bits
+ * A recording with no frames (or n_states 0) runs no iteration: n_iters 0, flags 0, its Li row all NaN, and its rows of
+ * pi_io, alpha_io and invL_io are left as passed in. */
 /* Stop rule: with a finite epsilon (and option "exact_stop") the test `ELBO_i - ELBO_{i-1} < epsilon` is decided on
  * float32 ELBO values only while the step is far from epsilon; a recording whose step comes near it re-evaluates its
  * last two iterations and all following ones in float64 (inputs: the same float32 rho / gamma), so iteration counts
@@ -181,6 +183,12 @@ int vbx_forward_backward(vbx_handle_t h, const double *lls, const double *tr, co
  *   doubles are then all-reduced (sum) over the ranks, on `stream`.  Li and trace_out are device pointers. */
 int vbx_attach_comm(vbx_handle_t h, void *nccl_comm, int32_t n_ranks, const char *libnccl_path);
 int vbx_elbo_trace(vbx_handle_t h, const double *Li, int32_t max_iters, double *trace_out, void *stream);
+
+/* Diagnostic: the per-recording ELBO constant G_b = sum_t -0.5 (sum_r rho_tr^2 / Phi_r + R log 2pi) that the last
+ * vbx_prepare_* call computed (the term of VBx/VBx.py:87 that vbx_run adds to every ELBO), copied device to device into
+ * gsum_out [n_rec] (float64, device pointer) on `stream`.  A recording with no frames has G_b = 0.
+ * VBX_ERR_STATE before a vbx_prepare_* call on the current plan and workspace. */
+int vbx_get_gsum(vbx_handle_t h, double *gsum_out, void *stream);
 
 /* Number of kernels launched by this handle since creation (bench.py reports it as gpu_launches). */
 int64_t vbx_launch_count(vbx_handle_t h);

@@ -54,6 +54,64 @@ def matmul_6x(a, b):
     return (small + (mm(a2, b1) + mm(a1, b2))) + mm(a1, b1)
 
 
+def matmul_3xtf32_dropped(a, b):
+    """3xTF32 with the cross term lo(a) * hi(b) lost: what a projection kernel missing one of its three MMAs computes."""
+    ah, _ = split2(a)
+    bh, bl = split2(b)
+    return mm(ah, bl) + mm(ah, bh)
+
+
+# Accuracy checks of the split-precision projection rho = X . V (tests/test_projection_gpu.py holds the kernel to them).
+#  per element: |rho - X V| <= elementwise_tolerance(D) * (|X| |V|)   -- 2^-20 covers the split (lo*lo dropped, both lo
+#               parts rounded to tf32: 3 * 2^-22 per product), D * 2^-23 the float32 accumulation of D products, with a
+#               factor 2 for the truncating adds of the tensor cores;
+#  normwise:    ||rho - X V||_F / || |X| |V| ||_F  at most normwise_ceiling(D, e) with e that of a float32 FFMA matmul:
+#               NORMWISE_FACTOR * sqrt(D / 32) * e.  The tensor cores truncate when they accumulate, so their rounding
+#               errors share a sign and grow like D * u where round-to-nearest ones grow like sqrt(D) * u: relative to
+#               FFMA the normwise error grows with sqrt(D) (measured on an H100: 2.4x FFMA at D = 32, 6.3x at 256,
+#               18x at 2048; this emulation rounds to nearest and stays at ~1x).
+# The per-element bound is a ceiling that grows with D, so at D >= ~1024 a lost cross term stays below it; the normwise
+# ratio catches that at every D.
+NORMWISE_FACTOR = 4.0
+
+
+def elementwise_tolerance(D):
+    return 2.0 ** -20 + D * 2.0 ** -23
+
+
+def normwise_ceiling(D, ffma_error):
+    return NORMWISE_FACTOR * np.sqrt(max(D, 32) / 32.0) * ffma_error
+
+
+def bound_ratio(got, X, V):
+    """max over elements of |got - X V| / (elementwise_tolerance(D) |X| |V|): <= 1 passes."""
+    X, V = X.astype(f64), V.astype(f64)
+    return float((np.abs(got.astype(f64) - X @ V) / (elementwise_tolerance(X.shape[1]) * (np.abs(X) @ np.abs(V)))).max())
+
+
+def normwise_error(got, X, V):
+    X, V = X.astype(f64), V.astype(f64)
+    return float(np.linalg.norm(got.astype(f64) - X @ V) / np.linalg.norm(np.abs(X) @ np.abs(V)))
+
+
+def test_projection_accuracy_checks_have_teeth():
+    """The two checks the wgmma projection must pass: 3xTF32 passes both at every D, plain TF32 and 3xTF32 with one
+    cross term lost fail them (the per-element bound alone up to D = 256, the normwise ratio at every D)."""
+    rng = np.random.default_rng(4)
+    for D in (32, 256, 2048):
+        X = rng.standard_normal((2000, D)).astype(f32)
+        V = rng.standard_normal((D, 128)).astype(f32)
+        ffma = normwise_error(mm(X, V), X, V)
+        r3, n3 = bound_ratio(matmul_3xtf32(X, V), X, V), normwise_error(matmul_3xtf32(X, V), X, V)
+        assert r3 <= 0.25 and n3 <= normwise_ceiling(D, ffma), (D, r3, n3, ffma)
+        for bad in (matmul_1xtf32, matmul_3xtf32_dropped):
+            got = bad(X, V)
+            rb, nb = bound_ratio(got, X, V), normwise_error(got, X, V)
+            assert nb > 5 * normwise_ceiling(D, ffma), (D, bad.__name__, nb, ffma)
+            if D <= 256:
+                assert rb > 1.0, (D, bad.__name__, rb)
+
+
 def test_splits_are_exact_where_the_kernels_rely_on_it():
     rng = np.random.default_rng(0)
     x = (rng.standard_normal(100000) * np.exp(rng.uniform(-20, 20, 100000))).astype(f32)

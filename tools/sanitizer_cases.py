@@ -1,5 +1,5 @@
-"""Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection and
-x-vector chain, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
+"""Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection at
+D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
 6..64, per-recording state masks, AHC, hard labels, the dense forward_backward() and the ELBO trace.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
@@ -18,7 +18,7 @@ dev = torch.device('cuda:0')
 
 
 def run(lens, S, iters, D=None, ns=None, fb_split=0, eps=-float('inf'), tag=''):
-    d = synth.make_batch(lens, R=128, S=S, seed=3, D=D, dtype=np.float32)
+    d = synth.make_batch([t for t in lens if t], R=128, S=S, seed=3, D=D, dtype=np.float32)   # T = 0: no rows
     nsa = np.full(len(lens), S, dtype=np.int32) if ns is None else np.asarray(ns, dtype=np.int32)
     vb = VbxBatch(lens, 128, nsa, device=dev, fb_split=fb_split)
     Sp = vb.S
@@ -55,6 +55,23 @@ run([513, 512, 1], 64, 2, fb_split=1, tag='S=64 split')
 run([100, 200], 31, 2, fb_split=1, tag='S=31 split')
 run([300, 120, 64], 8, 30, eps=1e-5, tag='stop rule, float64 finish')
 run([513, 40], 31, 25, eps=1e-6, fb_split=2, tag='stop rule fused')
+run([0, 300, 45, 0, 129, 0], 8, 30, D=256, eps=1e-5, fb_split=2, tag='empty recordings fused')
+run([0, 300, 45, 0, 129, 0], 8, 30, D=256, eps=1e-5, fb_split=1, tag='empty recordings split')
+
+# wgmma projection at the smallest and largest D, one frame and one frame past a full wave of tiles
+sms = torch.cuda.get_device_properties(0).multi_processor_count
+gen = np.random.default_rng(7)
+for D in (32, 2048):
+    for N in (1, 128 * sms + 1):
+        pb = VbxBatch([N], 128, 4, device=dev)
+        pb.set_option('projection', 2)
+        pb.prepare_project(torch.from_numpy(gen.standard_normal((N, D)).astype(np.float32)).to(dev),
+                           torch.from_numpy(gen.standard_normal((D, 128)).astype(np.float32)).to(dev),
+                           torch.ones(128, device=dev))
+        pg = pb.g_sum()
+        torch.cuda.synchronize()
+        pb.close()
+        print('projection ok', D, N, float(pg[0]))
 
 # real-data front end + AHC
 T = 300
@@ -70,6 +87,17 @@ labels, thr, _ = ahc.ahc_batch(front, xn)
 torch.cuda.synchronize()
 front.close()
 print('front end + AHC ok', int(labels[0].max()) + 1)
+
+# x-vector chain with Dx = 512 over more than one tile per CTA
+T = 128 * sms + 1
+front = VbxBatch([T], 128, 1, device=dev)
+model512 = [torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32)).to(dev) for a in (
+    gen.standard_normal(512) * 0.1, gen.standard_normal((512, 128)) / 16, gen.standard_normal(128) * 0.05,
+    gen.standard_normal(128) * 0.02, q * gen.uniform(2, 20, 128)[:, None], np.linspace(8.0, 0.05, 128))]
+rho, xn = front.prepare_xvectors(torch.from_numpy(gen.standard_normal((T, 512)).astype(np.float32)).to(dev), *model512)
+torch.cuda.synchronize()
+front.close()
+print('x-vector chain Dx=512 ok', float(rho[-1, 0]))
 
 # dense forward_backward()
 lls = gen.standard_normal((60, 9)) * 5

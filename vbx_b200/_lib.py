@@ -12,7 +12,7 @@ LIB_PATH = os.environ.get('VBX_B200_LIB', os.path.join(_HERE, 'libvbx_b200.so'))
 EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_create', 'vbx_destroy', 'vbx_last_error',
            'vbx_set_option', 'vbx_plan', 'vbx_bind_workspace', 'vbx_prepare_scale',
            'vbx_prepare_project', 'vbx_prepare_xvectors', 'vbx_run', 'vbx_hard_labels', 'vbx_ahc_workspace_bytes', 'vbx_ahc', 'vbx_launch_count', 'vbx_get_timings', 'vbx_f64_workspace_bytes',
-           'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace']
+           'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace', 'vbx_get_gsum']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 KERNEL_CLASSES = ['project', 'prepare', 'run_init', 'mstep_partial', 'speaker_model', 'loglik', 'forward_backward', 'exact64']
@@ -79,6 +79,8 @@ def load():
     lib.vbx_attach_comm.argtypes = [vp, vp, i32, ctypes.c_char_p]
     lib.vbx_elbo_trace.restype = ctypes.c_int
     lib.vbx_elbo_trace.argtypes = [vp, vp, i32, vp, vp]
+    lib.vbx_get_gsum.restype = ctypes.c_int
+    lib.vbx_get_gsum.argtypes = [vp, vp, vp]
     lib.vbx_get_timings.restype = ctypes.c_int
     lib.vbx_get_timings.argtypes = [vp, ctypes.POINTER(dbl), ctypes.POINTER(i64), i32]
     _lib = lib

@@ -137,6 +137,13 @@ class VbxBatch:
         self._check(self.lib.vbx_elbo_trace(self._h, _ptr(Li), n, _ptr(out), self._stream()))
         return out
 
+    def g_sum(self):
+        """The ELBO constant of every recording from the last prepare_*() call (a diagnostic, vbx_get_gsum):
+        float64 CUDA tensor [B], G_b = sum_t -0.5 * (sum_r rho_tr^2 / Phi_r + R log 2pi)."""
+        out = torch.empty(self.B, dtype=torch.float64, device=self.device)
+        self._check(self.lib.vbx_get_gsum(self._h, _ptr(out), self._stream()))
+        return out
+
     def set_option(self, name, value):
         self._check(self.lib.vbx_set_option(self._h, name.encode(), int(value)))
 

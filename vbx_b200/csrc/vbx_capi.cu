@@ -897,6 +897,19 @@ int vbx_elbo_trace(vbx_handle_t h, const double *Li, int32_t max_iters, double *
     return VBX_OK;
 }
 
+int vbx_get_gsum(vbx_handle_t h, double *gsum_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    if (!h->planned || !h->bound || !h->prepared) return fail(h, VBX_ERR_STATE, "vbx_get_gsum: call vbx_prepare_* first");
+    if (h->plan.n_rec == 0) return VBX_OK;
+    if (!gsum_out) return fail(h, VBX_ERR_ARG, "vbx_get_gsum: null pointer");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    const cudaError_t e = cudaMemcpyAsync(gsum_out, h->ws.gsum, sizeof(double) * h->plan.n_rec, cudaMemcpyDeviceToDevice,
+                                          (cudaStream_t)stream);
+    if (e != cudaSuccess) return cuda_fail(h, e, "vbx_get_gsum");
+    return VBX_OK;
+}
+
 int64_t vbx_launch_count(vbx_handle_t h) { return h ? h->launches : -1; }
 
 int vbx_get_timings(vbx_handle_t h, double *ms_out, int64_t *count_out, int32_t reset) {

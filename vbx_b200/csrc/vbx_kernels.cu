@@ -123,16 +123,17 @@ int launch_gsum_from_frames(const Plan &pl, const Workspace &ws, const float *gf
 
 int launch_prepare_scale(const Plan &pl, const Workspace &ws, const float *fea, const float *Phi, float *rho,
                          cudaStream_t st) {
-    if (pl.n_mtiles == 0) return 0;
-    prepare_kernel<0><<<pl.n_mtiles, 256, 0, st>>>(pl, ws, fea, Phi, rho);
+    if (pl.n_rec == 0) return 0;
+    // a batch of empty recordings has no M-tiles, but its G sums (zeros) are still written
+    if (pl.n_mtiles) prepare_kernel<0><<<pl.n_mtiles, 256, 0, st>>>(pl, ws, fea, Phi, rho);
     gsum_kernel<<<(pl.n_rec + 127) / 128, 128, 0, st>>>(pl, ws);
-    return cudaGetLastError() == cudaSuccess ? 2 : -1;
+    return cudaGetLastError() == cudaSuccess ? (pl.n_mtiles ? 2 : 1) : -1;
 }
 int launch_g_from_rho(const Plan &pl, const Workspace &ws, const float *rho, const float *Phi, cudaStream_t st) {
-    if (pl.n_mtiles == 0) return 0;
-    prepare_kernel<1><<<pl.n_mtiles, 256, 0, st>>>(pl, ws, rho, Phi, nullptr);
+    if (pl.n_rec == 0) return 0;
+    if (pl.n_mtiles) prepare_kernel<1><<<pl.n_mtiles, 256, 0, st>>>(pl, ws, rho, Phi, nullptr);
     gsum_kernel<<<(pl.n_rec + 127) / 128, 128, 0, st>>>(pl, ws);
-    return cudaGetLastError() == cudaSuccess ? 2 : -1;
+    return cudaGetLastError() == cudaSuccess ? (pl.n_mtiles ? 2 : 1) : -1;
 }
 
 // ------------------------------------------------------------------------------------------------
