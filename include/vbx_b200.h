@@ -51,9 +51,12 @@ enum vbx_flag {
 
 const char *vbx_version(void);
 
-/* Smallest supported padded state count >= n_states (4, 8, 16, 32 or 64); -1 if n_states > 64 or < 1.
- * (Limits of the float32 kernels: S <= 64, R <= 128 and a multiple of 4.  vbx_plan_f64 / vbx_run_f64 have no such limits.) */
+/* Smallest padded state count >= n_states of the tiers up to 64 (4, 8, 16, 32 or 64); -1 if n_states > 64 or < 1.
+ * (Limits of the float32 kernels: S <= 128, R <= 128 and a multiple of 4.  vbx_plan_f64 / vbx_run_f64 have no such limits.) */
 int32_t vbx_padded_states(int32_t n_states);
+/* The same with the wide tier: 4, 8, 16, 32, 64, or 128 for 65 <= n_states <= 128; -1 if n_states > 128 or < 1.
+ * S = 128 plans always run the split forward-backward schedule (see option "fb_split"). */
+int32_t vbx_padded_states_wide(int32_t n_states);
 
 int vbx_create(int32_t device, vbx_handle_t *out);
 int vbx_destroy(vbx_handle_t h);
@@ -67,7 +70,8 @@ const char *vbx_last_error(vbx_handle_t h);
  * "fb_split" (read by the next vbx_plan): 0 = auto, 1 = always, 2 = never run the forward and the backward sweep of a
  * recording concurrently on separate warps followed by a combine pass (the choice for batches too small to fill the GPU;
  * results differ from the fused sweep by float32 rounding only, so pin it to 1 or 2 where bit-identical results for a
- * recording alone / inside a large batch matter).
+ * recording alone / inside a large batch matter).  S = 128 plans always split: 0 and 1 mean the same there, and
+ * vbx_plan refuses S = 128 with VBX_ERR_ARG while fb_split = 2.
  * "graph": 0 = auto (small batches: plans on the split schedule), 1 = always, 2 = never replay a whole vbx_run as ONE CUDA
  * graph launch.  The second call with identical arguments (pointers and scalars) is captured on a stream of the handle,
  * later identical calls replay it (ordered against `stream` with events, no host synchronisation); any other call, and
@@ -75,14 +79,17 @@ const char *vbx_last_error(vbx_handle_t h);
  * "fb_priority": 0 = auto (large batches), 1 = always, 2 = never launch the forward-backward sweep on a high-priority side
  * stream of the handle (ordered against `stream` with events, still no host synchronisation), so that it interleaves with
  * the bandwidth-bound kernels of ANOTHER handle working on the same device (vbx_b200/parts.py runs two halves of a batch).
- * Tuning knobs: "fb_states_per_lane" (0 = auto, 1, 2, 4), "fb_classic" (forward-backward sweep: 0 = one-step
+ * "fold_speaker" (0/1, default 0): compute the speaker model inside the tensor-core M-step kernel; ignored at S = 128.
+ * Tuning knobs: "fb_states_per_lane" (0 = auto, 1, 2, 4; at S = 64 values below 2 and at S = 128 values below 4 are
+ * raised to those, since a recording's lane group must fit in a warp), "fb_classic" (forward-backward sweep: 0 = one-step
  * look-ahead recurrences, 1 = normalise-every-frame), "projection" (0 = auto, 1 = FFMA tiles,
  * 2 = wgmma 3xTF32), "gemm" (in-loop contractions: 0 = tensor cores in split-precision 3xTF32, 1 = FFMA),
  * "timing" (0/1, see vbx_get_timings).  Unknown names return VBX_ERR_ARG. */
 int vbx_set_option(vbx_handle_t h, const char *name, int32_t value);
 
 /* Describe a batch: offsets_host[n_rec+1] (HOST, int64, offsets_host[0] == 0), feature dim R
- * (VBx/VBx.py:74 `D`; multiple of 4, <= 128), padded state count S.  Builds the tile lists on the device
+ * (VBx/VBx.py:74 `D`; multiple of 4, <= 128), padded state count S (4, 8, 16, 32, 64 or 128, from vbx_padded_states_wide;
+ * S = 128 always takes the split forward-backward schedule).  Builds the tile lists on the device
  * and reports the workspace the caller must provide through vbx_bind_workspace (256-byte aligned). */
 int vbx_plan(vbx_handle_t h, const int64_t *offsets_host, int32_t n_rec, int32_t R, int32_t S,
              size_t *workspace_bytes_out);

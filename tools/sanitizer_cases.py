@@ -1,6 +1,6 @@
 """Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection at
 D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
-6..64, per-recording state masks, AHC, hard labels, the dense forward_backward() and the ELBO trace.
+6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels, the dense forward_backward() and the ELBO trace.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
 """
@@ -17,10 +17,11 @@ from vbx_b200.batch import VbxBatch           # noqa: E402
 dev = torch.device('cuda:0')
 
 
-def run(lens, S, iters, D=None, ns=None, fb_split=0, eps=-float('inf'), tag=''):
+def run(lens, S, iters, D=None, ns=None, fb_split=0, eps=-float('inf'), tag='', gemm=0):
     d = synth.make_batch([t for t in lens if t], R=128, S=S, seed=3, D=D, dtype=np.float32)   # T = 0: no rows
     nsa = np.full(len(lens), S, dtype=np.int32) if ns is None else np.asarray(ns, dtype=np.int32)
     vb = VbxBatch(lens, 128, nsa, device=dev, fb_split=fb_split)
+    vb.set_option('gemm', gemm)
     Sp = vb.S
     g = torch.zeros((sum(lens), Sp), device=dev)
     g0 = d['gamma0'].copy()
@@ -57,6 +58,11 @@ run([300, 120, 64], 8, 30, eps=1e-5, tag='stop rule, float64 finish')
 run([513, 40], 31, 25, eps=1e-6, fb_split=2, tag='stop rule fused')
 run([0, 300, 45, 0, 129, 0], 8, 30, D=256, eps=1e-5, fb_split=2, tag='empty recordings fused')
 run([0, 300, 45, 0, 129, 0], 8, 30, D=256, eps=1e-5, fb_split=1, tag='empty recordings split')
+# S = 128 tier (always the split schedule): both contraction modes, per-recording masks, the float64 finish
+for gm in (0, 1):
+    run([513, 512, 1, 2, 300], 128, 2, ns=[128, 100, 65, 3, 1], gemm=gm, tag=f'S=128 masks gemm={gm}')
+    run([4100, 0, 300], 100, 2, D=256, gemm=gm, tag=f'S=128 long + empty gemm={gm}')
+    run([300, 120, 64], 100, 30, eps=1e-5, gemm=gm, tag=f'S=128 stop rule, float64 finish gemm={gm}')
 
 # wgmma projection at the smallest and largest D, one frame and one frame past a full wave of tiles
 sms = torch.cuda.get_device_properties(0).multi_processor_count

@@ -9,7 +9,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('VBX_B200_LIB', os.path.join(_HERE, 'libvbx_b200.so'))   # override: A/B builds
 
-EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_create', 'vbx_destroy', 'vbx_last_error',
+EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_create', 'vbx_destroy', 'vbx_last_error',
            'vbx_set_option', 'vbx_plan', 'vbx_bind_workspace', 'vbx_prepare_scale',
            'vbx_prepare_project', 'vbx_prepare_xvectors', 'vbx_run', 'vbx_hard_labels', 'vbx_ahc_workspace_bytes', 'vbx_ahc', 'vbx_launch_count', 'vbx_get_timings', 'vbx_f64_workspace_bytes',
            'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace', 'vbx_get_gsum']
@@ -39,6 +39,8 @@ def load():
     lib.vbx_version.argtypes = []
     lib.vbx_padded_states.restype = i32
     lib.vbx_padded_states.argtypes = [i32]
+    lib.vbx_padded_states_wide.restype = i32
+    lib.vbx_padded_states_wide.argtypes = [i32]
     lib.vbx_create.restype = ctypes.c_int
     lib.vbx_create.argtypes = [i32, ctypes.POINTER(vp)]
     lib.vbx_destroy.restype = ctypes.c_int
@@ -87,8 +89,11 @@ def load():
     return lib
 
 
+MAX_STATES = 128     # largest live state count of the float32 kernels (65 .. 128 pad to the S = 128 tier)
+
+
 def padded_states(n):
-    s = load().vbx_padded_states(int(n))
+    s = load().vbx_padded_states_wide(int(n))
     if s < 0:
-        raise VbxError(f'unsupported number of HMM states {n} (1..64)')
+        raise VbxError(f'unsupported number of HMM states {n} (1..{MAX_STATES})')
     return s

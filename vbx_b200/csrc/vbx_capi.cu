@@ -143,7 +143,7 @@ size_t carve(const vbx::Plan &pl, void *base, vbx::Workspace *ws) {
     w.prev_elbo = c.take<double>(B);
     w.active = c.take<int32_t>(B);
     w.tile_done = c.take<int32_t>(B);
-    w.scratch = c.take<float>(2 * vbx::kMaxS);
+    w.scratch = c.take<float>(2 * std::max<size_t>(S, vbx::kMaxS));
     if (pl.R == 128) w.tc_scratch = c.take<float>(vbx::tc_scratch_floats());
     if (pl.split) {
         w.ahat = c.take<float>(N * S);
@@ -194,6 +194,11 @@ int32_t vbx_padded_states(int32_t n) {
     int32_t s = 4;
     while (s < n) s <<= 1;
     return s;
+}
+
+int32_t vbx_padded_states_wide(int32_t n) {
+    if (n > vbx::kMaxS && n <= vbx::kMaxSWide) return vbx::kMaxSWide;
+    return vbx_padded_states(n);
 }
 
 int vbx_create(int32_t device, vbx_handle_t *out) {
@@ -316,8 +321,11 @@ int vbx_plan(vbx_handle_t h, const int64_t *offsets_host, int32_t n_rec, int32_t
              size_t *workspace_bytes_out) {
     if (!h || !offsets_host || n_rec < 0) return fail(h, VBX_ERR_ARG, "vbx_plan: null argument");
     if (R < 4 || R > vbx::kMaxR || (R & 3)) return fail(h, VBX_ERR_ARG, "vbx_plan: R must be a multiple of 4 in [4,128]");
-    if (S != 4 && S != 8 && S != 16 && S != 32 && S != 64)
-        return fail(h, VBX_ERR_ARG, "vbx_plan: S must come from vbx_padded_states()");
+    if (S != 4 && S != 8 && S != 16 && S != 32 && S != 64 && S != vbx::kMaxSWide)
+        return fail(h, VBX_ERR_ARG, "vbx_plan: S must come from vbx_padded_states() or vbx_padded_states_wide()");
+    if (S == vbx::kMaxSWide && h->opt_fb_split == 2)
+        return fail(h, VBX_ERR_ARG, "vbx_plan: S = 128 plans always take the split forward-backward schedule (there is no fused "
+                                    "sweep at 128 states), so option fb_split = 2 (never) cannot be honoured");
     if (n_rec > 0 && offsets_host[0] != 0) return fail(h, VBX_ERR_ARG, "vbx_plan: offsets[0] must be 0");
     for (int b = 0; b < n_rec; ++b) {
         const int64_t T = offsets_host[b + 1] - offsets_host[b];
@@ -352,9 +360,9 @@ int vbx_plan(vbx_handle_t h, const int64_t *offsets_host, int32_t n_rec, int32_t
     mbegin[n_rec] = (int32_t)mrec.size();
     // Few recordings cannot fill the GPU with one warp-group each: run the forward and the backward sweep of every
     // recording concurrently on separate warps (vbx_fb_split.cu).  Auto: when the sweeps of the fused kernel would occupy
-    // at most two warps per SM.
-    bool split = h->opt_fb_split == 1;
-    if (h->opt_fb_split == 0) {
+    // at most two warps per SM.  S = 128 always splits (the fused sweep and the chunked scan stop at 64 states).
+    bool split = h->opt_fb_split == 1 || S == vbx::kMaxSWide;
+    if (h->opt_fb_split == 0 && !split) {
         const int spl = S >= 16 ? 2 : 1, rpw = 32 / (S / spl);
         const int warps = (n_rec + rpw - 1) / rpw;
         split = warps <= 2 * h->sms;
@@ -682,7 +690,8 @@ int vbx_run(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io,
                 if (rc) return rc;
             }
             // tensor-core M-step: the CTA finishing a recording's last tile also computes its speaker model (no extra launch)
-            const bool fold = !given && !h->opt_gemm && h->opt_fold_speaker;
+            // (not at S = 128: the M-step's two warp groups do not match the 128-thread speaker-model tail)
+            const bool fold = !given && !h->opt_gemm && h->opt_fold_speaker && pl.S <= vbx::kMaxS;
             if (!given) {
                 Timed t(h, st, VBX_K_MSTEP);
                 rc = counted(h, h->opt_gemm ? vbx::launch_mstep_partial(pl, h->ws, rho, gamma_io, st)

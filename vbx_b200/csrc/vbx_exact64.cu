@@ -73,15 +73,18 @@ __global__ void __launch_bounds__(256) restore64_kernel(Plan pl, Workspace ws, f
 // ---------------------------------------------------------------------------------------------------------
 // M-step accumulation in float64: partial64[tile][s][r] = sum_t gamma[t,s] rho[t,r], occp64[tile][s] = sum_t gamma
 // 256 threads: r = tid % 128, h = tid / 128 takes the frames of parity h; gamma is staged per 64-frame block in
-// shared memory and read as broadcast float4.
+// shared memory and read as broadcast float4.  S = 128: h takes the states of half h instead (every frame), so that a
+// thread keeps 64 accumulators and the two halves need no reduction.
 // ---------------------------------------------------------------------------------------------------------
 template <int S_PAD>
 __global__ void __launch_bounds__(256) mstep64_kernel(Plan pl, Workspace ws, const float *__restrict__ rho,
                                                       const float *__restrict__ gamma) {
     constexpr int FB = 64;
+    constexpr bool HALVES = S_PAD > kMaxS;
+    constexpr int SA = HALVES ? S_PAD / 2 : S_PAD;   // accumulators per thread
     __shared__ __align__(16) float gs[FB][S_PAD];
     __shared__ double occs[S_PAD];
-    extern __shared__ double red[];   // [S_PAD][kMaxR] reduction of the two frame parities
+    extern __shared__ double red[];   // [S_PAD][kMaxR] reduction of the two frame parities (not used with HALVES)
     const int tile = blockIdx.x;
     const int rec = pl.mtile_rec[tile];
     if (!ws.active64[rec]) return;
@@ -90,9 +93,9 @@ __global__ void __launch_bounds__(256) mstep64_kernel(Plan pl, Workspace ws, con
     const int R = pl.R;
     const int tid = threadIdx.x, r = tid & 127, h = tid >> 7;
     const bool rlive = r < R;
-    double acc[S_PAD];
+    double acc[SA];
 #pragma unroll
-    for (int s = 0; s < S_PAD; ++s) acc[s] = 0.0;
+    for (int s = 0; s < SA; ++s) acc[s] = 0.0;
     double occ = 0.0;
     for (int b0 = 0; b0 < len; b0 += FB) {
         const int bl = min(FB, len - b0);
@@ -110,12 +113,14 @@ __global__ void __launch_bounds__(256) mstep64_kernel(Plan pl, Workspace ws, con
         }
         if (rlive) {
             const float *xr = rho + (f0 + b0) * R + r;
+            constexpr int FSTEP = HALVES ? 1 : 2;
+            const int s0 = HALVES ? h * SA : 0;
 #pragma unroll 2
-            for (int f = h; f < bl; f += 2) {
+            for (int f = HALVES ? 0 : h; f < bl; f += FSTEP) {
                 const double x = (double)__ldg(xr + (int64_t)f * R);
 #pragma unroll
-                for (int q = 0; q < S_PAD / 4; ++q) {
-                    const float4 g = *reinterpret_cast<const float4 *>(&gs[f][4 * q]);
+                for (int q = 0; q < SA / 4; ++q) {
+                    const float4 g = *reinterpret_cast<const float4 *>(&gs[f][s0 + 4 * q]);
                     acc[4 * q + 0] = fma((double)g.x, x, acc[4 * q + 0]);
                     acc[4 * q + 1] = fma((double)g.y, x, acc[4 * q + 1]);
                     acc[4 * q + 2] = fma((double)g.z, x, acc[4 * q + 2]);
@@ -124,6 +129,14 @@ __global__ void __launch_bounds__(256) mstep64_kernel(Plan pl, Workspace ws, con
             }
         }
     }
+    if constexpr (HALVES) {
+        if (rlive) {
+            double *out = ws.partial64 + (int64_t)tile * S_PAD * R;
+#pragma unroll
+            for (int s = 0; s < SA; ++s) out[(int64_t)(h * SA + s) * R + r] = acc[s];
+        }
+        if (tid < S_PAD) ws.occp64[(int64_t)tile * S_PAD + tid] = occ;
+    } else {
     if (tid < S_PAD) occs[tid] = occ;
     if (h == 1) {
 #pragma unroll
@@ -136,6 +149,7 @@ __global__ void __launch_bounds__(256) mstep64_kernel(Plan pl, Workspace ws, con
         for (int s = 0; s < S_PAD; ++s) out[(int64_t)s * R + r] = acc[s] + red[s * kMaxR + r];
     }
     if (tid < S_PAD) ws.occp64[(int64_t)tile * S_PAD + tid] = occs[tid];
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -193,12 +207,16 @@ __global__ void __launch_bounds__(128) speaker64_kernel(Plan pl, Workspace ws, R
 
 // ---------------------------------------------------------------------------------------------------------
 // log-likelihoods in float64.  One CTA per M-tile, processed in blocks of 64 frames: rho block transposed in
-// shared memory, alpha [r][s] in shared memory, warp = (state quarter, frame half), lane = frame.
+// shared memory, alpha [r][s] in shared memory, warp = (state quarter, frame half), lane = frame.  S = 128: blocks of 32
+// frames and warp = state eighth (the 64-frame layout would need 225 KB of shared memory).
 //   ll[t,s] = Fa (sum_r rho[t,r] alpha[s,r] - bias[s]);  rowmax; p64 = exp(ll - rowmax)       VBx/VBx.py:97
 // ---------------------------------------------------------------------------------------------------------
 template <int S_PAD>
+__host__ __device__ constexpr int loglik64_frames() { return S_PAD > kMaxS ? 32 : 64; }
+
+template <int S_PAD>
 __global__ void __launch_bounds__(256) loglik64_kernel(Plan pl, Workspace ws, RunParams rp, const float *__restrict__ rho) {
-    constexpr int FB = 64, SJ = S_PAD / 4 > 0 ? S_PAD / 4 : 1, NSG = S_PAD / SJ;
+    constexpr int FB = loglik64_frames<S_PAD>(), SJ = S_PAD > kMaxS ? S_PAD / 8 : (S_PAD / 4 > 0 ? S_PAD / 4 : 1), NSG = S_PAD / SJ;
     extern __shared__ double sm64[];
     const int R = pl.R;
     double *aS = sm64;                                   // [S_PAD][kMaxR]
@@ -497,10 +515,11 @@ template <int S_PAD>
 static int launch_exact64_t(const Plan &pl, const Workspace &ws, const RunParams &rp, const float *rho, const float *Phi,
                             float *gamma, float *pi, const int32_t *n_states, float *alpha_io, float *invL_io, double *Li,
                             int32_t *n_iters, int32_t *flags, cudaStream_t st) {
-    constexpr int SPL = S_PAD >= 16 ? 2 : 1;
+    constexpr int SPL = S_PAD > kMaxS ? 4 : (S_PAD >= 16 ? 2 : 1);
     constexpr int RPW = 32 / (S_PAD / SPL);
-    const size_t sm_m = (size_t)S_PAD * kMaxR * sizeof(double);
-    const size_t sm_l = (size_t)(kMaxR * S_PAD + 64 * S_PAD) * sizeof(double) + (size_t)kMaxR * 65 * sizeof(float);
+    constexpr int FB = x64::loglik64_frames<S_PAD>();
+    const size_t sm_m = S_PAD > kMaxS ? 0 : (size_t)S_PAD * kMaxR * sizeof(double);   // S = 128: no parity reduction
+    const size_t sm_l = (size_t)(kMaxR * S_PAD + FB * S_PAD) * sizeof(double) + (size_t)kMaxR * (FB + 1) * sizeof(float);
     static bool configured = false;
     if (!configured) {
         if (cudaFuncSetAttribute(x64::mstep64_kernel<S_PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_m) != cudaSuccess ||
@@ -530,6 +549,7 @@ int launch_exact64_round(const Plan &pl, const Workspace &ws, const RunParams &r
         case 16: VBX_X64(16);
         case 32: VBX_X64(32);
         case 64: VBX_X64(64);
+        case kMaxSWide: VBX_X64(kMaxSWide);
         default: return -1;
     }
 #undef VBX_X64

@@ -130,7 +130,7 @@ __global__ void __launch_bounds__(128) fb_sweeps_kernel(Plan pl, Workspace ws, R
     if (!backward) {
         // ---------------- forward sweep, VBx/VBx.py:164,167-168 (look-ahead recurrences, see vbx_kernels.cu) ----------------
         float *ah = live ? ws.ahat + f0 * S_PAD + l * SPL : ws.scratch + l * SPL;
-        float *rs = live ? ws.rsigma + f0 : ws.scratch + kMaxS;
+        float *rs = live ? ws.rsigma + f0 : ws.scratch + (S_PAD > kMaxS ? S_PAD : kMaxS);
         const int rstr = live ? 1 : 0;
         float y[SPL];
         const Vec<SPL> p0 = ldg_vec<SPL>(pp);
@@ -410,7 +410,7 @@ __global__ void __launch_bounds__(128) fb_split_tail_kernel(Plan pl, Workspace w
     const int ns = n_states ? n_states[rec] : S_PAD;
     const int64_t f0 = pl.offsets[rec];
     const int t_lo = pl.mtile_begin[rec], t_hi = pl.mtile_begin[rec + 1];
-    constexpr int SPLc = S_PAD > 32 ? 2 : 1;
+    constexpr int SPLc = S_PAD > 32 ? S_PAD / 32 : 1;
     const double Q = 1.0 - (double)rp.loopP;
     double pn[SPLc];
     float loc = 0.f;
@@ -480,6 +480,7 @@ int launch_forward_backward_split(const Plan &pl, const Workspace &ws, const Run
         case 64:
             if (spl == 4) VBX_SP(64, 4);
             VBX_SP(64, 2);
+        case 128: VBX_SP(128, 4);   // a lane group must fit in a warp: 32 lanes x 4 states
         default: return -1;
     }
 #undef VBX_SP

@@ -16,6 +16,9 @@ constexpr int kLongT = 4096;   // recordings at least this long take the chunked
 constexpr int kChunk = 256;    // frames per chunk of that scan
 constexpr int kMaxR = 128;
 constexpr int kMaxS = 64;
+// The wide tier: 65 .. 128 live states run as S = 128 plans, always on the split forward-backward schedule
+// (vbx_fb_split.cu).  Buffers sized by kMaxS keep their size for S <= 64; the S = 128 instantiations size theirs by S.
+constexpr int kMaxSWide = 128;
 constexpr int kTcMaxD = 2048;  // largest raw dimension of the tensor-core front end (bounds its scratch in the workspace)
 
 // Device-resident description of a planned batch (arrays owned by the handle).
@@ -76,7 +79,7 @@ struct Workspace {
     double *bias64 = nullptr;    // [n_rec,S]
     double *reg64 = nullptr;     // [n_rec]
     double *pi64 = nullptr;      // [n_rec,S]
-    float *scratch = nullptr;  // [2*kMaxS] write sink for warp lanes that own no recording
+    float *scratch = nullptr;  // [2*max(S,kMaxS)] write sink for warp lanes that own no recording
     // split forward-backward (vbx_fb_split.cu); null unless the plan chose it
     float *ahat = nullptr, *bhat = nullptr;   // [N,S] normalised forward variables / self-scaled backward variables
     float *socc = nullptr, *sent = nullptr;   // [n_mtiles,S] per-tile sums of gamma / of the re-entry terms of eq. (24)

@@ -309,7 +309,11 @@ __global__ void __launch_bounds__(256) mstep_partial_kernel(Plan pl, Workspace w
     constexpr int SPT = S_PAD < 16 ? S_PAD : 16;
     constexpr int NG = S_PAD / SPT;
     constexpr int FS = 8 / NG;
-    __shared__ __align__(16) float red[S_PAD][kMaxR];
+    // S = 128: the 64 KB reduction buffer exceeds the static limit and lives in dynamic shared memory
+    constexpr bool DYN = S_PAD > kMaxS;
+    __shared__ __align__(16) float red_st[DYN ? 1 : S_PAD][kMaxR];
+    extern __shared__ float4 red_dyn[];
+    float (*red)[kMaxR] = DYN ? reinterpret_cast<float (*)[kMaxR]>(red_dyn) : red_st;
     const int tile = blockIdx.x;
     const int rec = pl.mtile_rec[tile];
     if (!ws.active[rec]) return;
@@ -388,6 +392,17 @@ int launch_mstep_partial(const Plan &pl, const Workspace &ws, const float *rho, 
         case 16: mstep_partial_kernel<16><<<pl.n_mtiles, 256, 0, st>>>(pl, ws, rho, gamma); break;
         case 32: mstep_partial_kernel<32><<<pl.n_mtiles, 256, 0, st>>>(pl, ws, rho, gamma); break;
         case 64: mstep_partial_kernel<64><<<pl.n_mtiles, 256, 0, st>>>(pl, ws, rho, gamma); break;
+        case kMaxSWide: {   // 64 KB reduction buffer in dynamic shared memory
+            constexpr int smem = kMaxSWide * kMaxR * sizeof(float);
+            static bool configured = false;
+            if (!configured) {
+                if (cudaFuncSetAttribute(mstep_partial_kernel<kMaxSWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+                    return -1;
+                configured = true;
+            }
+            mstep_partial_kernel<kMaxSWide><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, gamma);
+            break;
+        }
         default: return -1;
     }
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
@@ -415,20 +430,24 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
     const float phi = live ? Phi[r] : 0.f;
     const int t_lo = pl.mtile_begin[rec], t_hi = pl.mtile_begin[rec + 1];
     extern __shared__ float sAv[];                       // [S8][kMaxR] Fa*alpha, staged for the coalesced fragment writes
-    __shared__ double cpart[kMaxS][4], rpart[kMaxS][4];
-    // all tile sums of this thread's speakers first (independent loads in flight), then the per-speaker math
-    double grs[NSP];
+    __shared__ double cpart[S8 > kMaxS ? S8 : kMaxS][4], rpart[S8 > kMaxS ? S8 : kMaxS][4];
+    // the tile sums of up to 16 of this thread's speakers first (independent loads in flight), then the per-speaker math
+    // (S = 128: two rounds of 16, which keeps the sums in registers)
+    constexpr int NCH = NSP < 16 ? NSP : 16;
 #pragma unroll
-    for (int k = 0; k < NSP; ++k) {
-        const int s = wg + 4 * k;
+    for (int k0 = 0; k0 < NSP; k0 += NCH) {
+    double grs[NCH];
+#pragma unroll
+    for (int k = 0; k < NCH; ++k) {
+        const int s = wg + 4 * (k0 + k);
         double gr = 0.0;
         if (live && s < ns && !from_given)
             for (int t = t_lo; t < t_hi; ++t) gr += (double)__ldg(ws.partial + ((int64_t)t * S + s) * R + r);
         grs[k] = gr;
     }
 #pragma unroll
-    for (int k = 0; k < NSP; ++k) {
-        const int s = wg + 4 * k;
+    for (int k = 0; k < NCH; ++k) {
+        const int s = wg + 4 * (k0 + k);
         const int64_t o = ((int64_t)rec * S + s) * R + r;
         const bool dead = s >= ns;   // dead (or padding) column: never wins, never contributes
         float invL = 1.f, alpha = 0.f, Av = 0.f;
@@ -463,6 +482,7 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
             rpart[s][warp] = (double)reg;
         }
     }
+    }
     __syncthreads();
     if (threadIdx.x < S) {
         const int s = threadIdx.x;
@@ -495,12 +515,22 @@ int launch_speaker_model(const Plan &pl, const Workspace &ws, const RunParams &r
     const int S8 = pl.S > 8 ? pl.S : 8;
     const size_t smem = (size_t)S8 * kMaxR * sizeof(float);
     const int fg = from_given ? 1 : 0;
+    if (S8 == kMaxSWide) {   // 64 KB of staged Fa*alpha: above the default dynamic shared-memory limit
+        static bool configured = false;
+        if (!configured) {
+            if (cudaFuncSetAttribute(speaker_model_kernel<kMaxSWide, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
+                cudaFuncSetAttribute(speaker_model_kernel<kMaxSWide, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+                return -1;
+            configured = true;
+        }
+    }
 #define VBX_SM(S8_, R_) speaker_model_kernel<S8_, R_><<<pl.n_rec, 512, smem, st>>>(pl, ws, rp, Phi, n_states, alpha_io, invL_io, fg)
     if (pl.R == 128) {
         switch (S8) {
             case 8: VBX_SM(8, true); break;
             case 16: VBX_SM(16, true); break;
             case 32: VBX_SM(32, true); break;
+            case kMaxSWide: VBX_SM(kMaxSWide, true); break;
             default: VBX_SM(64, true); break;
         }
     } else {
@@ -508,6 +538,7 @@ int launch_speaker_model(const Plan &pl, const Workspace &ws, const RunParams &r
             case 8: VBX_SM(8, false); break;
             case 16: VBX_SM(16, false); break;
             case 32: VBX_SM(32, false); break;
+            case kMaxSWide: VBX_SM(kMaxSWide, false); break;
             default: VBX_SM(64, false); break;
         }
     }
@@ -640,6 +671,7 @@ int launch_loglik(const Plan &pl, const Workspace &ws, const float *rho, const f
         case 16: return launch_loglik_t<16>(pl, ws, rho, pi, n_states, loopP, st);
         case 32: return launch_loglik_t<32>(pl, ws, rho, pi, n_states, loopP, st);
         case 64: return launch_loglik_t<64>(pl, ws, rho, pi, n_states, loopP, st);
+        case kMaxSWide: return launch_loglik_t<kMaxSWide>(pl, ws, rho, pi, n_states, loopP, st);
         default: return -1;
     }
 }

@@ -136,19 +136,25 @@ __device__ __forceinline__ void speaker_model_tail(const Plan &pl, const Workspa
 }
 
 // FOLD: the CTA that finishes a recording's last tile also computes that recording's speaker model (no separate launch).
+// S = 128: two groups of four warps, one per half of the states, each tiled like S = 64; the 67 KB reduction buffer is
+// dynamic shared memory.  FOLD is not instantiated there (the speaker-model tail runs on 128 threads).
 template <int S_PAD, bool FOLD>
-__global__ void __launch_bounds__(128, 4) mstep_mma_kernel(Plan pl, Workspace ws, const float *__restrict__ rho,
-                                                           const float *__restrict__ gamma, RunParams rp,
-                                                           const float *__restrict__ Phi, const int32_t *__restrict__ n_states,
-                                                           float *alpha_io, float *invL_io) {
-    constexpr int MT = S_PAD > 16 ? S_PAD / 16 : 1;  // m-tiles of 16 states
+__global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 2 : 4)
+    mstep_mma_kernel(Plan pl, Workspace ws, const float *__restrict__ rho, const float *__restrict__ gamma, RunParams rp,
+                     const float *__restrict__ Phi, const int32_t *__restrict__ n_states, float *alpha_io, float *invL_io) {
+    constexpr int SH = S_PAD > kMaxS ? S_PAD / kMaxS : 1;  // state blocks, one warp group each
+    constexpr int SB = S_PAD / SH;                   // states of one warp group
+    constexpr int MT = SB > 16 ? SB / 16 : 1;        // m-tiles of 16 states
     constexpr int NTW = 16 / MT;                     // n-tiles (8 r each) per warp
     constexpr int RW = 8 * NTW;                      // r range of one warp
     constexpr int FS = 4 / MT;                       // frame slots
     constexpr int NQ = NTW / 4;                      // float4 per row per thread
     constexpr int S16 = 16 * MT;
     constexpr int LD = kMaxR + 4;
-    __shared__ __align__(16) float red[FS][S16][LD];
+    static_assert(!FOLD || SH == 1, "the folded speaker model needs one warp group");
+    __shared__ __align__(16) float red_st[SH > 1 ? 1 : FS][SH > 1 ? 1 : S16][LD];
+    extern __shared__ float4 red_dyn[];
+    float (*red)[S16 * SH][LD] = SH > 1 ? reinterpret_cast<float (*)[S16 * SH][LD]>(red_dyn) : reinterpret_cast<float (*)[S16 * SH][LD]>(red_st);
     const int tile = blockIdx.x;
     const int rec = pl.mtile_rec[tile];
     if (!ws.active[rec]) return;
@@ -156,10 +162,11 @@ __global__ void __launch_bounds__(128, 4) mstep_mma_kernel(Plan pl, Workspace ws
     const int len = (int)min((int64_t)kMTile, pl.offsets[rec + 1] - f0);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int g = lane >> 2, q = lane & 3;
-    const int rg = warp % MT, fs = warp / MT;
+    const int sh = SH > 1 ? warp >> 2 : 0, w4 = SH > 1 ? (warp & 3) : warp;
+    const int rg = w4 % MT, fs = w4 / MT;
     const int R = pl.R;
     const int col0 = rg * RW + 4 * g;
-    const float *grow = gamma + f0 * S_PAD;
+    const float *grow = gamma + f0 * S_PAD + sh * SB;
 
     float acc[MT][NTW][4];
 #pragma unroll
@@ -247,15 +254,15 @@ __global__ void __launch_bounds__(128, 4) mstep_mma_kernel(Plan pl, Workspace ws
 #pragma unroll
         for (int j = 0; j < NTW; ++j) {
             const int r0 = rg * RW + 32 * (j >> 2) + 8 * q + (j & 3), r1 = r0 + 4;   // n = 2q, 2q+1
-            red[fs][16 * m + g][r0] = acc[m][j][0];
-            red[fs][16 * m + g][r1] = acc[m][j][1];
-            red[fs][16 * m + g + 8][r0] = acc[m][j][2];
-            red[fs][16 * m + g + 8][r1] = acc[m][j][3];
+            red[fs][sh * S16 + 16 * m + g][r0] = acc[m][j][0];
+            red[fs][sh * S16 + 16 * m + g][r1] = acc[m][j][1];
+            red[fs][sh * S16 + 16 * m + g + 8][r0] = acc[m][j][2];
+            red[fs][sh * S16 + 16 * m + g + 8][r1] = acc[m][j][3];
         }
     __syncthreads();
     const int R4 = R >> 2;
     float *out = ws.partial + (int64_t)tile * S_PAD * R;
-    for (int i = threadIdx.x; i < S_PAD * R4; i += 128) {
+    for (int i = threadIdx.x; i < S_PAD * R4; i += 128 * SH) {
         const int s = i / R4, c4 = i - s * R4;
         float4 v = *reinterpret_cast<const float4 *>(&red[0][s][4 * c4]);
 #pragma unroll
@@ -268,7 +275,7 @@ __global__ void __launch_bounds__(128, 4) mstep_mma_kernel(Plan pl, Workspace ws
         }
         *reinterpret_cast<float4 *>(out + (int64_t)s * R + 4 * c4) = v;
     }
-    if (FOLD) {
+    if constexpr (FOLD) {
         // hand-over: the CTA that completes the recording's tile count sees every tile sum (fence + atomic, then L2 reads)
         __shared__ int s_last;
         __shared__ double cred[8];
@@ -283,7 +290,7 @@ __global__ void __launch_bounds__(128, 4) mstep_mma_kernel(Plan pl, Workspace ws
         __syncthreads();
         if (!s_last) return;
         __threadfence();
-        static_assert(sizeof(red) >= sizeof(float) * (S_PAD > 8 ? S_PAD : 8) * kMaxR, "speaker model reuses the reduction buffer");
+        static_assert(sizeof(red_st) >= sizeof(float) * (S_PAD > 8 ? S_PAD : 8) * kMaxR, "speaker model reuses the reduction buffer");
         const int ns = n_states ? n_states[rec] : S_PAD;
         if (R == 128)
             speaker_model_tail<S_PAD, true>(pl, ws, rp, Phi, rec, ns, alpha_io, invL_io, &red[0][0][0], cred);
@@ -305,6 +312,18 @@ int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, cons
         case 16: VBX_MS(16); break;
         case 32: VBX_MS(32); break;
         case 64: VBX_MS(64); break;
+        case kMaxSWide: {   // no folded speaker model at 128 states (vbx_run launches the speaker-model kernel)
+            constexpr int smem = kMaxSWide * (kMaxR + 4) * sizeof(float);
+            static bool configured = false;
+            if (!configured) {
+                if (cudaFuncSetAttribute(mstep_mma_kernel<kMaxSWide, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+                    return -1;
+                configured = true;
+            }
+            if (fold) return -1;
+            mstep_mma_kernel<kMaxSWide, false><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, gamma, rp, Phi, n_states, alpha_io, invL_io);
+            break;
+        }
         default: return -1;
     }
 #undef VBX_MS
@@ -323,11 +342,15 @@ int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, cons
 // WITH_C: also emit c_t = sum_j p[t,j] w_j (w = (1-loopP) pi + 1e-8), the reduction the split sweeps take out of their
 // recursion (vbx_fb_split.cu).  Costs ~14 % of this kernel's time on bandwidth-bound batches, so only plans that chose the
 // split sweeps (small batches) instantiate it.
+// S = 128 (split plans only, WITH_C): the staged fragments take 128 KB, one CTA per SM, so the CTA has 8 warps; the lo*hi /
+// hi*lo terms accumulate into D itself (16 n-tiles of separate E accumulators would not fit the register file).
 template <int S_PAD, bool R128, bool WITH_C>
-__global__ void __launch_bounds__(128, 3) loglik_mma_kernel(Plan pl, Workspace ws, const float *__restrict__ rho,
-                                                            const float *__restrict__ pi, const int32_t *__restrict__ n_states,
-                                                            const float Q) {
+__global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 1 : 3)
+    loglik_mma_kernel(Plan pl, Workspace ws, const float *__restrict__ rho, const float *__restrict__ pi,
+                      const int32_t *__restrict__ n_states, const float Q) {
     constexpr int NT = S_PAD > 8 ? S_PAD / 8 : 1;
+    constexpr int NW = S_PAD > kMaxS ? 8 : 4;      // warps per CTA
+    constexpr bool SPLIT_E = S_PAD <= kMaxS;       // separate accumulators for the small split terms
     extern __shared__ uint2 sfrag[];
     const int R = pl.R;
     const int KS = R128 ? 16 : (R + 7) >> 3;  // k-steps
@@ -344,7 +367,7 @@ __global__ void __launch_bounds__(128, 3) loglik_mma_kernel(Plan pl, Workspace w
         const int n16 = NT * KS * 32 / 2;  // 16-byte units per array
         const uint4 *gh = reinterpret_cast<const uint4 *>(ws.Afrag_hi + (int64_t)rec * NT * KS * 64);
         const uint4 *gl = reinterpret_cast<const uint4 *>(ws.Afrag_lo + (int64_t)rec * NT * KS * 64);
-        for (int i = tid; i < n16; i += 128) {
+        for (int i = tid; i < n16; i += 32 * NW) {
             cp_async16_(reinterpret_cast<uint4 *>(sBh) + i, gh + i);
             cp_async16_(reinterpret_cast<uint4 *>(sBl) + i, gl + i);
         }
@@ -363,10 +386,12 @@ __global__ void __launch_bounds__(128, 3) loglik_mma_kernel(Plan pl, Workspace w
     const int n_mt = (len + 15) >> 4;
 
     auto finish = [&](float (&D)[NT][4], const float (&E)[NT][4], const int mt) {
+        if constexpr (SPLIT_E) {
 #pragma unroll
-        for (int i = 0; i < NT; ++i)
+            for (int i = 0; i < NT; ++i)
 #pragma unroll
-            for (int e = 0; e < 4; ++e) D[i][e] += E[i][e];
+                for (int e = 0; e < 4; ++e) D[i][e] += E[i][e];
+        }
         float m0 = fmaxf(D[0][0], D[0][1]), m1 = fmaxf(D[0][2], D[0][3]);
 #pragma unroll
         for (int i = 1; i < NT; ++i) {
@@ -423,13 +448,19 @@ __global__ void __launch_bounds__(128, 3) loglik_mma_kernel(Plan pl, Workspace w
         for (int i = 0; i < NT; ++i) {
             const uint2 bh = sBh[(i * KS + j) * 32 + lane];
             const uint2 bl = sBl[(i * KS + j) * 32 + lane];
-            mma_tf32(E[i], al, bh.x, bh.y);
-            mma_tf32(D[i], ah, bh.x, bh.y);
-            mma_tf32(E[i], ah, bl.x, bl.y);
+            if constexpr (SPLIT_E) {
+                mma_tf32(E[i], al, bh.x, bh.y);
+                mma_tf32(D[i], ah, bh.x, bh.y);
+                mma_tf32(E[i], ah, bl.x, bl.y);
+            } else {
+                mma_tf32(D[i], al, bh.x, bh.y);
+                mma_tf32(D[i], ah, bl.x, bl.y);
+                mma_tf32(D[i], ah, bh.x, bh.y);
+            }
         }
     };
 
-    if (R128) {
+    if (R128 && SPLIT_E) {   // S = 128 takes the loop below: no room for a register copy of the two rows
         struct Raw {
             float4 xa[8], xb[8];
         };
@@ -466,20 +497,20 @@ __global__ void __launch_bounds__(128, 3) loglik_mma_kernel(Plan pl, Workspace w
             if (VBX_L2_PREFETCH && lane == 0 && mt * 16 + 16 <= len) prefetch_l2(rho + (f0 + mt * 16) * 128, 16 * 512);
         };
 #pragma unroll
-        for (int k = 1; k < PD; ++k) prefetch_mt(warp + 4 * k);
+        for (int k = 1; k < PD; ++k) prefetch_mt(warp + NW * k);
         Raw r0;
         load_mt(warp, r0);
         asm volatile("cp.async.wait_group 0;\n" ::: "memory");
         __syncthreads();
-        for (int mt = warp; mt < n_mt; mt += 4) {
-            prefetch_mt(mt + 4 * PD);
+        for (int mt = warp; mt < n_mt; mt += NW) {
+            prefetch_mt(mt + NW * PD);
             if (mt != warp) load_mt(mt, r0);
             compute(r0, mt);
         }
     } else {
         asm volatile("cp.async.wait_group 0;\n" ::: "memory");
         __syncthreads();
-        for (int mt = warp; mt < n_mt; mt += 4) {
+        for (int mt = warp; mt < n_mt; mt += NW) {
             float D[NT][4], E[NT][4];
 #pragma unroll
             for (int i = 0; i < NT; ++i) {
@@ -494,7 +525,9 @@ __global__ void __launch_bounds__(128, 3) loglik_mma_kernel(Plan pl, Workspace w
             const float *pb = rho + (f0 + rb) * R;
 #pragma unroll 4
             for (int j = 0; j < KS; ++j) {
-                const int col = KQ * q + 2 * j;           // columns >= R meet zero entries of the alpha fragments,
+                // columns of k-step j (R = 128: the coalesced permutation of the branch above)
+                const int col = R128 ? 16 * (j >> 1) + 4 * q + 2 * (j & 1) : KQ * q + 2 * j;
+                                                          // columns >= R meet zero entries of the alpha fragments,
                 const int cc = min(col, R - 2);           // so only the address needs clamping
                 const float2 va = __ldg(reinterpret_cast<const float2 *>(pa + cc));
                 const float2 vb = __ldg(reinterpret_cast<const float2 *>(pb + cc));
@@ -514,6 +547,22 @@ template <int S_PAD>
 static int launch_loglik_mma_t(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                                float loopP, cudaStream_t st) {
     static bool configured = false;
+    if constexpr (S_PAD > kMaxS) {   // split plans only (vbx_plan): the c_t variants, 8 warps per CTA
+        if (!configured) {
+            const int big = (int)loglik_mma_smem(S_PAD, kMaxR);
+            if (cudaFuncSetAttribute(loglik_mma_kernel<S_PAD, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
+                cudaFuncSetAttribute(loglik_mma_kernel<S_PAD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess)
+                return -1;
+            configured = true;
+        }
+        if (!pl.split) return -1;
+        const size_t smem = loglik_mma_smem(S_PAD, pl.R);
+        if (pl.R == 128)
+            loglik_mma_kernel<S_PAD, true, true><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, pi, n_states, 1.f - loopP);
+        else
+            loglik_mma_kernel<S_PAD, false, true><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, pi, n_states, 1.f - loopP);
+        return cudaGetLastError() == cudaSuccess ? 1 : -1;
+    } else {
     if (!configured) {
         const int big = (int)loglik_mma_smem(S_PAD, kMaxR);
         if (cudaFuncSetAttribute(loglik_mma_kernel<S_PAD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
@@ -537,6 +586,7 @@ static int launch_loglik_mma_t(const Plan &pl, const Workspace &ws, const float 
             loglik_mma_kernel<S_PAD, false, false><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states, Q);
     }
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
+    }
 }
 
 int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states, float loopP,
@@ -548,6 +598,7 @@ int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, con
         case 16: return launch_loglik_mma_t<16>(pl, ws, rho, pi, n_states, loopP, st);
         case 32: return launch_loglik_mma_t<32>(pl, ws, rho, pi, n_states, loopP, st);
         case 64: return launch_loglik_mma_t<64>(pl, ws, rho, pi, n_states, loopP, st);
+        case kMaxSWide: return launch_loglik_mma_t<kMaxSWide>(pl, ws, rho, pi, n_states, loopP, st);
         default: return -1;
     }
 }

@@ -13,6 +13,8 @@ host-side O(T) pass exactly like the reference's.  AHC itself (VBx/vbhmm.py:131-
 import numpy as np
 import torch
 
+from ._lib import MAX_STATES as MAX_STATES_F32
+
 
 def diagonalise_plda(plda_mu, plda_tr, plda_psi):
     """VBx/vbhmm.py:107-113: generalised eigen-problem B v = lambda W v; returns (mu, tr, psi) with psi descending."""
@@ -40,9 +42,9 @@ def plda_project(x, plda_mu, plda_tr, lda_dim):
     return ((x - plda_mu[None, :]) @ plda_tr.T)[:, :lda_dim]
 
 
-def soft_init(labels, n_states, smoothing):
+def soft_init(labels, n_states, smoothing, dtype=torch.float32):
     """VBx/vbhmm.py:150-152: qinit = softmax(onehot(labels) * smoothing) (rows), float32 on labels' device."""
-    q = torch.zeros((labels.shape[0], n_states), dtype=torch.float32, device=labels.device)
+    q = torch.zeros((labels.shape[0], n_states), dtype=dtype, device=labels.device)
     q.scatter_(1, labels.long()[:, None], float(smoothing))
     return torch.softmax(q, dim=1)
 
@@ -134,11 +136,41 @@ def diarize_recording(x_raw, seg_times, ahc_labels, transform, plda, Fa, Fb, loo
     return rttm_lines(recording, s, e, l), labels, g[:, :S]
 
 
+def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, **run_kw):
+    """The VB-HMM step (VBx/vbhmm.py:150-162) for the recordings of one state tier, packed: fea [N,R] float32, labels [N]
+    AHC labels (device).  f64: the float64 kernels (vbx_run_f64, any state count), else one float32 batch padded to the
+    tier.  Returns [(labels, second-best labels or None, iterations)] per recording."""
+    from .batch import VbxBatch, run_f64
+    offs = np.concatenate([[0], np.cumsum(lens)])
+    dt = torch.float64 if f64 else torch.float32
+    vb = VbxBatch(lens, int(fea.shape[1]), ns, device=dev, f64_only=f64)
+    g = torch.zeros((vb.N, vb.S), dtype=dt, device=dev)
+    p = torch.zeros((vb.B, vb.S), dtype=dt, device=dev)
+    for b in range(vb.B):              # VBx/vbhmm.py:150-152: qinit = softmax(onehot * smoothing)
+        g[offs[b]:offs[b + 1], :ns[b]] = soft_init(labels[offs[b]:offs[b + 1]], int(ns[b]), smoothing, dtype=dt)
+        p[b, :ns[b]] = 1.0 / ns[b]
+    if f64:
+        res = run_f64(vb, fea.double().contiguous(), Phi.double().contiguous(), g, p, **run_kw)   # VBx/vbhmm.py:154-158
+        top2 = [hard_labels(g[offs[b]:offs[b + 1], :ns[b]], second=True) for b in range(vb.B)]   # VBx/vbhmm.py:160-162
+        first, second = torch.cat([t[0] for t in top2]), torch.cat([t[1] for t in top2])
+    else:
+        vb.prepare_scale(fea, Phi)
+        res = vb.run(g, p, **run_kw)                                    # VBx/vbhmm.py:154-158
+        first, second = vb.hard_labels(g, second=True)                 # VBx/vbhmm.py:160-162
+    first, second = first.cpu().numpy().astype(np.int64), second.cpu().numpy().astype(np.int64)
+    iters = res['n_iters'].cpu().numpy().tolist()
+    vb.close()
+    return [(first[offs[b]:offs[b + 1]], second[offs[b]:offs[b + 1]] if ns[b] > 1 else None, int(iters[b]))
+            for b in range(len(lens))]
+
+
 def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
                   max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False):
-    """Every recording of an archive in ONE batch on the device - the body of the loop VBx/vbhmm.py:120-179 for all
-    recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors), AHC initialisation (vbx_ahc), the
-    VB-HMM with the reference's stop rule (vbx_run), hard labels (vbx_hard_labels); merging and RTTM lines on the host.
+    """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
+    recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
+    one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
+    per state tier (<= 64 and 65 .. 128 AHC clusters in float32, more than 128 on the float64 kernels, vbx_run_f64);
+    merging and RTTM lines on the host.
 
     recordings: {name: (x_raw [T,Dx] float array, seg_times [T,2])} in archive order.  transform = (mean1, mean2, lda),
     plda = (mu, tr, psi) as read from the Kaldi model (diagonalised here as VBx/vbhmm.py:107-113 does).
@@ -183,32 +215,27 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     iters = [0] * len(names)
     if init.endswith('VB'):
         ns = np.array([int(l.max()) + 1 if len(l) else 1 for l in ahc_labels], dtype=np.int32)
-        if ns.max() > 64:
-            bad = names[int(ns.argmax())]
-            raise ValueError(f'recording {bad!r}: AHC produced {int(ns.max())} clusters; the VB-HMM kernels hold at most 64 HMM states '
-                             '(raise --threshold, or run that recording with --init AHC)')
         R = int(fea.shape[1])
         pad = (-R) % 4
         if pad:                     # inert zero features (see api.VBx): labels do not depend on them
             fea = torch.cat([fea, torch.zeros((fea.shape[0], pad), device=dev)], dim=1).contiguous()
             Phi = torch.cat([Phi, torch.zeros(pad, device=dev)]).contiguous()
-        vb = VbxBatch(lens, R + pad, ns, device=dev)
         lab_d = torch.from_numpy(np.concatenate(ahc_labels)).to(dev)
-        g = torch.zeros((int(lens.sum()), vb.S), dtype=torch.float32, device=dev)
-        p = torch.zeros((len(names), vb.S), dtype=torch.float32, device=dev)
-        for b in range(len(names)):              # VBx/vbhmm.py:150-152: qinit = softmax(onehot * smoothing)
-            g[offs[b]:offs[b + 1], :ns[b]] = soft_init(lab_d[offs[b]:offs[b + 1]], int(ns[b]), smoothing)
-            p[b, :ns[b]] = 1.0 / ns[b]
-        vb.prepare_scale(fea, Phi)
-        res = vb.run(g, p, Fa=Fa, Fb=Fb, loopProb=loopP, maxIters=max_iters, epsilon=epsilon)     # VBx/vbhmm.py:154-158
-        first, second = vb.hard_labels(g, second=True)                     # VBx/vbhmm.py:160-162
-        first, second = first.cpu().numpy().astype(np.int64), second.cpu().numpy().astype(np.int64)
-        iters = res['n_iters'].cpu().numpy().tolist()
-        for b in range(len(names)):
-            labels1[b] = first[offs[b]:offs[b + 1]]
-            if ns[b] > 1:
-                labels2[b] = second[offs[b]:offs[b + 1]]
-        vb.close()
+        # VBx over-clusters in AHC and lets VB prune, so the state count varies by recording.  Each state tier is one
+        # batch: <= 64 states (planned exactly as in an archive without the larger recordings), 65 .. 128 (S = 128),
+        # more than 128 on the float64 kernels.  Padding every recording to the largest tier would multiply its bytes.
+        tiers = (ns <= 64, (ns > 64) & (ns <= MAX_STATES_F32), ns > MAX_STATES_F32)
+        for tier, sel in enumerate(tiers):
+            idx = np.nonzero(sel)[0]
+            if len(idx) == 0:
+                continue
+            rows = None if len(idx) == len(names) else \
+                torch.from_numpy(np.concatenate([np.arange(offs[b], offs[b + 1]) for b in idx])).to(dev)
+            pick = (lambda t: t) if rows is None else (lambda t: t.index_select(0, rows).contiguous())
+            sub = _vb_tier(lens[idx], ns[idx], pick(fea), Phi, pick(lab_d), tier == 2, smoothing, dev,
+                           Fa=Fa, Fb=Fb, loopProb=loopP, maxIters=max_iters, epsilon=epsilon)
+            for j, b in enumerate(idx):
+                labels1[b], labels2[b], iters[b] = sub[j]
     for b, n in enumerate(names):
         seg = np.asarray(recordings[n][1], dtype=np.float64)
         s, e, l = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels1[b])   # VBx/vbhmm.py:169
