@@ -139,6 +139,20 @@ int vbx_run(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io,
             float *alpha_io, float *invL_io, int32_t warm_start, double *Li_out, int32_t *n_iters_out,
             int32_t *flags_out, void *stream);
 
+/* vbx_run with per-recording hyperparameters: Fa, Fb and loop_prob are float64 DEVICE arrays [n_rec] (recording b runs
+ * with Fa[b], Fb[b], loop_prob[b]); every other argument and the stop rule are as in vbx_run.  One batch can so hold a
+ * whole hyperparameter grid (one entry per recording and setting) or recordings tuned for different domains.  A recording
+ * whose values equal vbx_run's scalars gets bit-identical results on the same plan and options.
+ * Null arrays return VBX_ERR_ARG.  The values are read on the device, so they are not validated: a recording whose
+ * values make its ELBO non-finite (Fb = 0, for example) ends with VBX_FLAG_NONFINITE, and the other recordings of the
+ * batch are not affected.  Option "graph": the identity of a call covers the three array POINTERS, not their contents;
+ * the arrays are read inside the replayed launch sequence, so a replay uses their contents at the time it runs (change
+ * them in place on `stream` between calls and the replay sees the new values).  vbx_run_f64 has no per-recording form. */
+int vbx_run_per_recording(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io, float *pi_io,
+                          const int32_t *n_states, const double *Fa, const double *Fb, const double *loop_prob,
+                          int32_t max_iters, double epsilon, float *alpha_io, float *invL_io, int32_t warm_start,
+                          double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream);
+
 /* AHC initialisation, VBx/vbhmm.py:131-146, for every recording of the planned batch, in float64 like the reference:
  *   cosine similarity of the recording's rows of x (VBx/diarization_lib.py:190-213; x [N,dim], float32 or float64),
  *   thr_out[b] = twoGMMcalib_lin(similarities)[0] (VBx/diarization_lib.py:13-31, 20 iterations),

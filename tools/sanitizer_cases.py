@@ -17,7 +17,7 @@ from vbx_b200.batch import VbxBatch           # noqa: E402
 dev = torch.device('cuda:0')
 
 
-def run(lens, S, iters, D=None, ns=None, fb_split=0, eps=-float('inf'), tag='', gemm=0):
+def run(lens, S, iters, D=None, ns=None, fb_split=0, eps=-float('inf'), tag='', gemm=0, per_rec=False):
     d = synth.make_batch([t for t in lens if t], R=128, S=S, seed=3, D=D, dtype=np.float32)   # T = 0: no rows
     nsa = np.full(len(lens), S, dtype=np.int32) if ns is None else np.asarray(ns, dtype=np.int32)
     vb = VbxBatch(lens, 128, nsa, device=dev, fb_split=fb_split)
@@ -37,7 +37,12 @@ def run(lens, S, iters, D=None, ns=None, fb_split=0, eps=-float('inf'), tag='', 
         vb.prepare_project(torch.from_numpy(d['X']).to(dev), torch.from_numpy(d['V']).to(dev), torch.from_numpy(d['Phi']).to(dev))
     else:
         vb.prepare_scale(torch.from_numpy(d['fea']).to(dev), torch.from_numpy(d['Phi']).to(dev))
-    out = vb.run(g, p, Fa=0.3, Fb=17.0, loopProb=0.99, maxIters=iters, epsilon=eps, return_model=True)
+    hp = dict(Fa=0.3, Fb=17.0, loopProb=0.99)
+    if per_rec:      # per-recording hyperparameters (vbx_run_per_recording): the recipe settings in turn
+        rec = [(0.3, 17.0, 0.99), (0.4, 64.0, 0.65), (0.2, 6.0, 0.35), (0.4, 17.0, 0.40)]
+        hp = {k: torch.tensor([rec[b % 4][i] for b in range(len(lens))], dtype=torch.float64, device=dev)
+              for i, k in enumerate(('Fa', 'Fb', 'loopProb'))}
+    out = vb.run(g, p, maxIters=iters, epsilon=eps, return_model=True, **hp)
     lab = vb.hard_labels(g, second=True)
     tr = vb.elbo_trace(out['Li'])
     torch.cuda.synchronize()
@@ -63,6 +68,11 @@ for gm in (0, 1):
     run([513, 512, 1, 2, 300], 128, 2, ns=[128, 100, 65, 3, 1], gemm=gm, tag=f'S=128 masks gemm={gm}')
     run([4100, 0, 300], 100, 2, D=256, gemm=gm, tag=f'S=128 long + empty gemm={gm}')
     run([300, 120, 64], 100, 30, eps=1e-5, gemm=gm, tag=f'S=128 stop rule, float64 finish gemm={gm}')
+# per-recording Fa / Fb / loopP on every schedule, with the float64 finish
+run([300, 45, 1, 129, 600], 16, 30, fb_split=1, eps=1e-5, per_rec=True, tag='per-recording split')
+run([300, 45, 1, 129, 600], 16, 30, fb_split=2, eps=1e-5, per_rec=True, tag='per-recording fused')
+run([4100, 300, 5000, 64], 8, 30, fb_split=2, eps=1e-5, per_rec=True, tag='per-recording chunked scan')
+run([513, 512, 1, 2, 300], 128, 30, ns=[128, 100, 65, 3, 1], eps=1e-5, per_rec=True, tag='per-recording S=128')
 
 # wgmma projection at the smallest and largest D, one frame and one frame past a full wave of tiles
 sms = torch.cuda.get_device_properties(0).multi_processor_count

@@ -11,7 +11,7 @@ LIB_PATH = os.environ.get('VBX_B200_LIB', os.path.join(_HERE, 'libvbx_b200.so'))
 
 EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_create', 'vbx_destroy', 'vbx_last_error',
            'vbx_set_option', 'vbx_plan', 'vbx_bind_workspace', 'vbx_prepare_scale',
-           'vbx_prepare_project', 'vbx_prepare_xvectors', 'vbx_run', 'vbx_hard_labels', 'vbx_ahc_workspace_bytes', 'vbx_ahc', 'vbx_launch_count', 'vbx_get_timings', 'vbx_f64_workspace_bytes',
+           'vbx_prepare_project', 'vbx_prepare_xvectors', 'vbx_run', 'vbx_run_per_recording', 'vbx_hard_labels', 'vbx_ahc_workspace_bytes', 'vbx_ahc', 'vbx_launch_count', 'vbx_get_timings', 'vbx_f64_workspace_bytes',
            'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace', 'vbx_get_gsum']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
@@ -69,6 +69,8 @@ def load():
     lib.vbx_prepare_xvectors.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.vbx_run.restype = ctypes.c_int
     lib.vbx_run.argtypes = [vp, vp, vp, vp, vp, vp, dbl, dbl, dbl, i32, dbl, vp, vp, i32, vp, vp, vp, vp]
+    lib.vbx_run_per_recording.restype = ctypes.c_int
+    lib.vbx_run_per_recording.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, dbl, vp, vp, i32, vp, vp, vp, vp]
     lib.vbx_launch_count.restype = i64
     lib.vbx_launch_count.argtypes = [vp]
     lib.vbx_f64_workspace_bytes.restype = ctypes.c_int

@@ -75,17 +75,22 @@ def ahc_batch(vb, x, threshold=-0.015, workspace=None):
     vb._check(vb.lib.vbx_ahc(vb._h, ptr(x), int(x.dtype == torch.float64), int(x.shape[1]), ptr(workspace),
                              workspace.numel(), ptr(Z), ptr(thr), vb._stream()))
     Zh, th = Z.cpu().numpy(), thr.cpu().numpy()       # 32 B per x-vector leave the device
-    labels, Zs = [], []
-    for b in range(vb.B):
-        o0, o1 = int(vb.offsets[b]), int(vb.offsets[b + 1])
-        Zb = Zh[o0:o1 - 1] if o1 > o0 else Zh[0:0]
-        Zs.append(Zb)
-        if o1 - o0 == 0:
+    Zs = [Zh[int(vb.offsets[b]):int(vb.offsets[b + 1]) - 1] if vb.offsets[b + 1] > vb.offsets[b] else Zh[0:0]
+          for b in range(vb.B)]
+    return cut(Zs, th, vb.lengths, threshold), th, Zs
+
+
+def cut(Zs, th, lengths, threshold):
+    """VBx/vbhmm.py:144-146 for every recording: the 0-based flat clusters of linkage Zs[b] at the calibrated threshold
+    th[b] shifted by `threshold`.  Host work only, so a threshold sweep repeats this and nothing else."""
+    labels = []
+    for b, T in enumerate(lengths):
+        if T == 0:
             labels.append(np.zeros(0, dtype=np.int64))
-        elif o1 - o0 == 1:
+        elif T == 1:
             labels.append(np.zeros(1, dtype=np.int64))
         else:
             # a degenerate calibration (NaN threshold, e.g. two x-vectors) leaves every x-vector on its own, exactly
             # what the reference's fcluster call does with a NaN cut
-            labels.append(flat_clusters(Zb, -(th[b] + threshold)).astype(np.int64) - 1)
-    return labels, th, Zs
+            labels.append(flat_clusters(Zs[b], -(th[b] + threshold)).astype(np.int64) - 1)
+    return labels

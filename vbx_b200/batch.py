@@ -232,9 +232,43 @@ class VbxBatch:
                     flags=torch.empty(self.B, dtype=torch.int32, device=dev))
 
     # ---- VBx/VBx.py:91-125 ----------------------------------------------------------------
+    def _hyper(self, Fa, Fb, loopProb):
+        """None when Fa, Fb and loopProb are all numbers, else the three as float64 CUDA tensors [B] (numbers broadcast),
+        checked on the host: the library reads per-recording values on the device and cannot validate them, so the
+        check copies them to the host and a per-recording run() waits for the device's current stream.  A broadcast
+        number keeps its tensor between calls (stable pointers: option 'graph' can replay the run)."""
+        vals = dict(Fa=Fa, Fb=Fb, loopProb=loopProb)
+        if not any(isinstance(v, torch.Tensor) for v in vals.values()):
+            return None
+        out = []
+        for name, v in vals.items():
+            if isinstance(v, torch.Tensor):
+                if not (v.dtype == torch.float64 and v.device == self.device and tuple(v.shape) == (self.B,)):
+                    raise ValueError(f'{name}: expected a float64 tensor of shape ({self.B},) on {self.device}, got '
+                                     f'{v.dtype} {tuple(v.shape)} on {v.device}')
+                t = v.contiguous()
+            else:
+                cache = self.__dict__.setdefault('_broadcast', {})
+                if (name, float(v)) not in cache:
+                    cache[(name, float(v))] = torch.full((self.B,), float(v), dtype=torch.float64, device=self.device)
+                t = cache[(name, float(v))]
+            out.append(t)
+        Fa_t, Fb_t, lp_t = out
+        host = torch.stack(out).cpu()
+        if not bool(torch.isfinite(host).all()):
+            raise ValueError('Fa, Fb and loopProb must be finite')
+        if bool((host[1] == 0).any()):
+            raise ValueError('Fb must be non-zero')
+        if bool(((host[2] < 0) | (host[2] > 1)).any()):
+            raise ValueError('loopProb must lie in [0, 1]')
+        return Fa_t, Fb_t, lp_t
+
     def run(self, gamma, pi, Fa=1.0, Fb=1.0, loopProb=0.9, maxIters=10, epsilon=1e-4,
             alpha=None, invL=None, warm_start=False, return_model=False, buffers=None):
         """gamma [N,S] and pi [B,S] float32 CUDA tensors, updated IN PLACE (padded columns must be 0).
+        Fa, Fb, loopProb: numbers for the whole batch, or any of them a float64 CUDA tensor [B] of per-recording values
+        (vbx_run_per_recording; numbers are then broadcast).  A recording gets bit-identical results either way.  The
+        per-recording values are validated on the host, so such a call synchronises with the current stream.
         Returns dict(gamma, pi, Li [B,maxIters] float64 (NaN padded), n_iters [B], flags [B][, alpha, invL]).
         buffers: optional dict(Li, n_iters, flags) of preallocated output tensors (see `output_buffers`)."""
         if self.rho is None:
@@ -256,11 +290,19 @@ class VbxBatch:
             Li = torch.empty((self.B, max(int(maxIters), 1)), dtype=torch.float64, device=dev)
             n_iters = torch.empty(self.B, dtype=torch.int32, device=dev)
             flags = torch.empty(self.B, dtype=torch.int32, device=dev)
-        self._check(self.lib.vbx_run(
-            self._h, _ptr(self.rho), _ptr(self.Phi), _ptr(gamma), _ptr(pi), _ptr(self.n_states),
-            float(Fa), float(Fb), float(loopProb), int(maxIters), float(epsilon),
-            _ptr(alpha), _ptr(invL), int(bool(warm_start)), _ptr(Li), _ptr(n_iters), _ptr(flags),
-            self._stream()))
+        hyper = self._hyper(Fa, Fb, loopProb)
+        if hyper is None:
+            self._check(self.lib.vbx_run(
+                self._h, _ptr(self.rho), _ptr(self.Phi), _ptr(gamma), _ptr(pi), _ptr(self.n_states),
+                float(Fa), float(Fb), float(loopProb), int(maxIters), float(epsilon),
+                _ptr(alpha), _ptr(invL), int(bool(warm_start)), _ptr(Li), _ptr(n_iters), _ptr(flags),
+                self._stream()))
+        else:
+            self._check(self.lib.vbx_run_per_recording(
+                self._h, _ptr(self.rho), _ptr(self.Phi), _ptr(gamma), _ptr(pi), _ptr(self.n_states),
+                *(_ptr(t) for t in hyper), int(maxIters), float(epsilon),
+                _ptr(alpha), _ptr(invL), int(bool(warm_start)), _ptr(Li), _ptr(n_iters), _ptr(flags),
+                self._stream()))
         out = dict(gamma=gamma, pi=pi, Li=Li[:, :int(maxIters)], n_iters=n_iters, flags=flags)
         if return_model or warm_start:
             out.update(alpha=alpha, invL=invL)

@@ -179,6 +179,7 @@ size_t carve(const vbx::Plan &pl, void *base, vbx::Workspace *ws) {
         w.reg64 = c.take<double>(B);
         w.pi64 = c.take<double>(B * S);
     }
+    w.hp = c.take<vbx::RecParams>(B);
     if (ws) *ws = w;
     return c.off + 256;
 }
@@ -634,33 +635,31 @@ int vbx_prepare_xvectors(vbx_handle_t h, const float *x_raw, int32_t Dx, const f
     return VBX_OK;
 }
 
-int vbx_run(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io, float *pi_io,
-            const int32_t *n_states, double Fa, double Fb, double loop_prob, int32_t max_iters, double epsilon,
-            float *alpha_io, float *invL_io, int32_t warm_start, double *Li_out, int32_t *n_iters_out,
-            int32_t *flags_out, void *stream) {
-    Range nvtx_range("vbx_run");
-    int rc = check_ready(h, "vbx_run");
+}  // extern "C"
+
+// vbx_run (per_rec = false: the scalars Fa, Fb, loop_prob hold for every recording) and vbx_run_per_recording (per_rec:
+// device arrays Fa_v, Fb_v, loopP_v [n_rec]); run_init_kernel turns either into the per-recording table the kernels read.
+static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *rho, const float *Phi, float *gamma_io, float *pi_io,
+                    const int32_t *n_states, double Fa, double Fb, double loop_prob, const double *Fa_v, const double *Fb_v,
+                    const double *loopP_v, int32_t max_iters, double epsilon, float *alpha_io, float *invL_io,
+                    int32_t warm_start, double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream) {
+    Range nvtx_range(who);
+    const std::string w(who);
+    int rc = check_ready(h, who);
     if (rc) return rc;
     DeviceGuard guard(h->device);
     if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
-    if (!h->prepared) return fail(h, VBX_ERR_STATE, "vbx_run: call vbx_prepare_scale/project first (G is part of the ELBO)");
-    if (max_iters < 0) return fail(h, VBX_ERR_ARG, "vbx_run: max_iters < 0");
-    if (!(Fb != 0.0)) return fail(h, VBX_ERR_ARG, "vbx_run: Fb must be non-zero");
-    if (warm_start && (!alpha_io || !invL_io)) return fail(h, VBX_ERR_ARG, "vbx_run: warm_start needs alpha_io and invL_io");
+    if (!h->prepared) return fail(h, VBX_ERR_STATE, w + ": call vbx_prepare_scale/project first (G is part of the ELBO)");
+    if (max_iters < 0) return fail(h, VBX_ERR_ARG, w + ": max_iters < 0");
+    if (!per_rec && !(Fb != 0.0)) return fail(h, VBX_ERR_ARG, w + ": Fb must be non-zero");
+    if (per_rec && (!Fa_v || !Fb_v || !loopP_v)) return fail(h, VBX_ERR_ARG, w + ": Fa, Fb and loop_prob must be device arrays [n_rec]");
+    if (warm_start && (!alpha_io || !invL_io)) return fail(h, VBX_ERR_ARG, w + ": warm_start needs alpha_io and invL_io");
     const vbx::Plan &pl = h->plan;
     if (pl.n_rec == 0) return VBX_OK;
-    if (!Li_out || !n_iters_out || !flags_out || !pi_io) return fail(h, VBX_ERR_ARG, "vbx_run: null output pointer");
-    if (pl.n_frames && (!rho || !Phi || !gamma_io)) return fail(h, VBX_ERR_ARG, "vbx_run: null pointer");
+    if (!Li_out || !n_iters_out || !flags_out || !pi_io) return fail(h, VBX_ERR_ARG, w + ": null output pointer");
+    if (pl.n_frames && (!rho || !Phi || !gamma_io)) return fail(h, VBX_ERR_ARG, w + ": null pointer");
     vbx::RunParams rp;
-    rp.dFa = Fa;
-    rp.dFb = Fb;
-    rp.dFaFb = Fa / Fb;
     rp.epsilon = epsilon;
-    rp.Fa = (float)Fa;
-    rp.Fb = (float)Fb;
-    rp.FaFb = (float)(Fa / Fb);
-    rp.loopP = (float)loop_prob;
-    rp.dloopP = loop_prob;
     rp.max_iters = max_iters;
     // epsilon = -inf (fixed iteration count) and NaN never stop: nothing to decide, everything stays float32
     rp.hybrid = (pl.exact && epsilon > -1e300 && epsilon < 1e300 && max_iters > 1) ? 1 : 0;
@@ -673,7 +672,8 @@ int vbx_run(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io,
     int rc = 0;
     {
         Timed t(h, st, VBX_K_RUN_INIT);
-        rc = counted(h, vbx::launch_run_init(pl, h->ws, gamma_io, n_states, Li_out, n_iters_out, flags_out, max_iters, st), "run_init");
+        rc = counted(h, vbx::launch_run_init(pl, h->ws, gamma_io, n_states, Li_out, n_iters_out, flags_out, max_iters, Fa, Fb,
+                                             loop_prob, Fa_v, Fb_v, loopP_v, st), "run_init");
     }
     if (rc) return rc;
     // With the float64 finishing phase a recording that switched lags one round behind (it redoes two iterations):
@@ -695,17 +695,17 @@ int vbx_run(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io,
             if (!given) {
                 Timed t(h, st, VBX_K_MSTEP);
                 rc = counted(h, h->opt_gemm ? vbx::launch_mstep_partial(pl, h->ws, rho, gamma_io, st)
-                                            : vbx::launch_mstep_mma(pl, h->ws, rho, gamma_io, fold, rp, Phi, n_states, alpha_io, invL_io, st), "mstep_partial");
+                                            : vbx::launch_mstep_mma(pl, h->ws, rho, gamma_io, fold, Phi, n_states, alpha_io, invL_io, st), "mstep_partial");
             }
             if (rc) return rc;
             if (!fold) {
                 Timed t(h, st, VBX_K_SPEAKER_MODEL);
-                rc = counted(h, vbx::launch_speaker_model(pl, h->ws, rp, Phi, n_states, alpha_io, invL_io, given, st), "speaker_model");
+                rc = counted(h, vbx::launch_speaker_model(pl, h->ws, Phi, n_states, alpha_io, invL_io, given, st), "speaker_model");
             }
             if (rc) return rc;
             {
                 Timed t(h, st, VBX_K_LOGLIK);
-                rc = counted(h, h->opt_gemm ? vbx::launch_loglik(pl, h->ws, rho, pi_io, n_states, rp.loopP, st) : vbx::launch_loglik_mma(pl, h->ws, rho, pi_io, n_states, rp.loopP, st), "loglik");
+                rc = counted(h, h->opt_gemm ? vbx::launch_loglik(pl, h->ws, rho, pi_io, n_states, st) : vbx::launch_loglik_mma(pl, h->ws, rho, pi_io, n_states, st), "loglik");
             }
             if (rc) return rc;
             if (fb_hi) {   // the sweep on the high-priority side stream, ordered after the log-likelihoods and before the next M-step
@@ -743,7 +743,8 @@ int vbx_run(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io,
     auto bits = [](double d) { uint64_t u; memcpy(&u, &d, 8); return u; };
     for (const void *p : {(const void *)rho, (const void *)Phi, (const void *)gamma_io, (const void *)pi_io, (const void *)n_states,
                           (const void *)alpha_io, (const void *)invL_io, (const void *)Li_out, (const void *)n_iters_out,
-                          (const void *)flags_out, (const void *)h->ws.p})
+                          (const void *)flags_out, (const void *)h->ws.p, (const void *)Fa_v, (const void *)Fb_v,
+                          (const void *)loopP_v})
         mix((uint64_t)(uintptr_t)p);
     mix(bits(Fa)); mix(bits(Fb)); mix(bits(loop_prob)); mix(bits(epsilon)); mix((uint64_t)max_iters); mix((uint64_t)warm_start);
     if (key == 0) key = 1;
@@ -789,6 +790,24 @@ int vbx_run(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io,
     h->graph_key = key;
     h->graph_launches = h->launches - before;
     return replay();
+}
+
+extern "C" {
+
+int vbx_run(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io, float *pi_io,
+            const int32_t *n_states, double Fa, double Fb, double loop_prob, int32_t max_iters, double epsilon,
+            float *alpha_io, float *invL_io, int32_t warm_start, double *Li_out, int32_t *n_iters_out,
+            int32_t *flags_out, void *stream) {
+    return run_impl(h, "vbx_run", false, rho, Phi, gamma_io, pi_io, n_states, Fa, Fb, loop_prob, nullptr, nullptr, nullptr, max_iters,
+                    epsilon, alpha_io, invL_io, warm_start, Li_out, n_iters_out, flags_out, stream);
+}
+
+int vbx_run_per_recording(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io, float *pi_io,
+                          const int32_t *n_states, const double *Fa, const double *Fb, const double *loop_prob,
+                          int32_t max_iters, double epsilon, float *alpha_io, float *invL_io, int32_t warm_start,
+                          double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream) {
+    return run_impl(h, "vbx_run_per_recording", true, rho, Phi, gamma_io, pi_io, n_states, 0.0, 1.0, 0.0, Fa, Fb, loop_prob, max_iters,
+                    epsilon, alpha_io, invL_io, warm_start, Li_out, n_iters_out, flags_out, stream);
 }
 
 int vbx_hard_labels(vbx_handle_t h, const float *gamma, const int32_t *n_states, int32_t *first_out,

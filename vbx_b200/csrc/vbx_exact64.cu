@@ -178,8 +178,8 @@ __global__ void __launch_bounds__(128) speaker64_kernel(Plan pl, Workspace ws, R
                 if (live) gr += ws.partial64[((int64_t)t * S + s) * R + r];
             }
             if (live) {
-                iL = 1.0 / (1.0 + rp.dFaFb * Ns * phi);
-                a = rp.dFaFb * iL * gr;
+                iL = 1.0 / (1.0 + ws.hp[rec].dFaFb * Ns * phi);
+                a = ws.hp[rec].dFaFb * iL * gr;
                 c = (iL + a * a) * phi;
                 reg = log(iL) - iL - a * a + 1.0;
             }
@@ -202,7 +202,7 @@ __global__ void __launch_bounds__(128) speaker64_kernel(Plan pl, Workspace ws, R
             regsum += (sh[1][0] + sh[1][1]) + (sh[1][2] + sh[1][3]);
         }
     }
-    if (r == 0) ws.reg64[rec] = 0.5 * rp.dFb * regsum;
+    if (r == 0) ws.reg64[rec] = 0.5 * ws.hp[rec].dFb * regsum;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -256,7 +256,7 @@ __global__ void __launch_bounds__(256) loglik64_kernel(Plan pl, Workspace ws, Ru
             for (int j = 0; j < SJ; ++j) acc[j] = fma(x, ar[j * kMaxR], acc[j]);
         }
 #pragma unroll
-        for (int j = 0; j < SJ; ++j) llS[f * S_PAD + sg * SJ + j] = nb[j] < CUDART_INF ? rp.dFa * (acc[j] - nb[j]) : -CUDART_INF;
+        for (int j = 0; j < SJ; ++j) llS[f * S_PAD + sg * SJ + j] = nb[j] < CUDART_INF ? ws.hp[rec].dFa * (acc[j] - nb[j]) : -CUDART_INF;
         __syncthreads();
         if (tid < FB) {
             double m = -CUDART_INF;
@@ -321,7 +321,7 @@ __global__ void __launch_bounds__(128) fb64_kernel(Plan pl, Workspace ws, RunPar
     if (Tmax == 0) return;
     const int Tlast = max(T - 1, 0);
     const int ns = live ? (n_states ? n_states[rec] : S_PAD) : 0;
-    const double P = rp.dloopP, Q = 1.0 - rp.dloopP, eps = 1e-8;
+    const double P = rec >= 0 ? ws.hp[rec].dloopP : 0.0, Q = 1.0 - P, eps = 1e-8;
     double pi[SPL], w[SPL], base[SPL], a[SPL];
 #pragma unroll
     for (int k = 0; k < SPL; ++k) {
@@ -480,7 +480,7 @@ __global__ void __launch_bounds__(128) elbo64_kernel(Plan pl, Workspace ws, RunP
     if (lane == 0) part[warp] = acc;
     __syncthreads();
     if (tid == 0) {
-        const double elbo = (part[0] + part[1]) + (part[2] + part[3]) + rp.dFa * ws.gsum[rec] + ws.reg64[rec];
+        const double elbo = (part[0] + part[1]) + (part[2] + part[3]) + ws.hp[rec].dFa * ws.gsum[rec] + ws.reg64[rec];
         const int idx = n_iters[rec];
         Li[(int64_t)rec * rp.max_iters + idx] = elbo;
         n_iters[rec] = idx + 1;

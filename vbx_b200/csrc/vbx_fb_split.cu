@@ -111,7 +111,7 @@ __global__ void __launch_bounds__(128) fb_sweeps_kernel(Plan pl, Workspace ws, R
     if (Tmax == 0) return;  // warp-uniform: no live recording in this warp
     const int Tlast = max(T - 1, 0);
     const int ns = live ? (n_states ? n_states[rec] : S_PAD) : 0;
-    const float P = rp.loopP, Q = 1.f - rp.loopP;
+    const float P = rec >= 0 ? ws.hp[rec].loopP : 0.f, Q = 1.f - P;
     float pi[SPL], w[SPL];
 #pragma unroll
     for (int k = 0; k < SPL; ++k) {
@@ -315,7 +315,7 @@ __global__ void __launch_bounds__(256) fb_combine_kernel(Plan pl, Workspace ws, 
     const int ns = n_states ? n_states[rec] : S_PAD;
     const int tid = threadIdx.x;
     const int fl = tid / LPF, sc = tid % LPF;     // frame slot, state chunk
-    const float P = rp.loopP, Q = 1.f - rp.loopP;
+    const float P = ws.hp[rec].loopP, Q = 1.f - P;
     float w[SC];
 #pragma unroll
     for (int k = 0; k < SC; ++k) {
@@ -411,7 +411,7 @@ __global__ void __launch_bounds__(128) fb_split_tail_kernel(Plan pl, Workspace w
     const int64_t f0 = pl.offsets[rec];
     const int t_lo = pl.mtile_begin[rec], t_hi = pl.mtile_begin[rec + 1];
     constexpr int SPLc = S_PAD > 32 ? S_PAD / 32 : 1;
-    const double Q = 1.0 - (double)rp.loopP;
+    const double Q = 1.0 - (double)ws.hp[rec].loopP;
     double pn[SPLc];
     float loc = 0.f;
 #pragma unroll

@@ -45,6 +45,14 @@ struct Plan {
     const int32_t *lchunk_idx = nullptr;   // [n_lchunks] chunk number inside its recording
 };
 
+// The VB-HMM hyperparameters of one recording, derived from the double inputs by run_init_kernel exactly as vbx_run
+// derived its batch-wide scalars before they became per recording: a scalar run and a per-recording run with equal
+// values do bit-identical arithmetic.
+struct RecParams {
+    float Fa, Fb, FaFb, loopP;
+    double dFa, dFb, dFaFb, dloopP;
+};
+
 // Caller-provided workspace, carved by the handle.
 struct Workspace {
     float *p = nullptr;        // [N,S]  exp(ll - rowmax)
@@ -88,11 +96,12 @@ struct Workspace {
     float *fa_u = nullptr, *fa_lam = nullptr, *fa_exp = nullptr, *astart = nullptr;   // [LC,S,S], [LC,S] mantissa, [LC,S] exponent, [LC,S]
     float *bb_v = nullptr, *bb_mu = nullptr, *bb_exp = nullptr, *beta = nullptr;      // same shapes, backward sweep
     float *occp = nullptr, *entp = nullptr;                        // [n_lchunks,S]
+    RecParams *hp = nullptr;   // [n_rec]  hyperparameters, filled by run_init_kernel from the scalars or arrays of the call
 };
 
+// Batch-wide run settings (the hyperparameters Fa, Fb, loopP are per recording: Workspace::hp).
 struct RunParams {
-    float Fa, Fb, FaFb, loopP;
-    double dFa, dFb, dFaFb, dloopP, epsilon;
+    double epsilon;
     int32_t max_iters;
     // stop rule at float64 resolution (vbx_exact64.cu): a recording leaves the float32 kernels when its ELBO step is
     // below epsilon + guard_mult * nb, nb = noise_c * 2^-24 * |ELBO| (bound on the float32 noise of an ELBO difference)
@@ -180,13 +189,15 @@ int launch_prepare_scale(const Plan &pl, const Workspace &ws, const float *fea, 
                          cudaStream_t st);
 int launch_project_ffma(const Plan &pl, const float *X, int D, const float *V, float *rho, cudaStream_t st);
 int launch_g_from_rho(const Plan &pl, const Workspace &ws, const float *rho, const float *Phi, cudaStream_t st);
+// Fa_v / Fb_v / loopP_v: per-recording double arrays [n_rec] (any of them null: that parameter's scalar for every recording)
 int launch_run_init(const Plan &pl, const Workspace &ws, const float *gamma, const int32_t *n_states, double *Li,
-                    int32_t *n_iters, int32_t *flags, int max_iters, cudaStream_t st);
+                    int32_t *n_iters, int32_t *flags, int max_iters, double Fa, double Fb, double loopP,
+                    const double *Fa_v, const double *Fb_v, const double *loopP_v, cudaStream_t st);
 int launch_mstep_partial(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, cudaStream_t st);
-int launch_speaker_model(const Plan &pl, const Workspace &ws, const RunParams &rp, const float *Phi,
+int launch_speaker_model(const Plan &pl, const Workspace &ws, const float *Phi,
                          const int32_t *n_states, float *alpha_io, float *invL_io, bool from_given,
                          cudaStream_t st);
-int launch_loglik(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states, float loopP,
+int launch_loglik(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                   cudaStream_t st);
 int launch_forward_backward(const Plan &pl, const Workspace &ws, const RunParams &rp, float *gamma, float *pi,
                             const int32_t *n_states, double *Li, int32_t *n_iters, int32_t *flags, int iter,
@@ -199,9 +210,9 @@ int launch_forward_backward_split(const Plan &pl, const Workspace &ws, const Run
 int launch_forward_backward_long(const Plan &pl, const Workspace &ws, const RunParams &rp, float *gamma, float *pi,
                                  const int32_t *n_states, cudaStream_t st);
 // tensor-core (mma.sync 3xTF32) versions of the two in-loop contractions (vbx_mma_kernels.cu)
-int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, bool fold, const RunParams &rp,
+int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, bool fold,
                      const float *Phi, const int32_t *n_states, float *alpha_io, float *invL_io, cudaStream_t st);
-int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states, float loopP,
+int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                       cudaStream_t st);
 // float64 finishing phase of vbx_run (vbx_exact64.cu)
 int launch_snapshot(const Plan &pl, const Workspace &ws, const float *gamma, const float *pi, int iter, cudaStream_t st);

@@ -215,7 +215,9 @@ int launch_project_ffma(const Plan &pl, const float *X, int D, const float *V, f
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) run_init_kernel(Plan pl, Workspace ws, const float *__restrict__ gamma,
                                                        const int32_t *__restrict__ n_states, double *Li,
-                                                       int32_t *n_iters, int32_t *flags, int max_iters) {
+                                                       int32_t *n_iters, int32_t *flags, int max_iters, double Fa, double Fb,
+                                                       double loopP, const double *__restrict__ Fa_v,
+                                                       const double *__restrict__ Fb_v, const double *__restrict__ loopP_v) {
     const int rec = blockIdx.x;
     const int S = pl.S;
     const int tid = threadIdx.x;
@@ -224,6 +226,18 @@ __global__ void __launch_bounds__(128) run_init_kernel(Plan pl, Workspace ws, co
     const int ns = n_states ? n_states[rec] : S;
     const bool ok = T > 0 && ns > 0;
     if (tid == 0) {
+        // this recording's hyperparameters, derived as the scalar run always derived them
+        const double a = Fa_v ? Fa_v[rec] : Fa, b = Fb_v ? Fb_v[rec] : Fb, lp = loopP_v ? loopP_v[rec] : loopP;
+        RecParams hp;
+        hp.dFa = a;
+        hp.dFb = b;
+        hp.dFaFb = a / b;
+        hp.dloopP = lp;
+        hp.Fa = (float)a;
+        hp.Fb = (float)b;
+        hp.FaFb = (float)(a / b);
+        hp.loopP = (float)lp;
+        ws.hp[rec] = hp;
         ws.active[rec] = ok ? 1 : 0;
         ws.tile_done[rec] = 0;
         if (ws.active64) {
@@ -249,9 +263,11 @@ __global__ void __launch_bounds__(128) run_init_kernel(Plan pl, Workspace ws, co
 }
 
 int launch_run_init(const Plan &pl, const Workspace &ws, const float *gamma, const int32_t *n_states, double *Li,
-                    int32_t *n_iters, int32_t *flags, int max_iters, cudaStream_t st) {
+                    int32_t *n_iters, int32_t *flags, int max_iters, double Fa, double Fb, double loopP,
+                    const double *Fa_v, const double *Fb_v, const double *loopP_v, cudaStream_t st) {
     if (pl.n_rec == 0) return 0;
-    run_init_kernel<<<pl.n_rec, 128, 0, st>>>(pl, ws, gamma, n_states, Li, n_iters, flags, max_iters);
+    run_init_kernel<<<pl.n_rec, 128, 0, st>>>(pl, ws, gamma, n_states, Li, n_iters, flags, max_iters, Fa, Fb, loopP, Fa_v,
+                                               Fb_v, loopP_v);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -414,8 +430,7 @@ int launch_mstep_partial(const Plan &pl, const Workspace &ws, const float *rho, 
 // recording, four 128-thread warp-groups each taking every 4th speaker, thread = r.  Sums over tiles run in tile order in float64 (deterministic).
 // ------------------------------------------------------------------------------------------------
 template <int S8, bool R128>
-__global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace ws, RunParams rp,
-                                                            const float *__restrict__ Phi,
+__global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace ws, const float *__restrict__ Phi,
                                                             const int32_t *__restrict__ n_states, float *alpha_io,
                                                             float *invL_io, int from_given) {
     // one CTA per recording; four 128-thread warp-groups, each takes every 4th speaker, thread = r
@@ -423,6 +438,7 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
     constexpr int NT = S8 / 8, NSP = S8 / 4;   // speakers per warp-group
     const int rec = blockIdx.x;
     if (!ws.active[rec]) return;            // CTA-uniform
+    const float FaFb = ws.hp[rec].FaFb, Fa = ws.hp[rec].Fa;
     const int wg = threadIdx.x >> 7;
     const int r = threadIdx.x & 127, warp = r >> 5, lane = r & 31;
     const bool live = r < R;
@@ -459,10 +475,10 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
             } else {
                 const double gr = grs[k];
                 const float Ns = ws.occ[(int64_t)rec * S + s];
-                invL = 1.f / (1.f + rp.FaFb * Ns * phi);
-                alpha = (float)((double)(rp.FaFb * invL) * gr);
+                invL = 1.f / (1.f + FaFb * Ns * phi);
+                alpha = (float)((double)(FaFb * invL) * gr);
             }
-            Av = rp.Fa * alpha;
+            Av = Fa * alpha;
             const float a2 = alpha * alpha;
             reg = logf(invL) - invL - a2 + 1.f;
             c = (invL + a2) * phi;
@@ -488,7 +504,7 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
         const int s = threadIdx.x;
         const bool dead = s >= ns;
         ws.bias[(int64_t)rec * S + s] =
-            dead ? CUDART_INF_F : (float)(rp.dFa * 0.5 * ((cpart[s][0] + cpart[s][1]) + (cpart[s][2] + cpart[s][3])));
+            dead ? CUDART_INF_F : (float)(ws.hp[rec].dFa * 0.5 * ((cpart[s][0] + cpart[s][1]) + (cpart[s][2] + cpart[s][3])));
         ws.regp[(int64_t)rec * S + s] = dead ? 0.0 : (rpart[s][0] + rpart[s][1]) + (rpart[s][2] + rpart[s][3]);
     }
     // mma fragment-major copy of Fa*alpha, split into TF32 hi/lo (consumed by loglik_mma_kernel): linear, coalesced
@@ -508,7 +524,7 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
     }
 }
 
-int launch_speaker_model(const Plan &pl, const Workspace &ws, const RunParams &rp, const float *Phi,
+int launch_speaker_model(const Plan &pl, const Workspace &ws, const float *Phi,
                          const int32_t *n_states, float *alpha_io, float *invL_io, bool from_given,
                          cudaStream_t st) {
     if (pl.n_rec == 0) return 0;
@@ -524,7 +540,7 @@ int launch_speaker_model(const Plan &pl, const Workspace &ws, const RunParams &r
             configured = true;
         }
     }
-#define VBX_SM(S8_, R_) speaker_model_kernel<S8_, R_><<<pl.n_rec, 512, smem, st>>>(pl, ws, rp, Phi, n_states, alpha_io, invL_io, fg)
+#define VBX_SM(S8_, R_) speaker_model_kernel<S8_, R_><<<pl.n_rec, 512, smem, st>>>(pl, ws, Phi, n_states, alpha_io, invL_io, fg)
     if (pl.R == 128) {
         switch (S8) {
             case 8: VBX_SM(8, true); break;
@@ -555,7 +571,7 @@ int launch_speaker_model(const Plan &pl, const Workspace &ws, const RunParams &r
 // ------------------------------------------------------------------------------------------------
 template <int S_PAD>
 __global__ void __launch_bounds__(128) loglik_kernel(Plan pl, Workspace ws, const float *__restrict__ rho,
-                                                     const float *__restrict__ pi, const int32_t *__restrict__ n_states, const float Q) {
+                                                     const float *__restrict__ pi, const int32_t *__restrict__ n_states) {
     constexpr int SL = S_PAD < 8 ? S_PAD : 8;  // state lanes
     constexpr int SJ = S_PAD / SL;             // states per thread (strided by SL)
     constexpr int FL = 128 / SL;               // frame lanes
@@ -613,6 +629,7 @@ __global__ void __launch_bounds__(128) loglik_kernel(Plan pl, Workspace ws, cons
     float wv[SJ];                    // transition weights w = Q pi + 1e-8 of this thread's states (VBx/VBx.py:98,159)
     {
         const int ns = n_states ? n_states[rec] : S_PAD;
+        const float Q = 1.f - ws.hp[rec].loopP;
 #pragma unroll
         for (int j = 0; j < SJ; ++j) {
             const int s = sl + SL * j;
@@ -648,7 +665,7 @@ __global__ void __launch_bounds__(128) loglik_kernel(Plan pl, Workspace ws, cons
 static size_t loglik_smem(int S_pad, int R) { return (size_t)(kLTile + S_pad) * (R + 4) * sizeof(float); }
 
 template <int S_PAD>
-static int launch_loglik_t(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states, float loopP,
+static int launch_loglik_t(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                            cudaStream_t st) {
     const size_t smem = loglik_smem(S_PAD, pl.R);
     static bool configured = false;
@@ -658,20 +675,20 @@ static int launch_loglik_t(const Plan &pl, const Workspace &ws, const float *rho
             return -1;
         configured = true;
     }
-    loglik_kernel<S_PAD><<<pl.n_ltiles, 128, smem, st>>>(pl, ws, rho, pi, n_states, 1.f - loopP);
+    loglik_kernel<S_PAD><<<pl.n_ltiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
-int launch_loglik(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states, float loopP,
+int launch_loglik(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                   cudaStream_t st) {
     if (pl.n_ltiles == 0) return 0;
     switch (pl.S) {
-        case 4: return launch_loglik_t<4>(pl, ws, rho, pi, n_states, loopP, st);
-        case 8: return launch_loglik_t<8>(pl, ws, rho, pi, n_states, loopP, st);
-        case 16: return launch_loglik_t<16>(pl, ws, rho, pi, n_states, loopP, st);
-        case 32: return launch_loglik_t<32>(pl, ws, rho, pi, n_states, loopP, st);
-        case 64: return launch_loglik_t<64>(pl, ws, rho, pi, n_states, loopP, st);
-        case kMaxSWide: return launch_loglik_t<kMaxSWide>(pl, ws, rho, pi, n_states, loopP, st);
+        case 4: return launch_loglik_t<4>(pl, ws, rho, pi, n_states, st);
+        case 8: return launch_loglik_t<8>(pl, ws, rho, pi, n_states, st);
+        case 16: return launch_loglik_t<16>(pl, ws, rho, pi, n_states, st);
+        case 32: return launch_loglik_t<32>(pl, ws, rho, pi, n_states, st);
+        case 64: return launch_loglik_t<64>(pl, ws, rho, pi, n_states, st);
+        case kMaxSWide: return launch_loglik_t<kMaxSWide>(pl, ws, rho, pi, n_states, st);
         default: return -1;
     }
 }
@@ -771,7 +788,7 @@ __global__ void __launch_bounds__(128) forward_backward_kernel(Plan pl, Workspac
     if (Tmax == 0) return;  // warp-uniform: no live recording in this warp
     const int Tlast = max(T - 1, 0);
     const int ns = live ? (n_states ? n_states[rec] : S_PAD) : 0;
-    const float P = rp.loopP, Q = 1.f - rp.loopP;
+    const float P = rec >= 0 ? ws.hp[rec].loopP : 0.f, Q = 1.f - P;
 
     float pi[SPL], w[SPL], base[SPL];
 #pragma unroll
@@ -1010,7 +1027,7 @@ __global__ void __launch_bounds__(128) forward_backward_la_kernel(Plan pl, Works
     if (Tmax == 0) return;  // warp-uniform: no live recording in this warp
     const int Tlast = max(T - 1, 0);
     const int ns = live ? (n_states ? n_states[rec] : S_PAD) : 0;
-    const float P = rp.loopP, Q = 1.f - rp.loopP;
+    const float P = rec >= 0 ? ws.hp[rec].loopP : 0.f, Q = 1.f - P;
 
     float pi[SPL], w[SPL];
 #pragma unroll
@@ -1302,7 +1319,7 @@ __global__ void __launch_bounds__(128) elbo_kernel(Plan pl, Workspace ws, RunPar
     if (tid == 0) {
         double reg = 0.0;                         // eq. (25) regulariser: per-speaker parts in speaker order
         for (int s = 0; s < pl.S; ++s) reg += ws.regp[(int64_t)rec * pl.S + s];
-        const double elbo = (part[0] + part[1]) + (part[2] + part[3]) + rp.dFa * ws.gsum[rec] + 0.5 * rp.dFb * reg;
+        const double elbo = (part[0] + part[1]) + (part[2] + part[3]) + ws.hp[rec].dFa * ws.gsum[rec] + 0.5 * ws.hp[rec].dFb * reg;
         const double d = elbo - ws.prev_elbo[rec];
         if (rp.hybrid && iter > 0 && isfinite(elbo)) {
             // float32 resolves an ELBO difference to about nb; decide here only what is decided safely

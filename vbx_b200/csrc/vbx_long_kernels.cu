@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(128) long_fwd_basis_kernel(Plan pl, Workspace 
     live = live && (c == 0 || i < ns);
     const int64_t f0 = live ? pl.offsets[rec] : 0;
     const int t0 = c * kChunk, t1 = t0 + kChunk;   // c < K-1: full chunk
-    const float P = rp.loopP, Q = 1.f - rp.loopP;
+    const float P = ws.hp[rec].loopP, Q = 1.f - P;   // rec = 0 on lanes without a chunk
     float w[SPL], base[SPL], a[SPL];
 #pragma unroll
     for (int k = 0; k < SPL; ++k) {
@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(128) long_fwd_rerun_kernel(Plan pl, Workspace 
     int lenmax = len;
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) lenmax = max(lenmax, __shfl_xor_sync(0xffffffffu, lenmax, off));
-    const float P = rp.loopP, Q = 1.f - rp.loopP;
+    const float P = ws.hp[rec].loopP, Q = 1.f - P;   // rec = 0 on lanes without a chunk
     float w[SPL], base[SPL];
 #pragma unroll
     for (int k = 0; k < SPL; ++k) {
@@ -313,7 +313,7 @@ __global__ void __launch_bounds__(128) long_bwd_basis_kernel(Plan pl, Workspace 
     int smax = steps;
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) smax = max(smax, __shfl_xor_sync(0xffffffffu, smax, off));
-    const float P = rp.loopP, Q = 1.f - rp.loopP;
+    const float P = ws.hp[rec].loopP, Q = 1.f - P;   // rec = 0 on lanes without a chunk
     float w[SPL], b[SPL];
 #pragma unroll
     for (int k = 0; k < SPL; ++k) {
@@ -462,7 +462,7 @@ __global__ void __launch_bounds__(128) long_bwd_rerun_kernel(Plan pl, Workspace 
     int smax = steps;
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) smax = max(smax, __shfl_xor_sync(0xffffffffu, smax, off));
-    const float P = rp.loopP, Q = 1.f - rp.loopP;
+    const float P = ws.hp[rec].loopP, Q = 1.f - P;   // rec = 0 on lanes without a chunk
     float w[SPL], b[SPL], occ[SPL], ent[SPL];
 #pragma unroll
     for (int k = 0; k < SPL; ++k) {
@@ -560,7 +560,7 @@ __global__ void __launch_bounds__(32) long_tail_kernel(Plan pl, Workspace ws, Ru
     const int ns = n_states ? n_states[rec] : S_PAD;
     const int64_t f0 = pl.offsets[rec];
     constexpr int SPLc = S_PAD > 32 ? 2 : 1;
-    const double Q = 1.0 - (double)rp.loopP;
+    const double Q = 1.0 - (double)ws.hp[rec].loopP;
     double pn[SPLc];
     float loc = 0.f;
 #pragma unroll

@@ -62,8 +62,8 @@ __device__ __forceinline__ void cp_async16_(void *smem, const void *gmem) {
 // sAv: [max(S_PAD,8)][kMaxR] floats of shared memory, cred: [2][4] doubles.
 // ------------------------------------------------------------------------------------------------
 template <int S_PAD, bool R128>
-__device__ __forceinline__ void speaker_model_tail(const Plan &pl, const Workspace &ws, const RunParams &rp,
-                                                   const float *__restrict__ Phi, const int rec, const int ns,
+__device__ __forceinline__ void speaker_model_tail(const Plan &pl, const Workspace &ws, const float *__restrict__ Phi,
+                                                   const int rec, const int ns,
                                                    float *alpha_io, float *invL_io, float *sAv, double *cred) {
     constexpr int S8 = S_PAD > 8 ? S_PAD : 8;
     constexpr int NT = S8 / 8;
@@ -72,6 +72,7 @@ __device__ __forceinline__ void speaker_model_tail(const Plan &pl, const Workspa
     const bool live = r < R;
     const float phi = live ? Phi[r] : 0.f;
     const int t_lo = pl.mtile_begin[rec], t_hi = pl.mtile_begin[rec + 1];
+    const float FaFb = ws.hp[rec].FaFb, Fa = ws.hp[rec].Fa;
     for (int s0 = 0; s0 < S8; s0 += 4) {
         double grs[4];
 #pragma unroll
@@ -90,9 +91,9 @@ __device__ __forceinline__ void speaker_model_tail(const Plan &pl, const Workspa
             float invL = 1.f, alpha = 0.f, Av = 0.f, c = 0.f, reg = 0.f;
             if (live && !dead) {
                 const float Ns = ws.occ[(int64_t)rec * S + s];
-                invL = 1.f / (1.f + rp.FaFb * Ns * phi);
-                alpha = (float)((double)(rp.FaFb * invL) * grs[k]);
-                Av = rp.Fa * alpha;
+                invL = 1.f / (1.f + FaFb * Ns * phi);
+                alpha = (float)((double)(FaFb * invL) * grs[k]);
+                Av = Fa * alpha;
                 const float a2 = alpha * alpha;
                 reg = logf(invL) - invL - a2 + 1.f;
                 c = (invL + a2) * phi;
@@ -115,7 +116,7 @@ __device__ __forceinline__ void speaker_model_tail(const Plan &pl, const Workspa
             }
             __syncthreads();
             if (r == 0 && s < S) {
-                ws.bias[(int64_t)rec * S + s] = dead ? CUDART_INF_F : (float)(rp.dFa * 0.5 * ((cred[0] + cred[1]) + (cred[2] + cred[3])));
+                ws.bias[(int64_t)rec * S + s] = dead ? CUDART_INF_F : (float)(ws.hp[rec].dFa * 0.5 * ((cred[0] + cred[1]) + (cred[2] + cred[3])));
                 ws.regp[(int64_t)rec * S + s] = dead ? 0.0 : (cred[4] + cred[5]) + (cred[6] + cred[7]);
             }
         }
@@ -140,7 +141,7 @@ __device__ __forceinline__ void speaker_model_tail(const Plan &pl, const Workspa
 // dynamic shared memory.  FOLD is not instantiated there (the speaker-model tail runs on 128 threads).
 template <int S_PAD, bool FOLD>
 __global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 2 : 4)
-    mstep_mma_kernel(Plan pl, Workspace ws, const float *__restrict__ rho, const float *__restrict__ gamma, RunParams rp,
+    mstep_mma_kernel(Plan pl, Workspace ws, const float *__restrict__ rho, const float *__restrict__ gamma,
                      const float *__restrict__ Phi, const int32_t *__restrict__ n_states, float *alpha_io, float *invL_io) {
     constexpr int SH = S_PAD > kMaxS ? S_PAD / kMaxS : 1;  // state blocks, one warp group each
     constexpr int SB = S_PAD / SH;                   // states of one warp group
@@ -293,19 +294,19 @@ __global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 2 :
         static_assert(sizeof(red_st) >= sizeof(float) * (S_PAD > 8 ? S_PAD : 8) * kMaxR, "speaker model reuses the reduction buffer");
         const int ns = n_states ? n_states[rec] : S_PAD;
         if (R == 128)
-            speaker_model_tail<S_PAD, true>(pl, ws, rp, Phi, rec, ns, alpha_io, invL_io, &red[0][0][0], cred);
+            speaker_model_tail<S_PAD, true>(pl, ws, Phi, rec, ns, alpha_io, invL_io, &red[0][0][0], cred);
         else
-            speaker_model_tail<S_PAD, false>(pl, ws, rp, Phi, rec, ns, alpha_io, invL_io, &red[0][0][0], cred);
+            speaker_model_tail<S_PAD, false>(pl, ws, Phi, rec, ns, alpha_io, invL_io, &red[0][0][0], cred);
     }
 }
 
 // fold != 0: also the speaker model (then no launch_speaker_model for this iteration)
-int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, bool fold, const RunParams &rp,
+int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, bool fold,
                      const float *Phi, const int32_t *n_states, float *alpha_io, float *invL_io, cudaStream_t st) {
     if (pl.n_mtiles == 0) return 0;
 #define VBX_MS(S_) \
-    if (fold) mstep_mma_kernel<S_, true><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma, rp, Phi, n_states, alpha_io, invL_io); \
-    else mstep_mma_kernel<S_, false><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma, rp, Phi, n_states, alpha_io, invL_io)
+    if (fold) mstep_mma_kernel<S_, true><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma, Phi, n_states, alpha_io, invL_io); \
+    else mstep_mma_kernel<S_, false><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma, Phi, n_states, alpha_io, invL_io)
     switch (pl.S) {
         case 4: VBX_MS(4); break;
         case 8: VBX_MS(8); break;
@@ -321,7 +322,7 @@ int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, cons
                 configured = true;
             }
             if (fold) return -1;
-            mstep_mma_kernel<kMaxSWide, false><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, gamma, rp, Phi, n_states, alpha_io, invL_io);
+            mstep_mma_kernel<kMaxSWide, false><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, gamma, Phi, n_states, alpha_io, invL_io);
             break;
         }
         default: return -1;
@@ -347,7 +348,7 @@ int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, cons
 template <int S_PAD, bool R128, bool WITH_C>
 __global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 1 : 3)
     loglik_mma_kernel(Plan pl, Workspace ws, const float *__restrict__ rho, const float *__restrict__ pi,
-                      const int32_t *__restrict__ n_states, const float Q) {
+                      const int32_t *__restrict__ n_states) {
     constexpr int NT = S_PAD > 8 ? S_PAD / 8 : 1;
     constexpr int NW = S_PAD > kMaxS ? 8 : 4;      // warps per CTA
     constexpr bool SPLIT_E = S_PAD <= kMaxS;       // separate accumulators for the small split terms
@@ -375,6 +376,7 @@ __global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 1 :
     }
     float nb[NT][2], wv[NT][2];      // -bias and the transition weights w = Q pi + 1e-8 of this thread's states
     const int ns = n_states ? n_states[rec] : S_PAD;
+    const float Q = WITH_C ? 1.f - ws.hp[rec].loopP : 0.f;
 #pragma unroll
     for (int i = 0; i < NT; ++i) {
         const int s = 8 * i + 2 * q;
@@ -545,7 +547,7 @@ static size_t loglik_mma_smem(int S_pad, int R) {
 
 template <int S_PAD>
 static int launch_loglik_mma_t(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
-                               float loopP, cudaStream_t st) {
+                               cudaStream_t st) {
     static bool configured = false;
     if constexpr (S_PAD > kMaxS) {   // split plans only (vbx_plan): the c_t variants, 8 warps per CTA
         if (!configured) {
@@ -558,9 +560,9 @@ static int launch_loglik_mma_t(const Plan &pl, const Workspace &ws, const float 
         if (!pl.split) return -1;
         const size_t smem = loglik_mma_smem(S_PAD, pl.R);
         if (pl.R == 128)
-            loglik_mma_kernel<S_PAD, true, true><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, pi, n_states, 1.f - loopP);
+            loglik_mma_kernel<S_PAD, true, true><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, pi, n_states);
         else
-            loglik_mma_kernel<S_PAD, false, true><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, pi, n_states, 1.f - loopP);
+            loglik_mma_kernel<S_PAD, false, true><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, pi, n_states);
         return cudaGetLastError() == cudaSuccess ? 1 : -1;
     } else {
     if (!configured) {
@@ -573,32 +575,31 @@ static int launch_loglik_mma_t(const Plan &pl, const Workspace &ws, const float 
         configured = true;
     }
     const size_t smem = loglik_mma_smem(S_PAD, pl.R);
-    const float Q = 1.f - loopP;
     if (pl.split) {
         if (pl.R == 128)
-            loglik_mma_kernel<S_PAD, true, true><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states, Q);
+            loglik_mma_kernel<S_PAD, true, true><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
         else
-            loglik_mma_kernel<S_PAD, false, true><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states, Q);
+            loglik_mma_kernel<S_PAD, false, true><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
     } else {
         if (pl.R == 128)
-            loglik_mma_kernel<S_PAD, true, false><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states, Q);
+            loglik_mma_kernel<S_PAD, true, false><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
         else
-            loglik_mma_kernel<S_PAD, false, false><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states, Q);
+            loglik_mma_kernel<S_PAD, false, false><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
     }
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
     }
 }
 
-int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states, float loopP,
+int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                       cudaStream_t st) {
     if (pl.n_mtiles == 0) return 0;
     switch (pl.S) {
-        case 4: return launch_loglik_mma_t<4>(pl, ws, rho, pi, n_states, loopP, st);
-        case 8: return launch_loglik_mma_t<8>(pl, ws, rho, pi, n_states, loopP, st);
-        case 16: return launch_loglik_mma_t<16>(pl, ws, rho, pi, n_states, loopP, st);
-        case 32: return launch_loglik_mma_t<32>(pl, ws, rho, pi, n_states, loopP, st);
-        case 64: return launch_loglik_mma_t<64>(pl, ws, rho, pi, n_states, loopP, st);
-        case kMaxSWide: return launch_loglik_mma_t<kMaxSWide>(pl, ws, rho, pi, n_states, loopP, st);
+        case 4: return launch_loglik_mma_t<4>(pl, ws, rho, pi, n_states, st);
+        case 8: return launch_loglik_mma_t<8>(pl, ws, rho, pi, n_states, st);
+        case 16: return launch_loglik_mma_t<16>(pl, ws, rho, pi, n_states, st);
+        case 32: return launch_loglik_mma_t<32>(pl, ws, rho, pi, n_states, st);
+        case 64: return launch_loglik_mma_t<64>(pl, ws, rho, pi, n_states, st);
+        case kMaxSWide: return launch_loglik_mma_t<kMaxSWide>(pl, ws, rho, pi, n_states, st);
         default: return -1;
     }
 }

@@ -155,7 +155,10 @@ class PartitionedBatch:
                 extra['alpha'] = alpha[rs]
             if invL is not None:
                 extra['invL'] = invL[rs]
-            return c.run(gamma[fs], pi[rs], **extra, **kw)
+            for k in ('Fa', 'Fb', 'loopProb'):      # per-recording values: each part takes its recordings' rows
+                if isinstance(kw.get(k), torch.Tensor):
+                    extra[k] = kw[k][rs]
+            return c.run(gamma[fs], pi[rs], **{**kw, **extra})
 
         outs = self._each(one)
         res = dict(gamma=gamma, pi=pi)

@@ -136,18 +136,22 @@ def diarize_recording(x_raw, seg_times, ahc_labels, transform, plda, Fa, Fb, loo
     return rttm_lines(recording, s, e, l), labels, g[:, :S]
 
 
-def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, **run_kw):
+def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, **run_kw):
     """The VB-HMM step (VBx/vbhmm.py:150-162) for the recordings of one state tier, packed: fea [N,R] float32, labels [N]
     AHC labels (device).  f64: the float64 kernels (vbx_run_f64, any state count), else one float32 batch padded to the
-    tier.  Returns [(labels, second-best labels or None, iterations)] per recording."""
+    tier, planned by `make` (default VbxBatch).  smoothing: a number or one per recording; run_kw go to run() (Fa, Fb,
+    loopProb may be per-recording tensors there).  Returns [(labels, second-best labels or None, iterations, flags)] per
+    recording."""
     from .batch import VbxBatch, run_f64
     offs = np.concatenate([[0], np.cumsum(lens)])
     dt = torch.float64 if f64 else torch.float32
-    vb = VbxBatch(lens, int(fea.shape[1]), ns, device=dev, f64_only=f64)
+    vb = VbxBatch(lens, int(fea.shape[1]), ns, device=dev, f64_only=True) if f64 else \
+        (make or VbxBatch)(lens, int(fea.shape[1]), ns, device=dev)
+    sm = np.broadcast_to(np.asarray(smoothing, dtype=np.float64), (len(lens),))
     g = torch.zeros((vb.N, vb.S), dtype=dt, device=dev)
     p = torch.zeros((vb.B, vb.S), dtype=dt, device=dev)
     for b in range(vb.B):              # VBx/vbhmm.py:150-152: qinit = softmax(onehot * smoothing)
-        g[offs[b]:offs[b + 1], :ns[b]] = soft_init(labels[offs[b]:offs[b + 1]], int(ns[b]), smoothing, dtype=dt)
+        g[offs[b]:offs[b + 1], :ns[b]] = soft_init(labels[offs[b]:offs[b + 1]], int(ns[b]), float(sm[b]), dtype=dt)
         p[b, :ns[b]] = 1.0 / ns[b]
     if f64:
         res = run_f64(vb, fea.double().contiguous(), Phi.double().contiguous(), g, p, **run_kw)   # VBx/vbhmm.py:154-158
@@ -159,36 +163,17 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, **run_kw):
         first, second = vb.hard_labels(g, second=True)                 # VBx/vbhmm.py:160-162
     first, second = first.cpu().numpy().astype(np.int64), second.cpu().numpy().astype(np.int64)
     iters = res['n_iters'].cpu().numpy().tolist()
+    flags = res['flags'].cpu().numpy().tolist()
     vb.close()
-    return [(first[offs[b]:offs[b + 1]], second[offs[b]:offs[b + 1]] if ns[b] > 1 else None, int(iters[b]))
+    return [(first[offs[b]:offs[b + 1]], second[offs[b]:offs[b + 1]] if ns[b] > 1 else None, int(iters[b]), int(flags[b]))
             for b in range(len(lens))]
 
 
-def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
-                  max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False):
-    """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
-    recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
-    one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
-    per state tier (<= 64 and 65 .. 128 AHC clusters in float32, more than 128 on the float64 kernels, vbx_run_f64);
-    merging and RTTM lines on the host.
-
-    recordings: {name: (x_raw [T,Dx] float array, seg_times [T,2])} in archive order.  transform = (mean1, mean2, lda),
-    plda = (mu, tr, psi) as read from the Kaldi model (diagonalised here as VBx/vbhmm.py:107-113 does).
-    init: 'AHC' (clustering only) or 'AHC+VB' (VBx/vbhmm.py:131,147).  chain: 'tcgen05' (fused tensor-core front end,
-    needs lda_dim == 128 and a 128-dim PLDA), 'float64' (float64 torch ops), 'auto' = tcgen05 when the shapes allow.
-    Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations)}."""
+def _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold):
+    """x-vector transform + PLDA projection and AHC (VBx/vbhmm.py:125-146) for the whole archive as one batch.  Returns
+    (fea [N,R] float32, Phi [R], AHC labels per recording at `threshold`, calibrated thresholds [B], linkage matrices)."""
     from .batch import VbxBatch
     from . import ahc as _ahc
-    if init not in ('AHC', 'AHC+VB'):
-        raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
-    if not torch.cuda.is_available():
-        from ._lib import VbxError
-        raise VbxError('diarize_batch(): no CUDA device - vbx_b200 has no CPU fallback')
-    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
-    names = list(recordings)
-    lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
-    if len(names) == 0:
-        return {}
     f64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(dev)
     f32 = lambda a: f64(a).float().contiguous()
     mu, tr, psi = diagonalise_plda(*plda)
@@ -206,8 +191,44 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
         x = xvector_transform(f64(x_all), f64(mean1), f64(mean2), f64(lda)).contiguous()
         fea = plda_project(x, f64(mu), f64(tr), lda_dim).float().contiguous()
         Phi = f64(psi[:lda_dim]).float().contiguous()
-    ahc_labels, _, _ = _ahc.ahc_batch(front, x, threshold=threshold)      # VBx/vbhmm.py:131-146
+    ahc_labels, th, Zs = _ahc.ahc_batch(front, x, threshold=threshold)      # VBx/vbhmm.py:131-146
     front.close()
+    return fea, Phi, ahc_labels, th, Zs
+
+
+def _pad_features(fea, Phi):
+    """R up to a multiple of 4 with inert zero features (see api.VBx): labels do not depend on them."""
+    pad = (-int(fea.shape[1])) % 4
+    if pad:
+        fea = torch.cat([fea, torch.zeros((fea.shape[0], pad), device=fea.device)], dim=1).contiguous()
+        Phi = torch.cat([Phi, torch.zeros(pad, device=Phi.device)]).contiguous()
+    return fea, Phi
+
+
+def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
+                  max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False):
+    """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
+    recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
+    one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
+    per state tier (<= 64 and 65 .. 128 AHC clusters in float32, more than 128 on the float64 kernels, vbx_run_f64);
+    merging and RTTM lines on the host.
+
+    recordings: {name: (x_raw [T,Dx] float array, seg_times [T,2])} in archive order.  transform = (mean1, mean2, lda),
+    plda = (mu, tr, psi) as read from the Kaldi model (diagonalised here as VBx/vbhmm.py:107-113 does).
+    init: 'AHC' (clustering only) or 'AHC+VB' (VBx/vbhmm.py:131,147).  chain: 'tcgen05' (fused tensor-core front end,
+    needs lda_dim == 128 and a 128-dim PLDA), 'float64' (float64 torch ops), 'auto' = tcgen05 when the shapes allow.
+    Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations)}."""
+    if init not in ('AHC', 'AHC+VB'):
+        raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
+    if not torch.cuda.is_available():
+        from ._lib import VbxError
+        raise VbxError('diarize_batch(): no CUDA device - vbx_b200 has no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    names = list(recordings)
+    lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
+    if len(names) == 0:
+        return {}
+    fea, Phi, ahc_labels, _, _ = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold)
     offs = np.concatenate([[0], np.cumsum(lens)])
     out = {}
     labels1 = [l.astype(np.int64) for l in ahc_labels]
@@ -215,11 +236,7 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     iters = [0] * len(names)
     if init.endswith('VB'):
         ns = np.array([int(l.max()) + 1 if len(l) else 1 for l in ahc_labels], dtype=np.int32)
-        R = int(fea.shape[1])
-        pad = (-R) % 4
-        if pad:                     # inert zero features (see api.VBx): labels do not depend on them
-            fea = torch.cat([fea, torch.zeros((fea.shape[0], pad), device=dev)], dim=1).contiguous()
-            Phi = torch.cat([Phi, torch.zeros(pad, device=dev)]).contiguous()
+        fea, Phi = _pad_features(fea, Phi)
         lab_d = torch.from_numpy(np.concatenate(ahc_labels)).to(dev)
         # VBx over-clusters in AHC and lets VB prune, so the state count varies by recording.  Each state tier is one
         # batch: <= 64 states (planned exactly as in an archive without the larger recordings), 65 .. 128 (S = 128),
@@ -235,14 +252,19 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
             sub = _vb_tier(lens[idx], ns[idx], pick(fea), Phi, pick(lab_d), tier == 2, smoothing, dev,
                            Fa=Fa, Fb=Fb, loopProb=loopP, maxIters=max_iters, epsilon=epsilon)
             for j, b in enumerate(idx):
-                labels1[b], labels2[b], iters[b] = sub[j]
+                labels1[b], labels2[b], iters[b] = sub[j][:3]
     for b, n in enumerate(names):
-        seg = np.asarray(recordings[n][1], dtype=np.float64)
-        s, e, l = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels1[b])   # VBx/vbhmm.py:169
-        item = dict(rttm=rttm_lines(n, s, e, l), labels=labels1[b], labels2nd=labels2[b], iterations=int(iters[b]),
-                    n_speakers=int(len(set(labels1[b].tolist()))), rttm2nd=None)
-        if output_2nd and labels2[b] is not None:
-            s2, e2, l2 = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels2[b])   # VBx/vbhmm.py:174-179
-            item['rttm2nd'] = rttm_lines(n, s2, e2, l2)
-        out[n] = item
+        out[n] = _result(n, recordings[n][1], labels1[b], labels2[b], iters[b], output_2nd)
     return out
+
+
+def _result(name, seg_times, labels, labels2, iterations, output_2nd):
+    """The per-recording result of diarize_batch: RTTM lines from merged label segments (VBx/vbhmm.py:169-179)."""
+    seg = np.asarray(seg_times, dtype=np.float64)
+    s, e, l = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels)   # VBx/vbhmm.py:169
+    item = dict(rttm=rttm_lines(name, s, e, l), labels=labels, labels2nd=labels2, iterations=int(iterations),
+                n_speakers=int(len(set(labels.tolist()))), rttm2nd=None)
+    if output_2nd and labels2 is not None:
+        s2, e2, l2 = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels2)   # VBx/vbhmm.py:174-179
+        item['rttm2nd'] = rttm_lines(name, s2, e2, l2)
+    return item

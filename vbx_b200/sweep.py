@@ -1,0 +1,239 @@
+"""Hyperparameter sweep: a whole grid of VBx settings over an archive as few large batches.
+
+Every VBx recipe tunes Fa, Fb, loopP, the AHC threshold and the init smoothing per dataset, by grid search on a dev set.
+Here the front end and the AHC linkage run once per archive; each threshold only repeats the host cut of the stored
+linkage (ahc.cut).  Every (recording, setting) pair is one entry of a batch with per-recording Fa, Fb and loopP
+(vbx_run_per_recording), so a grid is a handful of large batches instead of one small batch per setting.
+
+    python -m vbx_b200.sweep --out-dir sweep --xvec-ark-file exp/ES2005a.ark --segments-file exp/ES2005a.seg \\
+        --xvec-transform transform.h5 --plda-file plda --lda-dim 128 \\
+        --Fa 0.2,0.3,0.4 --Fb 6,17,64 --loopP 0.35,0.65,0.99 --threshold=-0.015,0.1 --init-smoothing 5
+
+(a list that starts with '-' needs the --option=list form) writes OUT/<setting>/<recording>.rttm and OUT/summary.json (speakers, iterations and flags per setting and recording).
+"""
+import argparse
+import itertools
+import json
+import os
+import sys
+from collections import namedtuple
+
+import numpy as np
+
+GRID_KEYS = ('Fa', 'Fb', 'loopP', 'threshold', 'smoothing')
+BUDGET_FRACTION = 0.5          # default max_batch_bytes: this share of the device memory free at the start
+
+
+def _fmt(v):
+    return f'{float(v):g}'
+
+
+class Setting(namedtuple('Setting', GRID_KEYS)):
+    """One point of the grid."""
+
+    @property
+    def name(self):
+        """Stable directory name, e.g. Fa0.3_Fb17_loopP0.99_thr-0.015_sm5."""
+        return f'Fa{_fmt(self.Fa)}_Fb{_fmt(self.Fb)}_loopP{_fmt(self.loopP)}_thr{_fmt(self.threshold)}_sm{_fmt(self.smoothing)}'
+
+
+def grid_settings(grid):
+    """grid: {'Fa': [...], 'Fb': [...], 'loopP': [...], 'threshold': [...], 'smoothing': [...]} -> list of Setting, the
+    product in that key order.  Missing keys, empty lists, Fb = 0, loopP outside [0, 1] or unknown keys raise ValueError."""
+    unknown = set(grid) - set(GRID_KEYS)
+    if unknown:
+        raise ValueError(f'unknown grid keys {sorted(unknown)}; expected {list(GRID_KEYS)}')
+    vals = []
+    for k in GRID_KEYS:
+        v = [float(x) for x in grid.get(k, [])]
+        if not v:
+            raise ValueError(f'grid[{k!r}] needs at least one value')
+        if not all(np.isfinite(v)):
+            raise ValueError(f'grid[{k!r}]: values must be finite')
+        vals.append(list(dict.fromkeys(v)))         # duplicates would only repeat work
+    if any(x == 0 for x in vals[1]):
+        raise ValueError('Fb must be non-zero')
+    if any(x < 0 or x > 1 for x in vals[2]):
+        raise ValueError('loopP must lie in [0, 1]')
+    return [Setting(*p) for p in itertools.product(*vals)]
+
+
+def parse_list(text):
+    """'0.3,0.4' -> [0.3, 0.4] (the command line's comma-separated lists)."""
+    try:
+        out = [float(t) for t in str(text).split(',') if t.strip()]
+    except ValueError:
+        raise ValueError(f'expected comma-separated numbers, got {text!r}')
+    if not out:
+        raise ValueError(f'expected comma-separated numbers, got {text!r}')
+    return out
+
+
+def pack(sizes, budget):
+    """Entries with byte sizes `sizes`, in order, into consecutive batches whose summed size stays within `budget`.
+    Returns a list of lists of entry indices (every entry in exactly one batch).  An entry larger than the budget on its
+    own raises ValueError."""
+    batches, cur, used = [], [], 0
+    for i, sz in enumerate(sizes):
+        if sz > budget:
+            raise ValueError(f'one entry needs {int(sz)} bytes, more than max_batch_bytes = {int(budget)}')
+        if cur and used + sz > budget:
+            batches.append(cur)
+            cur, used = [], 0
+        cur.append(i)
+        used += sz
+    if cur:
+        batches.append(cur)
+    return batches
+
+
+def entry_bytes(T, n_states, R, device):
+    """Device bytes one (recording, setting) entry adds to a float32 batch: its share of the plan's workspace (the larger
+    of the split and the fused-sweep plans of the recording alone, which bounds what it adds to any batch), plus its
+    replicated rho rows and gamma rows."""
+    from .batch import VbxBatch
+    ws = 0
+    for fb_split in (1, 2) if n_states <= 64 else (1,):
+        vb = VbxBatch([T], R, n_states, device=device, allocate=False, fb_split=fb_split)
+        ws = max(ws, vb.workspace_bytes)
+        S = vb.S
+        vb.close()
+    return ws + 4 * T * (R + S)
+
+
+def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
+                device=None, max_batch_bytes=None, output_2nd=False):
+    """Every setting of `grid` (see grid_settings) for every recording, with the front end and AHC run once.
+
+    recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
+    Entries (recording, setting) are grouped into diarize_batch's state tiers (<= 64, 65 .. 128 AHC clusters: float32
+    batches with per-recording Fa / Fb / loopP, packed into as few batches as fit max_batch_bytes, default half of the
+    free device memory; more than 128: one float64 run per setting).
+    Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags)}}; each recording's dict
+    is the one diarize_batch returns with that setting's scalars."""
+    import torch
+    from . import ahc as _ahc
+    from ._lib import VbxError, padded_states
+    from .parts import make_batch
+    from .pipeline import MAX_STATES_F32, _front_end, _pad_features, _result, _vb_tier
+    settings = grid_settings(grid)
+    if init not in ('AHC', 'AHC+VB'):
+        raise ValueError('Wrong option for args.initialization.')
+    if not torch.cuda.is_available():
+        raise VbxError('sweep_batch(): no CUDA device - vbx_b200 has no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    names = list(recordings)
+    if not names:
+        return {s: {} for s in settings}
+    lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
+    fea, Phi, _, th, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, 0.0)
+    fea, Phi = _pad_features(fea, Phi)
+    R = int(fea.shape[1])
+    offs = np.concatenate([[0], np.cumsum(lens)])
+    thresholds = list(dict.fromkeys(s.threshold for s in settings))
+    ahc_labels = {t: _ahc.cut(Zs, th, lens, t) for t in thresholds}              # VBx/vbhmm.py:144-146, host only
+    lab_d = {t: torch.from_numpy(np.concatenate(ahc_labels[t])).to(dev) for t in thresholds}
+    # per (setting, recording): labels, labels2nd, iterations, flags
+    res = {(k, b): (ahc_labels[s.threshold][b].astype(np.int64), None, 0, 0)
+           for k, s in enumerate(settings) for b in range(len(names))}
+    if init.endswith('VB'):
+        if max_batch_bytes is None:
+            max_batch_bytes = int(torch.cuda.mem_get_info(dev)[0] * BUDGET_FRACTION)
+        entries = [(k, b) for k in range(len(settings)) for b in range(len(names))]
+        ns = {(k, b): max(int(ahc_labels[settings[k].threshold][b].max()) + 1, 1) if lens[b] else 1 for k, b in entries}
+        tiers = ([e for e in entries if ns[e] <= 64], [e for e in entries if 64 < ns[e] <= MAX_STATES_F32],
+                 [e for e in entries if ns[e] > MAX_STATES_F32])
+        size_cache = {}
+
+        def run(group, f64, **hyper):
+            rows = torch.from_numpy(np.concatenate([np.arange(offs[b], offs[b + 1]) for _, b in group])).to(dev)
+            labs = torch.cat([lab_d[settings[k].threshold][offs[b]:offs[b + 1]] for k, b in group])
+            sub = _vb_tier(lens[[b for _, b in group]], np.array([ns[e] for e in group], dtype=np.int32),
+                           fea.index_select(0, rows).contiguous(), Phi, labs, f64,
+                           [settings[k].smoothing for k, _ in group], dev, make=make_batch,
+                           maxIters=max_iters, epsilon=epsilon, **hyper)
+            for e, r in zip(group, sub):
+                res[e] = r
+
+        for tier, group_all in enumerate(tiers[:2]):
+            if not group_all:
+                continue
+            sizes = []
+            for k, b in group_all:
+                key = (int(lens[b]), padded_states(ns[(k, b)]))      # the size depends on T and the padded S only
+                if key not in size_cache:
+                    size_cache[key] = entry_bytes(key[0], key[1], R, dev)
+                sizes.append(size_cache[key])
+            for idx in pack(sizes, max_batch_bytes):
+                group = [group_all[i] for i in idx]
+                hp = [torch.tensor([getattr(settings[k], a) for k, _ in group], dtype=torch.float64, device=dev)
+                      for a in ('Fa', 'Fb', 'loopP')]
+                run(group, False, Fa=hp[0], Fb=hp[1], loopProb=hp[2])
+        for k, s in enumerate(settings):           # no per-recording float64 path: one run per setting
+            group = [e for e in tiers[2] if e[0] == k]
+            if group:
+                run(group, True, Fa=s.Fa, Fb=s.Fb, loopProb=s.loopP)
+    out = {}
+    for k, s in enumerate(settings):
+        out[s] = {}
+        for b, n in enumerate(names):
+            l1, l2, it, fl = res[(k, b)]
+            item = _result(n, recordings[n][1], l1, l2, it, output_2nd)
+            item['flags'] = int(fl)
+            out[s][n] = item
+    return out
+
+
+def build_parser():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument('--init', default='AHC+VB', choices=['AHC', 'AHC+VB'])
+    ap.add_argument('--out-dir', required=True, type=str)
+    ap.add_argument('--xvec-ark-file', required=True, type=str)
+    ap.add_argument('--segments-file', required=True, type=str)
+    ap.add_argument('--xvec-transform', required=True, type=str)
+    ap.add_argument('--plda-file', required=True, type=str)
+    ap.add_argument('--lda-dim', required=True, type=int)
+    ap.add_argument('--Fa', required=True, type=parse_list, help='comma-separated values')
+    ap.add_argument('--Fb', required=True, type=parse_list, help='comma-separated values')
+    ap.add_argument('--loopP', required=True, type=parse_list, help='comma-separated values')
+    ap.add_argument('--threshold', required=True, type=parse_list, help='comma-separated values')
+    ap.add_argument('--init-smoothing', default=[5.0], type=parse_list, help='comma-separated values')
+    ap.add_argument('--max-iters', default=40, type=int)
+    ap.add_argument('--epsilon', default=1e-6, type=float)
+    ap.add_argument('--chain', default='auto', choices=['auto', 'tcgen05', 'float64'])
+    ap.add_argument('--device', default=None, help='CUDA device, e.g. cuda:0 (default: the current device)')
+    ap.add_argument('--max-batch-bytes', default=None, type=int)
+    return ap
+
+
+def main(argv=None):
+    args = build_parser().parse_args(argv)
+    from . import formats
+    segs = formats.read_segments(args.segments_file)
+    plda = formats.read_kaldi_plda(args.plda_file)
+    transform = formats.read_xvec_transform(args.xvec_transform)
+    recs = {}
+    for name, (keys, x) in formats.read_xvectors_by_recording(args.xvec_ark_file).items():
+        seg_names, times = segs[name]
+        assert np.all(np.array(seg_names) == np.array(keys))
+        recs[name] = (x, times)
+    grid = dict(Fa=args.Fa, Fb=args.Fb, loopP=args.loopP, threshold=args.threshold, smoothing=args.init_smoothing)
+    out = sweep_batch(recs, transform, plda, grid, lda_dim=args.lda_dim, max_iters=args.max_iters, epsilon=args.epsilon,
+                      init=args.init, chain=args.chain, device=args.device, max_batch_bytes=args.max_batch_bytes)
+    summary = {}
+    for s, per_rec in out.items():
+        d = os.path.join(args.out_dir, s.name)
+        os.makedirs(d, exist_ok=True)
+        summary[s.name] = dict(setting=s._asdict(), recordings={})
+        for name, item in per_rec.items():
+            with open(os.path.join(d, f'{name}.rttm'), 'w') as fp:
+                fp.write(''.join(line + os.linesep for line in item['rttm']))
+            summary[s.name]['recordings'][name] = dict(speakers=item['n_speakers'], iterations=item['iterations'],
+                                                       flags=item['flags'])
+    with open(os.path.join(args.out_dir, 'summary.json'), 'w') as fp:
+        json.dump(summary, fp, indent=1, sort_keys=True)
+    return 0
+
+
+if __name__ == '__main__':
+    sys.exit(main())
