@@ -64,9 +64,8 @@ const char *vbx_last_error(vbx_handle_t h);
 
 /* Options (ints).  "exact_stop" (default 1; read by the next vbx_plan): 1 = the workspace also holds the buffers of the
  * float64 finishing phase and vbx_run applies the stop rule of VBx/VBx.py:122-125 at float64 resolution (a recording
- * leaves the float32 kernels when its ELBO step comes within a guard band of epsilon, see vbx_run); 0 = float32 only.
- * "stop_noise_c" (default 2) / "stop_guard_mult" (default 16): the guard band = epsilon + guard_mult * nb with
- * nb = noise_c * 2^-24 * |ELBO|, the bound used for the float32 noise of an ELBO difference.
+ * leaves the float32 kernels when its ELBO step comes below epsilon + 16 nb, nb = 2 * 2^-24 * |ELBO| being the bound
+ * used for the float32 noise of an ELBO difference; see vbx_run); 0 = float32 only.
  * "fb_split" (read by the next vbx_plan): 0 = auto, 1 = always, 2 = never run the forward and the backward sweep of a
  * recording concurrently on separate warps followed by a combine pass (the choice for batches too small to fill the GPU;
  * results differ from the fused sweep by float32 rounding only, so pin it to 1 or 2 where bit-identical results for a
@@ -76,10 +75,6 @@ const char *vbx_last_error(vbx_handle_t h);
  * graph launch.  The second call with identical arguments (pointers and scalars) is captured on a stream of the handle,
  * later identical calls replay it (ordered against `stream` with events, no host synchronisation); any other call, and
  * any failure to capture, launches the kernels directly.  Off while "timing" is on.
- * "fb_priority": 0 = auto (large batches), 1 = always, 2 = never launch the forward-backward sweep on a high-priority side
- * stream of the handle (ordered against `stream` with events, still no host synchronisation), so that it interleaves with
- * the bandwidth-bound kernels of ANOTHER handle working on the same device (vbx_b200/parts.py runs two halves of a batch).
- * "fold_speaker" (0/1, default 0): compute the speaker model inside the tensor-core M-step kernel; ignored at S = 128.
  * Tuning knobs: "fb_states_per_lane" (0 = auto, 1, 2, 4; at S = 64 values below 2 and at S = 128 values below 4 are
  * raised to those, since a recording's lane group must fit in a warp), "fb_classic" (forward-backward sweep: 0 = one-step
  * look-ahead recurrences, 1 = normalise-every-frame), "projection" (0 = auto, 1 = FFMA tiles,

@@ -736,6 +736,8 @@ def test_c_abi_argument_errors():
     assert lib.vbx_bind_workspace(h, None, 0) == -3
     # entry points added with the section-8f rows: state and argument checks before anything is launched
     assert lib.vbx_set_option(h, b'fb_classic', 1) == 0 and lib.vbx_set_option(h, b'no_such_knob', 1) == -1
+    for removed in (b'fold_speaker', b'fb_priority', b'stop_noise_c', b'stop_guard_mult'):
+        assert lib.vbx_set_option(h, removed, 2) == -1 and b'unknown option' in lib.vbx_last_error(h), removed
     assert lib.vbx_prepare_xvectors(h, None, 256, None, None, None, None, None, None, None, None, None) == -3   # no workspace
     assert lib.vbx_hard_labels(h, None, None, None, None, None) == -1                                          # null pointers
     ahc_need = ctypes.c_size_t()

@@ -100,8 +100,6 @@ CASES = {
     'split-S64': (ragged(8, 12, 700), 64, 1, {}),
     'split-S128': (ragged(9, 8, 700), 100, 1, {}),
     'split-S128-ffma': (ragged(10, 8, 700), 128, 1, dict(gemm=1)),
-    'fold-S16': (ragged(11, 24, 900), 16, 2, dict(fold_speaker=1)),
-    'fold-S64-split': (ragged(12, 12, 700), 40, 1, dict(fold_speaker=1)),
     'chunked-S16': (LONG, 16, 2, {}),
     'chunked-S64-ffma': (LONG, 64, 2, dict(gemm=1)),
     'chunked-S32-classic': (LONG, 20, 2, dict(fb_classic=1)),

@@ -33,4 +33,6 @@ def test_python_padding_follows_the_tiers(lib):
 def test_header_documents_the_wide_tier():
     src = open(os.path.join(ROOT, 'include', 'vbx_b200.h')).read()
     assert re.search(r'int32_t\s+vbx_padded_states_wide\s*\(\s*int32_t', src)
-    assert 'S = 128' in src and 'fold_speaker' in src
+    flat = re.sub(r'\s*\n\s*\*\s*', ' ', src)      # comment text without its line breaks
+    assert 'vbx_plan refuses S = 128 with VBX_ERR_ARG while fb_split = 2' in flat
+    assert 'at S = 128 values below 4 are raised' in flat

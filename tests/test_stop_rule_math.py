@@ -18,7 +18,7 @@ from oracle import c_oracle
 from vbx_b200 import synth
 
 f32, f64 = np.float32, np.float64
-NOISE_C, GUARD, SAFE_STOP = 2.0, 16.0, 4.0      # vbx_capi.cu: opt_noise_c, opt_guard_mult; elbo_kernel: 4 nb
+NOISE_C, GUARD, SAFE_STOP = 2.0, 16.0, 4.0      # vbx_internal.cuh: kStopNoiseC, kStopGuardMult; elbo_kernel: 4 nb
 
 
 def em_iteration(rho, gsum, Phi, gamma, pi, Fa, Fb, P, dt):

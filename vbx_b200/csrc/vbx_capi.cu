@@ -27,21 +27,16 @@ struct vbx_handle_s {
     int opt_projection = 0;
     int opt_timing = 0;
     int opt_gemm = 0;  // 0 = mma.sync 3xTF32, 1 = FFMA
-    int opt_fold_speaker = 0;    // 1 = speaker model inside the tensor-core M-step kernel (last CTA of a recording).  Off by
-                                 // default: the 128-thread tails hold SM slots through S dependent L2 round trips, which makes
-                                 // the folded M-step slower than the separate speaker-model kernel on the headline batch
     int opt_debug_sync = 0;      // 1 = synchronise after every launch group and name it on stderr (debugging aid)
     int opt_fb_split = 0;        // 0 = auto (few recordings: sweeps on separate warps), 1 = always, 2 = never
     int opt_exact_stop = 1;      // 1 = finish recordings in float64 once the ELBO step nears epsilon (vbx_exact64.cu)
-    int opt_noise_c = 2;         // float32 noise bound of an ELBO difference = noise_c * 2^-24 * |ELBO|
-    int opt_guard_mult = 16;     // a recording switches when its ELBO step < epsilon + guard_mult * noise bound
     int64_t launches = 0;
     // The forward-backward sweep of a large batch is latency bound (a tenth of the warps an SM can hold).  When two
     // sub-batches run on two streams (vbx_b200/parts.py) it should interleave with the other sub-batch's bandwidth-bound
     // contractions, but the block scheduler hands out the CTAs of the grid that was launched first until none are left.
-    // The sweep therefore runs on a high-priority side stream of this handle (ordered against `stream` by two events):
-    // its CTAs take the next free SM slots ahead of the queued contraction CTAs of the other sub-batch.
-    int opt_fb_priority = 0;     // 0 = auto (large batches on the fused sweep), 1 = always, 2 = never
+    // The fused sweep of a batch of >= 1024 recordings therefore runs on a high-priority side stream of this handle
+    // (ordered against `stream` by two events): its CTAs take the next free SM slots ahead of the queued contraction CTAs
+    // of the other sub-batch (measured faster on the headline batch and ragged config 3, DESIGN.md section 5.6).
     cudaStream_t hi_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     // CUDA graph of a whole vbx_run (small batches are launch bound: a run is 41 rounds x up to 12 launches).  The second
@@ -142,7 +137,6 @@ size_t carve(const vbx::Plan &pl, void *base, vbx::Workspace *ws) {
     w.gpart = c.take<double>((size_t)pl.n_mtiles);
     w.prev_elbo = c.take<double>(B);
     w.active = c.take<int32_t>(B);
-    w.tile_done = c.take<int32_t>(B);
     w.scratch = c.take<float>(2 * std::max<size_t>(S, vbx::kMaxS));
     if (pl.R == 128) w.tc_scratch = c.take<float>(vbx::tc_scratch_floats());
     if (pl.split) {
@@ -224,9 +218,7 @@ int vbx_create(int32_t device, vbx_handle_t *out) {
             cudaStreamCreateWithFlags(&h->graph_stream, cudaStreamNonBlocking) != cudaSuccess ||
             cudaEventCreateWithFlags(&h->ev_g0, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&h->ev_g1, cudaEventDisableTiming) != cudaSuccess) {
-            if (h->hi_stream) cudaStreamDestroy(h->hi_stream);
-            if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-            delete h;
+            vbx_destroy(h);   // releases whatever was created (null members are skipped)
             return VBX_ERR_CUDA;
         }
     }
@@ -274,15 +266,6 @@ int vbx_set_option(vbx_handle_t h, const char *name, int32_t value) {
         h->opt_gemm = value;
         return VBX_OK;
     }
-    if (!strcmp(name, "fb_priority")) {
-        if (value < 0 || value > 2) return fail(h, VBX_ERR_ARG, "fb_priority must be 0 (auto), 1 (always) or 2 (never)");
-        h->opt_fb_priority = value;
-        return VBX_OK;
-    }
-    if (!strcmp(name, "fold_speaker")) {
-        h->opt_fold_speaker = value ? 1 : 0;
-        return VBX_OK;
-    }
     if (!strcmp(name, "debug_sync")) {
         h->opt_debug_sync = value ? 1 : 0;
         return VBX_OK;
@@ -294,16 +277,6 @@ int vbx_set_option(vbx_handle_t h, const char *name, int32_t value) {
     }
     if (!strcmp(name, "exact_stop")) {   // takes effect at the next vbx_plan (workspace layout)
         h->opt_exact_stop = value ? 1 : 0;
-        return VBX_OK;
-    }
-    if (!strcmp(name, "stop_noise_c")) {
-        if (value < 1) return fail(h, VBX_ERR_ARG, "stop_noise_c must be >= 1");
-        h->opt_noise_c = value;
-        return VBX_OK;
-    }
-    if (!strcmp(name, "stop_guard_mult")) {
-        if (value < 2) return fail(h, VBX_ERR_ARG, "stop_guard_mult must be >= 2");
-        h->opt_guard_mult = value;
         return VBX_OK;
     }
     if (!strcmp(name, "timing")) {
@@ -664,8 +637,6 @@ static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *
     // epsilon = -inf (fixed iteration count) and NaN never stop: nothing to decide, everything stays float32
     rp.hybrid = (pl.exact && epsilon > -1e300 && epsilon < 1e300 && max_iters > 1) ? 1 : 0;
     rp.warm = warm_start ? 1 : 0;
-    rp.noise_c = (double)h->opt_noise_c;
-    rp.guard_mult = (double)h->opt_guard_mult;
 
     // ---- the launch sequence of one run, on stream `st` (directly, or under stream capture) ----
     auto enqueue = [&](cudaStream_t st) -> int {
@@ -679,7 +650,7 @@ static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *
     // With the float64 finishing phase a recording that switched lags one round behind (it redoes two iterations):
     // one extra round, in which only the float64 kernels run.
     const int rounds = max_iters + (rp.hybrid ? 1 : 0);
-    const bool fb_hi = h->opt_fb_priority == 1 || (h->opt_fb_priority == 0 && !pl.split && pl.n_rec >= 1024);
+    const bool fb_hi = !pl.split && pl.n_rec >= 1024;
     for (int it = 0; it < rounds; ++it) {
         Range nvtx_iter("vbx_em_iteration");
         const bool given = it == 0 && warm_start;
@@ -689,16 +660,13 @@ static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *
                 rc = counted(h, vbx::launch_snapshot(pl, h->ws, gamma_io, pi_io, it, st), "snapshot");
                 if (rc) return rc;
             }
-            // tensor-core M-step: the CTA finishing a recording's last tile also computes its speaker model (no extra launch)
-            // (not at S = 128: the M-step's two warp groups do not match the 128-thread speaker-model tail)
-            const bool fold = !given && !h->opt_gemm && h->opt_fold_speaker && pl.S <= vbx::kMaxS;
             if (!given) {
                 Timed t(h, st, VBX_K_MSTEP);
                 rc = counted(h, h->opt_gemm ? vbx::launch_mstep_partial(pl, h->ws, rho, gamma_io, st)
-                                            : vbx::launch_mstep_mma(pl, h->ws, rho, gamma_io, fold, Phi, n_states, alpha_io, invL_io, st), "mstep_partial");
+                                            : vbx::launch_mstep_mma(pl, h->ws, rho, gamma_io, st), "mstep_partial");
             }
             if (rc) return rc;
-            if (!fold) {
+            {
                 Timed t(h, st, VBX_K_SPEAKER_MODEL);
                 rc = counted(h, vbx::launch_speaker_model(pl, h->ws, Phi, n_states, alpha_io, invL_io, given, st), "speaker_model");
             }

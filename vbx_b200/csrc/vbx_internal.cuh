@@ -71,7 +71,6 @@ struct Workspace {
     double *gpart = nullptr;   // [n_mtiles]
     double *prev_elbo = nullptr; // [n_rec]
     int32_t *active = nullptr; // [n_rec]  1 = the recording is iterating in the float32 kernels
-    int32_t *tile_done = nullptr; // [n_rec] M-tiles of the running M-step finished so far (last one computes the speaker model)
     // float64 finishing phase (vbx_exact64.cu); null when the plan was made with option "exact_stop" = 0
     int32_t *active64 = nullptr; // [n_rec] 1 = iterating in the float64 kernels
     int32_t *fresh = nullptr;    // [n_rec] 1/2 = the next float64 iteration is the recording's first (restore the snapshot);
@@ -103,11 +102,12 @@ struct Workspace {
 struct RunParams {
     double epsilon;
     int32_t max_iters;
-    // stop rule at float64 resolution (vbx_exact64.cu): a recording leaves the float32 kernels when its ELBO step is
-    // below epsilon + guard_mult * nb, nb = noise_c * 2^-24 * |ELBO| (bound on the float32 noise of an ELBO difference)
-    int32_t hybrid, warm;
-    double noise_c, guard_mult;
+    int32_t hybrid, warm;   // hybrid: the stop rule at float64 resolution (vbx_exact64.cu)
 };
+// Stop rule at float64 resolution: a recording leaves the float32 kernels when its ELBO step is below
+// epsilon + kStopGuardMult * nb, nb = kStopNoiseC * 2^-24 * |ELBO| (bound on the float32 noise of an ELBO difference).
+constexpr double kStopNoiseC = 2.0;
+constexpr double kStopGuardMult = 16.0;
 
 #ifdef __CUDACC__
 // small vector load/store helpers shared by the kernel translation units
@@ -210,8 +210,7 @@ int launch_forward_backward_split(const Plan &pl, const Workspace &ws, const Run
 int launch_forward_backward_long(const Plan &pl, const Workspace &ws, const RunParams &rp, float *gamma, float *pi,
                                  const int32_t *n_states, cudaStream_t st);
 // tensor-core (mma.sync 3xTF32) versions of the two in-loop contractions (vbx_mma_kernels.cu)
-int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, bool fold,
-                     const float *Phi, const int32_t *n_states, float *alpha_io, float *invL_io, cudaStream_t st);
+int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, cudaStream_t st);
 int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                       cudaStream_t st);
 // float64 finishing phase of vbx_run (vbx_exact64.cu)

@@ -239,7 +239,6 @@ __global__ void __launch_bounds__(128) run_init_kernel(Plan pl, Workspace ws, co
         hp.loopP = (float)lp;
         ws.hp[rec] = hp;
         ws.active[rec] = ok ? 1 : 0;
-        ws.tile_done[rec] = 0;
         if (ws.active64) {
             ws.active64[rec] = 0;
             ws.fresh[rec] = 0;
@@ -758,7 +757,7 @@ __device__ __forceinline__ float rcp_fast(float x) {
     return r;
 }
 
-template <int S_PAD, int SPL, bool NORM>
+template <int S_PAD, int SPL>
 __global__ void __launch_bounds__(128) forward_backward_kernel(Plan pl, Workspace ws, RunParams rp, float *gamma,
                                                                float *pi_io, const int32_t *__restrict__ n_states) {
     constexpr int LPR = S_PAD / SPL;
@@ -910,11 +909,10 @@ __global__ void __launch_bounds__(128) forward_backward_kernel(Plan pl, Workspac
                 gn[k] = c.a.v[k] * bn[k];
                 gs += gn[k];
             }
-            if (NORM) {  // remove the common-mode rounding drift: rows of gamma sum to one
-                const float sc = rcp_fast(group_sum<LPR>(gs));
+            // remove the common-mode rounding drift: rows of gamma sum to one
+            const float sc = rcp_fast(group_sum<LPR>(gs));
 #pragma unroll
-                for (int k = 0; k < SPL; ++k) gn[k] *= sc;
-            }
+            for (int k = 0; k < SPL; ++k) gn[k] *= sc;
             if (!check) {
 #pragma unroll
                 for (int k = 0; k < SPL; ++k) {
@@ -1290,7 +1288,7 @@ static int launch_fb_t(const Plan &pl, const Workspace &ws, const RunParams &rp,
     const int warps = (pl.n_rec + RPW - 1) / RPW;
     const int blocks = (warps + 3) / 4;
     if (classic)
-        forward_backward_kernel<S_PAD, SPL, true><<<blocks, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);
+        forward_backward_kernel<S_PAD, SPL><<<blocks, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);
     else
         forward_backward_la_kernel<S_PAD, SPL><<<blocks, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
@@ -1323,8 +1321,8 @@ __global__ void __launch_bounds__(128) elbo_kernel(Plan pl, Workspace ws, RunPar
         const double d = elbo - ws.prev_elbo[rec];
         if (rp.hybrid && iter > 0 && isfinite(elbo)) {
             // float32 resolves an ELBO difference to about nb; decide here only what is decided safely
-            const double nb = rp.noise_c * 5.9604644775390625e-8 * fabs(elbo);
-            const bool go_on = d >= rp.epsilon + rp.guard_mult * nb;     // far above epsilon: keep iterating in float32
+            const double nb = kStopNoiseC * 5.9604644775390625e-8 * fabs(elbo);
+            const bool go_on = d >= rp.epsilon + kStopGuardMult * nb;     // far above epsilon: keep iterating in float32
             const bool stop = d < rp.epsilon - 4.0 * nb;                  // clearly below epsilon: the reference stops too
             if (!go_on && !stop) {
                 // Hand the recording to the float64 kernels (vbx_exact64.cu).  This iteration AND the previous one are

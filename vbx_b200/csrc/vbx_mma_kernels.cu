@@ -15,10 +15,6 @@
 
 #include "vbx_internal.cuh"
 
-#ifndef VBX_L2_PREFETCH
-#define VBX_L2_PREFETCH 0
-#endif
-
 namespace vbx {
 
 __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t b0, const uint32_t b1) {
@@ -36,11 +32,6 @@ __device__ __forceinline__ void split_tf32(const float x, uint32_t &hi, uint32_t
     asm volatile("{\n\t.reg .b32 t;\n\tadd.u32 t, %1, 0x1000;\n\tand.b32 %0, t, 0xffffe000;\n\t}" : "=r"(hi) : "r"(__float_as_uint(x)));
     lo = (__float_as_uint(x - __uint_as_float(hi)) + 0x1000u) & 0xffffe000u;
 }
-// Bulk L2 prefetch (one instruction for a contiguous block): pulls future rows of rho from HBM into L2 so that the
-// register-staged fragment loads see L2 latency instead of DRAM latency, without holding registers for them.
-__device__ __forceinline__ void prefetch_l2(const void *gmem, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem), "r"(bytes) : "memory");
-}
 __device__ __forceinline__ void cp_async16_(void *smem, const void *gmem) {
     unsigned s = static_cast<unsigned>(__cvta_generic_to_shared(smem));
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
@@ -53,96 +44,11 @@ __device__ __forceinline__ void cp_async16_(void *smem, const void *gmem) {
 // full 128-byte line per instruction.  One CTA (4 warps) per <=kMTile-frame tile; warp = (frame slot, r-group);
 // the slots are summed through shared memory in fixed order (deterministic).
 // ------------------------------------------------------------------------------------------------
-// ------------------------------------------------------------------------------------------------
-// Speaker model of one recording by the 128 threads of the LAST M-step CTA of that recording (thread = r):
-// invL, alpha (eqs 17, 16; VBx/VBx.py:95-96), the per-speaker bias of eq. (23) (VBx/VBx.py:97), the per-speaker parts of
-// the ELBO regulariser (VBx/VBx.py:100) and the TF32 hi/lo fragment images of Fa*alpha for loglik_mma_kernel.  Same
-// arithmetic and summation order as speaker_model_kernel (vbx_kernels.cu), which stays for warm starts and the FFMA path.
-// The tile sums were written by other CTAs: they are read through L2 (__ldcg) after the fence/atomic hand-over.
-// sAv: [max(S_PAD,8)][kMaxR] floats of shared memory, cred: [2][4] doubles.
-// ------------------------------------------------------------------------------------------------
-template <int S_PAD, bool R128>
-__device__ __forceinline__ void speaker_model_tail(const Plan &pl, const Workspace &ws, const float *__restrict__ Phi,
-                                                   const int rec, const int ns,
-                                                   float *alpha_io, float *invL_io, float *sAv, double *cred) {
-    constexpr int S8 = S_PAD > 8 ? S_PAD : 8;
-    constexpr int NT = S8 / 8;
-    const int S = S_PAD, R = pl.R;
-    const int r = threadIdx.x, warp = r >> 5, lane = r & 31;
-    const bool live = r < R;
-    const float phi = live ? Phi[r] : 0.f;
-    const int t_lo = pl.mtile_begin[rec], t_hi = pl.mtile_begin[rec + 1];
-    const float FaFb = ws.hp[rec].FaFb, Fa = ws.hp[rec].Fa;
-    for (int s0 = 0; s0 < S8; s0 += 4) {
-        double grs[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {      // the tile sums of four speakers first: independent loads in flight
-            const int s = s0 + k;
-            double gr = 0.0;
-            if (live && s < ns)
-                for (int t = t_lo; t < t_hi; ++t) gr += (double)__ldcg(ws.partial + ((int64_t)t * S + s) * R + r);
-            grs[k] = gr;
-        }
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const int s = s0 + k;
-            const int64_t o = ((int64_t)rec * S + s) * R + r;
-            const bool dead = s >= ns;
-            float invL = 1.f, alpha = 0.f, Av = 0.f, c = 0.f, reg = 0.f;
-            if (live && !dead) {
-                const float Ns = ws.occ[(int64_t)rec * S + s];
-                invL = 1.f / (1.f + FaFb * Ns * phi);
-                alpha = (float)((double)(FaFb * invL) * grs[k]);
-                Av = Fa * alpha;
-                const float a2 = alpha * alpha;
-                reg = logf(invL) - invL - a2 + 1.f;
-                c = (invL + a2) * phi;
-            }
-            if (live && s < S) {
-                ws.A[o] = Av;
-                if (alpha_io) alpha_io[o] = dead ? 0.f : alpha;
-                if (invL_io) invL_io[o] = dead ? 0.f : invL;
-            }
-            sAv[s * kMaxR + r] = Av;
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) {
-                c += __shfl_xor_sync(0xffffffffu, c, off);
-                reg += __shfl_xor_sync(0xffffffffu, reg, off);
-            }
-            __syncthreads();
-            if (lane == 0) {
-                cred[warp] = (double)c;
-                cred[4 + warp] = (double)reg;
-            }
-            __syncthreads();
-            if (r == 0 && s < S) {
-                ws.bias[(int64_t)rec * S + s] = dead ? CUDART_INF_F : (float)(ws.hp[rec].dFa * 0.5 * ((cred[0] + cred[1]) + (cred[2] + cred[3])));
-                ws.regp[(int64_t)rec * S + s] = dead ? 0.0 : (cred[4] + cred[5]) + (cred[6] + cred[7]);
-            }
-        }
-    }
-    __syncthreads();
-    const int KS = R128 ? 16 : (R + 7) >> 3, KQ = 2 * KS;
-    float *fh = ws.Afrag_hi + (int64_t)rec * NT * KS * 64, *fl = ws.Afrag_lo + (int64_t)rec * NT * KS * 64;
-    for (int q = threadIdx.x; q < NT * KS * 64; q += 128) {
-        const int e = q & 1, ln = (q >> 1) & 31, ij = q >> 6;
-        const int j = R128 ? (ij & 15) : ij % KS, i = R128 ? (ij >> 4) : ij / KS;
-        const int st = 8 * i + (ln >> 2), fq = ln & 3;
-        const int col = R128 ? 16 * (j >> 1) + 4 * fq + 2 * (j & 1) + e : KQ * fq + 2 * j + e;
-        const float Av = col < kMaxR ? sAv[st * kMaxR + col] : 0.f;
-        const float hi = __uint_as_float(__float_as_uint(Av) & 0xffffe000u);
-        fh[q] = hi;
-        fl[q] = Av - hi;
-    }
-}
-
-// FOLD: the CTA that finishes a recording's last tile also computes that recording's speaker model (no separate launch).
 // S = 128: two groups of four warps, one per half of the states, each tiled like S = 64; the 67 KB reduction buffer is
-// dynamic shared memory.  FOLD is not instantiated there (the speaker-model tail runs on 128 threads).
-template <int S_PAD, bool FOLD>
+// dynamic shared memory.
+template <int S_PAD>
 __global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 2 : 4)
-    mstep_mma_kernel(Plan pl, Workspace ws, const float *__restrict__ rho, const float *__restrict__ gamma,
-                     const float *__restrict__ Phi, const int32_t *__restrict__ n_states, float *alpha_io, float *invL_io) {
+    mstep_mma_kernel(Plan pl, Workspace ws, const float *__restrict__ rho, const float *__restrict__ gamma) {
     constexpr int SH = S_PAD > kMaxS ? S_PAD / kMaxS : 1;  // state blocks, one warp group each
     constexpr int SB = S_PAD / SH;                   // states of one warp group
     constexpr int MT = SB > 16 ? SB / 16 : 1;        // m-tiles of 16 states
@@ -152,7 +58,6 @@ __global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 2 :
     constexpr int NQ = NTW / 4;                      // float4 per row per thread
     constexpr int S16 = 16 * MT;
     constexpr int LD = kMaxR + 4;
-    static_assert(!FOLD || SH == 1, "the folded speaker model needs one warp group");
     __shared__ __align__(16) float red_st[SH > 1 ? 1 : FS][SH > 1 ? 1 : S16][LD];
     extern __shared__ float4 red_dyn[];
     float (*red)[S16 * SH][LD] = SH > 1 ? reinterpret_cast<float (*)[S16 * SH][LD]>(red_dyn) : reinterpret_cast<float (*)[S16 * SH][LD]>(red_st);
@@ -233,21 +138,12 @@ __global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 2 :
         }
     };
     const int nchunks = (len + 7) >> 3;
-    constexpr int PD = 8;  // L2 prefetch distance in chunks of this warp's slot (8 frames x R floats each)
-    auto prefetch_chunk = [&](const int c) {
-        if (VBX_L2_PREFETCH && lane == 0 && rg == 0 && 8 * c + 8 <= len) prefetch_l2(rho + (f0 + 8 * c) * R, 8 * R * 4);
-    };
-    {
-        // Latency is covered by (a) the bulk L2 prefetch PD chunks ahead and (b) 16 resident warps per SM; the
-        // fragment registers are single-buffered to keep the kernel at <= 128 registers (4 CTAs per SM).
-#pragma unroll
-        for (int k = 1; k < PD; ++k) prefetch_chunk(fs + k * FS);
-        Raw ra;
-        for (int c = fs; c < nchunks; c += FS) {
-            prefetch_chunk(c + PD * FS);
-            load_chunk(c, ra);
-            compute(ra, c);
-        }
+    // Load latency is covered by the 16 resident warps per SM (4 CTAs of 4 warps, 2 of 8 at S = 128); the fragment
+    // registers are single-buffered to keep the kernel at <= 128 registers.
+    Raw ra;
+    for (int c = fs; c < nchunks; c += FS) {
+        load_chunk(c, ra);
+        compute(ra, c);
     }
     // every slot parks its fragment in shared memory, then the CTA sums the slots in fixed order
 #pragma unroll
@@ -276,58 +172,29 @@ __global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 2 :
         }
         *reinterpret_cast<float4 *>(out + (int64_t)s * R + 4 * c4) = v;
     }
-    if constexpr (FOLD) {
-        // hand-over: the CTA that completes the recording's tile count sees every tile sum (fence + atomic, then L2 reads)
-        __shared__ int s_last;
-        __shared__ double cred[8];
-        __threadfence();
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            const int n_tiles = pl.mtile_begin[rec + 1] - pl.mtile_begin[rec];
-            const int prev = atomicAdd(ws.tile_done + rec, 1);
-            s_last = prev == n_tiles - 1;
-            if (s_last) ws.tile_done[rec] = 0;        // ready for the next iteration
-        }
-        __syncthreads();
-        if (!s_last) return;
-        __threadfence();
-        static_assert(sizeof(red_st) >= sizeof(float) * (S_PAD > 8 ? S_PAD : 8) * kMaxR, "speaker model reuses the reduction buffer");
-        const int ns = n_states ? n_states[rec] : S_PAD;
-        if (R == 128)
-            speaker_model_tail<S_PAD, true>(pl, ws, Phi, rec, ns, alpha_io, invL_io, &red[0][0][0], cred);
-        else
-            speaker_model_tail<S_PAD, false>(pl, ws, Phi, rec, ns, alpha_io, invL_io, &red[0][0][0], cred);
-    }
 }
 
-// fold != 0: also the speaker model (then no launch_speaker_model for this iteration)
-int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, bool fold,
-                     const float *Phi, const int32_t *n_states, float *alpha_io, float *invL_io, cudaStream_t st) {
+int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, cudaStream_t st) {
     if (pl.n_mtiles == 0) return 0;
-#define VBX_MS(S_) \
-    if (fold) mstep_mma_kernel<S_, true><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma, Phi, n_states, alpha_io, invL_io); \
-    else mstep_mma_kernel<S_, false><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma, Phi, n_states, alpha_io, invL_io)
     switch (pl.S) {
-        case 4: VBX_MS(4); break;
-        case 8: VBX_MS(8); break;
-        case 16: VBX_MS(16); break;
-        case 32: VBX_MS(32); break;
-        case 64: VBX_MS(64); break;
-        case kMaxSWide: {   // no folded speaker model at 128 states (vbx_run launches the speaker-model kernel)
+        case 4: mstep_mma_kernel<4><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma); break;
+        case 8: mstep_mma_kernel<8><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma); break;
+        case 16: mstep_mma_kernel<16><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma); break;
+        case 32: mstep_mma_kernel<32><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma); break;
+        case 64: mstep_mma_kernel<64><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma); break;
+        case kMaxSWide: {
             constexpr int smem = kMaxSWide * (kMaxR + 4) * sizeof(float);
             static bool configured = false;
             if (!configured) {
-                if (cudaFuncSetAttribute(mstep_mma_kernel<kMaxSWide, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+                if (cudaFuncSetAttribute(mstep_mma_kernel<kMaxSWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
                     return -1;
                 configured = true;
             }
-            if (fold) return -1;
-            mstep_mma_kernel<kMaxSWide, false><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, gamma, Phi, n_states, alpha_io, invL_io);
+            mstep_mma_kernel<kMaxSWide><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, gamma);
             break;
         }
         default: return -1;
     }
-#undef VBX_MS
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -494,18 +361,11 @@ __global__ void __launch_bounds__(S_PAD > kMaxS ? 256 : 128, S_PAD > kMaxS ? 1 :
             }
             finish(D, E, mt);
         };
-        constexpr int PD = 4;  // L2 prefetch distance in m-tiles of this warp (16 frames x 512 B each)
-        auto prefetch_mt = [&](const int mt) {
-            if (VBX_L2_PREFETCH && lane == 0 && mt * 16 + 16 <= len) prefetch_l2(rho + (f0 + mt * 16) * 128, 16 * 512);
-        };
-#pragma unroll
-        for (int k = 1; k < PD; ++k) prefetch_mt(warp + NW * k);
         Raw r0;
         load_mt(warp, r0);
         asm volatile("cp.async.wait_group 0;\n" ::: "memory");
         __syncthreads();
         for (int mt = warp; mt < n_mt; mt += NW) {
-            prefetch_mt(mt + NW * PD);
             if (mt != warp) load_mt(mt, r0);
             compute(r0, mt);
         }
