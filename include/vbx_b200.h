@@ -206,6 +206,44 @@ int vbx_elbo_trace(vbx_handle_t h, const double *Li, int32_t max_iters, double *
  * VBX_ERR_STATE before a vbx_prepare_* call on the current plan and workspace. */
 int vbx_get_gsum(vbx_handle_t h, double *gsum_out, void *stream);
 
+/* per-entry bits written to flags_out by vbx_score */
+enum vbx_score_flag {
+    VBX_SCORE_BAD_LABEL = 1,     /* a label outside [0, n_labels[e]): that interval was not counted              */
+    VBX_SCORE_BAD_REGION = 2,    /* a region mask names a speaker >= n_ref[rec]: that overlap was not counted    */
+    VBX_SCORE_BAD_RECORDING = 4  /* entry_rec[e] outside [0, n_rec), n_ref > 64 or n_ref x n_labels > max_cells:
+                                    nothing of the entry was counted (covered 0, fa 0, O not written)             */
+};
+
+/* Diarization error rate accumulation (DESIGN.md section 5.11) for many (setting, recording) entries in one launch.
+ * Times are int64 microseconds ("ticks").  Per recording r of n_rec (all DEVICE arrays):
+ *   sys_offsets [n_rec+1]        the system intervals of r are sys_lo/sys_hi[sys_offsets[r] .. sys_offsets[r+1]-1]:
+ *                                one owned interval [lo, hi) per x-vector (empty when hi <= lo)
+ *   sys_join_hi                  same layout: where interval i is followed by interval i+1 of the SAME label, it ends at
+ *                                sys_join_hi[i] instead of sys_hi[i] (bridges the pauses that the RTTM writer merges;
+ *                                sys_join_hi = sys_hi where there is none)
+ *   reg_offsets [n_rec+1]        the scored regions of r are reg_lo/reg_hi/reg_mask[reg_offsets[r] .. reg_offsets[r+1]-1]:
+ *                                sorted, disjoint [lo, hi) with the bitmask of the active reference speakers (bit k =
+ *                                speaker k; 0 = scored non-speech).  Time outside every region is not scored.
+ *   n_ref [n_rec]                reference speakers of r, 0 .. 64
+ * Per entry e of n_entries:
+ *   entry_rec [n_entries]        its recording
+ *   label_offsets [n_entries]    labels[label_offsets[e] + i] (int32) is the label of the recording's interval i
+ *   n_labels [n_entries]         labels lie in [0, n_labels[e])
+ *   o_offsets [n_entries]        its overlap block O_out[o_offsets[e] ..] of n_ref[rec] x n_labels[e] int64 (row = reference
+ *                                speaker); blocks of different entries must not overlap
+ * Outputs (all written by the call, no zeroing needed): covered_out[e] = scored time in which the system speaks and a
+ *   reference speaker is active, fa_out[e] = scored time in which the system speaks over non-speech, O[k, s] = scored time
+ *   in which reference speaker k is active while the system says s, flags_out[e] = vbx_score_flag bits.
+ * max_cells (HOST): at least the largest n_ref x n_labels of any entry; blocks of up to min(max_cells, 64 x 128) cells
+ *   are accumulated in shared memory, larger ones in place in O_out (same results).  O_out may be NULL if max_cells is 0.
+ * Integer sums only: results are bit-identical whatever the batch and the launch order.  Needs no plan; does not
+ * synchronise with the host.  VBX_ERR_ARG for negative counts, max_cells < 0 or null pointers. */
+int vbx_score(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets, const int64_t *sys_lo, const int64_t *sys_hi,
+              const int64_t *sys_join_hi, const int64_t *reg_offsets, const int64_t *reg_lo, const int64_t *reg_hi, const uint64_t *reg_mask,
+              const int32_t *n_ref, int32_t n_entries, const int32_t *entry_rec, const int64_t *label_offsets,
+              const int32_t *labels, const int32_t *n_labels, const int64_t *o_offsets, int64_t max_cells,
+              int64_t *covered_out, int64_t *fa_out, int64_t *O_out, int32_t *flags_out, void *stream);
+
 /* Number of kernels launched by this handle since creation (bench.py reports it as gpu_launches). */
 int64_t vbx_launch_count(vbx_handle_t h);
 

@@ -1,0 +1,112 @@
+"""Times DER scoring of a 216-setting sweep (vbx_b200/score.py, kernel vbx_score) on a seeded synthetic archive, and the
+pure-Python line-sweep oracle (oracle/der_oracle.py) on a subset.  Prints one JSON line; --out also writes it there.
+
+The archive is shaped like tools/bench_sweep.py's: 17 recordings of 2 000 .. 8 000 x-vectors (1.5 s every 0.24 s, a few
+pauses), 2 .. 8 speakers, ground-truth labels whose merged segments are the reference RTTM.  Each of the 216 settings
+gets its own system labelling per recording: the truth under a random relabelling with a setting-dependent share of
+x-vectors reassigned, so every entry has misses, false alarms and confusion to count.  All three AMI protocols are scored.
+
+    python tools/bench_score.py --out profiles/h100_score.json
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), '..'))
+from oracle import der_oracle  # noqa: E402
+from vbx_b200 import pipeline, score, synth  # noqa: E402
+
+N_SETTINGS = 216
+
+
+def archive(seed=0):
+    rng = np.random.default_rng(seed)
+    lens = rng.integers(2000, 8001, 17)
+    arch = synth.make_scoring_archive(lens, seed=seed, gap_prob=0.02)
+    rows = []
+    for n, (seg, lab) in arch.items():
+        s, e, l = pipeline.merge_adjacent_labels(seg[:, 0], seg[:, 1], lab)
+        rows += [(n, float(a), float(z - a), f'spk{k}') for a, z, k in zip(s, e, l)]
+    turns = score.reference_turns(rows)
+    names = list(arch)
+    t0 = time.perf_counter()
+    recs = [score.prepare_recording(n, turns[n], score.owned_intervals(arch[n][0])) for n in names]
+    t_prep = time.perf_counter() - t0
+    entries = []
+    for k in range(N_SETTINGS):
+        flip = 0.01 + 0.2 * k / N_SETTINGS
+        for b, n in enumerate(names):
+            lab = arch[n][1]
+            perm = rng.permutation(int(lab.max()) + 2)
+            sysl = perm[lab]
+            sel = rng.random(len(lab)) < flip
+            sysl[sel] = rng.integers(0, len(perm), int(sel.sum()))
+            entries.append((b, sysl))
+    return arch, names, rows, recs, entries, t_prep
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--out', default=None)
+    ap.add_argument('--reps', default=5, type=int)
+    ap.add_argument('--oracle-entries', default=17, type=int)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit('bench_score.py needs a CUDA device')
+    dev = torch.device('cuda:0')
+    arch, names, rows, recs, entries, t_prep = archive()
+    n_int = sum(len(recs[b].sys_lo) for b, _ in entries)
+    score.score_entries(recs, entries[:17], device=dev)                # warm-up: module load, allocator
+    times = []
+    for _ in range(args.reps):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        res = score.score_entries(recs, entries, device=dev)
+        torch.cuda.synchronize()
+        times.append(time.perf_counter() - t0)
+    # kernel time per protocol launch, in a run of its own
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        score.score_entries(recs, entries, device=dev)
+        torch.cuda.synchronize()
+    kern = [e.time_range.elapsed_us() for e in prof.events() if "score_kernel" in e.name]
+    # the oracle on a subset: the first setting over all recordings
+    sub = entries[:args.oracle_entries]
+    t0 = time.perf_counter()
+    mismatches = 0
+    for i, (b, lab) in enumerate(sub):
+        seg = arch[names[b]][0]
+        s, e, l = pipeline.merge_adjacent_labels(seg[:, 0], seg[:, 1], lab)
+        ref = [(int(score.to_ticks(r[1])), int(score.to_ticks(r[1] + r[2])), r[3]) for r in rows if r[0] == names[b]]
+        sysseg = list(zip(score.to_ticks(s).tolist(), score.to_ticks(e).tolist(), l.tolist()))
+        for p, c, io in score.PROTOCOLS:
+            mismatches += der_oracle.der_ticks(ref, sysseg, int(score.to_ticks(c)), io) != res[i][p]['ticks']
+    t_oracle = time.perf_counter() - t0
+    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
+    lens = [len(a[0]) for a in arch.values()]
+    ders = {p: score.overall([r[p] for r in res])['der'] for p, _, _ in score.PROTOCOLS}
+    line = dict(
+        bench='DER scoring of a hyperparameter sweep', gpu=q.stdout.strip(),
+        archive=f'synthetic, seeded: {len(lens)} recordings, {min(lens)} .. {max(lens)} x-vectors, {sum(lens)} in all',
+        settings=N_SETTINGS, entries=len(entries), intervals_per_protocol=int(n_int), protocols=len(score.PROTOCOLS),
+        score_entries_s=dict(median=round(float(np.median(times)), 4), min=round(min(times), 4), max=round(max(times), 4),
+                             reps=len(times)),
+        kernel_ms_per_protocol=[round(k / 1000.0, 3) for k in kern],
+        host_region_prep_s=round(t_prep, 4),
+        oracle_s=round(t_oracle, 3), oracle_entries=len(sub), oracle_mismatches=int(mismatches),
+        overall_der=ders)
+    s = json.dumps(line)
+    print(s)
+    if args.out:
+        with open(args.out, 'w') as fp:
+            fp.write(s + '\n')
+
+
+if __name__ == '__main__':
+    main()

@@ -120,3 +120,28 @@ lls = gen.standard_normal((60, 9)) * 5
 tr_ = gen.dirichlet(np.ones(9), size=9)
 post, tll, lfw, lbw = api.forward_backward(lls, tr_, gen.dirichlet(np.ones(9)))
 print('forward_backward ok', tll)
+
+# DER scoring: ragged recordings (1 x-vector, pauses, none) and one with 64 reference speakers (up to 4 overlapping), so
+# that one launch takes the 64 KB shared-memory configuration, holds 64 x 128 overlap blocks in shared memory and
+# accumulates 64 x 200 blocks in place in global memory
+from vbx_b200 import pipeline, score          # noqa: E402
+arch = synth.make_scoring_archive([1, 300, 0, 900], seed=4, gap_prob=0.05)
+rows = []
+for n, (seg, lab) in list(arch.items())[:3]:
+    s_, e_, l_ = pipeline.merge_adjacent_labels(seg[:, 0], seg[:, 1], lab)
+    rows += [(n, float(a), float(z - a), f'spk{k}') for a, z, k in zip(s_, e_, l_)]
+big = list(arch)[3]
+span = float(arch[big][0][-1, 1])
+for layer in range(4):
+    t, k = float(gen.uniform(0, 2)), layer
+    while t < span:
+        d = float(gen.uniform(0.2, 2.0))
+        rows.append((big, round(t, 2), round(d, 2), f'spk{k % 64}'))
+        k += 4
+        t += d + float(gen.uniform(0, 1.5))
+turns = score.reference_turns(rows)
+recs = [score.prepare_recording(n, turns.get(n, []), score.owned_intervals(seg)) for n, (seg, _) in arch.items()]
+assert recs[3].n_ref == 64, recs[3].n_ref
+entries = [(b, gen.integers(0, L, len(seg))) for b, (seg, _) in enumerate(arch.values()) for L in (1, 128, 200)]
+res = score.score_entries(recs, entries, device=dev)
+print('score ok', res[-1]['full']['ticks'])

@@ -12,9 +12,11 @@ LIB_PATH = os.environ.get('VBX_B200_LIB', os.path.join(_HERE, 'libvbx_b200.so'))
 EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_create', 'vbx_destroy', 'vbx_last_error',
            'vbx_set_option', 'vbx_plan', 'vbx_bind_workspace', 'vbx_prepare_scale',
            'vbx_prepare_project', 'vbx_prepare_xvectors', 'vbx_run', 'vbx_run_per_recording', 'vbx_hard_labels', 'vbx_ahc_workspace_bytes', 'vbx_ahc', 'vbx_launch_count', 'vbx_get_timings', 'vbx_f64_workspace_bytes',
-           'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace', 'vbx_get_gsum']
+           'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace', 'vbx_get_gsum',
+           'vbx_score']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
+SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score flags
 KERNEL_CLASSES = ['project', 'prepare', 'run_init', 'mstep_partial', 'speaker_model', 'loglik', 'forward_backward', 'exact64']
 
 
@@ -85,6 +87,8 @@ def load():
     lib.vbx_elbo_trace.argtypes = [vp, vp, i32, vp, vp]
     lib.vbx_get_gsum.restype = ctypes.c_int
     lib.vbx_get_gsum.argtypes = [vp, vp, vp]
+    lib.vbx_score.restype = ctypes.c_int
+    lib.vbx_score.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, i64, vp, vp, vp, vp, vp]
     lib.vbx_get_timings.restype = ctypes.c_int
     lib.vbx_get_timings.argtypes = [vp, ctypes.POINTER(dbl), ctypes.POINTER(i64), i32]
     _lib = lib

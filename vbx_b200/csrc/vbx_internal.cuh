@@ -229,6 +229,13 @@ int launch_hard_labels(const Plan &pl, const float *gamma, const int32_t *n_stat
 // reference-module forward_backward() for a general transition matrix (vbx_fb_dense.cu)
 int launch_fb_dense(const double *lls, const double *tr, const double *ip, int T, int S, double *post, double *tll,
                     double *lfw, double *lbw, cudaStream_t st);
+// DER accumulation (vbx_score.cu)
+int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const int64_t *sys_hi, const int64_t *sys_join_hi,
+                 const int64_t *reg_off,
+                 const int64_t *reg_lo, const int64_t *reg_hi, const uint64_t *reg_mask, const int32_t *n_ref,
+                 int n_entries, const int32_t *entry_rec, const int64_t *label_off, const int32_t *labels,
+                 const int32_t *n_labels, const int64_t *o_off, int64_t max_cells, int64_t *covered_out,
+                 int64_t *fa_out, int64_t *O_out, int32_t *flags_out, cudaStream_t st);
 // AHC initialisation (vbx_ahc.cu)
 size_t ahc_workspace_bytes(const int64_t *offsets_host, int n_rec, std::vector<int64_t> *d_off_host);
 int launch_ahc(const Plan &pl, const std::vector<int64_t> &d_off, const void *x, int x_is_f64, int dim, void *workspace,

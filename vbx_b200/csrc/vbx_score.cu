@@ -1,0 +1,156 @@
+// Diarization error rate accumulation (include/vbx_b200.h vbx_score, DESIGN.md section 5.11).
+//
+// One CTA per (setting, recording) entry.  The entry's system output is one owned time interval per x-vector with one
+// label each.  An interval whose successor has the same label extends to its `join_hi` instead of its `hi`: that
+// bridges the short pauses that pipeline.merge_adjacent_labels treats as touching (np.isclose), so the entry scores
+// exactly the RTTM segments the project writes.  The recording's scored time is a sorted list of disjoint regions, each
+// with the bitmask of the reference speakers active in it (0 = scored non-speech).  Threads stride over the intervals;
+// each binary-searches the first region that ends after the interval's start and walks regions until its end, adding
+// the overlap (integer microseconds) to
+//   covered  (system speaks over reference speech), fa (system speaks over scored non-speech),
+//   O[r, s]  for every active reference speaker r and the interval's label s.
+// All sums are 64-bit integer atomics, so results do not depend on the order of the additions: bit-reproducible across
+// runs, batch compositions and launch shapes.  Each entry's O [n_ref x n_labels] sits in shared memory when it fits the
+// launch's shared block and is accumulated directly in its global block otherwise; either way one CTA owns it.
+#include "../../include/vbx_b200.h"
+#include "vbx_internal.cuh"
+
+namespace vbx {
+namespace {
+
+constexpr int kScoreThreads = 256;
+constexpr int64_t kScoreSmemCells = 64 * 128;      // 64 KB of int64: 64 reference speakers x 128 labels
+
+__device__ __forceinline__ unsigned long long warp_sum(unsigned long long v) {
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+__global__ void __launch_bounds__(kScoreThreads) score_kernel(
+    int32_t n_rec, const int64_t *__restrict__ sys_off, const int64_t *__restrict__ sys_lo,
+    const int64_t *__restrict__ sys_hi, const int64_t *__restrict__ sys_join_hi, const int64_t *__restrict__ reg_off, const int64_t *__restrict__ reg_lo,
+    const int64_t *__restrict__ reg_hi, const uint64_t *__restrict__ reg_mask, const int32_t *__restrict__ n_ref,
+    const int32_t *__restrict__ entry_rec, const int64_t *__restrict__ label_off, const int32_t *__restrict__ labels,
+    const int32_t *__restrict__ n_labels, const int64_t *__restrict__ o_off, int64_t max_cells, int64_t smem_cells,
+    int64_t *__restrict__ covered_out, int64_t *__restrict__ fa_out, int64_t *__restrict__ O_out,
+    int32_t *__restrict__ flags_out) {
+    extern __shared__ unsigned long long sO[];
+    __shared__ unsigned long long s_cov, s_fa;
+    __shared__ int s_flags;
+    const int e = blockIdx.x;
+    const int rec = entry_rec[e];
+    const int K = (rec >= 0 && rec < n_rec) ? n_ref[rec] : 0;
+    const int L = n_labels[e];
+    const int64_t cells = (K > 0 && L > 0) ? (int64_t)K * L : 0;
+    if (rec < 0 || rec >= n_rec || K > 64 || cells > max_cells) {    // uniform over the CTA: the entry is not counted
+        if (threadIdx.x == 0) {
+            covered_out[e] = 0;
+            fa_out[e] = 0;
+            flags_out[e] = VBX_SCORE_BAD_RECORDING;
+        }
+        return;
+    }
+    const bool shared_block = cells <= smem_cells;
+    unsigned long long *O = shared_block ? sO : reinterpret_cast<unsigned long long *>(O_out + o_off[e]);
+    for (int64_t i = threadIdx.x; i < cells; i += blockDim.x) O[i] = 0ull;
+    if (threadIdx.x == 0) {
+        s_cov = 0ull;
+        s_fa = 0ull;
+        s_flags = 0;
+    }
+    __syncthreads();
+
+    const int64_t t0 = sys_off[rec], t1 = sys_off[rec + 1];
+    const int64_t r0 = reg_off[rec], r1 = reg_off[rec + 1];
+    const int32_t *lab = labels + label_off[e];
+    const uint64_t live = K >= 64 ? ~0ull : ((1ull << (K < 0 ? 0 : K)) - 1ull);
+    unsigned long long cov = 0ull, fa = 0ull;
+    int flags = 0;
+    for (int64_t t = t0 + threadIdx.x; t < t1; t += blockDim.x) {
+        const int s = lab[t - t0];
+        if (s < 0 || s >= L) {
+            flags |= VBX_SCORE_BAD_LABEL;
+            continue;
+        }
+        const int64_t lo = sys_lo[t];
+        const int64_t hi = (t + 1 < t1 && lab[t + 1 - t0] == s) ? sys_join_hi[t] : sys_hi[t];
+        if (hi <= lo) continue;
+        int64_t a = r0, b = r1;            // first region that ends after lo
+        while (a < b) {
+            const int64_t m = (a + b) >> 1;
+            if (reg_hi[m] <= lo) a = m + 1;
+            else b = m;
+        }
+        for (int64_t r = a; r < r1; ++r) {
+            const int64_t rs = reg_lo[r];
+            if (rs >= hi) break;
+            const int64_t d = min(hi, reg_hi[r]) - max(lo, rs);
+            if (d <= 0) continue;
+            uint64_t msk = reg_mask[r];
+            if (msk & ~live) {
+                flags |= VBX_SCORE_BAD_REGION;
+                continue;
+            }
+            if (msk == 0ull) {
+                fa += (unsigned long long)d;
+                continue;
+            }
+            cov += (unsigned long long)d;
+            while (msk) {
+                const int k = __ffsll((long long)msk) - 1;
+                msk &= msk - 1ull;
+                atomicAdd(&O[(int64_t)k * L + s], (unsigned long long)d);
+            }
+        }
+    }
+    cov = warp_sum(cov);
+    fa = warp_sum(fa);
+    flags = __reduce_or_sync(0xffffffffu, flags);
+    if ((threadIdx.x & 31) == 0) {
+        if (cov) atomicAdd(&s_cov, cov);
+        if (fa) atomicAdd(&s_fa, fa);
+        if (flags) atomicOr(&s_flags, flags);
+    }
+    __syncthreads();
+    if (shared_block) {
+        int64_t *dst = O_out + o_off[e];
+        for (int64_t i = threadIdx.x; i < cells; i += blockDim.x) dst[i] = (int64_t)sO[i];
+    }
+    if (threadIdx.x == 0) {
+        covered_out[e] = (int64_t)s_cov;
+        fa_out[e] = (int64_t)s_fa;
+        flags_out[e] = s_flags;
+    }
+}
+
+// cudaFuncSetAttribute is per device
+bool g_score_configured[64] = {};
+
+}  // namespace
+
+int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const int64_t *sys_hi, const int64_t *sys_join_hi,
+                 const int64_t *reg_off,
+                 const int64_t *reg_lo, const int64_t *reg_hi, const uint64_t *reg_mask, const int32_t *n_ref,
+                 int n_entries, const int32_t *entry_rec, const int64_t *label_off, const int32_t *labels,
+                 const int32_t *n_labels, const int64_t *o_off, int64_t max_cells, int64_t *covered_out,
+                 int64_t *fa_out, int64_t *O_out, int32_t *flags_out, cudaStream_t st) {
+    if (n_entries == 0) return 0;
+    const int64_t smem_cells = max_cells < kScoreSmemCells ? max_cells : kScoreSmemCells;
+    const size_t smem = (size_t)smem_cells * sizeof(unsigned long long);
+    if (smem > 48 * 1024) {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return -1;
+        if (!g_score_configured[dev]) {
+            if (cudaFuncSetAttribute(score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)(kScoreSmemCells * sizeof(unsigned long long))) != cudaSuccess)
+                return -1;
+            g_score_configured[dev] = true;
+        }
+    }
+    score_kernel<<<n_entries, kScoreThreads, smem, st>>>(n_rec, sys_off, sys_lo, sys_hi, sys_join_hi, reg_off, reg_lo, reg_hi, reg_mask,
+                                                         n_ref, entry_rec, label_off, labels, n_labels, o_off, max_cells, smem_cells,
+                                                         covered_out, fa_out, O_out, flags_out);
+    return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+}  // namespace vbx

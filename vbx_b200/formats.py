@@ -202,3 +202,18 @@ def read_rttm(path):
             if p and p[0] == 'SPEAKER':
                 out.append((p[1], float(p[3]), float(p[4]), p[7]))
     return out
+
+
+def read_uem(path):
+    """Un-partitioned evaluation map, one 'file channel onset offset' line per scored interval (seconds)
+    -> {recording: [(onset, offset), ...]} in file order.  Blank lines and lines starting with ';;' are skipped."""
+    out = {}
+    with open(path) as f:
+        for n, line in enumerate(f, 1):
+            p = line.split()
+            if not p or p[0].startswith(';;'):
+                continue
+            if len(p) != 4:
+                raise ValueError(f'{path}:{n}: expected "file channel onset offset", got {line.strip()!r}')
+            out.setdefault(p[0], []).append((float(p[2]), float(p[3])))
+    return out

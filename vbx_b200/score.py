@@ -1,0 +1,370 @@
+"""Diarization error rate (DER) of single-speaker system output against reference RTTMs, accumulated on the GPU.
+
+The scoring contract (DESIGN.md section 5.11): every boundary is converted once to int64 microseconds ("ticks"); reference
+turns of one speaker that overlap or touch are merged; a collar c removes [x - c, x + c] around every merged reference
+onset and offset, `ignore_overlaps` removes time with two or more reference speakers, a UEM restricts the scored time.
+Over the scored time, with N_ref reference speakers active and the system silent or saying one label s,
+    covered += d if the system speaks and N_ref >= 1,   fa += d if it speaks and N_ref = 0,   O[r, s] += d for active r,
+    miss = ref_total - covered,  conf = covered - max one-to-one matching of O,  DER = (miss + fa + conf) / ref_total,
+with ref_total the scored reference speaker time.  The kernel (vbx_score) accumulates covered, fa and O for many
+(setting, recording) entries in one launch; the reference regions, ref_total and the matching are host work.
+
+    python -m vbx_b200.score --ref-rttm ref/ --sys-rttm out/ [--uem all.uem] [--collar 0.25] [--ignore-overlaps] [--json]
+
+PATH is an RTTM file or a directory of *.rttm.  Every reference recording is scored (one without system output counts as
+all missed); system output for a recording the reference lacks is an error.
+"""
+import argparse
+import ctypes
+import glob
+import json
+import os
+import sys
+from collections import namedtuple
+
+import numpy as np
+
+MAX_REF_SPEAKERS = 64
+# the three protocols of the AMI recipe (AMI-diarization-setup): (name, collar seconds, ignore overlaps)
+PROTOCOLS = (('forgiving', 0.25, True), ('fair', 0.25, False), ('full', 0.0, False))
+
+# One recording prepared for scoring: the system's owned intervals [sys_lo, sys_hi) in ticks with their joined ends
+# (sys_join_hi, see owned_intervals), the number of reference speakers and, per protocol name, the scored regions
+# (lo, hi, mask, ref_total).
+ScoredRecording = namedtuple('ScoredRecording', 'name sys_lo sys_hi sys_join_hi n_ref regions')
+
+
+def to_ticks(seconds):
+    """Seconds -> int64 microseconds, np.rint(seconds * 1e6)."""
+    return np.rint(np.asarray(seconds, dtype=np.float64) * 1e6).astype(np.int64)
+
+
+def merge_turns(starts, ends):
+    """Turns [start, end) in ticks -> sorted, disjoint turns: empty ones dropped, overlapping or touching ones merged."""
+    s, e = np.asarray(starts, dtype=np.int64).reshape(-1), np.asarray(ends, dtype=np.int64).reshape(-1)
+    keep = e > s
+    s, e = s[keep], e[keep]
+    o = np.argsort(s, kind='stable')
+    s, e = s[o], e[o]
+    if len(s) == 0:
+        return s, e
+    run = np.maximum.accumulate(e)
+    first = np.nonzero(np.concatenate([[True], s[1:] > run[:-1]]))[0]
+    return s[first], np.maximum.reduceat(e, first)
+
+
+def reference_turns(rows):
+    """formats.read_rttm rows -> {recording: [(starts, ends) merged ticks, one pair per speaker, speakers by name]}.
+    Speakers whose turns are all empty are dropped; more than 64 speakers in a recording raise ValueError."""
+    per = {}
+    for rec, start, dur, spk in rows:
+        per.setdefault(rec, {}).setdefault(spk, []).append((start, start + dur))
+    out = {}
+    for rec, spks in per.items():
+        turns = []
+        for spk in sorted(spks):
+            t = to_ticks(np.array(spks[spk], dtype=np.float64))
+            s, e = merge_turns(t[:, 0], t[:, 1])
+            if len(s):
+                turns.append((s, e))
+        if len(turns) > MAX_REF_SPEAKERS:
+            raise ValueError(f'recording {rec!r}: {len(turns)} reference speakers, at most {MAX_REF_SPEAKERS} are supported')
+        out[rec] = turns
+    return out
+
+
+def owned_intervals(seg_times):
+    """x-vector segment times (T x 2 seconds) -> (lo, hi, join_hi) in ticks.  Segment t owns [lo_t, hi_t), where
+    lo_t = (e_{t-1} + s_t) // 2 if s_t < e_{t-1} else s_t, and hi_t = (e_t + s_{t+1}) // 2 if s_{t+1} < e_t else e_t
+    (s, e in ticks).  pipeline.merge_adjacent_labels also joins equal labels across a pause it takes for touching
+    (np.isclose(e_t, s_{t+1}): up to about 1e-5 of the time, 10 ms at 1000 s); join_hi_t = lo_{t+1} there and hi_t
+    elsewhere, and an interval followed by one of the same label ends at join_hi_t.  Runs of equal labels over these
+    intervals are then exactly the segments merge_adjacent_labels writes to the RTTM."""
+    seg = np.asarray(seg_times, dtype=np.float64).reshape(-1, 2)
+    st = to_ticks(seg)
+    lo, hi = st[:, 0].copy(), st[:, 1].copy()
+    join_hi = hi.copy()
+    if len(seg) > 1:
+        over = st[1:, 0] < st[:-1, 1]
+        mid = (st[:-1, 1] + st[1:, 0]) // 2
+        lo[1:][over] = mid[over]
+        hi[:-1][over] = mid[over]
+        touching = np.isclose(seg[:-1, 1], seg[1:, 0])        # the test of pipeline.merge_adjacent_labels
+        join_hi = hi.copy()
+        join_hi[:-1] = np.where(touching, lo[1:], hi[:-1])
+    return lo, hi, join_hi
+
+
+def effective_hi(timeline, labels):
+    """Where each owned interval ends for a labelling: join_hi where the next interval has the same label, else hi."""
+    lo, hi, join_hi = timeline
+    labels = np.asarray(labels).reshape(-1)
+    out = np.asarray(hi, dtype=np.int64).copy()
+    if len(labels) > 1:
+        same = labels[1:] == labels[:-1]
+        out[:-1][same] = np.asarray(join_hi)[:-1][same]
+    return out
+
+
+def scored_regions(turns, collar, ignore_overlaps, scored):
+    """Scored time of one recording under one protocol.  turns: merged per-speaker (starts, ends) ticks; collar: ticks;
+    scored: (lo, hi) sorted disjoint ticks (the UEM, or one interval spanning everything).  Returns (lo, hi, mask,
+    ref_total): sorted disjoint regions, mask = uint64 bits of the active reference speakers (0 = scored non-speech),
+    neighbours with equal masks joined, and ref_total = sum of N_ref * duration (Python int)."""
+    slo, shi = (np.asarray(a, dtype=np.int64) for a in scored)
+    c = int(collar)
+    pts = [slo, shi]
+    for s, e in turns:
+        pts += [s, e] + ([s - c, s + c, e - c, e + c] if c else [])
+    b = np.unique(np.concatenate(pts))
+    lo, hi = b[:-1], b[1:]                           # elementary stretches: nothing changes inside one
+    mask = np.zeros(len(lo), dtype=np.uint64)
+    n = np.zeros(len(lo), dtype=np.int64)
+    for k, (s, e) in enumerate(turns):
+        j = np.searchsorted(s, lo, 'right') - 1
+        act = (j >= 0) & (e[np.maximum(j, 0)] > lo)
+        mask |= act.astype(np.uint64) << np.uint64(k)
+        n += act
+    if len(slo):
+        j = np.searchsorted(slo, lo, 'right') - 1
+        keep = (j >= 0) & (shi[np.maximum(j, 0)] > lo)
+    else:
+        keep = np.zeros(len(lo), dtype=bool)
+    if c and turns:
+        x = np.concatenate([np.concatenate([s, e]) for s, e in turns])
+        zs, ze = np.sort(x - c), np.sort(x + c)
+        keep &= np.searchsorted(zs, lo, 'right') - np.searchsorted(ze, lo, 'right') == 0
+    if ignore_overlaps:
+        keep &= n < 2
+    lo, hi, mask, n = lo[keep], hi[keep], mask[keep], n[keep]
+    ref_total = int(np.sum(n * (hi - lo)))
+    if len(lo):
+        first = np.nonzero(np.concatenate([[True], (lo[1:] != hi[:-1]) | (mask[1:] != mask[:-1])]))[0]
+        hi = np.concatenate([hi[first[1:] - 1], hi[-1:]])
+        lo, mask = lo[first], mask[first]
+    return lo, hi, mask, ref_total
+
+
+def collar_ticks(collar):
+    if not collar >= 0:
+        raise ValueError(f'collar must be >= 0 seconds, got {collar}')
+    return int(to_ticks(collar))
+
+
+def prepare_recording(name, turns, timeline, uem=None, protocols=PROTOCOLS):
+    """A ScoredRecording.  turns: reference_turns()[name]; timeline: the system's intervals in ticks as (lo, hi,
+    join_hi): owned_intervals() of the x-vectors, or (lo, hi, hi) for the turns of a system RTTM; uem: None (all time is
+    scored) or [(onset, offset)] seconds; protocols: (name, collar seconds, ignore_overlaps) triples."""
+    if len(turns) > MAX_REF_SPEAKERS:
+        raise ValueError(f'recording {name!r}: {len(turns)} reference speakers, at most {MAX_REF_SPEAKERS} are supported')
+    sys_lo, sys_hi, sys_join_hi = (np.asarray(a, dtype=np.int64) for a in timeline)
+    if uem is None:      # nothing speaks outside the span of all turns: scoring all time = scoring that span
+        cat = np.concatenate([sys_lo, sys_hi, sys_join_hi] + [a for t in turns for a in t])
+        scored = (np.array([cat.min()]), np.array([cat.max()])) if len(cat) else (cat, cat)
+    else:
+        u = to_ticks(np.asarray(uem, dtype=np.float64).reshape(-1, 2))
+        scored = merge_turns(u[:, 0], u[:, 1])
+    regions = {p: scored_regions(turns, collar_ticks(c), io, scored) for p, c, io in protocols}
+    return ScoredRecording(name, sys_lo, sys_hi, sys_join_hi, len(turns), regions)
+
+
+def result(miss, fa, conf, scored):
+    """Error dict from tick counts: der (None without scored reference speech) and seconds, plus the exact ticks."""
+    miss, fa, conf, scored = int(miss), int(fa), int(conf), int(scored)
+    return dict(der=(miss + fa + conf) / scored if scored else None, miss=miss * 1e-6, fa=fa * 1e-6, conf=conf * 1e-6,
+                scored=scored * 1e-6, ticks=dict(miss=miss, fa=fa, conf=conf, scored=scored))
+
+
+def overall(results):
+    """Sum of the numerators over the sum of the denominators of several result() dicts."""
+    t = [r['ticks'] for r in results]
+    return result(*(sum(x[k] for x in t) for k in ('miss', 'fa', 'conf', 'scored')))
+
+
+def finish(covered, fa, O, ref_total):
+    """result() from the accumulated covered / fa ticks and the overlap matrix O [n_ref x n_labels] (int64)."""
+    from scipy.optimize import linear_sum_assignment
+    O = np.asarray(O, dtype=np.int64)
+    matched = 0
+    if O.size:
+        r, c = linear_sum_assignment(O, maximize=True)
+        matched = int(O[r, c].sum())
+    covered = int(covered)
+    return result(int(ref_total) - covered, fa, covered - matched, ref_total)
+
+
+def rank(per_setting):
+    """{name: result dict} -> names by DER ascending (stable in the given order; settings without a DER last)."""
+    names = list(per_setting)
+    return sorted(names, key=lambda n: (per_setting[n]['der'] is None, per_setting[n]['der'] or 0.0))
+
+
+def score_entries(recordings, entries, device=None):
+    """Score many (recording, labels) entries in one vbx_score launch per protocol.
+    recordings: list of ScoredRecording (all with the same protocols); entries: [(recording index, labels)], labels int
+    [len(sys_lo)] in [0, n) (n = max label + 1).  Returns [{protocol: result dict}] in entry order.  A label outside
+    that range raises VbxError."""
+    import torch
+    from . import _lib
+    from ._lib import VbxError
+    if not entries:
+        return []
+    if not torch.cuda.is_available():
+        raise VbxError('score_entries(): no CUDA device - vbx_b200 has no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    lens = np.array([len(r.sys_lo) for r in recordings], dtype=np.int64)
+    sys_off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    n_ref = np.array([r.n_ref for r in recordings], dtype=np.int32)
+    rec_idx = np.array([b for b, _ in entries], dtype=np.int32)
+    labs = [np.asarray(l).reshape(-1) for _, l in entries]
+    for i, (b, l) in enumerate(zip(rec_idx, labs)):
+        if not 0 <= b < len(recordings):
+            raise ValueError(f'entry {i}: recording index {b} out of range')
+        if len(l) != lens[b]:
+            raise ValueError(f'entry {i}: {len(l)} labels for {lens[b]} intervals of {recordings[b].name!r}')
+    n_labels = np.array([max(int(l.max()) + 1, 1) if len(l) else 1 for l in labs], dtype=np.int32)
+    label_off = np.concatenate([[0], np.cumsum([len(l) for l in labs])[:-1]]).astype(np.int64)
+    cells = n_ref[rec_idx].astype(np.int64) * n_labels
+    o_off = np.concatenate([[0], np.cumsum(cells)[:-1]]).astype(np.int64)
+    protocols = list(recordings[0].regions)
+    lib = _lib.load()
+    # one unused trailing element: an empty array still gets a device pointer
+    d = lambda a: torch.from_numpy(np.concatenate([a, np.zeros(1, a.dtype)])).to(dev)
+    p = lambda t: ctypes.c_void_p(t.data_ptr())
+    common = [d(sys_off)] + [d(np.concatenate([getattr(r, f) for r in recordings])) for f in ('sys_lo', 'sys_hi', 'sys_join_hi')]
+    ent = [d(rec_idx), d(label_off), d(np.concatenate(labs).astype(np.int32)), d(n_labels), d(o_off)]
+    nref_d = d(n_ref)
+    h = ctypes.c_void_p()
+    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
+        raise VbxError('vbx_create failed: no usable sm_90 device')
+    outs = {}
+    try:
+        with torch.cuda.device(dev):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            for proto in protocols:
+                regs = [r.regions[proto] for r in recordings]
+                reg_off = np.concatenate([[0], np.cumsum([len(g[0]) for g in regs])]).astype(np.int64)
+                rd = [d(reg_off)] + [d(np.concatenate([g[i] for g in regs]).view(np.int64)) for i in range(3)]
+                cov = torch.empty(len(entries), dtype=torch.int64, device=dev)
+                fa = torch.empty_like(cov)
+                O = torch.empty(max(int(cells.sum()), 1), dtype=torch.int64, device=dev)
+                flags = torch.empty(len(entries), dtype=torch.int32, device=dev)
+                rc = lib.vbx_score(h, len(recordings), *map(p, common), *map(p, rd), p(nref_d), len(entries), *map(p, ent),
+                                   int(cells.max()), p(cov), p(fa), p(O), p(flags), stream)
+                if rc != 0:
+                    raise VbxError(f'vbx_score failed ({rc}): {lib.vbx_last_error(h).decode()}')
+                outs[proto] = (cov, fa, O, flags, rd)      # rd stays referenced until the results are read
+            host = {k: tuple(t.cpu().numpy() for t in v[:4]) for k, v in outs.items()}
+    finally:
+        lib.vbx_destroy(h)
+    res = [{} for _ in entries]
+    for proto in protocols:
+        cov, fa, O, flags = host[proto]
+        bad = np.nonzero(flags)[0]
+        if len(bad):
+            i = int(bad[0])
+            why = f'labels must lie in [0, {int(n_labels[i])})' if flags[i] & _lib.SCORE_BAD_LABEL else 'bad input'
+            raise VbxError(f'vbx_score: entry {i} ({recordings[rec_idx[i]].name!r}) flags {int(flags[i])}: {why}')
+        for i, b in enumerate(rec_idx):
+            blk = O[o_off[i]:o_off[i] + cells[i]].reshape(int(n_ref[b]), int(n_labels[i]))
+            res[i][proto] = finish(cov[i], fa[i], blk, recordings[b].regions[proto][3])
+    return res
+
+
+def _rows_by_recording(rows):
+    out = {}
+    for row in rows:
+        out.setdefault(row[0], []).append(row)
+    return out
+
+
+def system_turns(rows, recording=''):
+    """System RTTM rows of one recording -> (lo, hi, labels): turns in ticks sorted by start, turns of the same label
+    merged, labels numbered by name.  Overlapping turns of different labels raise ValueError (single-speaker output
+    only)."""
+    names = sorted(set(r[3] for r in rows))
+    lo, hi, lab = [], [], []
+    for k, spk in enumerate(names):
+        t = to_ticks(np.array([(r[1], r[1] + r[2]) for r in rows if r[3] == spk], dtype=np.float64))
+        s, e = merge_turns(t[:, 0], t[:, 1])
+        lo.append(s)
+        hi.append(e)
+        lab.append(np.full(len(s), k, dtype=np.int32))
+    if not names:
+        z = np.zeros(0, dtype=np.int64)
+        return z, z, np.zeros(0, dtype=np.int32)
+    lo, hi, lab = np.concatenate(lo), np.concatenate(hi), np.concatenate(lab)
+    o = np.argsort(lo, kind='stable')
+    lo, hi, lab = lo[o], hi[o], lab[o]
+    if len(lo) > 1 and np.any(lo[1:] < np.maximum.accumulate(hi)[:-1]):
+        raise ValueError(f'recording {recording!r}: the system RTTM has overlapping turns of different speakers; '
+                         'only single-speaker system output can be scored')
+    return lo, hi, lab
+
+
+def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=None):
+    """DER of system RTTM rows against reference RTTM rows (both as formats.read_rttm returns them).
+    uem: None or {recording: [(onset, offset)]} (formats.read_uem).  Returns ({recording: result dict}, overall result
+    dict) over the reference's recordings."""
+    collar_ticks(collar)
+    ref = reference_turns(ref_turns)
+    sys_by = _rows_by_recording(sys_turns)
+    extra = sorted(set(sys_by) - set(ref))
+    if extra:
+        raise ValueError(f'system output for recordings the reference lacks: {extra}')
+    names = sorted(ref)
+    recs, entries = [], []
+    for b, n in enumerate(names):
+        if uem is not None and n not in uem:
+            raise ValueError(f'recording {n!r} is missing from the UEM')
+        lo, hi, lab = system_turns(sys_by.get(n, []), n)
+        recs.append(prepare_recording(n, ref[n], (lo, hi, hi), None if uem is None else uem[n],
+                                      (('score', collar, bool(ignore_overlaps)),)))
+        entries.append((b, lab))
+    per = {n: r['score'] for n, r in zip(names, score_entries(recs, entries, device))}
+    return per, overall(list(per.values()))
+
+
+def read_rttm_path(path):
+    """formats.read_rttm rows of an RTTM file, or of every *.rttm in a directory (sorted by name)."""
+    from . import formats
+    files = sorted(glob.glob(os.path.join(path, '*.rttm'))) if os.path.isdir(path) else [path]
+    if not files:
+        raise ValueError(f'{path}: no *.rttm files')
+    return [row for f in files for row in formats.read_rttm(f)]
+
+
+def build_parser():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument('--ref-rttm', required=True, help='reference RTTM file or directory of *.rttm')
+    ap.add_argument('--sys-rttm', required=True, help='system RTTM file or directory of *.rttm')
+    ap.add_argument('--uem', default=None, help='UEM file (default: all time is scored)')
+    ap.add_argument('--collar', default=0.25, type=float, help='seconds removed either side of every reference boundary')
+    ap.add_argument('--ignore-overlaps', action='store_true', help='do not score time with 2 or more reference speakers')
+    ap.add_argument('--json', action='store_true', help='print one JSON object instead of the table')
+    return ap
+
+
+def main(argv=None):
+    args = build_parser().parse_args(argv)
+    from . import formats
+    uem = formats.read_uem(args.uem) if args.uem else None
+    per, tot = score_rttm(read_rttm_path(args.ref_rttm), read_rttm_path(args.sys_rttm), args.collar,
+                          args.ignore_overlaps, uem)
+    if args.json:
+        print(json.dumps(dict(collar=args.collar, ignore_overlaps=args.ignore_overlaps, files=per, overall=tot),
+                         sort_keys=True))
+        return 0
+    w = max([len('OVERALL')] + [len(n) for n in per])
+    print(f'{"file":<{w}}  {"DER %":>7}  {"miss %":>7}  {"FA %":>7}  {"conf %":>7}  {"scored s":>10}')
+    for n, r in list(per.items()) + [('OVERALL', tot)]:
+        pct = [100.0 * r[k] / r['scored'] if r['scored'] else float('nan') for k in ('miss', 'fa', 'conf')]
+        der = 100.0 * r['der'] if r['der'] is not None else float('nan')
+        print(f'{n:<{w}}  {der:7.2f}  {pct[0]:7.2f}  {pct[1]:7.2f}  {pct[2]:7.2f}  {r["scored"]:10.2f}')
+    return 0
+
+
+if __name__ == '__main__':
+    sys.exit(main())

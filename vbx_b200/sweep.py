@@ -10,6 +10,9 @@ linkage (ahc.cut).  Every (recording, setting) pair is one entry of a batch with
         --Fa 0.2,0.3,0.4 --Fb 6,17,64 --loopP 0.35,0.65,0.99 --threshold=-0.015,0.1 --init-smoothing 5
 
 (a list that starts with '-' needs the --option=list form) writes OUT/<setting>/<recording>.rttm and OUT/summary.json (speakers, iterations and flags per setting and recording).
+With --ref-rttm (a file or a directory of *.rttm; optionally --uem) every entry is also scored on the GPU (vbx_b200/score.py)
+under the three AMI protocols: summary.json then holds the DER per recording and setting, the overall DER per setting, and
+`ranking`: per protocol, the setting names by overall DER.
 """
 import argparse
 import itertools
@@ -102,15 +105,20 @@ def entry_bytes(T, n_states, R, device):
 
 
 def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
-                device=None, max_batch_bytes=None, output_2nd=False):
+                device=None, max_batch_bytes=None, output_2nd=False, ref_rttm=None, uem=None):
     """Every setting of `grid` (see grid_settings) for every recording, with the front end and AHC run once.
 
     recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
     Entries (recording, setting) are grouped into diarize_batch's state tiers (<= 64, 65 .. 128 AHC clusters: float32
     batches with per-recording Fa / Fb / loopP, packed into as few batches as fit max_batch_bytes, default half of the
     free device memory; more than 128: one float64 run per setting).
-    Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags)}}; each recording's dict
-    is the one diarize_batch returns with that setting's scalars."""
+    ref_rttm: None, or the reference as an RTTM path (file or directory of *.rttm) or formats.read_rttm rows; uem: None,
+    a UEM path or formats.read_uem's dict.  With a reference every (setting, recording) entry is scored after all batches
+    have run, in one vbx_score launch per protocol (score.PROTOCOLS), and each recording's dict gains
+    der = {protocol: score.result dict}.  A recording that the reference (or the UEM) lacks raises ValueError before any
+    work; reference recordings that `recordings` lacks are ignored.
+    Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags[, der])}}; each recording's
+    dict is the one diarize_batch returns with that setting's scalars."""
     import torch
     from . import ahc as _ahc
     from ._lib import VbxError, padded_states
@@ -123,6 +131,9 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
         raise VbxError('sweep_batch(): no CUDA device - vbx_b200 has no CPU fallback')
     dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
     names = list(recordings)
+    if uem is not None and ref_rttm is None:
+        raise ValueError('uem restricts the scored time: it needs ref_rttm')
+    ref = _load_reference(names, ref_rttm, uem) if ref_rttm is not None else None
     if not names:
         return {s: {} for s in settings}
     lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
@@ -173,6 +184,16 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
             group = [e for e in tiers[2] if e[0] == k]
             if group:
                 run(group, True, Fa=s.Fa, Fb=s.Fb, loopProb=s.loopP)
+    der = None
+    if ref is not None:
+        from . import score
+        turns, uem_map = ref
+        scored = []
+        for n in names:
+            timeline = score.owned_intervals(recordings[n][1])
+            scored.append(score.prepare_recording(n, turns[n], timeline, None if uem_map is None else uem_map[n]))
+        keys = [(k, b) for k in range(len(settings)) for b in range(len(names))]
+        der = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0]) for k, b in keys], device=dev)))
     out = {}
     for k, s in enumerate(settings):
         out[s] = {}
@@ -180,8 +201,38 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
             l1, l2, it, fl = res[(k, b)]
             item = _result(n, recordings[n][1], l1, l2, it, output_2nd)
             item['flags'] = int(fl)
+            if der is not None:
+                item['der'] = der[(k, b)]
             out[s][n] = item
     return out
+
+
+def _load_reference(names, ref_rttm, uem):
+    """-> (score.reference_turns of the recordings `names`, {recording: UEM intervals} or None), checked up front."""
+    from . import formats, score
+    rows = score.read_rttm_path(ref_rttm) if isinstance(ref_rttm, (str, os.PathLike)) else list(ref_rttm)
+    wanted = set(names)
+    turns = score.reference_turns([r for r in rows if r[0] in wanted])
+    missing = [n for n in names if n not in turns]
+    if missing:
+        raise ValueError(f'recordings missing from the reference RTTM: {missing}')
+    if isinstance(uem, (str, os.PathLike)):
+        uem = formats.read_uem(uem)
+    if uem is not None:
+        missing = [n for n in names if n not in uem]
+        if missing:
+            raise ValueError(f'recordings missing from the UEM: {missing}')
+    return turns, uem
+
+
+def summarize_der(out):
+    """sweep_batch output with `der` -> ({setting name: {protocol: overall result dict}}, {protocol: setting names by
+    overall DER, stable in grid order})."""
+    from . import score
+    tot = {s.name: {p: score.overall([item['der'][p] for item in per_rec.values()]) for p, _, _ in score.PROTOCOLS}
+           for s, per_rec in out.items()}
+    ranking = {p: score.rank({n: tot[n][p] for n in tot}) for p, _, _ in score.PROTOCOLS}
+    return tot, ranking
 
 
 def build_parser():
@@ -203,6 +254,8 @@ def build_parser():
     ap.add_argument('--chain', default='auto', choices=['auto', 'tcgen05', 'float64'])
     ap.add_argument('--device', default=None, help='CUDA device, e.g. cuda:0 (default: the current device)')
     ap.add_argument('--max-batch-bytes', default=None, type=int)
+    ap.add_argument('--ref-rttm', default=None, help='reference RTTM file or directory of *.rttm: score every setting')
+    ap.add_argument('--uem', default=None, help='UEM file restricting the scored time (with --ref-rttm)')
     return ap
 
 
@@ -219,7 +272,8 @@ def main(argv=None):
         recs[name] = (x, times)
     grid = dict(Fa=args.Fa, Fb=args.Fb, loopP=args.loopP, threshold=args.threshold, smoothing=args.init_smoothing)
     out = sweep_batch(recs, transform, plda, grid, lda_dim=args.lda_dim, max_iters=args.max_iters, epsilon=args.epsilon,
-                      init=args.init, chain=args.chain, device=args.device, max_batch_bytes=args.max_batch_bytes)
+                      init=args.init, chain=args.chain, device=args.device, max_batch_bytes=args.max_batch_bytes,
+                      ref_rttm=args.ref_rttm, uem=args.uem)
     summary = {}
     for s, per_rec in out.items():
         d = os.path.join(args.out_dir, s.name)
@@ -230,6 +284,12 @@ def main(argv=None):
                 fp.write(''.join(line + os.linesep for line in item['rttm']))
             summary[s.name]['recordings'][name] = dict(speakers=item['n_speakers'], iterations=item['iterations'],
                                                        flags=item['flags'])
+            if 'der' in item:
+                summary[s.name]['recordings'][name]['der'] = item['der']
+    if args.ref_rttm is not None:
+        tot, summary['ranking'] = summarize_der(out)
+        for name, d in tot.items():
+            summary[name]['der'] = d
     with open(os.path.join(args.out_dir, 'summary.json'), 'w') as fp:
         json.dump(summary, fp, indent=1, sort_keys=True)
     return 0

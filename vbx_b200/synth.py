@@ -74,3 +74,22 @@ def make_batch(lengths, R=128, S=16, seed=0, D=None, dtype=np.float32):
         out['X'] = (out['fea'].astype(np.float64) @ V0.T + 0.5 * noise).astype(dtype)
         out['V'] = (V0 * np.sqrt(Phi)[None, :]).astype(dtype)
     return out
+
+
+def make_scoring_archive(lengths, seed=0, n_spk=(2, 9), stay=0.97, gap_prob=0.0):
+    """Seeded recordings with ground-truth speaker labels for DER scoring, shaped like an x-vector archive: 1.5 s segments
+    every 0.24 s, after a segment a pause of 1.5 .. 4.5 s with probability gap_prob (times on a 10 ms grid), and a sticky
+    speaker chain over n_spk[0] .. n_spk[1]-1 speakers.  Returns {name: (seg_times [T,2] seconds, labels int64 [T])};
+    the reference turns are the merged label segments (pipeline.merge_adjacent_labels), so the labels score DER 0."""
+    rng = np.random.default_rng(seed)
+    out = {}
+    for r, T in enumerate(lengths):
+        T = int(T)
+        K = int(rng.integers(n_spk[0], n_spk[1]))
+        step = np.where(rng.random(T) < gap_prob, rng.integers(150, 451, T) + 150, 24)     # centiseconds
+        start = np.concatenate([[0], np.cumsum(step[:-1])]) if T else np.zeros(0, dtype=np.int64)
+        lab = np.zeros(T, dtype=np.int64)
+        for t in range(1, T):
+            lab[t] = lab[t - 1] if rng.random() < stay else rng.integers(K)
+        out[f'syn{r:02d}'] = (np.stack([start / 100.0, (start + 150) / 100.0], 1).reshape(-1, 2), lab)
+    return out
