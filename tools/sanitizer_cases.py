@@ -104,6 +104,21 @@ torch.cuda.synchronize()
 front.close()
 print('front end + AHC ok', int(labels[0].max()) + 1)
 
+# AHC at a feature width with a 1-wide tail tile and a recording of 1056 x-vectors (more than the linkage kernel's
+# 1024 threads), once with duplicated x-vectors (ties) and once with a NaN x-vector (the linkage stops early)
+for tag in ('duplicates', 'NaN row'):
+    lens = [1056, 40, 3]
+    xa = gen.standard_normal((sum(lens), 33))
+    if tag == 'duplicates':
+        xa[gen.choice(1056, 300, replace=False)] = xa[gen.integers(0, 1056, 300)]
+    else:
+        xa[500, 7] = np.nan
+    ab = VbxBatch(lens, 128, 1, device=dev, allocate=False)
+    labels, thr, _ = ahc.ahc_batch(ab, torch.from_numpy(xa).to(dev))
+    torch.cuda.synchronize()
+    ab.close()
+    print('AHC dim 33 ' + tag + ' ok', int(labels[0].max()) + 1)
+
 # x-vector chain with Dx = 512 over more than one tile per CTA
 T = 128 * sms + 1
 front = VbxBatch([T], 128, 1, device=dev)

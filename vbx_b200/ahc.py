@@ -89,6 +89,10 @@ def cut(Zs, th, lengths, threshold):
             labels.append(np.zeros(0, dtype=np.int64))
         elif T == 1:
             labels.append(np.zeros(1, dtype=np.int64))
+        elif not np.isfinite(Zs[b]).all():
+            # a NaN or infinite x-vector: its distances are NaN, so the linkage stops before it (its last rows are
+            # NaN) and the calibrated threshold is NaN as well; like any NaN cut, every x-vector stays on its own
+            labels.append(np.arange(T, dtype=np.int64))
         else:
             # a degenerate calibration (NaN threshold, e.g. two x-vectors) leaves every x-vector on its own, exactly
             # what the reference's fcluster call does with a NaN cut
