@@ -206,9 +206,10 @@ int vbx_elbo_trace(vbx_handle_t h, const double *Li, int32_t max_iters, double *
  * VBX_ERR_STATE before a vbx_prepare_* call on the current plan and workspace. */
 int vbx_get_gsum(vbx_handle_t h, double *gsum_out, void *stream);
 
-/* per-entry bits written to flags_out by vbx_score */
+/* per-entry bits written to flags_out by vbx_score and vbx_score_overlap */
 enum vbx_score_flag {
-    VBX_SCORE_BAD_LABEL = 1,     /* a label outside [0, n_labels[e]): that interval was not counted              */
+    VBX_SCORE_BAD_LABEL = 1,     /* a label outside [0, n_labels[e]) (a second label outside [-1, n_labels[e]) or
+                                    equal to the first): that interval was not counted                            */
     VBX_SCORE_BAD_REGION = 2,    /* a region mask names a speaker >= n_ref[rec]: that overlap was not counted    */
     VBX_SCORE_BAD_RECORDING = 4  /* entry_rec[e] outside [0, n_rec), n_ref > 64 or n_ref x n_labels > max_cells:
                                     nothing of the entry was counted (covered 0, fa 0, O not written)             */
@@ -243,6 +244,27 @@ int vbx_score(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets, const i
               const int32_t *n_ref, int32_t n_entries, const int32_t *entry_rec, const int64_t *label_offsets,
               const int32_t *labels, const int32_t *n_labels, const int64_t *o_offsets, int64_t max_cells,
               int64_t *covered_out, int64_t *fa_out, int64_t *O_out, int32_t *flags_out, void *stream);
+
+/* Overlap-aware DER accumulation (DESIGN.md section 5.12): vbx_score with a second system label per interval, counted
+ * inside overlap regions only.  Arguments as for vbx_score, plus (DEVICE arrays):
+ *   reg_overlap [same layout as reg_lo]  1 where the region lies inside the recording's overlap regions, else 0 (the
+ *                                        caller splits the scored regions at the overlap boundaries)
+ *   labels2 [same layout as labels]      the interval's second label, -1 = none; otherwise in [0, n_labels[e]) and
+ *                                        different from labels[] of the same interval
+ * Stream 1 is vbx_score's output.  Stream 2 is interval i saying labels2[i] from its lo to sys_join_hi[i] where interval
+ * i+1 has the same second label (sys_hi[i] elsewhere), in regions with reg_overlap set.  Over scored time with N_ref
+ * reference speakers and N_sys in {0, 1, 2} system labels:
+ *   both_out[e] = sum of min(N_ref, N_sys) x time, fa_out[e] = sum of max(0, N_sys - N_ref) x time,
+ *   O[k, s] = scored time in which reference speaker k is active while the system says s in either stream.
+ * With no reg_overlap set, or labels2 all -1, the results equal vbx_score's (both_out = covered_out).  A second label
+ * outside [-1, n_labels[e]) or equal to the first sets VBX_SCORE_BAD_LABEL (that interval is not counted).
+ * Integer sums only: results are bit-identical whatever the batch and the launch order.  VBX_ERR_ARG as for vbx_score. */
+int vbx_score_overlap(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets, const int64_t *sys_lo,
+                      const int64_t *sys_hi, const int64_t *sys_join_hi, const int64_t *reg_offsets, const int64_t *reg_lo,
+                      const int64_t *reg_hi, const uint64_t *reg_mask, const uint8_t *reg_overlap, const int32_t *n_ref,
+                      int32_t n_entries, const int32_t *entry_rec, const int64_t *label_offsets, const int32_t *labels,
+                      const int32_t *labels2, const int32_t *n_labels, const int64_t *o_offsets, int64_t max_cells,
+                      int64_t *both_out, int64_t *fa_out, int64_t *O_out, int32_t *flags_out, void *stream);
 
 /* Number of kernels launched by this handle since creation (bench.py reports it as gpu_launches). */
 int64_t vbx_launch_count(vbx_handle_t h);

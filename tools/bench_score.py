@@ -7,6 +7,12 @@ gets its own system labelling per recording: the truth under a random relabellin
 x-vectors reassigned, so every entry has misses, false alarms and confusion to count.  All three AMI protocols are scored.
 
     python tools/bench_score.py --out profiles/h100_score.json
+
+--overlap times overlap-aware scoring (vbx_score_overlap, DESIGN.md section 5.12) against vbx_score on the same entries in
+the same process, alternating the two: every entry also gets a second label per x-vector (different from the first), and
+each recording seeded overlap regions covering about 15 % of its reference speech time.
+
+    python tools/bench_score.py --overlap --out profiles/h100_score_overlap.json
 """
 import argparse
 import json
@@ -51,15 +57,103 @@ def archive(seed=0):
     return arch, names, rows, recs, entries, t_prep
 
 
+def overlap_inputs(arch, names, recs_turns, entries, seed=1):
+    """Seeded overlap regions (about OVERLAP_SHARE of each recording's speech time) and second labels for `entries`;
+    its own generator, so the single-label entries are those of the plain benchmark."""
+    rng = np.random.default_rng(seed)
+    ovl = []
+    for n in names:
+        lo, hi = score.merge_turns(np.concatenate([t[0] for t in recs_turns[n]]), np.concatenate([t[1] for t in recs_turns[n]]))
+        speech = int(np.sum(hi - lo))
+        span = int(arch[n][0][-1, 1] * 1e6)
+        k = int(np.ceil(OVERLAP_SHARE * speech / 1.75e6))
+        a = rng.integers(0, span, k)
+        ovl.append(score.merge_turns(a, a + rng.integers(500_000, 3_000_001, k)))
+    entries2 = []
+    for b, lab in entries:
+        L = int(lab.max()) + 1
+        entries2.append((b, lab, (lab + rng.integers(1, max(L, 2), len(lab))) % max(L, 2)))
+    return ovl, entries2
+
+
+OVERLAP_SHARE = 0.15
+
+
+def main_overlap(args, dev):
+    arch, names, rows, recs, entries, _ = archive()
+    turns = score.reference_turns(rows)
+    ovl, entries2 = overlap_inputs(arch, names, turns, entries)
+    t0 = time.perf_counter()
+    recs = [score.prepare_recording(n, turns[n], score.owned_intervals(arch[n][0]), overlap=o) for n, o in zip(names, ovl)]
+    t_prep = time.perf_counter() - t0
+    speech = sum(r.regions['full'][3] for r in recs)
+    share = sum(int(np.sum(o[1] - o[0])) for o in ovl)
+    n_int = sum(len(recs[b].sys_lo) for b, _ in entries)
+    score.score_entries(recs, entries[:17], device=dev)                # warm-up of both instantiations
+    score.score_entries(recs, entries2[:17], device=dev)
+    times = {'vbx_score': [], 'vbx_score_overlap': []}
+    for _ in range(args.reps):                                         # alternating, same entries
+        for key, ent in (('vbx_score', entries), ('vbx_score_overlap', entries2)):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            r = score.score_entries(recs, ent, device=dev)
+            torch.cuda.synchronize()
+            times[key].append(time.perf_counter() - t0)
+            if key == 'vbx_score':
+                res1 = r
+            else:
+                res2 = r
+    from torch.profiler import ProfilerActivity, profile
+    kern = {'vbx_score': [], 'vbx_score_overlap': []}
+    for _ in range(args.reps):
+        for key, ent in (('vbx_score', entries), ('vbx_score_overlap', entries2)):
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                score.score_entries(recs, ent, device=dev)
+                torch.cuda.synchronize()
+            kern[key] += [e.time_range.elapsed_us() / 1000.0 for e in prof.events() if 'score_kernel' in e.name]
+    sub = entries2[:args.oracle_entries]
+    mismatches = 0
+    for i, (b, lab, lab2) in enumerate(sub):
+        seg = arch[names[b]][0]
+        s, e, l = pipeline.overlap_segments(seg, lab, lab2, ovl[b])
+        ref = [(int(score.to_ticks(r[1])), int(score.to_ticks(r[1] + r[2])), r[3]) for r in rows if r[0] == names[b]]
+        sysseg = list(zip(score.to_ticks(s).tolist(), score.to_ticks(e).tolist(), l.tolist()))
+        for p, c, io in score.PROTOCOLS:
+            mismatches += der_oracle.der_ticks(ref, sysseg, int(score.to_ticks(c)), io) != res2[i][p]['ticks']
+    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
+    lens = [len(a[0]) for a in arch.values()]
+    stat = lambda v: dict(median=round(float(np.median(v)), 4), min=round(min(v), 4), max=round(max(v), 4), n=len(v))
+    line = dict(
+        bench='overlap-aware DER scoring of a hyperparameter sweep, against single-label scoring', gpu=q.stdout.strip(),
+        archive=f'synthetic, seeded: {len(lens)} recordings, {min(lens)} .. {max(lens)} x-vectors, {sum(lens)} in all',
+        settings=N_SETTINGS, entries=len(entries), intervals_per_protocol=int(n_int), protocols=len(score.PROTOCOLS),
+        overlap_share_of_speech=round(share / speech, 4),
+        score_entries_s={k: stat(v) for k, v in times.items()},
+        kernel_ms_per_protocol={k: stat(v) for k, v in kern.items()},
+        host_region_prep_s=round(t_prep, 4),
+        oracle_entries=len(sub), oracle_mismatches=int(mismatches),
+        overall_der={k: {p: score.overall([x[p] for x in r])['der'] for p, _, _ in score.PROTOCOLS}
+                     for k, r in (('vbx_score', res1), ('vbx_score_overlap', res2))})
+    return line
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', default=None)
     ap.add_argument('--reps', default=5, type=int)
     ap.add_argument('--oracle-entries', default=17, type=int)
+    ap.add_argument('--overlap', action='store_true', help='time vbx_score_overlap against vbx_score')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('bench_score.py needs a CUDA device')
     dev = torch.device('cuda:0')
+    if args.overlap:
+        s = json.dumps(main_overlap(args, dev))
+        print(s)
+        if args.out:
+            with open(args.out, 'w') as fp:
+                fp.write(s + '\n')
+        return
     arch, names, rows, recs, entries, t_prep = archive()
     n_int = sum(len(recs[b].sys_lo) for b, _ in entries)
     score.score_entries(recs, entries[:17], device=dev)                # warm-up: module load, allocator

@@ -160,3 +160,17 @@ assert recs[3].n_ref == 64, recs[3].n_ref
 entries = [(b, gen.integers(0, L, len(seg))) for b, (seg, _) in enumerate(arch.values()) for L in (1, 128, 200)]
 res = score.score_entries(recs, entries, device=dev)
 print('score ok', res[-1]['full']['ticks'])
+
+# overlap-aware scoring (vbx_score_overlap): the same recordings with their reference overlaps as the overlap regions,
+# second labels for the 128-label (shared O block) and 200-label (global O block) entries, and -1 rows (no second label)
+recs = [score.prepare_recording(n, turns.get(n, []), score.owned_intervals(seg),
+                                overlap=score.oracle_overlaps(turns.get(n, []))) for n, (seg, _) in arch.items()]
+entries2 = []
+for b, lab in entries:
+    L = int(lab.max()) + 1 if len(lab) else 1
+    lab2 = (lab + gen.integers(1, max(L, 2), len(lab))) % max(L, 2) if L > 1 else None
+    if lab2 is not None:
+        lab2[gen.random(len(lab)) < 0.3] = -1
+    entries2.append((b, lab, lab2))
+res2 = score.score_entries(recs, entries2, device=dev)
+print('score overlap ok', res2[-1]['full']['ticks'])

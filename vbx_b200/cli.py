@@ -7,6 +7,10 @@ recording of the archive is processed in ONE batch on the GPU (front end, AHC, V
 
 Reads Kaldi ark / segments / PLDA (binary or text) / transform.h5 through vbx_b200.formats (no kaldi_io, h5py or
 fastcluster needed) and writes one RTTM per recording, formatted as VBx/vbhmm.py:48-51.
+
+With --overlap-rttm PATH (an overlapped-speech detector's RTTM file or directory; speakers ignored) each written RTTM is
+overlap-aware (DESIGN.md section 5.12): the usual lines, plus each x-vector's second most likely speaker inside the
+overlap regions.  A recording the file lacks has no overlap regions.
 """
 import argparse
 import os
@@ -36,6 +40,8 @@ def build_parser():
     ap.add_argument('--chain', default='auto', choices=['auto', 'tcgen05', 'float64'],
                     help='front end arithmetic: fused tensor-core kernels (float32-level) or float64 torch ops')
     ap.add_argument('--device', default=None, help='CUDA device, e.g. cuda:0 (default: the current device)')
+    ap.add_argument('--overlap-rttm', default=None,
+                    help='overlap regions (RTTM file or directory): also write the second speaker inside them')
     return ap
 
 
@@ -44,6 +50,8 @@ def main(argv=None):
     assert 0 <= args.loopP <= 1, f'Expecting loopP between 0 and 1, got {args.loopP} instead.'     # VBx/vbhmm.py:103
     from . import formats
     from .pipeline import diarize_batch
+    from .score import read_overlaps
+    overlaps = read_overlaps(args.overlap_rttm) if args.overlap_rttm is not None else None
     segs = formats.read_segments(args.segments_file)                        # VBx/vbhmm.py:105
     plda = formats.read_kaldi_plda(args.plda_file)                          # VBx/vbhmm.py:107
     mean1, mean2, lda = formats.read_xvec_transform(args.xvec_transform)    # VBx/vbhmm.py:125-128
@@ -55,11 +63,11 @@ def main(argv=None):
         recs[name] = (x, times)
     out = diarize_batch(recs, (mean1, mean2, lda), plda, Fa=args.Fa, Fb=args.Fb, loopP=args.loopP, lda_dim=args.lda_dim,
                         threshold=args.threshold, smoothing=args.init_smoothing, init=args.init, chain=args.chain,
-                        device=args.device, output_2nd=args.output_2nd)
+                        device=args.device, output_2nd=args.output_2nd, overlaps=overlaps)
     os.makedirs(args.out_rttm_dir, exist_ok=True)                           # VBx/vbhmm.py:170
     for name, item in out.items():
         with open(os.path.join(args.out_rttm_dir, f'{name}.rttm'), 'w') as fp:
-            fp.write(''.join(line + os.linesep for line in item['rttm']))
+            fp.write(''.join(line + os.linesep for line in item['rttm' if overlaps is None else 'rttm_overlap']))
         if item['rttm2nd'] is not None:
             d2 = f'{args.out_rttm_dir}2nd'
             os.makedirs(d2, exist_ok=True)

@@ -232,8 +232,9 @@ int launch_fb_dense(const double *lls, const double *tr, const double *ip, int T
 // DER accumulation (vbx_score.cu)
 int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const int64_t *sys_hi, const int64_t *sys_join_hi,
                  const int64_t *reg_off,
-                 const int64_t *reg_lo, const int64_t *reg_hi, const uint64_t *reg_mask, const int32_t *n_ref,
-                 int n_entries, const int32_t *entry_rec, const int64_t *label_off, const int32_t *labels,
+                 const int64_t *reg_lo, const int64_t *reg_hi, const uint64_t *reg_mask, const uint8_t *reg_ovl,
+                 const int32_t *n_ref, int n_entries, const int32_t *entry_rec, const int64_t *label_off,
+                 const int32_t *labels, const int32_t *labels2,      // labels2 == nullptr: the single-label kernel
                  const int32_t *n_labels, const int64_t *o_off, int64_t max_cells, int64_t *covered_out,
                  int64_t *fa_out, int64_t *O_out, int32_t *flags_out, cudaStream_t st);
 // AHC initialisation (vbx_ahc.cu)

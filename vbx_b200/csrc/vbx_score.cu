@@ -1,4 +1,5 @@
-// Diarization error rate accumulation (include/vbx_b200.h vbx_score, DESIGN.md section 5.11).
+// Diarization error rate accumulation (include/vbx_b200.h vbx_score, DESIGN.md section 5.11; with a second label per
+// interval inside overlap regions, vbx_score_overlap, section 5.12).
 //
 // One CTA per (setting, recording) entry.  The entry's system output is one owned time interval per x-vector with one
 // label each.  An interval whose successor has the same label extends to its `join_hi` instead of its `hi`: that
@@ -26,11 +27,20 @@ __device__ __forceinline__ unsigned long long warp_sum(unsigned long long v) {
     return v;
 }
 
+// kSecond (vbx_score_overlap): interval t also says labels2[t] (-1 = nothing) inside the regions whose ovl flag is set,
+// up to its own end (join_hi where the next interval has the same second label).  Both streams start at lo, so a region
+// piece [a, b) carries stream 1 for its first d1 = clamp(end1 - a) ticks and stream 2 for its first d2; over that piece
+// min(d1, d2) ticks have two system labels and |d1 - d2| one, which is all the md-eval counting needs:
+//   both += min(N_ref, N_sys) d,  fa += max(0, N_sys - N_ref) d,  O[r, s] += d for every active r and s,
+// i.e. with d1 + d2 label-ticks in the piece: all of them covered when N_ref >= 2, all false alarm when N_ref = 0, and
+// for N_ref = 1 the min(d1, d2) ticks of the second label are a false alarm.  `covered` then holds `both`.
+template <bool kSecond>
 __global__ void __launch_bounds__(kScoreThreads) score_kernel(
     int32_t n_rec, const int64_t *__restrict__ sys_off, const int64_t *__restrict__ sys_lo,
     const int64_t *__restrict__ sys_hi, const int64_t *__restrict__ sys_join_hi, const int64_t *__restrict__ reg_off, const int64_t *__restrict__ reg_lo,
-    const int64_t *__restrict__ reg_hi, const uint64_t *__restrict__ reg_mask, const int32_t *__restrict__ n_ref,
-    const int32_t *__restrict__ entry_rec, const int64_t *__restrict__ label_off, const int32_t *__restrict__ labels,
+    const int64_t *__restrict__ reg_hi, const uint64_t *__restrict__ reg_mask, const uint8_t *__restrict__ reg_ovl,
+    const int32_t *__restrict__ n_ref, const int32_t *__restrict__ entry_rec, const int64_t *__restrict__ label_off,
+    const int32_t *__restrict__ labels, const int32_t *__restrict__ labels2,
     const int32_t *__restrict__ n_labels, const int64_t *__restrict__ o_off, int64_t max_cells, int64_t smem_cells,
     int64_t *__restrict__ covered_out, int64_t *__restrict__ fa_out, int64_t *__restrict__ O_out,
     int32_t *__restrict__ flags_out) {
@@ -63,6 +73,7 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
     const int64_t t0 = sys_off[rec], t1 = sys_off[rec + 1];
     const int64_t r0 = reg_off[rec], r1 = reg_off[rec + 1];
     const int32_t *lab = labels + label_off[e];
+    const int32_t *lab2 = kSecond ? labels2 + label_off[e] : nullptr;
     const uint64_t live = K >= 64 ? ~0ull : ((1ull << (K < 0 ? 0 : K)) - 1ull);
     unsigned long long cov = 0ull, fa = 0ull;
     int flags = 0;
@@ -74,32 +85,75 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
         }
         const int64_t lo = sys_lo[t];
         const int64_t hi = (t + 1 < t1 && lab[t + 1 - t0] == s) ? sys_join_hi[t] : sys_hi[t];
-        if (hi <= lo) continue;
-        int64_t a = r0, b = r1;            // first region that ends after lo
-        while (a < b) {
-            const int64_t m = (a + b) >> 1;
-            if (reg_hi[m] <= lo) a = m + 1;
-            else b = m;
-        }
-        for (int64_t r = a; r < r1; ++r) {
-            const int64_t rs = reg_lo[r];
-            if (rs >= hi) break;
-            const int64_t d = min(hi, reg_hi[r]) - max(lo, rs);
-            if (d <= 0) continue;
-            uint64_t msk = reg_mask[r];
-            if (msk & ~live) {
-                flags |= VBX_SCORE_BAD_REGION;
+        if constexpr (kSecond) {
+            const int s2 = lab2[t - t0];
+            if (s2 < -1 || s2 >= L || s2 == s) {
+                flags |= VBX_SCORE_BAD_LABEL;
                 continue;
             }
-            if (msk == 0ull) {
-                fa += (unsigned long long)d;
-                continue;
+            const int64_t hi2 = s2 < 0 ? lo : (t + 1 < t1 && lab2[t + 1 - t0] == s2) ? sys_join_hi[t] : sys_hi[t];
+            const int64_t end = max(hi, hi2);
+            if (end <= lo) continue;
+            int64_t a = r0, b = r1;            // first region that ends after lo
+            while (a < b) {
+                const int64_t m = (a + b) >> 1;
+                if (reg_hi[m] <= lo) a = m + 1;
+                else b = m;
             }
-            cov += (unsigned long long)d;
-            while (msk) {
-                const int k = __ffsll((long long)msk) - 1;
-                msk &= msk - 1ull;
-                atomicAdd(&O[(int64_t)k * L + s], (unsigned long long)d);
+            for (int64_t r = a; r < r1; ++r) {
+                const int64_t rs = reg_lo[r];
+                if (rs >= end) break;
+                const int64_t p0 = max(lo, rs), re = reg_hi[r];
+                const int64_t d1 = max((int64_t)0, min(hi, re) - p0);
+                const int64_t d2 = reg_ovl[r] ? max((int64_t)0, min(hi2, re) - p0) : 0;
+                if (d1 + d2 == 0) continue;
+                uint64_t msk = reg_mask[r];
+                if (msk & ~live) {
+                    flags |= VBX_SCORE_BAD_REGION;
+                    continue;
+                }
+                const unsigned long long two = (unsigned long long)min(d1, d2), all = (unsigned long long)(d1 + d2);
+                if (msk == 0ull) fa += all;                         // N_ref = 0: every system label is a false alarm
+                else if (msk & (msk - 1ull)) cov += all;            // N_ref >= 2: every system label is covered
+                else {                                              // N_ref = 1: the second of two is a false alarm
+                    cov += all - two;
+                    fa += two;
+                }
+                while (msk) {
+                    const int k = __ffsll((long long)msk) - 1;
+                    msk &= msk - 1ull;
+                    if (d1) atomicAdd(&O[(int64_t)k * L + s], (unsigned long long)d1);
+                    if (d2) atomicAdd(&O[(int64_t)k * L + s2], (unsigned long long)d2);
+                }
+            }
+        } else {
+            if (hi <= lo) continue;
+            int64_t a = r0, b = r1;            // first region that ends after lo
+            while (a < b) {
+                const int64_t m = (a + b) >> 1;
+                if (reg_hi[m] <= lo) a = m + 1;
+                else b = m;
+            }
+            for (int64_t r = a; r < r1; ++r) {
+                const int64_t rs = reg_lo[r];
+                if (rs >= hi) break;
+                const int64_t d = min(hi, reg_hi[r]) - max(lo, rs);
+                if (d <= 0) continue;
+                uint64_t msk = reg_mask[r];
+                if (msk & ~live) {
+                    flags |= VBX_SCORE_BAD_REGION;
+                    continue;
+                }
+                if (msk == 0ull) {
+                    fa += (unsigned long long)d;
+                    continue;
+                }
+                cov += (unsigned long long)d;
+                while (msk) {
+                    const int k = __ffsll((long long)msk) - 1;
+                    msk &= msk - 1ull;
+                    atomicAdd(&O[(int64_t)k * L + s], (unsigned long long)d);
+                }
             }
         }
     }
@@ -123,33 +177,36 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
     }
 }
 
-// cudaFuncSetAttribute is per device
-bool g_score_configured[64] = {};
+// cudaFuncSetAttribute is per device and per instantiation
+bool g_score_configured[2][64] = {};
 
 }  // namespace
 
 int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const int64_t *sys_hi, const int64_t *sys_join_hi,
                  const int64_t *reg_off,
-                 const int64_t *reg_lo, const int64_t *reg_hi, const uint64_t *reg_mask, const int32_t *n_ref,
-                 int n_entries, const int32_t *entry_rec, const int64_t *label_off, const int32_t *labels,
+                 const int64_t *reg_lo, const int64_t *reg_hi, const uint64_t *reg_mask, const uint8_t *reg_ovl,
+                 const int32_t *n_ref, int n_entries, const int32_t *entry_rec, const int64_t *label_off,
+                 const int32_t *labels, const int32_t *labels2,
                  const int32_t *n_labels, const int64_t *o_off, int64_t max_cells, int64_t *covered_out,
                  int64_t *fa_out, int64_t *O_out, int32_t *flags_out, cudaStream_t st) {
     if (n_entries == 0) return 0;
+    const bool second = labels2 != nullptr;
+    auto kernel = second ? score_kernel<true> : score_kernel<false>;
     const int64_t smem_cells = max_cells < kScoreSmemCells ? max_cells : kScoreSmemCells;
     const size_t smem = (size_t)smem_cells * sizeof(unsigned long long);
     if (smem > 48 * 1024) {
         int dev = 0;
         if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return -1;
-        if (!g_score_configured[dev]) {
-            if (cudaFuncSetAttribute(score_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        if (!g_score_configured[second][dev]) {
+            if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)(kScoreSmemCells * sizeof(unsigned long long))) != cudaSuccess)
                 return -1;
-            g_score_configured[dev] = true;
+            g_score_configured[second][dev] = true;
         }
     }
-    score_kernel<<<n_entries, kScoreThreads, smem, st>>>(n_rec, sys_off, sys_lo, sys_hi, sys_join_hi, reg_off, reg_lo, reg_hi, reg_mask,
-                                                         n_ref, entry_rec, label_off, labels, n_labels, o_off, max_cells, smem_cells,
-                                                         covered_out, fa_out, O_out, flags_out);
+    kernel<<<n_entries, kScoreThreads, smem, st>>>(n_rec, sys_off, sys_lo, sys_hi, sys_join_hi, reg_off, reg_lo, reg_hi, reg_mask,
+                                                   reg_ovl, n_ref, entry_rec, label_off, labels, labels2, n_labels, o_off,
+                                                   max_cells, smem_cells, covered_out, fa_out, O_out, flags_out);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

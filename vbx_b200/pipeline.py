@@ -75,6 +75,28 @@ def merge_adjacent_labels(starts, ends, labels):
     return s, e, l
 
 
+def overlap_segments(seg_times, labels, labels2, overlap):
+    """Overlap-aware output of one recording (DESIGN.md section 5.12) as (starts, ends, labels) in seconds: the merged
+    segments of `labels` (the single-speaker output), then those of `labels2` (None: no second speaker) cut to the overlap regions
+    overlap = (lo, hi) sorted disjoint ticks.  The cut is taken in seconds; seconds map to ticks monotonically, so in
+    ticks it is the intersection with the regions."""
+    seg = np.asarray(seg_times, dtype=np.float64).reshape(-1, 2)
+    s, e, l = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels)
+    rows = list(zip(s.tolist(), e.tolist(), l.tolist()))
+    if labels2 is not None:
+        olo, ohi = (np.asarray(a, dtype=np.int64) / 1e6 for a in overlap)
+        s2, e2, l2 = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels2)
+        for a, b, k in zip(s2.tolist(), e2.tolist(), l2.tolist()):
+            i = int(np.searchsorted(ohi, a, 'right'))            # first region that ends after a
+            while i < len(olo) and olo[i] < b:
+                x, y = max(a, float(olo[i])), min(b, float(ohi[i]))
+                if y > x:
+                    rows.append((x, y, k))
+                i += 1
+    return (np.array([r[0] for r in rows], dtype=np.float64), np.array([r[1] for r in rows], dtype=np.float64),
+            np.array([r[2] for r in rows], dtype=np.int64))
+
+
 def rttm_lines(recording, starts, ends, labels):
     """VBx/vbhmm.py:48-51."""
     return [f'SPEAKER {recording} 1 {s:03f} {e - s:03f} <NA> <NA> {int(l) + 1} <NA> <NA>'
@@ -206,7 +228,7 @@ def _pad_features(fea, Phi):
 
 
 def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
-                  max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False):
+                  max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False, overlaps=None):
     """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
     recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
     one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
@@ -217,9 +239,15 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     plda = (mu, tr, psi) as read from the Kaldi model (diagonalised here as VBx/vbhmm.py:107-113 does).
     init: 'AHC' (clustering only) or 'AHC+VB' (VBx/vbhmm.py:131,147).  chain: 'tcgen05' (fused tensor-core front end,
     needs lda_dim == 128 and a 128-dim PLDA), 'float64' (float64 torch ops), 'auto' = tcgen05 when the shapes allow.
-    Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations)}."""
+    overlaps: None, or overlap regions {name: [(onset, offset)] seconds} (score.read_overlaps; a recording it lacks has
+    none): each item then also has rttm_overlap, the overlap-aware RTTM lines (overlap_segments: the second most likely
+    speaker inside the overlap regions), and overlap_seconds, the length of the recording's overlap regions.  Needs
+    init='AHC+VB' (AHC alone has no second labels).
+    Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds])}."""
     if init not in ('AHC', 'AHC+VB'):
         raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
+    if overlaps is not None and init == 'AHC':
+        raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
     if not torch.cuda.is_available():
         from ._lib import VbxError
         raise VbxError('diarize_batch(): no CUDA device - vbx_b200 has no CPU fallback')
@@ -254,12 +282,17 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
             for j, b in enumerate(idx):
                 labels1[b], labels2[b], iters[b] = sub[j][:3]
     for b, n in enumerate(names):
-        out[n] = _result(n, recordings[n][1], labels1[b], labels2[b], iters[b], output_2nd)
+        ovl = None
+        if overlaps is not None:
+            from .score import overlap_ticks
+            ovl = overlap_ticks(overlaps.get(n))
+        out[n] = _result(n, recordings[n][1], labels1[b], labels2[b], iters[b], output_2nd, ovl)
     return out
 
 
-def _result(name, seg_times, labels, labels2, iterations, output_2nd):
-    """The per-recording result of diarize_batch: RTTM lines from merged label segments (VBx/vbhmm.py:169-179)."""
+def _result(name, seg_times, labels, labels2, iterations, output_2nd, overlap=None):
+    """The per-recording result of diarize_batch: RTTM lines from merged label segments (VBx/vbhmm.py:169-179), and with
+    overlap regions ((lo, hi) ticks) the overlap-aware lines and the regions' length in seconds."""
     seg = np.asarray(seg_times, dtype=np.float64)
     s, e, l = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels)   # VBx/vbhmm.py:169
     item = dict(rttm=rttm_lines(name, s, e, l), labels=labels, labels2nd=labels2, iterations=int(iterations),
@@ -267,4 +300,7 @@ def _result(name, seg_times, labels, labels2, iterations, output_2nd):
     if output_2nd and labels2 is not None:
         s2, e2, l2 = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels2)   # VBx/vbhmm.py:174-179
         item['rttm2nd'] = rttm_lines(name, s2, e2, l2)
+    if overlap is not None:
+        item['rttm_overlap'] = rttm_lines(name, *overlap_segments(seg, labels, labels2, overlap))
+        item['overlap_seconds'] = int(np.sum(overlap[1] - overlap[0])) * 1e-6
     return item

@@ -1,4 +1,4 @@
-"""Diarization error rate (DER) of single-speaker system output against reference RTTMs, accumulated on the GPU.
+"""Diarization error rate (DER) of system output against reference RTTMs, accumulated on the GPU.
 
 The scoring contract (DESIGN.md section 5.11): every boundary is converted once to int64 microseconds ("ticks"); reference
 turns of one speaker that overlap or touch are merged; a collar c removes [x - c, x + c] around every merged reference
@@ -9,10 +9,17 @@ Over the scored time, with N_ref reference speakers active and the system silent
 with ref_total the scored reference speaker time.  The kernel (vbx_score) accumulates covered, fa and O for many
 (setting, recording) entries in one launch; the reference regions, ref_total and the matching are host work.
 
-    python -m vbx_b200.score --ref-rttm ref/ --sys-rttm out/ [--uem all.uem] [--collar 0.25] [--ignore-overlaps] [--json]
+Overlap-aware output (DESIGN.md section 5.12) adds a second label per interval, said only inside overlap regions (an
+overlapped-speech detector's RTTM, or the reference's own overlaps).  With N_sys in {0, 1, 2} system labels the counts
+become  both += min(N_ref, N_sys) d,  fa += max(0, N_sys - N_ref) d,  O[r, s] += d for every active r and s;
+miss = ref_total - both, conf = both - matching (vbx_score_overlap).
+
+    python -m vbx_b200.score --ref-rttm ref/ --sys-rttm out/ [--uem all.uem] [--collar 0.25] [--ignore-overlaps]
+        [--overlapping-system] [--json]
 
 PATH is an RTTM file or a directory of *.rttm.  Every reference recording is scored (one without system output counts as
-all missed); system output for a recording the reference lacks is an error.
+all missed); system output for a recording the reference lacks is an error.  A system RTTM with overlapping speakers
+needs --overlapping-system (at most two at a time).
 """
 import argparse
 import ctypes
@@ -30,8 +37,10 @@ PROTOCOLS = (('forgiving', 0.25, True), ('fair', 0.25, False), ('full', 0.0, Fal
 
 # One recording prepared for scoring: the system's owned intervals [sys_lo, sys_hi) in ticks with their joined ends
 # (sys_join_hi, see owned_intervals), the number of reference speakers and, per protocol name, the scored regions
-# (lo, hi, mask, ref_total).
-ScoredRecording = namedtuple('ScoredRecording', 'name sys_lo sys_hi sys_join_hi n_ref regions')
+# (lo, hi, mask, ref_total); overlap_regions: None, or per protocol name the scored regions split at the boundaries of
+# the recording's overlap regions, (lo, hi, mask, ovl) with ovl = uint8 1 inside them (see split_regions).
+ScoredRecording = namedtuple('ScoredRecording', 'name sys_lo sys_hi sys_join_hi n_ref regions overlap_regions',
+                             defaults=(None,))
 
 
 def to_ticks(seconds):
@@ -71,6 +80,63 @@ def reference_turns(rows):
             raise ValueError(f'recording {rec!r}: {len(turns)} reference speakers, at most {MAX_REF_SPEAKERS} are supported')
         out[rec] = turns
     return out
+
+
+def overlap_ticks(intervals):
+    """Overlap regions [(onset, offset)] seconds (None = none) -> (lo, hi) int64 ticks, sorted and disjoint: the union
+    of the intervals (merge_turns)."""
+    t = to_ticks(np.asarray(intervals if intervals is not None else [], dtype=np.float64).reshape(-1, 2))
+    return merge_turns(t[:, 0], t[:, 1])
+
+
+def overlaps_from_rows(rows):
+    """formats.read_rttm rows (an overlapped-speech detector's output; the speaker field is ignored) -> {recording:
+    [(onset, offset)] seconds}, each recording's turns unioned.  A recording without rows has no overlap regions."""
+    per = {}
+    for rec, start, dur, _ in rows:
+        per.setdefault(rec, []).append((start, start + dur))
+    out = {}
+    for rec, iv in per.items():
+        lo, hi = overlap_ticks(iv)
+        out[rec] = [(a / 1e6, b / 1e6) for a, b in zip(lo.tolist(), hi.tolist())]
+    return out
+
+
+def oracle_overlaps(turns):
+    """reference_turns()[name] -> (lo, hi) ticks: the time in which two or more (merged) reference turns are active."""
+    if not turns:
+        z = np.zeros(0, dtype=np.int64)
+        return z, z
+    x = np.concatenate([a for t in turns for a in t])
+    step = np.concatenate([np.full(len(t[0]), k, dtype=np.int64) for t in turns for k in (1, -1)])
+    o = np.argsort(x, kind='stable')
+    x, n = x[o], np.cumsum(step[o])
+    on = n[:-1] >= 2                    # n[i] speakers on [x[i], x[i+1]); empty pieces at equal times are dropped
+    return merge_turns(x[:-1][on], x[1:][on])
+
+
+def split_regions(regions, overlap):
+    """Scored regions (lo, hi, mask, ...) split at the boundaries of the overlap regions overlap = (lo, hi) ticks ->
+    (lo, hi, mask, ovl): the same scored time and masks, ovl = uint8 1 where the piece lies inside an overlap region;
+    neighbours with equal mask and flag joined (so with no overlap regions the regions come back unchanged)."""
+    lo, hi, mask = (np.asarray(a) for a in regions[:3])
+    olo, ohi = (np.asarray(a, dtype=np.int64) for a in overlap)
+    if len(lo) == 0:
+        return lo, hi, mask, np.zeros(0, dtype=np.uint8)
+    b = np.unique(np.concatenate([lo, hi, olo, ohi]))
+    plo, phi = b[:-1], b[1:]
+    j = np.searchsorted(lo, plo, 'right') - 1
+    keep = (j >= 0) & (hi[np.maximum(j, 0)] > plo)
+    plo, phi, j = plo[keep], phi[keep], j[keep]
+    pmask = mask[j]
+    if len(olo):
+        k = np.searchsorted(olo, plo, 'right') - 1
+        ovl = ((k >= 0) & (ohi[np.maximum(k, 0)] > plo)).astype(np.uint8)
+    else:
+        ovl = np.zeros(len(plo), dtype=np.uint8)
+    first = np.nonzero(np.concatenate([[True], (plo[1:] != phi[:-1]) | (pmask[1:] != pmask[:-1])
+                                       | (ovl[1:] != ovl[:-1])]))[0]
+    return plo[first], np.concatenate([phi[first[1:] - 1], phi[-1:]]), pmask[first], ovl[first]
 
 
 def owned_intervals(seg_times):
@@ -151,10 +217,11 @@ def collar_ticks(collar):
     return int(to_ticks(collar))
 
 
-def prepare_recording(name, turns, timeline, uem=None, protocols=PROTOCOLS):
+def prepare_recording(name, turns, timeline, uem=None, protocols=PROTOCOLS, overlap=None):
     """A ScoredRecording.  turns: reference_turns()[name]; timeline: the system's intervals in ticks as (lo, hi,
     join_hi): owned_intervals() of the x-vectors, or (lo, hi, hi) for the turns of a system RTTM; uem: None (all time is
-    scored) or [(onset, offset)] seconds; protocols: (name, collar seconds, ignore_overlaps) triples."""
+    scored) or [(onset, offset)] seconds; protocols: (name, collar seconds, ignore_overlaps) triples; overlap: None, or
+    the overlap regions as sorted disjoint (lo, hi) ticks (overlap_ticks, oracle_overlaps) for overlap-aware entries."""
     if len(turns) > MAX_REF_SPEAKERS:
         raise ValueError(f'recording {name!r}: {len(turns)} reference speakers, at most {MAX_REF_SPEAKERS} are supported')
     sys_lo, sys_hi, sys_join_hi = (np.asarray(a, dtype=np.int64) for a in timeline)
@@ -165,7 +232,8 @@ def prepare_recording(name, turns, timeline, uem=None, protocols=PROTOCOLS):
         u = to_ticks(np.asarray(uem, dtype=np.float64).reshape(-1, 2))
         scored = merge_turns(u[:, 0], u[:, 1])
     regions = {p: scored_regions(turns, collar_ticks(c), io, scored) for p, c, io in protocols}
-    return ScoredRecording(name, sys_lo, sys_hi, sys_join_hi, len(turns), regions)
+    split = None if overlap is None else {p: split_regions(g, overlap) for p, g in regions.items()}
+    return ScoredRecording(name, sys_lo, sys_hi, sys_join_hi, len(turns), regions, split)
 
 
 def result(miss, fa, conf, scored):
@@ -182,7 +250,8 @@ def overall(results):
 
 
 def finish(covered, fa, O, ref_total):
-    """result() from the accumulated covered / fa ticks and the overlap matrix O [n_ref x n_labels] (int64)."""
+    """result() from the accumulated covered (overlap-aware: both) / fa ticks and the overlap matrix O [n_ref x n_labels]
+    (int64)."""
     from scipy.optimize import linear_sum_assignment
     O = np.asarray(O, dtype=np.int64)
     matched = 0
@@ -199,11 +268,21 @@ def rank(per_setting):
     return sorted(names, key=lambda n: (per_setting[n]['der'] is None, per_setting[n]['der'] or 0.0))
 
 
+def _overlap_split(rec, proto):
+    if rec.overlap_regions is not None:
+        return rec.overlap_regions[proto]
+    lo, hi, mask, _ = rec.regions[proto]
+    return lo, hi, mask, np.zeros(len(lo), dtype=np.uint8)
+
+
 def score_entries(recordings, entries, device=None):
     """Score many (recording, labels) entries in one vbx_score launch per protocol.
     recordings: list of ScoredRecording (all with the same protocols); entries: [(recording index, labels)], labels int
     [len(sys_lo)] in [0, n) (n = max label + 1).  Returns [{protocol: result dict}] in entry order.  A label outside
-    that range raises VbxError."""
+    that range raises VbxError.
+    Overlap-aware entries (recording index, labels, labels2) go to one vbx_score_overlap launch per protocol instead:
+    labels2 (None = no second speaker, or int with -1 = none) is said inside the recording's overlap regions
+    (prepare_recording(overlap=); none when it was not given).  A call takes one kind of entry only."""
     import torch
     from . import _lib
     from ._lib import VbxError
@@ -217,14 +296,21 @@ def score_entries(recordings, entries, device=None):
     lens = np.array([len(r.sys_lo) for r in recordings], dtype=np.int64)
     sys_off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
     n_ref = np.array([r.n_ref for r in recordings], dtype=np.int32)
-    rec_idx = np.array([b for b, _ in entries], dtype=np.int32)
-    labs = [np.asarray(l).reshape(-1) for _, l in entries]
+    second = len(entries[0]) == 3
+    if any(len(e) != len(entries[0]) or len(e) not in (2, 3) for e in entries):
+        raise ValueError('entries must all be (recording, labels) or all (recording, labels, labels2)')
+    rec_idx = np.array([e[0] for e in entries], dtype=np.int32)
+    labs = [np.asarray(e[1]).reshape(-1) for e in entries]
+    labs2 = [np.full(len(l), -1, dtype=np.int64) if e[2] is None else np.asarray(e[2]).reshape(-1)
+             for e, l in zip(entries, labs)] if second else []
     for i, (b, l) in enumerate(zip(rec_idx, labs)):
         if not 0 <= b < len(recordings):
             raise ValueError(f'entry {i}: recording index {b} out of range')
-        if len(l) != lens[b]:
+        if len(l) != lens[b] or (second and len(labs2[i]) != lens[b]):
             raise ValueError(f'entry {i}: {len(l)} labels for {lens[b]} intervals of {recordings[b].name!r}')
     n_labels = np.array([max(int(l.max()) + 1, 1) if len(l) else 1 for l in labs], dtype=np.int32)
+    if second:
+        n_labels = np.maximum(n_labels, [int(l.max()) + 1 if len(l) else 1 for l in labs2]).astype(np.int32)
     label_off = np.concatenate([[0], np.cumsum([len(l) for l in labs])[:-1]]).astype(np.int64)
     cells = n_ref[rec_idx].astype(np.int64) * n_labels
     o_off = np.concatenate([[0], np.cumsum(cells)[:-1]]).astype(np.int64)
@@ -234,7 +320,9 @@ def score_entries(recordings, entries, device=None):
     d = lambda a: torch.from_numpy(np.concatenate([a, np.zeros(1, a.dtype)])).to(dev)
     p = lambda t: ctypes.c_void_p(t.data_ptr())
     common = [d(sys_off)] + [d(np.concatenate([getattr(r, f) for r in recordings])) for f in ('sys_lo', 'sys_hi', 'sys_join_hi')]
-    ent = [d(rec_idx), d(label_off), d(np.concatenate(labs).astype(np.int32)), d(n_labels), d(o_off)]
+    ent = [d(rec_idx), d(label_off), d(np.concatenate(labs).astype(np.int32))]
+    ent += [d(np.concatenate(labs2).astype(np.int32))] if second else []
+    ent += [d(n_labels), d(o_off)]
     nref_d = d(n_ref)
     h = ctypes.c_void_p()
     if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
@@ -244,17 +332,19 @@ def score_entries(recordings, entries, device=None):
         with torch.cuda.device(dev):
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             for proto in protocols:
-                regs = [r.regions[proto] for r in recordings]
+                regs = [_overlap_split(r, proto) if second else r.regions[proto] for r in recordings]
                 reg_off = np.concatenate([[0], np.cumsum([len(g[0]) for g in regs])]).astype(np.int64)
                 rd = [d(reg_off)] + [d(np.concatenate([g[i] for g in regs]).view(np.int64)) for i in range(3)]
+                rd += [d(np.concatenate([g[3] for g in regs]).astype(np.uint8))] if second else []
                 cov = torch.empty(len(entries), dtype=torch.int64, device=dev)
                 fa = torch.empty_like(cov)
                 O = torch.empty(max(int(cells.sum()), 1), dtype=torch.int64, device=dev)
                 flags = torch.empty(len(entries), dtype=torch.int32, device=dev)
-                rc = lib.vbx_score(h, len(recordings), *map(p, common), *map(p, rd), p(nref_d), len(entries), *map(p, ent),
-                                   int(cells.max()), p(cov), p(fa), p(O), p(flags), stream)
+                fn = lib.vbx_score_overlap if second else lib.vbx_score
+                rc = fn(h, len(recordings), *map(p, common), *map(p, rd), p(nref_d), len(entries), *map(p, ent),
+                        int(cells.max()), p(cov), p(fa), p(O), p(flags), stream)
                 if rc != 0:
-                    raise VbxError(f'vbx_score failed ({rc}): {lib.vbx_last_error(h).decode()}')
+                    raise VbxError(f'{fn.__name__} failed ({rc}): {lib.vbx_last_error(h).decode()}')
                 outs[proto] = (cov, fa, O, flags, rd)      # rd stays referenced until the results are read
             host = {k: tuple(t.cpu().numpy() for t in v[:4]) for k, v in outs.items()}
     finally:
@@ -266,7 +356,9 @@ def score_entries(recordings, entries, device=None):
         if len(bad):
             i = int(bad[0])
             why = f'labels must lie in [0, {int(n_labels[i])})' if flags[i] & _lib.SCORE_BAD_LABEL else 'bad input'
-            raise VbxError(f'vbx_score: entry {i} ({recordings[rec_idx[i]].name!r}) flags {int(flags[i])}: {why}')
+            if second and flags[i] & _lib.SCORE_BAD_LABEL:
+                why += ', second labels in [-1, n) and different from the first'
+            raise VbxError(f'{"vbx_score_overlap" if second else "vbx_score"}: entry {i} ({recordings[rec_idx[i]].name!r}) flags {int(flags[i])}: {why}')
         for i, b in enumerate(rec_idx):
             blk = O[o_off[i]:o_off[i] + cells[i]].reshape(int(n_ref[b]), int(n_labels[i]))
             res[i][proto] = finish(cov[i], fa[i], blk, recordings[b].regions[proto][3])
@@ -304,10 +396,38 @@ def system_turns(rows, recording=''):
     return lo, hi, lab
 
 
-def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=None):
+def system_stretches(rows, recording=''):
+    """System RTTM rows of one recording whose speakers may overlap -> (lo, hi, labels, labels2): sorted disjoint
+    stretches in ticks in which one or two labels speak (labels numbered by name, turns of one label merged; labels2 =
+    -1 where one speaks, else the larger number).  Three or more simultaneous speakers raise ValueError."""
+    names = sorted(set(r[3] for r in rows))
+    turns = []
+    for spk in names:
+        t = to_ticks(np.array([(r[1], r[1] + r[2]) for r in rows if r[3] == spk], dtype=np.float64))
+        turns.append(merge_turns(t[:, 0], t[:, 1]))
+    b = np.unique(np.concatenate([a for t in turns for a in t] + [np.zeros(0, dtype=np.int64)]))
+    lo, hi = b[:-1], b[1:]
+    l1, l2 = np.full(len(lo), -1, dtype=np.int32), np.full(len(lo), -1, dtype=np.int32)
+    n = np.zeros(len(lo), dtype=np.int64)
+    for k, (s, e) in enumerate(turns):
+        j = np.searchsorted(s, lo, 'right') - 1
+        act = (j >= 0) & (e[np.maximum(j, 0)] > lo)
+        l2 = np.where(act & (l1 >= 0), k, l2)
+        l1 = np.where(act & (l1 < 0), k, l1)
+        n += act
+    if np.any(n > 2):
+        i = int(np.argmax(n > 2))
+        raise ValueError(f'recording {recording!r}: {int(n[i])} system speakers at {lo[i] / 1e6:.6f} s; '
+                         'at most two simultaneous system speakers can be scored')
+    keep = n > 0
+    return lo[keep], hi[keep], l1[keep], l2[keep]
+
+
+def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=None, overlapping=False):
     """DER of system RTTM rows against reference RTTM rows (both as formats.read_rttm returns them).
-    uem: None or {recording: [(onset, offset)]} (formats.read_uem).  Returns ({recording: result dict}, overall result
-    dict) over the reference's recordings."""
+    uem: None or {recording: [(onset, offset)]} (formats.read_uem).  overlapping: the system may have two speakers at
+    once (system_stretches, scored by vbx_score_overlap); otherwise overlapping system turns raise ValueError.  Returns
+    ({recording: result dict}, overall result dict) over the reference's recordings."""
     collar_ticks(collar)
     ref = reference_turns(ref_turns)
     sys_by = _rows_by_recording(sys_turns)
@@ -319,9 +439,15 @@ def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=N
     for b, n in enumerate(names):
         if uem is not None and n not in uem:
             raise ValueError(f'recording {n!r} is missing from the UEM')
+        proto = (('score', collar, bool(ignore_overlaps)),)
+        u = None if uem is None else uem[n]
+        if overlapping:                 # stream 2 is said wherever the system has a second speaker: no clipping
+            lo, hi, lab, lab2 = system_stretches(sys_by.get(n, []), n)
+            recs.append(prepare_recording(n, ref[n], (lo, hi, hi), u, proto, overlap=(lo[:1], hi[-1:])))
+            entries.append((b, lab, lab2))
+            continue
         lo, hi, lab = system_turns(sys_by.get(n, []), n)
-        recs.append(prepare_recording(n, ref[n], (lo, hi, hi), None if uem is None else uem[n],
-                                      (('score', collar, bool(ignore_overlaps)),)))
+        recs.append(prepare_recording(n, ref[n], (lo, hi, hi), u, proto))
         entries.append((b, lab))
     per = {n: r['score'] for n, r in zip(names, score_entries(recs, entries, device))}
     return per, overall(list(per.values()))
@@ -336,6 +462,11 @@ def read_rttm_path(path):
     return [row for f in files for row in formats.read_rttm(f)]
 
 
+def read_overlaps(path):
+    """Overlap regions from an RTTM file or directory (overlaps_from_rows): {recording: [(onset, offset)] seconds}."""
+    return overlaps_from_rows(read_rttm_path(path))
+
+
 def build_parser():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument('--ref-rttm', required=True, help='reference RTTM file or directory of *.rttm')
@@ -343,6 +474,8 @@ def build_parser():
     ap.add_argument('--uem', default=None, help='UEM file (default: all time is scored)')
     ap.add_argument('--collar', default=0.25, type=float, help='seconds removed either side of every reference boundary')
     ap.add_argument('--ignore-overlaps', action='store_true', help='do not score time with 2 or more reference speakers')
+    ap.add_argument('--overlapping-system', action='store_true',
+                    help='the system RTTM may have two speakers at once (overlap-aware output)')
     ap.add_argument('--json', action='store_true', help='print one JSON object instead of the table')
     return ap
 
@@ -352,7 +485,7 @@ def main(argv=None):
     from . import formats
     uem = formats.read_uem(args.uem) if args.uem else None
     per, tot = score_rttm(read_rttm_path(args.ref_rttm), read_rttm_path(args.sys_rttm), args.collar,
-                          args.ignore_overlaps, uem)
+                          args.ignore_overlaps, uem, overlapping=args.overlapping_system)
     if args.json:
         print(json.dumps(dict(collar=args.collar, ignore_overlaps=args.ignore_overlaps, files=per, overall=tot),
                          sort_keys=True))

@@ -13,6 +13,9 @@ linkage (ahc.cut).  Every (recording, setting) pair is one entry of a batch with
 With --ref-rttm (a file or a directory of *.rttm; optionally --uem) every entry is also scored on the GPU (vbx_b200/score.py)
 under the three AMI protocols: summary.json then holds the DER per recording and setting, the overall DER per setting, and
 `ranking`: per protocol, the setting names by overall DER.
+With --overlap-rttm PATH (an overlapped-speech detector's RTTM) or --oracle-overlaps (the reference's own overlaps; needs
+--ref-rttm) every setting also writes OUT/<setting>/overlap/<recording>.rttm, the overlap-aware output (DESIGN.md section
+5.12); with a reference it is scored too, and summary.json gains der_overlap and ranking_overlap next to der and ranking.
 """
 import argparse
 import itertools
@@ -105,7 +108,8 @@ def entry_bytes(T, n_states, R, device):
 
 
 def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
-                device=None, max_batch_bytes=None, output_2nd=False, ref_rttm=None, uem=None):
+                device=None, max_batch_bytes=None, output_2nd=False, ref_rttm=None, uem=None, overlaps=None,
+                oracle_overlaps=False):
     """Every setting of `grid` (see grid_settings) for every recording, with the front end and AHC run once.
 
     recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
@@ -117,8 +121,13 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     have run, in one vbx_score launch per protocol (score.PROTOCOLS), and each recording's dict gains
     der = {protocol: score.result dict}.  A recording that the reference (or the UEM) lacks raises ValueError before any
     work; reference recordings that `recordings` lacks are ignored.
-    Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags[, der])}}; each recording's
-    dict is the one diarize_batch returns with that setting's scalars."""
+    overlaps: None or {recording: [(onset, offset)] seconds} (score.read_overlaps); oracle_overlaps: use the time in which
+    the reference has two or more speakers instead (needs ref_rttm).  Either makes each recording's dict also hold
+    rttm_overlap and overlap_seconds as diarize_batch(overlaps=) does and, with a reference, der_overlap = {protocol:
+    score.result dict} of that output, scored in one more vbx_score_overlap launch per protocol.  Needs init='AHC+VB'.
+    Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags[, der][, rttm_overlap,
+    overlap_seconds][, der_overlap])}}; each recording's dict is the one diarize_batch returns with that setting's
+    scalars."""
     import torch
     from . import ahc as _ahc
     from ._lib import VbxError, padded_states
@@ -127,6 +136,13 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     settings = grid_settings(grid)
     if init not in ('AHC', 'AHC+VB'):
         raise ValueError('Wrong option for args.initialization.')
+    if oracle_overlaps and ref_rttm is None:
+        raise ValueError('oracle_overlaps are the overlaps of the reference: they need ref_rttm')
+    if oracle_overlaps and overlaps is not None:
+        raise ValueError('give overlaps or oracle_overlaps, not both')
+    with_overlap = oracle_overlaps or overlaps is not None
+    if with_overlap and init == 'AHC':
+        raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
     if not torch.cuda.is_available():
         raise VbxError('sweep_batch(): no CUDA device - vbx_b200 has no CPU fallback')
     dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
@@ -184,25 +200,35 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
             group = [e for e in tiers[2] if e[0] == k]
             if group:
                 run(group, True, Fa=s.Fa, Fb=s.Fb, loopProb=s.loopP)
-    der = None
+    from . import score
+    ovl = [None] * len(names)
+    if with_overlap:
+        ovl = [score.oracle_overlaps(ref[0][n]) if oracle_overlaps else score.overlap_ticks(overlaps.get(n))
+               for n in names]
+    der = der_ovl = None
     if ref is not None:
-        from . import score
         turns, uem_map = ref
         scored = []
-        for n in names:
+        for n, o in zip(names, ovl):
             timeline = score.owned_intervals(recordings[n][1])
-            scored.append(score.prepare_recording(n, turns[n], timeline, None if uem_map is None else uem_map[n]))
+            scored.append(score.prepare_recording(n, turns[n], timeline, None if uem_map is None else uem_map[n],
+                                                  overlap=o))
         keys = [(k, b) for k in range(len(settings)) for b in range(len(names))]
         der = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0]) for k, b in keys], device=dev)))
+        if with_overlap:
+            der_ovl = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0], res[(k, b)][1]) for k, b in keys],
+                                                         device=dev)))
     out = {}
     for k, s in enumerate(settings):
         out[s] = {}
         for b, n in enumerate(names):
             l1, l2, it, fl = res[(k, b)]
-            item = _result(n, recordings[n][1], l1, l2, it, output_2nd)
+            item = _result(n, recordings[n][1], l1, l2, it, output_2nd, ovl[b])
             item['flags'] = int(fl)
             if der is not None:
                 item['der'] = der[(k, b)]
+            if der_ovl is not None:
+                item['der_overlap'] = der_ovl[(k, b)]
             out[s][n] = item
     return out
 
@@ -225,11 +251,11 @@ def _load_reference(names, ref_rttm, uem):
     return turns, uem
 
 
-def summarize_der(out):
-    """sweep_batch output with `der` -> ({setting name: {protocol: overall result dict}}, {protocol: setting names by
-    overall DER, stable in grid order})."""
+def summarize_der(out, key='der'):
+    """sweep_batch output with `key` ('der' or 'der_overlap') -> ({setting name: {protocol: overall result dict}},
+    {protocol: setting names by overall DER, stable in grid order})."""
     from . import score
-    tot = {s.name: {p: score.overall([item['der'][p] for item in per_rec.values()]) for p, _, _ in score.PROTOCOLS}
+    tot = {s.name: {p: score.overall([item[key][p] for item in per_rec.values()]) for p, _, _ in score.PROTOCOLS}
            for s, per_rec in out.items()}
     ranking = {p: score.rank({n: tot[n][p] for n in tot}) for p, _, _ in score.PROTOCOLS}
     return tot, ranking
@@ -256,6 +282,10 @@ def build_parser():
     ap.add_argument('--max-batch-bytes', default=None, type=int)
     ap.add_argument('--ref-rttm', default=None, help='reference RTTM file or directory of *.rttm: score every setting')
     ap.add_argument('--uem', default=None, help='UEM file restricting the scored time (with --ref-rttm)')
+    ap.add_argument('--overlap-rttm', default=None,
+                    help='overlap regions (RTTM file or directory): also write and score overlap-aware output')
+    ap.add_argument('--oracle-overlaps', action='store_true',
+                    help="use the reference's overlaps (with --ref-rttm) as the overlap regions")
     return ap
 
 
@@ -270,10 +300,12 @@ def main(argv=None):
         seg_names, times = segs[name]
         assert np.all(np.array(seg_names) == np.array(keys))
         recs[name] = (x, times)
+    from .score import read_overlaps
+    overlaps = read_overlaps(args.overlap_rttm) if args.overlap_rttm is not None else None
     grid = dict(Fa=args.Fa, Fb=args.Fb, loopP=args.loopP, threshold=args.threshold, smoothing=args.init_smoothing)
     out = sweep_batch(recs, transform, plda, grid, lda_dim=args.lda_dim, max_iters=args.max_iters, epsilon=args.epsilon,
                       init=args.init, chain=args.chain, device=args.device, max_batch_bytes=args.max_batch_bytes,
-                      ref_rttm=args.ref_rttm, uem=args.uem)
+                      ref_rttm=args.ref_rttm, uem=args.uem, overlaps=overlaps, oracle_overlaps=args.oracle_overlaps)
     summary = {}
     for s, per_rec in out.items():
         d = os.path.join(args.out_dir, s.name)
@@ -284,12 +316,21 @@ def main(argv=None):
                 fp.write(''.join(line + os.linesep for line in item['rttm']))
             summary[s.name]['recordings'][name] = dict(speakers=item['n_speakers'], iterations=item['iterations'],
                                                        flags=item['flags'])
-            if 'der' in item:
-                summary[s.name]['recordings'][name]['der'] = item['der']
+            for key in ('der', 'der_overlap', 'overlap_seconds'):
+                if key in item:
+                    summary[s.name]['recordings'][name][key] = item[key]
+            if 'rttm_overlap' in item:
+                os.makedirs(os.path.join(d, 'overlap'), exist_ok=True)
+                with open(os.path.join(d, 'overlap', f'{name}.rttm'), 'w') as fp:
+                    fp.write(''.join(line + os.linesep for line in item['rttm_overlap']))
     if args.ref_rttm is not None:
         tot, summary['ranking'] = summarize_der(out)
         for name, d in tot.items():
             summary[name]['der'] = d
+        if overlaps is not None or args.oracle_overlaps:
+            tot, summary['ranking_overlap'] = summarize_der(out, 'der_overlap')
+            for name, d in tot.items():
+                summary[name]['der_overlap'] = d
     with open(os.path.join(args.out_dir, 'summary.json'), 'w') as fp:
         json.dump(summary, fp, indent=1, sort_keys=True)
     return 0
