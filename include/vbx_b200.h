@@ -206,7 +206,7 @@ int vbx_elbo_trace(vbx_handle_t h, const double *Li, int32_t max_iters, double *
  * VBX_ERR_STATE before a vbx_prepare_* call on the current plan and workspace. */
 int vbx_get_gsum(vbx_handle_t h, double *gsum_out, void *stream);
 
-/* per-entry bits written to flags_out by vbx_score and vbx_score_overlap */
+/* per-entry bits written to flags_out by vbx_score, vbx_score_overlap and vbx_score_jer */
 enum vbx_score_flag {
     VBX_SCORE_BAD_LABEL = 1,     /* a label outside [0, n_labels[e]) (a second label outside [-1, n_labels[e]) or
                                     equal to the first): that interval was not counted                            */
@@ -265,6 +265,26 @@ int vbx_score_overlap(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets,
                       int32_t n_entries, const int32_t *entry_rec, const int64_t *label_offsets, const int32_t *labels,
                       const int32_t *labels2, const int32_t *n_labels, const int64_t *o_offsets, int64_t max_cells,
                       int64_t *both_out, int64_t *fa_out, int64_t *O_out, int32_t *flags_out, void *stream);
+
+/* DER accumulation plus the per-label time that the Jaccard error rate needs (DESIGN.md section 5.13).  Arguments and
+ * outputs as for vbx_score_overlap; reg_overlap and labels2 may both be NULL for single-label entries (then everything
+ * vbx_score writes is written, bit-identical to it).  Plus:
+ *   t_offsets [n_entries] (DEVICE)   label_time_out[t_offsets[e] ..] is entry e's block of n_labels[e] int64; blocks of
+ *                                    different entries must not overlap
+ *   label_time_out (DEVICE, output)  S[s] = scored time in which the system says label s, in either stream (a label is
+ *                                    never said twice at one instant: labels2 differs from labels), non-speech included.
+ * Blocks of up to 128 labels are accumulated in shared memory, larger ones in place in label_time_out (same results).
+ * An entry flagged VBX_SCORE_BAD_RECORDING leaves its label-time block unwritten.  For the Jaccard error rate the
+ * scored regions are those of collar 0 with overlaps scored: O[k, s] is then |ref_k intersect sys_s|.
+ * Integer sums only: results are bit-identical whatever the batch and the launch order.  VBX_ERR_ARG as for vbx_score,
+ * and when only one of reg_overlap and labels2 is NULL. */
+int vbx_score_jer(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets, const int64_t *sys_lo,
+                  const int64_t *sys_hi, const int64_t *sys_join_hi, const int64_t *reg_offsets, const int64_t *reg_lo,
+                  const int64_t *reg_hi, const uint64_t *reg_mask, const uint8_t *reg_overlap, const int32_t *n_ref,
+                  int32_t n_entries, const int32_t *entry_rec, const int64_t *label_offsets, const int32_t *labels,
+                  const int32_t *labels2, const int32_t *n_labels, const int64_t *o_offsets, int64_t max_cells,
+                  int64_t *both_out, int64_t *fa_out, int64_t *O_out, int32_t *flags_out, const int64_t *t_offsets,
+                  int64_t *label_time_out, void *stream);
 
 /* Number of kernels launched by this handle since creation (bench.py reports it as gpu_launches). */
 int64_t vbx_launch_count(vbx_handle_t h);

@@ -13,6 +13,13 @@ the same process, alternating the two: every entry also gets a second label per 
 each recording seeded overlap regions covering about 15 % of its reference speech time.
 
     python tools/bench_score.py --overlap --out profiles/h100_score_overlap.json
+
+--jer times label-time accumulation for the Jaccard error rate (vbx_score_jer, DESIGN.md section 5.13) on the same
+archive and second labels: the kernel of each launch kind (vbx_score, vbx_score_overlap, vbx_score_jer single-label and
+two-stream) on the `full` regions, alternating, and whole score_entries calls with and without jer='full', broken down
+into uploads, kernels, readback, DER matchings and JER matchings.
+
+    python tools/bench_score.py --jer --out profiles/h100_score_jer.json
 """
 import argparse
 import json
@@ -137,18 +144,102 @@ def main_overlap(args, dev):
     return line
 
 
+def timed(fn, acc):
+    def wrapper(*a, **k):
+        t0 = time.perf_counter()
+        try:
+            return fn(*a, **k)
+        finally:
+            acc.append(time.perf_counter() - t0)
+    return wrapper
+
+
+def main_jer(args, dev):
+    from torch.profiler import ProfilerActivity, profile
+    arch, names, rows, recs, entries, _ = archive()
+    turns = score.reference_turns(rows)
+    ovl, entries2 = overlap_inputs(arch, names, turns, entries)
+    full = (('full', 0.0, False),)
+    one = [score.prepare_recording(n, turns[n], score.owned_intervals(arch[n][0]), protocols=full, overlap=o)
+           for n, o in zip(names, ovl)]
+    calls = {'vbx_score': lambda: score.score_entries(one, entries, device=dev),
+             'vbx_score_overlap': lambda: score.score_entries(one, entries2, device=dev),
+             'vbx_score_jer': lambda: score.score_entries(one, entries, device=dev, jer='full'),
+             'vbx_score_jer (two-stream)': lambda: score.score_entries(one, entries2, device=dev, jer='full')}
+    for f in calls.values():                                           # warm-up of every instantiation
+        f()
+    kern, kname = {k: [] for k in calls}, {}
+    for _ in range(args.launches):                                     # alternating, one launch per call
+        for key, f in calls.items():
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                f()
+                torch.cuda.synchronize()
+            ev = [e for e in prof.events() if 'score_kernel' in e.name]
+            kern[key] += [e.time_range.elapsed_us() / 1000.0 for e in ev]
+            kname[key] = sorted({'score_kernel' + e.name.split('score_kernel')[1].split('(')[0] for e in ev})
+    # whole score_entries calls over the three protocols, with and without jer, alternating
+    recs = [score.prepare_recording(n, turns[n], score.owned_intervals(arch[n][0])) for n in names]
+    whole = {'without jer': [], 'with jer': []}
+    res = {}
+    for _ in range(args.reps):
+        for key, jer in (('without jer', None), ('with jer', 'full')):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            res[key] = score.score_entries(recs, entries, device=dev, jer=jer)
+            torch.cuda.synchronize()
+            whole[key].append(time.perf_counter() - t0)
+    # breakdown of one call each: host time in the matchings (wrapped), device time of kernels and copies (profiler)
+    parts = {}
+    real = (score.finish, score.jer_finish, score.reference_time)
+    for key, jer in (('without jer', None), ('with jer', 'full')):
+        der_t, jer_t = [], []
+        score.finish, score.jer_finish, score.reference_time = (timed(real[0], der_t), timed(real[1], jer_t),
+                                                                timed(real[2], jer_t))
+        try:
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                score.score_entries(recs, entries, device=dev, jer=jer)
+                torch.cuda.synchronize()
+                total = time.perf_counter() - t0
+        finally:
+            score.finish, score.jer_finish, score.reference_time = real
+        ev = list(prof.events())
+        dev_ms = lambda pat: round(sum(e.time_range.elapsed_us() for e in ev if pat in e.name) / 1000.0, 3)
+        parts[key] = dict(total_s_profiled=round(total, 4), kernels_ms=dev_ms('score_kernel'),
+                          uploads_ms_device=dev_ms('HtoD'), readback_ms_device=dev_ms('DtoH'),
+                          der_matchings_s=round(sum(der_t), 4), der_matchings=len(der_t),
+                          jer_matchings_s=round(sum(jer_t), 4),
+                          rest_s=round(total - sum(der_t) - sum(jer_t), 4))
+    same_der = all({p: r[p] for p, _, _ in score.PROTOCOLS} == q for r, q in zip(res['with jer'], res['without jer']))
+    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
+    lens = [len(a[0]) for a in arch.values()]
+    stat = lambda v: dict(median=round(float(np.median(v)), 4), min=round(min(v), 4), max=round(max(v), 4), n=len(v))
+    return dict(
+        bench='JER label-time scoring of a hyperparameter sweep, against the DER launches', gpu=q.stdout.strip(),
+        archive=f'synthetic, seeded: {len(lens)} recordings, {min(lens)} .. {max(lens)} x-vectors, {sum(lens)} in all',
+        settings=N_SETTINGS, entries=len(entries), intervals_per_launch=int(sum(len(recs[b].sys_lo) for b, _ in entries)),
+        kernel_ms_full_regions={k: stat(v) for k, v in kern.items()}, kernel_names=kname,
+        score_entries_s={k: stat(v) for k, v in whole.items()},
+        breakdown=parts, der_unchanged_with_jer=bool(same_der),
+        overall_jer=score.overall_jer([r['jer'] for r in res['with jer']])['jer'],
+        overall_der={p: score.overall([r[p] for r in res['with jer']])['der'] for p, _, _ in score.PROTOCOLS})
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--out', default=None)
     ap.add_argument('--reps', default=5, type=int)
     ap.add_argument('--oracle-entries', default=17, type=int)
     ap.add_argument('--overlap', action='store_true', help='time vbx_score_overlap against vbx_score')
+    ap.add_argument('--jer', action='store_true', help='time vbx_score_jer against vbx_score and vbx_score_overlap')
+    ap.add_argument('--launches', default=15, type=int, help='--jer: profiled launches of each kind')
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('bench_score.py needs a CUDA device')
     dev = torch.device('cuda:0')
-    if args.overlap:
-        s = json.dumps(main_overlap(args, dev))
+    if args.overlap or args.jer:
+        s = json.dumps(main_jer(args, dev) if args.jer else main_overlap(args, dev))
         print(s)
         if args.out:
             with open(args.out, 'w') as fp:

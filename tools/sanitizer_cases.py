@@ -1,6 +1,7 @@
 """Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection at
 D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
-6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels, the dense forward_backward() and the ELBO trace.
+6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels, the dense forward_backward(), the ELBO trace
+and DER / JER scoring.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
 """
@@ -174,3 +175,13 @@ for b, lab in entries:
     entries2.append((b, lab, lab2))
 res2 = score.score_entries(recs, entries2, device=dev)
 print('score overlap ok', res2[-1]['full']['ticks'])
+
+# label time for the Jaccard error rate (vbx_score_jer): single-label entries, 128-label blocks in shared memory and
+# 200-label blocks in place in global memory, then two-stream entries
+recs = [score.prepare_recording(n, turns.get(n, []), score.owned_intervals(seg)) for n, (seg, _) in arch.items()]
+res3 = score.score_entries(recs, entries, device=dev, jer='full')
+print('score jer ok', res3[-1]['jer']['jer'])
+recs = [score.prepare_recording(n, turns.get(n, []), score.owned_intervals(seg),
+                                overlap=score.oracle_overlaps(turns.get(n, []))) for n, (seg, _) in arch.items()]
+res4 = score.score_entries(recs, entries2, device=dev, jer='full')
+print('score jer overlap ok', res4[-1]['jer']['jer'])

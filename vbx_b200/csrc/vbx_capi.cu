@@ -869,7 +869,8 @@ int vbx_score(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets, const i
     if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     return counted(h, vbx::launch_score(n_rec, sys_offsets, sys_lo, sys_hi, sys_join_hi, reg_offsets, reg_lo, reg_hi, reg_mask,
                                         nullptr, n_ref, n_entries, entry_rec, label_offsets, labels, nullptr, n_labels,
-                                        o_offsets, max_cells, covered_out, fa_out, O_out, flags_out, (cudaStream_t)stream),
+                                        o_offsets, max_cells, covered_out, fa_out, O_out, flags_out, nullptr, nullptr,
+                                        (cudaStream_t)stream),
                    "score");
 }
 
@@ -892,8 +893,36 @@ int vbx_score_overlap(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets,
     if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     return counted(h, vbx::launch_score(n_rec, sys_offsets, sys_lo, sys_hi, sys_join_hi, reg_offsets, reg_lo, reg_hi, reg_mask,
                                         reg_overlap, n_ref, n_entries, entry_rec, label_offsets, labels, labels2, n_labels,
-                                        o_offsets, max_cells, both_out, fa_out, O_out, flags_out, (cudaStream_t)stream),
+                                        o_offsets, max_cells, both_out, fa_out, O_out, flags_out, nullptr, nullptr,
+                                        (cudaStream_t)stream),
                    "score_overlap");
+}
+
+int vbx_score_jer(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets, const int64_t *sys_lo,
+                  const int64_t *sys_hi, const int64_t *sys_join_hi, const int64_t *reg_offsets, const int64_t *reg_lo,
+                  const int64_t *reg_hi, const uint64_t *reg_mask, const uint8_t *reg_overlap, const int32_t *n_ref,
+                  int32_t n_entries, const int32_t *entry_rec, const int64_t *label_offsets, const int32_t *labels,
+                  const int32_t *labels2, const int32_t *n_labels, const int64_t *o_offsets, int64_t max_cells,
+                  int64_t *both_out, int64_t *fa_out, int64_t *O_out, int32_t *flags_out, const int64_t *t_offsets,
+                  int64_t *label_time_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_score_jer");
+    if (n_rec < 0 || n_entries < 0 || max_cells < 0) return fail(h, VBX_ERR_ARG, "vbx_score_jer: negative count");
+    if (n_entries == 0) return VBX_OK;
+    if (n_rec == 0) return fail(h, VBX_ERR_ARG, "vbx_score_jer: entries need at least one recording");
+    if (!sys_offsets || !sys_lo || !sys_hi || !sys_join_hi || !reg_offsets || !reg_lo || !reg_hi || !reg_mask || !n_ref ||
+        !entry_rec || !label_offsets || !labels || !n_labels || !o_offsets || !t_offsets || !label_time_out || !both_out ||
+        !fa_out || !flags_out || (max_cells > 0 && !O_out))
+        return fail(h, VBX_ERR_ARG, "vbx_score_jer: null pointer");
+    if (!reg_overlap != !labels2)
+        return fail(h, VBX_ERR_ARG, "vbx_score_jer: reg_overlap and labels2 must both be given or both be NULL");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_score(n_rec, sys_offsets, sys_lo, sys_hi, sys_join_hi, reg_offsets, reg_lo, reg_hi, reg_mask,
+                                        reg_overlap, n_ref, n_entries, entry_rec, label_offsets, labels, labels2, n_labels,
+                                        o_offsets, max_cells, both_out, fa_out, O_out, flags_out, t_offsets,
+                                        label_time_out, (cudaStream_t)stream),
+                   labels2 ? "score_jer_overlap" : "score_jer");
 }
 
 int vbx_attach_comm(vbx_handle_t h, void *nccl_comm, int32_t n_ranks, const char *libnccl_path) {

@@ -236,7 +236,9 @@ int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const
                  const int32_t *n_ref, int n_entries, const int32_t *entry_rec, const int64_t *label_off,
                  const int32_t *labels, const int32_t *labels2,      // labels2 == nullptr: the single-label kernel
                  const int32_t *n_labels, const int64_t *o_off, int64_t max_cells, int64_t *covered_out,
-                 int64_t *fa_out, int64_t *O_out, int32_t *flags_out, cudaStream_t st);
+                 int64_t *fa_out, int64_t *O_out, int32_t *flags_out,
+                 const int64_t *t_off, int64_t *T_out,                // T_out == nullptr: no label time
+                 cudaStream_t st);
 // AHC initialisation (vbx_ahc.cu)
 size_t ahc_workspace_bytes(const int64_t *offsets_host, int n_rec, std::vector<int64_t> *d_off_host);
 int launch_ahc(const Plan &pl, const std::vector<int64_t> &d_off, const void *x, int x_is_f64, int dim, void *workspace,

@@ -13,6 +13,8 @@
 // All sums are 64-bit integer atomics, so results do not depend on the order of the additions: bit-reproducible across
 // runs, batch compositions and launch shapes.  Each entry's O [n_ref x n_labels] sits in shared memory when it fits the
 // launch's shared block and is accumulated directly in its global block otherwise; either way one CTA owns it.
+// With label time (vbx_score_jer, section 5.13) each entry also sums, per label, the scored time in which the system says
+// it (S [n_labels]); that block follows the same shared-or-global policy.
 #include "../../include/vbx_b200.h"
 #include "vbx_internal.cuh"
 
@@ -21,10 +23,31 @@ namespace {
 
 constexpr int kScoreThreads = 256;
 constexpr int64_t kScoreSmemCells = 64 * 128;      // 64 KB of int64: 64 reference speakers x 128 labels
+constexpr int64_t kScoreSmemLabels = 128;          // 1 KB of int64 label time after the O cells (label-time launches)
 
 __device__ __forceinline__ unsigned long long warp_sum(unsigned long long v) {
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
+}
+
+// Adds v to T[key] once per group of lanes in `act` with the same key (key < 0: nothing).  Consecutive intervals mostly
+// share a label, so one atomic usually serves the whole warp.  The group's sum is a tree over its lanes in rank order
+// (each round, every lane adds the value of the next remaining lane of its group; odd ranks drop out), which ends at
+// the group's lowest lane.  Integer sums: the result does not depend on the grouping.
+__device__ __forceinline__ void add_label_time(unsigned long long *T, int key, unsigned long long v) {
+    const unsigned act = __activemask();
+    const unsigned peers = __match_any_sync(act, key);
+    const unsigned lane = threadIdx.x & 31u;
+    unsigned rank = __popc(peers & ((1u << lane) - 1u));
+    unsigned rest = peers & ~((2u << lane) - 1u);       // lanes of my group above me (2u << 31 wraps to 0: none)
+    while (__any_sync(act, rest)) {
+        const int next = __ffs(rest);
+        const unsigned long long o = __shfl_sync(act, v, next ? next - 1 : (int)lane);
+        if (next) v += o;
+        rest &= __ballot_sync(act, !(rank & 1u));
+        rank >>= 1;
+    }
+    if (key >= 0 && v && lane == (unsigned)(__ffs(peers) - 1)) atomicAdd(&T[key], v);
 }
 
 // kSecond (vbx_score_overlap): interval t also says labels2[t] (-1 = nothing) inside the regions whose ovl flag is set,
@@ -34,7 +57,11 @@ __device__ __forceinline__ unsigned long long warp_sum(unsigned long long v) {
 //   both += min(N_ref, N_sys) d,  fa += max(0, N_sys - N_ref) d,  O[r, s] += d for every active r and s,
 // i.e. with d1 + d2 label-ticks in the piece: all of them covered when N_ref >= 2, all false alarm when N_ref = 0, and
 // for N_ref = 1 the min(d1, d2) ticks of the second label are a false alarm.  `covered` then holds `both`.
-template <bool kSecond>
+// kLabelTime (vbx_score_jer): also S[s] += d1 and S[s2] += d2 over every scored region piece, non-speech included, summed
+// per interval in registers and added once per interval (add_label_time).  S [n_labels] of entry e sits after the O cells
+// in shared memory when n_labels <= kScoreSmemLabels, else it is accumulated in place at T_out + t_off[e].  The extra
+// parameters come last, so the other instantiations keep their parameter layout.
+template <bool kSecond, bool kLabelTime>
 __global__ void __launch_bounds__(kScoreThreads) score_kernel(
     int32_t n_rec, const int64_t *__restrict__ sys_off, const int64_t *__restrict__ sys_lo,
     const int64_t *__restrict__ sys_hi, const int64_t *__restrict__ sys_join_hi, const int64_t *__restrict__ reg_off, const int64_t *__restrict__ reg_lo,
@@ -43,7 +70,7 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
     const int32_t *__restrict__ labels, const int32_t *__restrict__ labels2,
     const int32_t *__restrict__ n_labels, const int64_t *__restrict__ o_off, int64_t max_cells, int64_t smem_cells,
     int64_t *__restrict__ covered_out, int64_t *__restrict__ fa_out, int64_t *__restrict__ O_out,
-    int32_t *__restrict__ flags_out) {
+    int32_t *__restrict__ flags_out, const int64_t *__restrict__ t_off, int64_t *__restrict__ T_out) {
     extern __shared__ unsigned long long sO[];
     __shared__ unsigned long long s_cov, s_fa;
     __shared__ int s_flags;
@@ -63,6 +90,11 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
     const bool shared_block = cells <= smem_cells;
     unsigned long long *O = shared_block ? sO : reinterpret_cast<unsigned long long *>(O_out + o_off[e]);
     for (int64_t i = threadIdx.x; i < cells; i += blockDim.x) O[i] = 0ull;
+    unsigned long long *S = nullptr;
+    if constexpr (kLabelTime) {
+        S = L <= kScoreSmemLabels ? sO + smem_cells : reinterpret_cast<unsigned long long *>(T_out + t_off[e]);
+        for (int i = threadIdx.x; i < L; i += blockDim.x) S[i] = 0ull;
+    }
     if (threadIdx.x == 0) {
         s_cov = 0ull;
         s_fa = 0ull;
@@ -100,6 +132,7 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
                 if (reg_hi[m] <= lo) a = m + 1;
                 else b = m;
             }
+            unsigned long long v1 = 0ull, v2 = 0ull;            // label time of this interval (kLabelTime)
             for (int64_t r = a; r < r1; ++r) {
                 const int64_t rs = reg_lo[r];
                 if (rs >= end) break;
@@ -107,6 +140,10 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
                 const int64_t d1 = max((int64_t)0, min(hi, re) - p0);
                 const int64_t d2 = reg_ovl[r] ? max((int64_t)0, min(hi2, re) - p0) : 0;
                 if (d1 + d2 == 0) continue;
+                if constexpr (kLabelTime) {
+                    v1 += (unsigned long long)d1;
+                    v2 += (unsigned long long)d2;
+                }
                 uint64_t msk = reg_mask[r];
                 if (msk & ~live) {
                     flags |= VBX_SCORE_BAD_REGION;
@@ -126,6 +163,10 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
                     if (d2) atomicAdd(&O[(int64_t)k * L + s2], (unsigned long long)d2);
                 }
             }
+            if constexpr (kLabelTime) {
+                add_label_time(S, s, v1);
+                add_label_time(S, s2, v2);
+            }
         } else {
             if (hi <= lo) continue;
             int64_t a = r0, b = r1;            // first region that ends after lo
@@ -134,11 +175,13 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
                 if (reg_hi[m] <= lo) a = m + 1;
                 else b = m;
             }
+            unsigned long long v1 = 0ull;                       // label time of this interval (kLabelTime)
             for (int64_t r = a; r < r1; ++r) {
                 const int64_t rs = reg_lo[r];
                 if (rs >= hi) break;
                 const int64_t d = min(hi, reg_hi[r]) - max(lo, rs);
                 if (d <= 0) continue;
+                if constexpr (kLabelTime) v1 += (unsigned long long)d;
                 uint64_t msk = reg_mask[r];
                 if (msk & ~live) {
                     flags |= VBX_SCORE_BAD_REGION;
@@ -155,6 +198,7 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
                     atomicAdd(&O[(int64_t)k * L + s], (unsigned long long)d);
                 }
             }
+            if constexpr (kLabelTime) add_label_time(S, s, v1);
         }
     }
     cov = warp_sum(cov);
@@ -170,6 +214,12 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
         int64_t *dst = O_out + o_off[e];
         for (int64_t i = threadIdx.x; i < cells; i += blockDim.x) dst[i] = (int64_t)sO[i];
     }
+    if constexpr (kLabelTime) {
+        if (L <= kScoreSmemLabels) {
+            int64_t *dst = T_out + t_off[e];
+            for (int i = threadIdx.x; i < L; i += blockDim.x) dst[i] = (int64_t)S[i];
+        }
+    }
     if (threadIdx.x == 0) {
         covered_out[e] = (int64_t)s_cov;
         fa_out[e] = (int64_t)s_fa;
@@ -177,8 +227,8 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
     }
 }
 
-// cudaFuncSetAttribute is per device and per instantiation
-bool g_score_configured[2][64] = {};
+// cudaFuncSetAttribute is per device and per instantiation: [kSecond + 2 kLabelTime][device]
+bool g_score_configured[4][64] = {};
 
 }  // namespace
 
@@ -188,25 +238,31 @@ int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const
                  const int32_t *n_ref, int n_entries, const int32_t *entry_rec, const int64_t *label_off,
                  const int32_t *labels, const int32_t *labels2,
                  const int32_t *n_labels, const int64_t *o_off, int64_t max_cells, int64_t *covered_out,
-                 int64_t *fa_out, int64_t *O_out, int32_t *flags_out, cudaStream_t st) {
+                 int64_t *fa_out, int64_t *O_out, int32_t *flags_out, const int64_t *t_off, int64_t *T_out,
+                 cudaStream_t st) {
     if (n_entries == 0) return 0;
-    const bool second = labels2 != nullptr;
-    auto kernel = second ? score_kernel<true> : score_kernel<false>;
+    const bool second = labels2 != nullptr, label_time = T_out != nullptr;
+    const int variant = (int)second + 2 * (int)label_time;
+    auto kernel = label_time ? (second ? score_kernel<true, true> : score_kernel<false, true>)
+                             : (second ? score_kernel<true, false> : score_kernel<false, false>);
     const int64_t smem_cells = max_cells < kScoreSmemCells ? max_cells : kScoreSmemCells;
-    const size_t smem = (size_t)smem_cells * sizeof(unsigned long long);
+    // label-time launches add 1 KB after the O cells: 65 KB at most, still three CTAs per SM where O alone fits three
+    const int64_t smem_words = smem_cells + (label_time ? kScoreSmemLabels : 0);
+    const int64_t max_words = kScoreSmemCells + (label_time ? kScoreSmemLabels : 0);
+    const size_t smem = (size_t)smem_words * sizeof(unsigned long long);
     if (smem > 48 * 1024) {
         int dev = 0;
         if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return -1;
-        if (!g_score_configured[second][dev]) {
+        if (!g_score_configured[variant][dev]) {
             if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)(kScoreSmemCells * sizeof(unsigned long long))) != cudaSuccess)
+                                     (int)(max_words * sizeof(unsigned long long))) != cudaSuccess)
                 return -1;
-            g_score_configured[second][dev] = true;
+            g_score_configured[variant][dev] = true;
         }
     }
     kernel<<<n_entries, kScoreThreads, smem, st>>>(n_rec, sys_off, sys_lo, sys_hi, sys_join_hi, reg_off, reg_lo, reg_hi, reg_mask,
                                                    reg_ovl, n_ref, entry_rec, label_off, labels, labels2, n_labels, o_off,
-                                                   max_cells, smem_cells, covered_out, fa_out, O_out, flags_out);
+                                                   max_cells, smem_cells, covered_out, fa_out, O_out, flags_out, t_off, T_out);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 

@@ -14,8 +14,12 @@ overlapped-speech detector's RTTM, or the reference's own overlaps).  With N_sys
 become  both += min(N_ref, N_sys) d,  fa += max(0, N_sys - N_ref) d,  O[r, s] += d for every active r and s;
 miss = ref_total - both, conf = both - matching (vbx_score_overlap).
 
+Jaccard error rate (DESIGN.md section 5.13), dscore's second metric: per recording the mean over reference speakers of
+1 - |ref and sys| / |ref or sys| (scored time) after the one-to-one mapping that minimises it, without a collar and with overlaps scored.
+vbx_score_jer adds each system label's scored time to the DER counts; R per speaker and the mapping are host work.
+
     python -m vbx_b200.score --ref-rttm ref/ --sys-rttm out/ [--uem all.uem] [--collar 0.25] [--ignore-overlaps]
-        [--overlapping-system] [--json]
+        [--overlapping-system] [--jer] [--json]
 
 PATH is an RTTM file or a directory of *.rttm.  Every reference recording is scored (one without system output counts as
 all missed); system output for a recording the reference lacks is an error.  A system RTTM with overlapping speakers
@@ -38,9 +42,10 @@ PROTOCOLS = (('forgiving', 0.25, True), ('fair', 0.25, False), ('full', 0.0, Fal
 # One recording prepared for scoring: the system's owned intervals [sys_lo, sys_hi) in ticks with their joined ends
 # (sys_join_hi, see owned_intervals), the number of reference speakers and, per protocol name, the scored regions
 # (lo, hi, mask, ref_total); overlap_regions: None, or per protocol name the scored regions split at the boundaries of
-# the recording's overlap regions, (lo, hi, mask, ovl) with ovl = uint8 1 inside them (see split_regions).
-ScoredRecording = namedtuple('ScoredRecording', 'name sys_lo sys_hi sys_join_hi n_ref regions overlap_regions',
-                             defaults=(None,))
+# the recording's overlap regions, (lo, hi, mask, ovl) with ovl = uint8 1 inside them (see split_regions);
+# protocols: None, or per protocol name (collar ticks, ignore_overlaps), which decides where JER may be taken.
+ScoredRecording = namedtuple('ScoredRecording', 'name sys_lo sys_hi sys_join_hi n_ref regions overlap_regions protocols',
+                             defaults=(None, None))
 
 
 def to_ticks(seconds):
@@ -233,7 +238,8 @@ def prepare_recording(name, turns, timeline, uem=None, protocols=PROTOCOLS, over
         scored = merge_turns(u[:, 0], u[:, 1])
     regions = {p: scored_regions(turns, collar_ticks(c), io, scored) for p, c, io in protocols}
     split = None if overlap is None else {p: split_regions(g, overlap) for p, g in regions.items()}
-    return ScoredRecording(name, sys_lo, sys_hi, sys_join_hi, len(turns), regions, split)
+    return ScoredRecording(name, sys_lo, sys_hi, sys_join_hi, len(turns), regions, split,
+                           {p: (collar_ticks(c), bool(io)) for p, c, io in protocols})
 
 
 def result(miss, fa, conf, scored):
@@ -262,10 +268,64 @@ def finish(covered, fa, O, ref_total):
     return result(int(ref_total) - covered, fa, covered - matched, ref_total)
 
 
-def rank(per_setting):
-    """{name: result dict} -> names by DER ascending (stable in the given order; settings without a DER last)."""
+def rank(per_setting, key='der'):
+    """{name: result dict} -> names by result[key] ascending, 'der' (result, overall) or 'jer' (jer_finish, overall_jer);
+    stable in the given order, settings without a value last."""
     names = list(per_setting)
-    return sorted(names, key=lambda n: (per_setting[n]['der'] is None, per_setting[n]['der'] or 0.0))
+    return sorted(names, key=lambda n: (per_setting[n][key] is None, per_setting[n][key] or 0.0))
+
+
+def reference_time(regions, n_ref):
+    """Scored time of each reference speaker (list of n_ref Python ints) over a region set (lo, hi, mask, ...)."""
+    lo, hi = (np.asarray(a, dtype=np.int64) for a in regions[:2])
+    mask = np.asarray(regions[2], dtype=np.uint64)
+    return [int(np.sum((hi - lo)[((mask >> np.uint64(k)) & np.uint64(1)) == 1])) for k in range(n_ref)]
+
+
+def speaker_jer(t):
+    """One counted reference speaker's Jaccard error from its ticks (an element of jer_finish()['ticks']): 1 unmapped,
+    else 1 - I / (R + S - I)."""
+    if t['label'] is None:
+        return 1.0
+    u = t['R'] + t['S'] - t['I']
+    return (u - t['I']) / u
+
+
+def _jer_value(ticks):
+    return sum(speaker_jer(t) for t in ticks) / len(ticks) if ticks else None
+
+
+def jer_finish(R, S, O):
+    """Jaccard error rate of one recording (DESIGN.md section 5.13) from exact ticks under scored time without a collar
+    and with overlaps scored: R [K] reference speakers' scored time, S [L] the system labels' scored time, O [K x L]
+    their intersections.  Speakers with R = 0 and labels with S = 0 are not counted; the one-to-one mapping minimises
+    the summed cost c = (R + S - 2 I) / (R + S - I) (scipy.optimize.linear_sum_assignment); a mapped speaker's error is
+    its c, an unmapped one's 1.  Returns dict(jer=mean over counted speakers or None without one, speakers=their number,
+    ticks=[dict(ref=k, R, label=s or None, S, I) per counted speaker, by k]); jer is a pure function of ticks."""
+    from scipy.optimize import linear_sum_assignment
+    R = np.asarray(R, dtype=np.int64).reshape(-1)
+    S = np.asarray(S, dtype=np.int64).reshape(-1)
+    O = np.asarray(O, dtype=np.int64).reshape(len(R), len(S))
+    ks, ls = np.nonzero(R > 0)[0], np.nonzero(S > 0)[0]
+    label = {}
+    if len(ks) and len(ls):
+        Rk, Sl, I = R[ks][:, None], S[ls][None, :], O[np.ix_(ks, ls)]
+        cost = (Rk + Sl - 2 * I).astype(np.float64) / (Rk + Sl - I).astype(np.float64)
+        rows, cols = linear_sum_assignment(cost)
+        label = {int(ks[r]): int(ls[c]) for r, c in zip(rows, cols)}
+    ticks = []
+    for k in ks.tolist():
+        s = label.get(k)
+        ticks.append(dict(ref=k, R=int(R[k]), label=s, S=None if s is None else int(S[s]),
+                          I=None if s is None else int(O[k, s])))
+    return dict(jer=_jer_value(ticks), speakers=len(ticks), ticks=ticks)
+
+
+def overall_jer(results):
+    """JER of several recordings from their jer_finish() dicts: the mean over all their counted reference speakers, so
+    every speaker weighs the same whatever its recording.  dict(jer, speakers); jer None without any speaker."""
+    ticks = [t for r in results for t in r['ticks']]
+    return dict(jer=_jer_value(ticks), speakers=len(ticks))
 
 
 def _overlap_split(rec, proto):
@@ -275,17 +335,26 @@ def _overlap_split(rec, proto):
     return lo, hi, mask, np.zeros(len(lo), dtype=np.uint8)
 
 
-def score_entries(recordings, entries, device=None):
+def score_entries(recordings, entries, device=None, jer=None):
     """Score many (recording, labels) entries in one vbx_score launch per protocol.
     recordings: list of ScoredRecording (all with the same protocols); entries: [(recording index, labels)], labels int
     [len(sys_lo)] in [0, n) (n = max label + 1).  Returns [{protocol: result dict}] in entry order.  A label outside
     that range raises VbxError.
     Overlap-aware entries (recording index, labels, labels2) go to one vbx_score_overlap launch per protocol instead:
     labels2 (None = no second speaker, or int with -1 = none) is said inside the recording's overlap regions
-    (prepare_recording(overlap=); none when it was not given).  A call takes one kind of entry only."""
+    (prepare_recording(overlap=); none when it was not given).  A call takes one kind of entry only.
+    jer: None, or the name of a protocol with collar 0 and overlaps scored (DESIGN.md section 5.13).  That protocol's
+    launch goes to vbx_score_jer, which also sums each label's scored time, and every entry's dict gains
+    'jer': jer_finish() (replacing the DER of a protocol that is itself named 'jer').  Any other protocol raises
+    ValueError."""
     import torch
     from . import _lib
     from ._lib import VbxError
+    if jer is not None:
+        for r in recordings:
+            if (r.protocols or {}).get(jer) != (0, False):
+                raise ValueError(f'jer={jer!r}: the Jaccard error rate needs a protocol of these recordings with collar '
+                                 '0 and overlaps scored')
     if not entries:
         return []
     if not torch.cuda.is_available():
@@ -324,6 +393,9 @@ def score_entries(recordings, entries, device=None):
     ent += [d(np.concatenate(labs2).astype(np.int32))] if second else []
     ent += [d(n_labels), d(o_off)]
     nref_d = d(n_ref)
+    if jer is not None:
+        t_off = np.concatenate([[0], np.cumsum(n_labels.astype(np.int64))[:-1]]).astype(np.int64)
+        t_off_d = d(t_off)
     h = ctypes.c_void_p()
     if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
         raise VbxError('vbx_create failed: no usable sm_90 device')
@@ -340,28 +412,45 @@ def score_entries(recordings, entries, device=None):
                 fa = torch.empty_like(cov)
                 O = torch.empty(max(int(cells.sum()), 1), dtype=torch.int64, device=dev)
                 flags = torch.empty(len(entries), dtype=torch.int32, device=dev)
-                fn = lib.vbx_score_overlap if second else lib.vbx_score
-                rc = fn(h, len(recordings), *map(p, common), *map(p, rd), p(nref_d), len(entries), *map(p, ent),
-                        int(cells.max()), p(cov), p(fa), p(O), p(flags), stream)
+                if proto == jer:
+                    fn = lib.vbx_score_jer
+                    T = torch.empty(max(int(n_labels.sum()), 1), dtype=torch.int64, device=dev)
+                    # single-label entries pass NULL for reg_overlap and labels2
+                    args = [*map(p, rd), None] if not second else list(map(p, rd))
+                    args += [p(nref_d), len(entries)] + list(map(p, ent[:3])) + ([] if second else [None])
+                    args += list(map(p, ent[3:])) + [int(cells.max()), p(cov), p(fa), p(O), p(flags), p(t_off_d), p(T)]
+                    rc = fn(h, len(recordings), *map(p, common), *args, stream)
+                    outs[proto] = (cov, fa, O, flags, T, rd)
+                else:
+                    fn = lib.vbx_score_overlap if second else lib.vbx_score
+                    rc = fn(h, len(recordings), *map(p, common), *map(p, rd), p(nref_d), len(entries), *map(p, ent),
+                            int(cells.max()), p(cov), p(fa), p(O), p(flags), stream)
+                    outs[proto] = (cov, fa, O, flags, rd)      # rd stays referenced until the results are read
                 if rc != 0:
                     raise VbxError(f'{fn.__name__} failed ({rc}): {lib.vbx_last_error(h).decode()}')
-                outs[proto] = (cov, fa, O, flags, rd)      # rd stays referenced until the results are read
-            host = {k: tuple(t.cpu().numpy() for t in v[:4]) for k, v in outs.items()}
+            host = {k: tuple(t.cpu().numpy() for t in v[:-1]) for k, v in outs.items()}
     finally:
         lib.vbx_destroy(h)
     res = [{} for _ in entries]
     for proto in protocols:
-        cov, fa, O, flags = host[proto]
+        cov, fa, O, flags = host[proto][:4]
         bad = np.nonzero(flags)[0]
         if len(bad):
             i = int(bad[0])
             why = f'labels must lie in [0, {int(n_labels[i])})' if flags[i] & _lib.SCORE_BAD_LABEL else 'bad input'
             if second and flags[i] & _lib.SCORE_BAD_LABEL:
                 why += ', second labels in [-1, n) and different from the first'
-            raise VbxError(f'{"vbx_score_overlap" if second else "vbx_score"}: entry {i} ({recordings[rec_idx[i]].name!r}) flags {int(flags[i])}: {why}')
+            name = 'vbx_score_jer' if proto == jer else 'vbx_score_overlap' if second else 'vbx_score'
+            raise VbxError(f'{name}: entry {i} ({recordings[rec_idx[i]].name!r}) flags {int(flags[i])}: {why}')
         for i, b in enumerate(rec_idx):
             blk = O[o_off[i]:o_off[i] + cells[i]].reshape(int(n_ref[b]), int(n_labels[i]))
             res[i][proto] = finish(cov[i], fa[i], blk, recordings[b].regions[proto][3])
+    if jer is not None:
+        O, T = host[jer][2], host[jer][4]
+        R = [reference_time(r.regions[jer], r.n_ref) for r in recordings]
+        for i, b in enumerate(rec_idx):
+            blk = O[o_off[i]:o_off[i] + cells[i]].reshape(int(n_ref[b]), int(n_labels[i]))
+            res[i]['jer'] = jer_finish(R[b], T[t_off[i]:t_off[i] + n_labels[i]], blk)
     return res
 
 
@@ -423,12 +512,18 @@ def system_stretches(rows, recording=''):
     return lo[keep], hi[keep], l1[keep], l2[keep]
 
 
-def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=None, overlapping=False):
+def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=None, overlapping=False, jer=False):
     """DER of system RTTM rows against reference RTTM rows (both as formats.read_rttm returns them).
     uem: None or {recording: [(onset, offset)]} (formats.read_uem).  overlapping: the system may have two speakers at
     once (system_stretches, scored by vbx_score_overlap); otherwise overlapping system turns raise ValueError.  Returns
-    ({recording: result dict}, overall result dict) over the reference's recordings."""
-    collar_ticks(collar)
+    ({recording: result dict}, overall result dict) over the reference's recordings.
+    jer: also the Jaccard error rate (DESIGN.md section 5.13; no collar, overlaps scored, whatever the DER uses): every
+    result dict gains jer (None without a counted reference speaker) and each recording's also jer_ticks
+    (jer_finish()['ticks'])."""
+    c = collar_ticks(collar)
+    # JER is taken without a collar and with overlaps: from the DER's own launch when that is the protocol, else from
+    # one more region set
+    jer_proto = None if not jer else 'score' if c == 0 and not ignore_overlaps else 'jer'
     ref = reference_turns(ref_turns)
     sys_by = _rows_by_recording(sys_turns)
     extra = sorted(set(sys_by) - set(ref))
@@ -439,7 +534,7 @@ def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=N
     for b, n in enumerate(names):
         if uem is not None and n not in uem:
             raise ValueError(f'recording {n!r} is missing from the UEM')
-        proto = (('score', collar, bool(ignore_overlaps)),)
+        proto = (('score', collar, bool(ignore_overlaps)),) + ((('jer', 0.0, False),) if jer_proto == 'jer' else ())
         u = None if uem is None else uem[n]
         if overlapping:                 # stream 2 is said wherever the system has a second speaker: no clipping
             lo, hi, lab, lab2 = system_stretches(sys_by.get(n, []), n)
@@ -449,8 +544,14 @@ def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=N
         lo, hi, lab = system_turns(sys_by.get(n, []), n)
         recs.append(prepare_recording(n, ref[n], (lo, hi, hi), u, proto))
         entries.append((b, lab))
-    per = {n: r['score'] for n, r in zip(names, score_entries(recs, entries, device))}
-    return per, overall(list(per.values()))
+    res = score_entries(recs, entries, device, jer=jer_proto)
+    per = {n: r['score'] for n, r in zip(names, res)}
+    tot = overall(list(per.values()))
+    if jer:
+        for n, r in zip(names, res):
+            per[n] = dict(per[n], jer=r['jer']['jer'], jer_ticks=r['jer']['ticks'])
+        tot['jer'] = overall_jer([r['jer'] for r in res])['jer']
+    return per, tot
 
 
 def read_rttm_path(path):
@@ -477,6 +578,8 @@ def build_parser():
     ap.add_argument('--overlapping-system', action='store_true',
                     help='the system RTTM may have two speakers at once (overlap-aware output)')
     ap.add_argument('--json', action='store_true', help='print one JSON object instead of the table')
+    ap.add_argument('--jer', action='store_true',
+                    help='also the Jaccard error rate (no collar, overlaps scored, whatever the DER options)')
     return ap
 
 
@@ -485,17 +588,19 @@ def main(argv=None):
     from . import formats
     uem = formats.read_uem(args.uem) if args.uem else None
     per, tot = score_rttm(read_rttm_path(args.ref_rttm), read_rttm_path(args.sys_rttm), args.collar,
-                          args.ignore_overlaps, uem, overlapping=args.overlapping_system)
+                          args.ignore_overlaps, uem, overlapping=args.overlapping_system, jer=args.jer)
     if args.json:
         print(json.dumps(dict(collar=args.collar, ignore_overlaps=args.ignore_overlaps, files=per, overall=tot),
                          sort_keys=True))
         return 0
     w = max([len('OVERALL')] + [len(n) for n in per])
-    print(f'{"file":<{w}}  {"DER %":>7}  {"miss %":>7}  {"FA %":>7}  {"conf %":>7}  {"scored s":>10}')
+    jer_head = f'  {"JER %":>7}' if args.jer else ''
+    print(f'{"file":<{w}}  {"DER %":>7}  {"miss %":>7}  {"FA %":>7}  {"conf %":>7}  {"scored s":>10}{jer_head}')
     for n, r in list(per.items()) + [('OVERALL', tot)]:
         pct = [100.0 * r[k] / r['scored'] if r['scored'] else float('nan') for k in ('miss', 'fa', 'conf')]
         der = 100.0 * r['der'] if r['der'] is not None else float('nan')
-        print(f'{n:<{w}}  {der:7.2f}  {pct[0]:7.2f}  {pct[1]:7.2f}  {pct[2]:7.2f}  {r["scored"]:10.2f}')
+        jer_col = (f'  {100.0 * r["jer"] if r["jer"] is not None else float("nan"):7.2f}') if args.jer else ''
+        print(f'{n:<{w}}  {der:7.2f}  {pct[0]:7.2f}  {pct[1]:7.2f}  {pct[2]:7.2f}  {r["scored"]:10.2f}{jer_col}')
     return 0
 
 

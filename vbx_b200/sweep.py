@@ -16,6 +16,8 @@ under the three AMI protocols: summary.json then holds the DER per recording and
 With --overlap-rttm PATH (an overlapped-speech detector's RTTM) or --oracle-overlaps (the reference's own overlaps; needs
 --ref-rttm) every setting also writes OUT/<setting>/overlap/<recording>.rttm, the overlap-aware output (DESIGN.md section
 5.12); with a reference it is scored too, and summary.json gains der_overlap and ranking_overlap next to der and ranking.
+With --jer (needs --ref-rttm) the `full` launch also gives the Jaccard error rate (DESIGN.md section 5.13): summary.json
+gains jer per recording and setting and ranking_jer (with overlaps also jer_overlap and ranking_jer_overlap).
 """
 import argparse
 import itertools
@@ -109,7 +111,7 @@ def entry_bytes(T, n_states, R, device):
 
 def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
                 device=None, max_batch_bytes=None, output_2nd=False, ref_rttm=None, uem=None, overlaps=None,
-                oracle_overlaps=False):
+                oracle_overlaps=False, jer=False):
     """Every setting of `grid` (see grid_settings) for every recording, with the front end and AHC run once.
 
     recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
@@ -125,6 +127,8 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     the reference has two or more speakers instead (needs ref_rttm).  Either makes each recording's dict also hold
     rttm_overlap and overlap_seconds as diarize_batch(overlaps=) does and, with a reference, der_overlap = {protocol:
     score.result dict} of that output, scored in one more vbx_score_overlap launch per protocol.  Needs init='AHC+VB'.
+    jer: also the Jaccard error rate, from the `full` protocol's launch (no extra launch): items gain jer (and with
+    overlaps jer_overlap) = score.jer_finish dict.  Needs ref_rttm.
     Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags[, der][, rttm_overlap,
     overlap_seconds][, der_overlap])}}; each recording's dict is the one diarize_batch returns with that setting's
     scalars."""
@@ -141,6 +145,8 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     if oracle_overlaps and overlaps is not None:
         raise ValueError('give overlaps or oracle_overlaps, not both')
     with_overlap = oracle_overlaps or overlaps is not None
+    if jer and ref_rttm is None:
+        raise ValueError('jer scores against the reference: it needs ref_rttm')
     if with_overlap and init == 'AHC':
         raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
     if not torch.cuda.is_available():
@@ -214,10 +220,11 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
             scored.append(score.prepare_recording(n, turns[n], timeline, None if uem_map is None else uem_map[n],
                                                   overlap=o))
         keys = [(k, b) for k in range(len(settings)) for b in range(len(names))]
-        der = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0]) for k, b in keys], device=dev)))
+        jp = 'full' if jer else None
+        der = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0]) for k, b in keys], device=dev, jer=jp)))
         if with_overlap:
             der_ovl = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0], res[(k, b)][1]) for k, b in keys],
-                                                         device=dev)))
+                                                         device=dev, jer=jp)))
     out = {}
     for k, s in enumerate(settings):
         out[s] = {}
@@ -226,9 +233,13 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
             item = _result(n, recordings[n][1], l1, l2, it, output_2nd, ovl[b])
             item['flags'] = int(fl)
             if der is not None:
-                item['der'] = der[(k, b)]
+                item['der'] = {p: v for p, v in der[(k, b)].items() if p != 'jer'}
+                if jer:
+                    item['jer'] = der[(k, b)]['jer']
             if der_ovl is not None:
-                item['der_overlap'] = der_ovl[(k, b)]
+                item['der_overlap'] = {p: v for p, v in der_ovl[(k, b)].items() if p != 'jer'}
+                if jer:
+                    item['jer_overlap'] = der_ovl[(k, b)]['jer']
             out[s][n] = item
     return out
 
@@ -261,6 +272,14 @@ def summarize_der(out, key='der'):
     return tot, ranking
 
 
+def summarize_jer(out, key='jer'):
+    """sweep_batch(jer=True) output with `key` ('jer' or 'jer_overlap') -> ({setting name: score.overall_jer dict},
+    setting names by overall JER, stable in grid order, settings without a JER last)."""
+    from . import score
+    tot = {s.name: score.overall_jer([item[key] for item in per_rec.values()]) for s, per_rec in out.items()}
+    return tot, score.rank(tot, key='jer')
+
+
 def build_parser():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument('--init', default='AHC+VB', choices=['AHC', 'AHC+VB'])
@@ -286,6 +305,7 @@ def build_parser():
                     help='overlap regions (RTTM file or directory): also write and score overlap-aware output')
     ap.add_argument('--oracle-overlaps', action='store_true',
                     help="use the reference's overlaps (with --ref-rttm) as the overlap regions")
+    ap.add_argument('--jer', action='store_true', help='also score and rank by Jaccard error rate (with --ref-rttm)')
     return ap
 
 
@@ -305,7 +325,8 @@ def main(argv=None):
     grid = dict(Fa=args.Fa, Fb=args.Fb, loopP=args.loopP, threshold=args.threshold, smoothing=args.init_smoothing)
     out = sweep_batch(recs, transform, plda, grid, lda_dim=args.lda_dim, max_iters=args.max_iters, epsilon=args.epsilon,
                       init=args.init, chain=args.chain, device=args.device, max_batch_bytes=args.max_batch_bytes,
-                      ref_rttm=args.ref_rttm, uem=args.uem, overlaps=overlaps, oracle_overlaps=args.oracle_overlaps)
+                      ref_rttm=args.ref_rttm, uem=args.uem, overlaps=overlaps, oracle_overlaps=args.oracle_overlaps,
+                      jer=args.jer)
     summary = {}
     for s, per_rec in out.items():
         d = os.path.join(args.out_dir, s.name)
@@ -316,7 +337,7 @@ def main(argv=None):
                 fp.write(''.join(line + os.linesep for line in item['rttm']))
             summary[s.name]['recordings'][name] = dict(speakers=item['n_speakers'], iterations=item['iterations'],
                                                        flags=item['flags'])
-            for key in ('der', 'der_overlap', 'overlap_seconds'):
+            for key in ('der', 'der_overlap', 'overlap_seconds', 'jer', 'jer_overlap'):
                 if key in item:
                     summary[s.name]['recordings'][name][key] = item[key]
             if 'rttm_overlap' in item:
@@ -331,6 +352,11 @@ def main(argv=None):
             tot, summary['ranking_overlap'] = summarize_der(out, 'der_overlap')
             for name, d in tot.items():
                 summary[name]['der_overlap'] = d
+        if args.jer:
+            for key in ('jer', 'jer_overlap') if overlaps is not None or args.oracle_overlaps else ('jer',):
+                tot, summary['ranking_' + key] = summarize_jer(out, key)
+                for name, d in tot.items():
+                    summary[name][key] = d
     with open(os.path.join(args.out_dir, 'summary.json'), 'w') as fp:
         json.dump(summary, fp, indent=1, sort_keys=True)
     return 0
