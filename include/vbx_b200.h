@@ -167,6 +167,16 @@ int vbx_ahc(vbx_handle_t h, const void *x, int32_t x_is_f64, int32_t dim, void *
 int vbx_hard_labels(vbx_handle_t h, const float *gamma, const int32_t *n_states, int32_t *first_out,
                     int32_t *second_out, void *stream);
 
+/* Output step under an upper bound on the speaker count (DESIGN.md section 5.14).  mass_out [n_rec,S] float64 is written
+ * with N_s = sum_t gamma[t,s] of every live state (0 for the padded columns; a recording without frames has a row of
+ * zeros), summed in an order that depends on the recording's length only.  Of recording b the keep[b] live states of
+ * largest mass survive (ties: the lower index); first_out / second_out are vbx_hard_labels' outputs over the surviving
+ * states only (second_out may be NULL; -1 when one state survives).  keep >= n_states gives vbx_hard_labels' labels.
+ * keep [n_rec] int32; every keep[b] must be >= 1 (VBX_ERR_ARG otherwise: the call reads keep back, so it waits for
+ * `stream`).  All other arguments as vbx_hard_labels; all device pointers. */
+int vbx_hard_labels_keep(vbx_handle_t h, const float *gamma, const int32_t *n_states, const int32_t *keep,
+                         int32_t *first_out, int32_t *second_out, double *mass_out, void *stream);
+
 /* Float64 evaluation of the same EM loop ("exact" mode for the one-recording-per-call use of VBx/vbhmm.py:154-158,
  * where the reference stops on an ELBO improvement < 1e-6, VBx/vbhmm.py:157 -- below float32 resolution).
  * All arrays float64: fea [N,R] (the reference's X, VBx/VBx.py:30), Phi [R], gamma_io [N,S], pi_io [n_rec,S],

@@ -1,7 +1,7 @@
 """Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection at
 D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
-6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels, the dense forward_backward(), the ELBO trace
-and DER / JER scoring.
+6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels (also under a speaker-count bound),
+the dense forward_backward(), the ELBO trace and DER / JER scoring.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
 """
@@ -74,6 +74,16 @@ run([300, 45, 1, 129, 600], 16, 30, fb_split=1, eps=1e-5, per_rec=True, tag='per
 run([300, 45, 1, 129, 600], 16, 30, fb_split=2, eps=1e-5, per_rec=True, tag='per-recording fused')
 run([4100, 300, 5000, 64], 8, 30, fb_split=2, eps=1e-5, per_rec=True, tag='per-recording chunked scan')
 run([513, 512, 1, 2, 300], 128, 30, ns=[128, 100, 65, 3, 1], eps=1e-5, per_rec=True, tag='per-recording S=128')
+
+# labels under a speaker-count bound (vbx_hard_labels_keep) at S = 128: recordings without frames, keep = 1, keep >= n_states
+lens = [300, 0, 65, 1, 129, 0]
+nsk = np.array([128, 1, 100, 3, 65, 7], dtype=np.int32)
+kb = VbxBatch(lens, 128, nsk, device=dev, allocate=False)
+gk = torch.rand((kb.N, kb.S), device=dev) * (torch.arange(kb.S, device=dev)[None, :] < 65)
+fk, sk, mk = kb.hard_labels_keep(gk.contiguous(), [1, 1, 100, 5, 3, 1])
+torch.cuda.synchronize()
+kb.close()
+print('hard labels keep ok', int(fk.max()), float(mk.sum()))
 
 # wgmma projection at the smallest and largest D, one frame and one frame past a full wave of tiles
 sms = torch.cuda.get_device_properties(0).multi_processor_count

@@ -11,7 +11,7 @@ LIB_PATH = os.environ.get('VBX_B200_LIB', os.path.join(_HERE, 'libvbx_b200.so'))
 
 EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_create', 'vbx_destroy', 'vbx_last_error',
            'vbx_set_option', 'vbx_plan', 'vbx_bind_workspace', 'vbx_prepare_scale',
-           'vbx_prepare_project', 'vbx_prepare_xvectors', 'vbx_run', 'vbx_run_per_recording', 'vbx_hard_labels', 'vbx_ahc_workspace_bytes', 'vbx_ahc', 'vbx_launch_count', 'vbx_get_timings', 'vbx_f64_workspace_bytes',
+           'vbx_prepare_project', 'vbx_prepare_xvectors', 'vbx_run', 'vbx_run_per_recording', 'vbx_hard_labels', 'vbx_hard_labels_keep', 'vbx_ahc_workspace_bytes', 'vbx_ahc', 'vbx_launch_count', 'vbx_get_timings', 'vbx_f64_workspace_bytes',
            'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace', 'vbx_get_gsum',
            'vbx_score', 'vbx_score_overlap', 'vbx_score_jer']
 
@@ -67,6 +67,8 @@ def load():
     lib.vbx_ahc.argtypes = [vp, vp, i32, i32, vp, ctypes.c_size_t, vp, vp, vp]
     lib.vbx_hard_labels.restype = ctypes.c_int
     lib.vbx_hard_labels.argtypes = [vp, vp, vp, vp, vp, vp]
+    lib.vbx_hard_labels_keep.restype = ctypes.c_int
+    lib.vbx_hard_labels_keep.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     lib.vbx_prepare_xvectors.restype = ctypes.c_int
     lib.vbx_prepare_xvectors.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.vbx_run.restype = ctypes.c_int

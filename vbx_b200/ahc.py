@@ -98,3 +98,25 @@ def cut(Zs, th, lengths, threshold):
             # what the reference's fcluster call does with a NaN cut
             labels.append(flat_clusters(Zs[b], -(th[b] + threshold)).astype(np.int64) - 1)
     return labels
+
+
+def cut_count(Zs, lengths, counts):
+    """scipy's fcluster(Z, k, criterion='maxclust') for every recording, k = counts[b]: the 0-based flat clusters of
+    linkage Zs[b] cut at the lowest merge height that leaves at most k clusters, numbered like flat_clusters.  Merges at
+    a tied height all happen together, so ties can leave fewer than k clusters, exactly as in scipy; k >= T leaves every
+    x-vector on its own.  A linkage with non-finite heights leaves every x-vector on its own, as cut() does."""
+    labels = []
+    for b, T in enumerate(lengths):
+        T, k = int(T), int(counts[b])
+        if k < 1:
+            raise ValueError(f'cluster count must be >= 1, got {k}')
+        Z = np.asarray(Zs[b], dtype=np.float64)
+        if T <= 1:
+            labels.append(np.zeros(T, dtype=np.int64))
+        elif k >= T or not np.isfinite(Z).all():
+            labels.append(np.arange(T, dtype=np.int64))      # scipy numbers singletons in x-vector order
+        else:
+            # the clusters left at height t are T minus the merges whose subtree height is <= t
+            height = np.sort(np.maximum.accumulate(Z[:, 2]))
+            labels.append(flat_clusters(Z, height[T - k - 1]).astype(np.int64) - 1)
+    return labels

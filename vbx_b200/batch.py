@@ -156,6 +156,27 @@ class VbxBatch:
         self._check(self.lib.vbx_hard_labels(self._h, _ptr(gamma), _ptr(self.n_states), _ptr(first), _ptr(sec), self._stream()))
         return (first, sec) if second else first
 
+    def hard_labels_keep(self, gamma, keep):
+        """Labels under an upper bound on the speaker count (vbx_hard_labels_keep, DESIGN.md section 5.14): of recording b
+        only the keep[b] live states of largest posterior mass compete.  keep: ints [B] (host sequence or int32 CUDA
+        tensor), each >= 1; keep >= n_states gives hard_labels(second=True).  Returns (first, second) int32 [N] (second
+        -1 where one state is kept) and the masses N_s, float64 [B, S]."""
+        self._f32(gamma, (self.N, self.S), 'gamma', need_workspace=False)
+        if isinstance(keep, torch.Tensor):
+            if not (keep.is_cuda and keep.dtype == torch.int32 and tuple(keep.shape) == (self.B,)):
+                raise ValueError(f'keep: expected an int32 CUDA tensor of shape ({self.B},)')
+            keep = keep.contiguous()
+        else:
+            keep = torch.from_numpy(np.asarray(keep, dtype=np.int32).reshape(-1)).to(self.device)
+            if tuple(keep.shape) != (self.B,):
+                raise ValueError(f'keep: expected {self.B} counts, got {tuple(keep.shape)}')
+        first = torch.empty(self.N, dtype=torch.int32, device=self.device)
+        sec = torch.empty(self.N, dtype=torch.int32, device=self.device)
+        mass = torch.empty((self.B, self.S), dtype=torch.float64, device=self.device)
+        self._check(self.lib.vbx_hard_labels_keep(self._h, _ptr(gamma), _ptr(self.n_states), _ptr(keep), _ptr(first),
+                                                  _ptr(sec), _ptr(mass), self._stream()))
+        return first, sec, mass
+
     @property
     def launches(self):
         return int(self.lib.vbx_launch_count(self._h))

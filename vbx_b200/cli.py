@@ -11,12 +11,47 @@ fastcluster needed) and writes one RTTM per recording, formatted as VBx/vbhmm.py
 With --overlap-rttm PATH (an overlapped-speech detector's RTTM file or directory; speakers ignored) each written RTTM is
 overlap-aware (DESIGN.md section 5.12): the usual lines, plus each x-vector's second most likely speaker inside the
 overlap regions.  A recording the file lacks has no overlap regions.
+
+With --num-speakers K, or --min-speakers / --max-speakers, every recording's speaker count is held to K or to the bounds
+(DESIGN.md section 5.14).  Each takes an integer for the whole archive or a file of 'recording count' lines.
 """
 import argparse
 import os
 import sys
 
 import numpy as np
+
+
+def speaker_count_arg(text, allow_oracle=False):
+    """A speaker-count option: an integer for every recording, or the path of a two-column 'recording count' file
+    (formats.read_speaker_counts) -> int or {recording: int}; with allow_oracle also the word 'oracle'."""
+    from . import formats
+    text = str(text)
+    if allow_oracle and text == 'oracle':
+        return text
+    try:
+        return int(text)
+    except ValueError:
+        pass
+    if not os.path.isfile(text):
+        raise argparse.ArgumentTypeError(f'expected an integer{", oracle" if allow_oracle else ""} or a count file, '
+                                         f'got {text!r}')
+    try:
+        return formats.read_speaker_counts(text)
+    except ValueError as e:
+        raise argparse.ArgumentTypeError(str(e))
+
+
+def add_count_options(ap, allow_oracle=False):
+    """--num-speakers / --min-speakers / --max-speakers (speaker_count_arg)."""
+    what = 'an integer, oracle (with --ref-rttm) or a "recording count" file' if allow_oracle else \
+        'an integer or a "recording count" file'
+    ap.add_argument('--num-speakers', default=None, type=lambda t: speaker_count_arg(t, allow_oracle),
+                    help=f'known number of speakers: {what}')
+    ap.add_argument('--min-speakers', default=None, type=speaker_count_arg, help='lower bound on the speaker count: '
+                    'an integer or a "recording count" file')
+    ap.add_argument('--max-speakers', default=None, type=speaker_count_arg, help='upper bound on the speaker count: '
+                    'an integer or a "recording count" file')
 
 
 def build_parser():
@@ -42,6 +77,7 @@ def build_parser():
     ap.add_argument('--device', default=None, help='CUDA device, e.g. cuda:0 (default: the current device)')
     ap.add_argument('--overlap-rttm', default=None,
                     help='overlap regions (RTTM file or directory): also write the second speaker inside them')
+    add_count_options(ap)
     return ap
 
 
@@ -63,7 +99,8 @@ def main(argv=None):
         recs[name] = (x, times)
     out = diarize_batch(recs, (mean1, mean2, lda), plda, Fa=args.Fa, Fb=args.Fb, loopP=args.loopP, lda_dim=args.lda_dim,
                         threshold=args.threshold, smoothing=args.init_smoothing, init=args.init, chain=args.chain,
-                        device=args.device, output_2nd=args.output_2nd, overlaps=overlaps)
+                        device=args.device, output_2nd=args.output_2nd, overlaps=overlaps,
+                        num_speakers=args.num_speakers, min_speakers=args.min_speakers, max_speakers=args.max_speakers)
     os.makedirs(args.out_rttm_dir, exist_ok=True)                           # VBx/vbhmm.py:170
     for name, item in out.items():
         with open(os.path.join(args.out_rttm_dir, f'{name}.rttm'), 'w') as fp:

@@ -787,6 +787,25 @@ int vbx_hard_labels(vbx_handle_t h, const float *gamma, const int32_t *n_states,
     return counted(h, vbx::launch_hard_labels(h->plan, gamma, n_states, first_out, second_out, (cudaStream_t)stream), "hard_labels");
 }
 
+int vbx_hard_labels_keep(vbx_handle_t h, const float *gamma, const int32_t *n_states, const int32_t *keep,
+                         int32_t *first_out, int32_t *second_out, double *mass_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    if (!h->planned || h->f64_only) return fail(h, VBX_ERR_STATE, "vbx_hard_labels_keep: call vbx_plan first");
+    if (h->plan.n_rec == 0) return VBX_OK;
+    if (!keep || !mass_out || (h->plan.n_frames && (!gamma || !first_out)))
+        return fail(h, VBX_ERR_ARG, "vbx_hard_labels_keep: null pointer");
+    DeviceGuard guard(h->device);
+    // keep lives on the device: read it back once to refuse counts below 1 (the labels leave the device next anyway)
+    std::vector<int32_t> kh(h->plan.n_rec);
+    cudaError_t e = cudaMemcpyAsync(kh.data(), keep, kh.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
+    if (e != cudaSuccess) return cuda_fail(h, e, "vbx_hard_labels_keep: reading keep");
+    for (int b = 0; b < h->plan.n_rec; ++b)
+        if (kh[b] < 1) return fail(h, VBX_ERR_ARG, "vbx_hard_labels_keep: keep[" + std::to_string(b) + "] < 1");
+    return counted(h, vbx::launch_hard_labels_keep(h->plan, gamma, n_states, keep, first_out, second_out, mass_out,
+                                                   (cudaStream_t)stream), "hard_labels_keep");
+}
+
 int vbx_ahc_workspace_bytes(vbx_handle_t h, size_t *bytes_out) {
     if (!h || !bytes_out) return VBX_ERR_ARG;
     if (!h->planned || h->f64_only) return fail(h, VBX_ERR_STATE, "vbx_ahc_workspace_bytes: call vbx_plan first");

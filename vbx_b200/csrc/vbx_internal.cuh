@@ -226,6 +226,9 @@ int launch_run_f64(const Plan &pl, void *workspace, const double *fea, const dou
                    cudaStream_t st);
 int launch_hard_labels(const Plan &pl, const float *gamma, const int32_t *n_states, int32_t *first, int32_t *second,
                        cudaStream_t st);
+// labels over the keep[b] states of largest posterior mass (vbx_count.cu)
+int launch_hard_labels_keep(const Plan &pl, const float *gamma, const int32_t *n_states, const int32_t *keep,
+                            int32_t *first, int32_t *second, double *mass, cudaStream_t st);
 // reference-module forward_backward() for a general transition matrix (vbx_fb_dense.cu)
 int launch_fb_dense(const double *lls, const double *tr, const double *ip, int T, int S, double *post, double *tll,
                     double *lfw, double *lbw, cudaStream_t st);

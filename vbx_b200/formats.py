@@ -217,3 +217,20 @@ def read_uem(path):
                 raise ValueError(f'{path}:{n}: expected "file channel onset offset", got {line.strip()!r}')
             out.setdefault(p[0], []).append((float(p[2]), float(p[3])))
     return out
+
+
+def read_speaker_counts(path):
+    """Two-column 'recording count' file -> {recording: int}.  Blank lines and lines starting with '#' are skipped."""
+    out = {}
+    with open(path) as f:
+        for n, line in enumerate(f, 1):
+            p = line.split()
+            if not p or p[0].startswith('#'):
+                continue
+            if len(p) != 2:
+                raise ValueError(f'{path}:{n}: expected "recording count", got {line.strip()!r}')
+            try:
+                out[p[0]] = int(p[1])
+            except ValueError:
+                raise ValueError(f'{path}:{n}: the count {p[1]!r} is not an integer')
+    return out

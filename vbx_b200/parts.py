@@ -171,6 +171,10 @@ class PartitionedBatch:
         self.whole.n_states = self._n_states
         return self.whole.hard_labels(gamma, second=second)
 
+    def hard_labels_keep(self, gamma, keep):
+        self.whole.n_states = self._n_states
+        return self.whole.hard_labels_keep(gamma, keep)
+
     # ---- multi-GPU: the batch-wide ELBO trace and its collective live in the whole-batch handle ----
     def attach_comm(self, group=None):
         return self.whole.attach_comm(group)

@@ -158,12 +158,26 @@ def diarize_recording(x_raw, seg_times, ahc_labels, transform, plda, Fa, Fb, loo
     return rttm_lines(recording, s, e, l), labels, g[:, :S]
 
 
-def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, **run_kw):
+def keep_labels(gamma, keep):
+    """The labels of rule 2 of the speaker-count bound (DESIGN.md section 5.14) with torch ops, for the float64 tier:
+    gamma [T,S] of one recording; the `keep` states of largest mass sum_t gamma[t,s] survive (ties: the lower index) and
+    every frame takes its best and second best surviving state (ties: the lower index; second -1 when one survives), as
+    vbx_hard_labels_keep does on the float32 tier.  Returns (first, second) int64 [T]."""
+    S = int(gamma.shape[1])
+    order = torch.argsort(gamma.sum(0, dtype=torch.float64), descending=True, stable=True)
+    kept = torch.sort(order[:min(int(keep), S)]).values
+    f, s = hard_labels(gamma[:, kept], second=True) if len(kept) > 1 else (hard_labels(gamma[:, kept]), None)
+    return kept[f], (kept[s] if s is not None else torch.full_like(f, -1))
+
+
+def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None, **run_kw):
     """The VB-HMM step (VBx/vbhmm.py:150-162) for the recordings of one state tier, packed: fea [N,R] float32, labels [N]
     AHC labels (device).  f64: the float64 kernels (vbx_run_f64, any state count), else one float32 batch padded to the
     tier, planned by `make` (default VbxBatch).  smoothing: a number or one per recording; run_kw go to run() (Fa, Fb,
     loopProb may be per-recording tensors there).  Returns [(labels, second-best labels or None, iterations, flags)] per
-    recording."""
+    recording.  hi: None, or an upper bound on the speaker count per recording: a recording whose labels hold more
+    speakers takes rule 2 of DESIGN.md section 5.14 (the hi states of largest mass, one vbx_hard_labels_keep launch for
+    the tier), and each tuple gains the unconstrained speaker count and 'vb' or 'mass'."""
     from .batch import VbxBatch, run_f64
     offs = np.concatenate([[0], np.cumsum(lens)])
     dt = torch.float64 if f64 else torch.float32
@@ -186,9 +200,25 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, **run_k
     first, second = first.cpu().numpy().astype(np.int64), second.cpu().numpy().astype(np.int64)
     iters = res['n_iters'].cpu().numpy().tolist()
     flags = res['flags'].cpu().numpy().tolist()
+    out = [(first[offs[b]:offs[b + 1]], second[offs[b]:offs[b + 1]] if ns[b] > 1 else None, int(iters[b]), int(flags[b]))
+           for b in range(len(lens))]
+    if hi is not None:
+        k1 = [len(np.unique(o[0])) for o in out]
+        over = [b for b in range(len(lens)) if k1[b] > hi[b]]
+        if over and f64:
+            for b in over:
+                f, s = keep_labels(g[offs[b]:offs[b + 1], :ns[b]], hi[b])
+                out[b] = (f.cpu().numpy().astype(np.int64), s.cpu().numpy().astype(np.int64) if hi[b] > 1 else None) + out[b][2:]
+        elif over:
+            keep = np.maximum(np.asarray(ns, dtype=np.int64), 1)
+            keep[over] = np.asarray(hi, dtype=np.int64)[over]
+            f, s, _ = vb.hard_labels_keep(g, keep.astype(np.int32))
+            f, s = f.cpu().numpy().astype(np.int64), s.cpu().numpy().astype(np.int64)
+            for b in over:
+                out[b] = (f[offs[b]:offs[b + 1]], s[offs[b]:offs[b + 1]] if hi[b] > 1 else None) + out[b][2:]
+        out = [o + (k1[b], 'mass' if k1[b] > hi[b] else 'vb') for b, o in enumerate(out)]
     vb.close()
-    return [(first[offs[b]:offs[b + 1]], second[offs[b]:offs[b + 1]] if ns[b] > 1 else None, int(iters[b]), int(flags[b]))
-            for b in range(len(lens))]
+    return out
 
 
 def _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold):
@@ -227,8 +257,86 @@ def _pad_features(fea, Phi):
     return fea, Phi
 
 
+def count_bounds(names, num_speakers=None, min_speakers=None, max_speakers=None):
+    """The speaker-count constraint of every recording (DESIGN.md section 5.14), checked: None when none of the three is
+    given, else (lo, hi) int64 arrays over `names`, hi = UNBOUNDED where there is no upper bound.  Each argument is an
+    int for the whole archive or a {recording: int} dict holding every recording of `names`.  num_speakers = K means
+    lo = hi = K; a missing bound is 1 or unbounded.  ValueError: num_speakers with a bound, a value below 1, lo > hi, a
+    recording a dict lacks."""
+    if num_speakers is None and min_speakers is None and max_speakers is None:
+        return None
+    if num_speakers is not None and (min_speakers is not None or max_speakers is not None):
+        raise ValueError('give num_speakers or min_speakers / max_speakers, not both')
+
+    def per_rec(v, what, default):
+        if v is None:
+            return np.full(len(names), default, dtype=np.int64)
+        if isinstance(v, dict):
+            missing = [n for n in names if n not in v]
+            if missing:
+                raise ValueError(f'{what}: no count for recordings {missing}')
+            vals = [v[n] for n in names]
+        else:
+            vals = [v] * len(names)
+        out = []
+        for n, x in zip(names, vals):
+            if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, np.integer)):
+                raise ValueError(f'{what}: expected an integer for recording {n!r}, got {x!r}')
+            if x < 1:
+                raise ValueError(f'{what} must be >= 1, got {int(x)} for recording {n!r}')
+            out.append(int(x))
+        return np.array(out, dtype=np.int64)
+
+    if num_speakers is not None:
+        lo = per_rec(num_speakers, 'num_speakers', 1)
+        return lo, lo.copy()
+    lo = per_rec(min_speakers, 'min_speakers', 1)
+    hi = per_rec(max_speakers, 'max_speakers', UNBOUNDED)
+    bad = [n for n, a, z in zip(names, lo, hi) if a > z]
+    if bad:
+        raise ValueError(f'min_speakers > max_speakers for recordings {bad}')
+    return lo, hi
+
+
+UNBOUNDED = np.iinfo(np.int32).max     # hi of a recording without an upper bound on its speaker count
+
+
+def _count_ahc(Zs, lens, labels, bounds):
+    """Rule 4 of DESIGN.md section 5.14 (init='AHC'): the threshold cut's labels where their count lies in [lo, hi],
+    else the maxclust cut at hi (too many) or lo (too few).  Returns (labels, unconstrained counts, rules)."""
+    from . import ahc as _ahc
+    lo, hi = bounds
+    k1 = [len(np.unique(l)) for l in labels]
+    target = [hi[b] if k1[b] > hi[b] else lo[b] if k1[b] < lo[b] else 0 for b in range(len(lens))]
+    labels = list(labels)
+    rules = ['vb'] * len(lens)
+    for b in range(len(lens)):
+        if target[b]:
+            labels[b] = _ahc.cut_count([Zs[b]], [lens[b]], [target[b]])[0]
+            rules[b] = 'unmet' if lens[b] < lo[b] else 'ahc'
+    return labels, k1, rules
+
+
+def _recut_outcome(T, lo, mc_labels, rerun):
+    """Rule 3 of DESIGN.md section 5.14 for one recording: (labels, labels2nd, iterations, flags, rule) from the VB-HMM
+    re-run `rerun` (its _vb_tier tuple, None when the recording has fewer than lo x-vectors) started from the maxclust
+    labels mc_labels."""
+    if rerun is None:
+        return mc_labels, None, 0, 0, 'unmet'
+    if len(np.unique(rerun[0])) >= lo:
+        return tuple(rerun[:4]) + ('recut',)
+    return mc_labels, None, 0, 0, 'ahc'
+
+
+def _count_fields(item, k1, rule, lo, hi):
+    """The reporting fields of a constrained result (DESIGN.md section 5.14)."""
+    item.update(count_rule=rule, n_speakers_vb=int(k1), count=(int(lo), None if hi >= UNBOUNDED else int(hi)))
+    return item
+
+
 def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
-                  max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False, overlaps=None):
+                  max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False, overlaps=None,
+                  num_speakers=None, min_speakers=None, max_speakers=None):
     """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
     recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
     one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
@@ -243,11 +351,19 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     none): each item then also has rttm_overlap, the overlap-aware RTTM lines (overlap_segments: the second most likely
     speaker inside the overlap regions), and overlap_seconds, the length of the recording's overlap regions.  Needs
     init='AHC+VB' (AHC alone has no second labels).
-    Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds])}."""
+    num_speakers / min_speakers / max_speakers: a known or bounded speaker count, each an int for the whole archive or a
+    {name: int} dict (count_bounds).  The rules of DESIGN.md section 5.14 then apply: a recording whose output already
+    has a count inside the bounds keeps it ('vb'); too many speakers keep the hi states of largest posterior mass
+    ('mass'); too few re-run the VB-HMM from the AHC linkage cut at lo clusters ('recut', or the cut itself: 'ahc';
+    'unmet' when the recording has fewer than lo x-vectors).  Each item then also has count_rule, n_speakers_vb (the
+    unconstrained count) and count = (lo, hi or None).
+    Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds]
+    [, count_rule, n_speakers_vb, count])}."""
     if init not in ('AHC', 'AHC+VB'):
         raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
     if overlaps is not None and init == 'AHC':
         raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
+    bounds = count_bounds(list(recordings), num_speakers, min_speakers, max_speakers)
     if not torch.cuda.is_available():
         from ._lib import VbxError
         raise VbxError('diarize_batch(): no CUDA device - vbx_b200 has no CPU fallback')
@@ -256,12 +372,17 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
     if len(names) == 0:
         return {}
-    fea, Phi, ahc_labels, _, _ = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold)
+    fea, Phi, ahc_labels, _, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold)
     offs = np.concatenate([[0], np.cumsum(lens)])
     out = {}
     labels1 = [l.astype(np.int64) for l in ahc_labels]
     labels2 = [None] * len(names)
     iters = [0] * len(names)
+    k1 = rules = None
+    if bounds is not None and not init.endswith('VB'):
+        labels1, k1, rules = _count_ahc(Zs, lens, labels1, bounds)
+    elif bounds is not None:
+        k1, rules = [0] * len(names), [None] * len(names)
     if init.endswith('VB'):
         ns = np.array([int(l.max()) + 1 if len(l) else 1 for l in ahc_labels], dtype=np.int32)
         fea, Phi = _pad_features(fea, Phi)
@@ -278,16 +399,49 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
                 torch.from_numpy(np.concatenate([np.arange(offs[b], offs[b + 1]) for b in idx])).to(dev)
             pick = (lambda t: t) if rows is None else (lambda t: t.index_select(0, rows).contiguous())
             sub = _vb_tier(lens[idx], ns[idx], pick(fea), Phi, pick(lab_d), tier == 2, smoothing, dev,
+                           hi=None if bounds is None else bounds[1][idx],
                            Fa=Fa, Fb=Fb, loopProb=loopP, maxIters=max_iters, epsilon=epsilon)
             for j, b in enumerate(idx):
                 labels1[b], labels2[b], iters[b] = sub[j][:3]
+                if bounds is not None:
+                    k1[b], rules[b] = sub[j][4:6]
+        if bounds is not None:
+            _count_rerun(bounds, Zs, lens, offs, fea, Phi, dev, k1, rules, labels1, labels2, iters, smoothing,
+                         Fa=Fa, Fb=Fb, loopProb=loopP, maxIters=max_iters, epsilon=epsilon)
     for b, n in enumerate(names):
         ovl = None
         if overlaps is not None:
             from .score import overlap_ticks
             ovl = overlap_ticks(overlaps.get(n))
         out[n] = _result(n, recordings[n][1], labels1[b], labels2[b], iters[b], output_2nd, ovl)
+        if bounds is not None:
+            _count_fields(out[n], k1[b], rules[b], bounds[0][b], bounds[1][b])
     return out
+
+
+def _count_rerun(bounds, Zs, lens, offs, fea, Phi, dev, k1, rules, labels1, labels2, iters, smoothing, **run_kw):
+    """Rule 3 of DESIGN.md section 5.14 for diarize_batch: every recording with fewer than lo speakers re-runs the
+    VB-HMM from its linkage cut at lo clusters, all of them in one batch per state tier.  Updates the lists in place."""
+    from . import ahc as _ahc
+    lo = bounds[0]
+    low = [b for b in range(len(lens)) if k1[b] < lo[b]]
+    if not low:
+        return
+    mc = dict(zip(low, _ahc.cut_count([Zs[b] for b in low], lens[low], lo[low])))
+    runs = {}
+    met = [b for b in low if lens[b] >= lo[b]]
+    ns = {b: int(mc[b].max()) + 1 for b in met}
+    for tier, pred in enumerate((lambda n: n <= 64, lambda n: 64 < n <= MAX_STATES_F32, lambda n: n > MAX_STATES_F32)):
+        idx = [b for b in met if pred(ns[b])]
+        if not idx:
+            continue
+        rows = torch.from_numpy(np.concatenate([np.arange(offs[b], offs[b + 1]) for b in idx])).to(dev)
+        labs = torch.from_numpy(np.concatenate([mc[b] for b in idx])).to(dev)
+        sub = _vb_tier(lens[idx], np.array([ns[b] for b in idx], dtype=np.int32), fea.index_select(0, rows).contiguous(),
+                       Phi, labs, tier == 2, smoothing, dev, **run_kw)
+        runs.update(zip(idx, sub))
+    for b in low:
+        labels1[b], labels2[b], iters[b], _, rules[b] = _recut_outcome(lens[b], lo[b], mc[b], runs.get(b))
 
 
 def _result(name, seg_times, labels, labels2, iterations, output_2nd, overlap=None):

@@ -87,6 +87,26 @@ def reference_turns(rows):
     return out
 
 
+def reference_speaker_counts(turns, uem=None):
+    """The oracle speaker count of every recording: {recording: number of speakers of reference_turns() `turns` with
+    positive scored time}.  uem: None (all time is scored) or {recording: [(onset, offset)] seconds} (formats.read_uem),
+    which then holds every recording of `turns`; a speaker who talks only outside it does not count."""
+    out = {}
+    for rec, spk in turns.items():
+        if uem is None:
+            out[rec] = len(spk)        # reference_turns keeps speakers with at least one non-empty turn only
+            continue
+        u = to_ticks(np.asarray(uem[rec], dtype=np.float64).reshape(-1, 2))
+        ulo, uhi = merge_turns(u[:, 0], u[:, 1])
+        n = 0
+        for s, e in spk:
+            # time of the speaker's disjoint turns inside the disjoint scored intervals
+            inside = np.minimum(e[:, None], uhi[None, :]) - np.maximum(s[:, None], ulo[None, :])
+            n += bool((inside > 0).any())
+        out[rec] = n
+    return out
+
+
 def overlap_ticks(intervals):
     """Overlap regions [(onset, offset)] seconds (None = none) -> (lo, hi) int64 ticks, sorted and disjoint: the union
     of the intervals (merge_turns)."""

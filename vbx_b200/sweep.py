@@ -18,6 +18,10 @@ With --overlap-rttm PATH (an overlapped-speech detector's RTTM) or --oracle-over
 5.12); with a reference it is scored too, and summary.json gains der_overlap and ranking_overlap next to der and ranking.
 With --jer (needs --ref-rttm) the `full` launch also gives the Jaccard error rate (DESIGN.md section 5.13): summary.json
 gains jer per recording and setting and ranking_jer (with overlaps also jer_overlap and ranking_jer_overlap).
+With --num-speakers (an integer, a 'recording count' file, or oracle: the reference's speaker count, needs --ref-rttm) or
+--min-speakers / --max-speakers, every setting holds each recording to that speaker count (DESIGN.md section 5.14):
+summary.json gains count_rule and speakers_vb per recording and setting, and count_rules per setting (how many
+recordings took each rule).
 """
 import argparse
 import itertools
@@ -111,7 +115,7 @@ def entry_bytes(T, n_states, R, device):
 
 def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
                 device=None, max_batch_bytes=None, output_2nd=False, ref_rttm=None, uem=None, overlaps=None,
-                oracle_overlaps=False, jer=False):
+                oracle_overlaps=False, jer=False, num_speakers=None, min_speakers=None, max_speakers=None):
     """Every setting of `grid` (see grid_settings) for every recording, with the front end and AHC run once.
 
     recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
@@ -129,14 +133,20 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     score.result dict} of that output, scored in one more vbx_score_overlap launch per protocol.  Needs init='AHC+VB'.
     jer: also the Jaccard error rate, from the `full` protocol's launch (no extra launch): items gain jer (and with
     overlaps jer_overlap) = score.jer_finish dict.  Needs ref_rttm.
+    num_speakers / min_speakers / max_speakers: a known or bounded speaker count per recording, as for
+    pipeline.diarize_batch, the same for every setting; num_speakers='oracle' takes each recording's number of reference
+    speakers with scored time (needs ref_rttm; inside the UEM when one is given).  Every (recording, setting) entry then
+    follows the rules of DESIGN.md section 5.14 and its dict gains count_rule, n_speakers_vb and count.  The re-runs of
+    rule 3 of all settings are packed into batches per state tier like the first pass.
     Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags[, der][, rttm_overlap,
-    overlap_seconds][, der_overlap])}}; each recording's dict is the one diarize_batch returns with that setting's
-    scalars."""
+    overlap_seconds][, der_overlap][, count_rule, n_speakers_vb, count])}}; each recording's dict is the one
+    diarize_batch returns with that setting's scalars."""
     import torch
     from . import ahc as _ahc
     from ._lib import VbxError, padded_states
     from .parts import make_batch
-    from .pipeline import MAX_STATES_F32, _front_end, _pad_features, _result, _vb_tier
+    from .pipeline import (MAX_STATES_F32, _count_ahc, _count_fields, _front_end, _pad_features, _recut_outcome, _result,
+                           _vb_tier, count_bounds)
     settings = grid_settings(grid)
     if init not in ('AHC', 'AHC+VB'):
         raise ValueError('Wrong option for args.initialization.')
@@ -149,6 +159,14 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
         raise ValueError('jer scores against the reference: it needs ref_rttm')
     if with_overlap and init == 'AHC':
         raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
+    oracle_count = isinstance(num_speakers, str)
+    if oracle_count and num_speakers != 'oracle':
+        raise ValueError(f"num_speakers: expected an int, a dict or 'oracle', got {num_speakers!r}")
+    if oracle_count and ref_rttm is None:
+        raise ValueError("num_speakers='oracle' counts the reference's speakers: it needs ref_rttm")
+    if oracle_count and (min_speakers is not None or max_speakers is not None):
+        raise ValueError('give num_speakers or min_speakers / max_speakers, not both')
+    bounds = None if oracle_count else count_bounds(list(recordings), num_speakers, min_speakers, max_speakers)
     if not torch.cuda.is_available():
         raise VbxError('sweep_batch(): no CUDA device - vbx_b200 has no CPU fallback')
     dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
@@ -156,6 +174,13 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     if uem is not None and ref_rttm is None:
         raise ValueError('uem restricts the scored time: it needs ref_rttm')
     ref = _load_reference(names, ref_rttm, uem) if ref_rttm is not None else None
+    if oracle_count:
+        from .score import reference_speaker_counts
+        num_speakers = reference_speaker_counts({n: ref[0][n] for n in names}, ref[1])
+        empty = [n for n in names if num_speakers[n] < 1]
+        if empty:
+            raise ValueError(f'recordings without scored reference speech have no oracle speaker count: {empty}')
+        bounds = count_bounds(names, num_speakers, min_speakers, max_speakers)
     if not names:
         return {s: {} for s in settings}
     lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
@@ -169,43 +194,78 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     # per (setting, recording): labels, labels2nd, iterations, flags
     res = {(k, b): (ahc_labels[s.threshold][b].astype(np.int64), None, 0, 0)
            for k, s in enumerate(settings) for b in range(len(names))}
+    counted = {}           # with a speaker-count constraint, per (setting, recording): unconstrained count, rule
+    if bounds is not None and not init.endswith('VB'):
+        for k, s in enumerate(settings):
+            labels, k1, rules = _count_ahc(Zs, lens, [res[(k, b)][0] for b in range(len(names))], bounds)
+            for b in range(len(names)):
+                res[(k, b)] = (labels[b], None, 0, 0)
+                counted[(k, b)] = (k1[b], rules[b])
     if init.endswith('VB'):
         if max_batch_bytes is None:
             max_batch_bytes = int(torch.cuda.mem_get_info(dev)[0] * BUDGET_FRACTION)
         entries = [(k, b) for k in range(len(settings)) for b in range(len(names))]
         ns = {(k, b): max(int(ahc_labels[settings[k].threshold][b].max()) + 1, 1) if lens[b] else 1 for k, b in entries}
-        tiers = ([e for e in entries if ns[e] <= 64], [e for e in entries if 64 < ns[e] <= MAX_STATES_F32],
-                 [e for e in entries if ns[e] > MAX_STATES_F32])
         size_cache = {}
 
-        def run(group, f64, **hyper):
+        def run(group, f64, ns, labels_of, hi, out, **hyper):
             rows = torch.from_numpy(np.concatenate([np.arange(offs[b], offs[b + 1]) for _, b in group])).to(dev)
-            labs = torch.cat([lab_d[settings[k].threshold][offs[b]:offs[b + 1]] for k, b in group])
+            labs = torch.cat([labels_of(e) for e in group])
             sub = _vb_tier(lens[[b for _, b in group]], np.array([ns[e] for e in group], dtype=np.int32),
                            fea.index_select(0, rows).contiguous(), Phi, labs, f64,
                            [settings[k].smoothing for k, _ in group], dev, make=make_batch,
+                           hi=None if hi is None else hi[[b for _, b in group]],
                            maxIters=max_iters, epsilon=epsilon, **hyper)
             for e, r in zip(group, sub):
-                res[e] = r
+                out[e] = r
 
-        for tier, group_all in enumerate(tiers[:2]):
-            if not group_all:
-                continue
-            sizes = []
-            for k, b in group_all:
-                key = (int(lens[b]), padded_states(ns[(k, b)]))      # the size depends on T and the padded S only
-                if key not in size_cache:
-                    size_cache[key] = entry_bytes(key[0], key[1], R, dev)
-                sizes.append(size_cache[key])
-            for idx in pack(sizes, max_batch_bytes):
-                group = [group_all[i] for i in idx]
-                hp = [torch.tensor([getattr(settings[k], a) for k, _ in group], dtype=torch.float64, device=dev)
-                      for a in ('Fa', 'Fb', 'loopP')]
-                run(group, False, Fa=hp[0], Fb=hp[1], loopProb=hp[2])
-        for k, s in enumerate(settings):           # no per-recording float64 path: one run per setting
-            group = [e for e in tiers[2] if e[0] == k]
-            if group:
-                run(group, True, Fa=s.Fa, Fb=s.Fb, loopProb=s.loopP)
+        def run_tiers(entries, ns, labels_of, hi, out):
+            """The entries as diarize_batch's state tiers: float32 batches packed to max_batch_bytes with per-entry
+            Fa / Fb / loopP, the float64 tier one run per setting."""
+            tiers = ([e for e in entries if ns[e] <= 64], [e for e in entries if 64 < ns[e] <= MAX_STATES_F32],
+                     [e for e in entries if ns[e] > MAX_STATES_F32])
+            for tier, group_all in enumerate(tiers[:2]):
+                if not group_all:
+                    continue
+                sizes = []
+                for k, b in group_all:
+                    key = (int(lens[b]), padded_states(ns[(k, b)]))      # the size depends on T and the padded S only
+                    if key not in size_cache:
+                        size_cache[key] = entry_bytes(key[0], key[1], R, dev)
+                    sizes.append(size_cache[key])
+                for idx in pack(sizes, max_batch_bytes):
+                    group = [group_all[i] for i in idx]
+                    hp = [torch.tensor([getattr(settings[k], a) for k, _ in group], dtype=torch.float64, device=dev)
+                          for a in ('Fa', 'Fb', 'loopP')]
+                    run(group, False, ns, labels_of, hi, out, Fa=hp[0], Fb=hp[1], loopProb=hp[2])
+            for k, s in enumerate(settings):           # no per-recording float64 path: one run per setting
+                group = [e for e in tiers[2] if e[0] == k]
+                if group:
+                    run(group, True, ns, labels_of, hi, out, Fa=s.Fa, Fb=s.Fb, loopProb=s.loopP)
+
+        first = {}
+        run_tiers(entries, ns, lambda e: lab_d[settings[e[0]].threshold][offs[e[1]]:offs[e[1] + 1]],
+                  None if bounds is None else bounds[1], first)
+        for e, r in first.items():
+            res[e] = r[:4]
+            if bounds is not None:
+                counted[e] = r[4:6]
+        if bounds is not None:
+            # rule 3: entries with too few speakers re-run from the linkage cut at lo clusters, which does not depend on
+            # the setting; every setting's re-runs share the batches of their tier
+            lo = bounds[0]
+            low = [e for e in entries if counted[e][0] < lo[e[1]]]
+            recs = sorted(set(b for _, b in low))
+            mc = dict(zip(recs, _ahc.cut_count([Zs[b] for b in recs], lens[recs], lo[recs])))
+            met = [e for e in low if lens[e[1]] >= lo[e[1]]]
+            mc_d = {b: torch.from_numpy(mc[b]).to(dev) for b in set(b for _, b in met)}
+            again = {}
+            if met:
+                run_tiers(met, {e: int(mc[e[1]].max()) + 1 for e in met}, lambda e: mc_d[e[1]], None, again)
+            for e in low:
+                *r, rule = _recut_outcome(lens[e[1]], lo[e[1]], mc[e[1]], again.get(e))
+                res[e] = tuple(r)
+                counted[e] = (counted[e][0], rule)
     from . import score
     ovl = [None] * len(names)
     if with_overlap:
@@ -232,6 +292,8 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
             l1, l2, it, fl = res[(k, b)]
             item = _result(n, recordings[n][1], l1, l2, it, output_2nd, ovl[b])
             item['flags'] = int(fl)
+            if bounds is not None:
+                _count_fields(item, *counted[(k, b)], bounds[0][b], bounds[1][b])
             if der is not None:
                 item['der'] = {p: v for p, v in der[(k, b)].items() if p != 'jer'}
                 if jer:
@@ -306,6 +368,8 @@ def build_parser():
     ap.add_argument('--oracle-overlaps', action='store_true',
                     help="use the reference's overlaps (with --ref-rttm) as the overlap regions")
     ap.add_argument('--jer', action='store_true', help='also score and rank by Jaccard error rate (with --ref-rttm)')
+    from .cli import add_count_options
+    add_count_options(ap, allow_oracle=True)
     return ap
 
 
@@ -326,7 +390,8 @@ def main(argv=None):
     out = sweep_batch(recs, transform, plda, grid, lda_dim=args.lda_dim, max_iters=args.max_iters, epsilon=args.epsilon,
                       init=args.init, chain=args.chain, device=args.device, max_batch_bytes=args.max_batch_bytes,
                       ref_rttm=args.ref_rttm, uem=args.uem, overlaps=overlaps, oracle_overlaps=args.oracle_overlaps,
-                      jer=args.jer)
+                      jer=args.jer, num_speakers=args.num_speakers, min_speakers=args.min_speakers,
+                      max_speakers=args.max_speakers)
     summary = {}
     for s, per_rec in out.items():
         d = os.path.join(args.out_dir, s.name)
@@ -337,9 +402,13 @@ def main(argv=None):
                 fp.write(''.join(line + os.linesep for line in item['rttm']))
             summary[s.name]['recordings'][name] = dict(speakers=item['n_speakers'], iterations=item['iterations'],
                                                        flags=item['flags'])
-            for key in ('der', 'der_overlap', 'overlap_seconds', 'jer', 'jer_overlap'):
+            for key in ('der', 'der_overlap', 'overlap_seconds', 'jer', 'jer_overlap', 'count_rule'):
                 if key in item:
                     summary[s.name]['recordings'][name][key] = item[key]
+            if 'count_rule' in item:
+                summary[s.name]['recordings'][name]['speakers_vb'] = item['n_speakers_vb']
+                rules = summary[s.name].setdefault('count_rules', {})
+                rules[item['count_rule']] = rules.get(item['count_rule'], 0) + 1
             if 'rttm_overlap' in item:
                 os.makedirs(os.path.join(d, 'overlap'), exist_ok=True)
                 with open(os.path.join(d, 'overlap', f'{name}.rttm'), 'w') as fp:
