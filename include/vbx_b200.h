@@ -177,6 +177,30 @@ int vbx_hard_labels(vbx_handle_t h, const float *gamma, const int32_t *n_states,
 int vbx_hard_labels_keep(vbx_handle_t h, const float *gamma, const int32_t *n_states, const int32_t *keep,
                          int32_t *first_out, int32_t *second_out, double *mass_out, void *stream);
 
+/* Speaker linking across the recordings of an archive (DESIGN.md section 5.15); needs a handle, no plan.
+ * M speakers (a recording's VB-HMM labels, numbered across the archive); all arrays are DEVICE arrays:
+ *   fea [N,R] float32, Phi [R]   the features and between-speaker variances the VB-HMM ran with (R <= 128)
+ *   speaker [N] int32            the speaker of x-vector t in [0, M), or -1 (any value outside [0, M) counts as -1)
+ *   speaker_rec [M] int32        the recording of each speaker (speakers of one recording are never linked)
+ *   Fa, Fb (HOST)                the VB-HMM's scalars; c = Fa / Fb must be finite and >= 0
+ * Per speaker s, n_s = #{t : speaker[t] = s} and F_s = sum of those rows of fea, float64, summed in an order fixed by the
+ * positions of s's x-vectors relative to its first one.  Each speaker's CTA reads speaker[] over the whole span from its
+ * first to its last x-vector, so the statistics cost sum_s (span_s + n_s R) reads: about (K + R) N for speakers packed by
+ * recording with K speakers each, but up to M N when speakers spread across the whole array.  With L_s,r = 1 + c n_s Phi_r and b_s,r = c sqrt(Phi_r) F_s,r
+ *   LLR(s,u) = 1/2 sum_r [ (b_s,r + b_u,r)^2 / (L_s,r + L_u,r - 1) - b_s,r^2 / L_s,r - b_u,r^2 / L_u,r
+ *                          + log L_s,r + log L_u,r - log(L_s,r + L_u,r - 1) ]
+ * (0 when n_s or n_u is 0), and the distance of two speakers is -LLR; 1e30 between two speakers of one recording, 0 on
+ * the diagonal.  Z_out [M-1,4] (scipy layout) is the average linkage of those distances, computed by vbx_ahc's linkage
+ * kernel (ties: the lowest slot).  Optional outputs (NULL: not written): n_out [M], F_out [M,R], dist_out [M,M] float64.
+ * workspace: vbx_link_workspace_bytes(M) bytes (about 8 M^2 + 1.1 KB M), 256-byte aligned.  Stream ordered, no
+ * allocation, no host synchronisation.  M above VBX_LINK_MAX_SPEAKERS (the linkage kernel keeps 4 (M - 1) in int32)
+ * returns VBX_ERR_ARG. */
+#define VBX_LINK_MAX_SPEAKERS 536870912 /* 2^29 */
+int vbx_link_workspace_bytes(vbx_handle_t h, int64_t M, size_t *bytes_out);
+int vbx_link(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
+             int64_t M, const int32_t *speaker_rec, double Fa, double Fb, void *workspace, size_t workspace_bytes,
+             double *n_out, double *F_out, double *dist_out, double *Z_out, void *stream);
+
 /* Float64 evaluation of the same EM loop ("exact" mode for the one-recording-per-call use of VBx/vbhmm.py:154-158,
  * where the reference stops on an ELBO improvement < 1e-6, VBx/vbhmm.py:157 -- below float32 resolution).
  * All arrays float64: fea [N,R] (the reference's X, VBx/VBx.py:30), Phi [R], gamma_io [N,S], pi_io [n_rec,S],

@@ -1,7 +1,7 @@
 """Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection at
 D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
 6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels (also under a speaker-count bound),
-the dense forward_backward(), the ELBO trace and DER / JER scoring.
+the dense forward_backward(), the ELBO trace, DER / JER scoring and speaker linking across recordings.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
 """
@@ -84,6 +84,18 @@ fk, sk, mk = kb.hard_labels_keep(gk.contiguous(), [1, 1, 100, 5, 3, 1])
 torch.cuda.synchronize()
 kb.close()
 print('hard labels keep ok', int(fk.max()), float(mk.sum()))
+
+# speaker linking (vbx_link): recordings without x-vectors, a speaker with one x-vector, padded features, tile edges
+from vbx_b200 import link  # noqa: E402
+gl = np.random.default_rng(3)
+l_lens = [0, 40, 1, 300, 0, 77]
+l_labels = [gl.integers(0, k, n) for n, k in zip(l_lens, [1, 5, 1, 37, 1, 9])]
+l_fea = torch.randn((sum(l_lens), 16), device=dev)
+l_fea[:, 13:] = 0
+l_phi = torch.rand(16, device=dev) * (torch.arange(16, device=dev) < 13)
+l_out = link.link_speakers(l_fea, l_phi, np.concatenate([[0], np.cumsum(l_lens)]), l_labels, 0.3, 17.0, dev, dist=True)
+torch.cuda.synchronize()
+print('link ok', len(l_out[0].rec), float(l_out[3][:, 2].min()))
 
 # wgmma projection at the smallest and largest D, one frame and one frame past a full wave of tiles
 sms = torch.cuda.get_device_properties(0).multi_processor_count

@@ -14,6 +14,10 @@ overlap regions.  A recording the file lacks has no overlap regions.
 
 With --num-speakers K, or --min-speakers / --max-speakers, every recording's speaker count is held to K or to the bounds
 (DESIGN.md section 5.14).  Each takes an integer for the whole archive or a file of 'recording count' lines.
+
+With --link-threshold X the speakers of all recordings are linked across the archive (DESIGN.md section 5.15): every
+written RTTM (and with --output-2nd every second-label RTTM) names its speakers by archive-wide id, so the same speaker
+has the same name in every file.  Speakers are linked where their average same-speaker log-likelihood ratio is >= X.
 """
 import argparse
 import os
@@ -78,6 +82,9 @@ def build_parser():
     ap.add_argument('--overlap-rttm', default=None,
                     help='overlap regions (RTTM file or directory): also write the second speaker inside them')
     add_count_options(ap)
+    ap.add_argument('--link-threshold', default=None, type=float,
+                    help='link speakers across the recordings: one name per speaker in every file where their average '
+                         'same-speaker log-likelihood ratio is >= this')
     return ap
 
 
@@ -85,7 +92,7 @@ def main(argv=None):
     args = build_parser().parse_args(argv)
     assert 0 <= args.loopP <= 1, f'Expecting loopP between 0 and 1, got {args.loopP} instead.'     # VBx/vbhmm.py:103
     from . import formats
-    from .pipeline import diarize_batch
+    from .pipeline import diarize_batch, linked_lines
     from .score import read_overlaps
     overlaps = read_overlaps(args.overlap_rttm) if args.overlap_rttm is not None else None
     segs = formats.read_segments(args.segments_file)                        # VBx/vbhmm.py:105
@@ -100,16 +107,21 @@ def main(argv=None):
     out = diarize_batch(recs, (mean1, mean2, lda), plda, Fa=args.Fa, Fb=args.Fb, loopP=args.loopP, lda_dim=args.lda_dim,
                         threshold=args.threshold, smoothing=args.init_smoothing, init=args.init, chain=args.chain,
                         device=args.device, output_2nd=args.output_2nd, overlaps=overlaps,
-                        num_speakers=args.num_speakers, min_speakers=args.min_speakers, max_speakers=args.max_speakers)
+                        num_speakers=args.num_speakers, min_speakers=args.min_speakers, max_speakers=args.max_speakers,
+                        link_threshold=args.link_threshold)
+    linked = args.link_threshold is not None
     os.makedirs(args.out_rttm_dir, exist_ok=True)                           # VBx/vbhmm.py:170
     for name, item in out.items():
+        key = 'rttm_linked' if linked else 'rttm' if overlaps is None else 'rttm_overlap'
         with open(os.path.join(args.out_rttm_dir, f'{name}.rttm'), 'w') as fp:
-            fp.write(''.join(line + os.linesep for line in item['rttm' if overlaps is None else 'rttm_overlap']))
+            fp.write(''.join(line + os.linesep for line in item[key]))
         if item['rttm2nd'] is not None:
             d2 = f'{args.out_rttm_dir}2nd'
             os.makedirs(d2, exist_ok=True)
+            lines = item['rttm2nd'] if not linked else \
+                linked_lines(name, recs[name][1], item['labels2nd'], None, item['global_speakers'])
             with open(os.path.join(d2, f'{name}.rttm'), 'w') as fp:
-                fp.write(''.join(line + os.linesep for line in item['rttm2nd']))
+                fp.write(''.join(line + os.linesep for line in lines))
     return 0
 
 

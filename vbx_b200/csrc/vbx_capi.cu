@@ -832,6 +832,36 @@ int vbx_ahc(vbx_handle_t h, const void *x, int32_t x_is_f64, int32_t dim, void *
     return VBX_OK;
 }
 
+int vbx_link_workspace_bytes(vbx_handle_t h, int64_t M, size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    if (M < 0 || M > VBX_LINK_MAX_SPEAKERS)
+        return fail(h, VBX_ERR_ARG, "vbx_link_workspace_bytes: M must lie in [0, VBX_LINK_MAX_SPEAKERS]");
+    *bytes_out = vbx::link_workspace_bytes(M);
+    return VBX_OK;
+}
+
+int vbx_link(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
+             int64_t M, const int32_t *speaker_rec, double Fa, double Fb, void *workspace, size_t workspace_bytes,
+             double *n_out, double *F_out, double *dist_out, double *Z_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_link");
+    if (N < 0 || M < 0 || M > VBX_LINK_MAX_SPEAKERS)
+        return fail(h, VBX_ERR_ARG, "vbx_link: need N >= 0 and 0 <= M <= VBX_LINK_MAX_SPEAKERS");
+    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, "vbx_link: R must lie in [1, 128]");
+    const double c = Fa / Fb;
+    if (!(c >= 0.0) || c == INFINITY) return fail(h, VBX_ERR_ARG, "vbx_link: Fa / Fb must be finite and >= 0");
+    if (M == 0) return VBX_OK;
+    if (!Phi || !speaker_rec || !workspace || (N > 0 && (!fea || !speaker)) || (M >= 2 && !Z_out))
+        return fail(h, VBX_ERR_ARG, "vbx_link: null pointer");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VBX_ERR_ARG, "vbx_link: workspace must be 256-byte aligned");
+    if (workspace_bytes < vbx::link_workspace_bytes(M))
+        return fail(h, VBX_ERR_ARG, "vbx_link: workspace smaller than vbx_link_workspace_bytes()");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_link(fea, Phi, speaker, N, R, speaker_rec, M, c, workspace, n_out, F_out, dist_out,
+                                       Z_out, (cudaStream_t)stream), "link");
+}
+
 int vbx_f64_workspace_bytes(vbx_handle_t h, size_t *bytes_out) {
     if (!h || !bytes_out) return VBX_ERR_ARG;
     if (!h->planned) return fail(h, VBX_ERR_STATE, "vbx_f64_workspace_bytes: call vbx_plan first");

@@ -246,6 +246,15 @@ int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const
 size_t ahc_workspace_bytes(const int64_t *offsets_host, int n_rec, std::vector<int64_t> *d_off_host);
 int launch_ahc(const Plan &pl, const std::vector<int64_t> &d_off, const void *x, int x_is_f64, int dim, void *workspace,
                size_t workspace_bytes, double *Z_out, double *thr_out, cudaStream_t st, std::string *err);
+// ahc_linkage_kernel as one CTA over the recording described by the DEVICE arrays offsets [2] and d_off [1]; its region
+// of ws (linkage_workspace_bytes(T) bytes, the T x T distances first) is laid out as vbx_ahc's
+size_t linkage_workspace_bytes(int64_t T);
+void launch_linkage(const int64_t *offsets, const int64_t *d_off, void *ws, double *Z_out, cudaStream_t st);
+// speaker linking across recordings (vbx_link.cu)
+size_t link_workspace_bytes(int64_t M);
+int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
+                int64_t M, double c, void *workspace, double *n_out, double *F_out, double *dist_out, double *Z_out,
+                cudaStream_t st);
 // wgmma projection (vbx_project_tc.cu)
 size_t tc_scratch_floats();
 int launch_project_wgmma(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,

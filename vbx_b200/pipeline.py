@@ -336,7 +336,7 @@ def _count_fields(item, k1, rule, lo, hi):
 
 def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
                   max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False, overlaps=None,
-                  num_speakers=None, min_speakers=None, max_speakers=None):
+                  num_speakers=None, min_speakers=None, max_speakers=None, link_threshold=None):
     """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
     recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
     one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
@@ -357,13 +357,21 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     ('mass'); too few re-run the VB-HMM from the AHC linkage cut at lo clusters ('recut', or the cut itself: 'ahc';
     'unmet' when the recording has fewer than lo x-vectors).  Each item then also has count_rule, n_speakers_vb (the
     unconstrained count) and count = (lo, hi or None).
+    link_threshold: None, or an LLR threshold for speaker linking across the archive (DESIGN.md section 5.15, after the
+    count rules): the speakers of all recordings are scored pairwise from their VB-HMM posteriors and clustered on the
+    device (link.link_speakers), and speakers whose average LLR is at least the threshold share an archive-wide id.
+    Each item then also has global_speakers ({label: global id}, link.link_cut) and rttm_linked (its rttm lines, or
+    rttm_overlap's with overlaps, with the speaker field set to global id + 1).
     Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds]
-    [, count_rule, n_speakers_vb, count])}."""
+    [, count_rule, n_speakers_vb, count][, global_speakers, rttm_linked])}."""
     if init not in ('AHC', 'AHC+VB'):
         raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
     if overlaps is not None and init == 'AHC':
         raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
     bounds = count_bounds(list(recordings), num_speakers, min_speakers, max_speakers)
+    if link_threshold is not None:
+        from .link import check_threshold
+        check_threshold(link_threshold)
     if not torch.cuda.is_available():
         from ._lib import VbxError
         raise VbxError('diarize_batch(): no CUDA device - vbx_b200 has no CPU fallback')
@@ -408,6 +416,11 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
         if bounds is not None:
             _count_rerun(bounds, Zs, lens, offs, fea, Phi, dev, k1, rules, labels1, labels2, iters, smoothing,
                          Fa=Fa, Fb=Fb, loopProb=loopP, maxIters=max_iters, epsilon=epsilon)
+    maps = None
+    if link_threshold is not None:
+        from . import link as _link
+        table, _, _, Z = _link.link_speakers(fea, Phi, offs, labels1, Fa, Fb, dev)
+        maps = _link.link_cut(Z, table, link_threshold, labels2)
     for b, n in enumerate(names):
         ovl = None
         if overlaps is not None:
@@ -416,7 +429,22 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
         out[n] = _result(n, recordings[n][1], labels1[b], labels2[b], iters[b], output_2nd, ovl)
         if bounds is not None:
             _count_fields(out[n], k1[b], rules[b], bounds[0][b], bounds[1][b])
+        if maps is not None:
+            out[n].update(global_speakers=maps[b],
+                          rttm_linked=linked_lines(n, recordings[n][1], labels1[b], labels2[b], maps[b], ovl))
     return out
+
+
+def linked_lines(name, seg_times, labels, labels2, mapping, overlap=None):
+    """RTTM lines of one recording with archive-wide speakers (DESIGN.md section 5.15): the lines _result writes (the
+    overlap-aware ones when overlap regions (lo, hi) ticks are given, else the merged first labels) with every label
+    replaced by mapping[label] (link.link_cut).  The map is one-to-one within a recording, so the segments are the same.
+    labels2 is used inside the overlap regions only."""
+    from .link import relabel
+    seg = np.asarray(seg_times, dtype=np.float64)
+    if overlap is not None:
+        return rttm_lines(name, *overlap_segments(seg, relabel(labels, mapping), relabel(labels2, mapping), overlap))
+    return rttm_lines(name, *merge_adjacent_labels(seg[:, 0], seg[:, 1], relabel(labels, mapping)))
 
 
 def _count_rerun(bounds, Zs, lens, offs, fea, Phi, dev, k1, rules, labels1, labels2, iters, smoothing, **run_kw):

@@ -70,6 +70,11 @@ def merge_turns(starts, ends):
 def reference_turns(rows):
     """formats.read_rttm rows -> {recording: [(starts, ends) merged ticks, one pair per speaker, speakers by name]}.
     Speakers whose turns are all empty are dropped; more than 64 speakers in a recording raise ValueError."""
+    return {rec: [t for _, t in spk] for rec, spk in named_reference_turns(rows).items()}
+
+
+def named_reference_turns(rows):
+    """reference_turns() with each speaker's RTTM name kept: {recording: [(name, (starts, ends))]}, same order."""
     per = {}
     for rec, start, dur, spk in rows:
         per.setdefault(rec, {}).setdefault(spk, []).append((start, start + dur))
@@ -80,7 +85,7 @@ def reference_turns(rows):
             t = to_ticks(np.array(spks[spk], dtype=np.float64))
             s, e = merge_turns(t[:, 0], t[:, 1])
             if len(s):
-                turns.append((s, e))
+                turns.append((spk, (s, e)))
         if len(turns) > MAX_REF_SPEAKERS:
             raise ValueError(f'recording {rec!r}: {len(turns)} reference speakers, at most {MAX_REF_SPEAKERS} are supported')
         out[rec] = turns
@@ -355,7 +360,7 @@ def _overlap_split(rec, proto):
     return lo, hi, mask, np.zeros(len(lo), dtype=np.uint8)
 
 
-def score_entries(recordings, entries, device=None, jer=None):
+def score_entries(recordings, entries, device=None, jer=None, blocks=False):
     """Score many (recording, labels) entries in one vbx_score launch per protocol.
     recordings: list of ScoredRecording (all with the same protocols); entries: [(recording index, labels)], labels int
     [len(sys_lo)] in [0, n) (n = max label + 1).  Returns [{protocol: result dict}] in entry order.  A label outside
@@ -366,7 +371,8 @@ def score_entries(recordings, entries, device=None, jer=None):
     jer: None, or the name of a protocol with collar 0 and overlaps scored (DESIGN.md section 5.13).  That protocol's
     launch goes to vbx_score_jer, which also sums each label's scored time, and every entry's dict gains
     'jer': jer_finish() (replacing the DER of a protocol that is itself named 'jer').  Any other protocol raises
-    ValueError."""
+    ValueError.
+    blocks: every entry's dict also gains 'O': {protocol: its n_ref x n labels overlap block, int64 ticks}."""
     import torch
     from . import _lib
     from ._lib import VbxError
@@ -465,6 +471,8 @@ def score_entries(recordings, entries, device=None, jer=None):
         for i, b in enumerate(rec_idx):
             blk = O[o_off[i]:o_off[i] + cells[i]].reshape(int(n_ref[b]), int(n_labels[i]))
             res[i][proto] = finish(cov[i], fa[i], blk, recordings[b].regions[proto][3])
+            if blocks:
+                res[i].setdefault('O', {})[proto] = blk
     if jer is not None:
         O, T = host[jer][2], host[jer][4]
         R = [reference_time(r.regions[jer], r.n_ref) for r in recordings]
@@ -519,6 +527,8 @@ def system_stretches(rows, recording=''):
     l1, l2 = np.full(len(lo), -1, dtype=np.int32), np.full(len(lo), -1, dtype=np.int32)
     n = np.zeros(len(lo), dtype=np.int64)
     for k, (s, e) in enumerate(turns):
+        if len(s) == 0:                 # a speaker whose turns are all empty says nothing
+            continue
         j = np.searchsorted(s, lo, 'right') - 1
         act = (j >= 0) & (e[np.maximum(j, 0)] > lo)
         l2 = np.where(act & (l1 >= 0), k, l2)
@@ -532,19 +542,24 @@ def system_stretches(rows, recording=''):
     return lo[keep], hi[keep], l1[keep], l2[keep]
 
 
-def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=None, overlapping=False, jer=False):
+def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=None, overlapping=False, jer=False,
+               across_files=False):
     """DER of system RTTM rows against reference RTTM rows (both as formats.read_rttm returns them).
     uem: None or {recording: [(onset, offset)]} (formats.read_uem).  overlapping: the system may have two speakers at
     once (system_stretches, scored by vbx_score_overlap); otherwise overlapping system turns raise ValueError.  Returns
     ({recording: result dict}, overall result dict) over the reference's recordings.
     jer: also the Jaccard error rate (DESIGN.md section 5.13; no collar, overlaps scored, whatever the DER uses): every
     result dict gains jer (None without a counted reference speaker) and each recording's also jer_ticks
-    (jer_finish()['ticks'])."""
+    (jer_finish()['ticks']).
+    across_files: speakers are one speaker in every file where they have the same RTTM name, in the reference and in
+    the system (DESIGN.md section 5.15); the overall dict gains across_files, a result dict with the overall miss and fa
+    and conf = sum of covered - max one-to-one matching of the overlaps summed over all files by name."""
     c = collar_ticks(collar)
     # JER is taken without a collar and with overlaps: from the DER's own launch when that is the protocol, else from
     # one more region set
     jer_proto = None if not jer else 'score' if c == 0 and not ignore_overlaps else 'jer'
-    ref = reference_turns(ref_turns)
+    named = named_reference_turns(ref_turns)
+    ref = {rec: [t for _, t in spk] for rec, spk in named.items()}
     sys_by = _rows_by_recording(sys_turns)
     extra = sorted(set(sys_by) - set(ref))
     if extra:
@@ -564,14 +579,41 @@ def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=N
         lo, hi, lab = system_turns(sys_by.get(n, []), n)
         recs.append(prepare_recording(n, ref[n], (lo, hi, hi), u, proto))
         entries.append((b, lab))
-    res = score_entries(recs, entries, device, jer=jer_proto)
+    res = score_entries(recs, entries, device, jer=jer_proto, blocks=across_files)
     per = {n: r['score'] for n, r in zip(names, res)}
     tot = overall(list(per.values()))
+    if across_files:
+        sys_names = {n: sorted(set(r[3] for r in sys_by.get(n, []))) for n in names}
+        tot['across_files'] = across_files_result(tot, [[k for k, _ in named[n]] for n in names],
+                                                  [sys_names[n] for n in names], [r['O']['score'] for r in res])
     if jer:
         for n, r in zip(names, res):
             per[n] = dict(per[n], jer=r['jer']['jer'], jer_ticks=r['jer']['ticks'])
         tot['jer'] = overall_jer([r['jer'] for r in res])['jer']
     return per, tot
+
+
+def across_files_result(tot, ref_names, sys_names, blocks):
+    """DER across files (DESIGN.md section 5.15) from overall() `tot` of the per-file results and, per file, the names
+    of its reference speakers (block rows), of its system labels (sorted, as system_turns numbers them) and its overlap
+    block: the blocks are summed by name and matched once.  A block has a column for every label up to the last one with
+    a non-empty turn, so names past it (speakers whose turns are all empty) and a file without system names add nothing."""
+    from scipy.optimize import linear_sum_assignment
+    rows = {k: i for i, k in enumerate(sorted({k for ks in ref_names for k in ks}))}
+    cols = {k: i for i, k in enumerate(sorted({k for ks in sys_names for k in ks}))}
+    O = np.zeros((len(rows), len(cols)), dtype=np.int64)
+    for rk, sk, blk in zip(ref_names, sys_names, blocks):
+        blk = np.asarray(blk)
+        w = min(blk.shape[1], len(sk))
+        if rk and w:
+            np.add.at(O, np.ix_([rows[k] for k in rk], [cols[k] for k in sk[:w]]), blk[:, :w])
+    matched = 0
+    if O.size:
+        r, c = linear_sum_assignment(O, maximize=True)
+        matched = int(O[r, c].sum())
+    t = tot['ticks']
+    covered = t['scored'] - t['miss']
+    return result(t['miss'], t['fa'], covered - matched, t['scored'])
 
 
 def read_rttm_path(path):
@@ -600,6 +642,8 @@ def build_parser():
     ap.add_argument('--json', action='store_true', help='print one JSON object instead of the table')
     ap.add_argument('--jer', action='store_true',
                     help='also the Jaccard error rate (no collar, overlaps scored, whatever the DER options)')
+    ap.add_argument('--across-files', action='store_true',
+                    help='also the DER with each speaker name one speaker in every file (ACROSS FILES row)')
     return ap
 
 
@@ -608,18 +652,21 @@ def main(argv=None):
     from . import formats
     uem = formats.read_uem(args.uem) if args.uem else None
     per, tot = score_rttm(read_rttm_path(args.ref_rttm), read_rttm_path(args.sys_rttm), args.collar,
-                          args.ignore_overlaps, uem, overlapping=args.overlapping_system, jer=args.jer)
+                          args.ignore_overlaps, uem, overlapping=args.overlapping_system, jer=args.jer,
+                          across_files=args.across_files)
     if args.json:
         print(json.dumps(dict(collar=args.collar, ignore_overlaps=args.ignore_overlaps, files=per, overall=tot),
                          sort_keys=True))
         return 0
-    w = max([len('OVERALL')] + [len(n) for n in per])
+    rows = list(per.items()) + [('OVERALL', tot)] + ([('ACROSS FILES', tot['across_files'])] if args.across_files else [])
+    w = max(len(n) for n, _ in rows)
     jer_head = f'  {"JER %":>7}' if args.jer else ''
     print(f'{"file":<{w}}  {"DER %":>7}  {"miss %":>7}  {"FA %":>7}  {"conf %":>7}  {"scored s":>10}{jer_head}')
-    for n, r in list(per.items()) + [('OVERALL', tot)]:
+    for n, r in rows:
         pct = [100.0 * r[k] / r['scored'] if r['scored'] else float('nan') for k in ('miss', 'fa', 'conf')]
         der = 100.0 * r['der'] if r['der'] is not None else float('nan')
-        jer_col = (f'  {100.0 * r["jer"] if r["jer"] is not None else float("nan"):7.2f}') if args.jer else ''
+        jer = r.get('jer') if n != 'ACROSS FILES' else None
+        jer_col = (f'  {100.0 * jer if jer is not None else float("nan"):7.2f}') if args.jer else ''
         print(f'{n:<{w}}  {der:7.2f}  {pct[0]:7.2f}  {pct[1]:7.2f}  {pct[2]:7.2f}  {r["scored"]:10.2f}{jer_col}')
     return 0
 
