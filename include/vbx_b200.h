@@ -201,6 +201,29 @@ int vbx_link(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int3
              int64_t M, const int32_t *speaker_rec, double Fa, double Fb, void *workspace, size_t workspace_bytes,
              double *n_out, double *F_out, double *dist_out, double *Z_out, void *stream);
 
+/* Enrolment against known speakers (DESIGN.md section 5.16); needs a handle, no plan.  Archive speakers as for vbx_link
+ * (fea [N,R], Phi [R], speaker [N] in [0, M), DEVICE), packed by recording: speaker_rec_offsets [n_rec+1] (HOST int64,
+ * from 0 to M, non-decreasing) holds recording b's speakers at speaker_rec_offsets[b] .. [b+1]-1.  Enrolled speakers:
+ * enroll_fea [N_e,R] (DEVICE, the same features and Phi) with enroll_speaker [N_e] in [0, E) (DEVICE; packed by speaker
+ * the statistics cost about (E + R) N_e reads).  Both sets get vbx_link's statistics n, F, b, e (its kernels), and
+ *   llr [s][e] = LLR(s, e) of vbx_link, bit-identical to -dist of vbx_link run on the same speakers.
+ * Per recording with K speakers, the minimum-cost assignment of the K x (E + K) matrix C[k][e] = threshold - llr[k][e]
+ * (e < E), C[k][E + j] = 0, by shortest augmenting paths; ties to the lowest column.  Outputs (DEVICE):
+ *   assign_out [M] int32      the enrolled speaker of each archive speaker, -1 = unknown
+ *   best_llr_out [M]          llr of the assigned pair; for an unknown speaker its largest llr
+ *   llr_out [M,E], n_out [M], F_out [M,R], n_enroll_out [E], F_enroll_out [E,R]: optional (NULL: not written)
+ * workspace: vbx_enroll_workspace_bytes(M, E, max_k) bytes with max_k >= the largest K, 256-byte aligned (about
+ * 8 M E + 1.1 KB (M + E) + 2 x SMs x 50 (E + max_k) bytes).  The offsets are copied to the device from pageable memory:
+ * no host synchronisation, no allocation.  VBX_ERR_ARG: R outside 1..128, c = Fa / Fb negative or not finite,
+ * |threshold| > 1e15, E or N_e < 1, null pointers, misaligned or short workspace, offsets not from 0 to M or
+ * decreasing. */
+int vbx_enroll_workspace_bytes(vbx_handle_t h, int64_t M, int64_t E, int64_t max_k, size_t *bytes_out);
+int vbx_enroll(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
+               int64_t M, const int64_t *speaker_rec_offsets, int32_t n_rec, const float *enroll_fea, int64_t N_e,
+               const int32_t *enroll_speaker, int64_t E, double Fa, double Fb, double threshold, void *workspace,
+               size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
+               double *F_out, double *n_enroll_out, double *F_enroll_out, void *stream);
+
 /* Float64 evaluation of the same EM loop ("exact" mode for the one-recording-per-call use of VBx/vbhmm.py:154-158,
  * where the reference stops on an ELBO improvement < 1e-6, VBx/vbhmm.py:157 -- below float32 resolution).
  * All arrays float64: fea [N,R] (the reference's X, VBx/VBx.py:30), Phi [R], gamma_io [N,S], pi_io [n_rec,S],

@@ -1,7 +1,8 @@
 """Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection at
 D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
 6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels (also under a speaker-count bound),
-the dense forward_backward(), the ELBO trace, DER / JER scoring and speaker linking across recordings.
+the dense forward_backward(), the ELBO trace, DER / JER scoring, speaker linking across recordings and enrolment
+against known speakers.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
 """
@@ -96,6 +97,22 @@ l_phi = torch.rand(16, device=dev) * (torch.arange(16, device=dev) < 13)
 l_out = link.link_speakers(l_fea, l_phi, np.concatenate([[0], np.cumsum(l_lens)]), l_labels, 0.3, 17.0, dev, dist=True)
 torch.cuda.synchronize()
 print('link ok', len(l_out[0].rec), float(l_out[3][:, 2].min()))
+
+# enrolment (vbx_enroll): recordings without speakers, E = 1 and E < K_b, a tail tile (M, E not multiples of 32), and a
+# recording with 150 speakers (more than 128)
+from vbx_b200 import enroll  # noqa: E402
+e_lens = l_lens + [600]
+e_labels = l_labels + [np.concatenate([np.arange(150), gl.integers(0, 150, 450)])]
+e_fea = torch.cat([l_fea, torch.randn((600, 16), device=dev)])
+e_fea[:, 13:] = 0
+for E in (1, 7, 45):
+    e_x = torch.randn((2 * E + 1, 16), device=dev)
+    e_x[:, 13:] = 0
+    e_spk = np.concatenate([np.arange(E), np.arange(E), [0]])
+    e_out = enroll.enroll_speakers(e_fea, l_phi, np.concatenate([[0], np.cumsum(e_lens)]), e_labels, e_x, e_spk, 0.3,
+                                   17.0, 0.0, dev, llr=True, max_bytes=8 * E * 100)
+    torch.cuda.synchronize()
+    print('enroll ok', E, len(e_out.table.rec), int((e_out.assign >= 0).sum()))
 
 # wgmma projection at the smallest and largest D, one frame and one frame past a full wave of tiles
 sms = torch.cuda.get_device_properties(0).multi_processor_count

@@ -18,6 +18,12 @@ With --num-speakers K, or --min-speakers / --max-speakers, every recording's spe
 With --link-threshold X the speakers of all recordings are linked across the archive (DESIGN.md section 5.15): every
 written RTTM (and with --output-2nd every second-label RTTM) names its speakers by archive-wide id, so the same speaker
 has the same name in every file.  Speakers are linked where their average same-speaker log-likelihood ratio is >= X.
+
+With --enroll-ark FILE --enroll-utt2spk FILE --enroll-threshold X (all three or none) the speakers are named by the
+enrolled speakers of the ark (DESIGN.md section 5.16): a speaker whose log-likelihood ratio against an enrolled speaker
+reaches X takes that speaker's name, one name per speaker within a recording; the others are written as
+unknown-<recording>-<label>, or with --link-threshold linked among themselves and written as unknown-<id>.  With
+--output-2nd the second-label RTTMs use the same names.
 """
 import argparse
 import os
@@ -85,15 +91,24 @@ def build_parser():
     ap.add_argument('--link-threshold', default=None, type=float,
                     help='link speakers across the recordings: one name per speaker in every file where their average '
                          'same-speaker log-likelihood ratio is >= this')
+    ap.add_argument('--enroll-ark', default=None, help='x-vectors of known speakers (Kaldi ark) to name speakers by')
+    ap.add_argument('--enroll-utt2spk', default=None, help='the speaker of each x-vector of --enroll-ark (utt2spk)')
+    ap.add_argument('--enroll-threshold', default=None, type=float,
+                    help='least log-likelihood ratio at which a speaker takes an enrolled name')
     return ap
 
 
 def main(argv=None):
-    args = build_parser().parse_args(argv)
+    ap = build_parser()
+    args = ap.parse_args(argv)
     assert 0 <= args.loopP <= 1, f'Expecting loopP between 0 and 1, got {args.loopP} instead.'     # VBx/vbhmm.py:103
+    enr = [args.enroll_ark, args.enroll_utt2spk, args.enroll_threshold]
+    if any(v is not None for v in enr) and any(v is None for v in enr):
+        ap.error('--enroll-ark, --enroll-utt2spk and --enroll-threshold go together')
     from . import formats
-    from .pipeline import diarize_batch, linked_lines
+    from .pipeline import diarize_batch, linked_lines, named_lines
     from .score import read_overlaps
+    enroll = formats.read_enrolment(args.enroll_ark, args.enroll_utt2spk) if args.enroll_ark is not None else None
     overlaps = read_overlaps(args.overlap_rttm) if args.overlap_rttm is not None else None
     segs = formats.read_segments(args.segments_file)                        # VBx/vbhmm.py:105
     plda = formats.read_kaldi_plda(args.plda_file)                          # VBx/vbhmm.py:107
@@ -108,18 +123,22 @@ def main(argv=None):
                         threshold=args.threshold, smoothing=args.init_smoothing, init=args.init, chain=args.chain,
                         device=args.device, output_2nd=args.output_2nd, overlaps=overlaps,
                         num_speakers=args.num_speakers, min_speakers=args.min_speakers, max_speakers=args.max_speakers,
-                        link_threshold=args.link_threshold)
+                        link_threshold=args.link_threshold, enroll=enroll, enroll_threshold=args.enroll_threshold)
     linked = args.link_threshold is not None
     os.makedirs(args.out_rttm_dir, exist_ok=True)                           # VBx/vbhmm.py:170
     for name, item in out.items():
-        key = 'rttm_linked' if linked else 'rttm' if overlaps is None else 'rttm_overlap'
+        key = 'rttm_named' if enroll is not None else 'rttm_linked' if linked else \
+            'rttm' if overlaps is None else 'rttm_overlap'
         with open(os.path.join(args.out_rttm_dir, f'{name}.rttm'), 'w') as fp:
             fp.write(''.join(line + os.linesep for line in item[key]))
         if item['rttm2nd'] is not None:
             d2 = f'{args.out_rttm_dir}2nd'
             os.makedirs(d2, exist_ok=True)
-            lines = item['rttm2nd'] if not linked else \
-                linked_lines(name, recs[name][1], item['labels2nd'], None, item['global_speakers'])
+            if enroll is not None:
+                lines = named_lines(name, recs[name][1], item['labels2nd'], None, item['speaker_names'])
+            else:
+                lines = item['rttm2nd'] if not linked else \
+                    linked_lines(name, recs[name][1], item['labels2nd'], None, item['global_speakers'])
             with open(os.path.join(d2, f'{name}.rttm'), 'w') as fp:
                 fp.write(''.join(line + os.linesep for line in lines))
     return 0

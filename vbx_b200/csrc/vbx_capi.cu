@@ -3,6 +3,7 @@
 #include <nvtx3/nvToolsExt.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <numeric>
@@ -860,6 +861,50 @@ int vbx_link(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int3
     if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     return counted(h, vbx::launch_link(fea, Phi, speaker, N, R, speaker_rec, M, c, workspace, n_out, F_out, dist_out,
                                        Z_out, (cudaStream_t)stream), "link");
+}
+
+int vbx_enroll_workspace_bytes(vbx_handle_t h, int64_t M, int64_t E, int64_t max_k, size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    if (M < 0 || E < 1 || max_k < 0 || max_k > M)
+        return fail(h, VBX_ERR_ARG, "vbx_enroll_workspace_bytes: need M >= 0, E >= 1 and 0 <= max_k <= M");
+    *bytes_out = vbx::enroll_workspace_bytes(M, E, max_k, h->sms);
+    return VBX_OK;
+}
+
+int vbx_enroll(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
+               int64_t M, const int64_t *speaker_rec_offsets, int32_t n_rec, const float *enroll_fea, int64_t N_e,
+               const int32_t *enroll_speaker, int64_t E, double Fa, double Fb, double threshold, void *workspace,
+               size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
+               double *F_out, double *n_enroll_out, double *F_enroll_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_enroll");
+    if (N < 0 || M < 0 || n_rec < 0 || N_e < 1 || E < 1)
+        return fail(h, VBX_ERR_ARG, "vbx_enroll: need N, M, n_rec >= 0 and N_e, E >= 1");
+    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, "vbx_enroll: R must lie in [1, 128]");
+    const double c = Fa / Fb;
+    if (!(c >= 0.0) || c == INFINITY) return fail(h, VBX_ERR_ARG, "vbx_enroll: Fa / Fb must be finite and >= 0");
+    if (!(std::fabs(threshold) <= 1e15)) return fail(h, VBX_ERR_ARG, "vbx_enroll: |threshold| must be <= 1e15");
+    if (!Phi || !workspace || !speaker_rec_offsets || !enroll_fea || !enroll_speaker || (N > 0 && (!fea || !speaker)) ||
+        (M > 0 && (!assign_out || !best_llr_out)))
+        return fail(h, VBX_ERR_ARG, "vbx_enroll: null pointer");
+    if (speaker_rec_offsets[0] != 0 || speaker_rec_offsets[n_rec] != M)
+        return fail(h, VBX_ERR_ARG, "vbx_enroll: speaker_rec_offsets must run from 0 to M");
+    int64_t max_k = 0;
+    for (int32_t b = 0; b < n_rec; ++b) {
+        const int64_t k = speaker_rec_offsets[b + 1] - speaker_rec_offsets[b];
+        if (k < 0) return fail(h, VBX_ERR_ARG, "vbx_enroll: speakers are not packed by recording (offsets decrease)");
+        max_k = std::max(max_k, k);
+    }
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
+        return fail(h, VBX_ERR_ARG, "vbx_enroll: workspace must be 256-byte aligned");
+    if (workspace_bytes < vbx::enroll_workspace_bytes(M, E, max_k, h->sms))
+        return fail(h, VBX_ERR_ARG, "vbx_enroll: workspace smaller than vbx_enroll_workspace_bytes()");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_enroll(fea, Phi, N, R, speaker, M, speaker_rec_offsets, n_rec, enroll_fea, N_e,
+                                         enroll_speaker, E, c, threshold, workspace, h->sms, assign_out, best_llr_out,
+                                         llr_out, n_out, F_out, n_enroll_out, F_enroll_out, (cudaStream_t)stream),
+                   "enroll");
 }
 
 int vbx_f64_workspace_bytes(vbx_handle_t h, size_t *bytes_out) {

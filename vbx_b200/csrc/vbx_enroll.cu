@@ -1,0 +1,325 @@
+// Enrolment against known speakers (DESIGN.md section 5.16).  The archive's speakers (section 5.15's table) and the
+// enrolled speakers get the statistics n, F, b and e of vbx_link (its span and statistics kernels, through
+// launch_speaker_stats), every archive speaker s is scored against every enrolled speaker e with section 5.15's LLR,
+// and each recording's speakers are assigned one-to-one to enrolled speakers or to "unknown":
+//   enroll_score_kernel   llr [M, E], 32 x 32 tiles of the rectangle; per pair the operations of vbx_link's score_tile
+//                         in the same order, so llr[s][e] is bit-identical to -dist[s][e] of vbx_link on the same speakers
+//   enroll_assign_kernel  per recording b with K_b speakers the minimum-cost assignment of the K_b x (E + K_b) matrix
+//                         C[k][e] = threshold - llr[k][e] (e < E), C[k][E + j] = 0 ("unknown" columns), by shortest
+//                         augmenting paths (Jonker-Volgenant, the method of scipy's linear_sum_assignment): one
+//                         Dijkstra per row over the columns; a persistent grid, one recording per CTA at a time
+#include <algorithm>
+#include <climits>
+#include <vector>
+
+#include "vbx_internal.cuh"
+
+namespace vbx {
+
+namespace {
+
+constexpr int kLogGroup = 8;                // as vbx_link: log of a product of 8 denominators
+constexpr int64_t kScoreGrid = 1 << 20;     // CTAs of enroll_score_kernel at most; beyond that they stride over the tiles
+constexpr int kAssignThreads = 256;
+constexpr int kAssignWarps = kAssignThreads / 32;
+constexpr int kAssignCtasPerSm = 2;
+
+__host__ __device__ size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// one CTA's column and row state in the workspace: columns nc = E + K_b <= E + max_k, rows K_b <= max_k
+struct Slice {
+    double *v, *spc, *u;                // column duals, shortest path costs; row duals
+    int64_t *path, *row4col, *col4row;  // row reaching each column, row of each column, column of each row (-1: none)
+    uint8_t *sc, *sr;                   // columns / rows reached in the current Dijkstra
+};
+
+__host__ __device__ Slice slice_at(uint8_t *base, int64_t ncm, int64_t km, size_t *total) {
+    Slice s;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { uint8_t *p = base ? base + o : nullptr; o += al(bytes); return p; };
+    s.v = reinterpret_cast<double *>(take(ncm * 8));
+    s.spc = reinterpret_cast<double *>(take(ncm * 8));
+    s.u = reinterpret_cast<double *>(take(km * 8));
+    s.path = reinterpret_cast<int64_t *>(take(ncm * 8));
+    s.row4col = reinterpret_cast<int64_t *>(take(ncm * 8));
+    s.col4row = reinterpret_cast<int64_t *>(take(km * 8));
+    s.sc = take(ncm);
+    s.sr = take(km);
+    if (total) *total = o;
+    return s;
+}
+
+struct EnrollWs {
+    SpeakerStats a, en;      // archive speakers [M], enrolled speakers [E]
+    double *llr;             // [M, E]
+    int64_t *recs;           // [n_busy + 1]: speaker offsets of the recordings that have speakers
+    uint8_t *slices;         // ctas x slice_bytes
+    size_t slice_bytes;
+    int64_t ctas;
+};
+
+EnrollWs enroll_layout(uint8_t *ws, int64_t M, int64_t E, int64_t max_k, int sms, size_t *total) {
+    EnrollWs w;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { uint8_t *p = ws ? ws + o : nullptr; o += al(bytes); return p; };
+    auto stats = [&](int64_t n) {
+        SpeakerStats s;
+        s.n = reinterpret_cast<double *>(take(n * 8));
+        s.e = reinterpret_cast<double *>(take(n * 8));
+        s.b = reinterpret_cast<double *>(take(n * kMaxR * 8));
+        s.first = reinterpret_cast<long long *>(take(n * 8));
+        s.last = reinterpret_cast<long long *>(take(n * 8));
+        s.offs = reinterpret_cast<int64_t *>(take(4 * 8));
+        return s;
+    };
+    w.a = stats(M);
+    w.en = stats(E);
+    w.llr = reinterpret_cast<double *>(take((size_t)M * E * 8));
+    w.recs = reinterpret_cast<int64_t *>(take((M + 1) * 8));
+    slice_at(nullptr, E + max_k, max_k, &w.slice_bytes);
+    w.ctas = std::min<int64_t>((int64_t)kAssignCtasPerSm * std::max(sms, 1), std::max<int64_t>(M, 1));
+    w.slices = take(w.slice_bytes * w.ctas);
+    if (total) *total = o;
+    return w;
+}
+
+// Tile (bi, bj) of 32 archive speakers (rows) x 32 enrolled speakers (columns): 256 threads, 4 pairs each (rows ty,
+// ty + 8, ..), features in chunks of 32 through shared memory; every operation as in vbx_link's score_tile.
+__global__ void __launch_bounds__(256) enroll_score_kernel(SpeakerStats A, SpeakerStats En, const float *__restrict__ Phi,
+                                                           int64_t M, int64_t E, int R, double c, double *__restrict__ llr,
+                                                           double *__restrict__ llr_out) {
+    __shared__ double a[32][33], bt[32][33], ph[32];
+    const int64_t tiles_e = (E + 31) / 32, n_tiles = ((M + 31) / 32) * tiles_e;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const int64_t i0 = (t / tiles_e) * 32, j0 = (t % tiles_e) * 32;
+        const int64_t j = j0 + tx;
+        const double nj = j < E ? En.n[j] : 0.0;
+        double cm[4], q[4] = {0, 0, 0, 0}, lg[4] = {0, 0, 0, 0}, prod[4] = {1, 1, 1, 1};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int64_t i = i0 + ty + 8 * u;
+            cm[u] = c * ((i < M ? A.n[i] : 0.0) + nj);
+        }
+        for (int r0 = 0; r0 < R; r0 += 32) {
+            for (int v = ty; v < 32; v += 8) {
+                const int r = r0 + tx;
+                a[v][tx] = (i0 + v < M && r < R) ? A.b[(i0 + v) * kMaxR + r] : 0.0;
+                bt[v][tx] = (j0 + v < E && r < R) ? En.b[(j0 + v) * kMaxR + r] : 0.0;
+            }
+            if (ty == 0) ph[tx] = r0 + tx < R ? (double)Phi[r0 + tx] : 0.0;
+            __syncthreads();
+            const int len = min(32, R - r0);
+            for (int k = 0; k < len; ++k) {
+                const double bj_k = bt[tx][k], p = ph[k];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    const double den = fma(cm[u], p, 1.0), x = a[ty + 8 * u][k] + bj_k;
+                    q[u] += x * x / den;
+                    prod[u] *= den;
+                }
+                if (((r0 + k) % kLogGroup) == kLogGroup - 1 || r0 + k == R - 1) {
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) {
+                        lg[u] += log(prod[u]);
+                        prod[u] = 1.0;
+                    }
+                }
+            }
+            __syncthreads();                          // also keeps the next tile's loads behind this tile's reads
+        }
+        if (j >= E) continue;
+        const double ej = En.e[j];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int64_t i = i0 + ty + 8 * u;
+            if (i >= M) continue;
+            const double l = (A.n[i] == 0.0 || nj == 0.0) ? 0.0 : 0.5 * ((q[u] - lg[u]) - (A.e[i] + ej));
+            llr[i * E + j] = l;
+            if (llr_out) llr_out[i * E + j] = l;
+        }
+    }
+}
+
+// (value, column) pairs: the smaller value, on equal values the lower column (-1 only comes with +inf)
+__device__ __forceinline__ void take_min(double &bv, int64_t &bj, double ov, int64_t oj) {
+    if (ov < bv || (ov == bv && oj < bj)) {
+        bv = ov;
+        bj = oj;
+    }
+}
+
+// One CTA per recording at a time.  Per row (speaker) cur = 0 .. K-1 one Dijkstra over the columns: every step scans the
+// columns not yet reached, relaxes their path costs from row i (r = minVal + C[i][j] - u[i] - v[j], scipy's order) and
+// takes the block argmin; ties go to the lowest column index (so a real column at cost 0 wins over the unknown
+// columns).  A reached column that no row holds ends the path; otherwise its row is scanned next.  Then the duals are
+// updated and the path augmented as scipy's rectangular_lsap does.  A step that reaches no column (non-finite costs)
+// leaves the row unassigned.  Outputs per speaker: its enrolled index or -1, and the LLR of its pair, or for an
+// unknown speaker its largest LLR.
+__global__ void __launch_bounds__(kAssignThreads) enroll_assign_kernel(const double *__restrict__ llr,
+                                                                      const int64_t *__restrict__ recs, int64_t n_recs,
+                                                                      int64_t E, double theta, uint8_t *slices,
+                                                                      size_t slice_bytes, int64_t max_k,
+                                                                      int32_t *__restrict__ assign_out,
+                                                                      double *__restrict__ best_out) {
+    __shared__ double wv[kAssignWarps];
+    __shared__ int64_t wj[kAssignWarps];
+    __shared__ double s_min;
+    __shared__ int64_t s_i, s_sink;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const Slice sl = slice_at(slices + (size_t)blockIdx.x * slice_bytes, E + max_k, max_k, nullptr);
+    for (int64_t rec = blockIdx.x; rec < n_recs; rec += gridDim.x) {
+        const int64_t s0 = recs[rec], K = recs[rec + 1] - s0, nc = E + K;
+        for (int64_t j = tid; j < nc; j += kAssignThreads) {
+            sl.v[j] = 0.0;
+            sl.row4col[j] = -1;
+        }
+        for (int64_t k = tid; k < K; k += kAssignThreads) {
+            sl.u[k] = 0.0;
+            sl.col4row[k] = -1;
+        }
+        for (int64_t cur = 0; cur < K; ++cur) {
+            for (int64_t j = tid; j < nc; j += kAssignThreads) {
+                sl.spc[j] = INFINITY;
+                sl.sc[j] = 0;
+            }
+            for (int64_t k = tid; k < K; k += kAssignThreads) sl.sr[k] = 0;
+            if (tid == 0) {
+                s_i = cur;
+                s_sink = -1;
+                s_min = 0.0;
+            }
+            __syncthreads();
+            int64_t i = cur, sink = -1;
+            double minVal = 0.0;
+            for (int64_t step = 0; step < nc && sink == -1; ++step) {
+                const double ui = sl.u[i];
+                const double *lrow = llr + (s0 + i) * E;
+                double bv = INFINITY;
+                int64_t bj = -1;
+                for (int64_t j = tid; j < nc; j += kAssignThreads) {
+                    if (sl.sc[j]) continue;
+                    const double cost = j < E ? theta - lrow[j] : 0.0;
+                    const double r = minVal + cost - ui - sl.v[j];
+                    double p = sl.spc[j];
+                    if (r < p) {
+                        sl.path[j] = i;
+                        sl.spc[j] = r;
+                        p = r;
+                    }
+                    if (p < bv) {                             // strided in increasing j: the lowest column on ties
+                        bv = p;
+                        bj = j;
+                    }
+                }
+                for (int o = 16; o; o >>= 1)
+                    take_min(bv, bj, __shfl_xor_sync(0xffffffffu, bv, o), __shfl_xor_sync(0xffffffffu, bj, o));
+                if (lane == 0) {
+                    wv[warp] = bv;
+                    wj[warp] = bj;
+                }
+                __syncthreads();
+                if (tid == 0) {
+                    for (int q = 1; q < kAssignWarps; ++q) take_min(bv, bj, wv[q], wj[q]);
+                    sl.sr[i] = 1;
+                    if (bj < 0) {
+                        s_sink = -2;
+                    } else {
+                        sl.sc[bj] = 1;
+                        s_min = bv;
+                        if (sl.row4col[bj] < 0) s_sink = bj;
+                        else s_i = sl.row4col[bj];
+                    }
+                }
+                __syncthreads();
+                minVal = s_min;
+                sink = s_sink;
+                i = s_i;
+            }
+            if (sink >= 0) {                                  // every thread saw the same sink
+                for (int64_t k = tid; k < K; k += kAssignThreads)
+                    if (sl.sr[k] && k != cur) sl.u[k] += minVal - sl.spc[sl.col4row[k]];
+                for (int64_t j = tid; j < nc; j += kAssignThreads)
+                    if (sl.sc[j]) sl.v[j] -= minVal - sl.spc[j];
+                __syncthreads();
+                if (tid == 0) {
+                    sl.u[cur] += minVal;
+                    int64_t j = sink;
+                    while (true) {
+                        const int64_t r = sl.path[j];
+                        sl.row4col[j] = r;
+                        const int64_t prev = sl.col4row[r];
+                        sl.col4row[r] = j;
+                        j = prev;
+                        if (r == cur) break;
+                    }
+                }
+            }
+            __syncthreads();                                  // s_* and the slice are read before the next row
+        }
+        __syncthreads();
+        for (int64_t k = warp; k < K; k += kAssignWarps) {
+            const int64_t col = sl.col4row[k];
+            const double *lrow = llr + (s0 + k) * E;
+            const bool named = col >= 0 && col < E;
+            double m = -INFINITY;
+            if (named) {
+                m = lrow[col];
+            } else {
+                for (int64_t j = lane; j < E; j += 32) m = fmax(m, lrow[j]);
+                for (int o = 16; o; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+            }
+            if (lane == 0) {
+                assign_out[s0 + k] = named ? (int32_t)col : -1;
+                best_out[s0 + k] = m;
+            }
+        }
+        __syncthreads();                                      // the next recording rewrites the slice
+    }
+}
+
+}  // namespace
+
+size_t enroll_workspace_bytes(int64_t M, int64_t E, int64_t max_k, int sms) {
+    size_t total = 0;
+    enroll_layout(nullptr, M, E, max_k, sms, &total);
+    return total;
+}
+
+int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
+                  const int64_t *rec_off_host, int n_rec, const float *enroll_fea, int64_t N_e, const int32_t *enroll_spk,
+                  int64_t E, double c, double threshold, void *workspace, int sms, int32_t *assign_out,
+                  double *best_llr_out, double *llr_out, double *n_out, double *F_out, double *n_enroll_out,
+                  double *F_enroll_out, cudaStream_t st) {
+    std::vector<int64_t> busy(1, 0);                  // speaker offsets of the recordings that have speakers
+    int64_t max_k = 0;
+    for (int b = 0; b < n_rec; ++b) {
+        const int64_t k = rec_off_host[b + 1] - rec_off_host[b];
+        if (k > 0) busy.push_back(rec_off_host[b + 1]);
+        max_k = std::max(max_k, k);
+    }
+    const EnrollWs w = enroll_layout(reinterpret_cast<uint8_t *>(workspace), M, E, max_k, sms, nullptr);
+    const int64_t n_busy = (int64_t)busy.size() - 1;
+    int launches = 0;
+    if (n_busy > 0 &&   // pageable source: staged before the call returns, no wait on the stream
+        cudaMemcpyAsync(w.recs, busy.data(), busy.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return -1;
+    const int la = launch_speaker_stats(fea, Phi, spk, N, R, M, c, w.a, n_out, F_out, st);
+    const int le = launch_speaker_stats(enroll_fea, Phi, enroll_spk, N_e, R, E, c, w.en, n_enroll_out, F_enroll_out, st);
+    if (la < 0 || le < 0) return -1;
+    launches += la + le;
+    if (M > 0) {
+        const int64_t n_tiles = ((M + 31) / 32) * ((E + 31) / 32);
+        enroll_score_kernel<<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(w.a, w.en, Phi, M, E, R, c,
+                                                                                             w.llr, llr_out);
+        ++launches;
+    }
+    if (n_busy > 0) {
+        enroll_assign_kernel<<<(unsigned)std::min<int64_t>(n_busy, w.ctas), kAssignThreads, 0, st>>>(
+            w.llr, w.recs, n_busy, E, threshold, w.slices, w.slice_bytes, max_k, assign_out, best_llr_out);
+        ++launches;
+    }
+    return cudaGetLastError() == cudaSuccess ? launches : -1;
+}
+
+}  // namespace vbx

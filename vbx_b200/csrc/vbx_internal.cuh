@@ -255,6 +255,23 @@ size_t link_workspace_bytes(int64_t M);
 int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
                 int64_t M, double c, void *workspace, double *n_out, double *F_out, double *dist_out, double *Z_out,
                 cudaStream_t st);
+// vbx_link's span and statistics kernels over M speakers into caller-owned DEVICE arrays (n, e [M], b [M, kMaxR]
+// float64; first, last [M] and offs [4] int64 scratch): n_s, F_s, b_s and e_s exactly as vbx_link computes them.
+// Returns the number of launches, -1 on a launch error.
+struct SpeakerStats {
+    double *n, *e, *b;
+    long long *first, *last;
+    int64_t *offs;
+};
+int launch_speaker_stats(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, int64_t M, double c,
+                         const SpeakerStats &s, double *n_out, double *F_out, cudaStream_t st);
+// enrolment against known speakers (vbx_enroll.cu)
+size_t enroll_workspace_bytes(int64_t M, int64_t E, int64_t max_k, int sms);
+int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
+                  const int64_t *rec_off_host, int n_rec, const float *enroll_fea, int64_t N_e, const int32_t *enroll_spk,
+                  int64_t E, double c, double threshold, void *workspace, int sms, int32_t *assign_out,
+                  double *best_llr_out, double *llr_out, double *n_out, double *F_out, double *n_enroll_out,
+                  double *F_enroll_out, cudaStream_t st);
 // wgmma projection (vbx_project_tc.cu)
 size_t tc_scratch_floats();
 int launch_project_wgmma(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,

@@ -252,4 +252,25 @@ int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t 
     return cudaGetLastError() == cudaSuccess ? launches : -1;
 }
 
+int launch_speaker_stats(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, int64_t M, double c,
+                         const SpeakerStats &s, double *n_out, double *F_out, cudaStream_t st) {
+    if (M == 0) return 0;
+    LinkWs w;
+    w.lk = nullptr;
+    w.n = s.n;
+    w.e = s.e;
+    w.b = s.b;
+    w.first = s.first;
+    w.last = s.last;
+    w.offs = s.offs;
+    int launches = 2;
+    link_init_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(w, M);
+    if (N > 0) {
+        link_span_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(w, spk, N, M);
+        ++launches;
+    }
+    link_stats_kernel<<<(unsigned)M, kStatsThreads, 0, st>>>(w, fea, Phi, spk, R, c, n_out, F_out);
+    return cudaGetLastError() == cudaSuccess ? launches : -1;
+}
+
 }  // namespace vbx

@@ -1,0 +1,175 @@
+"""Enrolment against known speakers (DESIGN.md section 5.16).
+
+Each recording's VB-HMM numbers its speakers 1..K.  Enrolment names them: every archive speaker (section 5.15's table)
+is scored against every enrolled speaker with section 5.15's same-speaker LLR, and each recording's speakers are
+assigned one-to-one to enrolled speakers, or to "unknown", by a minimum-cost assignment on the device (vbx_enroll).  A
+speaker takes an enrolled name only where its LLR reaches the threshold, two speakers of one recording never share a
+name, and the sum of LLR - threshold over the named speakers is the largest possible.
+"""
+import ctypes
+from collections import namedtuple
+
+import numpy as np
+
+from .link import speaker_table
+
+UNKNOWN = 'unknown-'       # prefix of the names of speakers that match no enrolled speaker (reserved)
+MAX_THRESHOLD = 1e15
+
+# table: link.SpeakerTable; assign [M] enrolled index or -1; best_llr [M] the LLR of the assigned pair, or for an unknown
+# speaker its largest LLR; n [M], F [M,R], n_enroll [E], F_enroll [E,R] float64 statistics; llr [M,E] or None
+EnrollResult = namedtuple('EnrollResult', 'table assign best_llr n F n_enroll F_enroll llr')
+
+
+def check_threshold(threshold):
+    """The enrolment threshold as a float; ValueError when it is missing, not finite or beyond +-1e15."""
+    if threshold is None:
+        raise ValueError('enrolment needs a threshold: the LLR is not calibrated, so there is no default')
+    t = float(threshold)
+    if not abs(t) <= MAX_THRESHOLD:
+        raise ValueError(f'enrolment threshold must lie in [-{MAX_THRESHOLD:g}, {MAX_THRESHOLD:g}], got {threshold!r}')
+    return t
+
+
+def check_enrolment(enroll, dim):
+    """enroll = {name: x [n, dim]} checked: a name is non-empty, has no whitespace and does not start with 'unknown-';
+    every speaker has at least one x-vector of dimension dim.  Returns [(name, float64 array)] in dict order."""
+    if not isinstance(enroll, dict) or not enroll:
+        raise ValueError('enroll must be a non-empty {name: x-vectors} dict')
+    out = []
+    for name, x in enroll.items():
+        if not isinstance(name, str) or not name or any(ch.isspace() for ch in name):
+            raise ValueError(f'enrolled speaker name {name!r}: must be a non-empty string without whitespace')
+        if name.startswith(UNKNOWN):
+            raise ValueError(f'enrolled speaker name {name!r}: the prefix {UNKNOWN!r} is reserved')
+        x = np.asarray(x, dtype=np.float64)
+        if x.ndim != 2 or x.shape[0] == 0:
+            raise ValueError(f'enrolled speaker {name!r}: needs at least one x-vector as an [n, {dim}] array')
+        if x.shape[1] != dim:
+            raise ValueError(f'enrolled speaker {name!r}: x-vectors of dimension {x.shape[1]}, the archive has {dim}')
+        out.append((name, x))
+    return out
+
+
+def enroll_speakers(fea, Phi, offsets, labels, enroll_fea, enroll_speaker, Fa, Fb, threshold, device=None, llr=False,
+                    max_bytes=2 ** 31):
+    """Statistics, LLRs and the per-recording assignment of every archive speaker against the enrolled speakers on the
+    device (vbx_enroll).  fea [N,R], Phi [R]: the features the VB-HMM ran with, packed by recording at offsets [B+1];
+    labels: each recording's final first labels.  enroll_fea [N_e,R]: the enrolled x-vectors through the same front
+    end; enroll_speaker [N_e]: their speaker in [0, E), every speaker with at least one x-vector.  Archives whose M x E
+    LLR block exceeds max_bytes are split into chunks of whole recordings, one vbx_enroll call each (the results are
+    the same bits).  Returns EnrollResult (numpy, speaker_table order), with llr [M,E] when llr=True."""
+    import torch
+    from . import _lib
+    from ._lib import VbxError
+    t = check_threshold(threshold)
+    offsets = np.asarray(offsets, dtype=np.int64)
+    espk = np.asarray(enroll_speaker, dtype=np.int64).reshape(-1)
+    if len(espk) == 0 or espk.min() < 0:
+        raise ValueError('enroll_speaker must hold at least one speaker index, all >= 0')
+    E = int(espk.max()) + 1
+    if np.bincount(espk, minlength=E).min() == 0:
+        raise ValueError('every enrolled speaker 0 .. E-1 needs at least one x-vector')
+    table = speaker_table(labels)
+    M, B = len(table.rec), len(labels)
+    if not torch.cuda.is_available():
+        raise VbxError('enroll_speakers(): no CUDA device - vbx_b200 has no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    fea = torch.as_tensor(fea).to(dev, torch.float32).contiguous()
+    Phi = torch.as_tensor(Phi).to(dev, torch.float32).contiguous()
+    efea = torch.as_tensor(enroll_fea).to(dev, torch.float32).contiguous()
+    N, R = int(fea.shape[0]), int(fea.shape[1])
+    if int(offsets[-1]) != N or len(offsets) != B + 1:
+        raise ValueError('offsets must hold one more entry than labels and end at the number of x-vectors')
+    if tuple(efea.shape) != (len(espk), R):
+        raise ValueError(f'enroll_fea must be [{len(espk)}, {R}], got {tuple(efea.shape)}')
+    first = np.searchsorted(table.rec, np.arange(B + 1)).astype(np.int64)     # each recording's first speaker
+    spk = np.full(N, -1, dtype=np.int64)
+    for b, l in enumerate(labels):
+        l = np.asarray(l, dtype=np.int64).reshape(-1)
+        if len(l) != offsets[b + 1] - offsets[b]:
+            raise ValueError(f'recording {b}: {len(l)} labels for {offsets[b + 1] - offsets[b]} x-vectors')
+        own = table.label[first[b]:first[b + 1]]
+        spk[offsets[b]:offsets[b + 1]] = np.where(l >= 0, first[b] + np.searchsorted(own, l), -1)
+    # chunks of whole recordings with at most max_bytes of LLRs (a recording alone may exceed it)
+    chunks, b0 = [], 0
+    for b in range(B):
+        if b > b0 and (first[b + 1] - first[b0]) * E * 8 > max_bytes:
+            chunks.append((b0, b))
+            b0 = b
+    chunks.append((b0, B))
+    k_max = int(np.diff(first).max()) if B else 0
+    m_max = max(int(first[b1] - first[a]) for a, b1 in chunks)
+    lib = _lib.load()
+    h = ctypes.c_void_p()
+    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
+        raise VbxError('vbx_create failed: no usable sm_90 device')
+    at = lambda x, off=0: ctypes.c_void_p(x.data_ptr() + off * x.element_size()) if x is not None else None
+    try:
+        need = ctypes.c_size_t()
+        if lib.vbx_enroll_workspace_bytes(h, m_max, E, k_max, ctypes.byref(need)) != 0:
+            raise VbxError(f'vbx_enroll_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
+        with torch.cuda.device(dev):
+            ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=dev)
+            espk_d = torch.from_numpy(espk.astype(np.int32)).to(dev)
+            assign = torch.empty(M, dtype=torch.int32, device=dev)
+            best = torch.empty(M, dtype=torch.float64, device=dev)
+            n = torch.empty(M, dtype=torch.float64, device=dev)
+            F = torch.empty((M, R), dtype=torch.float64, device=dev)
+            n_e = torch.empty(E, dtype=torch.float64, device=dev)
+            F_e = torch.empty((E, R), dtype=torch.float64, device=dev)
+            L = torch.empty((M, E), dtype=torch.float64, device=dev) if llr else None
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            keep = []
+            for ci, (a, z) in enumerate(chunks):
+                s0, x0, x1 = int(first[a]), int(offsets[a]), int(offsets[z])
+                sp = spk[x0:x1]
+                spk_d = torch.from_numpy(np.where(sp >= 0, sp - s0, -1).astype(np.int32)).to(dev)
+                rec_off = np.ascontiguousarray(first[a:z + 1] - s0, dtype=np.int64)
+                keep.append(spk_d)
+                rc = lib.vbx_enroll(h, at(fea, x0 * R), at(Phi), x1 - x0, R, at(spk_d), int(first[z]) - s0,
+                                    rec_off.ctypes.data_as(ctypes.c_void_p), z - a, at(efea), len(espk), at(espk_d), E,
+                                    float(Fa), float(Fb), t, at(ws), ws.numel(), at(assign, s0), at(best, s0),
+                                    at(L, s0 * E), at(n, s0), at(F, s0 * R), at(n_e) if ci == 0 else None,
+                                    at(F_e) if ci == 0 else None, stream)
+                if rc != 0:
+                    raise VbxError(f'vbx_enroll failed ({rc}): {lib.vbx_last_error(h).decode()}')
+            out = EnrollResult(table, assign.cpu().numpy().astype(np.int64), best.cpu().numpy(), n.cpu().numpy(),
+                               F.cpu().numpy(), n_e.cpu().numpy(), F_e.cpu().numpy(),
+                               L.cpu().numpy() if llr else None)
+    finally:
+        lib.vbx_destroy(h)
+    return out
+
+
+def enroll_names(table, assign, best_llr, enrolled_names, recording_names, labels2=None, link=None):
+    """The names of every recording's speakers (DESIGN.md section 5.16): per recording ({label: name}, {label: llr}).
+    A speaker assigned to enrolled speaker e is enrolled_names[e]; any other is unknown-<recording>-<label + 1>, or with
+    `link` (per recording {label: id}, link.link_cut over the unknown speakers) unknown-<id + 1>.  labels2: None, or per
+    recording None or its second labels; a label used only there has no model and is unknown (it has no llr entry)."""
+    names = [{} for _ in range(table.n_recordings)]
+    llrs = [{} for _ in range(table.n_recordings)]
+    unknown = (lambda b, l: f'{UNKNOWN}{recording_names[b]}-{l + 1}') if link is None else \
+        (lambda b, l: f'{UNKNOWN}{link[b][l] + 1}')
+    for b, l, a, v in zip(table.rec.tolist(), table.label.tolist(), np.asarray(assign).tolist(),
+                          np.asarray(best_llr).tolist()):
+        names[b][l] = enrolled_names[a] if a >= 0 else unknown(b, l)
+        llrs[b][l] = float(v)
+    for b, l2 in enumerate(labels2 or []):
+        if l2 is None:
+            continue
+        for l in np.unique(np.asarray(l2, dtype=np.int64)).tolist():
+            if l >= 0 and l not in names[b]:
+                names[b][l] = unknown(b, l)
+    return names, llrs
+
+
+def mask_named(labels, names):
+    """An int label array with the labels of enrolled (not unknown-) speakers set to -1 (None stays None)."""
+    if labels is None:
+        return None
+    l = np.asarray(labels, dtype=np.int64)
+    named = [k for k, v in names.items() if not v.startswith(UNKNOWN)]
+    return np.where(np.isin(l, named), -1, l)

@@ -219,6 +219,39 @@ def read_uem(path):
     return out
 
 
+def read_utt2spk(path):
+    """Kaldi utt2spk, one 'utterance speaker' line each -> {utterance: speaker} in file order.  Blank lines are skipped;
+    a line without exactly two fields, or an utterance listed twice, is a ValueError."""
+    out = {}
+    with open(path) as f:
+        for n, line in enumerate(f, 1):
+            p = line.split()
+            if not p:
+                continue
+            if len(p) != 2:
+                raise ValueError(f'{path}:{n}: expected "utterance speaker", got {line.strip()!r}')
+            if p[0] in out:
+                raise ValueError(f'{path}:{n}: utterance {p[0]!r} listed twice')
+            out[p[0]] = p[1]
+    return out
+
+
+def read_enrolment(ark, utt2spk):
+    """Enrolment x-vectors: a Kaldi x-vector ark and its utt2spk file -> {speaker: x [n, Dx] float64}, speakers in order
+    of first appearance in the ark.  ValueError: an ark key missing from utt2spk, or a speaker of utt2spk none of whose
+    utterances is in the ark (utterances of utt2spk missing from the ark are otherwise ignored)."""
+    spk = read_utt2spk(utt2spk)
+    out = {}
+    for key, vec in read_vec_flt_ark(ark):
+        if key not in spk:
+            raise ValueError(f'{ark}: x-vector {key!r} has no speaker in {utt2spk}')
+        out.setdefault(spk[key], []).append(np.asarray(vec, dtype=np.float64))
+    empty = sorted(set(spk.values()) - set(out))
+    if empty:
+        raise ValueError(f'{utt2spk}: speakers without x-vectors in {ark}: {empty}')
+    return {k: np.stack(v) for k, v in out.items()}
+
+
 def read_speaker_counts(path):
     """Two-column 'recording count' file -> {recording: int}.  Blank lines and lines starting with '#' are skipped."""
     out = {}

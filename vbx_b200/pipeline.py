@@ -224,16 +224,33 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None
 def _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold):
     """x-vector transform + PLDA projection and AHC (VBx/vbhmm.py:125-146) for the whole archive as one batch.  Returns
     (fea [N,R] float32, Phi [R], AHC labels per recording at `threshold`, calibrated thresholds [B], linkage matrices)."""
-    from .batch import VbxBatch
     from . import ahc as _ahc
+    Dx = int(np.asarray(recordings[names[0]][0]).shape[1])
+    chain = _resolve_chain(chain, transform, plda, lda_dim, Dx)
+    x_all = np.concatenate([np.asarray(recordings[n][0], dtype=np.float64) for n in names])
+    front, x, fea, Phi = _project(x_all, lens, transform, plda, lda_dim, chain, dev)
+    ahc_labels, th, Zs = _ahc.ahc_batch(front, x, threshold=threshold)      # VBx/vbhmm.py:131-146
+    front.close()
+    return fea, Phi, ahc_labels, th, Zs
+
+
+def _resolve_chain(chain, transform, plda, lda_dim, Dx):
+    """'auto' -> 'tcgen05' when the shapes allow the fused tensor-core front end, else 'float64'."""
+    if chain != 'auto':
+        return chain
+    tr, lda = np.asarray(plda[1]), np.asarray(transform[2])
+    return 'tcgen05' if (lda_dim == 128 and tr.shape[0] == 128 and lda.shape[1] == 128 and Dx % 32 == 0) else 'float64'
+
+
+def _project(x_all, lens, transform, plda, lda_dim, chain, dev):
+    """x-vector transform + PLDA projection (VBx/vbhmm.py:125-129, :153) of raw x-vectors x_all [N,Dx] packed as
+    recordings of lens on `chain` ('tcgen05' or 'float64').  Returns (the front-end VbxBatch, for AHC and to close; the
+    transformed x-vectors; fea [N,R] float32; Phi [R])."""
+    from .batch import VbxBatch
     f64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(dev)
     f32 = lambda a: f64(a).float().contiguous()
     mu, tr, psi = diagonalise_plda(*plda)
     mean1, mean2, lda = transform
-    Dx = int(np.asarray(recordings[names[0]][0]).shape[1])
-    if chain == 'auto':
-        chain = 'tcgen05' if (lda_dim == 128 and tr.shape[0] == 128 and lda.shape[1] == 128 and Dx % 32 == 0) else 'float64'
-    x_all = np.concatenate([np.asarray(recordings[n][0], dtype=np.float64) for n in names])
     front = VbxBatch(lens, 128 if chain == 'tcgen05' else 4, 1, device=dev, exact_stop=False)
     if chain == 'tcgen05':
         rho, x = front.prepare_xvectors(f32(x_all), f32(mean1), f32(lda), f32(mean2), f32(mu), f32(tr), f32(psi))
@@ -243,9 +260,7 @@ def _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, th
         x = xvector_transform(f64(x_all), f64(mean1), f64(mean2), f64(lda)).contiguous()
         fea = plda_project(x, f64(mu), f64(tr), lda_dim).float().contiguous()
         Phi = f64(psi[:lda_dim]).float().contiguous()
-    ahc_labels, th, Zs = _ahc.ahc_batch(front, x, threshold=threshold)      # VBx/vbhmm.py:131-146
-    front.close()
-    return fea, Phi, ahc_labels, th, Zs
+    return front, x, fea, Phi
 
 
 def _pad_features(fea, Phi):
@@ -336,7 +351,8 @@ def _count_fields(item, k1, rule, lo, hi):
 
 def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
                   max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False, overlaps=None,
-                  num_speakers=None, min_speakers=None, max_speakers=None, link_threshold=None):
+                  num_speakers=None, min_speakers=None, max_speakers=None, link_threshold=None, enroll=None,
+                  enroll_threshold=None):
     """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
     recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
     one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
@@ -362,8 +378,15 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     device (link.link_speakers), and speakers whose average LLR is at least the threshold share an archive-wide id.
     Each item then also has global_speakers ({label: global id}, link.link_cut) and rttm_linked (its rttm lines, or
     rttm_overlap's with overlaps, with the speaker field set to global id + 1).
+    enroll: None, or known speakers {name: raw x-vectors [n, Dx]} to name the archive's speakers by (DESIGN.md section
+    5.16, after the count rules); needs enroll_threshold, an LLR threshold (there is no default).  The x-vectors go
+    through the archive's front end; each recording's speakers are assigned one-to-one to enrolled speakers where their
+    LLR reaches the threshold (enroll.enroll_speakers), the others are unknown-<recording>-<label + 1>, or with
+    link_threshold linked among themselves across the archive and named unknown-<id + 1>.  Each item then also has
+    speaker_names ({label: name}), speaker_llr ({label: the LLR that decided the name}) and rttm_named (its rttm lines,
+    or rttm_overlap's with overlaps, with the speaker field set to the name).
     Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds]
-    [, count_rule, n_speakers_vb, count][, global_speakers, rttm_linked])}."""
+    [, count_rule, n_speakers_vb, count][, global_speakers, rttm_linked][, speaker_names, speaker_llr, rttm_named])}."""
     if init not in ('AHC', 'AHC+VB'):
         raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
     if overlaps is not None and init == 'AHC':
@@ -372,6 +395,14 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     if link_threshold is not None:
         from .link import check_threshold
         check_threshold(link_threshold)
+    enrolled = None
+    if enroll is not None or enroll_threshold is not None:
+        from . import enroll as _enroll
+        if enroll is None:
+            raise ValueError('enroll_threshold without enroll')
+        _enroll.check_threshold(enroll_threshold)
+        dims = {int(np.asarray(r[0]).shape[1]) for r in recordings.values()}
+        enrolled = _enroll.check_enrolment(enroll, dims.pop() if len(dims) == 1 else -1)
     if not torch.cuda.is_available():
         from ._lib import VbxError
         raise VbxError('diarize_batch(): no CUDA device - vbx_b200 has no CPU fallback')
@@ -421,6 +452,9 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
         from . import link as _link
         table, _, _, Z = _link.link_speakers(fea, Phi, offs, labels1, Fa, Fb, dev)
         maps = _link.link_cut(Z, table, link_threshold, labels2)
+    if enrolled is not None:
+        spk_names, spk_llr = _enroll_archive(enrolled, enroll_threshold, link_threshold, recordings, names, transform,
+                                             plda, lda_dim, chain, dev, fea, Phi, offs, labels1, labels2, Fa, Fb)
     for b, n in enumerate(names):
         ovl = None
         if overlaps is not None:
@@ -432,7 +466,55 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
         if maps is not None:
             out[n].update(global_speakers=maps[b],
                           rttm_linked=linked_lines(n, recordings[n][1], labels1[b], labels2[b], maps[b], ovl))
+        if enrolled is not None:
+            out[n].update(speaker_names=spk_names[b], speaker_llr=spk_llr[b],
+                          rttm_named=named_lines(n, recordings[n][1], labels1[b], labels2[b], spk_names[b], ovl))
     return out
+
+
+def _enroll_archive(enrolled, threshold, link_threshold, recordings, names, transform, plda, lda_dim, chain, dev, fea,
+                    Phi, offs, labels1, labels2, Fa, Fb):
+    """DESIGN.md section 5.16 for diarize_batch: the enrolled x-vectors through the archive's front end (same chain,
+    padded as the archive's features), the device assignment, and the names (unknown speakers linked among themselves
+    with link_threshold).  Returns per recording ({label: name}, {label: llr})."""
+    from . import enroll as _enroll
+    from . import link as _link
+    Dx = int(np.asarray(recordings[names[0]][0]).shape[1])
+    chain = _resolve_chain(chain, transform, plda, lda_dim, Dx)
+    x_e = np.concatenate([x for _, x in enrolled])
+    front, _, fea_e, _ = _project(x_e, [len(x_e)], transform, plda, lda_dim, chain, dev)
+    front.close()
+    if fea_e.shape[1] < fea.shape[1]:
+        fea_e, _ = _pad_features(fea_e, Phi[:fea_e.shape[1]])
+    spk_e = np.repeat(np.arange(len(enrolled)), [len(x) for _, x in enrolled])
+    res = _enroll.enroll_speakers(fea, Phi, offs, labels1, fea_e, spk_e, Fa, Fb, threshold, dev)
+    enrolled_names = [k for k, _ in enrolled]
+    spk_names, spk_llr = _enroll.enroll_names(res.table, res.assign, res.best_llr, enrolled_names, names, labels2)
+    if link_threshold is not None:
+        l1 = [_enroll.mask_named(l, m) for l, m in zip(labels1, spk_names)]
+        l2 = [_enroll.mask_named(l, m) for l, m in zip(labels2, spk_names)]
+        table, _, _, Z = _link.link_speakers(fea, Phi, offs, l1, Fa, Fb, dev)
+        lk = _link.link_cut(Z, table, link_threshold, l2)
+        spk_names, spk_llr = _enroll.enroll_names(res.table, res.assign, res.best_llr, enrolled_names, names, labels2,
+                                                  link=lk)
+    return spk_names, spk_llr
+
+
+def rttm_name_lines(recording, starts, ends, names):
+    """rttm_lines with a string speaker field: names[i] is segment i's speaker."""
+    return [f'SPEAKER {recording} 1 {s:03f} {e - s:03f} <NA> <NA> {k} <NA> <NA>' for s, e, k in zip(starts, ends, names)]
+
+
+def named_lines(name, seg_times, labels, labels2, names, overlap=None):
+    """RTTM lines of one recording with named speakers (DESIGN.md section 5.16): the segments _result writes (the
+    overlap-aware ones when overlap regions (lo, hi) ticks are given, else the merged first labels) with every label's
+    speaker field set to names[label].  labels2 is used inside the overlap regions only."""
+    seg = np.asarray(seg_times, dtype=np.float64)
+    if overlap is not None:
+        s, e, l = overlap_segments(seg, labels, labels2, overlap)
+    else:
+        s, e, l = merge_adjacent_labels(seg[:, 0], seg[:, 1], labels)
+    return rttm_name_lines(name, s, e, [names[int(k)] for k in l])
 
 
 def linked_lines(name, seg_times, labels, labels2, mapping, overlap=None):

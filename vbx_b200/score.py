@@ -543,7 +543,7 @@ def system_stretches(rows, recording=''):
 
 
 def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=None, overlapping=False, jer=False,
-               across_files=False):
+               across_files=False, by_name=False):
     """DER of system RTTM rows against reference RTTM rows (both as formats.read_rttm returns them).
     uem: None or {recording: [(onset, offset)]} (formats.read_uem).  overlapping: the system may have two speakers at
     once (system_stretches, scored by vbx_score_overlap); otherwise overlapping system turns raise ValueError.  Returns
@@ -553,7 +553,10 @@ def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=N
     (jer_finish()['ticks']).
     across_files: speakers are one speaker in every file where they have the same RTTM name, in the reference and in
     the system (DESIGN.md section 5.15); the overall dict gains across_files, a result dict with the overall miss and fa
-    and conf = sum of covered - max one-to-one matching of the overlaps summed over all files by name."""
+    and conf = sum of covered - max one-to-one matching of the overlaps summed over all files by name.
+    by_name: a system speaker is right only where its RTTM name is the reference speaker's (DESIGN.md section 5.16): the
+    overall dict gains by_name, a result dict with the overall miss and fa and conf = sum of covered - the overlaps of
+    equal names summed over all files (so by_name conf >= across_files conf)."""
     c = collar_ticks(collar)
     # JER is taken without a collar and with overlaps: from the DER's own launch when that is the protocol, else from
     # one more region set
@@ -579,13 +582,17 @@ def score_rttm(ref_turns, sys_turns, collar, ignore_overlaps, uem=None, device=N
         lo, hi, lab = system_turns(sys_by.get(n, []), n)
         recs.append(prepare_recording(n, ref[n], (lo, hi, hi), u, proto))
         entries.append((b, lab))
-    res = score_entries(recs, entries, device, jer=jer_proto, blocks=across_files)
+    res = score_entries(recs, entries, device, jer=jer_proto, blocks=across_files or by_name)
     per = {n: r['score'] for n, r in zip(names, res)}
     tot = overall(list(per.values()))
-    if across_files:
+    if across_files or by_name:
         sys_names = {n: sorted(set(r[3] for r in sys_by.get(n, []))) for n in names}
-        tot['across_files'] = across_files_result(tot, [[k for k, _ in named[n]] for n in names],
-                                                  [sys_names[n] for n in names], [r['O']['score'] for r in res])
+        args = (tot, [[k for k, _ in named[n]] for n in names], [sys_names[n] for n in names],
+                [r['O']['score'] for r in res])
+        if across_files:
+            tot['across_files'] = across_files_result(*args)
+        if by_name:
+            tot['by_name'] = by_name_result(*args)
     if jer:
         for n, r in zip(names, res):
             per[n] = dict(per[n], jer=r['jer']['jer'], jer_ticks=r['jer']['ticks'])
@@ -599,6 +606,28 @@ def across_files_result(tot, ref_names, sys_names, blocks):
     block: the blocks are summed by name and matched once.  A block has a column for every label up to the last one with
     a non-empty turn, so names past it (speakers whose turns are all empty) and a file without system names add nothing."""
     from scipy.optimize import linear_sum_assignment
+    _, _, O = _blocks_by_name(ref_names, sys_names, blocks)
+    matched = 0
+    if O.size:
+        r, c = linear_sum_assignment(O, maximize=True)
+        matched = int(O[r, c].sum())
+    t = tot['ticks']
+    covered = t['scored'] - t['miss']
+    return result(t['miss'], t['fa'], covered - matched, t['scored'])
+
+
+def by_name_result(tot, ref_names, sys_names, blocks):
+    """Name-level DER (DESIGN.md section 5.16), arguments as across_files_result: the overlap blocks summed by name,
+    and only the cells whose reference and system names are equal count as matched."""
+    rows, cols, O = _blocks_by_name(ref_names, sys_names, blocks)
+    matched = sum(int(O[i, cols[k]]) for k, i in rows.items() if k in cols)
+    t = tot['ticks']
+    covered = t['scored'] - t['miss']
+    return result(t['miss'], t['fa'], covered - matched, t['scored'])
+
+
+def _blocks_by_name(ref_names, sys_names, blocks):
+    """The per-file overlap blocks summed by name: ({ref name: row}, {system name: column}, O [rows, columns])."""
     rows = {k: i for i, k in enumerate(sorted({k for ks in ref_names for k in ks}))}
     cols = {k: i for i, k in enumerate(sorted({k for ks in sys_names for k in ks}))}
     O = np.zeros((len(rows), len(cols)), dtype=np.int64)
@@ -607,13 +636,7 @@ def across_files_result(tot, ref_names, sys_names, blocks):
         w = min(blk.shape[1], len(sk))
         if rk and w:
             np.add.at(O, np.ix_([rows[k] for k in rk], [cols[k] for k in sk[:w]]), blk[:, :w])
-    matched = 0
-    if O.size:
-        r, c = linear_sum_assignment(O, maximize=True)
-        matched = int(O[r, c].sum())
-    t = tot['ticks']
-    covered = t['scored'] - t['miss']
-    return result(t['miss'], t['fa'], covered - matched, t['scored'])
+    return rows, cols, O
 
 
 def read_rttm_path(path):
@@ -644,6 +667,8 @@ def build_parser():
                     help='also the Jaccard error rate (no collar, overlaps scored, whatever the DER options)')
     ap.add_argument('--across-files', action='store_true',
                     help='also the DER with each speaker name one speaker in every file (ACROSS FILES row)')
+    ap.add_argument('--by-name', action='store_true',
+                    help='also the DER with system speakers right only under the reference name (BY NAME row)')
     return ap
 
 
@@ -653,19 +678,20 @@ def main(argv=None):
     uem = formats.read_uem(args.uem) if args.uem else None
     per, tot = score_rttm(read_rttm_path(args.ref_rttm), read_rttm_path(args.sys_rttm), args.collar,
                           args.ignore_overlaps, uem, overlapping=args.overlapping_system, jer=args.jer,
-                          across_files=args.across_files)
+                          across_files=args.across_files, by_name=args.by_name)
     if args.json:
         print(json.dumps(dict(collar=args.collar, ignore_overlaps=args.ignore_overlaps, files=per, overall=tot),
                          sort_keys=True))
         return 0
-    rows = list(per.items()) + [('OVERALL', tot)] + ([('ACROSS FILES', tot['across_files'])] if args.across_files else [])
+    rows = list(per.items()) + [('OVERALL', tot)] + ([('ACROSS FILES', tot['across_files'])] if args.across_files else []) \
+        + ([('BY NAME', tot['by_name'])] if args.by_name else [])
     w = max(len(n) for n, _ in rows)
     jer_head = f'  {"JER %":>7}' if args.jer else ''
     print(f'{"file":<{w}}  {"DER %":>7}  {"miss %":>7}  {"FA %":>7}  {"conf %":>7}  {"scored s":>10}{jer_head}')
     for n, r in rows:
         pct = [100.0 * r[k] / r['scored'] if r['scored'] else float('nan') for k in ('miss', 'fa', 'conf')]
         der = 100.0 * r['der'] if r['der'] is not None else float('nan')
-        jer = r.get('jer') if n != 'ACROSS FILES' else None
+        jer = r.get('jer') if n not in ('ACROSS FILES', 'BY NAME') else None
         jer_col = (f'  {100.0 * jer if jer is not None else float("nan"):7.2f}') if args.jer else ''
         print(f'{n:<{w}}  {der:7.2f}  {pct[0]:7.2f}  {pct[1]:7.2f}  {pct[2]:7.2f}  {r["scored"]:10.2f}{jer_col}')
     return 0
