@@ -61,22 +61,15 @@ def sequential(recs, transform, plda, grid, dev):
     lens = np.array([recs[n][0].shape[0] for n in names], dtype=np.int64)
     (fea, Phi, _, th, Zs), t_front = timed(lambda: pipeline._front_end(recs, names, lens, transform, plda, 128, 'auto', dev, 0.0))
     fea, Phi = pipeline._pad_features(fea, Phi)
-    offs = np.concatenate([[0], np.cumsum(lens)])
 
     def vb_all():
         from vbx_b200 import ahc
+        from vbx_b200.batch import VbxBatch
         for s in sweep.grid_settings(grid):
             labels = ahc.cut(Zs, th, lens, s.threshold)
-            ns = np.array([int(l.max()) + 1 for l in labels], dtype=np.int32)
             lab_d = torch.from_numpy(np.concatenate(labels)).to(dev)
-            for tier, sel in enumerate((ns <= 64, (ns > 64) & (ns <= 128), ns > 128)):
-                idx = np.nonzero(sel)[0]
-                if len(idx) == 0:
-                    continue
-                rows = torch.from_numpy(np.concatenate([np.arange(offs[b], offs[b + 1]) for b in idx])).to(dev)
-                pipeline._vb_tier(lens[idx], ns[idx], fea.index_select(0, rows).contiguous(), Phi,
-                                  lab_d.index_select(0, rows), tier == 2, s.smoothing, dev,
-                                  Fa=s.Fa, Fb=s.Fb, loopProb=s.loopP, maxIters=40, epsilon=1e-6)
+            pipeline._vb_stage([(s.Fa, s.Fb, s.loopP, s.smoothing)], [labels], [lab_d], Zs, lens, fea, Phi, None,
+                               'AHC+VB', dev, VbxBatch, None, maxIters=40, epsilon=1e-6)
     _, t_vb = timed(vb_all)
     return t_front, t_vb
 

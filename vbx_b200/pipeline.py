@@ -221,6 +221,99 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None
     return out
 
 
+def _tier(n_states):
+    """The state tier of a run whose AHC gave n_states clusters: 0 (<= 64 states, planned exactly as in an archive
+    without the larger recordings) and 1 (65 .. MAX_STATES_F32, S = 128) on the float32 kernels, 2 (more) on the float64
+    kernels.  VBx over-clusters in AHC and lets VB prune, so the state count varies by recording; each tier is batched on
+    its own because padding every recording to the largest tier would multiply its bytes."""
+    return 0 if n_states <= 64 else 1 if n_states <= MAX_STATES_F32 else 2
+
+
+def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, make, split, **run_kw):
+    """Everything after AHC (VBx/vbhmm.py:147-162 and the speaker-count rules of DESIGN.md section 5.14) for the entries
+    (k, b): setting k of `hyper`, a list of (Fa, Fb, loopP, smoothing), on recording b.  labels[k]: setting k's AHC
+    labels per recording; labels_d[k]: their concatenation on the device (used by init='AHC+VB' only).  fea [N,R] float32
+    and Phi [R] as _pad_features leaves them; Zs: the AHC linkages; bounds: None or count_bounds' (lo, hi).
+    init='AHC' returns the AHC labels (rule 4 under bounds, per setting).  init='AHC+VB' runs the VB-HMM with the entries
+    grouped by state tier (_tier).  A float32 tier runs as batches of consecutive entries planned by `make` (VbxBatch or
+    parts.make_batch) and cut by `split` (None: one batch per tier; else split(entries, ns) -> the tier's entries, in
+    order, as consecutive batches, e.g. sweep.packer), with Fa, Fb and loopP as numbers when `hyper` holds one setting,
+    else as per-recording float64 tensors; the float64 tier runs once per setting.  Under
+    bounds the first pass applies rule 2 inside _vb_tier, and rule 3 re-runs every entry with too few speakers from its
+    recording's maxclust cut (one cut per recording, shared by all settings) through the same tiers.  run_kw go to run()
+    (maxIters, epsilon).  Returns {(k, b): (labels, labels2nd or None, iterations, flags[, n_speakers_vb, count_rule])},
+    the last two under bounds."""
+    from . import ahc as _ahc
+    B = len(lens)
+    entries = [(k, b) for k in range(len(hyper)) for b in range(B)]
+    if init == 'AHC':
+        out = {(k, b): (labels[k][b].astype(np.int64), None, 0, 0) for k, b in entries}
+        if bounds is not None:
+            for k in range(len(hyper)):
+                l1, k1, rules = _count_ahc(Zs, lens, [out[(k, b)][0] for b in range(B)], bounds)
+                out.update(((k, b), (l1[b], None, 0, 0, k1[b], rules[b])) for b in range(B))
+        return out
+    offs = np.concatenate([[0], np.cumsum(lens)])
+
+    def run_tiers(entries, ns, labels_d, hi):
+        """The entries, with ns[e] states and their labels in labels_d[k], through the state tiers: {e: _vb_tier tuple}."""
+        tiers = [[], [], []]
+        for e in entries:
+            tiers[_tier(ns[e])].append(e)
+        batches = [(g, False) for group in tiers[:2] for g in ([group] if split is None else split(group, ns))]
+        batches += [([e for e in tiers[2] if e[0] == k], True) for k in range(len(hyper))]   # no per-recording float64 path
+        out = {}
+        for group, f64 in batches:
+            if not group:
+                continue
+            recs = [b for _, b in group]
+            if recs == list(range(B)) and all(k == group[0][0] for k, _ in group):
+                g_fea, g_labels = fea, labels_d[group[0][0]]
+            else:
+                g_fea = torch.cat([fea[offs[b]:offs[b + 1]] for b in recs])
+                g_labels = torch.cat([labels_d[k][offs[b]:offs[b + 1]] for k, b in group])
+            if f64 or len(hyper) == 1:
+                Fa, Fb, loopP, smoothing = hyper[group[0][0]]
+            else:
+                Fa, Fb, loopP = (torch.tensor([hyper[k][i] for k, _ in group], dtype=torch.float64, device=dev)
+                                 for i in range(3))
+                smoothing = [hyper[k][3] for k, _ in group]
+            sub = _vb_tier(lens[recs], np.array([ns[e] for e in group], dtype=np.int32), g_fea, Phi, g_labels, f64,
+                           smoothing, dev, make=make, hi=None if hi is None else hi[recs],
+                           Fa=Fa, Fb=Fb, loopProb=loopP, **run_kw)
+            out.update(zip(group, sub))
+        return out
+
+    ns = {(k, b): int(labels[k][b].max()) + 1 if lens[b] else 1 for k, b in entries}
+    out = run_tiers(entries, ns, labels_d, None if bounds is None else bounds[1])
+    if bounds is None:
+        return out
+    lo = bounds[0]
+    low = [e for e in entries if out[e][4] < lo[e[1]]]
+    recs = sorted({b for _, b in low})
+    mc = dict(zip(recs, _ahc.cut_count([Zs[b] for b in recs], lens[recs], lo[recs])))
+    met = [e for e in low if lens[e[1]] >= lo[e[1]]]
+    again = {}
+    if met:
+        mc_all = np.zeros(int(offs[-1]), dtype=np.int64)
+        for b in recs:
+            mc_all[offs[b]:offs[b + 1]] = mc[b]
+        again = run_tiers(met, {e: int(mc[e[1]].max()) + 1 for e in met},
+                          [torch.from_numpy(mc_all).to(dev)] * len(hyper), None)
+    for e in low:
+        *r, rule = _recut_outcome(lens[e[1]], lo[e[1]], mc[e[1]], again.get(e))
+        out[e] = tuple(r) + (out[e][4], rule)
+    return out
+
+
+def _check_init(init, overlaps):
+    """init is 'AHC' or 'AHC+VB', and overlap-aware output (overlaps true) has the VB-HMM's second labels."""
+    if init not in ('AHC', 'AHC+VB'):
+        raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
+    if overlaps and init == 'AHC':
+        raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
+
+
 def _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold):
     """x-vector transform + PLDA projection and AHC (VBx/vbhmm.py:125-146) for the whole archive as one batch.  Returns
     (fea [N,R] float32, Phi [R], AHC labels per recording at `threshold`, calibrated thresholds [B], linkage matrices)."""
@@ -387,10 +480,7 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     or rttm_overlap's with overlaps, with the speaker field set to the name).
     Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds]
     [, count_rule, n_speakers_vb, count][, global_speakers, rttm_linked][, speaker_names, speaker_llr, rttm_named])}."""
-    if init not in ('AHC', 'AHC+VB'):
-        raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
-    if overlaps is not None and init == 'AHC':
-        raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
+    _check_init(init, overlaps is not None)
     bounds = count_bounds(list(recordings), num_speakers, min_speakers, max_speakers)
     if link_threshold is not None:
         from .link import check_threshold
@@ -413,40 +503,16 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
         return {}
     fea, Phi, ahc_labels, _, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold)
     offs = np.concatenate([[0], np.cumsum(lens)])
-    out = {}
-    labels1 = [l.astype(np.int64) for l in ahc_labels]
-    labels2 = [None] * len(names)
-    iters = [0] * len(names)
-    k1 = rules = None
-    if bounds is not None and not init.endswith('VB'):
-        labels1, k1, rules = _count_ahc(Zs, lens, labels1, bounds)
-    elif bounds is not None:
-        k1, rules = [0] * len(names), [None] * len(names)
-    if init.endswith('VB'):
-        ns = np.array([int(l.max()) + 1 if len(l) else 1 for l in ahc_labels], dtype=np.int32)
+    labels_d = None
+    if init == 'AHC+VB':
         fea, Phi = _pad_features(fea, Phi)
-        lab_d = torch.from_numpy(np.concatenate(ahc_labels)).to(dev)
-        # VBx over-clusters in AHC and lets VB prune, so the state count varies by recording.  Each state tier is one
-        # batch: <= 64 states (planned exactly as in an archive without the larger recordings), 65 .. 128 (S = 128),
-        # more than 128 on the float64 kernels.  Padding every recording to the largest tier would multiply its bytes.
-        tiers = (ns <= 64, (ns > 64) & (ns <= MAX_STATES_F32), ns > MAX_STATES_F32)
-        for tier, sel in enumerate(tiers):
-            idx = np.nonzero(sel)[0]
-            if len(idx) == 0:
-                continue
-            rows = None if len(idx) == len(names) else \
-                torch.from_numpy(np.concatenate([np.arange(offs[b], offs[b + 1]) for b in idx])).to(dev)
-            pick = (lambda t: t) if rows is None else (lambda t: t.index_select(0, rows).contiguous())
-            sub = _vb_tier(lens[idx], ns[idx], pick(fea), Phi, pick(lab_d), tier == 2, smoothing, dev,
-                           hi=None if bounds is None else bounds[1][idx],
-                           Fa=Fa, Fb=Fb, loopProb=loopP, maxIters=max_iters, epsilon=epsilon)
-            for j, b in enumerate(idx):
-                labels1[b], labels2[b], iters[b] = sub[j][:3]
-                if bounds is not None:
-                    k1[b], rules[b] = sub[j][4:6]
-        if bounds is not None:
-            _count_rerun(bounds, Zs, lens, offs, fea, Phi, dev, k1, rules, labels1, labels2, iters, smoothing,
-                         Fa=Fa, Fb=Fb, loopProb=loopP, maxIters=max_iters, epsilon=epsilon)
+        labels_d = [torch.from_numpy(np.concatenate(ahc_labels)).to(dev)]
+    from .batch import VbxBatch
+    res = _vb_stage([(Fa, Fb, loopP, smoothing)], [ahc_labels], labels_d, Zs, lens, fea, Phi, bounds, init, dev,
+                    VbxBatch, None, maxIters=max_iters, epsilon=epsilon)
+    res = [res[(0, b)] for b in range(len(names))]
+    labels1, labels2 = [r[0] for r in res], [r[1] for r in res]
+    out = {}
     maps = None
     if link_threshold is not None:
         from . import link as _link
@@ -460,9 +526,9 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
         if overlaps is not None:
             from .score import overlap_ticks
             ovl = overlap_ticks(overlaps.get(n))
-        out[n] = _result(n, recordings[n][1], labels1[b], labels2[b], iters[b], output_2nd, ovl)
+        out[n] = _result(n, recordings[n][1], labels1[b], labels2[b], res[b][2], output_2nd, ovl)
         if bounds is not None:
-            _count_fields(out[n], k1[b], rules[b], bounds[0][b], bounds[1][b])
+            _count_fields(out[n], *res[b][4:6], bounds[0][b], bounds[1][b])
         if maps is not None:
             out[n].update(global_speakers=maps[b],
                           rttm_linked=linked_lines(n, recordings[n][1], labels1[b], labels2[b], maps[b], ovl))
@@ -527,31 +593,6 @@ def linked_lines(name, seg_times, labels, labels2, mapping, overlap=None):
     if overlap is not None:
         return rttm_lines(name, *overlap_segments(seg, relabel(labels, mapping), relabel(labels2, mapping), overlap))
     return rttm_lines(name, *merge_adjacent_labels(seg[:, 0], seg[:, 1], relabel(labels, mapping)))
-
-
-def _count_rerun(bounds, Zs, lens, offs, fea, Phi, dev, k1, rules, labels1, labels2, iters, smoothing, **run_kw):
-    """Rule 3 of DESIGN.md section 5.14 for diarize_batch: every recording with fewer than lo speakers re-runs the
-    VB-HMM from its linkage cut at lo clusters, all of them in one batch per state tier.  Updates the lists in place."""
-    from . import ahc as _ahc
-    lo = bounds[0]
-    low = [b for b in range(len(lens)) if k1[b] < lo[b]]
-    if not low:
-        return
-    mc = dict(zip(low, _ahc.cut_count([Zs[b] for b in low], lens[low], lo[low])))
-    runs = {}
-    met = [b for b in low if lens[b] >= lo[b]]
-    ns = {b: int(mc[b].max()) + 1 for b in met}
-    for tier, pred in enumerate((lambda n: n <= 64, lambda n: 64 < n <= MAX_STATES_F32, lambda n: n > MAX_STATES_F32)):
-        idx = [b for b in met if pred(ns[b])]
-        if not idx:
-            continue
-        rows = torch.from_numpy(np.concatenate([np.arange(offs[b], offs[b + 1]) for b in idx])).to(dev)
-        labs = torch.from_numpy(np.concatenate([mc[b] for b in idx])).to(dev)
-        sub = _vb_tier(lens[idx], np.array([ns[b] for b in idx], dtype=np.int32), fea.index_select(0, rows).contiguous(),
-                       Phi, labs, tier == 2, smoothing, dev, **run_kw)
-        runs.update(zip(idx, sub))
-    for b in low:
-        labels1[b], labels2[b], iters[b], _, rules[b] = _recut_outcome(lens[b], lo[b], mc[b], runs.get(b))
 
 
 def _result(name, seg_times, labels, labels2, iterations, output_2nd, overlap=None):

@@ -3,7 +3,8 @@
 Every VBx recipe tunes Fa, Fb, loopP, the AHC threshold and the init smoothing per dataset, by grid search on a dev set.
 Here the front end and the AHC linkage run once per archive; each threshold only repeats the host cut of the stored
 linkage (ahc.cut).  Every (recording, setting) pair is one entry of a batch with per-recording Fa, Fb and loopP
-(vbx_run_per_recording), so a grid is a handful of large batches instead of one small batch per setting.
+(vbx_run_per_recording; a one-setting grid passes numbers to vbx_run, with bit-identical results), so a grid is a
+handful of large batches instead of one small batch per setting.
 
     python -m vbx_b200.sweep --out-dir sweep --xvec-ark-file exp/ES2005a.ark --segments-file exp/ES2005a.seg \\
         --xvec-transform transform.h5 --plda-file plda --lda-dim 128 \\
@@ -104,13 +105,31 @@ def entry_bytes(T, n_states, R, device):
     of the split and the fused-sweep plans of the recording alone, which bounds what it adds to any batch), plus its
     replicated rho rows and gamma rows."""
     from .batch import VbxBatch
+    from .pipeline import _tier
     ws = 0
-    for fb_split in (1, 2) if n_states <= 64 else (1,):
+    for fb_split in (1, 2) if _tier(n_states) == 0 else (1,):
         vb = VbxBatch([T], R, n_states, device=device, allocate=False, fb_split=fb_split)
         ws = max(ws, vb.workspace_bytes)
         S = vb.S
         vb.close()
     return ws + 4 * T * (R + S)
+
+
+def packer(lens, R, device, budget):
+    """The split of pipeline._vb_stage for a sweep: split(entries, ns) packs a float32 tier's (setting, recording)
+    entries with ns[e] states, in order, into consecutive batches of at most `budget` bytes (pack, entry_bytes)."""
+    from ._lib import padded_states
+    size_cache = {}
+
+    def split(entries, ns):
+        sizes = []
+        for k, b in entries:
+            key = (int(lens[b]), padded_states(ns[(k, b)]))      # the size depends on T and the padded S only
+            if key not in size_cache:
+                size_cache[key] = entry_bytes(key[0], key[1], R, device)
+            sizes.append(size_cache[key])
+        return [[entries[i] for i in idx] for idx in pack(sizes, budget)]
+    return split
 
 
 def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
@@ -120,8 +139,9 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
 
     recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
     Entries (recording, setting) are grouped into diarize_batch's state tiers (<= 64, 65 .. 128 AHC clusters: float32
-    batches with per-recording Fa / Fb / loopP, packed into as few batches as fit max_batch_bytes, default half of the
-    free device memory; more than 128: one float64 run per setting).
+    batches with per-recording Fa / Fb / loopP, numbers when the grid has one setting, packed into as few batches as fit
+    max_batch_bytes, default half of the free device memory; more than 128: one float64 run per setting), all in
+    pipeline._vb_stage.
     ref_rttm: None, or the reference as an RTTM path (file or directory of *.rttm) or formats.read_rttm rows; uem: None,
     a UEM path or formats.read_uem's dict.  With a reference every (setting, recording) entry is scored after all batches
     have run, in one vbx_score launch per protocol (score.PROTOCOLS), and each recording's dict gains
@@ -143,22 +163,18 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     diarize_batch returns with that setting's scalars."""
     import torch
     from . import ahc as _ahc
-    from ._lib import VbxError, padded_states
+    from ._lib import VbxError
     from .parts import make_batch
-    from .pipeline import (MAX_STATES_F32, _count_ahc, _count_fields, _front_end, _pad_features, _recut_outcome, _result,
-                           _vb_tier, count_bounds)
+    from .pipeline import _check_init, _count_fields, _front_end, _pad_features, _result, _vb_stage, count_bounds
     settings = grid_settings(grid)
-    if init not in ('AHC', 'AHC+VB'):
-        raise ValueError('Wrong option for args.initialization.')
+    with_overlap = oracle_overlaps or overlaps is not None
+    _check_init(init, with_overlap)
     if oracle_overlaps and ref_rttm is None:
         raise ValueError('oracle_overlaps are the overlaps of the reference: they need ref_rttm')
     if oracle_overlaps and overlaps is not None:
         raise ValueError('give overlaps or oracle_overlaps, not both')
-    with_overlap = oracle_overlaps or overlaps is not None
     if jer and ref_rttm is None:
         raise ValueError('jer scores against the reference: it needs ref_rttm')
-    if with_overlap and init == 'AHC':
-        raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
     oracle_count = isinstance(num_speakers, str)
     if oracle_count and num_speakers != 'oracle':
         raise ValueError(f"num_speakers: expected an int, a dict or 'oracle', got {num_speakers!r}")
@@ -186,86 +202,15 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
     fea, Phi, _, th, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, 0.0)
     fea, Phi = _pad_features(fea, Phi)
-    R = int(fea.shape[1])
-    offs = np.concatenate([[0], np.cumsum(lens)])
     thresholds = list(dict.fromkeys(s.threshold for s in settings))
     ahc_labels = {t: _ahc.cut(Zs, th, lens, t) for t in thresholds}              # VBx/vbhmm.py:144-146, host only
     lab_d = {t: torch.from_numpy(np.concatenate(ahc_labels[t])).to(dev) for t in thresholds}
-    # per (setting, recording): labels, labels2nd, iterations, flags
-    res = {(k, b): (ahc_labels[s.threshold][b].astype(np.int64), None, 0, 0)
-           for k, s in enumerate(settings) for b in range(len(names))}
-    counted = {}           # with a speaker-count constraint, per (setting, recording): unconstrained count, rule
-    if bounds is not None and not init.endswith('VB'):
-        for k, s in enumerate(settings):
-            labels, k1, rules = _count_ahc(Zs, lens, [res[(k, b)][0] for b in range(len(names))], bounds)
-            for b in range(len(names)):
-                res[(k, b)] = (labels[b], None, 0, 0)
-                counted[(k, b)] = (k1[b], rules[b])
-    if init.endswith('VB'):
-        if max_batch_bytes is None:
-            max_batch_bytes = int(torch.cuda.mem_get_info(dev)[0] * BUDGET_FRACTION)
-        entries = [(k, b) for k in range(len(settings)) for b in range(len(names))]
-        ns = {(k, b): max(int(ahc_labels[settings[k].threshold][b].max()) + 1, 1) if lens[b] else 1 for k, b in entries}
-        size_cache = {}
-
-        def run(group, f64, ns, labels_of, hi, out, **hyper):
-            rows = torch.from_numpy(np.concatenate([np.arange(offs[b], offs[b + 1]) for _, b in group])).to(dev)
-            labs = torch.cat([labels_of(e) for e in group])
-            sub = _vb_tier(lens[[b for _, b in group]], np.array([ns[e] for e in group], dtype=np.int32),
-                           fea.index_select(0, rows).contiguous(), Phi, labs, f64,
-                           [settings[k].smoothing for k, _ in group], dev, make=make_batch,
-                           hi=None if hi is None else hi[[b for _, b in group]],
-                           maxIters=max_iters, epsilon=epsilon, **hyper)
-            for e, r in zip(group, sub):
-                out[e] = r
-
-        def run_tiers(entries, ns, labels_of, hi, out):
-            """The entries as diarize_batch's state tiers: float32 batches packed to max_batch_bytes with per-entry
-            Fa / Fb / loopP, the float64 tier one run per setting."""
-            tiers = ([e for e in entries if ns[e] <= 64], [e for e in entries if 64 < ns[e] <= MAX_STATES_F32],
-                     [e for e in entries if ns[e] > MAX_STATES_F32])
-            for tier, group_all in enumerate(tiers[:2]):
-                if not group_all:
-                    continue
-                sizes = []
-                for k, b in group_all:
-                    key = (int(lens[b]), padded_states(ns[(k, b)]))      # the size depends on T and the padded S only
-                    if key not in size_cache:
-                        size_cache[key] = entry_bytes(key[0], key[1], R, dev)
-                    sizes.append(size_cache[key])
-                for idx in pack(sizes, max_batch_bytes):
-                    group = [group_all[i] for i in idx]
-                    hp = [torch.tensor([getattr(settings[k], a) for k, _ in group], dtype=torch.float64, device=dev)
-                          for a in ('Fa', 'Fb', 'loopP')]
-                    run(group, False, ns, labels_of, hi, out, Fa=hp[0], Fb=hp[1], loopProb=hp[2])
-            for k, s in enumerate(settings):           # no per-recording float64 path: one run per setting
-                group = [e for e in tiers[2] if e[0] == k]
-                if group:
-                    run(group, True, ns, labels_of, hi, out, Fa=s.Fa, Fb=s.Fb, loopProb=s.loopP)
-
-        first = {}
-        run_tiers(entries, ns, lambda e: lab_d[settings[e[0]].threshold][offs[e[1]]:offs[e[1] + 1]],
-                  None if bounds is None else bounds[1], first)
-        for e, r in first.items():
-            res[e] = r[:4]
-            if bounds is not None:
-                counted[e] = r[4:6]
-        if bounds is not None:
-            # rule 3: entries with too few speakers re-run from the linkage cut at lo clusters, which does not depend on
-            # the setting; every setting's re-runs share the batches of their tier
-            lo = bounds[0]
-            low = [e for e in entries if counted[e][0] < lo[e[1]]]
-            recs = sorted(set(b for _, b in low))
-            mc = dict(zip(recs, _ahc.cut_count([Zs[b] for b in recs], lens[recs], lo[recs])))
-            met = [e for e in low if lens[e[1]] >= lo[e[1]]]
-            mc_d = {b: torch.from_numpy(mc[b]).to(dev) for b in set(b for _, b in met)}
-            again = {}
-            if met:
-                run_tiers(met, {e: int(mc[e[1]].max()) + 1 for e in met}, lambda e: mc_d[e[1]], None, again)
-            for e in low:
-                *r, rule = _recut_outcome(lens[e[1]], lo[e[1]], mc[e[1]], again.get(e))
-                res[e] = tuple(r)
-                counted[e] = (counted[e][0], rule)
+    if max_batch_bytes is None:
+        max_batch_bytes = int(torch.cuda.mem_get_info(dev)[0] * BUDGET_FRACTION)
+    # per (setting, recording): labels, labels2nd, iterations, flags[, unconstrained count, rule]
+    res = _vb_stage([(s.Fa, s.Fb, s.loopP, s.smoothing) for s in settings], [ahc_labels[s.threshold] for s in settings],
+                    [lab_d[s.threshold] for s in settings], Zs, lens, fea, Phi, bounds, init, dev, make_batch,
+                    packer(lens, int(fea.shape[1]), dev, max_batch_bytes), maxIters=max_iters, epsilon=epsilon)
     from . import score
     ovl = [None] * len(names)
     if with_overlap:
@@ -289,11 +234,11 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     for k, s in enumerate(settings):
         out[s] = {}
         for b, n in enumerate(names):
-            l1, l2, it, fl = res[(k, b)]
+            l1, l2, it, fl = res[(k, b)][:4]
             item = _result(n, recordings[n][1], l1, l2, it, output_2nd, ovl[b])
             item['flags'] = int(fl)
             if bounds is not None:
-                _count_fields(item, *counted[(k, b)], bounds[0][b], bounds[1][b])
+                _count_fields(item, *res[(k, b)][4:6], bounds[0][b], bounds[1][b])
             if der is not None:
                 item['der'] = {p: v for p, v in der[(k, b)].items() if p != 'jer'}
                 if jer:
