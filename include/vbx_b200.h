@@ -224,6 +224,39 @@ int vbx_enroll(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, in
                size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
                double *F_out, double *n_enroll_out, double *F_enroll_out, void *stream);
 
+/* Score normalisation against a cohort (adaptive symmetric normalisation, DESIGN.md section 5.17); needs a handle, no
+ * plan.  M scored speakers as for vbx_link (fea [N,R], Phi [R], speaker [N] in [0, M), DEVICE) and C >= 2 cohort
+ * speakers (cohort_fea [N_c,R] through the same front end, cohort_speaker [N_c] in [0, C), DEVICE).  Both sets get
+ * vbx_link's statistics; every scored speaker x is scored against every cohort speaker with vbx_link's LLR (the kernel of
+ * vbx_enroll: bit-identical to vbx_enroll's llr against the same speakers), and with K = min(top_k, C)
+ *   mean_out [x] = mean of x's K largest cohort scores, std_out [x] = their population standard deviation (ddof 0)
+ * (DEVICE float64 [M]; ties at the K-th value count as many copies as needed).  scores_out [M,C]: optional (NULL: not
+ * written).  Fixed-order sums: the bits do not depend on the run or on which other speakers share the call.
+ * workspace: vbx_cohort_workspace_bytes(M, C) bytes (about 8 M C + 1.1 KB (M + C)), 256-byte aligned.  Stream ordered,
+ * no allocation, no host synchronisation.  VBX_ERR_ARG: R outside 1..128, c = Fa / Fb negative or not finite, C < 2,
+ * top_k < 2, N_c < 1, M above 2^31 - 1, null pointers, misaligned or short workspace. */
+int vbx_cohort_workspace_bytes(vbx_handle_t h, int64_t M, int64_t C, size_t *bytes_out);
+int vbx_cohort_stats(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
+                     int64_t M, const float *cohort_fea, int64_t N_c, const int32_t *cohort_speaker, int64_t C,
+                     double Fa, double Fb, int32_t top_k, void *workspace, size_t workspace_bytes, double *mean_out,
+                     double *std_out, double *scores_out, void *stream);
+/* vbx_link with normalised scores: the distance of two speakers of different recordings is -S(s, u),
+ *   S(s, u) = 1/2 [ (LLR(s,u) - mean[s]) / std[s] + (LLR(s,u) - mean[u]) / std[u] ],
+ * with mean, std [M] (DEVICE, vbx_cohort_stats over the same speakers; every std must be finite and > 0); 1e30 within a
+ * recording and 0 on the diagonal as before, and the matrix stays symmetric bit for bit.  dist_out then holds these. */
+int vbx_link_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
+                  int64_t M, const int32_t *speaker_rec, double Fa, double Fb, void *workspace, size_t workspace_bytes,
+                  double *n_out, double *F_out, double *dist_out, double *Z_out, const double *mean, const double *std,
+                  void *stream);
+/* vbx_enroll on S(s, e) in place of LLR(s, e), with mean, std [M] of the archive speakers and enroll_mean, enroll_std [E]
+ * of the enrolled speakers (DEVICE, vbx_cohort_stats): the threshold is on S, and best_llr_out and llr_out hold S. */
+int vbx_enroll_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
+                    int64_t M, const int64_t *speaker_rec_offsets, int32_t n_rec, const float *enroll_fea, int64_t N_e,
+                    const int32_t *enroll_speaker, int64_t E, double Fa, double Fb, double threshold, void *workspace,
+                    size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
+                    double *F_out, double *n_enroll_out, double *F_enroll_out, const double *mean, const double *std,
+                    const double *enroll_mean, const double *enroll_std, void *stream);
+
 /* Float64 evaluation of the same EM loop ("exact" mode for the one-recording-per-call use of VBx/vbhmm.py:154-158,
  * where the reference stops on an ELBO improvement < 1e-6, VBx/vbhmm.py:157 -- below float32 resolution).
  * All arrays float64: fea [N,R] (the reference's X, VBx/VBx.py:30), Phi [R], gamma_io [N,S], pi_io [n_rec,S],

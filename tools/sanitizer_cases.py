@@ -1,8 +1,8 @@
 """Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection at
 D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
 6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels (also under a speaker-count bound),
-the dense forward_backward(), the ELBO trace, DER / JER scoring, speaker linking across recordings and enrolment
-against known speakers.
+the dense forward_backward(), the ELBO trace, DER / JER scoring, speaker linking across recordings, enrolment
+against known speakers and score normalisation against a cohort.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
 """
@@ -113,6 +113,22 @@ for E in (1, 7, 45):
                                    17.0, 0.0, dev, llr=True, max_bytes=8 * E * 100)
     torch.cuda.synchronize()
     print('enroll ok', E, len(e_out.table.rec), int((e_out.assign >= 0).sum()))
+
+# score normalisation against a cohort (vbx_cohort_stats, vbx_link_norm, vbx_enroll_norm): C = 45 and M not multiples
+# of 32, top_k > C, a run forced into chunks, and the recording with 150 speakers
+from vbx_b200 import cohort  # noqa: E402
+c_x = torch.randn((100, 16), device=dev)
+c_x[:, 13:] = 0
+c_spk = np.concatenate([np.arange(45), gl.integers(0, 45, 55)])
+e_offs = np.concatenate([[0], np.cumsum(e_lens)])
+c_st = cohort.cohort_stats(e_fea, l_phi, e_offs, e_labels, c_x, c_spk, 0.3, 17.0, top_k=50, device=dev,
+                           max_bytes=8 * 45 * 40, scores=True)
+c_en = cohort.cohort_stats(e_x, l_phi, None, e_spk, c_x, c_spk, 0.3, 17.0, top_k=50, device=dev)
+c_link = link.link_speakers(e_fea, l_phi, e_offs, e_labels, 0.3, 17.0, dev, dist=True, norm=c_st[:2])
+c_enr = enroll.enroll_speakers(e_fea, l_phi, e_offs, e_labels, e_x, e_spk, 0.3, 17.0, 0.0, dev, llr=True,
+                               max_bytes=8 * 45 * 100, norm=c_st[:2] + c_en[:2])
+torch.cuda.synchronize()
+print('cohort ok', len(c_st.mean), float(c_st.std.min()), float(c_link[3][:, 2].min()), int((c_enr.assign >= 0).sum()))
 
 # wgmma projection at the smallest and largest D, one frame and one frame past a full wave of tiles
 sms = torch.cuda.get_device_properties(0).multi_processor_count

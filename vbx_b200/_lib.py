@@ -14,7 +14,8 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_prepare_project', 'vbx_prepare_xvectors', 'vbx_run', 'vbx_run_per_recording', 'vbx_hard_labels', 'vbx_hard_labels_keep', 'vbx_ahc_workspace_bytes', 'vbx_ahc', 'vbx_launch_count', 'vbx_get_timings', 'vbx_f64_workspace_bytes',
            'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace', 'vbx_get_gsum',
            'vbx_score', 'vbx_score_overlap', 'vbx_score_jer', 'vbx_link_workspace_bytes', 'vbx_link',
-           'vbx_enroll_workspace_bytes', 'vbx_enroll']
+           'vbx_enroll_workspace_bytes', 'vbx_enroll', 'vbx_cohort_workspace_bytes', 'vbx_cohort_stats', 'vbx_link_norm',
+           'vbx_enroll_norm']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
@@ -108,6 +109,15 @@ def load():
     lib.vbx_enroll.restype = ctypes.c_int
     lib.vbx_enroll.argtypes = [vp, vp, vp, i64, i32, vp, i64, vp, i32, vp, i64, vp, i64, dbl, dbl, dbl, vp,
                                ctypes.c_size_t, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.vbx_cohort_workspace_bytes.restype = ctypes.c_int
+    lib.vbx_cohort_workspace_bytes.argtypes = [vp, i64, i64, ctypes.POINTER(ctypes.c_size_t)]
+    lib.vbx_cohort_stats.restype = ctypes.c_int
+    lib.vbx_cohort_stats.argtypes = [vp, vp, vp, i64, i32, vp, i64, vp, i64, vp, i64, dbl, dbl, i32, vp, ctypes.c_size_t,
+                                     vp, vp, vp, vp]
+    lib.vbx_link_norm.restype = ctypes.c_int
+    lib.vbx_link_norm.argtypes = lib.vbx_link.argtypes[:-1] + [vp, vp, vp]
+    lib.vbx_enroll_norm.restype = ctypes.c_int
+    lib.vbx_enroll_norm.argtypes = lib.vbx_enroll.argtypes[:-1] + [vp, vp, vp, vp, vp]
     lib.vbx_get_timings.restype = ctypes.c_int
     lib.vbx_get_timings.argtypes = [vp, ctypes.POINTER(dbl), ctypes.POINTER(i64), i32]
     _lib = lib

@@ -24,6 +24,11 @@ enrolled speakers of the ark (DESIGN.md section 5.16): a speaker whose log-likel
 reaches X takes that speaker's name, one name per speaker within a recording; the others are written as
 unknown-<recording>-<label>, or with --link-threshold linked among themselves and written as unknown-<id>.  With
 --output-2nd the second-label RTTMs use the same names.
+
+With --cohort-ark FILE --cohort-utt2spk FILE (both or neither; needs --link-threshold or the enrolment options) the
+linking and enrolment scores are normalised against the cohort speakers of the ark (DESIGN.md section 5.17), speakers
+known to be none of the archive's: each score is standardised by the mean and spread of both speakers' --cohort-top
+(default 200) largest cohort scores, and --link-threshold and --enroll-threshold are on that normalised score.
 """
 import argparse
 import os
@@ -95,6 +100,12 @@ def build_parser():
     ap.add_argument('--enroll-utt2spk', default=None, help='the speaker of each x-vector of --enroll-ark (utt2spk)')
     ap.add_argument('--enroll-threshold', default=None, type=float,
                     help='least log-likelihood ratio at which a speaker takes an enrolled name')
+    ap.add_argument('--cohort-ark', default=None,
+                    help='x-vectors of cohort speakers (Kaldi ark), none of them in the archive, to normalise the '
+                         'linking and enrolment scores by')
+    ap.add_argument('--cohort-utt2spk', default=None, help='the speaker of each x-vector of --cohort-ark (utt2spk)')
+    ap.add_argument('--cohort-top', default=None, type=int,
+                    help='how many of each speaker\'s largest cohort scores set its mean and spread (default 200)')
     return ap
 
 
@@ -105,10 +116,21 @@ def main(argv=None):
     enr = [args.enroll_ark, args.enroll_utt2spk, args.enroll_threshold]
     if any(v is not None for v in enr) and any(v is None for v in enr):
         ap.error('--enroll-ark, --enroll-utt2spk and --enroll-threshold go together')
+    coh = [args.cohort_ark, args.cohort_utt2spk]
+    if any(v is not None for v in coh) and any(v is None for v in coh):
+        ap.error('--cohort-ark and --cohort-utt2spk go together')
+    if args.cohort_top is not None and args.cohort_ark is None:
+        ap.error('--cohort-top needs --cohort-ark and --cohort-utt2spk')
+    if args.cohort_ark is not None and args.link_threshold is None and args.enroll_ark is None:
+        ap.error('a cohort normalises the linking and enrolment scores: give --link-threshold or the enrolment options')
+    if args.cohort_top is not None and args.cohort_top < 2:
+        ap.error('--cohort-top must be >= 2')
     from . import formats
     from .pipeline import diarize_batch, linked_lines, named_lines
     from .score import read_overlaps
     enroll = formats.read_enrolment(args.enroll_ark, args.enroll_utt2spk) if args.enroll_ark is not None else None
+    cohort = formats.read_enrolment(args.cohort_ark, args.cohort_utt2spk) if args.cohort_ark is not None else None
+    norm_kw = {} if cohort is None else dict(cohort=cohort, cohort_top=200 if args.cohort_top is None else args.cohort_top)
     overlaps = read_overlaps(args.overlap_rttm) if args.overlap_rttm is not None else None
     segs = formats.read_segments(args.segments_file)                        # VBx/vbhmm.py:105
     plda = formats.read_kaldi_plda(args.plda_file)                          # VBx/vbhmm.py:107
@@ -123,7 +145,8 @@ def main(argv=None):
                         threshold=args.threshold, smoothing=args.init_smoothing, init=args.init, chain=args.chain,
                         device=args.device, output_2nd=args.output_2nd, overlaps=overlaps,
                         num_speakers=args.num_speakers, min_speakers=args.min_speakers, max_speakers=args.max_speakers,
-                        link_threshold=args.link_threshold, enroll=enroll, enroll_threshold=args.enroll_threshold)
+                        link_threshold=args.link_threshold, enroll=enroll, enroll_threshold=args.enroll_threshold,
+                        **norm_kw)
     linked = args.link_threshold is not None
     os.makedirs(args.out_rttm_dir, exist_ok=True)                           # VBx/vbhmm.py:170
     for name, item in out.items():

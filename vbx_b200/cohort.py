@@ -1,0 +1,139 @@
+"""Score normalisation against a cohort (DESIGN.md section 5.17).
+
+The same-speaker LLR of section 5.15 is not calibrated: it grows with the number of x-vectors and with a speaker's
+offset from the PLDA mean, so one threshold means different things for different speakers and archives.  Adaptive
+symmetric normalisation (AS-norm) standardises every score by the scores of both speakers against a cohort of speakers
+known to be someone else: speaker x scores LLR(x, c) against each cohort speaker c, mu_x and sigma_x are the mean and
+population standard deviation of its K = min(top_k, C) largest cohort scores (on the device, vbx_cohort_stats), and
+
+    S(x, y) = 1/2 [ (LLR(x, y) - mu_x) / sigma_x + (LLR(x, y) - mu_y) / sigma_y ].
+
+link.link_speakers and enroll.enroll_speakers take the statistics (norm=) and then decide on S.
+"""
+import ctypes
+from collections import namedtuple
+
+import numpy as np
+
+DEFAULT_TOP_K = 200        # a conventional AS-norm value, not tuned here; top_k >= C is plain S-norm
+SIGMA_MIN = 1e-6           # smallest accepted sigma_x (DESIGN.md section 5.17: keeps |S| far below the cannot-link regime)
+
+# mean [M], std [M] float64 numpy; K = min(top_k, C); scores [M,C] or None
+CohortStats = namedtuple('CohortStats', 'mean std K scores')
+
+
+def check_top_k(top_k):
+    """top_k as an int; ValueError below 2 (one score has no spread)."""
+    if isinstance(top_k, (bool, np.bool_)) or not isinstance(top_k, (int, np.integer)) or top_k < 2:
+        raise ValueError(f'cohort top_k must be an integer >= 2, got {top_k!r}')
+    return int(top_k)
+
+
+def check_cohort(cohort, dim):
+    """cohort = {name: x [n, dim]} checked: at least two speakers, each with at least one x-vector of dimension dim.
+    Returns [(name, float64 array)] in dict order."""
+    if not isinstance(cohort, dict) or not cohort:
+        raise ValueError('cohort must be a non-empty {name: x-vectors} dict')
+    if len(cohort) < 2:
+        raise ValueError(f'a cohort needs at least 2 speakers, got {len(cohort)}')
+    out = []
+    for name, x in cohort.items():
+        x = np.asarray(x, dtype=np.float64)
+        if x.ndim != 2 or x.shape[0] == 0:
+            raise ValueError(f'cohort speaker {name!r}: needs at least one x-vector as an [n, {dim}] array')
+        if x.shape[1] != dim:
+            raise ValueError(f'cohort speaker {name!r}: x-vectors of dimension {x.shape[1]}, the archive has {dim}')
+        out.append((name, x))
+    return out
+
+
+def check_spread(std, names):
+    """ValueError naming the speakers whose sigma is not finite or below SIGMA_MIN (e.g. a cohort of identical
+    speakers: every top-K score is the same number)."""
+    std = np.asarray(std, dtype=np.float64)
+    bad = np.nonzero(~(std >= SIGMA_MIN) | ~np.isfinite(std))[0]
+    if len(bad):
+        shown = ', '.join(f'{names[i]} ({std[i]!r})' for i in bad[:10])
+        raise ValueError(f'cohort scores without spread (sigma not finite or below {SIGMA_MIN:g}) for {len(bad)} '
+                         f'speaker(s): {shown}')
+
+
+def cohort_stats(fea, Phi, offsets, labels, cohort_fea, cohort_speaker, Fa, Fb, top_k=DEFAULT_TOP_K, device=None,
+                 max_bytes=2 ** 31, scores=False):
+    """mu and sigma of every scored speaker's top_k cohort scores on the device (vbx_cohort_stats).  fea [N,R], Phi [R]:
+    the features the VB-HMM ran with.  Scored speakers: with offsets [B+1], labels holds each recording's first labels
+    and the speakers are link.speaker_table's; with offsets None, labels is a speaker index [N] in [0, M) (-1: none),
+    every speaker with at least one x-vector.  cohort_fea [N_c,R]: the cohort x-vectors through the same front end;
+    cohort_speaker [N_c]: their speaker in [0, C), C >= 2, every one with an x-vector.  Speakers whose M x C score block
+    exceeds max_bytes are split into chunks, one call each (the same bits).  Returns CohortStats (numpy), with the
+    scores [M,C] when scores=True."""
+    import torch
+    from . import _lib
+    from ._lib import VbxError
+    from .link import speaker_index
+    K_req = check_top_k(top_k)
+    cspk = np.asarray(cohort_speaker, dtype=np.int64).reshape(-1)
+    if len(cspk) == 0 or cspk.min() < 0:
+        raise ValueError('cohort_speaker must hold at least one speaker index, all >= 0')
+    C = int(cspk.max()) + 1
+    if C < 2:
+        raise ValueError(f'a cohort needs at least 2 speakers, got {C}')
+    if np.bincount(cspk, minlength=C).min() == 0:
+        raise ValueError('every cohort speaker 0 .. C-1 needs at least one x-vector')
+    if offsets is None:
+        spk = np.asarray(labels, dtype=np.int64).reshape(-1)
+        M = int(spk.max()) + 1 if len(spk) else 0
+        if M and np.bincount(spk[spk >= 0], minlength=M).min() == 0:
+            raise ValueError('every scored speaker 0 .. M-1 needs at least one x-vector')
+    else:
+        spk, M = speaker_index(offsets, labels)
+    if not torch.cuda.is_available():
+        raise VbxError('cohort_stats(): no CUDA device - vbx_b200 has no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    fea = torch.as_tensor(fea).to(dev, torch.float32).contiguous()
+    Phi = torch.as_tensor(Phi).to(dev, torch.float32).contiguous()
+    cfea = torch.as_tensor(cohort_fea).to(dev, torch.float32).contiguous()
+    N, R = int(fea.shape[0]), int(fea.shape[1])
+    if len(spk) != N:
+        raise ValueError(f'{len(spk)} speaker indices for {N} x-vectors')
+    if tuple(cfea.shape) != (len(cspk), R):
+        raise ValueError(f'cohort_fea must be [{len(cspk)}, {R}], got {tuple(cfea.shape)}')
+    # chunks of consecutive speakers with at most max_bytes of scores (one speaker alone may exceed it)
+    per = max(1, int(max_bytes) // (8 * C))
+    chunks = [(s0, min(s0 + per, M)) for s0 in range(0, M, per)]
+    lib = _lib.load()
+    h = ctypes.c_void_p()
+    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
+        raise VbxError('vbx_create failed: no usable sm_90 device')
+    at = lambda x, off=0: ctypes.c_void_p(x.data_ptr() + off * x.element_size()) if x is not None else None
+    try:
+        need = ctypes.c_size_t()
+        m_max = max((b - a for a, b in chunks), default=0)
+        if lib.vbx_cohort_workspace_bytes(h, m_max, C, ctypes.byref(need)) != 0:
+            raise VbxError(f'vbx_cohort_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
+        with torch.cuda.device(dev):
+            ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=dev)
+            cspk_d = torch.from_numpy(cspk.astype(np.int32)).to(dev)
+            mean = torch.empty(M, dtype=torch.float64, device=dev)
+            std = torch.empty(M, dtype=torch.float64, device=dev)
+            L = torch.empty((M, C), dtype=torch.float64, device=dev) if scores else None
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            keep = []
+            for s0, s1 in chunks:
+                mine = np.nonzero((spk >= s0) & (spk < s1))[0]
+                x0, x1 = int(mine[0]), int(mine[-1]) + 1        # every speaker has an x-vector
+                sp = spk[x0:x1]
+                spk_d = torch.from_numpy(np.where((sp >= s0) & (sp < s1), sp - s0, -1).astype(np.int32)).to(dev)
+                keep.append(spk_d)
+                rc = lib.vbx_cohort_stats(h, at(fea, x0 * R), at(Phi), x1 - x0, R, at(spk_d), s1 - s0, at(cfea),
+                                          len(cspk), at(cspk_d), C, float(Fa), float(Fb), K_req, at(ws), ws.numel(),
+                                          at(mean, s0), at(std, s0), at(L, s0 * C), stream)
+                if rc != 0:
+                    raise VbxError(f'vbx_cohort_stats failed ({rc}): {lib.vbx_last_error(h).decode()}')
+            out = CohortStats(mean.cpu().numpy(), std.cpu().numpy(), min(K_req, C),
+                              L.cpu().numpy() if scores else None)
+    finally:
+        lib.vbx_destroy(h)
+    return out

@@ -1,0 +1,179 @@
+// Adaptive symmetric score normalisation against a cohort (DESIGN.md section 5.17).  Every scored speaker x (archive or
+// enrolled speakers, with section 5.15's statistics) is scored against the C cohort speakers with section 5.15's LLR,
+// and mu_x, sigma_x are the mean and population standard deviation of its K = min(top_k, C) largest cohort scores:
+//   enroll_score_kernel  (vbx_enroll.cu, through launch_cohort_scores) the [M, C] cohort LLRs, unchanged
+//   cohort_topk_kernel   one CTA per speaker: the K-th largest score by a radix select on order-preserving 64-bit
+//                        keys (8 passes of 8 bits, histograms in shared memory), then mu and sigma by fixed-order sums
+//   norm_scores_kernel   S(x, y) = 1/2 [ (LLR - mu_x) / sigma_x + (LLR - mu_y) / sigma_y ] in place over the link
+//                        distances (d = -S; the diagonal and the cannot-link entries untouched) or the enrolment LLRs
+#include <algorithm>
+
+#include "vbx_internal.cuh"
+
+namespace vbx {
+
+namespace {
+
+constexpr int kTopThreads = 256;
+constexpr int kTopWarps = kTopThreads / 32;
+constexpr int64_t kNormGrid = 1 << 20;     // CTAs of norm_scores_kernel at most; beyond that they stride
+
+__host__ __device__ size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
+
+struct CohortWs {
+    SpeakerStats a, co;      // scored speakers [M], cohort speakers [C]
+    double *scores;          // [M, C]
+};
+
+CohortWs cohort_layout(uint8_t *ws, int64_t M, int64_t C, size_t *total) {
+    CohortWs w;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { uint8_t *p = ws ? ws + o : nullptr; o += al(bytes); return p; };
+    auto stats = [&](int64_t n) {
+        SpeakerStats s;
+        s.n = reinterpret_cast<double *>(take(n * 8));
+        s.e = reinterpret_cast<double *>(take(n * 8));
+        s.b = reinterpret_cast<double *>(take(n * kMaxR * 8));
+        s.first = reinterpret_cast<long long *>(take(n * 8));
+        s.last = reinterpret_cast<long long *>(take(n * 8));
+        s.offs = reinterpret_cast<int64_t *>(take(4 * 8));
+        return s;
+    };
+    w.a = stats(M);
+    w.co = stats(C);
+    w.scores = reinterpret_cast<double *>(take((size_t)M * C * 8));
+    if (total) *total = o;
+    return w;
+}
+
+// Doubles ordered as their keys are ordered (as unsigned integers): negative values bit-inverted, the others with the
+// sign bit set.  -0.0 sorts just below +0.0; equal values have equal keys.
+__device__ __forceinline__ unsigned long long order_key(double v) {
+    const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+
+__device__ __forceinline__ double key_value(unsigned long long k) {
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+// Sum over the CTA: a fixed butterfly in every warp, then the warps in order (the same bits on every run).
+__device__ __forceinline__ double block_sum(double v, double *red) {
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double t = 0.0;
+    for (int q = 0; q < kTopWarps; ++q) t += red[q];
+    __syncthreads();                                  // red is rewritten by the next call
+    return t;
+}
+
+// One CTA per scored speaker (row of scores [M, C]).  Pass p = 0 .. 7 histograms byte 7 - p of the keys that match the
+// bytes chosen so far and picks the byte of the K-th largest key from the top; after 8 passes `prefix` is that key and
+// `k` the rank of the K-th value among its tied copies, so the K largest are the values above it plus k copies of it.
+// Every thread sums its strided values in increasing column order and block_sum adds the threads in a fixed order, so
+// the result depends on C and the row alone (not on M, the chunk or the launch).
+__global__ void __launch_bounds__(kTopThreads) cohort_topk_kernel(const double *__restrict__ scores, int64_t C,
+                                                                  int64_t K, double *__restrict__ mean_out,
+                                                                  double *__restrict__ std_out) {
+    __shared__ unsigned int hist[256];
+    __shared__ double red[kTopWarps];
+    __shared__ unsigned long long s_prefix;
+    __shared__ long long s_k;
+    const double *v = scores + (int64_t)blockIdx.x * C;
+    unsigned long long prefix = 0, mask = 0;
+    long long k = K;
+    for (int shift = 56; shift >= 0; shift -= 8) {
+        hist[threadIdx.x] = 0u;
+        __syncthreads();
+        for (int64_t j = threadIdx.x; j < C; j += kTopThreads) {
+            const unsigned long long key = order_key(v[j]);
+            if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);   // integer counts: order-free
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            long long above = 0;
+            int b = 255;
+            for (; b > 0 && above + (long long)hist[b] < k; --b) above += hist[b];
+            s_k = k - above;
+            s_prefix = prefix | ((unsigned long long)b << shift);
+        }
+        __syncthreads();
+        k = s_k;
+        prefix = s_prefix;
+        mask |= 255ull << shift;
+    }
+    const double vk = key_value(prefix);
+    double s = 0.0;
+    for (int64_t j = threadIdx.x; j < C; j += kTopThreads) {
+        const double x = v[j];
+        if (order_key(x) > prefix) s += x;
+    }
+    const double mu = (block_sum(s, red) + (double)k * vk) / (double)K;
+    double q = 0.0;
+    for (int64_t j = threadIdx.x; j < C; j += kTopThreads) {
+        const double x = v[j];
+        if (order_key(x) > prefix) q += (x - mu) * (x - mu);
+    }
+    const double dk = vk - mu;
+    const double var = (block_sum(q, red) + (double)k * (dk * dk)) / (double)K;
+    if (threadIdx.x == 0) {
+        mean_out[blockIdx.x] = mu;
+        std_out[blockIdx.x] = sqrt(var);
+    }
+}
+
+// x [rows, cols] in place: LLR -> S(i, j) with row statistics (mr, sr) and column statistics (mc, sc).  link = 1: x holds
+// distances d = -LLR, written back as -S, and the diagonal and the entries equal to `skip` (cannot-link) stay as they
+// are.  S is 1/2 (a_i + a_j) with a_i = (LLR - mu_i) / sigma_i: the sum commutes, so d[i][j] and d[j][i] stay the same
+// number.  copy_out (optional) receives the result.
+__global__ void __launch_bounds__(256) norm_scores_kernel(double *__restrict__ x, int64_t rows, int64_t cols,
+                                                          const double *__restrict__ mr, const double *__restrict__ sr,
+                                                          const double *__restrict__ mc, const double *__restrict__ sc,
+                                                          int link, double skip, double *__restrict__ copy_out) {
+    const int64_t n = rows * cols, stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
+        const int64_t i = t / cols, j = t - i * cols;
+        double d = x[t];
+        if (!link || (i != j && d != skip)) {
+            const double l = link ? -d : d;
+            const double s = 0.5 * ((l - mr[i]) / sr[i] + (l - mc[j]) / sc[j]);
+            d = link ? -s : s;
+            x[t] = d;
+        }
+        if (copy_out) copy_out[t] = d;
+    }
+}
+
+}  // namespace
+
+size_t cohort_workspace_bytes(int64_t M, int64_t C) {
+    size_t total = 0;
+    cohort_layout(nullptr, M, C, &total);
+    return total;
+}
+
+int launch_cohort(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
+                  const float *cohort_fea, int64_t N_c, const int32_t *cohort_spk, int64_t C, double c, int64_t top_k,
+                  void *workspace, double *mean_out, double *std_out, double *scores_out, cudaStream_t st) {
+    if (M == 0) return 0;
+    const CohortWs w = cohort_layout(reinterpret_cast<uint8_t *>(workspace), M, C, nullptr);
+    const int la = launch_speaker_stats(fea, Phi, spk, N, R, M, c, w.a, nullptr, nullptr, st);
+    const int lc = launch_speaker_stats(cohort_fea, Phi, cohort_spk, N_c, R, C, c, w.co, nullptr, nullptr, st);
+    const int ls = launch_cohort_scores(w.a, w.co, Phi, M, C, R, c, w.scores, scores_out, st);
+    if (la < 0 || lc < 0 || ls < 0) return -1;
+    cohort_topk_kernel<<<(unsigned)M, kTopThreads, 0, st>>>(w.scores, C, std::min(top_k, C), mean_out, std_out);
+    return cudaGetLastError() == cudaSuccess ? la + lc + ls + 1 : -1;
+}
+
+int launch_norm_scores(double *x, int64_t rows, int64_t cols, const double *mean_r, const double *std_r,
+                       const double *mean_c, const double *std_c, bool link, double skip, double *copy_out,
+                       cudaStream_t st) {
+    const int64_t n = rows * cols;
+    if (n == 0) return 0;
+    norm_scores_kernel<<<(unsigned)std::min<int64_t>((n + 255) / 256, kNormGrid), 256, 0, st>>>(
+        x, rows, cols, mean_r, std_r, mean_c, std_c, link ? 1 : 0, skip, copy_out);
+    return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+}  // namespace vbx

@@ -8,6 +8,8 @@
 //                         C[k][e] = threshold - llr[k][e] (e < E), C[k][E + j] = 0 ("unknown" columns), by shortest
 //                         augmenting paths (Jonker-Volgenant, the method of scipy's linear_sum_assignment): one
 //                         Dijkstra per row over the columns; a persistent grid, one recording per CTA at a time
+// With cohort statistics (vbx_enroll_norm, section 5.17) vbx_cohort.cu's norm_scores_kernel turns llr into S in place
+// between the two.  launch_cohort_scores runs enroll_score_kernel against a cohort for vbx_cohort_stats.
 #include <algorithm>
 #include <climits>
 #include <vector>
@@ -290,7 +292,8 @@ int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const in
                   const int64_t *rec_off_host, int n_rec, const float *enroll_fea, int64_t N_e, const int32_t *enroll_spk,
                   int64_t E, double c, double threshold, void *workspace, int sms, int32_t *assign_out,
                   double *best_llr_out, double *llr_out, double *n_out, double *F_out, double *n_enroll_out,
-                  double *F_enroll_out, cudaStream_t st) {
+                  double *F_enroll_out, cudaStream_t st, const double *mean, const double *std,
+                  const double *enroll_mean, const double *enroll_std) {
     std::vector<int64_t> busy(1, 0);                  // speaker offsets of the recordings that have speakers
     int64_t max_k = 0;
     for (int b = 0; b < n_rec; ++b) {
@@ -311,8 +314,13 @@ int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const in
     if (M > 0) {
         const int64_t n_tiles = ((M + 31) / 32) * ((E + 31) / 32);
         enroll_score_kernel<<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(w.a, w.en, Phi, M, E, R, c,
-                                                                                             w.llr, llr_out);
+                                                                                             w.llr, mean ? nullptr : llr_out);
         ++launches;
+        if (mean) {                                   // normalised scores (section 5.17): assigned and written as llr
+            const int ln = launch_norm_scores(w.llr, M, E, mean, std, enroll_mean, enroll_std, false, 0.0, llr_out, st);
+            if (ln < 0) return -1;
+            launches += ln;
+        }
     }
     if (n_busy > 0) {
         enroll_assign_kernel<<<(unsigned)std::min<int64_t>(n_busy, w.ctas), kAssignThreads, 0, st>>>(
@@ -320,6 +328,15 @@ int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const in
         ++launches;
     }
     return cudaGetLastError() == cudaSuccess ? launches : -1;
+}
+
+int launch_cohort_scores(const SpeakerStats &a, const SpeakerStats &co, const float *Phi, int64_t M, int64_t C, int R,
+                         double c, double *llr, double *llr_out, cudaStream_t st) {
+    if (M == 0) return 0;
+    const int64_t n_tiles = ((M + 31) / 32) * ((C + 31) / 32);
+    enroll_score_kernel<<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(a, co, Phi, M, C, R, c, llr,
+                                                                                         llr_out);
+    return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
 }  // namespace vbx

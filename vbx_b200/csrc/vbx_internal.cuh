@@ -254,7 +254,7 @@ void launch_linkage(const int64_t *offsets, const int64_t *d_off, void *ws, doub
 size_t link_workspace_bytes(int64_t M);
 int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
                 int64_t M, double c, void *workspace, double *n_out, double *F_out, double *dist_out, double *Z_out,
-                cudaStream_t st);
+                cudaStream_t st, const double *mean = nullptr, const double *std = nullptr);
 // vbx_link's span and statistics kernels over M speakers into caller-owned DEVICE arrays (n, e [M], b [M, kMaxR]
 // float64; first, last [M] and offs [4] int64 scratch): n_s, F_s, b_s and e_s exactly as vbx_link computes them.
 // Returns the number of launches, -1 on a launch error.
@@ -271,7 +271,21 @@ int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const in
                   const int64_t *rec_off_host, int n_rec, const float *enroll_fea, int64_t N_e, const int32_t *enroll_spk,
                   int64_t E, double c, double threshold, void *workspace, int sms, int32_t *assign_out,
                   double *best_llr_out, double *llr_out, double *n_out, double *F_out, double *n_enroll_out,
-                  double *F_enroll_out, cudaStream_t st);
+                  double *F_enroll_out, cudaStream_t st, const double *mean = nullptr, const double *std = nullptr,
+                  const double *enroll_mean = nullptr, const double *enroll_std = nullptr);
+// enroll_score_kernel over M scored speakers and C cohort speakers whose statistics are already in a and co: llr [M, C]
+// (and llr_out when not null), bit-identical to vbx_enroll's llr against the same speakers.  Returns 1, 0 for M == 0.
+int launch_cohort_scores(const SpeakerStats &a, const SpeakerStats &co, const float *Phi, int64_t M, int64_t C, int R,
+                         double c, double *llr, double *llr_out, cudaStream_t st);
+// score normalisation against a cohort (vbx_cohort.cu)
+size_t cohort_workspace_bytes(int64_t M, int64_t C);
+int launch_cohort(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
+                  const float *cohort_fea, int64_t N_c, const int32_t *cohort_spk, int64_t C, double c, int64_t top_k,
+                  void *workspace, double *mean_out, double *std_out, double *scores_out, cudaStream_t st);
+// x [rows, cols] of LLRs (link: of distances -LLR, diagonal and `skip` entries kept) replaced by the normalised scores
+int launch_norm_scores(double *x, int64_t rows, int64_t cols, const double *mean_r, const double *std_r,
+                       const double *mean_c, const double *std_c, bool link, double skip, double *copy_out,
+                       cudaStream_t st);
 // wgmma projection (vbx_project_tc.cu)
 size_t tc_scratch_floats();
 int launch_project_wgmma(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,

@@ -9,6 +9,7 @@
 //   link_span_kernel    first / last x-vector of every speaker (integer atomics: order-free)
 //   link_stats_kernel   n_s, F_s (float64, fixed order), b_s and e_s; one CTA per speaker
 //   link_score_kernel   the M x M distances, 32 x 32 tiles of the upper triangle, each written twice
+//   norm_scores_kernel  (vbx_cohort.cu) only with cohort statistics (vbx_link_norm): d = -S in place, section 5.17
 //   ahc_linkage_kernel  (vbx_ahc.cu) unchanged, over the matrix as one "recording" of M items
 #include <algorithm>
 #include <climits>
@@ -231,7 +232,7 @@ size_t link_workspace_bytes(int64_t M) {
 
 int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
                 int64_t M, double c, void *workspace, double *n_out, double *F_out, double *dist_out, double *Z_out,
-                cudaStream_t st) {
+                cudaStream_t st, const double *mean, const double *std) {
     if (M == 0) return 0;
     const LinkWs w = link_layout(reinterpret_cast<uint8_t *>(workspace), M, nullptr);
     int launches = 0;
@@ -243,8 +244,15 @@ int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t 
     }
     link_stats_kernel<<<(unsigned)M, kStatsThreads, 0, st>>>(w, fea, Phi, spk, R, c, n_out, F_out);
     const int64_t tiles = (M + 31) / 32, n_tiles = tiles * (tiles + 1) / 2;
-    link_score_kernel<<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(w, Phi, spk_rec, M, R, c, dist_out);
+    link_score_kernel<<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(w, Phi, spk_rec, M, R, c,
+                                                                                        mean ? nullptr : dist_out);
     launches += 2;
+    if (mean) {                                       // normalised distances (section 5.17): dist_out gets those
+        const int ln = launch_norm_scores(reinterpret_cast<double *>(w.lk), M, M, mean, std, mean, std, true, kBig,
+                                          dist_out, st);
+        if (ln < 0) return -1;
+        launches += ln;
+    }
     if (M >= 2) {
         launch_linkage(w.offs, w.offs + 2, w.lk, Z_out, st);
         ++launches;

@@ -11,7 +11,7 @@ from collections import namedtuple
 
 import numpy as np
 
-from .link import speaker_table
+from .link import speaker_index, speaker_table
 
 UNKNOWN = 'unknown-'       # prefix of the names of speakers that match no enrolled speaker (reserved)
 MAX_THRESHOLD = 1e15
@@ -52,13 +52,16 @@ def check_enrolment(enroll, dim):
 
 
 def enroll_speakers(fea, Phi, offsets, labels, enroll_fea, enroll_speaker, Fa, Fb, threshold, device=None, llr=False,
-                    max_bytes=2 ** 31):
+                    max_bytes=2 ** 31, norm=None):
     """Statistics, LLRs and the per-recording assignment of every archive speaker against the enrolled speakers on the
     device (vbx_enroll).  fea [N,R], Phi [R]: the features the VB-HMM ran with, packed by recording at offsets [B+1];
     labels: each recording's final first labels.  enroll_fea [N_e,R]: the enrolled x-vectors through the same front
     end; enroll_speaker [N_e]: their speaker in [0, E), every speaker with at least one x-vector.  Archives whose M x E
     LLR block exceeds max_bytes are split into chunks of whole recordings, one vbx_enroll call each (the results are
-    the same bits).  Returns EnrollResult (numpy, speaker_table order), with llr [M,E] when llr=True."""
+    the same bits).  norm: None, or (mean [M], std [M], enroll_mean [E], enroll_std [E]) of the archive and enrolled
+    speakers' cohort scores (cohort.cohort_stats): the assignment then runs on the normalised scores S of DESIGN.md
+    section 5.17 with the threshold on S (vbx_enroll_norm), and best_llr and llr hold S.
+    Returns EnrollResult (numpy, speaker_table order), with llr [M,E] when llr=True."""
     import torch
     from . import _lib
     from ._lib import VbxError
@@ -86,13 +89,7 @@ def enroll_speakers(fea, Phi, offsets, labels, enroll_fea, enroll_speaker, Fa, F
     if tuple(efea.shape) != (len(espk), R):
         raise ValueError(f'enroll_fea must be [{len(espk)}, {R}], got {tuple(efea.shape)}')
     first = np.searchsorted(table.rec, np.arange(B + 1)).astype(np.int64)     # each recording's first speaker
-    spk = np.full(N, -1, dtype=np.int64)
-    for b, l in enumerate(labels):
-        l = np.asarray(l, dtype=np.int64).reshape(-1)
-        if len(l) != offsets[b + 1] - offsets[b]:
-            raise ValueError(f'recording {b}: {len(l)} labels for {offsets[b + 1] - offsets[b]} x-vectors')
-        own = table.label[first[b]:first[b + 1]]
-        spk[offsets[b]:offsets[b + 1]] = np.where(l >= 0, first[b] + np.searchsorted(own, l), -1)
+    spk = speaker_index(offsets, labels)[0]
     # chunks of whole recordings with at most max_bytes of LLRs (a recording alone may exceed it)
     chunks, b0 = [], 0
     for b in range(B):
@@ -122,6 +119,10 @@ def enroll_speakers(fea, Phi, offsets, labels, enroll_fea, enroll_speaker, Fa, F
             F_e = torch.empty((E, R), dtype=torch.float64, device=dev)
             L = torch.empty((M, E), dtype=torch.float64, device=dev) if llr else None
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            if norm is not None:
+                stats = [torch.as_tensor(np.asarray(a, dtype=np.float64)).to(dev).contiguous() for a in norm]
+                if [tuple(s.shape) for s in stats] != [(M,), (M,), (E,), (E,)]:
+                    raise ValueError(f'norm must hold mean and std of the {M} archive and the {E} enrolled speakers')
             keep = []
             for ci, (a, z) in enumerate(chunks):
                 s0, x0, x1 = int(first[a]), int(offsets[a]), int(offsets[z])
@@ -129,11 +130,16 @@ def enroll_speakers(fea, Phi, offsets, labels, enroll_fea, enroll_speaker, Fa, F
                 spk_d = torch.from_numpy(np.where(sp >= 0, sp - s0, -1).astype(np.int32)).to(dev)
                 rec_off = np.ascontiguousarray(first[a:z + 1] - s0, dtype=np.int64)
                 keep.append(spk_d)
-                rc = lib.vbx_enroll(h, at(fea, x0 * R), at(Phi), x1 - x0, R, at(spk_d), int(first[z]) - s0,
-                                    rec_off.ctypes.data_as(ctypes.c_void_p), z - a, at(efea), len(espk), at(espk_d), E,
-                                    float(Fa), float(Fb), t, at(ws), ws.numel(), at(assign, s0), at(best, s0),
-                                    at(L, s0 * E), at(n, s0), at(F, s0 * R), at(n_e) if ci == 0 else None,
-                                    at(F_e) if ci == 0 else None, stream)
+                args = (h, at(fea, x0 * R), at(Phi), x1 - x0, R, at(spk_d), int(first[z]) - s0,
+                        rec_off.ctypes.data_as(ctypes.c_void_p), z - a, at(efea), len(espk), at(espk_d), E,
+                        float(Fa), float(Fb), t, at(ws), ws.numel(), at(assign, s0), at(best, s0),
+                        at(L, s0 * E), at(n, s0), at(F, s0 * R), at(n_e) if ci == 0 else None,
+                        at(F_e) if ci == 0 else None)
+                if norm is None:
+                    rc = lib.vbx_enroll(*args, stream)
+                else:
+                    rc = lib.vbx_enroll_norm(*args, at(stats[0], s0), at(stats[1], s0), at(stats[2]), at(stats[3]),
+                                             stream)
                 if rc != 0:
                     raise VbxError(f'vbx_enroll failed ({rc}): {lib.vbx_last_error(h).decode()}')
             out = EnrollResult(table, assign.cpu().numpy().astype(np.int64), best.cpu().numpy(), n.cpu().numpy(),

@@ -38,10 +38,30 @@ def check_threshold(threshold):
     return t
 
 
-def link_speakers(fea, Phi, offsets, labels, Fa, Fb, device=None, dist=False):
+def speaker_index(offsets, labels):
+    """(speaker [N] int64, M): the speaker_table index of every x-vector (-1 where its label is negative) of the
+    recordings packed at offsets [B+1] with first labels `labels`."""
+    offsets = np.asarray(offsets, dtype=np.int64)
+    table = speaker_table(labels)
+    if len(offsets) != len(labels) + 1:
+        raise ValueError('offsets must hold one more entry than labels')
+    spk = np.full(int(offsets[-1]), -1, dtype=np.int64)
+    first = np.searchsorted(table.rec, np.arange(len(labels) + 1))
+    for b, l in enumerate(labels):
+        l = np.asarray(l, dtype=np.int64).reshape(-1)
+        if len(l) != offsets[b + 1] - offsets[b]:
+            raise ValueError(f'recording {b}: {len(l)} labels for {offsets[b + 1] - offsets[b]} x-vectors')
+        own = table.label[first[b]:first[b + 1]]
+        spk[offsets[b]:offsets[b + 1]] = np.where(l >= 0, first[b] + np.searchsorted(own, l), -1)
+    return spk, len(table.rec)
+
+
+def link_speakers(fea, Phi, offsets, labels, Fa, Fb, device=None, dist=False, norm=None):
     """Statistics, pairwise scores and average linkage of every speaker of an archive on the device (vbx_link).
     fea [N,R] and Phi [R]: the features the VB-HMM ran with (CUDA tensors or arrays, float32), packed by recording at
     offsets [B+1]; labels: the final first labels of each recording; Fa, Fb: the VB-HMM's scalars.
+    norm: None, or (mean [M], std [M]) of the speakers' cohort scores (cohort.cohort_stats over the same speakers):
+    the distances are then -S, the normalised scores of DESIGN.md section 5.17 (vbx_link_norm).
     Returns (table, n [M], F [M,R], Z [M-1,4]) as numpy float64 (speaker_table order), and dist [M,M] with dist=True.
     ValueError when the archive has more speakers than the linkage kernel indexes."""
     import torch
@@ -63,14 +83,7 @@ def link_speakers(fea, Phi, offsets, labels, Fa, Fb, device=None, dist=False):
     N, R = int(fea.shape[0]), int(fea.shape[1])
     if int(offsets[-1]) != N or len(offsets) != len(labels) + 1:
         raise ValueError('offsets must hold one more entry than labels and end at the number of x-vectors')
-    spk = np.full(N, -1, dtype=np.int32)
-    first = np.searchsorted(table.rec, np.arange(len(labels) + 1))      # the recording's first speaker
-    for b, l in enumerate(labels):
-        l = np.asarray(l, dtype=np.int64).reshape(-1)
-        if len(l) != offsets[b + 1] - offsets[b]:
-            raise ValueError(f'recording {b}: {len(l)} labels for {offsets[b + 1] - offsets[b]} x-vectors')
-        own = table.label[first[b]:first[b + 1]]
-        spk[offsets[b]:offsets[b + 1]] = np.where(l >= 0, first[b] + np.searchsorted(own, l), -1)
+    spk = speaker_index(offsets, labels)[0].astype(np.int32)
     lib = _lib.load()
     h = ctypes.c_void_p()
     if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
@@ -89,8 +102,15 @@ def link_speakers(fea, Phi, offsets, labels, Fa, Fb, device=None, dist=False):
             D = torch.empty((M, M), dtype=torch.float64, device=dev) if dist else None
             Z = torch.empty((max(M - 1, 0), 4), dtype=torch.float64, device=dev)
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            rc = lib.vbx_link(h, p(fea), p(Phi), N, R, p(spk_d), M, p(rec_d), float(Fa), float(Fb), p(ws), ws.numel(),
-                              p(n), p(F), p(D), p(Z), stream)
+            if norm is None:
+                rc = lib.vbx_link(h, p(fea), p(Phi), N, R, p(spk_d), M, p(rec_d), float(Fa), float(Fb), p(ws),
+                                  ws.numel(), p(n), p(F), p(D), p(Z), stream)
+            else:
+                mean, std = (torch.as_tensor(np.asarray(a, dtype=np.float64)).to(dev).contiguous() for a in norm)
+                if mean.shape != (M,) or std.shape != (M,):
+                    raise ValueError(f'norm must hold mean and std of the {M} speakers')
+                rc = lib.vbx_link_norm(h, p(fea), p(Phi), N, R, p(spk_d), M, p(rec_d), float(Fa), float(Fb), p(ws),
+                                       ws.numel(), p(n), p(F), p(D), p(Z), p(mean), p(std), stream)
             if rc != 0:
                 raise VbxError(f'vbx_link failed ({rc}): {lib.vbx_last_error(h).decode()}')
             out = (table, n.cpu().numpy(), F.cpu().numpy(), Z.cpu().numpy())

@@ -445,7 +445,7 @@ def _count_fields(item, k1, rule, lo, hi):
 def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
                   max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False, overlaps=None,
                   num_speakers=None, min_speakers=None, max_speakers=None, link_threshold=None, enroll=None,
-                  enroll_threshold=None):
+                  enroll_threshold=None, cohort=None, cohort_top=200):
     """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
     recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
     one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
@@ -478,21 +478,35 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     link_threshold linked among themselves across the archive and named unknown-<id + 1>.  Each item then also has
     speaker_names ({label: name}), speaker_llr ({label: the LLR that decided the name}) and rttm_named (its rttm lines,
     or rttm_overlap's with overlaps, with the speaker field set to the name).
+    cohort: None, or a cohort of speakers known to be none of the archive's {name: raw x-vectors [n, Dx]} (at least 2
+    speakers; DESIGN.md section 5.17).  It goes through the archive's front end, and linking and enrolment then decide
+    on the normalised score S (cohort.py: every score standardised by the mean and spread of both speakers' cohort_top
+    largest cohort scores), so link_threshold and enroll_threshold are on S; needs link_threshold or enroll.  Each item
+    then also has score_norm = {'top_k': min(cohort_top, C), 'cohort_speakers': C}, and with enroll speaker_score
+    ({label: the normalised score that decided the name}) in place of speaker_llr.
     Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds]
-    [, count_rule, n_speakers_vb, count][, global_speakers, rttm_linked][, speaker_names, speaker_llr, rttm_named])}."""
+    [, count_rule, n_speakers_vb, count][, global_speakers, rttm_linked][, speaker_names, speaker_llr or speaker_score,
+    rttm_named][, score_norm])}."""
     _check_init(init, overlaps is not None)
     bounds = count_bounds(list(recordings), num_speakers, min_speakers, max_speakers)
     if link_threshold is not None:
         from .link import check_threshold
         check_threshold(link_threshold)
     enrolled = None
+    dims = {int(np.asarray(r[0]).shape[1]) for r in recordings.values()}
     if enroll is not None or enroll_threshold is not None:
         from . import enroll as _enroll
         if enroll is None:
             raise ValueError('enroll_threshold without enroll')
         _enroll.check_threshold(enroll_threshold)
-        dims = {int(np.asarray(r[0]).shape[1]) for r in recordings.values()}
-        enrolled = _enroll.check_enrolment(enroll, dims.pop() if len(dims) == 1 else -1)
+        enrolled = _enroll.check_enrolment(enroll, next(iter(dims)) if len(dims) == 1 else -1)
+    cohort_set = None
+    if cohort is not None:
+        from . import cohort as _cohort
+        if link_threshold is None and enroll is None:
+            raise ValueError('a cohort normalises the linking and enrolment scores: it needs link_threshold or enroll')
+        _cohort.check_top_k(cohort_top)
+        cohort_set = _cohort.check_cohort(cohort, next(iter(dims)) if len(dims) == 1 else -1)
     if not torch.cuda.is_available():
         from ._lib import VbxError
         raise VbxError('diarize_batch(): no CUDA device - vbx_b200 has no CPU fallback')
@@ -514,13 +528,20 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     labels1, labels2 = [r[0] for r in res], [r[1] for r in res]
     out = {}
     maps = None
+    side = lambda sets: _side_features(sets, recordings, names, transform, plda, lda_dim, chain, dev, fea, Phi)
+    enrolled_fea = side(enrolled) if enrolled is not None else None
+    norm = None
+    if cohort_set is not None:
+        norm = _cohort_norm(side(cohort_set), cohort_top, enrolled, enrolled_fea, names, fea, Phi, offs, labels1, Fa,
+                            Fb, dev)
     if link_threshold is not None:
         from . import link as _link
-        table, _, _, Z = _link.link_speakers(fea, Phi, offs, labels1, Fa, Fb, dev)
+        table, _, _, Z = _link.link_speakers(fea, Phi, offs, labels1, Fa, Fb, dev,
+                                             norm=None if norm is None else norm['archive'][:2])
         maps = _link.link_cut(Z, table, link_threshold, labels2)
     if enrolled is not None:
-        spk_names, spk_llr = _enroll_archive(enrolled, enroll_threshold, link_threshold, recordings, names, transform,
-                                             plda, lda_dim, chain, dev, fea, Phi, offs, labels1, labels2, Fa, Fb)
+        spk_names, spk_llr = _enroll_archive(enrolled, enrolled_fea, enroll_threshold, link_threshold, names, dev, fea,
+                                             Phi, offs, labels1, labels2, Fa, Fb, norm)
     for b, n in enumerate(names):
         ovl = None
         if overlaps is not None:
@@ -533,33 +554,68 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
             out[n].update(global_speakers=maps[b],
                           rttm_linked=linked_lines(n, recordings[n][1], labels1[b], labels2[b], maps[b], ovl))
         if enrolled is not None:
-            out[n].update(speaker_names=spk_names[b], speaker_llr=spk_llr[b],
-                          rttm_named=named_lines(n, recordings[n][1], labels1[b], labels2[b], spk_names[b], ovl))
+            out[n].update(speaker_names=spk_names[b], rttm_named=named_lines(n, recordings[n][1], labels1[b], labels2[b],
+                                                                             spk_names[b], ovl))
+            out[n]['speaker_llr' if norm is None else 'speaker_score'] = spk_llr[b]
+        if norm is not None:
+            out[n]['score_norm'] = {'top_k': norm['K'], 'cohort_speakers': norm['C']}
     return out
 
 
-def _enroll_archive(enrolled, threshold, link_threshold, recordings, names, transform, plda, lda_dim, chain, dev, fea,
-                    Phi, offs, labels1, labels2, Fa, Fb):
-    """DESIGN.md section 5.16 for diarize_batch: the enrolled x-vectors through the archive's front end (same chain,
-    padded as the archive's features), the device assignment, and the names (unknown speakers linked among themselves
-    with link_threshold).  Returns per recording ({label: name}, {label: llr})."""
-    from . import enroll as _enroll
-    from . import link as _link
+def _side_features(sets, recordings, names, transform, plda, lda_dim, chain, dev, fea, Phi):
+    """Speakers outside the archive (enrolled or cohort speakers: [(name, raw x-vectors)]) through the archive's front
+    end: the same chain, padded as the archive's features.  Returns (fea_s [N_s,R] float32, speaker index [N_s])."""
     Dx = int(np.asarray(recordings[names[0]][0]).shape[1])
     chain = _resolve_chain(chain, transform, plda, lda_dim, Dx)
-    x_e = np.concatenate([x for _, x in enrolled])
-    front, _, fea_e, _ = _project(x_e, [len(x_e)], transform, plda, lda_dim, chain, dev)
+    x_s = np.concatenate([x for _, x in sets])
+    front, _, fea_s, _ = _project(x_s, [len(x_s)], transform, plda, lda_dim, chain, dev)
     front.close()
-    if fea_e.shape[1] < fea.shape[1]:
-        fea_e, _ = _pad_features(fea_e, Phi[:fea_e.shape[1]])
-    spk_e = np.repeat(np.arange(len(enrolled)), [len(x) for _, x in enrolled])
-    res = _enroll.enroll_speakers(fea, Phi, offs, labels1, fea_e, spk_e, Fa, Fb, threshold, dev)
+    if fea_s.shape[1] < fea.shape[1]:
+        fea_s, _ = _pad_features(fea_s, Phi[:fea_s.shape[1]])
+    return fea_s, np.repeat(np.arange(len(sets)), [len(x) for _, x in sets])
+
+
+def _cohort_norm(cohort_fea, top_k, enrolled, enrolled_fea, names, fea, Phi, offs, labels1, Fa, Fb, dev):
+    """DESIGN.md section 5.17 for diarize_batch: the cohort statistics of the archive's speakers and of the enrolled
+    speakers, each checked for spread (ValueError before any linking or enrolment kernel).  Returns dict(archive,
+    enrolled or None: cohort.CohortStats; table: the archive's speaker table; K; C)."""
+    from . import cohort as _cohort
+    from .link import speaker_table
+    fea_c, spk_c = cohort_fea
+    table = speaker_table(labels1)
+    st = _cohort.cohort_stats(fea, Phi, offs, labels1, fea_c, spk_c, Fa, Fb, top_k, dev)
+    _cohort.check_spread(st.std, [f'{names[b]} speaker {l + 1}' for b, l in zip(table.rec.tolist(), table.label.tolist())])
+    se = None
+    if enrolled is not None:
+        se = _cohort.cohort_stats(enrolled_fea[0], Phi, None, enrolled_fea[1], fea_c, spk_c, Fa, Fb, top_k, dev)
+        _cohort.check_spread(se.std, [f'enrolled {k}' for k, _ in enrolled])
+    return dict(archive=st, enrolled=se, table=table, K=st.K, C=int(spk_c.max()) + 1)
+
+
+def _enroll_archive(enrolled, enrolled_fea, threshold, link_threshold, names, dev, fea, Phi, offs, labels1, labels2,
+                    Fa, Fb, norm=None):
+    """DESIGN.md section 5.16 for diarize_batch: the device assignment of the enrolled speakers (their x-vectors through
+    the archive's front end, _side_features), and the names (unknown speakers linked among themselves with
+    link_threshold).  norm: None or _cohort_norm's statistics (section 5.17): both steps then run on the normalised
+    scores.  Returns per recording ({label: name}, {label: llr or normalised score})."""
+    from . import enroll as _enroll
+    from . import link as _link
+    fea_e, spk_e = enrolled_fea
+    en = None if norm is None else tuple(norm['archive'][:2]) + tuple(norm['enrolled'][:2])
+    res = _enroll.enroll_speakers(fea, Phi, offs, labels1, fea_e, spk_e, Fa, Fb, threshold, dev, norm=en)
     enrolled_names = [k for k, _ in enrolled]
     spk_names, spk_llr = _enroll.enroll_names(res.table, res.assign, res.best_llr, enrolled_names, names, labels2)
     if link_threshold is not None:
         l1 = [_enroll.mask_named(l, m) for l, m in zip(labels1, spk_names)]
         l2 = [_enroll.mask_named(l, m) for l, m in zip(labels2, spk_names)]
-        table, _, _, Z = _link.link_speakers(fea, Phi, offs, l1, Fa, Fb, dev)
+        sub = None
+        if norm is not None:                          # the unknown speakers' rows of the archive's statistics
+            t, st = norm['table'], norm['archive']
+            row = {(b, l): i for i, (b, l) in enumerate(zip(t.rec.tolist(), t.label.tolist()))}
+            t2 = _link.speaker_table(l1)
+            idx = np.array([row[(b, l)] for b, l in zip(t2.rec.tolist(), t2.label.tolist())], dtype=np.int64)
+            sub = (st.mean[idx], st.std[idx])
+        table, _, _, Z = _link.link_speakers(fea, Phi, offs, l1, Fa, Fb, dev, norm=sub)
         lk = _link.link_cut(Z, table, link_threshold, l2)
         spk_names, spk_llr = _enroll.enroll_names(res.table, res.assign, res.best_llr, enrolled_names, names, labels2,
                                                   link=lk)
