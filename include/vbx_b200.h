@@ -201,6 +201,26 @@ int vbx_link(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int3
              int64_t M, const int32_t *speaker_rec, double Fa, double Fb, void *workspace, size_t workspace_bytes,
              double *n_out, double *F_out, double *dist_out, double *Z_out, void *stream);
 
+/* G independent linking problems in one set of launches (DESIGN.md section 5.18), e.g. one per setting of a sweep; needs
+ * a handle, no plan.  The problems share fea [N,R] and Phi [R] (DEVICE, as for vbx_link); problem g has
+ *   speaker [G,N] int32 (DEVICE)   row g: the speaker of x-vector t in [0, M[g]), or -1 (other values count as -1)
+ *   M [G] (HOST)                   its number of speakers
+ *   speaker_rec [sum M] (DEVICE)   the recording of each speaker, problem g's at off_g = M[0] + .. + M[g-1]
+ *   Fa [G], Fb [G] (HOST)          its scalars; every c_g = Fa[g] / Fb[g] must be finite and >= 0
+ * The outputs are packed by the speaker offsets off_g: n_out [sum M], F_out [sum M, R] (optional, as for vbx_link),
+ * Z_out [sum M, 4] with problem g's M[g] - 1 rows from row off_g (vbx_ahc's layout; needed when some M[g] >= 2) and
+ * dist_out (optional) with problem g's M[g] x M[g] distances from element M[0]^2 + .. + M[g-1]^2.  Problem g's n, F,
+ * distances and Z are bit-identical to vbx_link run on that problem alone.  workspace: vbx_link_batch_workspace_bytes(G,
+ * M) bytes, 256-byte aligned; it is at most the sum of vbx_link_workspace_bytes(M[g]), so problems packed by those sizes
+ * fit a budget.  Stream ordered, no allocation; the problems' offsets and c_g go to the device in one copy from the
+ * host, as vbx_ahc's offsets do.  R outside 1..128, an M[g] outside [0, VBX_LINK_MAX_SPEAKERS], more than 2^31 - 1
+ * speakers in all, a bad c_g or a workspace too small return VBX_ERR_ARG. */
+int vbx_link_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, size_t *bytes_out);
+int vbx_link_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                   const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
+                   const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
+                   double *dist_out, double *Z_out, void *stream);
+
 /* Enrolment against known speakers (DESIGN.md section 5.16); needs a handle, no plan.  Archive speakers as for vbx_link
  * (fea [N,R], Phi [R], speaker [N] in [0, M), DEVICE), packed by recording: speaker_rec_offsets [n_rec+1] (HOST int64,
  * from 0 to M, non-decreasing) holds recording b's speakers at speaker_rec_offsets[b] .. [b+1]-1.  Enrolled speakers:

@@ -1,7 +1,8 @@
 """Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection at
 D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
 6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels (also under a speaker-count bound),
-the dense forward_backward(), the ELBO trace, DER / JER scoring, speaker linking across recordings, enrolment
+the dense forward_backward(), the ELBO trace, DER / JER scoring, speaker linking across recordings (one problem and
+batched), enrolment
 against known speakers and score normalisation against a cohort.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
@@ -97,6 +98,14 @@ l_phi = torch.rand(16, device=dev) * (torch.arange(16, device=dev) < 13)
 l_out = link.link_speakers(l_fea, l_phi, np.concatenate([[0], np.cumsum(l_lens)]), l_labels, 0.3, 17.0, dev, dist=True)
 torch.cuda.synchronize()
 print('link ok', len(l_out[0].rec), float(l_out[3][:, 2].min()))
+# batched linking (vbx_link_batch): a problem without speakers, one with a speaker per recording and the one above, each
+# with its own Fa / Fb, in one launch and under a budget that puts the last problem into a launch of its own
+lb_labels = [[np.full(n, -1) for n in l_lens], [np.where(np.arange(n) == 0, 0, -1) for n in l_lens], l_labels]
+for lb_max in (None, 80000):          # 80 000 bytes: the last problem needs 78 592, the others 5 888
+    lb_out = link.link_many(l_fea, l_phi, np.concatenate([[0], np.cumsum(l_lens)]), lb_labels, [0.3, 0.4, 0.2],
+                            [17.0, 6.0, 64.0], dev, max_bytes=lb_max, dist=True)
+    torch.cuda.synchronize()
+    print('link batch ok', [len(o[0].rec) for o in lb_out], float(lb_out[2][3][:, 2].min()))
 
 # enrolment (vbx_enroll): recordings without speakers, E = 1 and E < K_b, a tail tile (M, E not multiples of 32), and a
 # recording with 150 speakers (more than 128)

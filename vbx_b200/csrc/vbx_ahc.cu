@@ -383,8 +383,8 @@ int launch_ahc(const Plan &pl, const std::vector<int64_t> &d_off, const void *x,
 
 size_t linkage_workspace_bytes(int64_t T) { return (size_t)T * T * 8 + (size_t)T * (8 + 4 + 4 + 4 + 4) + (size_t)T; }
 
-void launch_linkage(const int64_t *offsets, const int64_t *d_off, void *ws, double *Z_out, cudaStream_t st) {
-    ahc_linkage_kernel<<<1, kLinkThreads, 0, st>>>(offsets, d_off, reinterpret_cast<uint8_t *>(ws), Z_out);
+void launch_linkage(const int64_t *offsets, const int64_t *d_off, int n, void *ws, double *Z_out, cudaStream_t st) {
+    ahc_linkage_kernel<<<n, kLinkThreads, 0, st>>>(offsets, d_off, reinterpret_cast<uint8_t *>(ws), Z_out);
 }
 
 }  // namespace vbx

@@ -882,6 +882,62 @@ int vbx_link_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N,
                      n_out, F_out, dist_out, Z_out, mean, std, stream);
 }
 
+// the sizes M [G] of vbx_link_batch's problems: each in [0, VBX_LINK_MAX_SPEAKERS], their sum within one launch's grid
+static int check_problem_sizes(vbx_handle_t h, const std::string &who, int32_t G, const int64_t *M) {
+    if (G < 0) return fail(h, VBX_ERR_ARG, who + ": G < 0");
+    if (G > 0 && !M) return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    int64_t total = 0;
+    for (int32_t g = 0; g < G; ++g) {
+        if (M[g] < 0 || M[g] > VBX_LINK_MAX_SPEAKERS)
+            return fail(h, VBX_ERR_ARG, who + ": M[" + std::to_string(g) + "] must lie in [0, VBX_LINK_MAX_SPEAKERS]");
+        total += M[g];
+        if (total > INT32_MAX) return fail(h, VBX_ERR_ARG, who + ": more than 2^31 - 1 speakers in all");
+    }
+    return VBX_OK;
+}
+
+int vbx_link_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    const int rc = check_problem_sizes(h, "vbx_link_batch_workspace_bytes", G, M);
+    if (rc != VBX_OK) return rc;
+    *bytes_out = vbx::link_batch_workspace_bytes(G, M);
+    return VBX_OK;
+}
+
+int vbx_link_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                   const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
+                   const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
+                   double *dist_out, double *Z_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_link_batch");
+    const std::string who("vbx_link_batch");
+    int rc = check_problem_sizes(h, who, G, M);
+    if (rc != VBX_OK) return rc;
+    if (N < 0) return fail(h, VBX_ERR_ARG, who + ": N < 0");
+    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, who + ": R must lie in [1, 128]");
+    if (G > 0 && (!Fa || !Fb)) return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    std::vector<double> c(G);
+    int64_t total = 0, largest = 0;
+    for (int32_t g = 0; g < G; ++g) {
+        c[g] = Fa[g] / Fb[g];
+        if (!(c[g] >= 0.0) || c[g] == INFINITY)
+            return fail(h, VBX_ERR_ARG, who + ": Fa[" + std::to_string(g) + "] / Fb[" + std::to_string(g) +
+                                            "] must be finite and >= 0");
+        total += M[g];
+        largest = std::max(largest, M[g]);
+    }
+    if (total == 0) return VBX_OK;
+    if (!Phi || !speaker_rec || !workspace || (N > 0 && (!fea || !speaker)) || (largest >= 2 && !Z_out))
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
+    if (workspace_bytes < vbx::link_batch_workspace_bytes(G, M))
+        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_link_batch_workspace_bytes()");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_link_batch(fea, Phi, speaker, N, R, speaker_rec, G, M, c.data(), workspace, n_out,
+                                             F_out, dist_out, Z_out, (cudaStream_t)stream), "link_batch");
+}
+
 int vbx_enroll_workspace_bytes(vbx_handle_t h, int64_t M, int64_t E, int64_t max_k, size_t *bytes_out) {
     if (!h || !bytes_out) return VBX_ERR_ARG;
     if (M < 0 || E < 1 || max_k < 0 || max_k > M)

@@ -246,15 +246,22 @@ int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const
 size_t ahc_workspace_bytes(const int64_t *offsets_host, int n_rec, std::vector<int64_t> *d_off_host);
 int launch_ahc(const Plan &pl, const std::vector<int64_t> &d_off, const void *x, int x_is_f64, int dim, void *workspace,
                size_t workspace_bytes, double *Z_out, double *thr_out, cudaStream_t st, std::string *err);
-// ahc_linkage_kernel as one CTA over the recording described by the DEVICE arrays offsets [2] and d_off [1]; its region
-// of ws (linkage_workspace_bytes(T) bytes, the T x T distances first) is laid out as vbx_ahc's
+// ahc_linkage_kernel with one CTA per problem over the n problems described by the DEVICE arrays offsets [n+1] and
+// d_off [n]; problem b's region of ws (linkage_workspace_bytes(T_b) bytes at d_off[b], the T_b x T_b distances first) is
+// laid out as vbx_ahc's, and its Z rows start at row offsets[b] of Z_out
 size_t linkage_workspace_bytes(int64_t T);
-void launch_linkage(const int64_t *offsets, const int64_t *d_off, void *ws, double *Z_out, cudaStream_t st);
+void launch_linkage(const int64_t *offsets, const int64_t *d_off, int n, void *ws, double *Z_out, cudaStream_t st);
 // speaker linking across recordings (vbx_link.cu)
 size_t link_workspace_bytes(int64_t M);
 int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
                 int64_t M, double c, void *workspace, double *n_out, double *F_out, double *dist_out, double *Z_out,
                 cudaStream_t st, const double *mean = nullptr, const double *std = nullptr);
+// G linking problems in one set of launches (vbx_link_batch): M_host [G] speakers and c_host [G] = Fa_g / Fb_g on the
+// HOST; lk_off (when not null) gets the byte offsets [G+1] of the problems' linkage regions
+size_t link_batch_workspace_bytes(int G, const int64_t *M_host, std::vector<int64_t> *lk_off = nullptr);
+int launch_link_batch(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
+                      int G, const int64_t *M_host, const double *c_host, void *workspace, double *n_out,
+                      double *F_out, double *dist_out, double *Z_out, cudaStream_t st);
 // vbx_link's span and statistics kernels over M speakers into caller-owned DEVICE arrays (n, e [M], b [M, kMaxR]
 // float64; first, last [M] and offs [4] int64 scratch): n_s, F_s, b_s and e_s exactly as vbx_link computes them.
 // Returns the number of launches, -1 on a launch error.

@@ -11,8 +11,14 @@
 //   link_score_kernel   the M x M distances, 32 x 32 tiles of the upper triangle, each written twice
 //   norm_scores_kernel  (vbx_cohort.cu) only with cohort statistics (vbx_link_norm): d = -S in place, section 5.17
 //   ahc_linkage_kernel  (vbx_ahc.cu) unchanged, over the matrix as one "recording" of M items
+// Batched (vbx_link_batch, section 5.18): G independent problems over one fea / Phi, each with its own speaker index
+// [G, N], speaker_rec slice and c_g.  Their speakers are packed by the offsets off [G+1]; the statistics kernels run one
+// CTA per (problem, speaker), the score kernel's flat tile index runs over the upper-triangle tiles of all problems, and
+// one linkage launch has one CTA per problem.  vbx_link is the G = 1 case of the same kernels (LinkProblems with null
+// arrays), so a problem's results do not depend on the others.
 #include <algorithm>
 #include <climits>
+#include <cstring>
 
 #include "vbx_internal.cuh"
 
@@ -23,23 +29,45 @@ namespace {
 constexpr double kBig = 1.0e30;            // cannot-link distance: finite (scipy and the linkage stop at non-finite ones)
 constexpr int kStatsThreads = 256;
 constexpr int kStatsPhases = kStatsThreads / 32;   // x-vector t = first + k, first + k + 8, ... makes phase k
-constexpr int kLogGroup = 8;
-constexpr int64_t kScoreGrid = 1 << 20;    // CTAs of link_score_kernel at most; beyond that they stride over the tiles               // log of a product of 8 denominators: each is 1 + c n Phi, so no overflow
+constexpr int kLogGroup = 8;               // log of a product of 8 denominators: each is 1 + c n Phi, so no overflow
+constexpr int64_t kScoreGrid = 1 << 20;    // CTAs of link_score_kernel at most; beyond that they stride over the tiles
 
 struct LinkWs {
-    uint8_t *lk;             // the linkage's region (carve() in vbx_ahc.cu): D [M,M] first
-    double *n, *e, *b;       // [M], [M], [M,kMaxR]
+    uint8_t *lk;             // the linkage regions (carve() in vbx_ahc.cu), each D [M_g,M_g] first
+    double *n, *e, *b;       // [M], [M], [M,kMaxR]  (M: the speakers of all problems)
     long long *first, *last; // [M]
-    int64_t *offs;           // {0, M} and {0, 0}: the linkage's offsets and workspace offsets
+    int64_t *offs;           // the problem arrays of LinkProblems (G = 1: {0, M} and {0, 0}, the linkage's offsets and
+                             // workspace offsets)
+};
+
+// The problems of one call.  G = 1 with null arrays: one problem of M speakers with c = c0 (vbx_link, and the statistics
+// of vbx_enroll / vbx_cohort_stats); the kernels then read no problem arrays.
+struct LinkProblems {
+    int G;
+    int64_t M, N;            // speakers of all problems; x-vectors (speaker index [G, N])
+    const int64_t *off;      // [G+1] speaker offsets (the linkage's offsets)
+    const int64_t *lk_off;   // [G+1] byte offsets of the linkage regions in lk (the linkage's workspace offsets)
+    const int64_t *tile_off; // [G+1] first flat score tile of each problem
+    const int64_t *dist_off; // [G+1] first element of each problem's distances in dist_out
+    const double *c;         // [G] Fa_g / Fb_g
+    double c0;
 };
 
 size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
 
-LinkWs link_layout(uint8_t *ws, int64_t M, size_t *total) {
+size_t problem_array_bytes(int64_t G) { return (size_t)(5 * G + 4) * 8; }   // off, lk_off, tile_off, dist_off, c
+
+__host__ __device__ int64_t score_tiles(int64_t M) {
+    const int64_t tiles = (M + 31) / 32;
+    return tiles * (tiles + 1) / 2;
+}
+
+// lk_bytes: the linkage regions of all problems (each al(linkage_workspace_bytes(M_g))), M: their speakers
+LinkWs link_layout(uint8_t *ws, size_t lk_bytes, int64_t M, int64_t G, size_t *total) {
     LinkWs w;
     size_t o = 0;
     w.lk = ws;
-    o += al(linkage_workspace_bytes(M));
+    o += lk_bytes;
     w.n = reinterpret_cast<double *>(ws + o);
     o += al((size_t)M * 8);
     w.e = reinterpret_cast<double *>(ws + o);
@@ -51,52 +79,81 @@ LinkWs link_layout(uint8_t *ws, int64_t M, size_t *total) {
     w.last = reinterpret_cast<long long *>(ws + o);
     o += al((size_t)M * 8);
     w.offs = reinterpret_cast<int64_t *>(ws + o);
-    o += al(4 * 8);
+    o += al(problem_array_bytes(G));
     if (total) *total = o;
     return w;
 }
 
-__global__ void link_init_kernel(LinkWs w, int64_t M) {
+// The problem g whose range [pref[g], pref[g+1]) holds x, for non-decreasing pref with pref[0] = 0 <= x < pref[G]:
+// the largest g with pref[g] <= x (never an empty problem's, whose range is empty).
+__device__ __forceinline__ int find_problem(const int64_t *__restrict__ pref, int G, int64_t x) {
+    int lo = 0, hi = G;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (pref[mid] <= x) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
+__global__ void link_init_kernel(LinkWs w, LinkProblems p) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < M) {
+    if (i < p.M) {
         w.first[i] = LLONG_MAX;
         w.last[i] = -1;
     }
-    if (i == 0) {
+    if (i == 0 && !p.off) {
         w.offs[0] = 0;
-        w.offs[1] = M;
+        w.offs[1] = p.M;
         w.offs[2] = 0;
         w.offs[3] = 0;
     }
 }
 
-__global__ void link_span_kernel(LinkWs w, const int32_t *__restrict__ spk, int64_t N, int64_t M) {
-    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= N) return;
-    const int s = spk[t];
+// One thread per (problem, x-vector); speaker[g, t] is a local index of problem g.
+__global__ void link_span_kernel(LinkWs w, LinkProblems p, const int32_t *__restrict__ spk) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (int64_t)p.G * p.N) return;
+    const int s = spk[i];
+    int64_t t = i, base = 0, M = p.M;
+    if (p.off) {
+        const int64_t g = i / p.N;
+        t = i - g * p.N;
+        base = p.off[g];
+        M = p.off[g + 1] - base;
+    }
     if (s < 0 || s >= M) return;
-    atomicMin(&w.first[s], (long long)t);
-    atomicMax(&w.last[s], (long long)t);
+    atomicMin(&w.first[base + s], (long long)t);
+    atomicMax(&w.last[base + s], (long long)t);
 }
 
 // One CTA per speaker over its span first .. last.  Warp k sums phase k of the span sequentially (lane = feature,
 // 4 features per lane), then the 8 phase sums are added in phase order: the order depends on the positions of the
-// speaker's x-vectors relative to its first one, not on the batch, the launch or the other speakers.
-__global__ void __launch_bounds__(kStatsThreads) link_stats_kernel(LinkWs w, const float *__restrict__ fea,
+// speaker's x-vectors relative to its first one, not on the batch, the launch, the problem or the other speakers.
+// CTA s is speaker s of all problems: local speaker s - off[g] of problem g.
+__global__ void __launch_bounds__(kStatsThreads) link_stats_kernel(LinkWs w, LinkProblems p, const float *__restrict__ fea,
                                                                    const float *__restrict__ Phi,
-                                                                   const int32_t *__restrict__ spk, int R, double c,
+                                                                   const int32_t *__restrict__ spk, int R,
                                                                    double *__restrict__ n_out, double *__restrict__ F_out) {
     __shared__ double part[kStatsPhases][kMaxR];
     __shared__ double cnt[kStatsPhases];
     __shared__ double red[kStatsThreads / 32];
     const int s = blockIdx.x;
+    int ls = s;
+    double c = p.c0;
+    if (p.off) {
+        const int g = find_problem(p.off, p.G, s);
+        ls = s - (int)p.off[g];
+        spk += (int64_t)g * p.N;
+        c = p.c[g];
+    }
     const int k = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long f = w.first[s], l = w.last[s];
     double acc[kMaxR / 32] = {0, 0, 0, 0};
     double m = 0.0;
     if (l >= 0) {
         for (long long t = f + k; t <= l; t += kStatsPhases) {
-            if (spk[t] != s) continue;
+            if (spk[t] != ls) continue;
             m += 1.0;
             const float *x = fea + (int64_t)t * R;
 #pragma unroll
@@ -208,17 +265,35 @@ __device__ __forceinline__ void score_tile(const LinkWs &w, const float *__restr
     __syncthreads();                                  // the CTA's next tile rewrites the shared arrays
 }
 
-__global__ void __launch_bounds__(256) link_score_kernel(LinkWs w, const float *__restrict__ Phi,
-                                                         const int32_t *__restrict__ spk_rec, int64_t M, int R, double c,
+// The flat tile index t runs over the tiles of all problems, tile_off[g] .. tile_off[g+1] - 1 being problem g's, so the
+// grid stays one-dimensional and capped for any G and M_g.
+__global__ void __launch_bounds__(256) link_score_kernel(LinkWs w, LinkProblems p, const float *__restrict__ Phi,
+                                                         const int32_t *__restrict__ spk_rec, int R,
                                                          double *__restrict__ dist_out) {
-    const int64_t tiles = (M + 31) / 32, n_tiles = tiles * (tiles + 1) / 2;
-    const double tt = 2.0 * (double)tiles + 1.0;
-    auto row0 = [tiles](int64_t b) { return b * tiles - b * (b - 1) / 2; };   // first tile of row b
-    for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        int64_t bi = (int64_t)((tt - sqrt(tt * tt - 8.0 * (double)t)) / 2.0);  // row0 inverted, then rounding corrected
-        while (bi > 0 && row0(bi) > t) --bi;
-        while (bi + 1 < tiles && row0(bi + 1) <= t) ++bi;
-        score_tile(w, Phi, spk_rec, M, R, c, dist_out, bi, bi + (t - row0(bi)));
+    const int64_t all = p.tile_off ? p.tile_off[p.G] : score_tiles(p.M);
+    for (int64_t t = blockIdx.x; t < all; t += gridDim.x) {
+        LinkWs wg = w;
+        int64_t M = p.M, lt = t, base = 0;
+        double c = p.c0, *dist = dist_out;
+        if (p.tile_off) {
+            const int g = find_problem(p.tile_off, p.G, t);
+            base = p.off[g];
+            M = p.off[g + 1] - base;
+            lt = t - p.tile_off[g];
+            c = p.c[g];
+            wg.lk += p.lk_off[g];
+            wg.n += base;
+            wg.e += base;
+            wg.b += base * kMaxR;
+            if (dist) dist += p.dist_off[g];
+        }
+        const int64_t tiles = (M + 31) / 32;
+        const double tt = 2.0 * (double)tiles + 1.0;
+        auto row0 = [tiles](int64_t b) { return b * tiles - b * (b - 1) / 2; };   // first tile of row b
+        int64_t bi = (int64_t)((tt - sqrt(tt * tt - 8.0 * (double)lt)) / 2.0);   // row0 inverted, then rounding corrected
+        while (bi > 0 && row0(bi) > lt) --bi;
+        while (bi + 1 < tiles && row0(bi + 1) <= lt) ++bi;
+        score_tile(wg, Phi, spk_rec + base, M, R, c, dist, bi, bi + (lt - row0(bi)));
     }
 }
 
@@ -226,27 +301,65 @@ __global__ void __launch_bounds__(256) link_score_kernel(LinkWs w, const float *
 
 size_t link_workspace_bytes(int64_t M) {
     size_t total = 0;
-    link_layout(nullptr, M, &total);
+    link_layout(nullptr, al(linkage_workspace_bytes(M)), M, 1, &total);
     return total;
 }
+
+size_t link_batch_workspace_bytes(int G, const int64_t *M_host, std::vector<int64_t> *lk_off) {
+    size_t lk = 0, total = 0;
+    int64_t M = 0;
+    if (lk_off) lk_off->assign(G + 1, 0);
+    for (int g = 0; g < G; ++g) {
+        if (lk_off) (*lk_off)[g] = (int64_t)lk;
+        lk += al(linkage_workspace_bytes(M_host[g]));
+        M += M_host[g];
+    }
+    if (lk_off) (*lk_off)[G] = (int64_t)lk;
+    link_layout(nullptr, lk, M, G, &total);
+    return total;
+}
+
+namespace {
+
+// The statistics (and, with Z_out or dist_out, the distances) of the problems p over the workspace w.
+int launch_problems(const LinkWs &w, const LinkProblems &p, int64_t n_tiles, const float *fea, const float *Phi,
+                    const int32_t *spk, int R, const int32_t *spk_rec, double *n_out, double *F_out, double *dist_out,
+                    bool score, cudaStream_t st) {
+    int launches = 2;
+    link_init_kernel<<<(unsigned)((p.M + 255) / 256), 256, 0, st>>>(w, p);
+    if (p.N > 0) {
+        link_span_kernel<<<(unsigned)(((int64_t)p.G * p.N + 255) / 256), 256, 0, st>>>(w, p, spk);
+        ++launches;
+    }
+    link_stats_kernel<<<(unsigned)p.M, kStatsThreads, 0, st>>>(w, p, fea, Phi, spk, R, n_out, F_out);
+    if (score && n_tiles > 0) {
+        link_score_kernel<<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(w, p, Phi, spk_rec, R,
+                                                                                           dist_out);
+        ++launches;
+    }
+    return launches;
+}
+
+LinkProblems single(int64_t M, int64_t N, double c) {
+    LinkProblems p;
+    p.G = 1;
+    p.M = M;
+    p.N = N;
+    p.off = p.lk_off = p.tile_off = p.dist_off = nullptr;
+    p.c = nullptr;
+    p.c0 = c;
+    return p;
+}
+
+}  // namespace
 
 int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
                 int64_t M, double c, void *workspace, double *n_out, double *F_out, double *dist_out, double *Z_out,
                 cudaStream_t st, const double *mean, const double *std) {
     if (M == 0) return 0;
-    const LinkWs w = link_layout(reinterpret_cast<uint8_t *>(workspace), M, nullptr);
-    int launches = 0;
-    link_init_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(w, M);
-    ++launches;
-    if (N > 0) {
-        link_span_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(w, spk, N, M);
-        ++launches;
-    }
-    link_stats_kernel<<<(unsigned)M, kStatsThreads, 0, st>>>(w, fea, Phi, spk, R, c, n_out, F_out);
-    const int64_t tiles = (M + 31) / 32, n_tiles = tiles * (tiles + 1) / 2;
-    link_score_kernel<<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(w, Phi, spk_rec, M, R, c,
-                                                                                        mean ? nullptr : dist_out);
-    launches += 2;
+    const LinkWs w = link_layout(reinterpret_cast<uint8_t *>(workspace), al(linkage_workspace_bytes(M)), M, 1, nullptr);
+    int launches = launch_problems(w, single(M, N, c), score_tiles(M), fea, Phi, spk, R, spk_rec, n_out, F_out,
+                                   mean ? nullptr : dist_out, true, st);
     if (mean) {                                       // normalised distances (section 5.17): dist_out gets those
         const int ln = launch_norm_scores(reinterpret_cast<double *>(w.lk), M, M, mean, std, mean, std, true, kBig,
                                           dist_out, st);
@@ -254,7 +367,47 @@ int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t 
         launches += ln;
     }
     if (M >= 2) {
-        launch_linkage(w.offs, w.offs + 2, w.lk, Z_out, st);
+        launch_linkage(w.offs, w.offs + 2, 1, w.lk, Z_out, st);
+        ++launches;
+    }
+    return cudaGetLastError() == cudaSuccess ? launches : -1;
+}
+
+int launch_link_batch(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
+                      int G, const int64_t *M_host, const double *c_host, void *workspace, double *n_out,
+                      double *F_out, double *dist_out, double *Z_out, cudaStream_t st) {
+    std::vector<int64_t> lk_off;
+    link_batch_workspace_bytes(G, M_host, &lk_off);
+    // the problem arrays: off, lk_off, tile_off, dist_off [G+1] and c [G], uploaded in one copy
+    std::vector<int64_t> host(5 * (size_t)G + 4, 0);
+    int64_t *off = host.data(), *tile = off + 2 * (G + 1), *dist = off + 3 * (G + 1);
+    bool linkage = false;
+    for (int g = 0; g < G; ++g) {
+        off[g + 1] = off[g] + M_host[g];
+        tile[g + 1] = tile[g] + score_tiles(M_host[g]);
+        dist[g + 1] = dist[g] + M_host[g] * M_host[g];
+        linkage = linkage || M_host[g] >= 2;
+    }
+    std::copy(lk_off.begin(), lk_off.end(), host.begin() + (G + 1));
+    std::memcpy(host.data() + 4 * (G + 1), c_host, (size_t)G * sizeof(double));
+    const int64_t M = off[G];
+    if (M == 0) return 0;
+    const LinkWs w = link_layout(reinterpret_cast<uint8_t *>(workspace), (size_t)lk_off[G], M, G, nullptr);
+    if (cudaMemcpyAsync(w.offs, host.data(), host.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st) != cudaSuccess)
+        return -1;
+    LinkProblems p;
+    p.G = G;
+    p.M = M;
+    p.N = N;
+    p.off = w.offs;
+    p.lk_off = w.offs + (G + 1);
+    p.tile_off = w.offs + 2 * (G + 1);
+    p.dist_off = w.offs + 3 * (G + 1);
+    p.c = reinterpret_cast<const double *>(w.offs + 4 * (G + 1));
+    p.c0 = 0.0;
+    int launches = launch_problems(w, p, tile[G], fea, Phi, spk, R, spk_rec, n_out, F_out, dist_out, true, st);
+    if (linkage) {
+        launch_linkage(p.off, p.lk_off, G, w.lk, Z_out, st);
         ++launches;
     }
     return cudaGetLastError() == cudaSuccess ? launches : -1;
@@ -271,13 +424,8 @@ int launch_speaker_stats(const float *fea, const float *Phi, const int32_t *spk,
     w.first = s.first;
     w.last = s.last;
     w.offs = s.offs;
-    int launches = 2;
-    link_init_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(w, M);
-    if (N > 0) {
-        link_span_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(w, spk, N, M);
-        ++launches;
-    }
-    link_stats_kernel<<<(unsigned)M, kStatsThreads, 0, st>>>(w, fea, Phi, spk, R, c, n_out, F_out);
+    const int launches = launch_problems(w, single(M, N, c), 0, fea, Phi, spk, R, nullptr, n_out, F_out, nullptr, false,
+                                         st);
     return cudaGetLastError() == cudaSuccess ? launches : -1;
 }
 

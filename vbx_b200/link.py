@@ -121,6 +121,91 @@ def link_speakers(fea, Phi, offsets, labels, Fa, Fb, device=None, dist=False, no
     return out
 
 
+def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_bytes=None, dist=False):
+    """link_speakers for G independent problems over the same features in few launches (vbx_link_batch, DESIGN.md
+    section 5.18), e.g. the final labels of every setting of a sweep.  fea, Phi, offsets: as for link_speakers;
+    labels_per_problem: G lists of first labels per recording; Fa, Fb: numbers or G values, problem g's scalars.
+    The problems are packed in order into launches whose workspaces stay within max_bytes (None: one launch), each
+    problem sized by vbx_link_workspace_bytes (sweep.pack: a problem larger than max_bytes on its own raises ValueError).
+    Returns one (table, n, F, Z) per problem (with dist=True also dist [M,M]), bit-identical to link_speakers on that
+    problem alone."""
+    import torch
+    from . import _lib
+    from ._lib import VbxError
+    from .sweep import pack
+    G = len(labels_per_problem)
+    Fa, Fb = (np.broadcast_to(np.asarray(v, dtype=np.float64), (G,)).copy() for v in (Fa, Fb))
+    offsets = np.asarray(offsets, dtype=np.int64)
+    tables = [speaker_table(l) for l in labels_per_problem]
+    Ms = [len(t.rec) for t in tables]
+    for g, M in enumerate(Ms):
+        if M > _lib.LINK_MAX_SPEAKERS:
+            raise ValueError(f'problem {g}: {M} speakers to link: at most {_lib.LINK_MAX_SPEAKERS} are supported')
+    if not torch.cuda.is_available():
+        raise VbxError('link_many(): no CUDA device - vbx_b200 has no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    fea = torch.as_tensor(fea).to(dev, torch.float32).contiguous()
+    Phi = torch.as_tensor(Phi).to(dev, torch.float32).contiguous()
+    N, R = int(fea.shape[0]), int(fea.shape[1])
+    for labels in labels_per_problem:
+        if int(offsets[-1]) != N or len(offsets) != len(labels) + 1:
+            raise ValueError('offsets must hold one more entry than labels and end at the number of x-vectors')
+    lib = _lib.load()
+    h = ctypes.c_void_p()
+    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
+        raise VbxError('vbx_create failed: no usable sm_90 device')
+    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+    out = [None] * G
+    try:
+        sizes = []
+        for M in Ms:
+            need = ctypes.c_size_t()
+            if lib.vbx_link_workspace_bytes(h, M, ctypes.byref(need)) != 0:
+                raise VbxError(f'vbx_link_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
+            sizes.append(int(need.value))
+        batches = [list(range(G))] if max_bytes is None else pack(sizes, max_bytes)
+        with torch.cuda.device(dev):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            for idx in batches:
+                if not idx:
+                    continue
+                M_h = np.array([Ms[g] for g in idx], dtype=np.int64)
+                tot = int(M_h.sum())
+                spk = np.stack([speaker_index(offsets, labels_per_problem[g])[0] for g in idx]).astype(np.int32)
+                rec = np.concatenate([tables[g].rec for g in idx]).astype(np.int32)
+                fa, fb = np.ascontiguousarray(Fa[idx]), np.ascontiguousarray(Fb[idx])
+                need = ctypes.c_size_t()
+                if lib.vbx_link_batch_workspace_bytes(h, len(idx), M_h.ctypes.data_as(ctypes.c_void_p),
+                                                      ctypes.byref(need)) != 0:
+                    raise VbxError(f'vbx_link_batch_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
+                ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=dev)
+                spk_d = torch.from_numpy(spk).to(dev)
+                rec_d = torch.from_numpy(rec).to(dev)
+                n = torch.empty(tot, dtype=torch.float64, device=dev)
+                F = torch.empty((tot, R), dtype=torch.float64, device=dev)
+                D = torch.empty(int((M_h * M_h).sum()), dtype=torch.float64, device=dev) if dist else None
+                Z = torch.empty((tot, 4), dtype=torch.float64, device=dev)
+                rc = lib.vbx_link_batch(h, p(fea), p(Phi), N, R, len(idx), p(spk_d), M_h.ctypes.data_as(ctypes.c_void_p),
+                                        p(rec_d), fa.ctypes.data_as(ctypes.c_void_p), fb.ctypes.data_as(ctypes.c_void_p),
+                                        p(ws), ws.numel(), p(n), p(F), p(D), p(Z), stream)
+                if rc != 0:
+                    raise VbxError(f'vbx_link_batch failed ({rc}): {lib.vbx_last_error(h).decode()}')
+                n, F, Z = n.cpu().numpy(), F.cpu().numpy(), Z.cpu().numpy()
+                D = D.cpu().numpy() if dist else None
+                o = d = 0
+                for g, M in zip(idx, M_h.tolist()):
+                    out[g] = (tables[g], n[o:o + M], F[o:o + M], Z[o:o + max(M - 1, 0)])
+                    if dist:
+                        out[g] += (D[d:d + M * M].reshape(M, M),)
+                    o += M
+                    d += M * M
+    finally:
+        lib.vbx_destroy(h)
+    return out
+
+
 def link_cut(Z, table, threshold, labels2=None):
     """Archive-wide speaker ids from the linkage Z of table's speakers: speakers whose average LLR is at least
     `threshold` share an id (ahc.flat_clusters(Z, -threshold)); ids are numbered by first appearance over the table.

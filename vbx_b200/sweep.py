@@ -23,6 +23,12 @@ With --num-speakers (an integer, a 'recording count' file, or oracle: the refere
 --min-speakers / --max-speakers, every setting holds each recording to that speaker count (DESIGN.md section 5.14):
 summary.json gains count_rule and speakers_vb per recording and setting, and count_rules per setting (how many
 recordings took each rule).
+With --link-threshold LIST (comma-separated LLR thresholds, the --option=list form when the list starts with '-') the
+speakers of every setting are linked across the archive (DESIGN.md sections 5.15 and 5.18): all settings in one batched
+vbx_link_batch call, every threshold a host cut of the setting's linkage.  summary.json then gains linked = {threshold:
+global_speakers per recording[, der_across_files][, der_across_files_overlap]} per setting and, with a reference,
+ranking_across_files (and ranking_across_files_overlap): per protocol, the names <setting>_link<threshold> by DER across
+files.  No linked RTTM files are written: the maps and cli --link-threshold at the chosen setting reproduce them.
 """
 import argparse
 import itertools
@@ -134,7 +140,8 @@ def packer(lens, R, device, budget):
 
 def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
                 device=None, max_batch_bytes=None, output_2nd=False, ref_rttm=None, uem=None, overlaps=None,
-                oracle_overlaps=False, jer=False, num_speakers=None, min_speakers=None, max_speakers=None):
+                oracle_overlaps=False, jer=False, num_speakers=None, min_speakers=None, max_speakers=None,
+                link_thresholds=None):
     """Every setting of `grid` (see grid_settings) for every recording, with the front end and AHC run once.
 
     recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
@@ -158,15 +165,23 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     speakers with scored time (needs ref_rttm; inside the UEM when one is given).  Every (recording, setting) entry then
     follows the rules of DESIGN.md section 5.14 and its dict gains count_rule, n_speakers_vb and count.  The re-runs of
     rule 3 of all settings are packed into batches per state tier like the first pass.
+    link_thresholds: None, or LLR thresholds for speaker linking across the archive (DESIGN.md sections 5.15 and 5.18;
+    each checked by link.check_threshold before any device work, duplicates dropped).  The final first labels of every
+    setting are linked in one link.link_many call within max_batch_bytes, and each threshold is a host cut of the
+    setting's linkage (link.link_cut, second labels as diarize_batch handles them).  Each recording's dict gains
+    global_speakers = {threshold: {label: global id}}, equal to diarize_batch(link_threshold=threshold)'s with that
+    setting's scalars; with a reference also ref_speakers (the reference speaker names, in the rows of the blocks) and
+    der_blocks = {protocol: overlap block} (with overlaps der_overlap_blocks too), what summarize_across_files needs.
     Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags[, der][, rttm_overlap,
-    overlap_seconds][, der_overlap][, count_rule, n_speakers_vb, count])}}; each recording's dict is the one
-    diarize_batch returns with that setting's scalars."""
+    overlap_seconds][, der_overlap][, count_rule, n_speakers_vb, count][, global_speakers][, ref_speakers, der_blocks
+    [, der_overlap_blocks]])}}; each recording's dict is the one diarize_batch returns with that setting's scalars."""
     import torch
     from . import ahc as _ahc
     from ._lib import VbxError
     from .parts import make_batch
     from .pipeline import _check_init, _count_fields, _front_end, _pad_features, _result, _vb_stage, count_bounds
     settings = grid_settings(grid)
+    links = check_link_thresholds(link_thresholds)
     with_overlap = oracle_overlaps or overlaps is not None
     _check_init(init, with_overlap)
     if oracle_overlaps and ref_rttm is None:
@@ -211,6 +226,14 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     res = _vb_stage([(s.Fa, s.Fb, s.loopP, s.smoothing) for s in settings], [ahc_labels[s.threshold] for s in settings],
                     [lab_d[s.threshold] for s in settings], Zs, lens, fea, Phi, bounds, init, dev, make_batch,
                     packer(lens, int(fea.shape[1]), dev, max_batch_bytes), maxIters=max_iters, epsilon=epsilon)
+    maps = None
+    if links is not None:
+        from . import link
+        labels = [[res[(k, b)][0] for b in range(len(names))] for k in range(len(settings))]
+        linked = link.link_many(fea, Phi, np.concatenate([[0], np.cumsum(lens)]), labels, [s.Fa for s in settings],
+                                [s.Fb for s in settings], dev, max_batch_bytes)
+        maps = [{t: link.link_cut(Z, table, t, [res[(k, b)][1] for b in range(len(names))]) for t in links}
+                for k, (table, _, _, Z) in enumerate(linked)]
     from . import score
     ovl = [None] * len(names)
     if with_overlap:
@@ -218,7 +241,7 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
                for n in names]
     der = der_ovl = None
     if ref is not None:
-        turns, uem_map = ref
+        turns, uem_map = ref[:2]
         scored = []
         for n, o in zip(names, ovl):
             timeline = score.owned_intervals(recordings[n][1])
@@ -226,10 +249,12 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
                                                   overlap=o))
         keys = [(k, b) for k in range(len(settings)) for b in range(len(names))]
         jp = 'full' if jer else None
-        der = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0]) for k, b in keys], device=dev, jer=jp)))
+        blk = maps is not None
+        der = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0]) for k, b in keys], device=dev, jer=jp,
+                                                 blocks=blk)))
         if with_overlap:
             der_ovl = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0], res[(k, b)][1]) for k, b in keys],
-                                                         device=dev, jer=jp)))
+                                                         device=dev, jer=jp, blocks=blk)))
     out = {}
     for k, s in enumerate(settings):
         out[s] = {}
@@ -240,23 +265,44 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
             if bounds is not None:
                 _count_fields(item, *res[(k, b)][4:6], bounds[0][b], bounds[1][b])
             if der is not None:
-                item['der'] = {p: v for p, v in der[(k, b)].items() if p != 'jer'}
+                item['der'] = {p: v for p, v in der[(k, b)].items() if p not in ('jer', 'O')}
                 if jer:
                     item['jer'] = der[(k, b)]['jer']
             if der_ovl is not None:
-                item['der_overlap'] = {p: v for p, v in der_ovl[(k, b)].items() if p != 'jer'}
+                item['der_overlap'] = {p: v for p, v in der_ovl[(k, b)].items() if p not in ('jer', 'O')}
                 if jer:
                     item['jer_overlap'] = der_ovl[(k, b)]['jer']
+            if maps is not None:
+                item['global_speakers'] = {t: maps[k][t][b] for t in links}
+                if der is not None:
+                    item['ref_speakers'] = ref[2][n]
+                    item['der_blocks'] = der[(k, b)]['O']
+                    if der_ovl is not None:
+                        item['der_overlap_blocks'] = der_ovl[(k, b)]['O']
             out[s][n] = item
     return out
 
 
+def check_link_thresholds(thresholds):
+    """None, or the link thresholds as floats without duplicates (first occurrence kept).  A threshold that
+    link.check_threshold refuses, or an empty list, raises ValueError."""
+    if thresholds is None:
+        return None
+    from .link import check_threshold
+    out = list(dict.fromkeys(check_threshold(t) for t in thresholds))
+    if not out:
+        raise ValueError('link_thresholds needs at least one value')
+    return out
+
+
 def _load_reference(names, ref_rttm, uem):
-    """-> (score.reference_turns of the recordings `names`, {recording: UEM intervals} or None), checked up front."""
+    """-> (score.reference_turns of the recordings `names`, {recording: UEM intervals} or None, {recording: the
+    reference speaker names in the order of the turns}), checked up front."""
     from . import formats, score
     rows = score.read_rttm_path(ref_rttm) if isinstance(ref_rttm, (str, os.PathLike)) else list(ref_rttm)
     wanted = set(names)
-    turns = score.reference_turns([r for r in rows if r[0] in wanted])
+    named = score.named_reference_turns([r for r in rows if r[0] in wanted])
+    turns = {rec: [t for _, t in spk] for rec, spk in named.items()}
     missing = [n for n in names if n not in turns]
     if missing:
         raise ValueError(f'recordings missing from the reference RTTM: {missing}')
@@ -266,7 +312,7 @@ def _load_reference(names, ref_rttm, uem):
         missing = [n for n in names if n not in uem]
         if missing:
             raise ValueError(f'recordings missing from the UEM: {missing}')
-    return turns, uem
+    return turns, uem, {rec: [k for k, _ in spk] for rec, spk in named.items()}
 
 
 def summarize_der(out, key='der'):
@@ -275,6 +321,54 @@ def summarize_der(out, key='der'):
     from . import score
     tot = {s.name: {p: score.overall([item[key][p] for item in per_rec.values()]) for p, _, _ in score.PROTOCOLS}
            for s, per_rec in out.items()}
+    ranking = {p: score.rank({n: tot[n][p] for n in tot}) for p, _, _ in score.PROTOCOLS}
+    return tot, ranking
+
+
+def link_key(setting, threshold):
+    """The ranking name of a setting linked at a threshold, e.g. Fa0.3_Fb17_loopP0.99_thr-0.015_sm5_link48."""
+    return f'{setting.name}_link{threshold:g}'
+
+
+def across_files_by_id(tot, ref_names, blocks, maps):
+    """DER across files (DESIGN.md section 5.15) of linked output: tot, an overall() result of the files; per file the
+    reference names of its block rows, its overlap block [n_ref, labels] and its {label: global id} map.  The blocks'
+    columns are summed by global id (a label the map lacks has no turns, so its column is empty) and matched once,
+    as score.across_files_result does with RTTM names."""
+    from scipy.optimize import linear_sum_assignment
+    from . import score
+    rows = {k: i for i, k in enumerate(sorted({k for ks in ref_names for k in ks}))}
+    n_ids = 1 + max((g for m in maps for g in m.values()), default=-1)
+    O = np.zeros((len(rows), n_ids), dtype=np.int64)
+    for rk, blk, m in zip(ref_names, blocks, maps):
+        blk = np.asarray(blk, dtype=np.int64)
+        cols = [l for l in range(blk.shape[1]) if l in m]
+        if rk and cols:
+            np.add.at(O, np.ix_([rows[k] for k in rk], [m[l] for l in cols]), blk[:, cols])
+    matched = 0
+    if O.size:
+        r, c = linear_sum_assignment(O, maximize=True)
+        matched = int(O[r, c].sum())
+    t = tot['ticks']
+    return score.result(t['miss'], t['fa'], t['scored'] - t['miss'] - matched, t['scored'])
+
+
+def summarize_across_files(out, key='der'):
+    """sweep_batch(link_thresholds=, ref_rttm=) output with `key` ('der' or 'der_overlap') -> ({link_key(setting,
+    threshold): {protocol: DER across files}}, {protocol: those names by DER across files, stable in grid order, then
+    threshold order}).  Per (setting, threshold) the per-file blocks are summed by global id and matched once
+    (across_files_by_id)."""
+    from . import score
+    tot = {}
+    for s, per_rec in out.items():
+        items = list(per_rec.values())
+        if not items:
+            continue
+        for t in items[0]['global_speakers']:
+            tot[link_key(s, t)] = {
+                p: across_files_by_id(score.overall([it[key][p] for it in items]), [it['ref_speakers'] for it in items],
+                                      [it[key + '_blocks'][p] for it in items], [it['global_speakers'][t] for it in items])
+                for p, _, _ in score.PROTOCOLS}
     ranking = {p: score.rank({n: tot[n][p] for n in tot}) for p, _, _ in score.PROTOCOLS}
     return tot, ranking
 
@@ -313,6 +407,8 @@ def build_parser():
     ap.add_argument('--oracle-overlaps', action='store_true',
                     help="use the reference's overlaps (with --ref-rttm) as the overlap regions")
     ap.add_argument('--jer', action='store_true', help='also score and rank by Jaccard error rate (with --ref-rttm)')
+    ap.add_argument('--link-threshold', default=None, type=parse_list,
+                    help='comma-separated LLR thresholds: link every setting\'s speakers across the archive')
     from .cli import add_count_options
     add_count_options(ap, allow_oracle=True)
     return ap
@@ -336,7 +432,7 @@ def main(argv=None):
                       init=args.init, chain=args.chain, device=args.device, max_batch_bytes=args.max_batch_bytes,
                       ref_rttm=args.ref_rttm, uem=args.uem, overlaps=overlaps, oracle_overlaps=args.oracle_overlaps,
                       jer=args.jer, num_speakers=args.num_speakers, min_speakers=args.min_speakers,
-                      max_speakers=args.max_speakers)
+                      max_speakers=args.max_speakers, link_thresholds=args.link_threshold)
     summary = {}
     for s, per_rec in out.items():
         d = os.path.join(args.out_dir, s.name)
@@ -371,6 +467,18 @@ def main(argv=None):
                 tot, summary['ranking_' + key] = summarize_jer(out, key)
                 for name, d in tot.items():
                     summary[name][key] = d
+    if args.link_threshold is not None:
+        ovl = overlaps is not None or args.oracle_overlaps
+        for s, per_rec in out.items():
+            linked = summary[s.name]['linked'] = {}
+            for t in check_link_thresholds(args.link_threshold):
+                linked[f'{t:g}'] = dict(global_speakers={n: it['global_speakers'][t] for n, it in per_rec.items()})
+        if args.ref_rttm is not None:
+            for key in ('der', 'der_overlap') if ovl else ('der',):
+                tot, summary['ranking_across_files' + key[3:]] = summarize_across_files(out, key)
+                for s in out:
+                    for t in check_link_thresholds(args.link_threshold):
+                        summary[s.name]['linked'][f'{t:g}']['der_across_files' + key[3:]] = tot[link_key(s, t)]
     with open(os.path.join(args.out_dir, 'summary.json'), 'w') as fp:
         json.dump(summary, fp, indent=1, sort_keys=True)
     return 0

@@ -93,3 +93,31 @@ def make_scoring_archive(lengths, seed=0, n_spk=(2, 9), stay=0.97, gap_prob=0.0)
             lab[t] = lab[t - 1] if rng.random() < stay else rng.integers(K)
         out[f'syn{r:02d}'] = (np.stack([start / 100.0, (start + 150) / 100.0], 1).reshape(-1, 2), lab)
     return out
+
+
+def multi_session_archive(x_ref, n_rec=8, pool=10, lengths=(300, 600), speakers=(2, 5), seed=13, stay=0.97):
+    """Seeded recordings whose speakers are drawn from one shared pool, as in an archive of meetings with recurring
+    participants (speaker linking, DESIGN.md sections 5.15 and 5.18).  x_ref [n, D]: real x-vectors whose mean and
+    per-dimension spread place the pool: speaker k's centre is mean + 2 sd * N(0, 1), its x-vectors the centre plus
+    0.5 sd * N(0, 1) noise.  Each recording has lengths[0] .. lengths[1] x-vectors (1.5 s segments every 0.24 s) and
+    speakers[0] .. speakers[1] distinct pool speakers with sticky turns.  Returns (recordings {name: (x [T,D] float64,
+    seg_times [T,2])}, reference rows [(recording, onset, duration, 'p<k>')], one 0.24 s row per x-vector, and the pool
+    index of every x-vector {name: int64 [T]})."""
+    rng = np.random.default_rng(seed)
+    x_ref = np.asarray(x_ref, dtype=np.float64)
+    sd = x_ref.std(0)
+    centres = x_ref.mean(0) + 2.0 * sd * rng.standard_normal((pool, x_ref.shape[1]))
+    recs, rows, truth = {}, [], {}
+    for r in range(n_rec):
+        T = int(rng.integers(lengths[0], lengths[1] + 1))
+        who = rng.choice(pool, int(rng.integers(speakers[0], speakers[1] + 1)), replace=False)
+        spk = np.zeros(T, dtype=np.int64)
+        for t in range(1, T):
+            spk[t] = spk[t - 1] if rng.random() < stay else rng.integers(len(who))
+        x = centres[who[spk]] + 0.5 * sd * rng.standard_normal((T, x_ref.shape[1]))
+        seg = np.stack([np.arange(T) * 0.24, np.arange(T) * 0.24 + 1.5], 1)
+        name = f'ses{r:02d}'
+        recs[name] = (x, seg)
+        truth[name] = who[spk]
+        rows += [(name, round(t * 0.24, 2), 0.24, f'p{k}') for t, k in enumerate(who[spk])]
+    return recs, rows, truth
