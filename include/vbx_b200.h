@@ -277,6 +277,49 @@ int vbx_enroll_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t 
                     double *F_out, double *n_enroll_out, double *F_enroll_out, const double *mean, const double *std,
                     const double *enroll_mean, const double *enroll_std, void *stream);
 
+/* Enrolment, cohort statistics and normalised linking of G independent problems in one set of launches (DESIGN.md
+ * section 5.19), e.g. the settings of a sweep; each needs a handle, no plan.  The problems share fea [N,R] and Phi [R]
+ * (DEVICE); problem g has its row g of speaker [G,N] (DEVICE, local speakers in [0, M[g]), -1 = none), M [G] (HOST)
+ * and Fa [g], Fb [g] (HOST; every c_g = Fa[g] / Fb[g] finite and >= 0).  Per-speaker arrays are packed by the speaker
+ * offsets off_g = M[0] + .. + M[g-1].  Problem g's outputs are bit-identical to the single-problem entry run on it
+ * alone, in one launch or over several.  Stream ordered, no allocation, no host synchronisation: the problems'
+ * offsets and scalars go to the device in one copy from pageable host memory.  VBX_ERR_ARG as for the single entries,
+ * and for G < 0 or more than 2^31 - 1 speakers in all.
+ *
+ * vbx_enroll_batch: vbx_enroll of every problem against the one enrolled set (enroll_fea [N_e,R], enroll_speaker [N_e]
+ * in [0, E), DEVICE) at n_thr >= 1 thresholds (HOST, each |t| <= 1e15).  speaker_rec_offsets [G, n_rec + 1] (HOST):
+ * row g as vbx_enroll's for problem g, from 0 to M[g].  Outputs (DEVICE): assign_out [n_thr, sum M] int32 and
+ * best_llr_out [n_thr, sum M] (plane h: threshold h); optional llr_out [sum M, E], n_out [sum M], F_out [sum M, R],
+ * n_enroll_out [G, E], F_enroll_out [G, E, R].  mean, std [sum M] and enroll_mean, enroll_std [G, E] (DEVICE, all four
+ * or none): the normalised path of vbx_enroll_norm, problem g with its own rows.  workspace:
+ * vbx_enroll_batch_workspace_bytes(G, M, E, N_e, max_k, n_thr) bytes with max_k >= the largest K of any recording of
+ * any problem, 256-byte aligned. */
+int vbx_enroll_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, int64_t E, int64_t N_e,
+                                     int64_t max_k, int32_t n_thr, size_t *bytes_out);
+int vbx_enroll_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                     const int32_t *speaker, const int64_t *M, const int64_t *speaker_rec_offsets, int32_t n_rec,
+                     const float *enroll_fea, int64_t N_e, const int32_t *enroll_speaker, int64_t E, const double *Fa,
+                     const double *Fb, const double *thresholds, int32_t n_thr, void *workspace,
+                     size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
+                     double *F_out, double *n_enroll_out, double *F_enroll_out, const double *mean, const double *std,
+                     const double *enroll_mean, const double *enroll_std, void *stream);
+/* vbx_cohort_stats_batch: vbx_cohort_stats of every problem against one cohort (cohort_fea [N_c,R], cohort_speaker
+ * [N_c] in [0, C), C >= 2, DEVICE), top_k >= 2.  Outputs mean_out, std_out [sum M] (DEVICE).  The enrolled speakers'
+ * statistics per problem come from the same entry with fea = enroll_fea and speaker = enroll_speaker repeated G times.
+ * workspace: vbx_cohort_stats_batch_workspace_bytes(G, M, C, N_c) bytes, 256-byte aligned. */
+int vbx_cohort_stats_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, int64_t C, int64_t N_c,
+                                           size_t *bytes_out);
+int vbx_cohort_stats_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                           const int32_t *speaker, const int64_t *M, const float *cohort_fea, int64_t N_c,
+                           const int32_t *cohort_speaker, int64_t C, const double *Fa, const double *Fb, int32_t top_k,
+                           void *workspace, size_t workspace_bytes, double *mean_out, double *std_out, void *stream);
+/* vbx_link_batch_norm: vbx_link_batch with every problem's distances -S as vbx_link_norm computes them, from mean, std
+ * [sum M] (DEVICE, problem g's at off_g).  Workspace: vbx_link_batch_workspace_bytes. */
+int vbx_link_batch_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                        const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
+                        const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
+                        double *dist_out, double *Z_out, const double *mean, const double *std, void *stream);
+
 /* Float64 evaluation of the same EM loop ("exact" mode for the one-recording-per-call use of VBx/vbhmm.py:154-158,
  * where the reference stops on an ELBO improvement < 1e-6, VBx/vbhmm.py:157 -- below float32 resolution).
  * All arrays float64: fea [N,R] (the reference's X, VBx/VBx.py:30), Phi [R], gamma_io [N,S], pi_io [n_rec,S],

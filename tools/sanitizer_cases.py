@@ -3,7 +3,7 @@ D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings w
 6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels (also under a speaker-count bound),
 the dense forward_backward(), the ELBO trace, DER / JER scoring, speaker linking across recordings (one problem and
 batched), enrolment
-against known speakers and score normalisation against a cohort.
+against known speakers and score normalisation against a cohort (one problem and batched).
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
 """
@@ -138,6 +138,22 @@ c_enr = enroll.enroll_speakers(e_fea, l_phi, e_offs, e_labels, e_x, e_spk, 0.3, 
                                max_bytes=8 * 45 * 100, norm=c_st[:2] + c_en[:2])
 torch.cuda.synchronize()
 print('cohort ok', len(c_st.mean), float(c_st.std.min()), float(c_link[3][:, 2].min()), int((c_enr.assign >= 0).sum()))
+
+# batched enrolment and cohort statistics (vbx_enroll_batch, vbx_cohort_stats_batch, vbx_link_batch_norm): a problem
+# without speakers, one with a speaker per recording and the one with 150 speakers, each with its own Fa / Fb; E = 45 <
+# K_b = 150 and tail tiles; three thresholds; plain and normalised
+eb_labels = [[np.full(n, -1) for n in e_lens], [np.where(np.arange(n) == 0, 0, -1) for n in e_lens], e_labels]
+eb_fa, eb_fb = [0.3, 0.4, 0.2], [17.0, 6.0, 64.0]
+eb_st = cohort.cohort_stats_many(e_fea, l_phi, e_offs, eb_labels, c_x, c_spk, eb_fa, eb_fb, 50, dev)
+eb_en = cohort.cohort_stats_many(e_x, l_phi, None, [e_spk] * 3, c_x, c_spk, eb_fa, eb_fb, 50, dev)
+for eb_norm in (None, [a[:2] + b[:2] for a, b in zip(eb_st, eb_en)]):
+    eb_out = enroll.enroll_many(e_fea, l_phi, e_offs, eb_labels, e_x, e_spk, eb_fa, eb_fb, [-10.0, 0.0, 10.0], dev,
+                                llr=True, norm=eb_norm)
+    torch.cuda.synchronize()
+    print('enroll batch ok', [len(o.table.rec) for o in eb_out], int((eb_out[2].assign >= 0).sum()))
+eb_link = link.link_many(e_fea, l_phi, e_offs, eb_labels, eb_fa, eb_fb, dev, dist=True, norm=[a[:2] for a in eb_st])
+torch.cuda.synchronize()
+print('cohort batch ok', float(eb_st[2].std.min()), float(eb_en[2].std.min()), float(eb_link[2][3][:, 2].min()))
 
 # wgmma projection at the smallest and largest D, one frame and one frame past a full wave of tiles
 sms = torch.cuda.get_device_properties(0).multi_processor_count

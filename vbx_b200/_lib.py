@@ -15,7 +15,9 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace', 'vbx_get_gsum',
            'vbx_score', 'vbx_score_overlap', 'vbx_score_jer', 'vbx_link_workspace_bytes', 'vbx_link',
            'vbx_enroll_workspace_bytes', 'vbx_enroll', 'vbx_cohort_workspace_bytes', 'vbx_cohort_stats', 'vbx_link_norm',
-           'vbx_enroll_norm', 'vbx_link_batch_workspace_bytes', 'vbx_link_batch']
+           'vbx_enroll_norm', 'vbx_link_batch_workspace_bytes', 'vbx_link_batch', 'vbx_link_batch_norm',
+           'vbx_enroll_batch_workspace_bytes', 'vbx_enroll_batch', 'vbx_cohort_stats_batch_workspace_bytes',
+           'vbx_cohort_stats_batch']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
@@ -122,6 +124,18 @@ def load():
     lib.vbx_link_batch_workspace_bytes.argtypes = [vp, i32, vp, ctypes.POINTER(ctypes.c_size_t)]
     lib.vbx_link_batch.restype = ctypes.c_int
     lib.vbx_link_batch.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.c_size_t, vp, vp, vp, vp, vp]
+    lib.vbx_link_batch_norm.restype = ctypes.c_int
+    lib.vbx_link_batch_norm.argtypes = lib.vbx_link_batch.argtypes[:-1] + [vp, vp, vp]
+    lib.vbx_enroll_batch_workspace_bytes.restype = ctypes.c_int
+    lib.vbx_enroll_batch_workspace_bytes.argtypes = [vp, i32, vp, i64, i64, i64, i32, ctypes.POINTER(ctypes.c_size_t)]
+    lib.vbx_enroll_batch.restype = ctypes.c_int
+    lib.vbx_enroll_batch.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, i32, vp, i64, vp, i64, vp, vp, vp, i32, vp,
+                                     ctypes.c_size_t, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.vbx_cohort_stats_batch_workspace_bytes.restype = ctypes.c_int
+    lib.vbx_cohort_stats_batch_workspace_bytes.argtypes = [vp, i32, vp, i64, i64, ctypes.POINTER(ctypes.c_size_t)]
+    lib.vbx_cohort_stats_batch.restype = ctypes.c_int
+    lib.vbx_cohort_stats_batch.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, i64, vp, i64, vp, vp, i32, vp,
+                                           ctypes.c_size_t, vp, vp, vp]
     lib.vbx_get_timings.restype = ctypes.c_int
     lib.vbx_get_timings.argtypes = [vp, ctypes.POINTER(dbl), ctypes.POINTER(i64), i32]
     _lib = lib

@@ -137,3 +137,95 @@ def cohort_stats(fea, Phi, offsets, labels, cohort_fea, cohort_speaker, Fa, Fb, 
     finally:
         lib.vbx_destroy(h)
     return out
+
+
+def cohort_stats_many(fea, Phi, offsets, labels_per_problem, cohort_fea, cohort_speaker, Fa, Fb, top_k=DEFAULT_TOP_K,
+                      device=None, max_bytes=None):
+    """cohort_stats for G independent problems over the same features and cohort in few launches
+    (vbx_cohort_stats_batch, DESIGN.md section 5.19), e.g. the final labels of every setting of a sweep.  fea, Phi,
+    offsets, cohort_fea, cohort_speaker, top_k: as for cohort_stats; labels_per_problem: G label sets as cohort_stats
+    takes them (per recording first labels with offsets, or a speaker index [N] with offsets None); Fa, Fb: numbers or
+    G values.  The enrolled speakers of every setting: fea = the enrolled features, offsets None and their speaker index
+    once per setting.  Launches as enroll_many packs them (max_bytes None: one).  Returns one CohortStats per problem
+    (scores None), bit-identical to cohort_stats on that problem alone."""
+    import torch
+    from . import _lib
+    from ._lib import VbxError
+    from .link import speaker_index
+    from .sweep import pack_by
+    K_req = check_top_k(top_k)
+    G = len(labels_per_problem)
+    Fa, Fb = (np.broadcast_to(np.asarray(v, dtype=np.float64), (G,)).copy() for v in (Fa, Fb))
+    cspk = np.asarray(cohort_speaker, dtype=np.int64).reshape(-1)
+    if len(cspk) == 0 or cspk.min() < 0:
+        raise ValueError('cohort_speaker must hold at least one speaker index, all >= 0')
+    C = int(cspk.max()) + 1
+    if C < 2:
+        raise ValueError(f'a cohort needs at least 2 speakers, got {C}')
+    if np.bincount(cspk, minlength=C).min() == 0:
+        raise ValueError('every cohort speaker 0 .. C-1 needs at least one x-vector')
+    spks, Ms = [], []
+    for labels in labels_per_problem:
+        if offsets is None:
+            spk = np.asarray(labels, dtype=np.int64).reshape(-1)
+            M = int(spk.max()) + 1 if len(spk) else 0
+            if M and np.bincount(spk[spk >= 0], minlength=M).min() == 0:
+                raise ValueError('every scored speaker 0 .. M-1 needs at least one x-vector')
+        else:
+            spk, M = speaker_index(offsets, labels)
+        spks.append(spk)
+        Ms.append(M)
+    Ms = np.array(Ms, dtype=np.int64)
+    if not torch.cuda.is_available():
+        raise VbxError('cohort_stats_many(): no CUDA device - vbx_b200 has no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    fea = torch.as_tensor(fea).to(dev, torch.float32).contiguous()
+    Phi = torch.as_tensor(Phi).to(dev, torch.float32).contiguous()
+    cfea = torch.as_tensor(cohort_fea).to(dev, torch.float32).contiguous()
+    N, R = int(fea.shape[0]), int(fea.shape[1])
+    if any(len(s) != N for s in spks):
+        raise ValueError(f'every problem needs one speaker index per x-vector ({N})')
+    if tuple(cfea.shape) != (len(cspk), R):
+        raise ValueError(f'cohort_fea must be [{len(cspk)}, {R}], got {tuple(cfea.shape)}')
+    lib = _lib.load()
+    h = ctypes.c_void_p()
+    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
+        raise VbxError('vbx_create failed: no usable sm_90 device')
+    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+    v = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    out = [None] * G
+
+    def ws_bytes(idx):
+        need = ctypes.c_size_t()
+        M_h = np.ascontiguousarray(Ms[idx])
+        if lib.vbx_cohort_stats_batch_workspace_bytes(h, len(idx), v(M_h), C, len(cspk), ctypes.byref(need)) != 0:
+            raise VbxError(f'vbx_cohort_stats_batch_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
+        return int(need.value)
+    try:
+        batches = pack_by(G, ws_bytes, max_bytes)
+        with torch.cuda.device(dev):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            cspk_d = torch.from_numpy(cspk.astype(np.int32)).to(dev)
+            for idx in batches:
+                M_h = np.ascontiguousarray(Ms[idx])
+                tot = int(M_h.sum())
+                ws = torch.empty(max(ws_bytes(idx), 1), dtype=torch.uint8, device=dev)
+                spk_d = torch.from_numpy(np.stack([spks[g] for g in idx]).astype(np.int32)).to(dev)
+                fa, fb = np.ascontiguousarray(Fa[idx]), np.ascontiguousarray(Fb[idx])
+                mean = torch.empty(tot, dtype=torch.float64, device=dev)
+                std = torch.empty(tot, dtype=torch.float64, device=dev)
+                rc = lib.vbx_cohort_stats_batch(h, p(fea), p(Phi), N, R, len(idx), p(spk_d), v(M_h), p(cfea),
+                                                len(cspk), p(cspk_d), C, v(fa), v(fb), K_req, p(ws), ws.numel(),
+                                                p(mean), p(std), stream)
+                if rc != 0:
+                    raise VbxError(f'vbx_cohort_stats_batch failed ({rc}): {lib.vbx_last_error(h).decode()}')
+                mean, std = mean.cpu().numpy(), std.cpu().numpy()
+                o = 0
+                for g, M in zip(idx, M_h.tolist()):
+                    out[g] = CohortStats(mean[o:o + M], std[o:o + M], min(K_req, C), None)
+                    o += M
+    finally:
+        lib.vbx_destroy(h)
+    return out

@@ -904,25 +904,38 @@ int vbx_link_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, 
     return VBX_OK;
 }
 
-int vbx_link_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
-                   const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
-                   const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
-                   double *dist_out, double *Z_out, void *stream) {
+// c [G] = Fa[g] / Fb[g], each finite and >= 0
+static int problem_scalars(vbx_handle_t h, const std::string &who, int32_t G, const double *Fa, const double *Fb,
+                           std::vector<double> *c) {
+    if (G > 0 && (!Fa || !Fb)) return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    c->assign(G, 0.0);
+    for (int32_t g = 0; g < G; ++g) {
+        (*c)[g] = Fa[g] / Fb[g];
+        if (!((*c)[g] >= 0.0) || (*c)[g] == INFINITY)
+            return fail(h, VBX_ERR_ARG, who + ": Fa[" + std::to_string(g) + "] / Fb[" + std::to_string(g) +
+                                            "] must be finite and >= 0");
+    }
+    return VBX_OK;
+}
+
+// vbx_link_batch and vbx_link_batch_norm (mean, std null for the former)
+static int link_batch_call(vbx_handle_t h, const char *name, const float *fea, const float *Phi, int64_t N, int32_t R,
+                           int32_t G, const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec,
+                           const double *Fa, const double *Fb, void *workspace, size_t workspace_bytes, double *n_out,
+                           double *F_out, double *dist_out, double *Z_out, const double *mean, const double *std,
+                           void *stream) {
     if (!h) return VBX_ERR_ARG;
-    Range nvtx_range("vbx_link_batch");
-    const std::string who("vbx_link_batch");
+    Range nvtx_range(name);
+    const std::string who(name);
     int rc = check_problem_sizes(h, who, G, M);
     if (rc != VBX_OK) return rc;
     if (N < 0) return fail(h, VBX_ERR_ARG, who + ": N < 0");
     if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, who + ": R must lie in [1, 128]");
-    if (G > 0 && (!Fa || !Fb)) return fail(h, VBX_ERR_ARG, who + ": null pointer");
-    std::vector<double> c(G);
+    std::vector<double> c;
+    rc = problem_scalars(h, who, G, Fa, Fb, &c);
+    if (rc != VBX_OK) return rc;
     int64_t total = 0, largest = 0;
     for (int32_t g = 0; g < G; ++g) {
-        c[g] = Fa[g] / Fb[g];
-        if (!(c[g] >= 0.0) || c[g] == INFINITY)
-            return fail(h, VBX_ERR_ARG, who + ": Fa[" + std::to_string(g) + "] / Fb[" + std::to_string(g) +
-                                            "] must be finite and >= 0");
         total += M[g];
         largest = std::max(largest, M[g]);
     }
@@ -935,7 +948,138 @@ int vbx_link_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N
     DeviceGuard guard(h->device);
     if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     return counted(h, vbx::launch_link_batch(fea, Phi, speaker, N, R, speaker_rec, G, M, c.data(), workspace, n_out,
-                                             F_out, dist_out, Z_out, (cudaStream_t)stream), "link_batch");
+                                             F_out, dist_out, Z_out, (cudaStream_t)stream, mean, std), "link_batch");
+}
+
+int vbx_link_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                   const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
+                   const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
+                   double *dist_out, double *Z_out, void *stream) {
+    return link_batch_call(h, "vbx_link_batch", fea, Phi, N, R, G, speaker, M, speaker_rec, Fa, Fb, workspace,
+                           workspace_bytes, n_out, F_out, dist_out, Z_out, nullptr, nullptr, stream);
+}
+
+int vbx_link_batch_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                        const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
+                        const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
+                        double *dist_out, double *Z_out, const double *mean, const double *std, void *stream) {
+    if (h && (!mean || !std)) {
+        int64_t total = 0;
+        for (int32_t g = 0; M && g < G; ++g) total += M[g];
+        if (total > 0) return fail(h, VBX_ERR_ARG, "vbx_link_batch_norm: null pointer");
+    }
+    return link_batch_call(h, "vbx_link_batch_norm", fea, Phi, N, R, G, speaker, M, speaker_rec, Fa, Fb, workspace,
+                           workspace_bytes, n_out, F_out, dist_out, Z_out, mean, std, stream);
+}
+
+int vbx_enroll_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, int64_t E, int64_t N_e,
+                                     int64_t max_k, int32_t n_thr, size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    const std::string who("vbx_enroll_batch_workspace_bytes");
+    const int rc = check_problem_sizes(h, who, G, M);
+    if (rc != VBX_OK) return rc;
+    if (E < 1 || N_e < 1 || max_k < 0 || n_thr < 1)
+        return fail(h, VBX_ERR_ARG, who + ": need E, N_e, n_thr >= 1 and max_k >= 0");
+    *bytes_out = vbx::enroll_batch_workspace_bytes(G, M, E, N_e, max_k, n_thr, h->sms);
+    return VBX_OK;
+}
+
+int vbx_enroll_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                     const int32_t *speaker, const int64_t *M, const int64_t *speaker_rec_offsets, int32_t n_rec,
+                     const float *enroll_fea, int64_t N_e, const int32_t *enroll_speaker, int64_t E, const double *Fa,
+                     const double *Fb, const double *thresholds, int32_t n_thr, void *workspace,
+                     size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
+                     double *F_out, double *n_enroll_out, double *F_enroll_out, const double *mean, const double *std,
+                     const double *enroll_mean, const double *enroll_std, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_enroll_batch");
+    const std::string who("vbx_enroll_batch");
+    int rc = check_problem_sizes(h, who, G, M);
+    if (rc != VBX_OK) return rc;
+    if (N < 0 || n_rec < 0 || N_e < 1 || E < 1 || n_thr < 1)
+        return fail(h, VBX_ERR_ARG, who + ": need N, n_rec >= 0 and N_e, E, n_thr >= 1");
+    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, who + ": R must lie in [1, 128]");
+    std::vector<double> c;
+    rc = problem_scalars(h, who, G, Fa, Fb, &c);
+    if (rc != VBX_OK) return rc;
+    if (!thresholds) return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    for (int32_t k = 0; k < n_thr; ++k)
+        if (!(std::fabs(thresholds[k]) <= 1e15))
+            return fail(h, VBX_ERR_ARG, who + ": |thresholds[" + std::to_string(k) + "]| must be <= 1e15");
+    const bool norm = mean || std || enroll_mean || enroll_std;
+    if (norm && !(mean && std && enroll_mean && enroll_std))
+        return fail(h, VBX_ERR_ARG, who + ": give all four of mean, std, enroll_mean and enroll_std, or none");
+    int64_t total = 0;
+    for (int32_t g = 0; g < G; ++g) total += M[g];
+    if (!Phi || !workspace || !enroll_fea || !enroll_speaker || (G > 0 && !speaker_rec_offsets) ||
+        (N > 0 && (!fea || !speaker)) || (total > 0 && (!assign_out || !best_llr_out)))
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    int64_t max_k = 0;
+    for (int32_t g = 0; g < G; ++g) {
+        const int64_t *ro = speaker_rec_offsets + (size_t)g * (n_rec + 1);
+        if (ro[0] != 0 || ro[n_rec] != M[g])
+            return fail(h, VBX_ERR_ARG, who + ": speaker_rec_offsets row " + std::to_string(g) + " must run from 0 to M[" +
+                                            std::to_string(g) + "]");
+        for (int32_t b = 0; b < n_rec; ++b) {
+            const int64_t k = ro[b + 1] - ro[b];
+            if (k < 0) return fail(h, VBX_ERR_ARG, who + ": speakers are not packed by recording (offsets decrease)");
+            max_k = std::max(max_k, k);
+        }
+    }
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
+        return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
+    if (workspace_bytes < vbx::enroll_batch_workspace_bytes(G, M, E, N_e, max_k, n_thr, h->sms))
+        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_enroll_batch_workspace_bytes()");
+    if (G == 0) return VBX_OK;
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_enroll_batch(fea, Phi, N, R, speaker, G, M, speaker_rec_offsets, n_rec, enroll_fea,
+                                               N_e, enroll_speaker, E, c.data(), thresholds, n_thr, workspace, h->sms,
+                                               assign_out, best_llr_out, llr_out, n_out, F_out, n_enroll_out,
+                                               F_enroll_out, (cudaStream_t)stream, mean, std, enroll_mean, enroll_std),
+                   "enroll_batch");
+}
+
+int vbx_cohort_stats_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, int64_t C, int64_t N_c,
+                                           size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    const std::string who("vbx_cohort_stats_batch_workspace_bytes");
+    const int rc = check_problem_sizes(h, who, G, M);
+    if (rc != VBX_OK) return rc;
+    if (C < 2 || N_c < 1) return fail(h, VBX_ERR_ARG, who + ": need C >= 2 and N_c >= 1");
+    *bytes_out = vbx::cohort_batch_workspace_bytes(G, M, C, N_c);
+    return VBX_OK;
+}
+
+int vbx_cohort_stats_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                           const int32_t *speaker, const int64_t *M, const float *cohort_fea, int64_t N_c,
+                           const int32_t *cohort_speaker, int64_t C, const double *Fa, const double *Fb, int32_t top_k,
+                           void *workspace, size_t workspace_bytes, double *mean_out, double *std_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_cohort_stats_batch");
+    const std::string who("vbx_cohort_stats_batch");
+    int rc = check_problem_sizes(h, who, G, M);
+    if (rc != VBX_OK) return rc;
+    if (N < 0 || N_c < 1 || C < 2) return fail(h, VBX_ERR_ARG, who + ": need N >= 0, N_c >= 1 and C >= 2");
+    if (top_k < 2) return fail(h, VBX_ERR_ARG, who + ": top_k must be >= 2");
+    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, who + ": R must lie in [1, 128]");
+    std::vector<double> c;
+    rc = problem_scalars(h, who, G, Fa, Fb, &c);
+    if (rc != VBX_OK) return rc;
+    int64_t total = 0;
+    for (int32_t g = 0; g < G; ++g) total += M[g];
+    if (total == 0) return VBX_OK;
+    if (!Phi || !workspace || !cohort_fea || !cohort_speaker || !mean_out || !std_out || (N > 0 && (!fea || !speaker)))
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
+        return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
+    if (workspace_bytes < vbx::cohort_batch_workspace_bytes(G, M, C, N_c))
+        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_cohort_stats_batch_workspace_bytes()");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_cohort_batch(fea, Phi, N, R, speaker, G, M, cohort_fea, N_c, cohort_speaker, C,
+                                               c.data(), top_k, workspace, mean_out, std_out, (cudaStream_t)stream),
+                   "cohort_batch");
 }
 
 int vbx_enroll_workspace_bytes(vbx_handle_t h, int64_t M, int64_t E, int64_t max_k, size_t *bytes_out) {

@@ -6,7 +6,12 @@
 //                        keys (8 passes of 8 bits, histograms in shared memory), then mu and sigma by fixed-order sums
 //   norm_scores_kernel   S(x, y) = 1/2 [ (LLR - mu_x) / sigma_x + (LLR - mu_y) / sigma_y ] in place over the link
 //                        distances (d = -S; the diagonal and the cannot-link entries untouched) or the enrolment LLRs
+// Batched (vbx_cohort_stats_batch, section 5.19): G problems against one cohort, each with its c_g: the statistics of
+// the scored speakers of all problems and of the cohort once per problem, enroll_score_kernel over every problem's
+// rectangle in one launch, and cohort_topk_kernel over all rows (a row's result depends on the row and C alone).
+// norm_scores_kernel takes NormProblems for vbx_enroll_batch and vbx_link_batch_norm.
 #include <algorithm>
+#include <cstring>
 
 #include "vbx_internal.cuh"
 
@@ -29,18 +34,8 @@ CohortWs cohort_layout(uint8_t *ws, int64_t M, int64_t C, size_t *total) {
     CohortWs w;
     size_t o = 0;
     auto take = [&](size_t bytes) { uint8_t *p = ws ? ws + o : nullptr; o += al(bytes); return p; };
-    auto stats = [&](int64_t n) {
-        SpeakerStats s;
-        s.n = reinterpret_cast<double *>(take(n * 8));
-        s.e = reinterpret_cast<double *>(take(n * 8));
-        s.b = reinterpret_cast<double *>(take(n * kMaxR * 8));
-        s.first = reinterpret_cast<long long *>(take(n * 8));
-        s.last = reinterpret_cast<long long *>(take(n * 8));
-        s.offs = reinterpret_cast<int64_t *>(take(4 * 8));
-        return s;
-    };
-    w.a = stats(M);
-    w.co = stats(C);
+    w.a = take_stats(take, M);
+    w.co = take_stats(take, C);
     w.scores = reinterpret_cast<double *>(take((size_t)M * C * 8));
     if (total) *total = o;
     return w;
@@ -126,22 +121,54 @@ __global__ void __launch_bounds__(kTopThreads) cohort_topk_kernel(const double *
 // x [rows, cols] in place: LLR -> S(i, j) with row statistics (mr, sr) and column statistics (mc, sc).  link = 1: x holds
 // distances d = -LLR, written back as -S, and the diagonal and the entries equal to `skip` (cannot-link) stay as they
 // are.  S is 1/2 (a_i + a_j) with a_i = (LLR - mu_i) / sigma_i: the sum commutes, so d[i][j] and d[j][i] stay the same
-// number.  copy_out (optional) receives the result.
+// number.  copy_out (optional) receives the result.  q.off set: several problems (NormProblems, section 5.19), each
+// element with the statistics of its own problem, so problem g's entries are those of a call on g alone.  kMode: 0 one
+// problem (q unused; the code of the single-problem entries), 1 the rectangle of several, 2 their square blocks.
+template <int kMode>
 __global__ void __launch_bounds__(256) norm_scores_kernel(double *__restrict__ x, int64_t rows, int64_t cols,
                                                           const double *__restrict__ mr, const double *__restrict__ sr,
                                                           const double *__restrict__ mc, const double *__restrict__ sc,
-                                                          int link, double skip, double *__restrict__ copy_out) {
+                                                          int link, double skip, double *__restrict__ copy_out,
+                                                          NormProblems q) {
     const int64_t n = rows * cols, stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
-        const int64_t i = t / cols, j = t - i * cols;
-        double d = x[t];
-        if (!link || (i != j && d != skip)) {
-            const double l = link ? -d : d;
-            const double s = 0.5 * ((l - mr[i]) / sr[i] + (l - mc[j]) / sc[j]);
-            d = link ? -s : s;
-            x[t] = d;
+    if constexpr (kMode == 0) {
+        for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
+            const int64_t i = t / cols, j = t - i * cols;
+            double d = x[t];
+            if (!link || (i != j && d != skip)) {
+                const double l = link ? -d : d;
+                const double s = 0.5 * ((l - mr[i]) / sr[i] + (l - mc[j]) / sc[j]);
+                d = link ? -s : s;
+                x[t] = d;
+            }
+            if (copy_out) copy_out[t] = d;
         }
-        if (copy_out) copy_out[t] = d;
+    } else {
+        for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
+            int64_t i, j, ri, cj;                         // local row and column; indices of their statistics
+            double *xt = x + t;
+            if (kMode == 2) {                             // square blocks: problem g's M x M block
+                const int g = find_problem(q.blk, q.G, t);
+                const int64_t base = q.off[g], M = q.off[g + 1] - base, lt = t - q.blk[g];
+                i = lt / M;
+                j = lt - i * M;
+                ri = base + i;
+                cj = base + j;
+                xt = reinterpret_cast<double *>(reinterpret_cast<uint8_t *>(x) + q.x_bytes[g]) + lt;
+            } else {                                      // rectangle: rows of every problem against its own columns
+                i = ri = t / cols;
+                j = t - i * cols;
+                cj = (int64_t)find_problem(q.off, q.G, i) * cols + j;
+            }
+            double d = *xt;
+            if (!link || (i != j && d != skip)) {
+                const double l = link ? -d : d;
+                const double s = 0.5 * ((l - mr[ri]) / sr[ri] + (l - mc[cj]) / sc[cj]);
+                d = link ? -s : s;
+                *xt = d;
+            }
+            if (copy_out) copy_out[t] = d;
+        }
     }
 }
 
@@ -168,12 +195,85 @@ int launch_cohort(const float *fea, const float *Phi, int64_t N, int R, const in
 
 int launch_norm_scores(double *x, int64_t rows, int64_t cols, const double *mean_r, const double *std_r,
                        const double *mean_c, const double *std_c, bool link, double skip, double *copy_out,
-                       cudaStream_t st) {
+                       cudaStream_t st, const NormProblems *q) {
     const int64_t n = rows * cols;
     if (n == 0) return 0;
-    norm_scores_kernel<<<(unsigned)std::min<int64_t>((n + 255) / 256, kNormGrid), 256, 0, st>>>(
-        x, rows, cols, mean_r, std_r, mean_c, std_c, link ? 1 : 0, skip, copy_out);
+    const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, kNormGrid);
+    const NormProblems one{1, nullptr, nullptr, nullptr};
+    if (!q)
+        norm_scores_kernel<0><<<grid, 256, 0, st>>>(x, rows, cols, mean_r, std_r, mean_c, std_c, link ? 1 : 0, skip,
+                                                    copy_out, one);
+    else if (q->blk)
+        norm_scores_kernel<2><<<grid, 256, 0, st>>>(x, rows, cols, mean_r, std_r, mean_c, std_c, link ? 1 : 0, skip,
+                                                    copy_out, *q);
+    else
+        norm_scores_kernel<1><<<grid, 256, 0, st>>>(x, rows, cols, mean_r, std_r, mean_c, std_c, link ? 1 : 0, skip,
+                                                    copy_out, *q);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
+namespace {
+
+// vbx_cohort_stats_batch: the scored speakers of every problem [sum M], the cohort speakers once per problem [G C] with
+// their index [G, N_c], the scores [sum M, C] and the problem arrays off, coff (g C), tile_off [G+1] and c [G]
+struct CohortBatchWs {
+    SpeakerStats a, co;
+    int32_t *cspk;
+    double *scores;
+    int64_t *arrays;
+};
+
+CohortBatchWs cohort_batch_layout(uint8_t *ws, int64_t G, int64_t M, int64_t C, int64_t N_c, size_t *total) {
+    CohortBatchWs w;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { uint8_t *p = ws ? ws + o : nullptr; o += al(bytes); return p; };
+    w.a = take_stats(take, M);
+    w.co = take_stats(take, G * C);
+    w.cspk = reinterpret_cast<int32_t *>(take((size_t)G * N_c * 4));
+    w.scores = reinterpret_cast<double *>(take((size_t)M * C * 8));
+    w.arrays = reinterpret_cast<int64_t *>(take((size_t)(4 * G + 3) * 8));
+    if (total) *total = o;
+    return w;
+}
+
+}  // namespace
+
+size_t cohort_batch_workspace_bytes(int G, const int64_t *M_host, int64_t C, int64_t N_c) {
+    int64_t M = 0;
+    for (int g = 0; g < G; ++g) M += M_host[g];
+    size_t total = 0;
+    cohort_batch_layout(nullptr, G, M, C, N_c, &total);
+    return total;
+}
+
+int launch_cohort_batch(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int G,
+                        const int64_t *M_host, const float *cohort_fea, int64_t N_c, const int32_t *cohort_spk,
+                        int64_t C, const double *c_host, int64_t top_k, void *workspace, double *mean_out,
+                        double *std_out, cudaStream_t st) {
+    std::vector<int64_t> host(4 * (size_t)G + 3, 0);       // off, coff, tile_off [G+1], c [G]: one copy
+    int64_t *off = host.data(), *coff = off + (G + 1), *tile = coff + (G + 1);
+    for (int g = 0; g < G; ++g) {
+        off[g + 1] = off[g] + M_host[g];
+        coff[g + 1] = coff[g] + C;
+        tile[g + 1] = tile[g] + rect_tiles(M_host[g], C);
+    }
+    std::memcpy(tile + (G + 1), c_host, (size_t)G * sizeof(double));
+    const int64_t M = off[G];
+    if (M == 0) return 0;
+    const CohortBatchWs w = cohort_batch_layout(reinterpret_cast<uint8_t *>(workspace), G, M, C, N_c, nullptr);
+    if (cudaMemcpyAsync(w.arrays, host.data(), host.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st) !=
+        cudaSuccess)
+        return -1;
+    const int64_t *d_off = w.arrays, *d_coff = d_off + (G + 1), *d_tile = d_coff + (G + 1);
+    const double *d_c = reinterpret_cast<const double *>(d_tile + (G + 1));
+    const int lr = launch_repeat_index(cohort_spk, N_c, G, w.cspk, st);
+    const int la = launch_speaker_stats_batch(fea, Phi, spk, N, R, G, d_off, d_c, M, w.a, nullptr, nullptr, st);
+    const int lc = launch_speaker_stats_batch(cohort_fea, Phi, w.cspk, N_c, R, G, d_coff, d_c, (int64_t)G * C, w.co,
+                                              nullptr, nullptr, st);
+    const int ls = launch_cohort_scores_batch(w.a, w.co, Phi, G, d_off, d_tile, d_c, tile[G], C, R, w.scores, st);
+    if (lr < 0 || la < 0 || lc < 0 || ls < 0) return -1;
+    cohort_topk_kernel<<<(unsigned)M, kTopThreads, 0, st>>>(w.scores, C, std::min(top_k, C), mean_out, std_out);
+    return cudaGetLastError() == cudaSuccess ? lr + la + lc + ls + 1 : -1;
 }
 
 }  // namespace vbx

@@ -182,6 +182,19 @@ __device__ __forceinline__ void st_vec<4>(float *p, const float *v) {
     *reinterpret_cast<float4 *>(p) = make_float4(v[0], v[1], v[2], v[3]);
 }
 
+// The problem g whose range [pref[g], pref[g+1]) holds x, for non-decreasing pref with pref[0] = 0 <= x < pref[G]:
+// the largest g with pref[g] <= x (never an empty problem's, whose range is empty).  The batched speaker kernels
+// (vbx_link_batch, vbx_enroll_batch, vbx_cohort_stats_batch) decode their flat indices with it.
+__device__ __forceinline__ int find_problem(const int64_t *__restrict__ pref, int G, int64_t x) {
+    int lo = 0, hi = G;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (pref[mid] <= x) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+
 #endif  // __CUDACC__
 
 // launchers (vbx_kernels.cu); each returns the number of kernels launched or -1 on launch error
@@ -261,7 +274,8 @@ int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t 
 size_t link_batch_workspace_bytes(int G, const int64_t *M_host, std::vector<int64_t> *lk_off = nullptr);
 int launch_link_batch(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
                       int G, const int64_t *M_host, const double *c_host, void *workspace, double *n_out,
-                      double *F_out, double *dist_out, double *Z_out, cudaStream_t st);
+                      double *F_out, double *dist_out, double *Z_out, cudaStream_t st, const double *mean = nullptr,
+                      const double *std = nullptr);
 // vbx_link's span and statistics kernels over M speakers into caller-owned DEVICE arrays (n, e [M], b [M, kMaxR]
 // float64; first, last [M] and offs [4] int64 scratch): n_s, F_s, b_s and e_s exactly as vbx_link computes them.
 // Returns the number of launches, -1 on a launch error.
@@ -270,8 +284,33 @@ struct SpeakerStats {
     long long *first, *last;
     int64_t *offs;
 };
+// The statistics of n speakers carved from a workspace by take(bytes) (host), as the enrolment and cohort layouts hold them
+template <class Take>
+SpeakerStats take_stats(Take &take, int64_t n) {
+    SpeakerStats s;
+    s.n = reinterpret_cast<double *>(take(n * 8));
+    s.e = reinterpret_cast<double *>(take(n * 8));
+    s.b = reinterpret_cast<double *>(take(n * kMaxR * 8));
+    s.first = reinterpret_cast<long long *>(take(n * 8));
+    s.last = reinterpret_cast<long long *>(take(n * 8));
+    s.offs = reinterpret_cast<int64_t *>(take(4 * 8));
+    return s;
+}
 int launch_speaker_stats(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, int64_t M, double c,
                          const SpeakerStats &s, double *n_out, double *F_out, cudaStream_t st);
+// The same over G problems as vbx_link_batch runs them: spk [G,N] (row g: local speakers of problem g), off [G+1] and
+// c [G] DEVICE; s holds M = off[G] speakers.  Problem g's statistics are bit-identical to launch_speaker_stats on it alone.
+int launch_speaker_stats_batch(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, int G,
+                               const int64_t *off, const double *c, int64_t M, const SpeakerStats &s, double *n_out,
+                               double *F_out, cudaStream_t st);
+// Several problems of norm_scores_kernel (DESIGN.md section 5.19), DEVICE arrays [G+1].  Rectangle (blk null): x holds
+// the rows of every problem, problem g's off[g] .. off[g+1]-1, with row statistics at the row and column statistics at
+// g * cols + column.  Square blocks (blk set): problem g's off[g+1] - off[g] square block starts at element blk[g] of
+// copy_out and at byte x_bytes[g] of x, its statistics at off[g] + row and off[g] + column; rows * cols = blk[G].
+struct NormProblems {
+    int G;
+    const int64_t *off, *blk, *x_bytes;
+};
 // enrolment against known speakers (vbx_enroll.cu)
 size_t enroll_workspace_bytes(int64_t M, int64_t E, int64_t max_k, int sms);
 int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
@@ -284,15 +323,42 @@ int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const in
 // (and llr_out when not null), bit-identical to vbx_enroll's llr against the same speakers.  Returns 1, 0 for M == 0.
 int launch_cohort_scores(const SpeakerStats &a, const SpeakerStats &co, const float *Phi, int64_t M, int64_t C, int R,
                          double c, double *llr, double *llr_out, cudaStream_t st);
+// The same over G problems: rows off[g] .. off[g+1]-1 of a against columns g C .. g C + C - 1 of co with c[g], flat
+// tiles tile_off [G+1] (every array DEVICE; n_tiles = tile_off[G] on the host).  Problem g's rows of llr [off[G], C]
+// are bit-identical to launch_cohort_scores on it alone.
+int launch_cohort_scores_batch(const SpeakerStats &a, const SpeakerStats &co, const float *Phi, int G,
+                               const int64_t *off, const int64_t *tile_off, const double *c, int64_t n_tiles, int64_t C,
+                               int R, double *llr, cudaStream_t st);
+// score tiles of an M x C rectangle (host)
+int64_t rect_tiles(int64_t M, int64_t C);
+// dst [G, n] = G copies of src [n] (DEVICE)
+int launch_repeat_index(const int32_t *src, int64_t n, int G, int32_t *dst, cudaStream_t st);
+// G enrolment problems (vbx_enroll_batch): M_host [G], rec_off_host [G, n_rec + 1], c_host [G], thresholds [n_thr] HOST
+size_t enroll_batch_workspace_bytes(int G, const int64_t *M_host, int64_t E, int64_t N_e, int64_t max_k, int64_t n_thr,
+                                    int sms);
+int launch_enroll_batch(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int G,
+                        const int64_t *M_host, const int64_t *rec_off_host, int n_rec, const float *enroll_fea,
+                        int64_t N_e, const int32_t *enroll_spk, int64_t E, const double *c_host,
+                        const double *thresholds, int64_t n_thr, void *workspace, int sms, int32_t *assign_out,
+                        double *best_llr_out, double *llr_out, double *n_out, double *F_out, double *n_enroll_out,
+                        double *F_enroll_out, cudaStream_t st, const double *mean, const double *std,
+                        const double *enroll_mean, const double *enroll_std);
 // score normalisation against a cohort (vbx_cohort.cu)
 size_t cohort_workspace_bytes(int64_t M, int64_t C);
 int launch_cohort(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
                   const float *cohort_fea, int64_t N_c, const int32_t *cohort_spk, int64_t C, double c, int64_t top_k,
                   void *workspace, double *mean_out, double *std_out, double *scores_out, cudaStream_t st);
-// x [rows, cols] of LLRs (link: of distances -LLR, diagonal and `skip` entries kept) replaced by the normalised scores
+// G problems against one cohort (vbx_cohort_stats_batch): M_host [G], c_host [G] HOST
+size_t cohort_batch_workspace_bytes(int G, const int64_t *M_host, int64_t C, int64_t N_c);
+int launch_cohort_batch(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int G,
+                        const int64_t *M_host, const float *cohort_fea, int64_t N_c, const int32_t *cohort_spk,
+                        int64_t C, const double *c_host, int64_t top_k, void *workspace, double *mean_out,
+                        double *std_out, cudaStream_t st);
+// x [rows, cols] of LLRs (link: of distances -LLR, diagonal and `skip` entries kept) replaced by the normalised scores;
+// q: several problems (NormProblems), null for one
 int launch_norm_scores(double *x, int64_t rows, int64_t cols, const double *mean_r, const double *std_r,
                        const double *mean_c, const double *std_c, bool link, double skip, double *copy_out,
-                       cudaStream_t st);
+                       cudaStream_t st, const NormProblems *q = nullptr);
 // wgmma projection (vbx_project_tc.cu)
 size_t tc_scratch_floats();
 int launch_project_wgmma(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,

@@ -15,7 +15,9 @@
 // [G, N], speaker_rec slice and c_g.  Their speakers are packed by the offsets off [G+1]; the statistics kernels run one
 // CTA per (problem, speaker), the score kernel's flat tile index runs over the upper-triangle tiles of all problems, and
 // one linkage launch has one CTA per problem.  vbx_link is the G = 1 case of the same kernels (LinkProblems with null
-// arrays), so a problem's results do not depend on the others.
+// arrays), so a problem's results do not depend on the others.  vbx_link_batch_norm (section 5.19) adds
+// norm_scores_kernel over every problem's block, as vbx_link_norm does for one; vbx_enroll_batch and
+// vbx_cohort_stats_batch take the batched statistics through launch_speaker_stats_batch.
 #include <algorithm>
 #include <climits>
 #include <cstring>
@@ -82,18 +84,6 @@ LinkWs link_layout(uint8_t *ws, size_t lk_bytes, int64_t M, int64_t G, size_t *t
     o += al(problem_array_bytes(G));
     if (total) *total = o;
     return w;
-}
-
-// The problem g whose range [pref[g], pref[g+1]) holds x, for non-decreasing pref with pref[0] = 0 <= x < pref[G]:
-// the largest g with pref[g] <= x (never an empty problem's, whose range is empty).
-__device__ __forceinline__ int find_problem(const int64_t *__restrict__ pref, int G, int64_t x) {
-    int lo = 0, hi = G;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (pref[mid] <= x) lo = mid;
-        else hi = mid;
-    }
-    return lo;
 }
 
 __global__ void link_init_kernel(LinkWs w, LinkProblems p) {
@@ -375,7 +365,8 @@ int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t 
 
 int launch_link_batch(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
                       int G, const int64_t *M_host, const double *c_host, void *workspace, double *n_out,
-                      double *F_out, double *dist_out, double *Z_out, cudaStream_t st) {
+                      double *F_out, double *dist_out, double *Z_out, cudaStream_t st, const double *mean,
+                      const double *std) {
     std::vector<int64_t> lk_off;
     link_batch_workspace_bytes(G, M_host, &lk_off);
     // the problem arrays: off, lk_off, tile_off, dist_off [G+1] and c [G], uploaded in one copy
@@ -405,7 +396,15 @@ int launch_link_batch(const float *fea, const float *Phi, const int32_t *spk, in
     p.dist_off = w.offs + 3 * (G + 1);
     p.c = reinterpret_cast<const double *>(w.offs + 4 * (G + 1));
     p.c0 = 0.0;
-    int launches = launch_problems(w, p, tile[G], fea, Phi, spk, R, spk_rec, n_out, F_out, dist_out, true, st);
+    int launches = launch_problems(w, p, tile[G], fea, Phi, spk, R, spk_rec, n_out, F_out, mean ? nullptr : dist_out,
+                                   true, st);
+    if (mean) {                                       // vbx_link_batch_norm: each problem's block as vbx_link_norm's
+        const NormProblems q{G, p.off, p.dist_off, p.lk_off};
+        const int ln = launch_norm_scores(reinterpret_cast<double *>(w.lk), dist[G], 1, mean, std, mean, std, true,
+                                          kBig, dist_out, st, &q);
+        if (ln < 0) return -1;
+        launches += ln;
+    }
     if (linkage) {
         launch_linkage(p.off, p.lk_off, G, w.lk, Z_out, st);
         ++launches;
@@ -426,6 +425,30 @@ int launch_speaker_stats(const float *fea, const float *Phi, const int32_t *spk,
     w.offs = s.offs;
     const int launches = launch_problems(w, single(M, N, c), 0, fea, Phi, spk, R, nullptr, n_out, F_out, nullptr, false,
                                          st);
+    return cudaGetLastError() == cudaSuccess ? launches : -1;
+}
+
+int launch_speaker_stats_batch(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, int G,
+                               const int64_t *off, const double *c, int64_t M, const SpeakerStats &s, double *n_out,
+                               double *F_out, cudaStream_t st) {
+    if (M == 0) return 0;
+    LinkWs w;
+    w.lk = nullptr;
+    w.n = s.n;
+    w.e = s.e;
+    w.b = s.b;
+    w.first = s.first;
+    w.last = s.last;
+    w.offs = s.offs;
+    LinkProblems p;
+    p.G = G;
+    p.M = M;
+    p.N = N;
+    p.off = off;
+    p.lk_off = p.tile_off = p.dist_off = nullptr;
+    p.c = c;
+    p.c0 = 0.0;
+    const int launches = launch_problems(w, p, 0, fea, Phi, spk, R, nullptr, n_out, F_out, nullptr, false, st);
     return cudaGetLastError() == cudaSuccess ? launches : -1;
 }
 

@@ -150,6 +150,123 @@ def enroll_speakers(fea, Phi, offsets, labels, enroll_fea, enroll_speaker, Fa, F
     return out
 
 
+def check_thresholds(thresholds):
+    """The enrolment thresholds of a sweep as floats without duplicates (first occurrence kept); each as check_threshold
+    takes it.  An empty list raises ValueError."""
+    out = list(dict.fromkeys(check_threshold(t) for t in thresholds))
+    if not out:
+        raise ValueError('enroll_thresholds needs at least one value')
+    return out
+
+
+def enroll_many(fea, Phi, offsets, labels_per_problem, enroll_fea, enroll_speaker, Fa, Fb, thresholds, device=None,
+                llr=False, max_bytes=None, norm=None):
+    """enroll_speakers for G independent problems over the same features and enrolled set, at every threshold, in few
+    launches (vbx_enroll_batch, DESIGN.md section 5.19), e.g. the final labels of every setting of a sweep.  fea, Phi,
+    offsets, enroll_fea, enroll_speaker: as for enroll_speakers; labels_per_problem: G lists of first labels per
+    recording; Fa, Fb: numbers or G values; thresholds: a list (check_thresholds).  Each problem's LLR block is computed
+    once and assigned at every threshold.  norm: None, or per problem (mean [M_g], std [M_g], enroll_mean [E],
+    enroll_std [E]) (cohort.cohort_stats_many): the normalised path of enroll_speakers(norm=).  The problems are packed
+    in order into launches whose workspace stays within max_bytes (None: one launch; sweep.pack_by with the batch's own
+    vbx_enroll_batch_workspace_bytes; a problem larger than max_bytes alone raises ValueError).
+    Returns one EnrollResult per problem with assign and best_llr [n_thr, M_g] (row h: thresholds[h]); row h is
+    bit-identical to enroll_speakers(threshold=thresholds[h]) on that problem alone, and so are n, F, n_enroll, F_enroll
+    and llr [M_g, E] (llr=True)."""
+    import torch
+    from . import _lib
+    from ._lib import VbxError
+    from .sweep import pack_by
+    thr = np.ascontiguousarray(check_thresholds(thresholds), dtype=np.float64)
+    G, T = len(labels_per_problem), len(thr)
+    Fa, Fb = (np.broadcast_to(np.asarray(v, dtype=np.float64), (G,)).copy() for v in (Fa, Fb))
+    offsets = np.asarray(offsets, dtype=np.int64)
+    espk = np.asarray(enroll_speaker, dtype=np.int64).reshape(-1)
+    if len(espk) == 0 or espk.min() < 0:
+        raise ValueError('enroll_speaker must hold at least one speaker index, all >= 0')
+    E = int(espk.max()) + 1
+    if np.bincount(espk, minlength=E).min() == 0:
+        raise ValueError('every enrolled speaker 0 .. E-1 needs at least one x-vector')
+    tables = [speaker_table(l) for l in labels_per_problem]
+    Ms = np.array([len(t.rec) for t in tables], dtype=np.int64)
+    B = len(offsets) - 1
+    firsts = [np.searchsorted(t.rec, np.arange(B + 1)).astype(np.int64) for t in tables]
+    if norm is not None:
+        norm = [tuple(np.asarray(a, dtype=np.float64) for a in nm) for nm in norm]
+        if len(norm) != G or any([a.shape for a in nm] != [(M,), (M,), (E,), (E,)] for nm, M in zip(norm, Ms.tolist())):
+            raise ValueError('norm must hold per problem mean and std of its archive speakers and of the E enrolled ones')
+    if not torch.cuda.is_available():
+        raise VbxError('enroll_many(): no CUDA device - vbx_b200 has no CPU fallback')
+    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    fea = torch.as_tensor(fea).to(dev, torch.float32).contiguous()
+    Phi = torch.as_tensor(Phi).to(dev, torch.float32).contiguous()
+    efea = torch.as_tensor(enroll_fea).to(dev, torch.float32).contiguous()
+    N, R = int(fea.shape[0]), int(fea.shape[1])
+    for labels in labels_per_problem:
+        if int(offsets[-1]) != N or len(labels) != B:
+            raise ValueError('offsets must hold one more entry than labels and end at the number of x-vectors')
+    if tuple(efea.shape) != (len(espk), R):
+        raise ValueError(f'enroll_fea must be [{len(espk)}, {R}], got {tuple(efea.shape)}')
+    max_k = [int(np.diff(f).max()) if B else 0 for f in firsts]
+    lib = _lib.load()
+    h = ctypes.c_void_p()
+    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
+        raise VbxError('vbx_create failed: no usable sm_90 device')
+    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+    v = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    out = [None] * G
+
+    def ws_bytes(idx):
+        need = ctypes.c_size_t()
+        M_h = np.ascontiguousarray(Ms[idx])
+        if lib.vbx_enroll_batch_workspace_bytes(h, len(idx), v(M_h), E, len(espk), max(max_k[g] for g in idx), T,
+                                                ctypes.byref(need)) != 0:
+            raise VbxError(f'vbx_enroll_batch_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
+        return int(need.value)
+    try:
+        batches = pack_by(G, ws_bytes, max_bytes)
+        with torch.cuda.device(dev):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            espk_d = torch.from_numpy(espk.astype(np.int32)).to(dev)
+            thr_h = np.ascontiguousarray(thr)
+            for idx in batches:
+                M_h = np.ascontiguousarray(Ms[idx])
+                tot, Gb = int(M_h.sum()), len(idx)
+                ws = torch.empty(max(ws_bytes(idx), 1), dtype=torch.uint8, device=dev)
+                spk = np.stack([speaker_index(offsets, labels_per_problem[g])[0] for g in idx]).astype(np.int32)
+                spk_d = torch.from_numpy(spk).to(dev)
+                rec_off = np.ascontiguousarray(np.stack([firsts[g] for g in idx]))
+                fa, fb = np.ascontiguousarray(Fa[idx]), np.ascontiguousarray(Fb[idx])
+                assign = torch.empty((T, tot), dtype=torch.int32, device=dev)
+                best = torch.empty((T, tot), dtype=torch.float64, device=dev)
+                n = torch.empty(tot, dtype=torch.float64, device=dev)
+                F = torch.empty((tot, R), dtype=torch.float64, device=dev)
+                n_e = torch.empty((Gb, E), dtype=torch.float64, device=dev)
+                F_e = torch.empty((Gb, E, R), dtype=torch.float64, device=dev)
+                L = torch.empty((tot, E), dtype=torch.float64, device=dev) if llr else None
+                stats = [None] * 4
+                if norm is not None:
+                    stats = [torch.from_numpy(np.concatenate([norm[g][k] for g in idx])).to(dev) for k in range(4)]
+                rc = lib.vbx_enroll_batch(h, p(fea), p(Phi), N, R, Gb, p(spk_d), v(M_h), v(rec_off), B, p(efea),
+                                          len(espk), p(espk_d), E, v(fa), v(fb), v(thr_h), T, p(ws), ws.numel(),
+                                          p(assign), p(best), p(L), p(n), p(F), p(n_e), p(F_e), *map(p, stats), stream)
+                if rc != 0:
+                    raise VbxError(f'vbx_enroll_batch failed ({rc}): {lib.vbx_last_error(h).decode()}')
+                assign = assign.cpu().numpy().astype(np.int64)
+                best, n, F = best.cpu().numpy(), n.cpu().numpy(), F.cpu().numpy()
+                n_e, F_e = n_e.cpu().numpy(), F_e.cpu().numpy()
+                L = L.cpu().numpy() if llr else None
+                o = 0
+                for j, (g, M) in enumerate(zip(idx, M_h.tolist())):
+                    out[g] = EnrollResult(tables[g], assign[:, o:o + M], best[:, o:o + M], n[o:o + M], F[o:o + M],
+                                          n_e[j], F_e[j], L[o:o + M] if llr else None)
+                    o += M
+    finally:
+        lib.vbx_destroy(h)
+    return out
+
+
 def enroll_names(table, assign, best_llr, enrolled_names, recording_names, labels2=None, link=None):
     """The names of every recording's speakers (DESIGN.md section 5.16): per recording ({label: name}, {label: llr}).
     A speaker assigned to enrolled speaker e is enrolled_names[e]; any other is unknown-<recording>-<label + 1>, or with

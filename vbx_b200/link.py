@@ -121,14 +121,16 @@ def link_speakers(fea, Phi, offsets, labels, Fa, Fb, device=None, dist=False, no
     return out
 
 
-def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_bytes=None, dist=False):
+def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_bytes=None, dist=False, norm=None):
     """link_speakers for G independent problems over the same features in few launches (vbx_link_batch, DESIGN.md
     section 5.18), e.g. the final labels of every setting of a sweep.  fea, Phi, offsets: as for link_speakers;
     labels_per_problem: G lists of first labels per recording; Fa, Fb: numbers or G values, problem g's scalars.
     The problems are packed in order into launches whose workspaces stay within max_bytes (None: one launch), each
     problem sized by vbx_link_workspace_bytes (sweep.pack: a problem larger than max_bytes on its own raises ValueError).
+    norm: None, or per problem (mean [M_g], std [M_g]) of its speakers' cohort scores (cohort.cohort_stats_many): the
+    distances are then -S as link_speakers(norm=) computes them (vbx_link_batch_norm, DESIGN.md section 5.19).
     Returns one (table, n, F, Z) per problem (with dist=True also dist [M,M]), bit-identical to link_speakers on that
-    problem alone."""
+    problem alone (with the same norm)."""
     import torch
     from . import _lib
     from ._lib import VbxError
@@ -152,6 +154,10 @@ def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_by
     for labels in labels_per_problem:
         if int(offsets[-1]) != N or len(offsets) != len(labels) + 1:
             raise ValueError('offsets must hold one more entry than labels and end at the number of x-vectors')
+    if norm is not None:
+        norm = [tuple(np.asarray(a, dtype=np.float64) for a in nm) for nm in norm]
+        if len(norm) != G or any([a.shape for a in nm] != [(M,), (M,)] for nm, M in zip(norm, Ms)):
+            raise ValueError('norm must hold per problem mean and std of its speakers')
     lib = _lib.load()
     h = ctypes.c_void_p()
     if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
@@ -187,9 +193,14 @@ def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_by
                 F = torch.empty((tot, R), dtype=torch.float64, device=dev)
                 D = torch.empty(int((M_h * M_h).sum()), dtype=torch.float64, device=dev) if dist else None
                 Z = torch.empty((tot, 4), dtype=torch.float64, device=dev)
-                rc = lib.vbx_link_batch(h, p(fea), p(Phi), N, R, len(idx), p(spk_d), M_h.ctypes.data_as(ctypes.c_void_p),
-                                        p(rec_d), fa.ctypes.data_as(ctypes.c_void_p), fb.ctypes.data_as(ctypes.c_void_p),
-                                        p(ws), ws.numel(), p(n), p(F), p(D), p(Z), stream)
+                args = (h, p(fea), p(Phi), N, R, len(idx), p(spk_d), M_h.ctypes.data_as(ctypes.c_void_p), p(rec_d),
+                        fa.ctypes.data_as(ctypes.c_void_p), fb.ctypes.data_as(ctypes.c_void_p), p(ws), ws.numel(), p(n),
+                        p(F), p(D), p(Z))
+                if norm is None:
+                    rc = lib.vbx_link_batch(*args, stream)
+                else:
+                    mean, std = (torch.from_numpy(np.concatenate([norm[g][k] for g in idx])).to(dev) for k in (0, 1))
+                    rc = lib.vbx_link_batch_norm(*args, p(mean), p(std), stream)
                 if rc != 0:
                     raise VbxError(f'vbx_link_batch failed ({rc}): {lib.vbx_last_error(h).decode()}')
                 n, F, Z = n.cpu().numpy(), F.cpu().numpy(), Z.cpu().numpy()

@@ -29,6 +29,13 @@ vbx_link_batch call, every threshold a host cut of the setting's linkage.  summa
 global_speakers per recording[, der_across_files][, der_across_files_overlap]} per setting and, with a reference,
 ranking_across_files (and ranking_across_files_overlap): per protocol, the names <setting>_link<threshold> by DER across
 files.  No linked RTTM files are written: the maps and cli --link-threshold at the chosen setting reproduce them.
+With --enroll-ark FILE --enroll-utt2spk FILE (both or neither) and --enroll-threshold LIST the speakers of every setting
+are named by the enrolled speakers at every threshold (DESIGN.md sections 5.16 and 5.19): all settings in one batched
+vbx_enroll_batch call.  summary.json then gains named = {threshold: speaker_names per recording[, der_by_name]
+[, der_by_name_overlap]} per setting and, with a reference, ranking_by_name (and ranking_by_name_overlap): per protocol,
+the names <setting>_enroll<threshold> by DER by name.  With --cohort-ark FILE --cohort-utt2spk FILE (both or neither;
+--cohort-top, default 200) both link and enrolment thresholds are on the normalised score of section 5.17.  No named
+RTTM files are written: cli with --enroll-threshold at the chosen setting reproduces them.
 """
 import argparse
 import itertools
@@ -106,6 +113,27 @@ def pack(sizes, budget):
     return batches
 
 
+def pack_by(n, size_of, budget):
+    """Entries 0 .. n-1, in order, into consecutive batches whose size_of(list of entries) stays within `budget` (for
+    workspaces that are not a plain sum of per-entry sizes).  None: one batch.  An entry larger than the budget on its
+    own raises ValueError."""
+    if budget is None:
+        return [list(range(n))] if n else []
+    batches, cur = [], []
+    for i in range(n):
+        if cur and size_of(cur + [i]) <= budget:
+            cur.append(i)
+            continue
+        if size_of([i]) > budget:
+            raise ValueError(f'one entry needs {int(size_of([i]))} bytes, more than max_batch_bytes = {int(budget)}')
+        if cur:
+            batches.append(cur)
+        cur = [i]
+    if cur:
+        batches.append(cur)
+    return batches
+
+
 def entry_bytes(T, n_states, R, device):
     """Device bytes one (recording, setting) entry adds to a float32 batch: its share of the plan's workspace (the larger
     of the split and the fused-sweep plans of the recording alone, which bounds what it adds to any batch), plus its
@@ -141,7 +169,7 @@ def packer(lens, R, device, budget):
 def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
                 device=None, max_batch_bytes=None, output_2nd=False, ref_rttm=None, uem=None, overlaps=None,
                 oracle_overlaps=False, jer=False, num_speakers=None, min_speakers=None, max_speakers=None,
-                link_thresholds=None):
+                link_thresholds=None, enroll=None, enroll_thresholds=None, cohort=None, cohort_top=200):
     """Every setting of `grid` (see grid_settings) for every recording, with the front end and AHC run once.
 
     recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
@@ -172,16 +200,42 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     global_speakers = {threshold: {label: global id}}, equal to diarize_batch(link_threshold=threshold)'s with that
     setting's scalars; with a reference also ref_speakers (the reference speaker names, in the rows of the blocks) and
     der_blocks = {protocol: overlap block} (with overlaps der_overlap_blocks too), what summarize_across_files needs.
+    enroll, enroll_thresholds: None, or known speakers {name: raw x-vectors [n, Dx]} as for diarize_batch and a list of
+    LLR thresholds (DESIGN.md sections 5.16 and 5.19; each checked by enroll.check_threshold before any device work,
+    duplicates dropped; there is no default).  The enrolled x-vectors go through the front end once; the final first
+    labels of every setting are scored against them in one enroll.enroll_many call within max_batch_bytes, each
+    setting's LLR block assigned at every threshold.  Each recording's dict gains speaker_names = {threshold: {label:
+    name}} and speaker_llr = {threshold: {label: llr}}, equal to diarize_batch(enroll_threshold=threshold)'s with that
+    setting's scalars (unknown speakers are unknown-<recording>-<label + 1>: with link_thresholds as well, linking and
+    enrolment are each what diarize_batch gives with that option alone), and with a reference ref_speakers and
+    der_blocks as for linking (what summarize_by_name needs).
+    cohort, cohort_top: None, or a cohort {name: raw x-vectors [n, Dx]} as for diarize_batch (section 5.17; needs
+    link_thresholds or enroll).  Its statistics for every setting's speakers (and enrolled speakers) come from batched
+    cohort.cohort_stats_many calls; a speaker without spread raises ValueError naming the setting and the speaker before
+    any linking or enrolment kernel runs.  link_thresholds and enroll_thresholds are then on the normalised score S,
+    every dict gains score_norm, and with enroll speaker_score replaces speaker_llr.
     Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags[, der][, rttm_overlap,
-    overlap_seconds][, der_overlap][, count_rule, n_speakers_vb, count][, global_speakers][, ref_speakers, der_blocks
-    [, der_overlap_blocks]])}}; each recording's dict is the one diarize_batch returns with that setting's scalars."""
+    overlap_seconds][, der_overlap][, count_rule, n_speakers_vb, count][, global_speakers][, speaker_names, speaker_llr
+    or speaker_score][, score_norm][, ref_speakers, der_blocks[, der_overlap_blocks]])}}; each recording's dict is the
+    one diarize_batch returns with that setting's scalars."""
     import torch
     from . import ahc as _ahc
     from ._lib import VbxError
     from .parts import make_batch
-    from .pipeline import _check_init, _count_fields, _front_end, _pad_features, _result, _vb_stage, count_bounds
+    from .pipeline import (_check_init, _count_fields, _front_end, _pad_features, _result, _side_features, _vb_stage,
+                           count_bounds)
     settings = grid_settings(grid)
     links = check_link_thresholds(link_thresholds)
+    dims = {int(np.asarray(r[0]).shape[1]) for r in recordings.values()}
+    dim = next(iter(dims)) if len(dims) == 1 else -1
+    enrolled, enroll_thr = check_enroll_options(enroll, enroll_thresholds, dim)
+    cohort_set = None
+    if cohort is not None:
+        from . import cohort as _cohort
+        if links is None and enrolled is None:
+            raise ValueError('a cohort normalises the linking and enrolment scores: it needs link_thresholds or enroll')
+        _cohort.check_top_k(cohort_top)
+        cohort_set = _cohort.check_cohort(cohort, dim)
     with_overlap = oracle_overlaps or overlaps is not None
     _check_init(init, with_overlap)
     if oracle_overlaps and ref_rttm is None:
@@ -226,14 +280,32 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     res = _vb_stage([(s.Fa, s.Fb, s.loopP, s.smoothing) for s in settings], [ahc_labels[s.threshold] for s in settings],
                     [lab_d[s.threshold] for s in settings], Zs, lens, fea, Phi, bounds, init, dev, make_batch,
                     packer(lens, int(fea.shape[1]), dev, max_batch_bytes), maxIters=max_iters, epsilon=epsilon)
-    maps = None
+    maps = named = norm = None
+    if links is not None or enrolled is not None:
+        offs = np.concatenate([[0], np.cumsum(lens)])
+        labels = [[res[(k, b)][0] for b in range(len(names))] for k in range(len(settings))]
+        Fa, Fb = [s.Fa for s in settings], [s.Fb for s in settings]
+        side = lambda sets: _side_features(sets, recordings, names, transform, plda, lda_dim, chain, dev, fea, Phi)
+        enrolled_fea = side(enrolled) if enrolled is not None else None
+        if cohort_set is not None:
+            norm = _cohort_norm_many(side(cohort_set), cohort_top, settings, enrolled, enrolled_fea, names, fea, Phi,
+                                     offs, labels, dev, max_batch_bytes)
     if links is not None:
         from . import link
-        labels = [[res[(k, b)][0] for b in range(len(names))] for k in range(len(settings))]
-        linked = link.link_many(fea, Phi, np.concatenate([[0], np.cumsum(lens)]), labels, [s.Fa for s in settings],
-                                [s.Fb for s in settings], dev, max_batch_bytes)
+        linked = link.link_many(fea, Phi, offs, labels, Fa, Fb, dev, max_batch_bytes,
+                                norm=None if norm is None else [st[:2] for st in norm['archive']])
         maps = [{t: link.link_cut(Z, table, t, [res[(k, b)][1] for b in range(len(names))]) for t in links}
                 for k, (table, _, _, Z) in enumerate(linked)]
+    if enrolled is not None:
+        from . import enroll as _enroll
+        en_norm = None if norm is None else [tuple(a[:2]) + tuple(e[:2]) for a, e in zip(norm['archive'],
+                                                                                          norm['enrolled'])]
+        en = _enroll.enroll_many(fea, Phi, offs, labels, enrolled_fea[0], enrolled_fea[1], Fa, Fb, enroll_thr, dev,
+                                 max_bytes=max_batch_bytes, norm=en_norm)
+        enrolled_names = [k for k, _ in enrolled]
+        named = [{t: _enroll.enroll_names(r.table, r.assign[h], r.best_llr[h], enrolled_names, names,
+                                          [res[(k, b)][1] for b in range(len(names))])
+                  for h, t in enumerate(enroll_thr)} for k, r in enumerate(en)]
     from . import score
     ovl = [None] * len(names)
     if with_overlap:
@@ -249,7 +321,7 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
                                                   overlap=o))
         keys = [(k, b) for k in range(len(settings)) for b in range(len(names))]
         jp = 'full' if jer else None
-        blk = maps is not None
+        blk = maps is not None or named is not None
         der = dict(zip(keys, score.score_entries(scored, [(b, res[(k, b)][0]) for k, b in keys], device=dev, jer=jp,
                                                  blocks=blk)))
         if with_overlap:
@@ -274,11 +346,16 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
                     item['jer_overlap'] = der_ovl[(k, b)]['jer']
             if maps is not None:
                 item['global_speakers'] = {t: maps[k][t][b] for t in links}
-                if der is not None:
-                    item['ref_speakers'] = ref[2][n]
-                    item['der_blocks'] = der[(k, b)]['O']
-                    if der_ovl is not None:
-                        item['der_overlap_blocks'] = der_ovl[(k, b)]['O']
+            if named is not None:
+                item['speaker_names'] = {t: named[k][t][0][b] for t in enroll_thr}
+                item['speaker_llr' if norm is None else 'speaker_score'] = {t: named[k][t][1][b] for t in enroll_thr}
+            if norm is not None:
+                item['score_norm'] = {'top_k': norm['K'], 'cohort_speakers': norm['C']}
+            if (maps is not None or named is not None) and der is not None:
+                item['ref_speakers'] = ref[2][n]
+                item['der_blocks'] = der[(k, b)]['O']
+                if der_ovl is not None:
+                    item['der_overlap_blocks'] = der_ovl[(k, b)]['O']
             out[s][n] = item
     return out
 
@@ -293,6 +370,50 @@ def check_link_thresholds(thresholds):
     if not out:
         raise ValueError('link_thresholds needs at least one value')
     return out
+
+
+def check_enroll_options(enroll, thresholds, dim):
+    """(enroll.check_enrolment's list or None, the enrolment thresholds or None) of sweep_batch's enroll and
+    enroll_thresholds: both or neither; the thresholds as enroll.check_thresholds takes them (duplicates dropped), and
+    no two with the same name f'{t:g}' (enroll_key), which would share one entry of the rankings."""
+    if enroll is None and thresholds is None:
+        return None, None
+    if enroll is None:
+        raise ValueError('enroll_thresholds without enroll')
+    if thresholds is None:
+        raise ValueError('enroll needs enroll_thresholds: the LLR is not calibrated, so there is no default')
+    from . import enroll as _enroll
+    thr = _enroll.check_thresholds(thresholds)
+    names = {}
+    for t in thr:                                     # their name in enroll_key and summary.json
+        if names.setdefault(f'{t:g}', t) != t:
+            raise ValueError(f'enrolment thresholds {names[f"{t:g}"]!r} and {t!r} have the same name {t:g} in the '
+                             'rankings and summary.json: give thresholds that differ in their first 6 significant digits')
+    return _enroll.check_enrolment(enroll, dim), thr
+
+
+def _cohort_norm_many(cohort_fea, top_k, settings, enrolled, enrolled_fea, names, fea, Phi, offs, labels, dev,
+                      max_bytes):
+    """DESIGN.md sections 5.17 and 5.19 for sweep_batch: the cohort statistics of every setting's speakers and of the
+    enrolled speakers under every setting's scalars, in batched cohort.cohort_stats_many calls, each checked for spread
+    per setting (ValueError naming the setting and the speaker, before any linking or enrolment kernel).  Returns
+    dict(archive: [CohortStats] per setting, enrolled: [CohortStats] per setting or None, K, C)."""
+    from . import cohort as _cohort
+    from .link import speaker_table
+    fea_c, spk_c = cohort_fea
+    Fa, Fb = [s.Fa for s in settings], [s.Fb for s in settings]
+    arch = _cohort.cohort_stats_many(fea, Phi, offs, labels, fea_c, spk_c, Fa, Fb, top_k, dev, max_bytes)
+    for s, st, l1 in zip(settings, arch, labels):
+        t = speaker_table(l1)
+        _cohort.check_spread(st.std, [f'setting {s.name}: {names[b]} speaker {l + 1}'
+                                      for b, l in zip(t.rec.tolist(), t.label.tolist())])
+    enr = None
+    if enrolled is not None:
+        enr = _cohort.cohort_stats_many(enrolled_fea[0], Phi, None, [enrolled_fea[1]] * len(settings), fea_c, spk_c,
+                                        Fa, Fb, top_k, dev, max_bytes)
+        for s, st in zip(settings, enr):
+            _cohort.check_spread(st.std, [f'setting {s.name}: enrolled {k}' for k, _ in enrolled])
+    return dict(archive=arch, enrolled=enr, K=min(top_k, int(spk_c.max()) + 1), C=int(spk_c.max()) + 1)
 
 
 def _load_reference(names, ref_rttm, uem):
@@ -373,6 +494,37 @@ def summarize_across_files(out, key='der'):
     return tot, ranking
 
 
+def enroll_key(setting, threshold):
+    """The ranking name of a setting named at an enrolment threshold, e.g. Fa0.3_Fb17_loopP0.99_thr-0.015_sm5_enroll20."""
+    return f'{setting.name}_enroll{threshold:g}'
+
+
+def summarize_by_name(out, key='der'):
+    """sweep_batch(enroll=, enroll_thresholds=, ref_rttm=) output with `key` ('der' or 'der_overlap') -> ({enroll_key(
+    setting, threshold): {protocol: DER by name}}, {protocol: those names by DER by name, stable in grid order, then
+    threshold order}).  Per (setting, threshold) each file's block columns (one per label) take the labels' names and
+    score.by_name_result sums them by name: host work only, no assignment is solved."""
+    from . import score
+    from .enroll import UNKNOWN
+    tot = {}
+    for s, per_rec in out.items():
+        if not per_rec:
+            continue
+        items = list(per_rec.values())
+        for t in items[0]['speaker_names']:
+            cols = []
+            for rec, it in per_rec.items():
+                m = it['speaker_names'][t]
+                n_cols = max((np.asarray(it[key + '_blocks'][p]).shape[1] for p, _, _ in score.PROTOCOLS), default=0)
+                cols.append([m.get(l, f'{UNKNOWN}{rec}-{l + 1}') for l in range(n_cols)])    # a label without turns
+            tot[enroll_key(s, t)] = {
+                p: score.by_name_result(score.overall([it[key][p] for it in items]), [it['ref_speakers'] for it in items],
+                                        cols, [it[key + '_blocks'][p] for it in items])
+                for p, _, _ in score.PROTOCOLS}
+    ranking = {p: score.rank({n: tot[n][p] for n in tot}) for p, _, _ in score.PROTOCOLS}
+    return tot, ranking
+
+
 def summarize_jer(out, key='jer'):
     """sweep_batch(jer=True) output with `key` ('jer' or 'jer_overlap') -> ({setting name: score.overall_jer dict},
     setting names by overall JER, stable in grid order, settings without a JER last)."""
@@ -409,13 +561,28 @@ def build_parser():
     ap.add_argument('--jer', action='store_true', help='also score and rank by Jaccard error rate (with --ref-rttm)')
     ap.add_argument('--link-threshold', default=None, type=parse_list,
                     help='comma-separated LLR thresholds: link every setting\'s speakers across the archive')
+    ap.add_argument('--enroll-ark', default=None, help='x-vectors of known speakers (Kaldi ark) to name speakers by')
+    ap.add_argument('--enroll-utt2spk', default=None, help='the speaker of each x-vector of --enroll-ark (utt2spk)')
+    ap.add_argument('--enroll-threshold', default=None, type=parse_list,
+                    help='comma-separated LLR thresholds at which a speaker takes an enrolled name')
+    ap.add_argument('--cohort-ark', default=None,
+                    help='x-vectors of cohort speakers (Kaldi ark), none of them in the archive, to normalise the '
+                         'linking and enrolment scores by')
+    ap.add_argument('--cohort-utt2spk', default=None, help='the speaker of each x-vector of --cohort-ark (utt2spk)')
+    ap.add_argument('--cohort-top', default=200, type=int,
+                    help="how many of each speaker's largest cohort scores set its mean and spread (default 200)")
     from .cli import add_count_options
     add_count_options(ap, allow_oracle=True)
     return ap
 
 
 def main(argv=None):
-    args = build_parser().parse_args(argv)
+    ap = build_parser()
+    args = ap.parse_args(argv)
+    if (args.enroll_ark is None) != (args.enroll_utt2spk is None):
+        ap.error('--enroll-ark and --enroll-utt2spk go together')
+    if (args.cohort_ark is None) != (args.cohort_utt2spk is None):
+        ap.error('--cohort-ark and --cohort-utt2spk go together')
     from . import formats
     segs = formats.read_segments(args.segments_file)
     plda = formats.read_kaldi_plda(args.plda_file)
@@ -432,7 +599,11 @@ def main(argv=None):
                       init=args.init, chain=args.chain, device=args.device, max_batch_bytes=args.max_batch_bytes,
                       ref_rttm=args.ref_rttm, uem=args.uem, overlaps=overlaps, oracle_overlaps=args.oracle_overlaps,
                       jer=args.jer, num_speakers=args.num_speakers, min_speakers=args.min_speakers,
-                      max_speakers=args.max_speakers, link_thresholds=args.link_threshold)
+                      max_speakers=args.max_speakers, link_thresholds=args.link_threshold,
+                      enroll=formats.read_enrolment(args.enroll_ark, args.enroll_utt2spk) if args.enroll_ark else None,
+                      enroll_thresholds=args.enroll_threshold,
+                      cohort=formats.read_enrolment(args.cohort_ark, args.cohort_utt2spk) if args.cohort_ark else None,
+                      cohort_top=args.cohort_top)
     summary = {}
     for s, per_rec in out.items():
         d = os.path.join(args.out_dir, s.name)
@@ -479,6 +650,18 @@ def main(argv=None):
                 for s in out:
                     for t in check_link_thresholds(args.link_threshold):
                         summary[s.name]['linked'][f'{t:g}']['der_across_files' + key[3:]] = tot[link_key(s, t)]
+    if args.enroll_threshold is not None:
+        ovl = overlaps is not None or args.oracle_overlaps
+        thr = list(dict.fromkeys(args.enroll_threshold))
+        for s, per_rec in out.items():
+            summary[s.name]['named'] = {f'{t:g}': dict(speaker_names={n: it['speaker_names'][t]
+                                                                        for n, it in per_rec.items()}) for t in thr}
+        if args.ref_rttm is not None:
+            for key in ('der', 'der_overlap') if ovl else ('der',):
+                tot, summary['ranking_by_name' + key[3:]] = summarize_by_name(out, key)
+                for s in out:
+                    for t in thr:
+                        summary[s.name]['named'][f'{t:g}']['der_by_name' + key[3:]] = tot[enroll_key(s, t)]
     with open(os.path.join(args.out_dir, 'summary.json'), 'w') as fp:
         json.dump(summary, fp, indent=1, sort_keys=True)
     return 0
