@@ -177,6 +177,27 @@ int vbx_hard_labels(vbx_handle_t h, const float *gamma, const int32_t *n_states,
 int vbx_hard_labels_keep(vbx_handle_t h, const float *gamma, const int32_t *n_states, const int32_t *keep,
                          int32_t *first_out, int32_t *second_out, double *mass_out, void *stream);
 
+/* Initial responsibilities from speaker turns (VB resegmentation of an existing diarization, DESIGN.md section 5.20),
+ * the generalisation of VBx/vbhmm.py:150-152's qinit to segments covered by several speakers or by none.  Runs on the
+ * handle's plan (vbx_plan or vbx_plan_f64: offsets, n_rec, S).  All arrays are DEVICE arrays:
+ *   seg [N,2] int64               x-vector t's segment [lo, hi) in ticks
+ *   spk_off [n_rec+1] int64       recording b has the speakers spk_off[b] .. spk_off[b+1]-1, K_b = their number <= S
+ *   turn_off [n_spk+1] int64      speaker k has the turns turn_off[k] .. turn_off[k+1]-1 (n_spk = spk_off[n_rec])
+ *   turn_lo, turn_hi [n_turns]    each speaker's turns [lo, hi) in ticks, sorted and disjoint
+ *   turn_cum [n_turns] int64      the exclusive prefix sum of the turn lengths within each speaker
+ *   smoothing [n_rec] float64
+ * With c_k = (ticks of [lo, hi) inside speaker k's turns) / (hi - lo) (0 when hi <= lo), the outputs are
+ *   gamma_out [N,S]   softmax_k(smoothing_b c_k) over k < K_b, 0 in the other columns (a segment no speaker covers gets
+ *                     a uniform row; a recording with K_b = 0 a row of zeros)
+ *   pi_out [n_rec,S]  1 / K_b in the first K_b columns, 0 in the others
+ * float64 (out_is_f64 != 0) or float32; the softmax is evaluated in float64 and rounded once.  A group of lanes per
+ * x-vector (S rounded up to a power of two, at most a warp) runs over the recording's speakers; the covered time is P(hi) - P(lo), P(x) = the speaker's turn time before x
+ * (binary search over turn_lo plus turn_cum, int64).  spk_off and turn_off are read back to check them (K_b > S or a
+ * negative count returns VBX_ERR_ARG), so the call waits for `stream`; otherwise stream ordered, no allocation. */
+int vbx_init_turns(vbx_handle_t h, const int64_t *seg, const int64_t *spk_off, const int64_t *turn_off,
+                   const int64_t *turn_lo, const int64_t *turn_hi, const int64_t *turn_cum, const double *smoothing,
+                   void *gamma_out, void *pi_out, int32_t out_is_f64, void *stream);
+
 /* Speaker linking across the recordings of an archive (DESIGN.md section 5.15); needs a handle, no plan.
  * M speakers (a recording's VB-HMM labels, numbered across the archive); all arrays are DEVICE arrays:
  *   fea [N,R] float32, Phi [R]   the features and between-speaker variances the VB-HMM ran with (R <= 128)

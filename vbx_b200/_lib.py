@@ -17,7 +17,7 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_enroll_workspace_bytes', 'vbx_enroll', 'vbx_cohort_workspace_bytes', 'vbx_cohort_stats', 'vbx_link_norm',
            'vbx_enroll_norm', 'vbx_link_batch_workspace_bytes', 'vbx_link_batch', 'vbx_link_batch_norm',
            'vbx_enroll_batch_workspace_bytes', 'vbx_enroll_batch', 'vbx_cohort_stats_batch_workspace_bytes',
-           'vbx_cohort_stats_batch']
+           'vbx_cohort_stats_batch', 'vbx_init_turns']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
@@ -136,6 +136,8 @@ def load():
     lib.vbx_cohort_stats_batch.restype = ctypes.c_int
     lib.vbx_cohort_stats_batch.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, i64, vp, i64, vp, vp, i32, vp,
                                            ctypes.c_size_t, vp, vp, vp]
+    lib.vbx_init_turns.restype = ctypes.c_int
+    lib.vbx_init_turns.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp]
     lib.vbx_get_timings.restype = ctypes.c_int
     lib.vbx_get_timings.argtypes = [vp, ctypes.POINTER(dbl), ctypes.POINTER(i64), i32]
     _lib = lib

@@ -177,6 +177,26 @@ class VbxBatch:
                                                   _ptr(sec), _ptr(mass), self._stream()))
         return first, sec, mass
 
+    def init_turns(self, pack, smoothing, gamma, pi):
+        """Initial responsibilities and priors of VB resegmentation (vbx_init_turns, DESIGN.md section 5.20) on this
+        batch's plan: pack, a resegment.TurnPack of the batch's recordings (host arrays); smoothing, a number or one per
+        recording.  gamma [N,S] and pi [B,S]: contiguous CUDA tensors, both float32 or both float64, overwritten."""
+        dt = gamma.dtype
+        for t, shape, name in ((gamma, (self.N, self.S), 'gamma'), (pi, (self.B, self.S), 'pi')):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dt and t.is_contiguous()
+                    and dt in (torch.float32, torch.float64) and tuple(t.shape) == shape):
+                raise ValueError(f'{name}: expected a contiguous float32 or float64 CUDA tensor of shape {shape}, '
+                                 'gamma and pi of one type')
+        if tuple(pack.seg.shape) != (self.N, 2) or len(pack.spk_off) != self.B + 1:
+            raise ValueError(f'pack: expected the segments of {self.N} x-vectors and the speakers of {self.B} recordings')
+        sm = np.broadcast_to(np.asarray(smoothing, dtype=np.float64), (self.B,)).copy()
+        if not np.all(np.isfinite(sm)):
+            raise ValueError('smoothing must be finite')
+        dev = lambda a, t=np.int64: torch.from_numpy(np.ascontiguousarray(a, dtype=t)).to(self.device)
+        arrays = [dev(a) for a in pack] + [dev(sm, np.float64)]
+        self._check(self.lib.vbx_init_turns(self._h, *(_ptr(a) for a in arrays), _ptr(gamma), _ptr(pi),
+                                            int(dt == torch.float64), self._stream()))
+
     @property
     def launches(self):
         return int(self.lib.vbx_launch_count(self._h))

@@ -29,6 +29,12 @@ With --cohort-ark FILE --cohort-utt2spk FILE (both or neither; needs --link-thre
 linking and enrolment scores are normalised against the cohort speakers of the ark (DESIGN.md section 5.17), speakers
 known to be none of the archive's: each score is standardised by the mean and spread of both speakers' --cohort-top
 (default 200) largest cohort scores, and --link-threshold and --enroll-threshold are on that normalised score.
+
+With --init RTTM+VB --init-rttm PATH (an RTTM file or directory holding every recording of the archive) the VB-HMM
+resegments an existing diarization instead of starting from AHC (DESIGN.md section 5.20): one state per speaker of the
+RTTM, each x-vector started from the speakers' shares of its segment.  The written RTTMs keep the input's speaker names
+(with --output-2nd the second-label RTTMs too) unless linking or enrolment name the speakers.  --threshold is still
+required, as by the reference's parser, and is used only by the AHC that the count bounds' rule 3 needs.
 """
 import argparse
 import os
@@ -72,7 +78,7 @@ def add_count_options(ap, allow_oracle=False):
 def build_parser():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     # option names, types and defaults of VBx/vbhmm.py:55-102
-    ap.add_argument('--init', required=True, type=str, choices=['AHC', 'AHC+VB'])
+    ap.add_argument('--init', required=True, type=str, choices=['AHC', 'AHC+VB', 'RTTM+VB'])
     ap.add_argument('--out-rttm-dir', required=True, type=str)
     ap.add_argument('--xvec-ark-file', required=True, type=str)
     ap.add_argument('--segments-file', required=True, type=str)
@@ -106,6 +112,8 @@ def build_parser():
     ap.add_argument('--cohort-utt2spk', default=None, help='the speaker of each x-vector of --cohort-ark (utt2spk)')
     ap.add_argument('--cohort-top', default=None, type=int,
                     help='how many of each speaker\'s largest cohort scores set its mean and spread (default 200)')
+    ap.add_argument('--init-rttm', default=None,
+                    help='with --init RTTM+VB: the diarization (RTTM file or directory of *.rttm) the VB-HMM starts from')
     return ap
 
 
@@ -125,6 +133,8 @@ def main(argv=None):
         ap.error('a cohort normalises the linking and enrolment scores: give --link-threshold or the enrolment options')
     if args.cohort_top is not None and args.cohort_top < 2:
         ap.error('--cohort-top must be >= 2')
+    if (args.init == 'RTTM+VB') != (args.init_rttm is not None):
+        ap.error('--init RTTM+VB and --init-rttm go together')
     from . import formats
     from .pipeline import diarize_batch, linked_lines, named_lines
     from .score import read_overlaps
@@ -146,11 +156,12 @@ def main(argv=None):
                         device=args.device, output_2nd=args.output_2nd, overlaps=overlaps,
                         num_speakers=args.num_speakers, min_speakers=args.min_speakers, max_speakers=args.max_speakers,
                         link_threshold=args.link_threshold, enroll=enroll, enroll_threshold=args.enroll_threshold,
-                        **norm_kw)
+                        init_rttm=args.init_rttm, **norm_kw)
     linked = args.link_threshold is not None
+    named_init = args.init == 'RTTM+VB' and enroll is None and not linked
     os.makedirs(args.out_rttm_dir, exist_ok=True)                           # VBx/vbhmm.py:170
     for name, item in out.items():
-        key = 'rttm_named' if enroll is not None else 'rttm_linked' if linked else \
+        key = 'rttm_named' if enroll is not None else 'rttm_linked' if linked else 'rttm_init' if named_init else \
             'rttm' if overlaps is None else 'rttm_overlap'
         with open(os.path.join(args.out_rttm_dir, f'{name}.rttm'), 'w') as fp:
             fp.write(''.join(line + os.linesep for line in item[key]))
@@ -159,6 +170,8 @@ def main(argv=None):
             os.makedirs(d2, exist_ok=True)
             if enroll is not None:
                 lines = named_lines(name, recs[name][1], item['labels2nd'], None, item['speaker_names'])
+            elif named_init and item['init_speakers'] is not None:
+                lines = named_lines(name, recs[name][1], item['labels2nd'], None, item['init_speakers'])
             else:
                 lines = item['rttm2nd'] if not linked else \
                     linked_lines(name, recs[name][1], item['labels2nd'], None, item['global_speakers'])

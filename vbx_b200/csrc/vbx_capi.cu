@@ -807,6 +807,44 @@ int vbx_hard_labels_keep(vbx_handle_t h, const float *gamma, const int32_t *n_st
                                                    (cudaStream_t)stream), "hard_labels_keep");
 }
 
+int vbx_init_turns(vbx_handle_t h, const int64_t *seg, const int64_t *spk_off, const int64_t *turn_off,
+                   const int64_t *turn_lo, const int64_t *turn_hi, const int64_t *turn_cum, const double *smoothing,
+                   void *gamma_out, void *pi_out, int32_t out_is_f64, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    if (!h->planned) return fail(h, VBX_ERR_STATE, "vbx_init_turns: call vbx_plan or vbx_plan_f64 first");
+    const vbx::Plan &pl = h->plan;
+    if (pl.n_rec == 0) return VBX_OK;
+    if (!spk_off || !turn_off || !smoothing || !pi_out || (pl.n_frames && (!seg || !gamma_out)))
+        return fail(h, VBX_ERR_ARG, "vbx_init_turns: null pointer");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    // the speaker and turn offsets live on the device: read them back once to refuse negative counts and K_b > S
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<int64_t> so(pl.n_rec + 1);
+    cudaError_t e = cudaMemcpyAsync(so.data(), spk_off, so.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return cuda_fail(h, e, "vbx_init_turns: reading spk_off");
+    if (so[0] != 0) return fail(h, VBX_ERR_ARG, "vbx_init_turns: spk_off[0] must be 0");
+    for (int b = 0; b < pl.n_rec; ++b) {
+        const int64_t K = so[b + 1] - so[b];
+        if (K < 0) return fail(h, VBX_ERR_ARG, "vbx_init_turns: recording " + std::to_string(b) + " has a negative speaker count");
+        if (K > pl.S)
+            return fail(h, VBX_ERR_ARG, "vbx_init_turns: recording " + std::to_string(b) + " has " + std::to_string(K) +
+                                            " speakers, more than the plan's S = " + std::to_string(pl.S));
+    }
+    std::vector<int64_t> to(so[pl.n_rec] + 1);
+    e = cudaMemcpyAsync(to.data(), turn_off, to.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return cuda_fail(h, e, "vbx_init_turns: reading turn_off");
+    if (to[0] != 0) return fail(h, VBX_ERR_ARG, "vbx_init_turns: turn_off[0] must be 0");
+    for (size_t k = 0; k + 1 < to.size(); ++k)
+        if (to[k + 1] < to[k])
+            return fail(h, VBX_ERR_ARG, "vbx_init_turns: speaker " + std::to_string(k) + " has a negative turn count");
+    if (to.back() > 0 && (!turn_lo || !turn_hi || !turn_cum)) return fail(h, VBX_ERR_ARG, "vbx_init_turns: null pointer");
+    return counted(h, vbx::launch_init_turns(pl, seg, spk_off, turn_off, turn_lo, turn_hi, turn_cum, smoothing, gamma_out,
+                                             pi_out, out_is_f64 != 0, st), "init_turns");
+}
+
 int vbx_ahc_workspace_bytes(vbx_handle_t h, size_t *bytes_out) {
     if (!h || !bytes_out) return VBX_ERR_ARG;
     if (!h->planned || h->f64_only) return fail(h, VBX_ERR_STATE, "vbx_ahc_workspace_bytes: call vbx_plan first");

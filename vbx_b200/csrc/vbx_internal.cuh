@@ -242,6 +242,10 @@ int launch_hard_labels(const Plan &pl, const float *gamma, const int32_t *n_stat
 // labels over the keep[b] states of largest posterior mass (vbx_count.cu)
 int launch_hard_labels_keep(const Plan &pl, const float *gamma, const int32_t *n_states, const int32_t *keep,
                             int32_t *first, int32_t *second, double *mass, cudaStream_t st);
+// initial responsibilities and priors from speaker turns (vbx_init.cu); gamma / pi are float64 when f64, else float32
+int launch_init_turns(const Plan &pl, const int64_t *seg, const int64_t *spk_off, const int64_t *turn_off,
+                      const int64_t *turn_lo, const int64_t *turn_hi, const int64_t *turn_cum, const double *smoothing,
+                      void *gamma, void *pi, bool f64, cudaStream_t st);
 // reference-module forward_backward() for a general transition matrix (vbx_fb_dense.cu)
 int launch_fb_dense(const double *lls, const double *tr, const double *ip, int T, int S, double *post, double *tll,
                     double *lfw, double *lbw, cudaStream_t st);

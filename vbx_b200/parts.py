@@ -175,6 +175,9 @@ class PartitionedBatch:
         self.whole.n_states = self._n_states
         return self.whole.hard_labels_keep(gamma, keep)
 
+    def init_turns(self, pack, smoothing, gamma, pi):
+        return self.whole.init_turns(pack, smoothing, gamma, pi)
+
     # ---- multi-GPU: the batch-wide ELBO trace and its collective live in the whole-batch handle ----
     def attach_comm(self, group=None):
         return self.whole.attach_comm(group)

@@ -170,10 +170,11 @@ def keep_labels(gamma, keep):
     return kept[f], (kept[s] if s is not None else torch.full_like(f, -1))
 
 
-def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None, **run_kw):
+def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None, turns=None, **run_kw):
     """The VB-HMM step (VBx/vbhmm.py:150-162) for the recordings of one state tier, packed: fea [N,R] float32, labels [N]
-    AHC labels (device).  f64: the float64 kernels (vbx_run_f64, any state count), else one float32 batch padded to the
-    tier, planned by `make` (default VbxBatch).  smoothing: a number or one per recording; run_kw go to run() (Fa, Fb,
+    AHC labels (device); turns: None, or a resegment.TurnPack of the recordings, which then start from their init
+    RTTM's turns instead (vbx_init_turns, DESIGN.md section 5.20; labels is not read).  f64: the float64 kernels
+    (vbx_run_f64, any state count), else one float32 batch padded to the tier, planned by `make` (default VbxBatch).  smoothing: a number or one per recording; run_kw go to run() (Fa, Fb,
     loopProb may be per-recording tensors there).  Returns [(labels, second-best labels or None, iterations, flags)] per
     recording.  hi: None, or an upper bound on the speaker count per recording: a recording whose labels hold more
     speakers takes rule 2 of DESIGN.md section 5.14 (the hi states of largest mass, one vbx_hard_labels_keep launch for
@@ -186,9 +187,12 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None
     sm = np.broadcast_to(np.asarray(smoothing, dtype=np.float64), (len(lens),))
     g = torch.zeros((vb.N, vb.S), dtype=dt, device=dev)
     p = torch.zeros((vb.B, vb.S), dtype=dt, device=dev)
-    for b in range(vb.B):              # VBx/vbhmm.py:150-152: qinit = softmax(onehot * smoothing)
-        g[offs[b]:offs[b + 1], :ns[b]] = soft_init(labels[offs[b]:offs[b + 1]], int(ns[b]), float(sm[b]), dtype=dt)
-        p[b, :ns[b]] = 1.0 / ns[b]
+    if turns is not None:              # softmax(smoothing * coverage) on the device, section 5.20
+        vb.init_turns(turns, sm, g, p)
+    else:
+        for b in range(vb.B):          # VBx/vbhmm.py:150-152: qinit = softmax(onehot * smoothing)
+            g[offs[b]:offs[b + 1], :ns[b]] = soft_init(labels[offs[b]:offs[b + 1]], int(ns[b]), float(sm[b]), dtype=dt)
+            p[b, :ns[b]] = 1.0 / ns[b]
     if f64:
         res = run_f64(vb, fea.double().contiguous(), Phi.double().contiguous(), g, p, **run_kw)   # VBx/vbhmm.py:154-158
         top2 = [hard_labels(g[offs[b]:offs[b + 1], :ns[b]], second=True) for b in range(vb.B)]   # VBx/vbhmm.py:160-162
@@ -229,7 +233,7 @@ def _tier(n_states):
     return 0 if n_states <= 64 else 1 if n_states <= MAX_STATES_F32 else 2
 
 
-def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, make, split, **run_kw):
+def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, make, split, turns=None, **run_kw):
     """Everything after AHC (VBx/vbhmm.py:147-162 and the speaker-count rules of DESIGN.md section 5.14) for the entries
     (k, b): setting k of `hyper`, a list of (Fa, Fb, loopP, smoothing), on recording b.  labels[k]: setting k's AHC
     labels per recording; labels_d[k]: their concatenation on the device (used by init='AHC+VB' only).  fea [N,R] float32
@@ -241,8 +245,11 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
     else as per-recording float64 tensors; the float64 tier runs once per setting.  Under
     bounds the first pass applies rule 2 inside _vb_tier, and rule 3 re-runs every entry with too few speakers from its
     recording's maxclust cut (one cut per recording, shared by all settings) through the same tiers.  run_kw go to run()
-    (maxIters, epsilon).  Returns {(k, b): (labels, labels2nd or None, iterations, flags[, n_speakers_vb, count_rule])},
-    the last two under bounds."""
+    (maxIters, epsilon).  init='RTTM+VB' (DESIGN.md section 5.20) runs the first pass from turns instead, one
+    (seg_times, resegment.load_init speaker list) per recording: recording b has one state per init speaker and each
+    batch starts from one vbx_init_turns launch (labels and labels_d are not read; Zs only by rule 3, whose re-runs start
+    from the AHC cut as above).  Returns {(k, b): (labels, labels2nd or None, iterations, flags[, n_speakers_vb,
+    count_rule])}, the last two under bounds."""
     from . import ahc as _ahc
     B = len(lens)
     entries = [(k, b) for k in range(len(hyper)) for b in range(B)]
@@ -255,8 +262,9 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
         return out
     offs = np.concatenate([[0], np.cumsum(lens)])
 
-    def run_tiers(entries, ns, labels_d, hi):
-        """The entries, with ns[e] states and their labels in labels_d[k], through the state tiers: {e: _vb_tier tuple}."""
+    def run_tiers(entries, ns, labels_d, hi, from_turns=False):
+        """The entries, with ns[e] states and their labels in labels_d[k] (from_turns: their recordings' init turns
+        instead), through the state tiers: {e: _vb_tier tuple}."""
         tiers = [[], [], []]
         for e in entries:
             tiers[_tier(ns[e])].append(e)
@@ -267,7 +275,13 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
             if not group:
                 continue
             recs = [b for _, b in group]
-            if recs == list(range(B)) and all(k == group[0][0] for k, _ in group):
+            init_kw = {}
+            if from_turns:
+                from .resegment import pack_turns
+                init_kw = dict(turns=pack_turns([turns[b] for b in recs]))
+                g_fea = fea if recs == list(range(B)) else torch.cat([fea[offs[b]:offs[b + 1]] for b in recs])
+                g_labels = None
+            elif recs == list(range(B)) and all(k == group[0][0] for k, _ in group):
                 g_fea, g_labels = fea, labels_d[group[0][0]]
             else:
                 g_fea = torch.cat([fea[offs[b]:offs[b + 1]] for b in recs])
@@ -280,12 +294,15 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
                 smoothing = [hyper[k][3] for k, _ in group]
             sub = _vb_tier(lens[recs], np.array([ns[e] for e in group], dtype=np.int32), g_fea, Phi, g_labels, f64,
                            smoothing, dev, make=make, hi=None if hi is None else hi[recs],
-                           Fa=Fa, Fb=Fb, loopProb=loopP, **run_kw)
+                           Fa=Fa, Fb=Fb, loopProb=loopP, **init_kw, **run_kw)
             out.update(zip(group, sub))
         return out
 
-    ns = {(k, b): int(labels[k][b].max()) + 1 if lens[b] else 1 for k, b in entries}
-    out = run_tiers(entries, ns, labels_d, None if bounds is None else bounds[1])
+    if init == 'RTTM+VB':
+        ns = {(k, b): len(turns[b][1]) for k, b in entries}
+    else:
+        ns = {(k, b): int(labels[k][b].max()) + 1 if lens[b] else 1 for k, b in entries}
+    out = run_tiers(entries, ns, labels_d, None if bounds is None else bounds[1], from_turns=init == 'RTTM+VB')
     if bounds is None:
         return out
     lo = bounds[0]
@@ -306,23 +323,31 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
     return out
 
 
-def _check_init(init, overlaps):
-    """init is 'AHC' or 'AHC+VB', and overlap-aware output (overlaps true) has the VB-HMM's second labels."""
-    if init not in ('AHC', 'AHC+VB'):
+def _check_init(init, overlaps, init_rttm=None):
+    """init is 'AHC', 'AHC+VB' or 'RTTM+VB', an init RTTM is given with 'RTTM+VB' and only with it, and overlap-aware
+    output (overlaps true) has the VB-HMM's second labels."""
+    if init not in ('AHC', 'AHC+VB', 'RTTM+VB'):
         raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
+    if init == 'RTTM+VB' and init_rttm is None:
+        raise ValueError("init='RTTM+VB' starts from an existing diarization: it needs init_rttm")
+    if init != 'RTTM+VB' and init_rttm is not None:
+        raise ValueError(f"init_rttm is the starting point of init='RTTM+VB', not of init={init!r}")
     if overlaps and init == 'AHC':
         raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
 
 
-def _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold):
+def _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold, ahc=True):
     """x-vector transform + PLDA projection and AHC (VBx/vbhmm.py:125-146) for the whole archive as one batch.  Returns
-    (fea [N,R] float32, Phi [R], AHC labels per recording at `threshold`, calibrated thresholds [B], linkage matrices)."""
+    (fea [N,R] float32, Phi [R], AHC labels per recording at `threshold`, calibrated thresholds [B], linkage matrices);
+    ahc=False: the projection only, and None for the last three."""
     from . import ahc as _ahc
     Dx = int(np.asarray(recordings[names[0]][0]).shape[1])
     chain = _resolve_chain(chain, transform, plda, lda_dim, Dx)
     x_all = np.concatenate([np.asarray(recordings[n][0], dtype=np.float64) for n in names])
     front, x, fea, Phi = _project(x_all, lens, transform, plda, lda_dim, chain, dev)
-    ahc_labels, th, Zs = _ahc.ahc_batch(front, x, threshold=threshold)      # VBx/vbhmm.py:131-146
+    ahc_labels = th = Zs = None
+    if ahc:
+        ahc_labels, th, Zs = _ahc.ahc_batch(front, x, threshold=threshold)      # VBx/vbhmm.py:131-146
     front.close()
     return fea, Phi, ahc_labels, th, Zs
 
@@ -445,7 +470,7 @@ def _count_fields(item, k1, rule, lo, hi):
 def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
                   max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False, overlaps=None,
                   num_speakers=None, min_speakers=None, max_speakers=None, link_threshold=None, enroll=None,
-                  enroll_threshold=None, cohort=None, cohort_top=200):
+                  enroll_threshold=None, cohort=None, cohort_top=200, init_rttm=None):
     """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
     recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
     one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
@@ -454,7 +479,15 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
 
     recordings: {name: (x_raw [T,Dx] float array, seg_times [T,2])} in archive order.  transform = (mean1, mean2, lda),
     plda = (mu, tr, psi) as read from the Kaldi model (diagonalised here as VBx/vbhmm.py:107-113 does).
-    init: 'AHC' (clustering only) or 'AHC+VB' (VBx/vbhmm.py:131,147).  chain: 'tcgen05' (fused tensor-core front end,
+    init: 'AHC' (clustering only), 'AHC+VB' (VBx/vbhmm.py:131,147) or 'RTTM+VB' (VB resegmentation, DESIGN.md section
+    5.20: the VB-HMM starts from init_rttm's speaker turns instead of AHC, one state per init speaker, gamma0 =
+    softmax(smoothing * the share of each segment inside each speaker's turns) from vbx_init_turns).  init_rttm: with
+    'RTTM+VB' only, an RTTM file or directory (score.read_rttm_path) or formats.read_rttm rows holding every recording
+    (ValueError naming the missing ones, or those without a speaker, before any device work).  Without count bounds
+    'RTTM+VB' runs no AHC; with them rule 2 applies as for 'AHC+VB' and rule 3 re-runs from the AHC linkage cut (its
+    states then have no init names).  Each item then also has init_speakers (the init speaker name of each state; None
+    for a rule 3 outcome) and rttm_init (its rttm lines, or rttm_overlap's with overlaps, with the speaker field set to
+    that name; the rttm or rttm_overlap lines themselves for a rule 3 outcome).  chain: 'tcgen05' (fused tensor-core front end,
     needs lda_dim == 128 and a 128-dim PLDA), 'float64' (float64 torch ops), 'auto' = tcgen05 when the shapes allow.
     overlaps: None, or overlap regions {name: [(onset, offset)] seconds} (score.read_overlaps; a recording it lacks has
     none): each item then also has rttm_overlap, the overlap-aware RTTM lines (overlap_segments: the second most likely
@@ -486,8 +519,8 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     ({label: the normalised score that decided the name}) in place of speaker_llr.
     Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds]
     [, count_rule, n_speakers_vb, count][, global_speakers, rttm_linked][, speaker_names, speaker_llr or speaker_score,
-    rttm_named][, score_norm])}."""
-    _check_init(init, overlaps is not None)
+    rttm_named][, score_norm][, init_speakers, rttm_init])}."""
+    _check_init(init, overlaps is not None, init_rttm)
     bounds = count_bounds(list(recordings), num_speakers, min_speakers, max_speakers)
     if link_threshold is not None:
         from .link import check_threshold
@@ -507,6 +540,11 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
             raise ValueError('a cohort normalises the linking and enrolment scores: it needs link_threshold or enroll')
         _cohort.check_top_k(cohort_top)
         cohort_set = _cohort.check_cohort(cohort, next(iter(dims)) if len(dims) == 1 else -1)
+    turns = None
+    if init == 'RTTM+VB':
+        from .resegment import load_init
+        init_turns = load_init(init_rttm, list(recordings))
+        turns = [(recordings[n][1], init_turns[n]) for n in recordings]
     if not torch.cuda.is_available():
         from ._lib import VbxError
         raise VbxError('diarize_batch(): no CUDA device - vbx_b200 has no CPU fallback')
@@ -515,15 +553,18 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
     if len(names) == 0:
         return {}
-    fea, Phi, ahc_labels, _, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold)
+    # resegmentation needs the AHC linkage for rule 3 of the count bounds only
+    fea, Phi, ahc_labels, _, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold,
+                                             ahc=init != 'RTTM+VB' or bounds is not None)
     offs = np.concatenate([[0], np.cumsum(lens)])
     labels_d = None
-    if init == 'AHC+VB':
+    if init != 'AHC':
         fea, Phi = _pad_features(fea, Phi)
+    if init == 'AHC+VB':
         labels_d = [torch.from_numpy(np.concatenate(ahc_labels)).to(dev)]
     from .batch import VbxBatch
     res = _vb_stage([(Fa, Fb, loopP, smoothing)], [ahc_labels], labels_d, Zs, lens, fea, Phi, bounds, init, dev,
-                    VbxBatch, None, maxIters=max_iters, epsilon=epsilon)
+                    VbxBatch, None, turns=turns, maxIters=max_iters, epsilon=epsilon)
     res = [res[(0, b)] for b in range(len(names))]
     labels1, labels2 = [r[0] for r in res], [r[1] for r in res]
     out = {}
@@ -559,7 +600,24 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
             out[n]['speaker_llr' if norm is None else 'speaker_score'] = spk_llr[b]
         if norm is not None:
             out[n]['score_norm'] = {'top_k': norm['K'], 'cohort_speakers': norm['C']}
+        if turns is not None:
+            init_fields(out[n], n, recordings[n][1], labels1[b], labels2[b], turns[b][1],
+                        None if bounds is None else res[b][5], ovl)
     return out
+
+
+def init_fields(item, name, seg_times, labels, labels2, turns, rule=None, overlap=None):
+    """The fields of an init='RTTM+VB' result (DESIGN.md section 5.20): init_speakers, the init RTTM's name of each state
+    (resegment.load_init speaker list `turns`), and rttm_init, the item's lines (overlap-aware with overlap regions)
+    with the speaker field set to that name.  A rule 3 outcome of the count bounds ('recut', 'ahc', 'unmet') has states
+    from the AHC cut: init_speakers None, rttm_init the item's own lines."""
+    if rule in ('recut', 'ahc', 'unmet'):
+        item.update(init_speakers=None, rttm_init=item['rttm' if overlap is None else 'rttm_overlap'])
+        return item
+    from .resegment import speaker_names
+    spk = speaker_names(turns)
+    item.update(init_speakers=spk, rttm_init=named_lines(name, seg_times, labels, labels2, spk, overlap))
+    return item
 
 
 def _side_features(sets, recordings, names, transform, plda, lda_dim, chain, dev, fea, Phi):

@@ -75,6 +75,15 @@ def reference_turns(rows):
 
 def named_reference_turns(rows):
     """reference_turns() with each speaker's RTTM name kept: {recording: [(name, (starts, ends))]}, same order."""
+    out = named_turns(rows)
+    for rec, turns in out.items():
+        if len(turns) > MAX_REF_SPEAKERS:
+            raise ValueError(f'recording {rec!r}: {len(turns)} reference speakers, at most {MAX_REF_SPEAKERS} are supported')
+    return out
+
+
+def named_turns(rows):
+    """named_reference_turns() without its cap on the number of speakers (which belongs to the score kernel)."""
     per = {}
     for rec, start, dur, spk in rows:
         per.setdefault(rec, {}).setdefault(spk, []).append((start, start + dur))
@@ -86,8 +95,6 @@ def named_reference_turns(rows):
             s, e = merge_turns(t[:, 0], t[:, 1])
             if len(s):
                 turns.append((spk, (s, e)))
-        if len(turns) > MAX_REF_SPEAKERS:
-            raise ValueError(f'recording {rec!r}: {len(turns)} reference speakers, at most {MAX_REF_SPEAKERS} are supported')
         out[rec] = turns
     return out
 

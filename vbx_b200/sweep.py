@@ -36,6 +36,9 @@ vbx_enroll_batch call.  summary.json then gains named = {threshold: speaker_name
 the names <setting>_enroll<threshold> by DER by name.  With --cohort-ark FILE --cohort-utt2spk FILE (both or neither;
 --cohort-top, default 200) both link and enrolment thresholds are on the normalised score of section 5.17.  No named
 RTTM files are written: cli with --enroll-threshold at the chosen setting reproduces them.
+With --init RTTM+VB --init-rttm PATH every setting resegments that diarization instead of starting from AHC (DESIGN.md
+section 5.20); --threshold must then hold one value.  The RTTM files keep their numbered speakers: cli with --init
+RTTM+VB at the chosen setting writes them with the input's speaker names.
 """
 import argparse
 import itertools
@@ -169,7 +172,7 @@ def packer(lens, R, device, budget):
 def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
                 device=None, max_batch_bytes=None, output_2nd=False, ref_rttm=None, uem=None, overlaps=None,
                 oracle_overlaps=False, jer=False, num_speakers=None, min_speakers=None, max_speakers=None,
-                link_thresholds=None, enroll=None, enroll_thresholds=None, cohort=None, cohort_top=200):
+                link_thresholds=None, enroll=None, enroll_thresholds=None, cohort=None, cohort_top=200, init_rttm=None):
     """Every setting of `grid` (see grid_settings) for every recording, with the front end and AHC run once.
 
     recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
@@ -214,6 +217,10 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     cohort.cohort_stats_many calls; a speaker without spread raises ValueError naming the setting and the speaker before
     any linking or enrolment kernel runs.  link_thresholds and enroll_thresholds are then on the normalised score S,
     every dict gains score_norm, and with enroll speaker_score replaces speaker_llr.
+    init='RTTM+VB', init_rttm: VB resegmentation as for diarize_batch (DESIGN.md section 5.20).  The init turns are read
+    and checked once and packed for every batch; each entry starts from its recording's turns with its setting's
+    smoothing.  The grid's threshold axis has no effect then and must hold exactly one value (ValueError otherwise).
+    Each dict gains init_speakers and rttm_init; the written RTTM files keep their numbered speakers.
     Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags[, der][, rttm_overlap,
     overlap_seconds][, der_overlap][, count_rule, n_speakers_vb, count][, global_speakers][, speaker_names, speaker_llr
     or speaker_score][, score_norm][, ref_speakers, der_blocks[, der_overlap_blocks]])}}; each recording's dict is the
@@ -223,7 +230,7 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     from ._lib import VbxError
     from .parts import make_batch
     from .pipeline import (_check_init, _count_fields, _front_end, _pad_features, _result, _side_features, _vb_stage,
-                           count_bounds)
+                           count_bounds, init_fields)
     settings = grid_settings(grid)
     links = check_link_thresholds(link_thresholds)
     dims = {int(np.asarray(r[0]).shape[1]) for r in recordings.values()}
@@ -237,7 +244,14 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
         _cohort.check_top_k(cohort_top)
         cohort_set = _cohort.check_cohort(cohort, dim)
     with_overlap = oracle_overlaps or overlaps is not None
-    _check_init(init, with_overlap)
+    _check_init(init, with_overlap, init_rttm)
+    init_from = None                                         # (seg_times, init speakers) per recording
+    if init == 'RTTM+VB':
+        from .resegment import load_init
+        if len({s.threshold for s in settings}) != 1:
+            raise ValueError("init='RTTM+VB' runs no AHC threshold cut: the grid's threshold axis must hold one value")
+        init_turns = load_init(init_rttm, list(recordings))
+        init_from = [(recordings[n][1], init_turns[n]) for n in recordings]
     if oracle_overlaps and ref_rttm is None:
         raise ValueError('oracle_overlaps are the overlaps of the reference: they need ref_rttm')
     if oracle_overlaps and overlaps is not None:
@@ -269,17 +283,21 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     if not names:
         return {s: {} for s in settings}
     lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
-    fea, Phi, _, th, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, 0.0)
+    with_ahc = init_from is None or bounds is not None          # resegmentation: the AHC linkage serves rule 3 only
+    fea, Phi, _, th, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, 0.0, ahc=with_ahc)
     fea, Phi = _pad_features(fea, Phi)
     thresholds = list(dict.fromkeys(s.threshold for s in settings))
-    ahc_labels = {t: _ahc.cut(Zs, th, lens, t) for t in thresholds}              # VBx/vbhmm.py:144-146, host only
-    lab_d = {t: torch.from_numpy(np.concatenate(ahc_labels[t])).to(dev) for t in thresholds}
+    ahc_labels = lab_d = {t: None for t in thresholds}
+    if init_from is None:
+        ahc_labels = {t: _ahc.cut(Zs, th, lens, t) for t in thresholds}              # VBx/vbhmm.py:144-146, host only
+        lab_d = {t: torch.from_numpy(np.concatenate(ahc_labels[t])).to(dev) for t in thresholds}
     if max_batch_bytes is None:
         max_batch_bytes = int(torch.cuda.mem_get_info(dev)[0] * BUDGET_FRACTION)
     # per (setting, recording): labels, labels2nd, iterations, flags[, unconstrained count, rule]
     res = _vb_stage([(s.Fa, s.Fb, s.loopP, s.smoothing) for s in settings], [ahc_labels[s.threshold] for s in settings],
                     [lab_d[s.threshold] for s in settings], Zs, lens, fea, Phi, bounds, init, dev, make_batch,
-                    packer(lens, int(fea.shape[1]), dev, max_batch_bytes), maxIters=max_iters, epsilon=epsilon)
+                    packer(lens, int(fea.shape[1]), dev, max_batch_bytes), turns=init_from, maxIters=max_iters,
+                    epsilon=epsilon)
     maps = named = norm = None
     if links is not None or enrolled is not None:
         offs = np.concatenate([[0], np.cumsum(lens)])
@@ -351,6 +369,9 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
                 item['speaker_llr' if norm is None else 'speaker_score'] = {t: named[k][t][1][b] for t in enroll_thr}
             if norm is not None:
                 item['score_norm'] = {'top_k': norm['K'], 'cohort_speakers': norm['C']}
+            if init_from is not None:
+                init_fields(item, n, recordings[n][1], l1, l2, init_from[b][1],
+                            None if bounds is None else res[(k, b)][5], ovl[b])
             if (maps is not None or named is not None) and der is not None:
                 item['ref_speakers'] = ref[2][n]
                 item['der_blocks'] = der[(k, b)]['O']
@@ -535,7 +556,9 @@ def summarize_jer(out, key='jer'):
 
 def build_parser():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
-    ap.add_argument('--init', default='AHC+VB', choices=['AHC', 'AHC+VB'])
+    ap.add_argument('--init', default='AHC+VB', choices=['AHC', 'AHC+VB', 'RTTM+VB'])
+    ap.add_argument('--init-rttm', default=None,
+                    help='with --init RTTM+VB: the diarization (RTTM file or directory of *.rttm) the VB-HMM starts from')
     ap.add_argument('--out-dir', required=True, type=str)
     ap.add_argument('--xvec-ark-file', required=True, type=str)
     ap.add_argument('--segments-file', required=True, type=str)
@@ -583,6 +606,8 @@ def main(argv=None):
         ap.error('--enroll-ark and --enroll-utt2spk go together')
     if (args.cohort_ark is None) != (args.cohort_utt2spk is None):
         ap.error('--cohort-ark and --cohort-utt2spk go together')
+    if (args.init == 'RTTM+VB') != (args.init_rttm is not None):
+        ap.error('--init RTTM+VB and --init-rttm go together')
     from . import formats
     segs = formats.read_segments(args.segments_file)
     plda = formats.read_kaldi_plda(args.plda_file)
@@ -603,7 +628,7 @@ def main(argv=None):
                       enroll=formats.read_enrolment(args.enroll_ark, args.enroll_utt2spk) if args.enroll_ark else None,
                       enroll_thresholds=args.enroll_threshold,
                       cohort=formats.read_enrolment(args.cohort_ark, args.cohort_utt2spk) if args.cohort_ark else None,
-                      cohort_top=args.cohort_top)
+                      cohort_top=args.cohort_top, init_rttm=args.init_rttm)
     summary = {}
     for s, per_rec in out.items():
         d = os.path.join(args.out_dir, s.name)
