@@ -460,6 +460,53 @@ int vbx_score_jer(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets, con
                   int64_t *both_out, int64_t *fa_out, int64_t *O_out, int32_t *flags_out, const int64_t *t_offsets,
                   int64_t *label_time_out, void *stream);
 
+/* per-recording bits written to flags_out by vbx_combine */
+enum vbx_combine_flag {
+    VBX_COMBINE_BAD_LABEL = 1,       /* a label of some hypothesis outside [-1, n_labels), a second label without a
+                                        first or equal to it: that interval of that hypothesis counted as silent   */
+    VBX_COMBINE_TOO_MANY_LABELS = 2  /* more than 255 global labels: n_global 0, every output label of the recording
+                                        -1, its map rows incomplete                                                */
+};
+
+/* Combination of K diarizations of the same intervals into one by label mapping and weighted voting (DESIGN.md section
+ * 5.21; DOVER with up to two labels per interval), many recordings per call; needs a handle, no plan.
+ * Times are int64 microseconds ("ticks").  DEVICE arrays unless marked HOST:
+ *   offsets [n_rec+1]            recording r owns intervals offsets[r] .. offsets[r+1]-1 of the N = offsets[n_rec] packed
+ *                                ones (N is passed on the host as well)
+ *   lo, hi [N]                   interval i is [lo, hi), sorted and disjoint inside a recording; empty when hi <= lo
+ *   labels, labels2 [K, N] int32 row k: hypothesis k's first and second label of every interval, -1 = none
+ *   n_labels [n_rec, K] (HOST)   hypothesis k's labels in recording r lie in [-1, n_labels[r, k]); 0 <= it <= max_labels
+ *   max_labels (HOST)            1 .. 128: the row length of the O and L blocks
+ *   weights [K] (HOST) or NULL   w_k, finite and > 0; NULL: rank ** -0.1 by ascending summed disagreement
+ * Per recording: O_ab[s, u] = ticks in which hypothesis a says s and b says u (either stream), L_a[s] = ticks in which a
+ * says s; D[a, b] = sum L_a + sum L_b - 2 x the maximum one-to-one matching of O_ab; the hypotheses ordered by their row
+ * sum of D (ties: the lower index), the first being the anchor; global labels = the anchor's labels with time, then
+ * every later hypothesis in that order assigned one-to-one to the global labels by the ticks it shares with the labels
+ * already mapped to them (no pair without shared ticks; its unmatched labels with time get new ids in label order);
+ * per interval n = floor(0.5 + sum_k w_k c_k / sum_k w_k) labels are kept (c_k = labels hypothesis k gives it), those
+ * of largest summed weight, ties to the lower global id.  Outputs:
+ *   labels_out, labels2_out [N] int32        the combined first and second global label, -1 = none
+ *   order_out [n_rec, K] int32               hypotheses by rank (order_out[r, 0] is the anchor)
+ *   weights_out [n_rec, K]                   w_k by hypothesis index
+ *   D_out [n_rec, K, K] int64                the disagreements, symmetric, zero diagonal
+ *   map_out [n_rec, K, 128] int32            the global label of label s of hypothesis k, -1 for a label without time
+ *   n_global_out [n_rec] int32, flags_out [n_rec] int32 (vbx_combine_flag bits)
+ *   O_out [n_rec, K (K-1)/2, max_labels, max_labels], L_out [n_rec, K, max_labels] int64: optional (NULL: kept in the
+ *     workspace); pair (a, b), a < b, is block a (2 K - a - 1) / 2 + b - a - 1, rows = a's labels
+ * Integer sums and fixed-order float64 sums: a recording's outputs are bit-identical whatever else shares the call.
+ * Where an assignment has several optima the one returned is that of shortest augmenting paths over the rows in label
+ * order with ties in a step going to the lowest column (global ids before "unmatched").
+ * workspace: vbx_combine_workspace_bytes(n_rec, K, max_labels) bytes, 256-byte aligned.  Stream ordered, no allocation,
+ * no host synchronisation: n_labels goes to the device in one copy from pageable host memory.  VBX_ERR_ARG: null
+ * pointers, K outside 2..32, negative counts, max_labels outside 1..128, an n_labels outside [0, max_labels], a weight
+ * that is not finite and > 0, n_rec (K (K-1)/2 + K) above 2^31 - 1, a short or misaligned workspace. */
+int vbx_combine_workspace_bytes(vbx_handle_t h, int32_t n_rec, int32_t K, int32_t max_labels, size_t *bytes_out);
+int vbx_combine(vbx_handle_t h, int32_t n_rec, const int64_t *offsets, int64_t N, const int64_t *lo, const int64_t *hi,
+                int32_t K, const int32_t *labels, const int32_t *labels2, const int32_t *n_labels, int32_t max_labels,
+                const double *weights, void *workspace, size_t workspace_bytes, int32_t *labels_out,
+                int32_t *labels2_out, int32_t *order_out, double *weights_out, int64_t *D_out, int32_t *map_out,
+                int32_t *n_global_out, int32_t *flags_out, int64_t *O_out, int64_t *L_out, void *stream);
+
 /* Number of kernels launched by this handle since creation (bench.py reports it as gpu_launches). */
 int64_t vbx_launch_count(vbx_handle_t h);
 

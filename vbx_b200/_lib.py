@@ -17,10 +17,11 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_enroll_workspace_bytes', 'vbx_enroll', 'vbx_cohort_workspace_bytes', 'vbx_cohort_stats', 'vbx_link_norm',
            'vbx_enroll_norm', 'vbx_link_batch_workspace_bytes', 'vbx_link_batch', 'vbx_link_batch_norm',
            'vbx_enroll_batch_workspace_bytes', 'vbx_enroll_batch', 'vbx_cohort_stats_batch_workspace_bytes',
-           'vbx_cohort_stats_batch', 'vbx_init_turns']
+           'vbx_cohort_stats_batch', 'vbx_init_turns', 'vbx_combine_workspace_bytes', 'vbx_combine']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
+COMBINE_BAD_LABEL, COMBINE_TOO_MANY_LABELS = 1, 2                  # vbx_combine flags
 LINK_MAX_SPEAKERS = 1 << 29                                        # VBX_LINK_MAX_SPEAKERS
 KERNEL_CLASSES = ['project', 'prepare', 'run_init', 'mstep_partial', 'speaker_model', 'loglik', 'forward_backward', 'exact64']
 
@@ -138,6 +139,11 @@ def load():
                                            ctypes.c_size_t, vp, vp, vp]
     lib.vbx_init_turns.restype = ctypes.c_int
     lib.vbx_init_turns.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp]
+    lib.vbx_combine_workspace_bytes.restype = ctypes.c_int
+    lib.vbx_combine_workspace_bytes.argtypes = [vp, i32, i32, i32, ctypes.POINTER(ctypes.c_size_t)]
+    lib.vbx_combine.restype = ctypes.c_int
+    lib.vbx_combine.argtypes = [vp, i32, vp, i64, vp, vp, i32, vp, vp, vp, i32, vp, vp, ctypes.c_size_t, vp, vp, vp, vp,
+                                vp, vp, vp, vp, vp, vp, vp]
     lib.vbx_get_timings.restype = ctypes.c_int
     lib.vbx_get_timings.argtypes = [vp, ctypes.POINTER(dbl), ctypes.POINTER(i64), i32]
     _lib = lib

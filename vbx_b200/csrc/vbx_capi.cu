@@ -1338,6 +1338,61 @@ int vbx_score_jer(vbx_handle_t h, int32_t n_rec, const int64_t *sys_offsets, con
                    labels2 ? "score_jer_overlap" : "score_jer");
 }
 
+static int check_combine_sizes(vbx_handle_t h, const std::string &who, int32_t n_rec, int32_t K, int32_t max_labels) {
+    if (n_rec < 0) return fail(h, VBX_ERR_ARG, who + ": negative count");
+    if (K < 2 || K > 32) return fail(h, VBX_ERR_ARG, who + ": K must lie in [2, 32]");
+    if (max_labels < 1 || max_labels > 128) return fail(h, VBX_ERR_ARG, who + ": max_labels must lie in [1, 128]");
+    if ((int64_t)n_rec * (K * (K - 1) / 2 + K) > INT32_MAX)
+        return fail(h, VBX_ERR_ARG, who + ": n_rec (K (K - 1) / 2 + K) must stay below 2^31");
+    return VBX_OK;
+}
+
+int vbx_combine_workspace_bytes(vbx_handle_t h, int32_t n_rec, int32_t K, int32_t max_labels, size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    const int rc = check_combine_sizes(h, "vbx_combine_workspace_bytes", n_rec, K, max_labels);
+    if (rc != VBX_OK) return rc;
+    *bytes_out = vbx::combine_workspace_bytes(n_rec, K, max_labels);
+    return VBX_OK;
+}
+
+int vbx_combine(vbx_handle_t h, int32_t n_rec, const int64_t *offsets, int64_t N, const int64_t *lo, const int64_t *hi,
+                int32_t K, const int32_t *labels, const int32_t *labels2, const int32_t *n_labels, int32_t max_labels,
+                const double *weights, void *workspace, size_t workspace_bytes, int32_t *labels_out,
+                int32_t *labels2_out, int32_t *order_out, double *weights_out, int64_t *D_out, int32_t *map_out,
+                int32_t *n_global_out, int32_t *flags_out, int64_t *O_out, int64_t *L_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_combine");
+    const std::string who("vbx_combine");
+    const int rc = check_combine_sizes(h, who, n_rec, K, max_labels);
+    if (rc != VBX_OK) return rc;
+    if (N < 0) return fail(h, VBX_ERR_ARG, who + ": negative count");
+    if (weights)
+        for (int32_t k = 0; k < K; ++k)
+            if (!(std::isfinite(weights[k]) && weights[k] > 0.0))
+                return fail(h, VBX_ERR_ARG, who + ": weights[" + std::to_string(k) + "] must be finite and > 0");
+    if (n_rec == 0) {
+        if (N != 0) return fail(h, VBX_ERR_ARG, who + ": intervals need at least one recording");
+        return VBX_OK;
+    }
+    if (!offsets || !n_labels || !workspace || !order_out || !weights_out || !D_out || !map_out || !n_global_out ||
+        !flags_out || (N > 0 && (!lo || !hi || !labels || !labels2 || !labels_out || !labels2_out)))
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    for (int64_t i = 0; i < (int64_t)n_rec * K; ++i)
+        if (n_labels[i] < 0 || n_labels[i] > max_labels)
+            return fail(h, VBX_ERR_ARG, who + ": n_labels[" + std::to_string(i / K) + ", " + std::to_string(i % K) +
+                                            "] must lie in [0, max_labels]");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
+        return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
+    if (workspace_bytes < vbx::combine_workspace_bytes(n_rec, K, max_labels))
+        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_combine_workspace_bytes()");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_combine(n_rec, offsets, N, lo, hi, K, labels, labels2, n_labels, max_labels, weights,
+                                          workspace, labels_out, labels2_out, order_out, weights_out, D_out, map_out,
+                                          n_global_out, flags_out, O_out, L_out, (cudaStream_t)stream),
+                   "combine");
+}
+
 int vbx_attach_comm(vbx_handle_t h, void *nccl_comm, int32_t n_ranks, const char *libnccl_path) {
     if (!h) return VBX_ERR_ARG;
     if (!nccl_comm) {   // detach

@@ -259,6 +259,13 @@ int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const
                  int64_t *fa_out, int64_t *O_out, int32_t *flags_out,
                  const int64_t *t_off, int64_t *T_out,                // T_out == nullptr: no label time
                  cudaStream_t st);
+// combination of K diarizations (vbx_combine.cu): n_labels_host [n_rec, K] and weights_host [K] (or null) on the HOST
+size_t combine_workspace_bytes(int64_t n_rec, int K, int max_labels);
+int launch_combine(int64_t n_rec, const int64_t *offsets, int64_t N, const int64_t *lo, const int64_t *hi, int K,
+                   const int32_t *labels, const int32_t *labels2, const int32_t *n_labels_host, int max_labels,
+                   const double *weights_host, void *workspace, int32_t *labels_out, int32_t *labels2_out,
+                   int32_t *order_out, double *weights_out, int64_t *D_out, int32_t *map_out, int32_t *n_global_out,
+                   int32_t *flags_out, int64_t *O_out, int64_t *L_out, cudaStream_t st);
 // AHC initialisation (vbx_ahc.cu)
 size_t ahc_workspace_bytes(const int64_t *offsets_host, int n_rec, std::vector<int64_t> *d_off_host);
 int launch_ahc(const Plan &pl, const std::vector<int64_t> &d_off, const void *x, int x_is_f64, int dim, void *workspace,

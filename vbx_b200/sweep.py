@@ -39,6 +39,10 @@ RTTM files are written: cli with --enroll-threshold at the chosen setting reprod
 With --init RTTM+VB --init-rttm PATH every setting resegments that diarization instead of starting from AHC (DESIGN.md
 section 5.20); --threshold must then hold one value.  The RTTM files keep their numbered speakers: cli with --init
 RTTM+VB at the chosen setting writes them with the input's speaker names.
+With --combine N (the N best settings of ranking['full']; needs --ref-rttm) or --combine all, those settings' outputs are
+combined into one by label mapping and weighted voting (DESIGN.md section 5.21): OUT/combined/<recording>.rttm, and
+summary.json gains combined = {hypotheses, recordings: {name: order, weights, speakers}[, der][, jer]}, scored under
+the same protocols.  Every other key of summary.json is as without --combine.
 """
 import argparse
 import itertools
@@ -554,8 +558,68 @@ def summarize_jer(out, key='jer'):
     return tot, score.rank(tot, key='jer')
 
 
+def combine_settings(out, recordings, settings=None, weights=None, device=None):
+    """Combine the outputs of several settings of sweep_batch's return value `out` into one diarization per recording
+    (DESIGN.md section 5.21), in one vbx_combine call over all recordings.  recordings: the dict sweep_batch was given
+    (its segment times are the shared intervals, score.owned_intervals, so no timeline union is needed); settings: the
+    Settings to combine, in the order that breaks ties (None: all, in grid order), 2 .. 32 of them; weights: None (rank
+    ** -0.1 per recording) or one per setting.  Each setting votes with its first labels: labels2nd is its second most
+    likely speaker of every x-vector, not a claim that two people speak, and as a second label it would vote for a second
+    speaker everywhere.  Returns {recording: dict(rttm, labels, n_speakers, order (indices into settings), weights, D,
+    map, n_global)}."""
+    from . import combine, score
+    from .pipeline import merge_adjacent_labels, rttm_lines
+    settings = list(out) if settings is None else list(settings)
+    missing = [s for s in settings if s not in out]
+    if missing:
+        raise ValueError(f'settings the sweep did not run: {[getattr(s, "name", s) for s in missing]}')
+    if not 2 <= len(settings) <= combine.MAX_HYPOTHESES:
+        raise ValueError(f'{len(settings)} settings: combination takes 2 .. {combine.MAX_HYPOTHESES}')
+    names = list(out[settings[0]])
+    intervals = [score.owned_intervals(recordings[n][1])[:2] for n in names]
+    hyps = [[(out[s][n]['labels'], None) for n in names] for s in settings]
+    res = combine.combine_labels(intervals, hyps, weights, device)
+    comb = {}
+    for n, item in zip(names, res):
+        seg = np.asarray(recordings[n][1], dtype=np.float64).reshape(-1, 2)
+        lines = rttm_lines(n, *merge_adjacent_labels(seg[:, 0], seg[:, 1], item['labels']))
+        comb[n] = dict(rttm=lines, labels=item['labels'], n_speakers=int(len(set(item['labels'].tolist()))),
+                       order=item['order'], weights=item['weights'], D=item['D'], map=item['map'],
+                       n_global=item['n_global'])
+    return comb
+
+
+def score_combined(comb, recordings, ref_rttm, uem=None, jer=False, device=None):
+    """The DER (and JER) of combine_settings' output under score.PROTOCOLS, as sweep_batch scores a setting: ({protocol:
+    overall result dict}, overall JER dict or None)."""
+    from . import score
+    names = list(comb)
+    turns, uem_map, _ = _load_reference(names, ref_rttm, uem)
+    scored = [score.prepare_recording(n, turns[n], score.owned_intervals(recordings[n][1]),
+                                      None if uem_map is None else uem_map[n]) for n in names]
+    res = score.score_entries(scored, [(b, comb[n]['labels']) for b, n in enumerate(names)], device=device,
+                              jer='full' if jer else None)
+    der = {p: score.overall([r[p] for r in res]) for p, _, _ in score.PROTOCOLS}
+    return der, score.overall_jer([r['jer'] for r in res]) if jer else None
+
+
+def parse_combine(text):
+    """--combine: 'all' or an integer >= 2."""
+    if str(text) == 'all':
+        return 'all'
+    try:
+        n = int(text)
+    except ValueError:
+        n = 0
+    if n < 2:
+        raise argparse.ArgumentTypeError(f"expected 'all' or an integer >= 2, got {text!r}")
+    return n
+
+
 def build_parser():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument('--combine', default=None, type=parse_combine,
+                    help="combine the N best settings (needs --ref-rttm), or 'all', into OUT/combined/*.rttm")
     ap.add_argument('--init', default='AHC+VB', choices=['AHC', 'AHC+VB', 'RTTM+VB'])
     ap.add_argument('--init-rttm', default=None,
                     help='with --init RTTM+VB: the diarization (RTTM file or directory of *.rttm) the VB-HMM starts from')
@@ -608,6 +672,8 @@ def main(argv=None):
         ap.error('--cohort-ark and --cohort-utt2spk go together')
     if (args.init == 'RTTM+VB') != (args.init_rttm is not None):
         ap.error('--init RTTM+VB and --init-rttm go together')
+    if isinstance(args.combine, int) and args.ref_rttm is None:
+        ap.error('--combine N takes the N best settings by DER: it needs --ref-rttm (or --combine all)')
     from . import formats
     segs = formats.read_segments(args.segments_file)
     plda = formats.read_kaldi_plda(args.plda_file)
@@ -687,6 +753,21 @@ def main(argv=None):
                 for s in out:
                     for t in thr:
                         summary[s.name]['named'][f'{t:g}']['der_by_name' + key[3:]] = tot[enroll_key(s, t)]
+    if args.combine is not None:
+        by_name = {s.name: s for s in out}
+        chosen = list(out) if args.combine == 'all' else [by_name[n] for n in summary['ranking']['full'][:args.combine]]
+        comb = combine_settings(out, recs, chosen, device=args.device)
+        os.makedirs(os.path.join(args.out_dir, 'combined'), exist_ok=True)
+        block = summary['combined'] = dict(hypotheses=[s.name for s in chosen], recordings={})
+        for name, item in comb.items():
+            with open(os.path.join(args.out_dir, 'combined', f'{name}.rttm'), 'w') as fp:
+                fp.write(''.join(line + os.linesep for line in item['rttm']))
+            block['recordings'][name] = dict(order=item['order'], weights=[float(w) for w in item['weights']],
+                                             speakers=item['n_speakers'])
+        if args.ref_rttm is not None:
+            block['der'], jer_tot = score_combined(comb, recs, args.ref_rttm, args.uem, args.jer, args.device)
+            if args.jer:
+                block['jer'] = jer_tot
     with open(os.path.join(args.out_dir, 'summary.json'), 'w') as fp:
         json.dump(summary, fp, indent=1, sort_keys=True)
     return 0
