@@ -198,6 +198,21 @@ int vbx_init_turns(vbx_handle_t h, const int64_t *seg, const int64_t *spk_off, c
                    const int64_t *turn_lo, const int64_t *turn_hi, const int64_t *turn_cum, const double *smoothing,
                    void *gamma_out, void *pi_out, int32_t out_is_f64, void *stream);
 
+/* Random initial responsibilities (the VB-HMM started without AHC, DESIGN.md section 5.22): the flat-Dirichlet rows of
+ * VBx/VBx.py:79-83 drawn from a counter-based generator, so that every restart of every recording can share one batch.
+ * Runs on the handle's plan (vbx_plan or vbx_plan_f64: offsets, n_rec, S).  All arrays are DEVICE arrays:
+ *   rec_key [n_rec] uint64   the recording's stream (the first 8 bytes, little-endian, of SHA-256 of its name)
+ *   seed [n_rec] uint64      the restart's seed
+ *   n_states [n_rec] int32   live states N_b <= S per recording, or NULL = S for all (as for vbx_run)
+ * For x-vector t of recording b (its index inside the recording) and state block j = s / 4, Philox4x64-10 (Salmon et
+ * al. 2011) on counter (t, j, rec_key[b], 0) with key (seed[b], 0) gives four words; word i belongs to state 4j + i:
+ *   u = ((w >> 11) + 0.5) 2^-53,  e_s = -log u,  gamma_out[t, s] = e_s / sum_{s' < N_b} e_s'  (0 in the other columns)
+ *   pi_out [n_rec,S] = 1 / N_b in the first N_b columns, 0 in the others
+ * float64 (out_is_f64 != 0) or float32; evaluated in float64 and rounded once.  A row's bits depend on (rec_key, seed,
+ * t, N_b) only, not on S or the rest of the batch.  Stream ordered, no allocation, no host synchronisation. */
+int vbx_init_random(vbx_handle_t h, const uint64_t *rec_key, const uint64_t *seed, const int32_t *n_states,
+                    void *gamma_out, void *pi_out, int32_t out_is_f64, void *stream);
+
 /* Speaker linking across the recordings of an archive (DESIGN.md section 5.15); needs a handle, no plan.
  * M speakers (a recording's VB-HMM labels, numbered across the archive); all arrays are DEVICE arrays:
  *   fea [N,R] float32, Phi [R]   the features and between-speaker variances the VB-HMM ran with (R <= 128)

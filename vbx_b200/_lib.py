@@ -17,7 +17,8 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_enroll_workspace_bytes', 'vbx_enroll', 'vbx_cohort_workspace_bytes', 'vbx_cohort_stats', 'vbx_link_norm',
            'vbx_enroll_norm', 'vbx_link_batch_workspace_bytes', 'vbx_link_batch', 'vbx_link_batch_norm',
            'vbx_enroll_batch_workspace_bytes', 'vbx_enroll_batch', 'vbx_cohort_stats_batch_workspace_bytes',
-           'vbx_cohort_stats_batch', 'vbx_init_turns', 'vbx_combine_workspace_bytes', 'vbx_combine']
+           'vbx_cohort_stats_batch', 'vbx_init_turns', 'vbx_combine_workspace_bytes', 'vbx_combine',
+           'vbx_init_random']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
@@ -139,6 +140,8 @@ def load():
                                            ctypes.c_size_t, vp, vp, vp]
     lib.vbx_init_turns.restype = ctypes.c_int
     lib.vbx_init_turns.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp]
+    lib.vbx_init_random.restype = ctypes.c_int
+    lib.vbx_init_random.argtypes = [vp, vp, vp, vp, vp, vp, i32, vp]
     lib.vbx_combine_workspace_bytes.restype = ctypes.c_int
     lib.vbx_combine_workspace_bytes.argtypes = [vp, i32, i32, i32, ctypes.POINTER(ctypes.c_size_t)]
     lib.vbx_combine.restype = ctypes.c_int

@@ -197,6 +197,27 @@ class VbxBatch:
         self._check(self.lib.vbx_init_turns(self._h, *(_ptr(a) for a in arrays), _ptr(gamma), _ptr(pi),
                                             int(dt == torch.float64), self._stream()))
 
+    def init_random(self, rec_keys, seeds, gamma, pi):
+        """Random initial responsibilities and uniform priors (vbx_init_random, DESIGN.md section 5.22) on this batch's
+        plan and live state counts: rec_keys and seeds, one integer in [0, 2^64) per recording (random_init.name_key and
+        the restart's seed).  gamma [N,S] and pi [B,S]: contiguous CUDA tensors, both float32 or both float64,
+        overwritten."""
+        dt = gamma.dtype
+        for t, shape, name in ((gamma, (self.N, self.S), 'gamma'), (pi, (self.B, self.S), 'pi')):
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == dt and t.is_contiguous()
+                    and dt in (torch.float32, torch.float64) and tuple(t.shape) == shape):
+                raise ValueError(f'{name}: expected a contiguous float32 or float64 CUDA tensor of shape {shape}, '
+                                 'gamma and pi of one type')
+        words = []
+        for vals, name in ((rec_keys, 'rec_keys'), (seeds, 'seeds')):
+            vals = list(vals)
+            if len(vals) != self.B or not all(isinstance(v, (int, np.integer)) and 0 <= int(v) < 1 << 64 for v in vals):
+                raise ValueError(f'{name}: expected {self.B} integers in [0, 2**64)')
+            a = np.array([int(v) for v in vals], dtype=np.uint64).view(np.int64)     # the bits, as torch has no uint64
+            words.append(torch.from_numpy(a).to(self.device))
+        self._check(self.lib.vbx_init_random(self._h, _ptr(words[0]), _ptr(words[1]), _ptr(self.n_states), _ptr(gamma),
+                                             _ptr(pi), int(dt == torch.float64), self._stream()))
+
     @property
     def launches(self):
         return int(self.lib.vbx_launch_count(self._h))

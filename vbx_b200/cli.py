@@ -35,6 +35,11 @@ resegments an existing diarization instead of starting from AHC (DESIGN.md secti
 RTTM, each x-vector started from the speakers' shares of its segment.  The written RTTMs keep the input's speaker names
 (with --output-2nd the second-label RTTMs too) unless linking or enrolment name the speakers.  --threshold is still
 required, as by the reference's parser, and is used only by the AHC that the count bounds' rule 3 needs.
+
+With --init RANDOM+VB --init-states N [--restarts R] [--seed S] the VB-HMM starts from random flat-Dirichlet
+responsibilities over N states instead of AHC (DESIGN.md section 5.22), R starts per recording side by side (default 1),
+restart r drawn with seed S + r (default 0); each recording keeps the restart of largest final ELBO.  No AHC runs unless
+count bounds need it, so long recordings are not held up by it.  --threshold is still required, as above.
 """
 import argparse
 import os
@@ -75,10 +80,36 @@ def add_count_options(ap, allow_oracle=False):
                     'an integer or a "recording count" file')
 
 
+def add_random_options(ap):
+    """--init-states / --restarts / --seed of --init RANDOM+VB."""
+    ap.add_argument('--init-states', default=None, type=int,
+                    help='with --init RANDOM+VB: the number of HMM states the random start draws (required there)')
+    ap.add_argument('--restarts', default=None, type=int,
+                    help='with --init RANDOM+VB: random starts per recording; the largest final ELBO wins (default 1)')
+    ap.add_argument('--seed', default=None, type=int,
+                    help='with --init RANDOM+VB: seed of restart 0, an integer in [0, 2**64); restart r uses seed + r '
+                         '(default 0)')
+
+
+def check_random_options(ap, args):
+    """Usage errors (exit 2) of the --init RANDOM+VB options."""
+    random = args.init == 'RANDOM+VB'
+    if random != (args.init_states is not None):
+        ap.error('--init RANDOM+VB and --init-states go together')
+    if not random and (args.restarts is not None or args.seed is not None):
+        ap.error('--restarts and --seed are options of --init RANDOM+VB')
+    if random and args.init_states < 1:
+        ap.error('--init-states must be >= 1')
+    if args.restarts is not None and args.restarts < 1:
+        ap.error('--restarts must be >= 1')
+    if args.seed is not None and not 0 <= args.seed < 1 << 64:
+        ap.error('--seed must lie in [0, 2**64)')
+
+
 def build_parser():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     # option names, types and defaults of VBx/vbhmm.py:55-102
-    ap.add_argument('--init', required=True, type=str, choices=['AHC', 'AHC+VB', 'RTTM+VB'])
+    ap.add_argument('--init', required=True, type=str, choices=['AHC', 'AHC+VB', 'RTTM+VB', 'RANDOM+VB'])
     ap.add_argument('--out-rttm-dir', required=True, type=str)
     ap.add_argument('--xvec-ark-file', required=True, type=str)
     ap.add_argument('--segments-file', required=True, type=str)
@@ -114,6 +145,7 @@ def build_parser():
                     help='how many of each speaker\'s largest cohort scores set its mean and spread (default 200)')
     ap.add_argument('--init-rttm', default=None,
                     help='with --init RTTM+VB: the diarization (RTTM file or directory of *.rttm) the VB-HMM starts from')
+    add_random_options(ap)
     return ap
 
 
@@ -135,6 +167,7 @@ def main(argv=None):
         ap.error('--cohort-top must be >= 2')
     if (args.init == 'RTTM+VB') != (args.init_rttm is not None):
         ap.error('--init RTTM+VB and --init-rttm go together')
+    check_random_options(ap, args)
     from . import formats
     from .pipeline import diarize_batch, linked_lines, named_lines
     from .score import read_overlaps
@@ -156,7 +189,8 @@ def main(argv=None):
                         device=args.device, output_2nd=args.output_2nd, overlaps=overlaps,
                         num_speakers=args.num_speakers, min_speakers=args.min_speakers, max_speakers=args.max_speakers,
                         link_threshold=args.link_threshold, enroll=enroll, enroll_threshold=args.enroll_threshold,
-                        init_rttm=args.init_rttm, **norm_kw)
+                        init_rttm=args.init_rttm, init_states=args.init_states, restarts=args.restarts, seed=args.seed,
+                        **norm_kw)
     linked = args.link_threshold is not None
     named_init = args.init == 'RTTM+VB' and enroll is None and not linked
     os.makedirs(args.out_rttm_dir, exist_ok=True)                           # VBx/vbhmm.py:170

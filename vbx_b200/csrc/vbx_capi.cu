@@ -845,6 +845,20 @@ int vbx_init_turns(vbx_handle_t h, const int64_t *seg, const int64_t *spk_off, c
                                              pi_out, out_is_f64 != 0, st), "init_turns");
 }
 
+int vbx_init_random(vbx_handle_t h, const uint64_t *rec_key, const uint64_t *seed, const int32_t *n_states,
+                    void *gamma_out, void *pi_out, int32_t out_is_f64, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    if (!h->planned) return fail(h, VBX_ERR_STATE, "vbx_init_random: call vbx_plan or vbx_plan_f64 first");
+    const vbx::Plan &pl = h->plan;
+    if (pl.n_rec == 0) return VBX_OK;
+    if (!rec_key || !seed || !pi_out || (pl.n_frames && !gamma_out))
+        return fail(h, VBX_ERR_ARG, "vbx_init_random: null pointer");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_init_random(pl, rec_key, seed, n_states, gamma_out, pi_out, out_is_f64 != 0,
+                                              (cudaStream_t)stream), "init_random");
+}
+
 int vbx_ahc_workspace_bytes(vbx_handle_t h, size_t *bytes_out) {
     if (!h || !bytes_out) return VBX_ERR_ARG;
     if (!h->planned || h->f64_only) return fail(h, VBX_ERR_STATE, "vbx_ahc_workspace_bytes: call vbx_plan first");

@@ -246,6 +246,9 @@ int launch_hard_labels_keep(const Plan &pl, const float *gamma, const int32_t *n
 int launch_init_turns(const Plan &pl, const int64_t *seg, const int64_t *spk_off, const int64_t *turn_off,
                       const int64_t *turn_lo, const int64_t *turn_hi, const int64_t *turn_cum, const double *smoothing,
                       void *gamma, void *pi, bool f64, cudaStream_t st);
+// random initial responsibilities (Philox4x64-10 exponentials, normalised) and uniform priors (vbx_init.cu)
+int launch_init_random(const Plan &pl, const uint64_t *rec_key, const uint64_t *seed, const int32_t *n_states,
+                       void *gamma, void *pi, bool f64, cudaStream_t st);
 // reference-module forward_backward() for a general transition matrix (vbx_fb_dense.cu)
 int launch_fb_dense(const double *lls, const double *tr, const double *ip, int T, int S, double *post, double *tll,
                     double *lfw, double *lbw, cudaStream_t st);

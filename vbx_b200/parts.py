@@ -178,6 +178,10 @@ class PartitionedBatch:
     def init_turns(self, pack, smoothing, gamma, pi):
         return self.whole.init_turns(pack, smoothing, gamma, pi)
 
+    def init_random(self, rec_keys, seeds, gamma, pi):
+        self.whole.n_states = self._n_states
+        return self.whole.init_random(rec_keys, seeds, gamma, pi)
+
     # ---- multi-GPU: the batch-wide ELBO trace and its collective live in the whole-batch handle ----
     def attach_comm(self, group=None):
         return self.whole.attach_comm(group)

@@ -170,7 +170,8 @@ def keep_labels(gamma, keep):
     return kept[f], (kept[s] if s is not None else torch.full_like(f, -1))
 
 
-def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None, turns=None, **run_kw):
+def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None, turns=None, random=None, elbo=False,
+             **run_kw):
     """The VB-HMM step (VBx/vbhmm.py:150-162) for the recordings of one state tier, packed: fea [N,R] float32, labels [N]
     AHC labels (device); turns: None, or a resegment.TurnPack of the recordings, which then start from their init
     RTTM's turns instead (vbx_init_turns, DESIGN.md section 5.20; labels is not read).  f64: the float64 kernels
@@ -178,7 +179,10 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None
     loopProb may be per-recording tensors there).  Returns [(labels, second-best labels or None, iterations, flags)] per
     recording.  hi: None, or an upper bound on the speaker count per recording: a recording whose labels hold more
     speakers takes rule 2 of DESIGN.md section 5.14 (the hi states of largest mass, one vbx_hard_labels_keep launch for
-    the tier), and each tuple gains the unconstrained speaker count and 'vb' or 'mass'."""
+    the tier), and each tuple gains the unconstrained speaker count and 'vb' or 'mass'.  random: None, or (keys, seeds),
+    one integer each per recording: the recordings then start from vbx_init_random's draws (DESIGN.md section 5.22;
+    labels is not read).  elbo: every tuple also ends with the recording's final ELBO Li[b, n_iters[b] - 1] (NaN
+    without iterations)."""
     from .batch import VbxBatch, run_f64
     offs = np.concatenate([[0], np.cumsum(lens)])
     dt = torch.float64 if f64 else torch.float32
@@ -189,6 +193,8 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None
     p = torch.zeros((vb.B, vb.S), dtype=dt, device=dev)
     if turns is not None:              # softmax(smoothing * coverage) on the device, section 5.20
         vb.init_turns(turns, sm, g, p)
+    elif random is not None:           # flat-Dirichlet rows from Philox on the device, section 5.22
+        vb.init_random(random[0], random[1], g, p)
     else:
         for b in range(vb.B):          # VBx/vbhmm.py:150-152: qinit = softmax(onehot * smoothing)
             g[offs[b]:offs[b + 1], :ns[b]] = soft_init(labels[offs[b]:offs[b + 1]], int(ns[b]), float(sm[b]), dtype=dt)
@@ -221,6 +227,10 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None
             for b in over:
                 out[b] = (f[offs[b]:offs[b + 1]], s[offs[b]:offs[b + 1]] if hi[b] > 1 else None) + out[b][2:]
         out = [o + (k1[b], 'mass' if k1[b] > hi[b] else 'vb') for b, o in enumerate(out)]
+    if elbo:
+        from .random_init import final_elbo
+        last = final_elbo(res['Li'].cpu().numpy(), iters)
+        out = [o + (float(last[b]),) for b, o in enumerate(out)]
     vb.close()
     return out
 
@@ -233,7 +243,8 @@ def _tier(n_states):
     return 0 if n_states <= 64 else 1 if n_states <= MAX_STATES_F32 else 2
 
 
-def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, make, split, turns=None, **run_kw):
+def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, make, split, turns=None, random=None,
+              **run_kw):
     """Everything after AHC (VBx/vbhmm.py:147-162 and the speaker-count rules of DESIGN.md section 5.14) for the entries
     (k, b): setting k of `hyper`, a list of (Fa, Fb, loopP, smoothing), on recording b.  labels[k]: setting k's AHC
     labels per recording; labels_d[k]: their concatenation on the device (used by init='AHC+VB' only).  fea [N,R] float32
@@ -248,8 +259,12 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
     (maxIters, epsilon).  init='RTTM+VB' (DESIGN.md section 5.20) runs the first pass from turns instead, one
     (seg_times, resegment.load_init speaker list) per recording: recording b has one state per init speaker and each
     batch starts from one vbx_init_turns launch (labels and labels_d are not read; Zs only by rule 3, whose re-runs start
-    from the AHC cut as above).  Returns {(k, b): (labels, labels2nd or None, iterations, flags[, n_speakers_vb,
-    count_rule])}, the last two under bounds."""
+    from the AHC cut as above).  init='RANDOM+VB' (DESIGN.md section 5.22) runs the first pass as the entries (k, b, r),
+    restart r of (k, b), with random = random_init.RandomStart: random.n_states states each, every batch started by one
+    vbx_init_random launch (key random.keys[b], seed random.seed + r); each (k, b) then keeps the restart of largest
+    final ELBO (random_init.best_restart) before the count rules, and its tuple ends with (restart, [final ELBO of every
+    restart]).  Returns {(k, b): (labels, labels2nd or None, iterations, flags[, n_speakers_vb, count_rule])}, the last
+    two under bounds."""
     from . import ahc as _ahc
     B = len(lens)
     entries = [(k, b) for k in range(len(hyper)) for b in range(B)]
@@ -262,9 +277,10 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
         return out
     offs = np.concatenate([[0], np.cumsum(lens)])
 
-    def run_tiers(entries, ns, labels_d, hi, from_turns=False):
-        """The entries, with ns[e] states and their labels in labels_d[k] (from_turns: their recordings' init turns
-        instead), through the state tiers: {e: _vb_tier tuple}."""
+    def run_tiers(entries, ns, labels_d, hi, from_turns=False, from_random=False):
+        """The entries e = (k, b[, r]), with ns[e] states and their labels in labels_d[k] (from_turns: their recordings'
+        init turns instead; from_random: restart r's draws, and the tuples end with the final ELBO), through the state
+        tiers: {e: _vb_tier tuple}."""
         tiers = [[], [], []]
         for e in entries:
             tiers[_tier(ns[e])].append(e)
@@ -274,11 +290,16 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
         for group, f64 in batches:
             if not group:
                 continue
-            recs = [b for _, b in group]
+            recs = [e[1] for e in group]
             init_kw = {}
-            if from_turns:
-                from .resegment import pack_turns
-                init_kw = dict(turns=pack_turns([turns[b] for b in recs]))
+            if from_turns or from_random:
+                if from_turns:
+                    from .resegment import pack_turns
+                    init_kw = dict(turns=pack_turns([turns[b] for b in recs]))
+                else:
+                    from .random_init import restart_seed
+                    init_kw = dict(random=([random.keys[b] for b in recs], [restart_seed(random.seed, e[2]) for e in group]),
+                                   elbo=True)
                 g_fea = fea if recs == list(range(B)) else torch.cat([fea[offs[b]:offs[b + 1]] for b in recs])
                 g_labels = None
             elif recs == list(range(B)) and all(k == group[0][0] for k, _ in group):
@@ -289,22 +310,34 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
             if f64 or len(hyper) == 1:
                 Fa, Fb, loopP, smoothing = hyper[group[0][0]]
             else:
-                Fa, Fb, loopP = (torch.tensor([hyper[k][i] for k, _ in group], dtype=torch.float64, device=dev)
+                Fa, Fb, loopP = (torch.tensor([hyper[e[0]][i] for e in group], dtype=torch.float64, device=dev)
                                  for i in range(3))
-                smoothing = [hyper[k][3] for k, _ in group]
+                smoothing = [hyper[e[0]][3] for e in group]
             sub = _vb_tier(lens[recs], np.array([ns[e] for e in group], dtype=np.int32), g_fea, Phi, g_labels, f64,
                            smoothing, dev, make=make, hi=None if hi is None else hi[recs],
                            Fa=Fa, Fb=Fb, loopProb=loopP, **init_kw, **run_kw)
             out.update(zip(group, sub))
         return out
 
-    if init == 'RTTM+VB':
-        ns = {(k, b): len(turns[b][1]) for k, b in entries}
+    hi = None if bounds is None else bounds[1]
+    chosen = {}
+    if init == 'RANDOM+VB':
+        from .random_init import best_restart
+        runs = [(k, b, r) for k, b in entries for r in range(random.restarts)]     # a recording's restarts side by side
+        runs = run_tiers(runs, {e: random.n_states for e in runs}, None, hi, from_random=True)
+        out = {}
+        for k, b in entries:
+            elbos = [runs[(k, b, r)][-1] for r in range(random.restarts)]
+            chosen[(k, b)] = (best_restart(elbos), elbos)
+            out[(k, b)] = runs[(k, b, chosen[(k, b)][0])][:-1]
     else:
-        ns = {(k, b): int(labels[k][b].max()) + 1 if lens[b] else 1 for k, b in entries}
-    out = run_tiers(entries, ns, labels_d, None if bounds is None else bounds[1], from_turns=init == 'RTTM+VB')
+        if init == 'RTTM+VB':
+            ns = {(k, b): len(turns[b][1]) for k, b in entries}
+        else:
+            ns = {(k, b): int(labels[k][b].max()) + 1 if lens[b] else 1 for k, b in entries}
+        out = run_tiers(entries, ns, labels_d, hi, from_turns=init == 'RTTM+VB')
     if bounds is None:
-        return out
+        return {e: v + (chosen[e],) for e, v in out.items()} if chosen else out
     lo = bounds[0]
     low = [e for e in entries if out[e][4] < lo[e[1]]]
     recs = sorted({b for _, b in low})
@@ -320,13 +353,16 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
     for e in low:
         *r, rule = _recut_outcome(lens[e[1]], lo[e[1]], mc[e[1]], again.get(e))
         out[e] = tuple(r) + (out[e][4], rule)
-    return out
+    return {e: v + (chosen[e],) for e, v in out.items()} if chosen else out
 
 
-def _check_init(init, overlaps, init_rttm=None):
-    """init is 'AHC', 'AHC+VB' or 'RTTM+VB', an init RTTM is given with 'RTTM+VB' and only with it, and overlap-aware
-    output (overlaps true) has the VB-HMM's second labels."""
-    if init not in ('AHC', 'AHC+VB', 'RTTM+VB'):
+def _check_init(init, overlaps, init_rttm=None, init_states=None, restarts=None, seed=None):
+    """init is 'AHC', 'AHC+VB', 'RTTM+VB' or 'RANDOM+VB', an init RTTM is given with 'RTTM+VB' and only with it,
+    init_states / restarts / seed only with 'RANDOM+VB' (init_states required there; random_init.check_options), and
+    overlap-aware output (overlaps true) has the VB-HMM's second labels.  Returns random_init.RandomStart (without
+    keys) for 'RANDOM+VB', else None."""
+    from .random_init import check_options
+    if init not in ('AHC', 'AHC+VB', 'RTTM+VB', 'RANDOM+VB'):
         raise ValueError('Wrong option for args.initialization.')          # VBx/vbhmm.py:163-164
     if init == 'RTTM+VB' and init_rttm is None:
         raise ValueError("init='RTTM+VB' starts from an existing diarization: it needs init_rttm")
@@ -334,6 +370,7 @@ def _check_init(init, overlaps, init_rttm=None):
         raise ValueError(f"init_rttm is the starting point of init='RTTM+VB', not of init={init!r}")
     if overlaps and init == 'AHC':
         raise ValueError("overlap-aware output needs the VB-HMM's second labels: init='AHC+VB'")
+    return check_options(init, init_states, restarts, seed)
 
 
 def _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold, ahc=True):
@@ -470,7 +507,8 @@ def _count_fields(item, k1, rule, lo, hi):
 def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, threshold=-0.015, smoothing=5.0, init='AHC+VB',
                   max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False, overlaps=None,
                   num_speakers=None, min_speakers=None, max_speakers=None, link_threshold=None, enroll=None,
-                  enroll_threshold=None, cohort=None, cohort_top=200, init_rttm=None):
+                  enroll_threshold=None, cohort=None, cohort_top=200, init_rttm=None, init_states=None, restarts=None,
+                  seed=None):
     """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
     recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
     one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
@@ -487,7 +525,15 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     'RTTM+VB' runs no AHC; with them rule 2 applies as for 'AHC+VB' and rule 3 re-runs from the AHC linkage cut (its
     states then have no init names).  Each item then also has init_speakers (the init speaker name of each state; None
     for a rule 3 outcome) and rttm_init (its rttm lines, or rttm_overlap's with overlaps, with the speaker field set to
-    that name; the rttm or rttm_overlap lines themselves for a rule 3 outcome).  chain: 'tcgen05' (fused tensor-core front end,
+    that name; the rttm or rttm_overlap lines themselves for a rule 3 outcome).
+    init='RANDOM+VB' (DESIGN.md section 5.22): the VB-HMM starts from random flat-Dirichlet gamma0 rows with init_states
+    states (required, no default) and pi0 = 1 / init_states, drawn on the device by vbx_init_random; restarts (default
+    1) runs that many starts of every recording side by side in one batch, restart r with seed (seed + r) mod 2^64
+    (seed: default 0, an integer in [0, 2^64)), and each recording keeps the restart of largest final ELBO (ties: the
+    lowest r).  A recording's draws depend on its name, not on the archive.  Without count bounds no AHC runs; with them
+    rule 2 applies to the chosen restart and rule 3 re-runs from the AHC linkage cut.  Each item then also has restart
+    (the chosen index), init_seed (seed + restart mod 2^64: restarts=1 with that seed reruns it alone), elbo (its final
+    ELBO) and restart_elbos (the final ELBO of every restart; NaN where a restart ran no iteration).  chain: 'tcgen05' (fused tensor-core front end,
     needs lda_dim == 128 and a 128-dim PLDA), 'float64' (float64 torch ops), 'auto' = tcgen05 when the shapes allow.
     overlaps: None, or overlap regions {name: [(onset, offset)] seconds} (score.read_overlaps; a recording it lacks has
     none): each item then also has rttm_overlap, the overlap-aware RTTM lines (overlap_segments: the second most likely
@@ -520,7 +566,7 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds]
     [, count_rule, n_speakers_vb, count][, global_speakers, rttm_linked][, speaker_names, speaker_llr or speaker_score,
     rttm_named][, score_norm][, init_speakers, rttm_init])}."""
-    _check_init(init, overlaps is not None, init_rttm)
+    random = _check_init(init, overlaps is not None, init_rttm, init_states, restarts, seed)
     bounds = count_bounds(list(recordings), num_speakers, min_speakers, max_speakers)
     if link_threshold is not None:
         from .link import check_threshold
@@ -553,18 +599,21 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
     if len(names) == 0:
         return {}
-    # resegmentation needs the AHC linkage for rule 3 of the count bounds only
+    # resegmentation and random starts need the AHC linkage for rule 3 of the count bounds only
     fea, Phi, ahc_labels, _, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, threshold,
-                                             ahc=init != 'RTTM+VB' or bounds is not None)
+                                             ahc=init in ('AHC', 'AHC+VB') or bounds is not None)
     offs = np.concatenate([[0], np.cumsum(lens)])
     labels_d = None
     if init != 'AHC':
         fea, Phi = _pad_features(fea, Phi)
     if init == 'AHC+VB':
         labels_d = [torch.from_numpy(np.concatenate(ahc_labels)).to(dev)]
+    if random is not None:
+        from .random_init import name_key
+        random = random._replace(keys=[name_key(n) for n in names])
     from .batch import VbxBatch
     res = _vb_stage([(Fa, Fb, loopP, smoothing)], [ahc_labels], labels_d, Zs, lens, fea, Phi, bounds, init, dev,
-                    VbxBatch, None, turns=turns, maxIters=max_iters, epsilon=epsilon)
+                    VbxBatch, None, turns=turns, random=random, maxIters=max_iters, epsilon=epsilon)
     res = [res[(0, b)] for b in range(len(names))]
     labels1, labels2 = [r[0] for r in res], [r[1] for r in res]
     out = {}
@@ -603,7 +652,19 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
         if turns is not None:
             init_fields(out[n], n, recordings[n][1], labels1[b], labels2[b], turns[b][1],
                         None if bounds is None else res[b][5], ovl)
+        if random is not None:
+            restart_fields(out[n], random.seed, *res[b][-1])
     return out
+
+
+def restart_fields(item, seed, restart, elbos):
+    """The fields of an init='RANDOM+VB' result (DESIGN.md section 5.22): the chosen restart, its seed (to rerun it
+    alone), its final ELBO and every restart's.  They describe the choice also when rule 3 of the count bounds replaced
+    the chosen restart's labels by a re-run from the AHC cut."""
+    from .random_init import restart_seed
+    item.update(restart=int(restart), init_seed=restart_seed(seed, restart), elbo=float(elbos[restart]),
+                restart_elbos=[float(v) for v in elbos])
+    return item
 
 
 def init_fields(item, name, seg_times, labels, labels2, turns, rule=None, overlap=None):

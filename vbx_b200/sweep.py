@@ -39,6 +39,9 @@ RTTM files are written: cli with --enroll-threshold at the chosen setting reprod
 With --init RTTM+VB --init-rttm PATH every setting resegments that diarization instead of starting from AHC (DESIGN.md
 section 5.20); --threshold must then hold one value.  The RTTM files keep their numbered speakers: cli with --init
 RTTM+VB at the chosen setting writes them with the input's speaker names.
+With --init RANDOM+VB --init-states N [--restarts R] [--seed S] every setting starts from random responsibilities
+instead of AHC (DESIGN.md section 5.22), the same draws for every setting; --threshold and --init-smoothing must then
+hold one value each.
 With --combine N (the N best settings of ranking['full']; needs --ref-rttm) or --combine all, those settings' outputs are
 combined into one by label mapping and weighted voting (DESIGN.md section 5.21): OUT/combined/<recording>.rttm, and
 summary.json gains combined = {hypotheses, recordings: {name: order, weights, speakers}[, der][, jer]}, scored under
@@ -164,8 +167,8 @@ def packer(lens, R, device, budget):
 
     def split(entries, ns):
         sizes = []
-        for k, b in entries:
-            key = (int(lens[b]), padded_states(ns[(k, b)]))      # the size depends on T and the padded S only
+        for e in entries:                                     # (setting, recording[, restart])
+            key = (int(lens[e[1]]), padded_states(ns[e]))         # the size depends on T and the padded S only
             if key not in size_cache:
                 size_cache[key] = entry_bytes(key[0], key[1], R, device)
             sizes.append(size_cache[key])
@@ -176,7 +179,8 @@ def packer(lens, R, device, budget):
 def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, epsilon=1e-6, init='AHC+VB', chain='auto',
                 device=None, max_batch_bytes=None, output_2nd=False, ref_rttm=None, uem=None, overlaps=None,
                 oracle_overlaps=False, jer=False, num_speakers=None, min_speakers=None, max_speakers=None,
-                link_thresholds=None, enroll=None, enroll_thresholds=None, cohort=None, cohort_top=200, init_rttm=None):
+                link_thresholds=None, enroll=None, enroll_thresholds=None, cohort=None, cohort_top=200, init_rttm=None,
+                init_states=None, restarts=None, seed=None):
     """Every setting of `grid` (see grid_settings) for every recording, with the front end and AHC run once.
 
     recordings, transform, plda, lda_dim, max_iters, epsilon, init, chain, output_2nd: as for pipeline.diarize_batch.
@@ -225,6 +229,10 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     and checked once and packed for every batch; each entry starts from its recording's turns with its setting's
     smoothing.  The grid's threshold axis has no effect then and must hold exactly one value (ValueError otherwise).
     Each dict gains init_speakers and rttm_init; the written RTTM files keep their numbered speakers.
+    init='RANDOM+VB', init_states, restarts, seed: random starts as for diarize_batch (DESIGN.md section 5.22), the same
+    for every setting: every (setting, recording, restart) is one entry of the tiers and packing, and each (setting,
+    recording) keeps its restart of largest final ELBO.  The grid's threshold and smoothing axes have no effect then and
+    must each hold exactly one value (ValueError otherwise).  Each dict gains restart, init_seed, elbo and restart_elbos.
     Returns {Setting: {recording: dict(rttm, labels, labels2nd, n_speakers, iterations, flags[, der][, rttm_overlap,
     overlap_seconds][, der_overlap][, count_rule, n_speakers_vb, count][, global_speakers][, speaker_names, speaker_llr
     or speaker_score][, score_norm][, ref_speakers, der_blocks[, der_overlap_blocks]])}}; each recording's dict is the
@@ -234,7 +242,7 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     from ._lib import VbxError
     from .parts import make_batch
     from .pipeline import (_check_init, _count_fields, _front_end, _pad_features, _result, _side_features, _vb_stage,
-                           count_bounds, init_fields)
+                           count_bounds, init_fields, restart_fields)
     settings = grid_settings(grid)
     links = check_link_thresholds(link_thresholds)
     dims = {int(np.asarray(r[0]).shape[1]) for r in recordings.values()}
@@ -248,7 +256,12 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
         _cohort.check_top_k(cohort_top)
         cohort_set = _cohort.check_cohort(cohort, dim)
     with_overlap = oracle_overlaps or overlaps is not None
-    _check_init(init, with_overlap, init_rttm)
+    random = _check_init(init, with_overlap, init_rttm, init_states, restarts, seed)
+    if random is not None:
+        for axis in ('threshold', 'smoothing'):
+            if len({getattr(s, axis) for s in settings}) != 1:
+                raise ValueError(f"init='RANDOM+VB' runs no AHC threshold cut and no smoothed init: the grid's {axis} "
+                                 'axis must hold one value')
     init_from = None                                         # (seg_times, init speakers) per recording
     if init == 'RTTM+VB':
         from .resegment import load_init
@@ -287,21 +300,24 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
     if not names:
         return {s: {} for s in settings}
     lens = np.array([np.asarray(recordings[n][0]).shape[0] for n in names], dtype=np.int64)
-    with_ahc = init_from is None or bounds is not None          # resegmentation: the AHC linkage serves rule 3 only
+    with_ahc = init in ('AHC', 'AHC+VB') or bounds is not None     # other inits: the AHC linkage serves rule 3 only
     fea, Phi, _, th, Zs = _front_end(recordings, names, lens, transform, plda, lda_dim, chain, dev, 0.0, ahc=with_ahc)
     fea, Phi = _pad_features(fea, Phi)
     thresholds = list(dict.fromkeys(s.threshold for s in settings))
     ahc_labels = lab_d = {t: None for t in thresholds}
-    if init_from is None:
+    if init in ('AHC', 'AHC+VB'):
         ahc_labels = {t: _ahc.cut(Zs, th, lens, t) for t in thresholds}              # VBx/vbhmm.py:144-146, host only
         lab_d = {t: torch.from_numpy(np.concatenate(ahc_labels[t])).to(dev) for t in thresholds}
     if max_batch_bytes is None:
         max_batch_bytes = int(torch.cuda.mem_get_info(dev)[0] * BUDGET_FRACTION)
+    if random is not None:
+        from .random_init import name_key
+        random = random._replace(keys=[name_key(n) for n in names])
     # per (setting, recording): labels, labels2nd, iterations, flags[, unconstrained count, rule]
     res = _vb_stage([(s.Fa, s.Fb, s.loopP, s.smoothing) for s in settings], [ahc_labels[s.threshold] for s in settings],
                     [lab_d[s.threshold] for s in settings], Zs, lens, fea, Phi, bounds, init, dev, make_batch,
-                    packer(lens, int(fea.shape[1]), dev, max_batch_bytes), turns=init_from, maxIters=max_iters,
-                    epsilon=epsilon)
+                    packer(lens, int(fea.shape[1]), dev, max_batch_bytes), turns=init_from, random=random,
+                    maxIters=max_iters, epsilon=epsilon)
     maps = named = norm = None
     if links is not None or enrolled is not None:
         offs = np.concatenate([[0], np.cumsum(lens)])
@@ -376,6 +392,8 @@ def sweep_batch(recordings, transform, plda, grid, lda_dim=128, max_iters=40, ep
             if init_from is not None:
                 init_fields(item, n, recordings[n][1], l1, l2, init_from[b][1],
                             None if bounds is None else res[(k, b)][5], ovl[b])
+            if random is not None:
+                restart_fields(item, random.seed, *res[(k, b)][-1])
             if (maps is not None or named is not None) and der is not None:
                 item['ref_speakers'] = ref[2][n]
                 item['der_blocks'] = der[(k, b)]['O']
@@ -620,7 +638,7 @@ def build_parser():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument('--combine', default=None, type=parse_combine,
                     help="combine the N best settings (needs --ref-rttm), or 'all', into OUT/combined/*.rttm")
-    ap.add_argument('--init', default='AHC+VB', choices=['AHC', 'AHC+VB', 'RTTM+VB'])
+    ap.add_argument('--init', default='AHC+VB', choices=['AHC', 'AHC+VB', 'RTTM+VB', 'RANDOM+VB'])
     ap.add_argument('--init-rttm', default=None,
                     help='with --init RTTM+VB: the diarization (RTTM file or directory of *.rttm) the VB-HMM starts from')
     ap.add_argument('--out-dir', required=True, type=str)
@@ -658,8 +676,9 @@ def build_parser():
     ap.add_argument('--cohort-utt2spk', default=None, help='the speaker of each x-vector of --cohort-ark (utt2spk)')
     ap.add_argument('--cohort-top', default=200, type=int,
                     help="how many of each speaker's largest cohort scores set its mean and spread (default 200)")
-    from .cli import add_count_options
+    from .cli import add_count_options, add_random_options
     add_count_options(ap, allow_oracle=True)
+    add_random_options(ap)
     return ap
 
 
@@ -672,6 +691,8 @@ def main(argv=None):
         ap.error('--cohort-ark and --cohort-utt2spk go together')
     if (args.init == 'RTTM+VB') != (args.init_rttm is not None):
         ap.error('--init RTTM+VB and --init-rttm go together')
+    from .cli import check_random_options
+    check_random_options(ap, args)
     if isinstance(args.combine, int) and args.ref_rttm is None:
         ap.error('--combine N takes the N best settings by DER: it needs --ref-rttm (or --combine all)')
     from . import formats
@@ -694,7 +715,8 @@ def main(argv=None):
                       enroll=formats.read_enrolment(args.enroll_ark, args.enroll_utt2spk) if args.enroll_ark else None,
                       enroll_thresholds=args.enroll_threshold,
                       cohort=formats.read_enrolment(args.cohort_ark, args.cohort_utt2spk) if args.cohort_ark else None,
-                      cohort_top=args.cohort_top, init_rttm=args.init_rttm)
+                      cohort_top=args.cohort_top, init_rttm=args.init_rttm, init_states=args.init_states,
+                      restarts=args.restarts, seed=args.seed)
     summary = {}
     for s, per_rec in out.items():
         d = os.path.join(args.out_dir, s.name)
@@ -705,7 +727,8 @@ def main(argv=None):
                 fp.write(''.join(line + os.linesep for line in item['rttm']))
             summary[s.name]['recordings'][name] = dict(speakers=item['n_speakers'], iterations=item['iterations'],
                                                        flags=item['flags'])
-            for key in ('der', 'der_overlap', 'overlap_seconds', 'jer', 'jer_overlap', 'count_rule'):
+            for key in ('der', 'der_overlap', 'overlap_seconds', 'jer', 'jer_overlap', 'count_rule', 'restart',
+                        'init_seed'):
                 if key in item:
                     summary[s.name]['recordings'][name][key] = item[key]
             if 'count_rule' in item:
