@@ -6,15 +6,20 @@
 // The same kernel, templated on MODE, also runs the real-data front end (x-vector transform and PLDA projection,
 // VBx/vbhmm.py:125-129,153; launch_xvector_chain_wgmma below).
 //
-// One persistent CTA per SM, 16 warps, tiles of 128 frames:
-//   warps 0-7   producers: coalesced LDG of a 128-frame x 32-column block of X (prefetched one block ahead in
-//               registers), split into TF32 parts, stored into the 128B-swizzled K-major wgmma layout;
-//               thread 0 also issues the bulk-async (TMA, cp.async.bulk) copies of the pre-split V block.
-//   warps 8-15  two consumer warpgroups, 64 frames each: wgmma.mma_async m64n128k8 tf32 from shared memory into
-//               64 fp32 registers per thread (4 k-steps x NS(NS+1)/2 split terms per 32-column block); a stage is
-//               released to the producers one block later (wgmma.wait_group 1).  The epilogue works on the register
-//               accumulators: the per-frame constant G_t (quad shuffles) and float2 stores of rho.
-// Shared memory: NS = 2: 3 stages x (A hi/lo 32 KB + B hi/lo 32 KB) = 192 KB; NS = 3: 2 stages x (A 48 KB + B 48 KB).
+// One persistent CTA per SM, 12 warps, tiles of 256 frames:
+//   warps 0-7   two consumer warpgroups, 128 frames each as two wgmma M=64 row sets.  Each thread ld.shared's its A
+//               fragments from the raw fp32 X block, splits them into TF32 parts in registers and issues
+//               wgmma.mma_async m64n128k8 tf32 with A from registers and B (V) by shared-memory descriptor, into
+//               2 x 64 fp32 accumulator registers (4 k-steps x NS(NS+1)/2 split terms x 2 row sets per 32-column block).
+//               One commit group per k-step; a stage is released to the producer when its last group has retired.
+//               The epilogue works on the register accumulators: the per-frame constant G_t (quad shuffles) and
+//               float2 stores of rho.
+//   warps 8-11  producer: one thread issues, per 32-column block, the TMA tile copy of the raw 256-frame x 32-column X
+//               block (128-byte swizzle; rows past N are zero-filled by the copy and never stored) and the bulk-async
+//               copy (cp.async.bulk) of the pre-split V images, both completing on the stage's full barrier.
+// Shared memory: NS = 2: 3 stages x (X 32 KB + V hi/lo 32 KB) = 192 KB; NS = 3: 2 stages x (X 32 KB + V 48 KB).
+// X is read from shared memory once (by the thread whose fragment it is) and V once per wgmma M=64 row set, so the 256-frame
+// tile halves the V bytes streamed from L2 per frame against a 128-frame tile.
 //
 // NS = 3 (the real-data front end): operands are split three ways, x = x1 + x2 + x3 exactly (3 x 11 mantissa bits), and
 // six products are accumulated (x3 v1, x1 v3, x2 v2, x2 v1, x1 v2, x1 v1): the dropped terms are below 2^-33, i.e. the
@@ -28,18 +33,18 @@ namespace vbx {
 
 namespace {
 
-constexpr int kTileM = 128;                 // frames per CTA tile: two wgmma M=64 tiles
+constexpr int kTileM = 256;                 // frames per CTA tile: two warpgroups x two wgmma M=64 row sets
 constexpr int kKB = 32;                     // columns of X per pipeline block (= one 128-byte swizzle row)
-constexpr int kABytes = 128 * 128;          // one 128-row x 128-byte operand image
-constexpr int kProducerThreads = 256;
+constexpr int kVBytes = 128 * 128;          // one image of V^T: 128 rows x 128 bytes
+constexpr int kXBytes = kTileM * 128;       // the raw fp32 X block of a tile: 256 rows x 128 bytes
 constexpr int kConsumerThreads = 256;       // two warpgroups
-constexpr int kThreads = kProducerThreads + kConsumerThreads;
+constexpr int kThreads = kConsumerThreads + 128;  // + the producer warpgroup (one thread of it issues the copies)
 
 template <int NS> struct Pipe {
     static constexpr int kStages = NS == 2 ? 3 : 2;
-    static constexpr int kStageBytes = 2 * NS * kABytes;   // A: NS images of 128 frames, B: NS images of V^T
-    // 1 KB alignment slack, stages, barriers (128 B), 1/Phi or e_off (512 B), row norms [2][128] (1 KB)
-    static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + 128 + 512 + 2 * kTileM * 4;
+    static constexpr int kStageBytes = kXBytes + NS * kVBytes;   // raw X block, NS images of V^T
+    // 1 KB alignment slack, stages, barriers (128 B), 1/Phi or e_off (512 B)
+    static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + 128 + 512;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
@@ -69,23 +74,30 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
                  "l"(src), "r"(bytes), "r"(bar)
                  : "memory");
 }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// TMA copy of the box at (column c0, row c1) of a 2-D tensor map into shared memory
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, int c0, int c1, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
+                 "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
+                 : "memory");
+}
 
 // wgmma shared-memory matrix descriptor: K-major, 128-byte swizzle, dense 8-row groups (SBO = 1024 B, LBO unused = 1).
-// Advancing along K inside the 128-byte swizzle row, or by whole 1024-byte row groups, only adds to the start address
-// (bits 0-13, in 16-byte units), so the consumers add small integers to one descriptor per stage.
+// Advancing along K inside the 128-byte swizzle row only adds to the start address (bits 0-13, in 16-byte units), so
+// the consumers add small integers to one descriptor per stage.
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
     const uint32_t lo = ((smem_addr >> 4) & 0x3fffu) | (1u << 16);
     const uint32_t hi = (1024u >> 4) | (1u << 30);                 // SBO, layout type 1 = SWIZZLE_128B
     return ((uint64_t)hi << 32) | lo;
 }
-// D[64 x 128] (+)= A[smem, 64 x 8] * B[smem, 128 x 8]^T, tf32, fp32 accumulators in registers
-__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+// D[64 x 128] (+)= A[registers, 64 x 8] * B[smem, 128 x 8]^T, tf32, fp32 accumulators in registers.  A fragment of the
+// thread (warp w of the warpgroup, g = lane / 4, t = lane % 4): a0 = A[16w + g][t], a1 = A[16w + g + 8][t],
+// a2 = A[16w + g][t + 4], a3 = A[16w + g + 8][t + 4].
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %66, 0;\n\t"
+        "setp.ne.b32 p, %69, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
           "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
           "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
@@ -94,7 +106,7 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t
           "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
           "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
           "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(da), "l"(db), "r"(accumulate));
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -105,16 +117,6 @@ __device__ __forceinline__ void fence_operands(float (&d)[64]) {
     for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// streaming 16-byte load that does not allocate in L1: with ~195 KB of shared memory only ~30 KB of L1 remain, and
-// allocating loads would cap the bytes in flight at that size
-__device__ __forceinline__ float4 ldg_stream(const float4 *p) {
-    float4 v;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, const float4 v) {
-    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
 __device__ __forceinline__ void split_rn(const float x, float &hi, float &lo) {
     const uint32_t h = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;
     hi = __uint_as_float(h);
@@ -157,25 +159,25 @@ __global__ void build_v_images_kernel(const float *__restrict__ V, int D, float 
 // MODE 0  rho = X . V, G_t from rho and Phi                                   (the projection of SURVEY 8d)
 // MODE 2  rho = (X - a_off) . V, G_t as above                                  (PLDA stage, VBx/vbhmm.py:153)
 // MODE 1  out = l2norm(l2norm(X - a_off) . V - e_off)                          (x-vector transform, VBx/vbhmm.py:125-129)
-//         the producers also accumulate ||x - a_off||^2 per row and hand it to the epilogue through shared memory
+//         the consumers also accumulate ||x - a_off||^2 of their rows from the A fragments, summed over the quad
+// xmap: TMA map of X [N rows, D columns] fp32, box 32 columns x kTileM rows, 128-byte swizzle.
+// Registers are allocated per warpgroup: the CTA starts at 168 per thread (3 x 128 x 168 <= 64K), then the producer
+// warpgroup gives up all but 40 and the consumers take 232, which the register-A wgmma pipeline needs without spills.
 template <int MODE, int NS>
 __global__ void __launch_bounds__(kThreads, 1)
-project_wgmma_kernel(const float *__restrict__ X, const float *__restrict__ vimg, float *__restrict__ rho, int64_t N,
-                     int D, const float *__restrict__ Phi, float *__restrict__ gframe,
+project_wgmma_kernel(const __grid_constant__ CUtensorMap xmap, const float *__restrict__ vimg, float *__restrict__ rho,
+                     int64_t N, int D, const float *__restrict__ Phi, float *__restrict__ gframe,
                      const float *__restrict__ a_off, const float *__restrict__ e_off) {
     constexpr int kStages = Pipe<NS>::kStages, kStageBytes = Pipe<NS>::kStageBytes;
-    constexpr int ROWS_PT = kTileM / 32;         // rows per producer thread
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // the stage buffers must be 1024-byte aligned (128-byte swizzle)
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint64_t *bars = reinterpret_cast<uint64_t *>(smem + kStages * kStageBytes);
     float *s_inv_phi = reinterpret_cast<float *>(bars + 16);   // 128 floats: 1/Phi (MODE 0, 2) or e_off (MODE 1)
-    float *s_n1 = s_inv_phi + 128;                             // [2][kTileM] row norms (MODE 1), by tile parity
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t bar_base = smem_u32(bars);
-    auto full_a = [&](int s) { return bar_base + 8u * s; };
-    auto full_b = [&](int s) { return bar_base + 8u * (kStages + s); };
-    auto empty = [&](int s) { return bar_base + 8u * (2 * kStages + s); };
+    auto full = [&](int s) { return bar_base + 8u * s; };
+    auto empty = [&](int s) { return bar_base + 8u * (kStages + s); };
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int n_kb = D / kKB;
@@ -184,144 +186,112 @@ project_wgmma_kernel(const float *__restrict__ X, const float *__restrict__ vimg
     if (tid < 128) s_inv_phi[tid] = MODE == 1 ? e_off[tid] : 1.f / Phi[tid];
     if (tid == 0) {
         for (int s = 0; s < kStages; ++s) {
-            mbar_init(full_a(s), kProducerThreads);
-            mbar_init(full_b(s), 1);
+            mbar_init(full(s), 1);
             mbar_init(empty(s), kConsumerThreads);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
 
-    if (warp < 8) {
-        // ======================= producers =======================
-        // Blocks of this CTA in order: b -> (tile = blockIdx.x + (b / n_kb) * gridDim.x, kb = b % n_kb).  Two
-        // ping-pong register sets keep the loads of the next block in flight while one is split and stored.
-        const int c = tid & 7;            // 16-byte chunk inside the 128-byte row
-        const int r0 = tid >> 3;          // rows r0 + 32 i
-        const int64_t my_tiles = blockIdx.x < n_tiles ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-        const int64_t n_blocks = my_tiles * n_kb;
-        float4 bufA[ROWS_PT], bufB[ROWS_PT];
-        float ss[ROWS_PT];                // MODE 1: running ||x - a_off||^2 of this thread's rows (its 4 columns)
-#pragma unroll
-        for (int i = 0; i < ROWS_PT; ++i) ss[i] = 0.f;
-        auto issue = [&](const int64_t b, float4(&buf)[ROWS_PT]) {
-            if (b >= n_blocks) return;
-            const int64_t tile = blockIdx.x + (b / n_kb) * gridDim.x;
-            const int kb = (int)(b % n_kb);
-            const int64_t row_base = tile * kTileM;
-#pragma unroll
-            for (int i = 0; i < ROWS_PT; ++i) {
-                const int64_t row = min(row_base + r0 + 32 * i, N - 1);
-                buf[i] = ldg_stream(reinterpret_cast<const float4 *>(X + row * D + kb * kKB) + c);
-            }
-        };
-        auto process = [&](const int64_t b, const float4(&buf)[ROWS_PT]) {
-            const int s = (int)(b % kStages);
-            const uint32_t ph = (uint32_t)((b / kStages) & 1);
-            const int kb = (int)(b % n_kb);
-            float4 aoff = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (MODE != 0) aoff = __ldg(reinterpret_cast<const float4 *>(a_off + kb * kKB) + c);
-            mbar_wait(empty(s), ph ^ 1);               // the MMAs that read this stage have completed
-            const uint32_t stage = smem_base + s * kStageBytes;
-            if (tid == 0) {
-                mbar_expect_tx(full_b(s), NS * kABytes);
-                bulk_g2s(stage + NS * kABytes, vimg + (int64_t)kb * NS * 4096, NS * kABytes, full_b(s));
-            }
-#pragma unroll
-            for (int i = 0; i < ROWS_PT; ++i) {
-                const int m = r0 + 32 * i;             // 0..kTileM-1
-                float4 hi, lo, x = buf[i];
-                if (MODE != 0) {
-                    x.x -= aoff.x;
-                    x.y -= aoff.y;
-                    x.z -= aoff.z;
-                    x.w -= aoff.w;
-                }
-                if (MODE == 1) ss[i] = fmaf(x.x, x.x, fmaf(x.y, x.y, fmaf(x.z, x.z, fmaf(x.w, x.w, ss[i]))));
-                const uint32_t off = (uint32_t)(m * 128 + ((c ^ (m & 7)) << 4));
-                if (NS == 2) {
-                    split_rn(x.x, hi.x, lo.x);
-                    split_rn(x.y, hi.y, lo.y);
-                    split_rn(x.z, hi.z, lo.z);
-                    split_rn(x.w, hi.w, lo.w);
-                    st_shared_v4(stage + 0 * kABytes + off, hi);
-                    st_shared_v4(stage + 1 * kABytes + off, lo);
-                } else {
-                    float4 lo2;
-                    split3_rn(x.x, hi.x, lo.x, lo2.x);
-                    split3_rn(x.y, hi.y, lo.y, lo2.y);
-                    split3_rn(x.z, hi.z, lo.z, lo2.z);
-                    split3_rn(x.w, hi.w, lo.w, lo2.w);
-                    st_shared_v4(stage + 0 * kABytes + off, hi);
-                    st_shared_v4(stage + 1 * kABytes + off, lo);
-                    st_shared_v4(stage + 2 * kABytes + off, lo2);
-                }
-            }
-            if (MODE == 1 && kb == n_kb - 1) {
-                // row norms of the finished tile: the 8 lanes that share a row are adjacent
-                float *dst = s_n1 + ((b / n_kb) & 1) * kTileM;
-#pragma unroll
-                for (int i = 0; i < ROWS_PT; ++i) {
-                    float v = ss[i];
-                    v += __shfl_xor_sync(0xffffffffu, v, 1);
-                    v += __shfl_xor_sync(0xffffffffu, v, 2);
-                    v += __shfl_xor_sync(0xffffffffu, v, 4);
-                    if (c == 0) dst[r0 + 32 * i] = v;
-                    ss[i] = 0.f;
-                }
-            }
-            fence_proxy_async_smem();                  // make the generic-proxy stores visible to the tensor core
-            mbar_arrive(full_a(s));
-        };
-        issue(0, bufA);
-        for (int64_t b = 0; b < n_blocks; b += 2) {
-            issue(b + 1, bufB);
-            process(b, bufA);
-            if (b + 1 < n_blocks) {
-                issue(b + 2, bufA);
-                process(b + 1, bufB);
+    if (tid >= kConsumerThreads) {
+        // ======================= producer =======================
+        // Blocks of this CTA in order: b -> (tile = blockIdx.x + (b / n_kb) * gridDim.x, kb = b % n_kb).
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (tid == kConsumerThreads) {
+            const int64_t my_tiles = blockIdx.x < n_tiles ? (n_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+            const int64_t n_blocks = my_tiles * n_kb;
+            for (int64_t b = 0; b < n_blocks; ++b) {
+                const int s = (int)(b % kStages);
+                const uint32_t ph = (uint32_t)((b / kStages) & 1);
+                const int64_t tile = blockIdx.x + (b / n_kb) * gridDim.x;
+                const int kb = (int)(b % n_kb);
+                mbar_wait(empty(s), ph ^ 1);               // the consumers are done with this stage
+                const uint32_t stage = smem_base + s * kStageBytes;
+                mbar_expect_tx(full(s), kXBytes + NS * kVBytes);   // a box past the last row still counts in full
+                tma_load_2d(stage, &xmap, kb * kKB, (int)(tile * kTileM), full(s));
+                bulk_g2s(stage + kXBytes, vimg + (int64_t)kb * NS * 4096, NS * kVBytes, full(s));
             }
         }
     } else {
-        // ======================= consumers: MMA + epilogue =======================
-        const int ct = tid - kProducerThreads;
-        const int wg = ct >> 7;                        // warpgroup: frames 64 wg .. 64 wg + 63 of the tile
-        const int rq = 16 * ((ct >> 5) & 3) + (lane >> 2);   // accumulator rows rq and rq + 8 of the warpgroup
-        const int cq = 2 * (lane & 3);                 // accumulator columns 8 j + cq, + 1
-        constexpr uint64_t kImg = kABytes >> 4;        // one operand image, in 16-byte descriptor units
-        float d[64];
+        // ======================= consumers: split, MMA, epilogue =======================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        const int wg = tid >> 7;                       // warpgroup: frames 128 wg .. 128 wg + 127 of the tile
+        const int g = lane >> 2, t = lane & 3;
+        const int rq = 16 * (warp & 3) + g;            // accumulator rows rq and rq + 8 of each 64-row set
+        const int cq = 2 * t;                          // accumulator columns 8 j + cq, + 1
+        // this thread's A elements inside a stage: row 128 wg + 64 m + rq (+ 8), column 8 ks + t (+ 4) of the
+        // 128-byte swizzled block, i.e. 16-byte chunk (2 ks (+ 1)) ^ (row & 7) = (2 ks (+ 1)) ^ g, word t
+        const float *a_rows = reinterpret_cast<const float *>(smem) + (128 * wg + rq) * 32 + t;
+        float d0[64], d1[64];
+        float ss[2][2];                                // MODE 1: ||x - a_off||^2 partial of rows (set m, +0 / +8)
         int s = 0, last = 0;
         uint32_t ph = 0;
-        int it = 0;
-        for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+        for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+#pragma unroll
+            for (int m = 0; m < 2; ++m) ss[m][0] = ss[m][1] = 0.f;
             for (int kb = 0; kb < n_kb; ++kb) {
-                mbar_wait(full_a(s), ph);
-                mbar_wait(full_b(s), ph);
-                const uint32_t stage = smem_base + s * kStageBytes;
-                const uint64_t a0 = make_desc(stage + wg * 64 * 128);     // this warpgroup's 64 rows of the A images
-                const uint64_t b0 = make_desc(stage + NS * kABytes);
-                wgmma_fence();
+                float ao[8];                           // a_off of columns 8 ks + t, 8 ks + t + 4
+#pragma unroll
+                for (int i = 0; i < 8; ++i) ao[i] = MODE != 0 ? __ldg(a_off + kb * kKB + 4 * i + t) : 0.f;
+                mbar_wait(full(s), ph);
+                const float *xs = a_rows + s * (kStageBytes / 4);
+                const uint64_t b0 = make_desc(smem_base + s * kStageBytes + kXBytes);
+                constexpr uint64_t kImg = kVBytes >> 4;        // one V image, in 16-byte descriptor units
 #pragma unroll
                 for (int ks = 0; ks < 4; ++ks) {
-                    const uint64_t k = ks * 2;         // 8 tf32 = 32 bytes inside the swizzle row (16-byte units)
-                    const uint32_t first = (kb == 0 && ks == 0) ? 0u : 1u;
-                    if (NS == 2) {                      // lo*hi + hi*lo + hi*hi
-                        wgmma_tf32(d, a0 + kImg + k, b0 + k, first);
-                        wgmma_tf32(d, a0 + k, b0 + kImg + k, 1u);
-                        wgmma_tf32(d, a0 + k, b0 + k, 1u);
-                    } else {                            // smallest terms first: x3 v1, x1 v3, x2 v2, x2 v1, x1 v2, x1 v1
-                        wgmma_tf32(d, a0 + 2 * kImg + k, b0 + k, first);
-                        wgmma_tf32(d, a0 + k, b0 + 2 * kImg + k, 1u);
-                        wgmma_tf32(d, a0 + kImg + k, b0 + kImg + k, 1u);
-                        wgmma_tf32(d, a0 + kImg + k, b0 + k, 1u);
-                        wgmma_tf32(d, a0 + k, b0 + kImg + k, 1u);
-                        wgmma_tf32(d, a0 + k, b0 + k, 1u);
+                    const int o0 = ((2 * ks) ^ g) << 2, o1 = ((2 * ks + 1) ^ g) << 2;   // float offsets of the chunks
+                    uint32_t p1[2][4], p2[2][4], p3[2][4];     // split parts (hi, lo[, lo2]) of the two row sets
+#pragma unroll
+                    for (int m = 0; m < 2; ++m) {
+                        float x[4] = {xs[m * 64 * 32 + o0], xs[m * 64 * 32 + 8 * 32 + o0], xs[m * 64 * 32 + o1],
+                                      xs[m * 64 * 32 + 8 * 32 + o1]};
+                        if (MODE != 0) {
+                            x[0] -= ao[2 * ks];
+                            x[1] -= ao[2 * ks];
+                            x[2] -= ao[2 * ks + 1];
+                            x[3] -= ao[2 * ks + 1];
+                        }
+                        if (MODE == 1) {
+                            ss[m][0] = fmaf(x[2], x[2], fmaf(x[0], x[0], ss[m][0]));
+                            ss[m][1] = fmaf(x[3], x[3], fmaf(x[1], x[1], ss[m][1]));
+                        }
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            float h, l, l2 = 0.f;
+                            if (NS == 2) split_rn(x[j], h, l);
+                            else split3_rn(x[j], h, l, l2);
+                            p1[m][j] = __float_as_uint(h);
+                            p2[m][j] = __float_as_uint(l);
+                            p3[m][j] = __float_as_uint(l2);
+                        }
                     }
-                }
-                wgmma_commit();
-                if (kb > 0) {                          // the previous block's MMAs have retired: release its stage
-                    wgmma_wait<1>();
-                    mbar_arrive(empty(last));
+                    const uint64_t k = ks * 2;             // 8 tf32 = 32 bytes inside the swizzle row (16-byte units)
+                    const uint32_t first = (kb == 0 && ks == 0) ? 0u : 1u;
+                    wgmma_fence();                         // the A registers were just written
+                    if (NS == 2) {                         // lo*hi + hi*lo + hi*hi
+                        wgmma_tf32(d0, p2[0], b0 + k, first);
+                        wgmma_tf32(d0, p1[0], b0 + kImg + k, 1u);
+                        wgmma_tf32(d0, p1[0], b0 + k, 1u);
+                        wgmma_tf32(d1, p2[1], b0 + k, first);
+                        wgmma_tf32(d1, p1[1], b0 + kImg + k, 1u);
+                        wgmma_tf32(d1, p1[1], b0 + k, 1u);
+                    } else {                               // smallest terms first: x3 v1, x1 v3, x2 v2, x2 v1, x1 v2, x1 v1
+                        wgmma_tf32(d0, p3[0], b0 + k, first);
+                        wgmma_tf32(d0, p1[0], b0 + 2 * kImg + k, 1u);
+                        wgmma_tf32(d0, p2[0], b0 + kImg + k, 1u);
+                        wgmma_tf32(d0, p2[0], b0 + k, 1u);
+                        wgmma_tf32(d0, p1[0], b0 + kImg + k, 1u);
+                        wgmma_tf32(d0, p1[0], b0 + k, 1u);
+                        wgmma_tf32(d1, p3[1], b0 + k, first);
+                        wgmma_tf32(d1, p1[1], b0 + 2 * kImg + k, 1u);
+                        wgmma_tf32(d1, p2[1], b0 + kImg + k, 1u);
+                        wgmma_tf32(d1, p2[1], b0 + k, 1u);
+                        wgmma_tf32(d1, p1[1], b0 + kImg + k, 1u);
+                        wgmma_tf32(d1, p1[1], b0 + k, 1u);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();                       // the previous k-step's MMAs have retired
+                    if (ks == 0 && kb > 0) mbar_arrive(empty(last));   // ... and with them the previous block's stage
                 }
                 last = s;
                 if (++s == kStages) {
@@ -330,55 +300,60 @@ project_wgmma_kernel(const float *__restrict__ X, const float *__restrict__ vimg
                 }
             }
             wgmma_wait<0>();
-            fence_operands(d);
-            const int64_t ra = tile * kTileM + wg * 64 + rq, rb = ra + 8;
-            float n1a = 0.f, n1b = 0.f;
-            if (MODE == 1) {                           // read before the release: the producers reuse this slot two tiles on
-                n1a = s_n1[(it & 1) * kTileM + wg * 64 + rq];
-                n1b = s_n1[(it & 1) * kTileM + wg * 64 + rq + 8];
-            }
+            fence_operands(d0);
+            fence_operands(d1);
             mbar_arrive(empty(last));
-            float na = 0.f, nb = 0.f;
-            if (MODE == 1) {
-                // y = acc / ||x - mean1|| - mean2 ; out = y / ||y||
-                const float ia = 1.f / sqrtf(n1a), ib = 1.f / sqrtf(n1b);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const float2 e = *reinterpret_cast<const float2 *>(s_inv_phi + 8 * j + cq);
-                    d[4 * j] = fmaf(d[4 * j], ia, -e.x);
-                    d[4 * j + 1] = fmaf(d[4 * j + 1], ia, -e.y);
-                    d[4 * j + 2] = fmaf(d[4 * j + 2], ib, -e.x);
-                    d[4 * j + 3] = fmaf(d[4 * j + 3], ib, -e.y);
-                    na = fmaf(d[4 * j], d[4 * j], fmaf(d[4 * j + 1], d[4 * j + 1], na));
-                    nb = fmaf(d[4 * j + 2], d[4 * j + 2], fmaf(d[4 * j + 3], d[4 * j + 3], nb));
-                }
-                na += __shfl_xor_sync(0xffffffffu, na, 1);
-                na += __shfl_xor_sync(0xffffffffu, na, 2);
-                nb += __shfl_xor_sync(0xffffffffu, nb, 1);
-                nb += __shfl_xor_sync(0xffffffffu, nb, 2);
-                const float sa = 1.f / sqrtf(na), sb = 1.f / sqrtf(nb);
+            for (int m = 0; m < 2; ++m) {
+                float(&d)[64] = m == 0 ? d0 : d1;
+                const int64_t ra = tile * kTileM + 128 * wg + 64 * m + rq, rb = ra + 8;
+                float na = 0.f, nb = 0.f;
+                if (MODE == 1) {
+                    // y = acc / ||x - mean1|| - mean2 ; out = y / ||y||
+                    float n1a = ss[m][0], n1b = ss[m][1];
+                    n1a += __shfl_xor_sync(0xffffffffu, n1a, 1);
+                    n1a += __shfl_xor_sync(0xffffffffu, n1a, 2);
+                    n1b += __shfl_xor_sync(0xffffffffu, n1b, 1);
+                    n1b += __shfl_xor_sync(0xffffffffu, n1b, 2);
+                    const float ia = 1.f / sqrtf(n1a), ib = 1.f / sqrtf(n1b);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    if (ra < N) *reinterpret_cast<float2 *>(rho + ra * 128 + 8 * j + cq) = make_float2(d[4 * j] * sa, d[4 * j + 1] * sa);
-                    if (rb < N) *reinterpret_cast<float2 *>(rho + rb * 128 + 8 * j + cq) = make_float2(d[4 * j + 2] * sb, d[4 * j + 3] * sb);
-                }
-            } else {
-                // ||fea||^2 = sum_r rho^2 / Phi_r   (VBx/VBx.py:87); a row's 128 columns are spread over a quad of lanes
+                    for (int j = 0; j < 16; ++j) {
+                        const float2 e = *reinterpret_cast<const float2 *>(s_inv_phi + 8 * j + cq);
+                        d[4 * j] = fmaf(d[4 * j], ia, -e.x);
+                        d[4 * j + 1] = fmaf(d[4 * j + 1], ia, -e.y);
+                        d[4 * j + 2] = fmaf(d[4 * j + 2], ib, -e.x);
+                        d[4 * j + 3] = fmaf(d[4 * j + 3], ib, -e.y);
+                        na = fmaf(d[4 * j], d[4 * j], fmaf(d[4 * j + 1], d[4 * j + 1], na));
+                        nb = fmaf(d[4 * j + 2], d[4 * j + 2], fmaf(d[4 * j + 3], d[4 * j + 3], nb));
+                    }
+                    na += __shfl_xor_sync(0xffffffffu, na, 1);
+                    na += __shfl_xor_sync(0xffffffffu, na, 2);
+                    nb += __shfl_xor_sync(0xffffffffu, nb, 1);
+                    nb += __shfl_xor_sync(0xffffffffu, nb, 2);
+                    const float sa = 1.f / sqrtf(na), sb = 1.f / sqrtf(nb);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const float2 ip = *reinterpret_cast<const float2 *>(s_inv_phi + 8 * j + cq);
-                    na = fmaf(d[4 * j] * d[4 * j], ip.x, fmaf(d[4 * j + 1] * d[4 * j + 1], ip.y, na));
-                    nb = fmaf(d[4 * j + 2] * d[4 * j + 2], ip.x, fmaf(d[4 * j + 3] * d[4 * j + 3], ip.y, nb));
-                    if (ra < N) *reinterpret_cast<float2 *>(rho + ra * 128 + 8 * j + cq) = make_float2(d[4 * j], d[4 * j + 1]);
-                    if (rb < N) *reinterpret_cast<float2 *>(rho + rb * 128 + 8 * j + cq) = make_float2(d[4 * j + 2], d[4 * j + 3]);
-                }
-                na += __shfl_xor_sync(0xffffffffu, na, 1);
-                na += __shfl_xor_sync(0xffffffffu, na, 2);
-                nb += __shfl_xor_sync(0xffffffffu, nb, 1);
-                nb += __shfl_xor_sync(0xffffffffu, nb, 2);
-                if ((lane & 3) == 0) {                 // G_t, R = 128
-                    if (ra < N) gframe[ra] = -0.5f * (na + 128.f * 1.8378770664093453f);
-                    if (rb < N) gframe[rb] = -0.5f * (nb + 128.f * 1.8378770664093453f);
+                    for (int j = 0; j < 16; ++j) {
+                        if (ra < N) *reinterpret_cast<float2 *>(rho + ra * 128 + 8 * j + cq) = make_float2(d[4 * j] * sa, d[4 * j + 1] * sa);
+                        if (rb < N) *reinterpret_cast<float2 *>(rho + rb * 128 + 8 * j + cq) = make_float2(d[4 * j + 2] * sb, d[4 * j + 3] * sb);
+                    }
+                } else {
+                    // ||fea||^2 = sum_r rho^2 / Phi_r   (VBx/VBx.py:87); a row's 128 columns are spread over a quad of lanes
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const float2 ip = *reinterpret_cast<const float2 *>(s_inv_phi + 8 * j + cq);
+                        na = fmaf(d[4 * j] * d[4 * j], ip.x, fmaf(d[4 * j + 1] * d[4 * j + 1], ip.y, na));
+                        nb = fmaf(d[4 * j + 2] * d[4 * j + 2], ip.x, fmaf(d[4 * j + 3] * d[4 * j + 3], ip.y, nb));
+                        if (ra < N) *reinterpret_cast<float2 *>(rho + ra * 128 + 8 * j + cq) = make_float2(d[4 * j], d[4 * j + 1]);
+                        if (rb < N) *reinterpret_cast<float2 *>(rho + rb * 128 + 8 * j + cq) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+                    }
+                    na += __shfl_xor_sync(0xffffffffu, na, 1);
+                    na += __shfl_xor_sync(0xffffffffu, na, 2);
+                    nb += __shfl_xor_sync(0xffffffffu, nb, 1);
+                    nb += __shfl_xor_sync(0xffffffffu, nb, 2);
+                    if (t == 0) {                          // G_t, R = 128
+                        if (ra < N) gframe[ra] = -0.5f * (na + 128.f * 1.8378770664093453f);
+                        if (rb < N) gframe[rb] = -0.5f * (nb + 128.f * 1.8378770664093453f);
+                    }
                 }
             }
         }
@@ -398,10 +373,59 @@ __global__ void build_plda_v_kernel(const float *__restrict__ tr, const float *_
 // cudaFuncSetAttribute is per device; everything else the launches need comes from the caller's workspace
 bool g_configured[64][3][2] = {};
 
+using EncodeTiledFn = CUresult (*)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
+                                   const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// the driver's tensor-map encoder through the runtime, so that the library does not link against libcuda itself
+EncodeTiledFn encode_tiled() {
+    static const EncodeTiledFn fn = [] {
+        void *p = nullptr;
+        cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+        if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &p, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            p = nullptr;
+        return reinterpret_cast<EncodeTiledFn>(p);
+    }();
+    return fn;
+}
+
+// TMA map of X [N, D] fp32 row-major: boxes of 32 columns x kTileM rows, 128-byte swizzle (the wgmma K-major layout),
+// rows past N read as zeros.  False, with the reason, when TMA cannot address X.
+bool encode_x_map(CUtensorMap *map, const float *X, int64_t N, int D, std::string *err) {
+    if (reinterpret_cast<uintptr_t>(X) & 15) {
+        if (err) *err = "the tensor-core projection needs X 16-byte aligned (TMA)";
+        return false;
+    }
+    if (N > INT32_MAX - kTileM) {
+        if (err) *err = "the tensor-core projection needs fewer than 2^31 - 256 frames (TMA row coordinate)";
+        return false;
+    }
+    const EncodeTiledFn encode = encode_tiled();
+    if (!encode) {
+        if (err) *err = "cuTensorMapEncodeTiled is not available from the driver";
+        return false;
+    }
+    const cuuint64_t dims[2] = {(cuuint64_t)D, (cuuint64_t)N};
+    const cuuint64_t strides[1] = {(cuuint64_t)D * sizeof(float)};
+    const cuuint32_t box[2] = {kKB, kTileM};
+    const cuuint32_t elem_strides[2] = {1, 1};
+    const CUresult r = encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(X), dims, strides, box, elem_strides,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        if (err) *err = "cuTensorMapEncodeTiled failed for X (error " + std::to_string((int)r) + ")";
+        return false;
+    }
+    return true;
+}
+
 // one GEMM pass [N,D] x [D,128] of the given MODE; V is row-major [D,128] in device memory
 template <int MODE, int NS>
 int launch_gemm_tc(float *vimg, int64_t N, const float *X, int D, const float *V, const float *Phi, float *out, float *gframe,
                    const float *a_off, const float *e_off, cudaStream_t st, std::string *err) {
+    CUtensorMap xmap;
+    if (!encode_x_map(&xmap, X, N, D, err)) return -1;
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev < 0 || dev >= 64) {
@@ -424,9 +448,10 @@ int launch_gemm_tc(float *vimg, int64_t N, const float *X, int D, const float *V
     build_v_images_kernel<NS><<<D / kKB, 256, 0, st>>>(V, D, vimg);
     const int64_t n_tiles = (N + kTileM - 1) / kTileM;
     const int grid = (int)std::min<int64_t>(n_tiles, sms);
-    project_wgmma_kernel<MODE, NS><<<grid, kThreads, Pipe<NS>::kSmemBytes, st>>>(X, vimg, out, N, D, Phi, gframe, a_off, e_off);
-    if (cudaGetLastError() != cudaSuccess) {
-        if (err) *err = "wgmma projection launch failed";
+    project_wgmma_kernel<MODE, NS><<<grid, kThreads, Pipe<NS>::kSmemBytes, st>>>(xmap, vimg, out, N, D, Phi, gframe, a_off, e_off);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+        if (err) *err = std::string("wgmma projection launch failed: ") + cudaGetErrorString(e);
         return -1;
     }
     return 2;
