@@ -213,123 +213,76 @@ int vbx_init_turns(vbx_handle_t h, const int64_t *seg, const int64_t *spk_off, c
 int vbx_init_random(vbx_handle_t h, const uint64_t *rec_key, const uint64_t *seed, const int32_t *n_states,
                     void *gamma_out, void *pi_out, int32_t out_is_f64, void *stream);
 
-/* Speaker linking across the recordings of an archive (DESIGN.md section 5.15); needs a handle, no plan.
- * M speakers (a recording's VB-HMM labels, numbered across the archive); all arrays are DEVICE arrays:
- *   fea [N,R] float32, Phi [R]   the features and between-speaker variances the VB-HMM ran with (R <= 128)
- *   speaker [N] int32            the speaker of x-vector t in [0, M), or -1 (any value outside [0, M) counts as -1)
- *   speaker_rec [M] int32        the recording of each speaker (speakers of one recording are never linked)
- *   Fa, Fb (HOST)                the VB-HMM's scalars; c = Fa / Fb must be finite and >= 0
- * Per speaker s, n_s = #{t : speaker[t] = s} and F_s = sum of those rows of fea, float64, summed in an order fixed by the
- * positions of s's x-vectors relative to its first one.  Each speaker's CTA reads speaker[] over the whole span from its
- * first to its last x-vector, so the statistics cost sum_s (span_s + n_s R) reads: about (K + R) N for speakers packed by
- * recording with K speakers each, but up to M N when speakers spread across the whole array.  With L_s,r = 1 + c n_s Phi_r and b_s,r = c sqrt(Phi_r) F_s,r
+/* Speaker linking across the recordings of an archive (DESIGN.md sections 5.15, 5.18, 5.19) for G independent
+ * problems in one set of launches, e.g. one per setting of a sweep; one archive is G = 1.  Needs a handle, no plan.  The
+ * problems share fea [N,R] float32 and Phi [R] (DEVICE: the features and between-speaker variances the VB-HMM ran with,
+ * R <= 128); problem g has
+ *   speaker [G,N] int32 (DEVICE)   row g: the speaker of x-vector t in [0, M[g]), or -1 (other values count as -1)
+ *   M [G] (HOST)                   its number of speakers (a recording's VB-HMM labels, numbered across the archive)
+ *   speaker_rec [sum M] (DEVICE)   the recording of each speaker (speakers of one recording are never linked), problem
+ *                                  g's at off_g = M[0] + .. + M[g-1]
+ *   Fa [G], Fb [G] (HOST)          the VB-HMM's scalars; every c_g = Fa[g] / Fb[g] must be finite and >= 0
+ * Per speaker s, n_s = #{t : speaker[g,t] = s} and F_s = sum of those rows of fea, float64, summed in an order fixed by
+ * the positions of s's x-vectors relative to its first one.  Each speaker's CTA reads its row of speaker[] over the
+ * whole span from its first to its last x-vector, so the statistics cost sum_s (span_s + n_s R) reads: about (K + R) N
+ * per problem for speakers packed by recording with K speakers each, but up to M N when speakers spread across the
+ * whole array.  With L_s,r = 1 + c_g n_s Phi_r and b_s,r = c_g sqrt(Phi_r) F_s,r
  *   LLR(s,u) = 1/2 sum_r [ (b_s,r + b_u,r)^2 / (L_s,r + L_u,r - 1) - b_s,r^2 / L_s,r - b_u,r^2 / L_u,r
  *                          + log L_s,r + log L_u,r - log(L_s,r + L_u,r - 1) ]
  * (0 when n_s or n_u is 0), and the distance of two speakers is -LLR; 1e30 between two speakers of one recording, 0 on
- * the diagonal.  Z_out [M-1,4] (scipy layout) is the average linkage of those distances, computed by vbx_ahc's linkage
- * kernel (ties: the lowest slot).  Optional outputs (NULL: not written): n_out [M], F_out [M,R], dist_out [M,M] float64.
- * workspace: vbx_link_workspace_bytes(M) bytes (about 8 M^2 + 1.1 KB M), 256-byte aligned.  Stream ordered, no
- * allocation, no host synchronisation.  M above VBX_LINK_MAX_SPEAKERS (the linkage kernel keeps 4 (M - 1) in int32)
- * returns VBX_ERR_ARG. */
+ * the diagonal.  With mean, std [sum M] (DEVICE, problem g's at off_g: cohort statistics of the same speakers from
+ * vbx_cohort_stats_batch; every std must be finite and > 0) the distance of two speakers of different recordings is
+ * -S(s, u) instead, the adaptive symmetric normalisation (AS-norm) of DESIGN.md section 5.17
+ *   S(s, u) = 1/2 [ (LLR(s,u) - mean[s]) / std[s] + (LLR(s,u) - mean[u]) / std[u] ],
+ * with 1e30 within a recording and 0 on the diagonal as before; the matrix stays symmetric bit for bit.  Give both of
+ * mean and std or neither.  Z_out [sum M, 4] holds problem g's average linkage of those distances (M[g] - 1 rows from
+ * row off_g, scipy's layout), computed by vbx_ahc's linkage kernel (ties: the lowest slot); it is needed when some
+ * M[g] >= 2.  Optional outputs (NULL: not written): n_out [sum M], F_out [sum M, R] and dist_out with problem g's
+ * M[g] x M[g] distances from element M[0]^2 + .. + M[g-1]^2, float64.  Problem g's n, F, distances and Z do not depend
+ * on the other problems: they are the same bits in one launch or over several.  workspace:
+ * vbx_link_batch_workspace_bytes(G, M) bytes, 256-byte aligned: about 8 M[g]^2 + 1.1 KB M[g] per problem, and the
+ * size of a batch is at most the sum of the sizes of its problems alone, so problems packed by those sizes fit a
+ * budget.  Stream ordered, no allocation, no host synchronisation; the problems' offsets and c_g go to the device in
+ * one copy from the host, as vbx_ahc's offsets do.  R outside 1..128, an M[g] outside [0, VBX_LINK_MAX_SPEAKERS] (the
+ * linkage kernel keeps 4 (M - 1) in int32), more than 2^31 - 1 speakers in all, a bad c_g, mean without std (or std
+ * without mean), null pointers or a workspace too small return VBX_ERR_ARG. */
 #define VBX_LINK_MAX_SPEAKERS 536870912 /* 2^29 */
-int vbx_link_workspace_bytes(vbx_handle_t h, int64_t M, size_t *bytes_out);
-int vbx_link(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-             int64_t M, const int32_t *speaker_rec, double Fa, double Fb, void *workspace, size_t workspace_bytes,
-             double *n_out, double *F_out, double *dist_out, double *Z_out, void *stream);
-
-/* G independent linking problems in one set of launches (DESIGN.md section 5.18), e.g. one per setting of a sweep; needs
- * a handle, no plan.  The problems share fea [N,R] and Phi [R] (DEVICE, as for vbx_link); problem g has
- *   speaker [G,N] int32 (DEVICE)   row g: the speaker of x-vector t in [0, M[g]), or -1 (other values count as -1)
- *   M [G] (HOST)                   its number of speakers
- *   speaker_rec [sum M] (DEVICE)   the recording of each speaker, problem g's at off_g = M[0] + .. + M[g-1]
- *   Fa [G], Fb [G] (HOST)          its scalars; every c_g = Fa[g] / Fb[g] must be finite and >= 0
- * The outputs are packed by the speaker offsets off_g: n_out [sum M], F_out [sum M, R] (optional, as for vbx_link),
- * Z_out [sum M, 4] with problem g's M[g] - 1 rows from row off_g (vbx_ahc's layout; needed when some M[g] >= 2) and
- * dist_out (optional) with problem g's M[g] x M[g] distances from element M[0]^2 + .. + M[g-1]^2.  Problem g's n, F,
- * distances and Z are bit-identical to vbx_link run on that problem alone.  workspace: vbx_link_batch_workspace_bytes(G,
- * M) bytes, 256-byte aligned; it is at most the sum of vbx_link_workspace_bytes(M[g]), so problems packed by those sizes
- * fit a budget.  Stream ordered, no allocation; the problems' offsets and c_g go to the device in one copy from the
- * host, as vbx_ahc's offsets do.  R outside 1..128, an M[g] outside [0, VBX_LINK_MAX_SPEAKERS], more than 2^31 - 1
- * speakers in all, a bad c_g or a workspace too small return VBX_ERR_ARG. */
 int vbx_link_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, size_t *bytes_out);
 int vbx_link_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
                    const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
                    const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
-                   double *dist_out, double *Z_out, void *stream);
+                   double *dist_out, double *Z_out, const double *mean, const double *std, void *stream);
 
-/* Enrolment against known speakers (DESIGN.md section 5.16); needs a handle, no plan.  Archive speakers as for vbx_link
- * (fea [N,R], Phi [R], speaker [N] in [0, M), DEVICE), packed by recording: speaker_rec_offsets [n_rec+1] (HOST int64,
- * from 0 to M, non-decreasing) holds recording b's speakers at speaker_rec_offsets[b] .. [b+1]-1.  Enrolled speakers:
- * enroll_fea [N_e,R] (DEVICE, the same features and Phi) with enroll_speaker [N_e] in [0, E) (DEVICE; packed by speaker
- * the statistics cost about (E + R) N_e reads).  Both sets get vbx_link's statistics n, F, b, e (its kernels), and
- *   llr [s][e] = LLR(s, e) of vbx_link, bit-identical to -dist of vbx_link run on the same speakers.
- * Per recording with K speakers, the minimum-cost assignment of the K x (E + K) matrix C[k][e] = threshold - llr[k][e]
- * (e < E), C[k][E + j] = 0, by shortest augmenting paths; ties to the lowest column.  Outputs (DEVICE):
- *   assign_out [M] int32      the enrolled speaker of each archive speaker, -1 = unknown
- *   best_llr_out [M]          llr of the assigned pair; for an unknown speaker its largest llr
- *   llr_out [M,E], n_out [M], F_out [M,R], n_enroll_out [E], F_enroll_out [E,R]: optional (NULL: not written)
- * workspace: vbx_enroll_workspace_bytes(M, E, max_k) bytes with max_k >= the largest K, 256-byte aligned (about
- * 8 M E + 1.1 KB (M + E) + 2 x SMs x 50 (E + max_k) bytes).  The offsets are copied to the device from pageable memory:
- * no host synchronisation, no allocation.  VBX_ERR_ARG: R outside 1..128, c = Fa / Fb negative or not finite,
- * |threshold| > 1e15, E or N_e < 1, null pointers, misaligned or short workspace, offsets not from 0 to M or
- * decreasing. */
-int vbx_enroll_workspace_bytes(vbx_handle_t h, int64_t M, int64_t E, int64_t max_k, size_t *bytes_out);
-int vbx_enroll(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-               int64_t M, const int64_t *speaker_rec_offsets, int32_t n_rec, const float *enroll_fea, int64_t N_e,
-               const int32_t *enroll_speaker, int64_t E, double Fa, double Fb, double threshold, void *workspace,
-               size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
-               double *F_out, double *n_enroll_out, double *F_enroll_out, void *stream);
-
-/* Score normalisation against a cohort (adaptive symmetric normalisation, DESIGN.md section 5.17); needs a handle, no
- * plan.  M scored speakers as for vbx_link (fea [N,R], Phi [R], speaker [N] in [0, M), DEVICE) and C >= 2 cohort
- * speakers (cohort_fea [N_c,R] through the same front end, cohort_speaker [N_c] in [0, C), DEVICE).  Both sets get
- * vbx_link's statistics; every scored speaker x is scored against every cohort speaker with vbx_link's LLR (the kernel of
- * vbx_enroll: bit-identical to vbx_enroll's llr against the same speakers), and with K = min(top_k, C)
- *   mean_out [x] = mean of x's K largest cohort scores, std_out [x] = their population standard deviation (ddof 0)
- * (DEVICE float64 [M]; ties at the K-th value count as many copies as needed).  scores_out [M,C]: optional (NULL: not
- * written).  Fixed-order sums: the bits do not depend on the run or on which other speakers share the call.
- * workspace: vbx_cohort_workspace_bytes(M, C) bytes (about 8 M C + 1.1 KB (M + C)), 256-byte aligned.  Stream ordered,
- * no allocation, no host synchronisation.  VBX_ERR_ARG: R outside 1..128, c = Fa / Fb negative or not finite, C < 2,
- * top_k < 2, N_c < 1, M above 2^31 - 1, null pointers, misaligned or short workspace. */
-int vbx_cohort_workspace_bytes(vbx_handle_t h, int64_t M, int64_t C, size_t *bytes_out);
-int vbx_cohort_stats(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-                     int64_t M, const float *cohort_fea, int64_t N_c, const int32_t *cohort_speaker, int64_t C,
-                     double Fa, double Fb, int32_t top_k, void *workspace, size_t workspace_bytes, double *mean_out,
-                     double *std_out, double *scores_out, void *stream);
-/* vbx_link with normalised scores: the distance of two speakers of different recordings is -S(s, u),
- *   S(s, u) = 1/2 [ (LLR(s,u) - mean[s]) / std[s] + (LLR(s,u) - mean[u]) / std[u] ],
- * with mean, std [M] (DEVICE, vbx_cohort_stats over the same speakers; every std must be finite and > 0); 1e30 within a
- * recording and 0 on the diagonal as before, and the matrix stays symmetric bit for bit.  dist_out then holds these. */
-int vbx_link_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-                  int64_t M, const int32_t *speaker_rec, double Fa, double Fb, void *workspace, size_t workspace_bytes,
-                  double *n_out, double *F_out, double *dist_out, double *Z_out, const double *mean, const double *std,
-                  void *stream);
-/* vbx_enroll on S(s, e) in place of LLR(s, e), with mean, std [M] of the archive speakers and enroll_mean, enroll_std [E]
- * of the enrolled speakers (DEVICE, vbx_cohort_stats): the threshold is on S, and best_llr_out and llr_out hold S. */
-int vbx_enroll_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-                    int64_t M, const int64_t *speaker_rec_offsets, int32_t n_rec, const float *enroll_fea, int64_t N_e,
-                    const int32_t *enroll_speaker, int64_t E, double Fa, double Fb, double threshold, void *workspace,
-                    size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
-                    double *F_out, double *n_enroll_out, double *F_enroll_out, const double *mean, const double *std,
-                    const double *enroll_mean, const double *enroll_std, void *stream);
-
-/* Enrolment, cohort statistics and normalised linking of G independent problems in one set of launches (DESIGN.md
- * section 5.19), e.g. the settings of a sweep; each needs a handle, no plan.  The problems share fea [N,R] and Phi [R]
- * (DEVICE); problem g has its row g of speaker [G,N] (DEVICE, local speakers in [0, M[g]), -1 = none), M [G] (HOST)
- * and Fa [g], Fb [g] (HOST; every c_g = Fa[g] / Fb[g] finite and >= 0).  Per-speaker arrays are packed by the speaker
- * offsets off_g = M[0] + .. + M[g-1].  Problem g's outputs are bit-identical to the single-problem entry run on it
- * alone, in one launch or over several.  Stream ordered, no allocation, no host synchronisation: the problems'
- * offsets and scalars go to the device in one copy from pageable host memory.  VBX_ERR_ARG as for the single entries,
- * and for G < 0 or more than 2^31 - 1 speakers in all.
+/* Enrolment and cohort statistics of G independent problems in one set of launches (DESIGN.md sections 5.16, 5.17,
+ * 5.19), e.g. the settings of a sweep; one archive is G = 1.  Each needs a handle, no plan.  The problems share fea
+ * [N,R] and Phi [R] (DEVICE, as for vbx_link_batch); problem g has its row g of speaker [G,N] (DEVICE, local speakers
+ * in [0, M[g]), -1 = none), M [G] (HOST) and Fa [g], Fb [g] (HOST; every c_g = Fa[g] / Fb[g] finite and >= 0).
+ * Per-speaker arrays are packed by the speaker offsets off_g = M[0] + .. + M[g-1].  Every speaker set gets
+ * vbx_link_batch's statistics n, F (and the b, e of its LLR) with c_g.  Problem g's outputs do not depend on the other
+ * problems: they are the same bits in one launch or over several.  Stream ordered, no allocation, no host
+ * synchronisation: the problems' offsets and scalars go to the device in one copy from pageable host memory.
+ * VBX_ERR_ARG: R outside 1..128, a bad c_g, G < 0, an M[g] outside [0, VBX_LINK_MAX_SPEAKERS], more than 2^31 - 1
+ * speakers in all, null pointers, misaligned or short workspace, and the conditions given below.
  *
- * vbx_enroll_batch: vbx_enroll of every problem against the one enrolled set (enroll_fea [N_e,R], enroll_speaker [N_e]
- * in [0, E), DEVICE) at n_thr >= 1 thresholds (HOST, each |t| <= 1e15).  speaker_rec_offsets [G, n_rec + 1] (HOST):
- * row g as vbx_enroll's for problem g, from 0 to M[g].  Outputs (DEVICE): assign_out [n_thr, sum M] int32 and
- * best_llr_out [n_thr, sum M] (plane h: threshold h); optional llr_out [sum M, E], n_out [sum M], F_out [sum M, R],
- * n_enroll_out [G, E], F_enroll_out [G, E, R].  mean, std [sum M] and enroll_mean, enroll_std [G, E] (DEVICE, all four
- * or none): the normalised path of vbx_enroll_norm, problem g with its own rows.  workspace:
+ * vbx_enroll_batch: every problem's archive speakers against one set of E known speakers (enroll_fea [N_e,R] through
+ * the same front end, enroll_speaker [N_e] in [0, E), DEVICE; packed by speaker the enrolled statistics cost about
+ * (E + R) N_e reads per problem) at n_thr >= 1 thresholds (HOST, each |t| <= 1e15).  Problem g's archive speakers are
+ * packed by recording: row g of speaker_rec_offsets [G, n_rec + 1] (HOST int64, from 0 to M[g], non-decreasing) holds
+ * recording b's speakers at [b] .. [b+1]-1.  Every archive speaker s is scored against every enrolled speaker e,
+ *   llr [s][e] = LLR(s, e) of vbx_link_batch, bit-identical to -dist of vbx_link_batch run on the same speakers.
+ * Per recording with K speakers and threshold t, the minimum-cost assignment of the K x (E + K) matrix
+ * C[k][e] = t - llr[k][e] (e < E), C[k][E + j] = 0 ("unknown" columns), by shortest augmenting paths; ties go to the
+ * lowest column, so a real column at cost 0 wins over the unknown ones.  Outputs (DEVICE):
+ *   assign_out [n_thr, sum M] int32   the enrolled speaker of each archive speaker, -1 = unknown (plane h: threshold h)
+ *   best_llr_out [n_thr, sum M]       llr of the assigned pair; for an unknown speaker its largest llr
+ *   llr_out [sum M, E], n_out [sum M], F_out [sum M, R], n_enroll_out [G, E], F_enroll_out [G, E, R]: optional (NULL:
+ *   not written)
+ * mean, std [sum M] and enroll_mean, enroll_std [G, E] (DEVICE, all four or none, except that mean and std may be NULL
+ * when sum M = 0; cohort statistics from vbx_cohort_stats_batch): the assignment runs on S(s, e) of vbx_link_batch in place of LLR(s, e), problem g with its
+ * own rows; the thresholds are on S, and best_llr_out and llr_out hold S.  workspace:
  * vbx_enroll_batch_workspace_bytes(G, M, E, N_e, max_k, n_thr) bytes with max_k >= the largest K of any recording of
- * any problem, 256-byte aligned. */
+ * any problem, 256-byte aligned: about 8 sum M E + 1.1 KB (sum M + G E) + 4 G N_e + 2 x SMs x 50 (E + max_k) bytes.
+ * Further VBX_ERR_ARG: E, N_e or n_thr < 1, n_rec < 0, offsets not from 0 to M[g] or decreasing. */
 int vbx_enroll_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, int64_t E, int64_t N_e,
                                      int64_t max_k, int32_t n_thr, size_t *bytes_out);
 int vbx_enroll_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
@@ -339,22 +292,24 @@ int vbx_enroll_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t
                      size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
                      double *F_out, double *n_enroll_out, double *F_enroll_out, const double *mean, const double *std,
                      const double *enroll_mean, const double *enroll_std, void *stream);
-/* vbx_cohort_stats_batch: vbx_cohort_stats of every problem against one cohort (cohort_fea [N_c,R], cohort_speaker
- * [N_c] in [0, C), C >= 2, DEVICE), top_k >= 2.  Outputs mean_out, std_out [sum M] (DEVICE).  The enrolled speakers'
- * statistics per problem come from the same entry with fea = enroll_fea and speaker = enroll_speaker repeated G times.
- * workspace: vbx_cohort_stats_batch_workspace_bytes(G, M, C, N_c) bytes, 256-byte aligned. */
+/* vbx_cohort_stats_batch: the statistics that score normalisation (AS-norm, DESIGN.md section 5.17) needs, for every
+ * problem against one cohort of C >= 2 speakers known to be someone else (cohort_fea [N_c,R] through the same front
+ * end, cohort_speaker [N_c] in [0, C), DEVICE).  Every scored speaker x is scored against every cohort speaker with
+ * vbx_link_batch's LLR (the kernel of vbx_enroll_batch: bit-identical to its llr against the same speakers), and with
+ * the top K = min(top_k, C) of x's cohort scores, top_k >= 2,
+ *   mean_out [x] = mean of x's K largest cohort scores, std_out [x] = their population standard deviation (ddof 0)
+ * (DEVICE float64 [sum M]; ties at the K-th value count as many copies as needed), by fixed-order sums.  scores_out
+ * [sum M, C] (DEVICE): the cohort scores, optional (NULL: not written).  The enrolled speakers' statistics per problem
+ * come from the same entry with fea = enroll_fea and speaker = enroll_speaker repeated G times.  workspace:
+ * vbx_cohort_stats_batch_workspace_bytes(G, M, C, N_c) bytes, 256-byte aligned: about 8 sum M C + 1.1 KB (sum M + G C)
+ * + 4 G N_c bytes.  Further VBX_ERR_ARG: C < 2, top_k < 2, N_c < 1. */
 int vbx_cohort_stats_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, int64_t C, int64_t N_c,
                                            size_t *bytes_out);
 int vbx_cohort_stats_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
                            const int32_t *speaker, const int64_t *M, const float *cohort_fea, int64_t N_c,
                            const int32_t *cohort_speaker, int64_t C, const double *Fa, const double *Fb, int32_t top_k,
-                           void *workspace, size_t workspace_bytes, double *mean_out, double *std_out, void *stream);
-/* vbx_link_batch_norm: vbx_link_batch with every problem's distances -S as vbx_link_norm computes them, from mean, std
- * [sum M] (DEVICE, problem g's at off_g).  Workspace: vbx_link_batch_workspace_bytes. */
-int vbx_link_batch_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
-                        const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
-                        const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
-                        double *dist_out, double *Z_out, const double *mean, const double *std, void *stream);
+                           void *workspace, size_t workspace_bytes, double *mean_out, double *std_out,
+                           double *scores_out, void *stream);
 
 /* Float64 evaluation of the same EM loop ("exact" mode for the one-recording-per-call use of VBx/vbhmm.py:154-158,
  * where the reference stops on an ELBO improvement < 1e-6, VBx/vbhmm.py:157 -- below float32 resolution).

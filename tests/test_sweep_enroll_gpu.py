@@ -1,9 +1,9 @@
 """Enrolment and cohort normalisation inside the sweep on the device (DESIGN.md section 5.19): vbx_enroll_batch through
 enroll.enroll_many against enroll_speakers problem by problem and threshold by threshold (bit for bit, with and without
-normalisation, one launch and several), vbx_cohort_stats_batch against cohort_stats, vbx_link_batch_norm against
-link_speakers(norm=), and sweep_batch's names, scores and DER by name against diarize_batch(enroll_threshold=) and
-score_rttm(by_name=True), with a UEM, oracle overlaps, the oracle speaker count, AHC init, a cohort, ES2005a and the
-command line."""
+normalisation, one launch and several), vbx_cohort_stats_batch against cohort_stats, vbx_link_batch with mean and std
+against link_speakers(norm=), and sweep_batch's names, scores and DER by name against
+diarize_batch(enroll_threshold=) and score_rttm(by_name=True), with a UEM, oracle overlaps, the oracle speaker count,
+AHC init, a cohort, ES2005a and the command line."""
 import ctypes
 import json
 import os
@@ -83,7 +83,7 @@ def _largest_single(kind, offs, problems, *shape):
             elif kind == 'cohort':
                 rc = lib.vbx_cohort_stats_batch_workspace_bytes(h, 1, v, shape[0], shape[1], ctypes.byref(need))
             else:
-                rc = lib.vbx_link_workspace_bytes(h, int(M[0]), ctypes.byref(need))
+                rc = lib.vbx_link_batch_workspace_bytes(h, 1, v, ctypes.byref(need))
             assert rc == 0
             sizes.append(int(need.value))
         return max(sizes) + 1
@@ -150,7 +150,7 @@ def test_enroll_many_is_enroll_speakers_problem_by_problem(R, E, normalised):
                 assert np.array_equal(getattr(a, k), getattr(b, k)), k
 
 
-def test_cohort_stats_many_and_link_many_norm():
+def test_cohort_stats_many_and_link_many_with_statistics():
     fea, Phi, offs, problems, efea, espk, Fa, Fb = _archive(3, 128, 7)
     norm, cfea, cspk = _norms(fea, Phi, offs, problems, efea, espk, Fa, Fb, np.random.default_rng(3))
     for mb in (None, _largest_single('cohort', offs, problems, 12, 30)):

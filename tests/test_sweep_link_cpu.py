@@ -87,7 +87,7 @@ def test_workspace_layout_and_packing():
         lk, total = batch_layout(Ms)
         assert all(o % 256 == 0 for o in lk)                 # every problem's linkage region 256-byte aligned
         assert [lk[g + 1] - lk[g] for g in range(len(Ms))] == [al(linkage_bytes(M)) for M in Ms]
-        single = [batch_layout([M])[1] for M in Ms]          # vbx_link_workspace_bytes(M) = the batch of one
+        single = [batch_layout([M])[1] for M in Ms]          # each problem sized alone, as link_many packs them
         assert total <= sum(single)                          # so packing by the single sizes bounds every launch
         budget = max(single) + int(rng.integers(0, 2 * max(single)))
         batches = sweep.pack(single, budget)

@@ -107,15 +107,10 @@ def _workspace_bytes(*Ms):
         lib.vbx_destroy(h)
 
 
-def test_workspace_bytes_and_argument_errors():
+def test_batch_workspace_bytes_and_argument_errors():
     lib, h = _handle()
     try:
-        single = []
-        for M in MS:
-            need = ctypes.c_size_t()
-            assert lib.vbx_link_workspace_bytes(h, M, ctypes.byref(need)) == 0
-            single.append(int(need.value))
-            assert _workspace_bytes(M) == single[-1]
+        single = [_workspace_bytes(M) for M in MS]
         assert _workspace_bytes(*MS) <= sum(single)
         M = np.array([3, 2], dtype=np.int64)
         need = ctypes.c_size_t()
@@ -126,18 +121,21 @@ def test_workspace_bytes_and_argument_errors():
         rec = torch.arange(5, dtype=torch.int32, device=DEV)
         ws = torch.empty(need.value, dtype=torch.uint8, device=DEV)
         Z = torch.empty((5, 4), dtype=torch.float64, device=DEV)
-        p = lambda t: ctypes.c_void_p(t.data_ptr())
+        stat = torch.ones(5, dtype=torch.float64, device=DEV)
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
         a = lambda x: np.ascontiguousarray(x, dtype=np.float64)
 
-        def call(R=8, Ms=M, Fa=(0.3, 0.3), Fb=(17.0, 17.0), size=need.value):
+        def call(R=8, Ms=M, Fa=(0.3, 0.3), Fb=(17.0, 17.0), size=need.value, mean=None, std=None):
             Ms, Fa, Fb = np.asarray(Ms, dtype=np.int64), a(Fa), a(Fb)
             v = lambda x: x.ctypes.data_as(ctypes.c_void_p)
             return lib.vbx_link_batch(h, p(fea), p(Phi), 4, R, 2, p(spk), v(Ms), p(rec), v(Fa), v(Fb), p(ws), size,
-                                      None, None, None, p(Z), None)
+                                      None, None, None, p(Z), p(mean), p(std), None)
         assert call() == 0
+        assert call(mean=stat, std=stat) == 0
         torch.cuda.synchronize()
         for bad in (dict(R=0), dict(R=129), dict(Ms=[3, _lib.LINK_MAX_SPEAKERS + 1]), dict(Ms=[3, -1]),
-                    dict(Fa=(0.3, -0.3)), dict(Fa=(0.3, float('nan'))), dict(Fb=(17.0, 0.0)), dict(size=need.value - 1)):
+                    dict(Fa=(0.3, -0.3)), dict(Fa=(0.3, float('nan'))), dict(Fb=(17.0, 0.0)), dict(size=need.value - 1),
+                    dict(mean=stat), dict(std=stat)):
             assert call(**bad) == -1, bad                                  # VBX_ERR_ARG
     finally:
         lib.vbx_destroy(h)

@@ -1,10 +1,11 @@
 """Times score normalisation against a cohort (DESIGN.md section 5.17).
 
-1. vbx_cohort_stats on synthetic archives of M = 16 000 speakers (4 per recording, 1 .. 15 x-vectors each, R = 128)
-   against C = 1 000 and 10 000 cohort speakers (1 .. 15 x-vectors each) at top_k = 200: device time of every kernel
-   from torch.profiler over --rounds calls after one warm-up call, next to the pairs and bytes the score kernel needs.
-   The statistics row sums the span and statistics kernels of both speaker sets.  Also the normalisation kernel inside
-   vbx_link_norm at M = 4 000 (the linkage dominates that call).
+1. cohort_stats (vbx_cohort_stats_batch) on synthetic archives of M = 16 000 speakers (4 per recording, 1 .. 15
+   x-vectors each, R = 128) against C = 1 000 and 10 000 cohort speakers (1 .. 15 x-vectors each) at top_k = 200: device
+   time of every kernel from torch.profiler over --rounds calls after one warm-up call, next to the pairs and bytes the
+   score kernel needs. The statistics row sums the span and statistics kernels of both speaker sets and the copy of the
+   cohort speaker index.  Also the normalisation kernel inside link_speakers(norm=) at M = 4 000 (the linkage dominates
+   that call).
 2. Whole diarize_batch calls on the synthetic archive of tools/bench_sweep.py (17 recordings) with linking and an
    enrolment of 10 speakers, without and with a cohort of 200 speakers (20 x-vectors each), alternating in one process
    (medians, minima, maxima).
@@ -29,7 +30,7 @@ from bench_link import speakers  # noqa: E402
 from bench_sweep import GOLD, synthetic_archive  # noqa: E402
 from vbx_b200 import cohort, link, pipeline  # noqa: E402
 
-KERNELS = {'statistics': ('link_init_kernel', 'link_span_kernel', 'link_stats_kernel'),
+KERNELS = {'statistics': ('link_init_kernel', 'link_span_kernel', 'link_stats_kernel', 'repeat_index_kernel'),
            'score': ('enroll_score_kernel',), 'top_k': ('cohort_topk_kernel',), 'normalise': ('norm_scores_kernel',)}
 
 
@@ -75,7 +76,7 @@ def main():
                            top_k_bytes_read=10 * 8 * M * C)
         del fea, cfea
         torch.cuda.empty_cache()
-    # the normalisation kernel inside vbx_link_norm
+    # the normalisation kernel inside link_speakers(norm=)
     M = 4000
     fea, Phi, offs, labels = speakers(M)
     cfea, cspk = enrolled(1000, seed=2)

@@ -1,9 +1,10 @@
 """Times enrolment against known speakers (DESIGN.md section 5.16).
 
-1. vbx_enroll on synthetic archives of (M, E) = (1 000, 100), (16 000, 1 000) and (100 000, 1 000) speakers (4 per
-   recording, 1 .. 15 x-vectors each; enrolled speakers 1 .. 15 x-vectors each; R = 128): device time of every kernel
-   from torch.profiler over --rounds calls after one warm-up call, next to the pairs and bytes the score kernel needs.
-   The statistics row sums the span and statistics kernels of both speaker sets.
+1. enroll_speakers (vbx_enroll_batch) on synthetic archives of (M, E) = (1 000, 100), (16 000, 1 000) and
+   (100 000, 1 000) speakers (4 per recording, 1 .. 15 x-vectors each; enrolled speakers 1 .. 15 x-vectors each;
+   R = 128): device time of every kernel from torch.profiler over --rounds calls after one warm-up call, next to the
+   pairs and bytes the score kernel needs.  The statistics row sums the span and statistics kernels of both speaker sets
+   and the copy of the enrolled speaker index.
 2. Whole diarize_batch calls on the synthetic archive of tools/bench_sweep.py (17 recordings) without and with an
    enrolment of 10 speakers (20 x-vectors each), alternating in one process (medians, minima, maxima).
 The card's name, power limit and maximum SM clock are read in the same run.  Prints one JSON line; --out also writes it.
@@ -26,7 +27,7 @@ from bench_link import speakers  # noqa: E402
 from bench_sweep import GOLD, synthetic_archive  # noqa: E402
 from vbx_b200 import enroll, pipeline  # noqa: E402
 
-KERNELS = {'statistics': ('link_init_kernel', 'link_span_kernel', 'link_stats_kernel'),
+KERNELS = {'statistics': ('link_init_kernel', 'link_span_kernel', 'link_stats_kernel', 'repeat_index_kernel'),
            'score': ('enroll_score_kernel',), 'assignment': ('enroll_assign_kernel',)}
 
 

@@ -38,7 +38,7 @@ THRESHOLDS = [-20.0, -10.0, 0.0, 10.0, 20.0, 30.0, 40.0, 60.0]
 WORKED_T = [-40.0, -20.0, -10.0, 0.0, 10.0, 20.0, 40.0, 80.0]
 WORKED_GRID = dict(Fa=[0.1, 0.3, 0.5], Fb=[6.0, 17.0, 64.0], loopP=[0.99], threshold=[-0.015], smoothing=[5.0])
 KERNELS = ('link_init_kernel', 'link_span_kernel', 'link_stats_kernel', 'enroll_score_kernel', 'enroll_assign_kernel',
-           'enroll_assign_batch_kernel', 'repeat_index_kernel', 'norm_scores_kernel')
+           'repeat_index_kernel', 'norm_scores_kernel')
 
 
 def timed(fn):

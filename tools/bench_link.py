@@ -1,8 +1,9 @@
 """Times speaker linking across recordings (DESIGN.md section 5.15).
 
-1. vbx_link on synthetic archives of M = 1 000, 4 000 and 16 000 speakers (4 per recording, 1 .. 15 x-vectors each,
-   R = 128): device time of every kernel from torch.profiler (one warm-up call first), next to the bytes and operations
-   the statistics and score kernels need, computed from the shapes.  The linkage is one CTA doing M - 1 dependent merges.
+1. link_speakers (vbx_link_batch) on synthetic archives of M = 1 000, 4 000 and 16 000 speakers (4 per recording,
+   1 .. 15 x-vectors each, R = 128): device time of every kernel from torch.profiler (one warm-up call first), next to
+   the bytes and operations the statistics and score kernels need, computed from the shapes.  The linkage is one CTA
+   doing M - 1 dependent merges.
 2. Whole diarize_batch calls on the synthetic archive of tools/bench_sweep.py (17 recordings) without and with
    link_threshold, alternating in one process (medians, minima, maxima), and the time of each linking step inside
    linked calls (link_speakers, link_cut, linked_lines).

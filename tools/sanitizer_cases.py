@@ -87,7 +87,8 @@ torch.cuda.synchronize()
 kb.close()
 print('hard labels keep ok', int(fk.max()), float(mk.sum()))
 
-# speaker linking (vbx_link): recordings without x-vectors, a speaker with one x-vector, padded features, tile edges
+# speaker linking (link_speakers): recordings without x-vectors, a speaker with one x-vector, padded features, tile
+# edges
 from vbx_b200 import link  # noqa: E402
 gl = np.random.default_rng(3)
 l_lens = [0, 40, 1, 300, 0, 77]
@@ -107,8 +108,8 @@ for lb_max in (None, 80000):          # 80 000 bytes: the last problem needs 78 
     torch.cuda.synchronize()
     print('link batch ok', [len(o[0].rec) for o in lb_out], float(lb_out[2][3][:, 2].min()))
 
-# enrolment (vbx_enroll): recordings without speakers, E = 1 and E < K_b, a tail tile (M, E not multiples of 32), and a
-# recording with 150 speakers (more than 128)
+# enrolment (enroll_speakers): recordings without speakers, E = 1 and E < K_b, a tail tile (M, E not multiples of 32),
+# and a recording with 150 speakers (more than 128)
 from vbx_b200 import enroll  # noqa: E402
 e_lens = l_lens + [600]
 e_labels = l_labels + [np.concatenate([np.arange(150), gl.integers(0, 150, 450)])]
@@ -123,8 +124,8 @@ for E in (1, 7, 45):
     torch.cuda.synchronize()
     print('enroll ok', E, len(e_out.table.rec), int((e_out.assign >= 0).sum()))
 
-# score normalisation against a cohort (vbx_cohort_stats, vbx_link_norm, vbx_enroll_norm): C = 45 and M not multiples
-# of 32, top_k > C, a run forced into chunks, and the recording with 150 speakers
+# score normalisation against a cohort (cohort_stats, link_speakers and enroll_speakers with norm): C = 45 and M not
+# multiples of 32, top_k > C, a run forced into chunks, and the recording with 150 speakers
 from vbx_b200 import cohort  # noqa: E402
 c_x = torch.randn((100, 16), device=dev)
 c_x[:, 13:] = 0
@@ -139,7 +140,7 @@ c_enr = enroll.enroll_speakers(e_fea, l_phi, e_offs, e_labels, e_x, e_spk, 0.3, 
 torch.cuda.synchronize()
 print('cohort ok', len(c_st.mean), float(c_st.std.min()), float(c_link[3][:, 2].min()), int((c_enr.assign >= 0).sum()))
 
-# batched enrolment and cohort statistics (vbx_enroll_batch, vbx_cohort_stats_batch, vbx_link_batch_norm): a problem
+# batched enrolment and cohort statistics (enroll_many, cohort_stats_many, link_many with norm): a problem
 # without speakers, one with a speaker per recording and the one with 150 speakers, each with its own Fa / Fb; E = 45 <
 # K_b = 150 and tail tiles; three thresholds; plain and normalised
 eb_labels = [[np.full(n, -1) for n in e_lens], [np.where(np.arange(n) == 0, 0, -1) for n in e_lens], e_labels]

@@ -13,9 +13,7 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_set_option', 'vbx_plan', 'vbx_bind_workspace', 'vbx_prepare_scale',
            'vbx_prepare_project', 'vbx_prepare_xvectors', 'vbx_run', 'vbx_run_per_recording', 'vbx_hard_labels', 'vbx_hard_labels_keep', 'vbx_ahc_workspace_bytes', 'vbx_ahc', 'vbx_launch_count', 'vbx_get_timings', 'vbx_f64_workspace_bytes',
            'vbx_run_f64', 'vbx_plan_f64', 'vbx_forward_backward', 'vbx_attach_comm', 'vbx_elbo_trace', 'vbx_get_gsum',
-           'vbx_score', 'vbx_score_overlap', 'vbx_score_jer', 'vbx_link_workspace_bytes', 'vbx_link',
-           'vbx_enroll_workspace_bytes', 'vbx_enroll', 'vbx_cohort_workspace_bytes', 'vbx_cohort_stats', 'vbx_link_norm',
-           'vbx_enroll_norm', 'vbx_link_batch_workspace_bytes', 'vbx_link_batch', 'vbx_link_batch_norm',
+           'vbx_score', 'vbx_score_overlap', 'vbx_score_jer', 'vbx_link_batch_workspace_bytes', 'vbx_link_batch',
            'vbx_enroll_batch_workspace_bytes', 'vbx_enroll_batch', 'vbx_cohort_stats_batch_workspace_bytes',
            'vbx_cohort_stats_batch', 'vbx_init_turns', 'vbx_combine_workspace_bytes', 'vbx_combine',
            'vbx_init_random']
@@ -104,30 +102,11 @@ def load():
     lib.vbx_score_jer.restype = ctypes.c_int
     lib.vbx_score_jer.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp,
                                   vp, vp, vp, vp]
-    lib.vbx_link_workspace_bytes.restype = ctypes.c_int
-    lib.vbx_link_workspace_bytes.argtypes = [vp, i64, ctypes.POINTER(ctypes.c_size_t)]
-    lib.vbx_link.restype = ctypes.c_int
-    lib.vbx_link.argtypes = [vp, vp, vp, i64, i32, vp, i64, vp, dbl, dbl, vp, ctypes.c_size_t, vp, vp, vp, vp, vp]
-    lib.vbx_enroll_workspace_bytes.restype = ctypes.c_int
-    lib.vbx_enroll_workspace_bytes.argtypes = [vp, i64, i64, i64, ctypes.POINTER(ctypes.c_size_t)]
-    lib.vbx_enroll.restype = ctypes.c_int
-    lib.vbx_enroll.argtypes = [vp, vp, vp, i64, i32, vp, i64, vp, i32, vp, i64, vp, i64, dbl, dbl, dbl, vp,
-                               ctypes.c_size_t, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.vbx_cohort_workspace_bytes.restype = ctypes.c_int
-    lib.vbx_cohort_workspace_bytes.argtypes = [vp, i64, i64, ctypes.POINTER(ctypes.c_size_t)]
-    lib.vbx_cohort_stats.restype = ctypes.c_int
-    lib.vbx_cohort_stats.argtypes = [vp, vp, vp, i64, i32, vp, i64, vp, i64, vp, i64, dbl, dbl, i32, vp, ctypes.c_size_t,
-                                     vp, vp, vp, vp]
-    lib.vbx_link_norm.restype = ctypes.c_int
-    lib.vbx_link_norm.argtypes = lib.vbx_link.argtypes[:-1] + [vp, vp, vp]
-    lib.vbx_enroll_norm.restype = ctypes.c_int
-    lib.vbx_enroll_norm.argtypes = lib.vbx_enroll.argtypes[:-1] + [vp, vp, vp, vp, vp]
     lib.vbx_link_batch_workspace_bytes.restype = ctypes.c_int
     lib.vbx_link_batch_workspace_bytes.argtypes = [vp, i32, vp, ctypes.POINTER(ctypes.c_size_t)]
     lib.vbx_link_batch.restype = ctypes.c_int
-    lib.vbx_link_batch.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.c_size_t, vp, vp, vp, vp, vp]
-    lib.vbx_link_batch_norm.restype = ctypes.c_int
-    lib.vbx_link_batch_norm.argtypes = lib.vbx_link_batch.argtypes[:-1] + [vp, vp, vp]
+    lib.vbx_link_batch.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, vp, vp, vp, ctypes.c_size_t, vp, vp, vp, vp, vp,
+                                   vp, vp]
     lib.vbx_enroll_batch_workspace_bytes.restype = ctypes.c_int
     lib.vbx_enroll_batch_workspace_bytes.argtypes = [vp, i32, vp, i64, i64, i64, i32, ctypes.POINTER(ctypes.c_size_t)]
     lib.vbx_enroll_batch.restype = ctypes.c_int
@@ -137,7 +116,7 @@ def load():
     lib.vbx_cohort_stats_batch_workspace_bytes.argtypes = [vp, i32, vp, i64, i64, ctypes.POINTER(ctypes.c_size_t)]
     lib.vbx_cohort_stats_batch.restype = ctypes.c_int
     lib.vbx_cohort_stats_batch.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp, i64, vp, i64, vp, vp, i32, vp,
-                                           ctypes.c_size_t, vp, vp, vp]
+                                           ctypes.c_size_t, vp, vp, vp, vp]
     lib.vbx_init_turns.restype = ctypes.c_int
     lib.vbx_init_turns.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp]
     lib.vbx_init_random.restype = ctypes.c_int

@@ -4,7 +4,8 @@ The same-speaker LLR of section 5.15 is not calibrated: it grows with the number
 offset from the PLDA mean, so one threshold means different things for different speakers and archives.  Adaptive
 symmetric normalisation (AS-norm) standardises every score by the scores of both speakers against a cohort of speakers
 known to be someone else: speaker x scores LLR(x, c) against each cohort speaker c, mu_x and sigma_x are the mean and
-population standard deviation of its K = min(top_k, C) largest cohort scores (on the device, vbx_cohort_stats), and
+population standard deviation of its K = min(top_k, C) largest cohort scores (on the device, vbx_cohort_stats_batch),
+and
 
     S(x, y) = 1/2 [ (LLR(x, y) - mu_x) / sigma_x + (LLR(x, y) - mu_y) / sigma_y ].
 
@@ -58,20 +59,8 @@ def check_spread(std, names):
                          f'speaker(s): {shown}')
 
 
-def cohort_stats(fea, Phi, offsets, labels, cohort_fea, cohort_speaker, Fa, Fb, top_k=DEFAULT_TOP_K, device=None,
-                 max_bytes=2 ** 31, scores=False):
-    """mu and sigma of every scored speaker's top_k cohort scores on the device (vbx_cohort_stats).  fea [N,R], Phi [R]:
-    the features the VB-HMM ran with.  Scored speakers: with offsets [B+1], labels holds each recording's first labels
-    and the speakers are link.speaker_table's; with offsets None, labels is a speaker index [N] in [0, M) (-1: none),
-    every speaker with at least one x-vector.  cohort_fea [N_c,R]: the cohort x-vectors through the same front end;
-    cohort_speaker [N_c]: their speaker in [0, C), C >= 2, every one with an x-vector.  Speakers whose M x C score block
-    exceeds max_bytes are split into chunks, one call each (the same bits).  Returns CohortStats (numpy), with the
-    scores [M,C] when scores=True."""
-    import torch
-    from . import _lib
-    from ._lib import VbxError
-    from .link import speaker_index
-    K_req = check_top_k(top_k)
+def _cohort_speakers(cohort_speaker):
+    """(cspk [N_c] int64, C) checked: at least two cohort speakers, each with an x-vector."""
     cspk = np.asarray(cohort_speaker, dtype=np.int64).reshape(-1)
     if len(cspk) == 0 or cspk.min() < 0:
         raise ValueError('cohort_speaker must hold at least one speaker index, all >= 0')
@@ -80,101 +69,70 @@ def cohort_stats(fea, Phi, offsets, labels, cohort_fea, cohort_speaker, Fa, Fb, 
         raise ValueError(f'a cohort needs at least 2 speakers, got {C}')
     if np.bincount(cspk, minlength=C).min() == 0:
         raise ValueError('every cohort speaker 0 .. C-1 needs at least one x-vector')
-    if offsets is None:
-        spk = np.asarray(labels, dtype=np.int64).reshape(-1)
-        M = int(spk.max()) + 1 if len(spk) else 0
-        if M and np.bincount(spk[spk >= 0], minlength=M).min() == 0:
-            raise ValueError('every scored speaker 0 .. M-1 needs at least one x-vector')
-    else:
-        spk, M = speaker_index(offsets, labels)
-    if not torch.cuda.is_available():
-        raise VbxError('cohort_stats(): no CUDA device - vbx_b200 has no CPU fallback')
-    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
-    if dev.index is None:
-        dev = torch.device('cuda', torch.cuda.current_device())
-    fea = torch.as_tensor(fea).to(dev, torch.float32).contiguous()
-    Phi = torch.as_tensor(Phi).to(dev, torch.float32).contiguous()
-    cfea = torch.as_tensor(cohort_fea).to(dev, torch.float32).contiguous()
-    N, R = int(fea.shape[0]), int(fea.shape[1])
+    return cspk, C
+
+
+def _scored_speakers(offsets, labels):
+    """(speaker [N] int64, M) of the scored speakers as cohort_stats takes them (see there)."""
+    from .link import speaker_index
+    if offsets is not None:
+        return speaker_index(offsets, labels)
+    spk = np.asarray(labels, dtype=np.int64).reshape(-1)
+    M = int(spk.max()) + 1 if len(spk) else 0
+    if M and np.bincount(spk[spk >= 0], minlength=M).min() == 0:
+        raise ValueError('every scored speaker 0 .. M-1 needs at least one x-vector')
+    return spk, M
+
+
+def cohort_stats(fea, Phi, offsets, labels, cohort_fea, cohort_speaker, Fa, Fb, top_k=DEFAULT_TOP_K, device=None,
+                 max_bytes=2 ** 31, scores=False):
+    """mu and sigma of every scored speaker's top_k cohort scores on the device (vbx_cohort_stats_batch on a batch of
+    one).  fea [N,R], Phi [R]: the features the VB-HMM ran with.  Scored speakers: with offsets [B+1], labels holds each
+    recording's first labels and the speakers are link.speaker_table's; with offsets None, labels is a speaker index [N]
+    in [0, M) (-1: none), every speaker with at least one x-vector.  cohort_fea [N_c,R]: the cohort x-vectors through
+    the same front end; cohort_speaker [N_c]: their speaker in [0, C), C >= 2, every one with an x-vector.  Speakers
+    whose M x C score block exceeds max_bytes are split into chunks of consecutive speakers, one cohort_stats_many call
+    each (the same bits).  Returns CohortStats (numpy), with the scores [M,C] when scores=True."""
+    K_req = check_top_k(top_k)
+    C = _cohort_speakers(cohort_speaker)[1]
+    spk, M = _scored_speakers(offsets, labels)
+    N = int(fea.shape[0])
     if len(spk) != N:
         raise ValueError(f'{len(spk)} speaker indices for {N} x-vectors')
-    if tuple(cfea.shape) != (len(cspk), R):
-        raise ValueError(f'cohort_fea must be [{len(cspk)}, {R}], got {tuple(cfea.shape)}')
     # chunks of consecutive speakers with at most max_bytes of scores (one speaker alone may exceed it)
     per = max(1, int(max_bytes) // (8 * C))
-    chunks = [(s0, min(s0 + per, M)) for s0 in range(0, M, per)]
-    lib = _lib.load()
-    h = ctypes.c_void_p()
-    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
-        raise VbxError('vbx_create failed: no usable sm_90 device')
-    at = lambda x, off=0: ctypes.c_void_p(x.data_ptr() + off * x.element_size()) if x is not None else None
-    try:
-        need = ctypes.c_size_t()
-        m_max = max((b - a for a, b in chunks), default=0)
-        if lib.vbx_cohort_workspace_bytes(h, m_max, C, ctypes.byref(need)) != 0:
-            raise VbxError(f'vbx_cohort_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
-        with torch.cuda.device(dev):
-            ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=dev)
-            cspk_d = torch.from_numpy(cspk.astype(np.int32)).to(dev)
-            mean = torch.empty(M, dtype=torch.float64, device=dev)
-            std = torch.empty(M, dtype=torch.float64, device=dev)
-            L = torch.empty((M, C), dtype=torch.float64, device=dev) if scores else None
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            keep = []
-            for s0, s1 in chunks:
-                mine = np.nonzero((spk >= s0) & (spk < s1))[0]
-                x0, x1 = int(mine[0]), int(mine[-1]) + 1        # every speaker has an x-vector
-                sp = spk[x0:x1]
-                spk_d = torch.from_numpy(np.where((sp >= s0) & (sp < s1), sp - s0, -1).astype(np.int32)).to(dev)
-                keep.append(spk_d)
-                rc = lib.vbx_cohort_stats(h, at(fea, x0 * R), at(Phi), x1 - x0, R, at(spk_d), s1 - s0, at(cfea),
-                                          len(cspk), at(cspk_d), C, float(Fa), float(Fb), K_req, at(ws), ws.numel(),
-                                          at(mean, s0), at(std, s0), at(L, s0 * C), stream)
-                if rc != 0:
-                    raise VbxError(f'vbx_cohort_stats failed ({rc}): {lib.vbx_last_error(h).decode()}')
-            out = CohortStats(mean.cpu().numpy(), std.cpu().numpy(), min(K_req, C),
-                              L.cpu().numpy() if scores else None)
-    finally:
-        lib.vbx_destroy(h)
-    return out
+    parts = []
+    for s0 in range(0, M, per) if M else [0]:
+        s1 = min(s0 + per, M)
+        x0, x1 = 0, N
+        if M:
+            mine = np.nonzero((spk >= s0) & (spk < s1))[0]
+            x0, x1 = int(mine[0]), int(mine[-1]) + 1    # every speaker has an x-vector
+        sp = spk[x0:x1]
+        parts += cohort_stats_many(fea[x0:x1], Phi, None, [np.where((sp >= s0) & (sp < s1), sp - s0, -1)],
+                                   cohort_fea, cohort_speaker, Fa, Fb, top_k=K_req, device=device, scores=scores)
+    return CohortStats(np.concatenate([c.mean for c in parts]), np.concatenate([c.std for c in parts]), min(K_req, C),
+                       np.concatenate([c.scores for c in parts]) if scores else None)
 
 
 def cohort_stats_many(fea, Phi, offsets, labels_per_problem, cohort_fea, cohort_speaker, Fa, Fb, top_k=DEFAULT_TOP_K,
-                      device=None, max_bytes=None):
+                      device=None, max_bytes=None, scores=False):
     """cohort_stats for G independent problems over the same features and cohort in few launches
     (vbx_cohort_stats_batch, DESIGN.md section 5.19), e.g. the final labels of every setting of a sweep.  fea, Phi,
     offsets, cohort_fea, cohort_speaker, top_k: as for cohort_stats; labels_per_problem: G label sets as cohort_stats
     takes them (per recording first labels with offsets, or a speaker index [N] with offsets None); Fa, Fb: numbers or
     G values.  The enrolled speakers of every setting: fea = the enrolled features, offsets None and their speaker index
-    once per setting.  Launches as enroll_many packs them (max_bytes None: one).  Returns one CohortStats per problem
-    (scores None), bit-identical to cohort_stats on that problem alone."""
+    once per setting.  Launches as enroll_many packs them (max_bytes None: one).  Returns one CohortStats per problem,
+    with its scores [M_g,C] when scores=True, bit-identical to cohort_stats on that problem alone."""
     import torch
     from . import _lib
     from ._lib import VbxError
-    from .link import speaker_index
     from .sweep import pack_by
     K_req = check_top_k(top_k)
     G = len(labels_per_problem)
     Fa, Fb = (np.broadcast_to(np.asarray(v, dtype=np.float64), (G,)).copy() for v in (Fa, Fb))
-    cspk = np.asarray(cohort_speaker, dtype=np.int64).reshape(-1)
-    if len(cspk) == 0 or cspk.min() < 0:
-        raise ValueError('cohort_speaker must hold at least one speaker index, all >= 0')
-    C = int(cspk.max()) + 1
-    if C < 2:
-        raise ValueError(f'a cohort needs at least 2 speakers, got {C}')
-    if np.bincount(cspk, minlength=C).min() == 0:
-        raise ValueError('every cohort speaker 0 .. C-1 needs at least one x-vector')
-    spks, Ms = [], []
-    for labels in labels_per_problem:
-        if offsets is None:
-            spk = np.asarray(labels, dtype=np.int64).reshape(-1)
-            M = int(spk.max()) + 1 if len(spk) else 0
-            if M and np.bincount(spk[spk >= 0], minlength=M).min() == 0:
-                raise ValueError('every scored speaker 0 .. M-1 needs at least one x-vector')
-        else:
-            spk, M = speaker_index(offsets, labels)
-        spks.append(spk)
-        Ms.append(M)
+    cspk, C = _cohort_speakers(cohort_speaker)
+    spks, Ms = zip(*[_scored_speakers(offsets, labels) for labels in labels_per_problem]) if G else ((), ())
     Ms = np.array(Ms, dtype=np.int64)
     if not torch.cuda.is_available():
         raise VbxError('cohort_stats_many(): no CUDA device - vbx_b200 has no CPU fallback')
@@ -216,15 +174,17 @@ def cohort_stats_many(fea, Phi, offsets, labels_per_problem, cohort_fea, cohort_
                 fa, fb = np.ascontiguousarray(Fa[idx]), np.ascontiguousarray(Fb[idx])
                 mean = torch.empty(tot, dtype=torch.float64, device=dev)
                 std = torch.empty(tot, dtype=torch.float64, device=dev)
+                L = torch.empty((tot, C), dtype=torch.float64, device=dev) if scores else None
                 rc = lib.vbx_cohort_stats_batch(h, p(fea), p(Phi), N, R, len(idx), p(spk_d), v(M_h), p(cfea),
                                                 len(cspk), p(cspk_d), C, v(fa), v(fb), K_req, p(ws), ws.numel(),
-                                                p(mean), p(std), stream)
+                                                p(mean), p(std), p(L), stream)
                 if rc != 0:
                     raise VbxError(f'vbx_cohort_stats_batch failed ({rc}): {lib.vbx_last_error(h).decode()}')
                 mean, std = mean.cpu().numpy(), std.cpu().numpy()
+                L = L.cpu().numpy() if scores else None
                 o = 0
                 for g, M in zip(idx, M_h.tolist()):
-                    out[g] = CohortStats(mean[o:o + M], std[o:o + M], min(K_req, C), None)
+                    out[g] = CohortStats(mean[o:o + M], std[o:o + M], min(K_req, C), L[o:o + M] if scores else None)
                     o += M
     finally:
         lib.vbx_destroy(h)

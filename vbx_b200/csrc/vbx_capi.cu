@@ -183,7 +183,7 @@ size_t carve(const vbx::Plan &pl, void *base, vbx::Workspace *ws) {
 
 extern "C" {
 
-const char *vbx_version(void) { return "vbx_b200 0.1 (sm_90a)"; }
+const char *vbx_version(void) { return "vbx_b200 0.2 (sm_90a)"; }
 
 int32_t vbx_padded_states(int32_t n) {
     if (n < 1 || n > vbx::kMaxS) return -1;
@@ -885,55 +885,6 @@ int vbx_ahc(vbx_handle_t h, const void *x, int32_t x_is_f64, int32_t dim, void *
     return VBX_OK;
 }
 
-int vbx_link_workspace_bytes(vbx_handle_t h, int64_t M, size_t *bytes_out) {
-    if (!h || !bytes_out) return VBX_ERR_ARG;
-    if (M < 0 || M > VBX_LINK_MAX_SPEAKERS)
-        return fail(h, VBX_ERR_ARG, "vbx_link_workspace_bytes: M must lie in [0, VBX_LINK_MAX_SPEAKERS]");
-    *bytes_out = vbx::link_workspace_bytes(M);
-    return VBX_OK;
-}
-
-// vbx_link and vbx_link_norm (mean, std null for the former)
-static int link_call(vbx_handle_t h, const char *name, const float *fea, const float *Phi, int64_t N, int32_t R,
-                     const int32_t *speaker, int64_t M, const int32_t *speaker_rec, double Fa, double Fb,
-                     void *workspace, size_t workspace_bytes, double *n_out, double *F_out, double *dist_out,
-                     double *Z_out, const double *mean, const double *std, void *stream) {
-    if (!h) return VBX_ERR_ARG;
-    Range nvtx_range(name);
-    const std::string who(name);
-    if (N < 0 || M < 0 || M > VBX_LINK_MAX_SPEAKERS)
-        return fail(h, VBX_ERR_ARG, who + ": need N >= 0 and 0 <= M <= VBX_LINK_MAX_SPEAKERS");
-    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, who + ": R must lie in [1, 128]");
-    const double c = Fa / Fb;
-    if (!(c >= 0.0) || c == INFINITY) return fail(h, VBX_ERR_ARG, who + ": Fa / Fb must be finite and >= 0");
-    if (M == 0) return VBX_OK;
-    if (!Phi || !speaker_rec || !workspace || (N > 0 && (!fea || !speaker)) || (M >= 2 && !Z_out))
-        return fail(h, VBX_ERR_ARG, who + ": null pointer");
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
-    if (workspace_bytes < vbx::link_workspace_bytes(M))
-        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_link_workspace_bytes()");
-    DeviceGuard guard(h->device);
-    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
-    return counted(h, vbx::launch_link(fea, Phi, speaker, N, R, speaker_rec, M, c, workspace, n_out, F_out, dist_out,
-                                       Z_out, (cudaStream_t)stream, mean, std), "link");
-}
-
-int vbx_link(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-             int64_t M, const int32_t *speaker_rec, double Fa, double Fb, void *workspace, size_t workspace_bytes,
-             double *n_out, double *F_out, double *dist_out, double *Z_out, void *stream) {
-    return link_call(h, "vbx_link", fea, Phi, N, R, speaker, M, speaker_rec, Fa, Fb, workspace, workspace_bytes, n_out,
-                     F_out, dist_out, Z_out, nullptr, nullptr, stream);
-}
-
-int vbx_link_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-                  int64_t M, const int32_t *speaker_rec, double Fa, double Fb, void *workspace, size_t workspace_bytes,
-                  double *n_out, double *F_out, double *dist_out, double *Z_out, const double *mean, const double *std,
-                  void *stream) {
-    if (h && M > 0 && (!mean || !std)) return fail(h, VBX_ERR_ARG, "vbx_link_norm: null pointer");
-    return link_call(h, "vbx_link_norm", fea, Phi, N, R, speaker, M, speaker_rec, Fa, Fb, workspace, workspace_bytes,
-                     n_out, F_out, dist_out, Z_out, mean, std, stream);
-}
-
 // the sizes M [G] of vbx_link_batch's problems: each in [0, VBX_LINK_MAX_SPEAKERS], their sum within one launch's grid
 static int check_problem_sizes(vbx_handle_t h, const std::string &who, int32_t G, const int64_t *M) {
     if (G < 0) return fail(h, VBX_ERR_ARG, who + ": G < 0");
@@ -970,15 +921,13 @@ static int problem_scalars(vbx_handle_t h, const std::string &who, int32_t G, co
     return VBX_OK;
 }
 
-// vbx_link_batch and vbx_link_batch_norm (mean, std null for the former)
-static int link_batch_call(vbx_handle_t h, const char *name, const float *fea, const float *Phi, int64_t N, int32_t R,
-                           int32_t G, const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec,
-                           const double *Fa, const double *Fb, void *workspace, size_t workspace_bytes, double *n_out,
-                           double *F_out, double *dist_out, double *Z_out, const double *mean, const double *std,
-                           void *stream) {
+int vbx_link_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
+                   const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
+                   const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
+                   double *dist_out, double *Z_out, const double *mean, const double *std, void *stream) {
     if (!h) return VBX_ERR_ARG;
-    Range nvtx_range(name);
-    const std::string who(name);
+    Range nvtx_range("vbx_link_batch");
+    const std::string who("vbx_link_batch");
     int rc = check_problem_sizes(h, who, G, M);
     if (rc != VBX_OK) return rc;
     if (N < 0) return fail(h, VBX_ERR_ARG, who + ": N < 0");
@@ -986,6 +935,7 @@ static int link_batch_call(vbx_handle_t h, const char *name, const float *fea, c
     std::vector<double> c;
     rc = problem_scalars(h, who, G, Fa, Fb, &c);
     if (rc != VBX_OK) return rc;
+    if (!mean != !std) return fail(h, VBX_ERR_ARG, who + ": give both of mean and std, or neither");
     int64_t total = 0, largest = 0;
     for (int32_t g = 0; g < G; ++g) {
         total += M[g];
@@ -1001,27 +951,6 @@ static int link_batch_call(vbx_handle_t h, const char *name, const float *fea, c
     if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     return counted(h, vbx::launch_link_batch(fea, Phi, speaker, N, R, speaker_rec, G, M, c.data(), workspace, n_out,
                                              F_out, dist_out, Z_out, (cudaStream_t)stream, mean, std), "link_batch");
-}
-
-int vbx_link_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
-                   const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
-                   const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
-                   double *dist_out, double *Z_out, void *stream) {
-    return link_batch_call(h, "vbx_link_batch", fea, Phi, N, R, G, speaker, M, speaker_rec, Fa, Fb, workspace,
-                           workspace_bytes, n_out, F_out, dist_out, Z_out, nullptr, nullptr, stream);
-}
-
-int vbx_link_batch_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
-                        const int32_t *speaker, const int64_t *M, const int32_t *speaker_rec, const double *Fa,
-                        const double *Fb, void *workspace, size_t workspace_bytes, double *n_out, double *F_out,
-                        double *dist_out, double *Z_out, const double *mean, const double *std, void *stream) {
-    if (h && (!mean || !std)) {
-        int64_t total = 0;
-        for (int32_t g = 0; M && g < G; ++g) total += M[g];
-        if (total > 0) return fail(h, VBX_ERR_ARG, "vbx_link_batch_norm: null pointer");
-    }
-    return link_batch_call(h, "vbx_link_batch_norm", fea, Phi, N, R, G, speaker, M, speaker_rec, Fa, Fb, workspace,
-                           workspace_bytes, n_out, F_out, dist_out, Z_out, mean, std, stream);
 }
 
 int vbx_enroll_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int64_t *M, int64_t E, int64_t N_e,
@@ -1058,11 +987,11 @@ int vbx_enroll_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t
     for (int32_t k = 0; k < n_thr; ++k)
         if (!(std::fabs(thresholds[k]) <= 1e15))
             return fail(h, VBX_ERR_ARG, who + ": |thresholds[" + std::to_string(k) + "]| must be <= 1e15");
-    const bool norm = mean || std || enroll_mean || enroll_std;
-    if (norm && !(mean && std && enroll_mean && enroll_std))
-        return fail(h, VBX_ERR_ARG, who + ": give all four of mean, std, enroll_mean and enroll_std, or none");
     int64_t total = 0;
     for (int32_t g = 0; g < G; ++g) total += M[g];
+    const bool norm = mean || std || enroll_mean || enroll_std;
+    if (norm && !(enroll_mean && enroll_std && ((mean && std) || total == 0)))
+        return fail(h, VBX_ERR_ARG, who + ": give all four of mean, std, enroll_mean and enroll_std, or none");
     if (!Phi || !workspace || !enroll_fea || !enroll_speaker || (G > 0 && !speaker_rec_offsets) ||
         (N > 0 && (!fea || !speaker)) || (total > 0 && (!assign_out || !best_llr_out)))
         return fail(h, VBX_ERR_ARG, who + ": null pointer");
@@ -1106,7 +1035,8 @@ int vbx_cohort_stats_batch_workspace_bytes(vbx_handle_t h, int32_t G, const int6
 int vbx_cohort_stats_batch(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, int32_t G,
                            const int32_t *speaker, const int64_t *M, const float *cohort_fea, int64_t N_c,
                            const int32_t *cohort_speaker, int64_t C, const double *Fa, const double *Fb, int32_t top_k,
-                           void *workspace, size_t workspace_bytes, double *mean_out, double *std_out, void *stream) {
+                           void *workspace, size_t workspace_bytes, double *mean_out, double *std_out,
+                           double *scores_out, void *stream) {
     if (!h) return VBX_ERR_ARG;
     Range nvtx_range("vbx_cohort_stats_batch");
     const std::string who("vbx_cohort_stats_batch");
@@ -1130,114 +1060,9 @@ int vbx_cohort_stats_batch(vbx_handle_t h, const float *fea, const float *Phi, i
     DeviceGuard guard(h->device);
     if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     return counted(h, vbx::launch_cohort_batch(fea, Phi, N, R, speaker, G, M, cohort_fea, N_c, cohort_speaker, C,
-                                               c.data(), top_k, workspace, mean_out, std_out, (cudaStream_t)stream),
+                                               c.data(), top_k, workspace, mean_out, std_out, scores_out,
+                                               (cudaStream_t)stream),
                    "cohort_batch");
-}
-
-int vbx_enroll_workspace_bytes(vbx_handle_t h, int64_t M, int64_t E, int64_t max_k, size_t *bytes_out) {
-    if (!h || !bytes_out) return VBX_ERR_ARG;
-    if (M < 0 || E < 1 || max_k < 0 || max_k > M)
-        return fail(h, VBX_ERR_ARG, "vbx_enroll_workspace_bytes: need M >= 0, E >= 1 and 0 <= max_k <= M");
-    *bytes_out = vbx::enroll_workspace_bytes(M, E, max_k, h->sms);
-    return VBX_OK;
-}
-
-// vbx_enroll and vbx_enroll_norm (the four statistics arrays null for the former)
-static int enroll_call(vbx_handle_t h, const char *name, const float *fea, const float *Phi, int64_t N, int32_t R,
-                       const int32_t *speaker, int64_t M, const int64_t *speaker_rec_offsets, int32_t n_rec,
-                       const float *enroll_fea, int64_t N_e, const int32_t *enroll_speaker, int64_t E, double Fa,
-                       double Fb, double threshold, void *workspace, size_t workspace_bytes, int32_t *assign_out,
-                       double *best_llr_out, double *llr_out, double *n_out, double *F_out, double *n_enroll_out,
-                       double *F_enroll_out, const double *mean, const double *std, const double *enroll_mean,
-                       const double *enroll_std, void *stream) {
-    if (!h) return VBX_ERR_ARG;
-    Range nvtx_range(name);
-    const std::string who(name);
-    if (N < 0 || M < 0 || n_rec < 0 || N_e < 1 || E < 1)
-        return fail(h, VBX_ERR_ARG, who + ": need N, M, n_rec >= 0 and N_e, E >= 1");
-    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, who + ": R must lie in [1, 128]");
-    const double c = Fa / Fb;
-    if (!(c >= 0.0) || c == INFINITY) return fail(h, VBX_ERR_ARG, who + ": Fa / Fb must be finite and >= 0");
-    if (!(std::fabs(threshold) <= 1e15)) return fail(h, VBX_ERR_ARG, who + ": |threshold| must be <= 1e15");
-    if (!Phi || !workspace || !speaker_rec_offsets || !enroll_fea || !enroll_speaker || (N > 0 && (!fea || !speaker)) ||
-        (M > 0 && (!assign_out || !best_llr_out)))
-        return fail(h, VBX_ERR_ARG, who + ": null pointer");
-    if (speaker_rec_offsets[0] != 0 || speaker_rec_offsets[n_rec] != M)
-        return fail(h, VBX_ERR_ARG, who + ": speaker_rec_offsets must run from 0 to M");
-    int64_t max_k = 0;
-    for (int32_t b = 0; b < n_rec; ++b) {
-        const int64_t k = speaker_rec_offsets[b + 1] - speaker_rec_offsets[b];
-        if (k < 0) return fail(h, VBX_ERR_ARG, who + ": speakers are not packed by recording (offsets decrease)");
-        max_k = std::max(max_k, k);
-    }
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
-        return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
-    if (workspace_bytes < vbx::enroll_workspace_bytes(M, E, max_k, h->sms))
-        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_enroll_workspace_bytes()");
-    DeviceGuard guard(h->device);
-    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
-    return counted(h, vbx::launch_enroll(fea, Phi, N, R, speaker, M, speaker_rec_offsets, n_rec, enroll_fea, N_e,
-                                         enroll_speaker, E, c, threshold, workspace, h->sms, assign_out, best_llr_out,
-                                         llr_out, n_out, F_out, n_enroll_out, F_enroll_out, (cudaStream_t)stream, mean,
-                                         std, enroll_mean, enroll_std),
-                   "enroll");
-}
-
-int vbx_enroll(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-               int64_t M, const int64_t *speaker_rec_offsets, int32_t n_rec, const float *enroll_fea, int64_t N_e,
-               const int32_t *enroll_speaker, int64_t E, double Fa, double Fb, double threshold, void *workspace,
-               size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
-               double *F_out, double *n_enroll_out, double *F_enroll_out, void *stream) {
-    return enroll_call(h, "vbx_enroll", fea, Phi, N, R, speaker, M, speaker_rec_offsets, n_rec, enroll_fea, N_e,
-                       enroll_speaker, E, Fa, Fb, threshold, workspace, workspace_bytes, assign_out, best_llr_out,
-                       llr_out, n_out, F_out, n_enroll_out, F_enroll_out, nullptr, nullptr, nullptr, nullptr, stream);
-}
-
-int vbx_enroll_norm(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-                    int64_t M, const int64_t *speaker_rec_offsets, int32_t n_rec, const float *enroll_fea, int64_t N_e,
-                    const int32_t *enroll_speaker, int64_t E, double Fa, double Fb, double threshold, void *workspace,
-                    size_t workspace_bytes, int32_t *assign_out, double *best_llr_out, double *llr_out, double *n_out,
-                    double *F_out, double *n_enroll_out, double *F_enroll_out, const double *mean, const double *std,
-                    const double *enroll_mean, const double *enroll_std, void *stream) {
-    if (h && (!enroll_mean || !enroll_std || (M > 0 && (!mean || !std))))
-        return fail(h, VBX_ERR_ARG, "vbx_enroll_norm: null pointer");
-    return enroll_call(h, "vbx_enroll_norm", fea, Phi, N, R, speaker, M, speaker_rec_offsets, n_rec, enroll_fea, N_e,
-                       enroll_speaker, E, Fa, Fb, threshold, workspace, workspace_bytes, assign_out, best_llr_out,
-                       llr_out, n_out, F_out, n_enroll_out, F_enroll_out, mean, std, enroll_mean, enroll_std, stream);
-}
-
-int vbx_cohort_workspace_bytes(vbx_handle_t h, int64_t M, int64_t C, size_t *bytes_out) {
-    if (!h || !bytes_out) return VBX_ERR_ARG;
-    if (M < 0 || M > INT32_MAX || C < 2)
-        return fail(h, VBX_ERR_ARG, "vbx_cohort_workspace_bytes: need 0 <= M <= 2^31 - 1 and C >= 2");
-    *bytes_out = vbx::cohort_workspace_bytes(M, C);
-    return VBX_OK;
-}
-
-int vbx_cohort_stats(vbx_handle_t h, const float *fea, const float *Phi, int64_t N, int32_t R, const int32_t *speaker,
-                     int64_t M, const float *cohort_fea, int64_t N_c, const int32_t *cohort_speaker, int64_t C,
-                     double Fa, double Fb, int32_t top_k, void *workspace, size_t workspace_bytes, double *mean_out,
-                     double *std_out, double *scores_out, void *stream) {
-    if (!h) return VBX_ERR_ARG;
-    Range nvtx_range("vbx_cohort_stats");
-    if (N < 0 || M < 0 || M > INT32_MAX || N_c < 1 || C < 2)
-        return fail(h, VBX_ERR_ARG, "vbx_cohort_stats: need N >= 0, 0 <= M <= 2^31 - 1, N_c >= 1 and C >= 2");
-    if (top_k < 2) return fail(h, VBX_ERR_ARG, "vbx_cohort_stats: top_k must be >= 2");
-    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, "vbx_cohort_stats: R must lie in [1, 128]");
-    const double c = Fa / Fb;
-    if (!(c >= 0.0) || c == INFINITY) return fail(h, VBX_ERR_ARG, "vbx_cohort_stats: Fa / Fb must be finite and >= 0");
-    if (M == 0) return VBX_OK;
-    if (!Phi || !workspace || !cohort_fea || !cohort_speaker || !mean_out || !std_out || (N > 0 && (!fea || !speaker)))
-        return fail(h, VBX_ERR_ARG, "vbx_cohort_stats: null pointer");
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
-        return fail(h, VBX_ERR_ARG, "vbx_cohort_stats: workspace must be 256-byte aligned");
-    if (workspace_bytes < vbx::cohort_workspace_bytes(M, C))
-        return fail(h, VBX_ERR_ARG, "vbx_cohort_stats: workspace smaller than vbx_cohort_workspace_bytes()");
-    DeviceGuard guard(h->device);
-    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
-    return counted(h, vbx::launch_cohort(fea, Phi, N, R, speaker, M, cohort_fea, N_c, cohort_speaker, C, c, top_k,
-                                         workspace, mean_out, std_out, scores_out, (cudaStream_t)stream),
-                   "cohort");
 }
 
 int vbx_f64_workspace_bytes(vbx_handle_t h, size_t *bytes_out) {

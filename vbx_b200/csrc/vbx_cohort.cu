@@ -1,15 +1,17 @@
 // Adaptive symmetric score normalisation against a cohort (DESIGN.md section 5.17).  Every scored speaker x (archive or
 // enrolled speakers, with section 5.15's statistics) is scored against the C cohort speakers with section 5.15's LLR,
-// and mu_x, sigma_x are the mean and population standard deviation of its K = min(top_k, C) largest cohort scores:
-//   enroll_score_kernel  (vbx_enroll.cu, through launch_cohort_scores) the [M, C] cohort LLRs, unchanged
-//   cohort_topk_kernel   one CTA per speaker: the K-th largest score by a radix select on order-preserving 64-bit
-//                        keys (8 passes of 8 bits, histograms in shared memory), then mu and sigma by fixed-order sums
+// and mu_x, sigma_x are the mean and population standard deviation of its K = min(top_k, C) largest cohort scores.
+// vbx_cohort_stats_batch (section 5.19) runs G problems against one cohort, each with its c_g (one set of scored
+// speakers is the batch of one): the statistics of the scored speakers of all problems and of the cohort once per
+// problem, then
+//   enroll_score_kernel  (vbx_enroll.cu, through launch_cohort_scores_batch) the [sum M, C] cohort LLRs of every
+//                        problem's rectangle in one launch, unchanged
+//   cohort_topk_kernel   one CTA per speaker of all problems: the K-th largest score by a radix select on
+//                        order-preserving 64-bit keys (8 passes of 8 bits, histograms in shared memory), then mu and
+//                        sigma by fixed-order sums (a row's result depends on the row and C alone)
 //   norm_scores_kernel   S(x, y) = 1/2 [ (LLR - mu_x) / sigma_x + (LLR - mu_y) / sigma_y ] in place over the link
-//                        distances (d = -S; the diagonal and the cannot-link entries untouched) or the enrolment LLRs
-// Batched (vbx_cohort_stats_batch, section 5.19): G problems against one cohort, each with its c_g: the statistics of
-// the scored speakers of all problems and of the cohort once per problem, enroll_score_kernel over every problem's
-// rectangle in one launch, and cohort_topk_kernel over all rows (a row's result depends on the row and C alone).
-// norm_scores_kernel takes NormProblems for vbx_enroll_batch and vbx_link_batch_norm.
+//                        distances (d = -S; the diagonal and the cannot-link entries untouched) or the enrolment LLRs,
+//                        every problem with its own statistics (NormProblems), for vbx_link_batch and vbx_enroll_batch
 #include <algorithm>
 #include <cstring>
 
@@ -24,22 +26,6 @@ constexpr int kTopWarps = kTopThreads / 32;
 constexpr int64_t kNormGrid = 1 << 20;     // CTAs of norm_scores_kernel at most; beyond that they stride
 
 __host__ __device__ size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
-
-struct CohortWs {
-    SpeakerStats a, co;      // scored speakers [M], cohort speakers [C]
-    double *scores;          // [M, C]
-};
-
-CohortWs cohort_layout(uint8_t *ws, int64_t M, int64_t C, size_t *total) {
-    CohortWs w;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { uint8_t *p = ws ? ws + o : nullptr; o += al(bytes); return p; };
-    w.a = take_stats(take, M);
-    w.co = take_stats(take, C);
-    w.scores = reinterpret_cast<double *>(take((size_t)M * C * 8));
-    if (total) *total = o;
-    return w;
-}
 
 // Doubles ordered as their keys are ordered (as unsigned integers): negative values bit-inverted, the others with the
 // sign bit set.  -0.0 sorts just below +0.0; equal values have equal keys.
@@ -121,9 +107,9 @@ __global__ void __launch_bounds__(kTopThreads) cohort_topk_kernel(const double *
 // x [rows, cols] in place: LLR -> S(i, j) with row statistics (mr, sr) and column statistics (mc, sc).  link = 1: x holds
 // distances d = -LLR, written back as -S, and the diagonal and the entries equal to `skip` (cannot-link) stay as they
 // are.  S is 1/2 (a_i + a_j) with a_i = (LLR - mu_i) / sigma_i: the sum commutes, so d[i][j] and d[j][i] stay the same
-// number.  copy_out (optional) receives the result.  q.off set: several problems (NormProblems, section 5.19), each
-// element with the statistics of its own problem, so problem g's entries are those of a call on g alone.  kMode: 0 one
-// problem (q unused; the code of the single-problem entries), 1 the rectangle of several, 2 their square blocks.
+// number.  copy_out (optional) receives the result.  Every element takes the statistics of its own problem (q,
+// section 5.19), so problem g's entries are those of a call on g alone.  kMode: 1 the rectangle of the problems' rows,
+// 2 their square blocks.
 template <int kMode>
 __global__ void __launch_bounds__(256) norm_scores_kernel(double *__restrict__ x, int64_t rows, int64_t cols,
                                                           const double *__restrict__ mr, const double *__restrict__ sr,
@@ -131,84 +117,47 @@ __global__ void __launch_bounds__(256) norm_scores_kernel(double *__restrict__ x
                                                           int link, double skip, double *__restrict__ copy_out,
                                                           NormProblems q) {
     const int64_t n = rows * cols, stride = (int64_t)gridDim.x * blockDim.x;
-    if constexpr (kMode == 0) {
-        for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
-            const int64_t i = t / cols, j = t - i * cols;
-            double d = x[t];
-            if (!link || (i != j && d != skip)) {
-                const double l = link ? -d : d;
-                const double s = 0.5 * ((l - mr[i]) / sr[i] + (l - mc[j]) / sc[j]);
-                d = link ? -s : s;
-                x[t] = d;
-            }
-            if (copy_out) copy_out[t] = d;
+    for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
+        int64_t i, j, ri, cj;                             // local row and column; indices of their statistics
+        double *xt = x + t;
+        if (kMode == 2) {                                 // square blocks: problem g's M x M block
+            const int g = find_problem(q.blk, q.G, t);
+            const int64_t base = q.off[g], M = q.off[g + 1] - base, lt = t - q.blk[g];
+            i = lt / M;
+            j = lt - i * M;
+            ri = base + i;
+            cj = base + j;
+            xt = reinterpret_cast<double *>(reinterpret_cast<uint8_t *>(x) + q.x_bytes[g]) + lt;
+        } else {                                          // rectangle: rows of every problem against its own columns
+            i = ri = t / cols;
+            j = t - i * cols;
+            cj = (int64_t)find_problem(q.off, q.G, i) * cols + j;
         }
-    } else {
-        for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += stride) {
-            int64_t i, j, ri, cj;                         // local row and column; indices of their statistics
-            double *xt = x + t;
-            if (kMode == 2) {                             // square blocks: problem g's M x M block
-                const int g = find_problem(q.blk, q.G, t);
-                const int64_t base = q.off[g], M = q.off[g + 1] - base, lt = t - q.blk[g];
-                i = lt / M;
-                j = lt - i * M;
-                ri = base + i;
-                cj = base + j;
-                xt = reinterpret_cast<double *>(reinterpret_cast<uint8_t *>(x) + q.x_bytes[g]) + lt;
-            } else {                                      // rectangle: rows of every problem against its own columns
-                i = ri = t / cols;
-                j = t - i * cols;
-                cj = (int64_t)find_problem(q.off, q.G, i) * cols + j;
-            }
-            double d = *xt;
-            if (!link || (i != j && d != skip)) {
-                const double l = link ? -d : d;
-                const double s = 0.5 * ((l - mr[ri]) / sr[ri] + (l - mc[cj]) / sc[cj]);
-                d = link ? -s : s;
-                *xt = d;
-            }
-            if (copy_out) copy_out[t] = d;
+        double d = *xt;
+        if (!link || (i != j && d != skip)) {
+            const double l = link ? -d : d;
+            const double s = 0.5 * ((l - mr[ri]) / sr[ri] + (l - mc[cj]) / sc[cj]);
+            d = link ? -s : s;
+            *xt = d;
         }
+        if (copy_out) copy_out[t] = d;
     }
 }
 
 }  // namespace
 
-size_t cohort_workspace_bytes(int64_t M, int64_t C) {
-    size_t total = 0;
-    cohort_layout(nullptr, M, C, &total);
-    return total;
-}
-
-int launch_cohort(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
-                  const float *cohort_fea, int64_t N_c, const int32_t *cohort_spk, int64_t C, double c, int64_t top_k,
-                  void *workspace, double *mean_out, double *std_out, double *scores_out, cudaStream_t st) {
-    if (M == 0) return 0;
-    const CohortWs w = cohort_layout(reinterpret_cast<uint8_t *>(workspace), M, C, nullptr);
-    const int la = launch_speaker_stats(fea, Phi, spk, N, R, M, c, w.a, nullptr, nullptr, st);
-    const int lc = launch_speaker_stats(cohort_fea, Phi, cohort_spk, N_c, R, C, c, w.co, nullptr, nullptr, st);
-    const int ls = launch_cohort_scores(w.a, w.co, Phi, M, C, R, c, w.scores, scores_out, st);
-    if (la < 0 || lc < 0 || ls < 0) return -1;
-    cohort_topk_kernel<<<(unsigned)M, kTopThreads, 0, st>>>(w.scores, C, std::min(top_k, C), mean_out, std_out);
-    return cudaGetLastError() == cudaSuccess ? la + lc + ls + 1 : -1;
-}
-
 int launch_norm_scores(double *x, int64_t rows, int64_t cols, const double *mean_r, const double *std_r,
                        const double *mean_c, const double *std_c, bool link, double skip, double *copy_out,
-                       cudaStream_t st, const NormProblems *q) {
+                       cudaStream_t st, const NormProblems &q) {
     const int64_t n = rows * cols;
     if (n == 0) return 0;
     const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, kNormGrid);
-    const NormProblems one{1, nullptr, nullptr, nullptr};
-    if (!q)
-        norm_scores_kernel<0><<<grid, 256, 0, st>>>(x, rows, cols, mean_r, std_r, mean_c, std_c, link ? 1 : 0, skip,
-                                                    copy_out, one);
-    else if (q->blk)
+    if (q.blk)
         norm_scores_kernel<2><<<grid, 256, 0, st>>>(x, rows, cols, mean_r, std_r, mean_c, std_c, link ? 1 : 0, skip,
-                                                    copy_out, *q);
+                                                    copy_out, q);
     else
         norm_scores_kernel<1><<<grid, 256, 0, st>>>(x, rows, cols, mean_r, std_r, mean_c, std_c, link ? 1 : 0, skip,
-                                                    copy_out, *q);
+                                                    copy_out, q);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -249,7 +198,7 @@ size_t cohort_batch_workspace_bytes(int G, const int64_t *M_host, int64_t C, int
 int launch_cohort_batch(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int G,
                         const int64_t *M_host, const float *cohort_fea, int64_t N_c, const int32_t *cohort_spk,
                         int64_t C, const double *c_host, int64_t top_k, void *workspace, double *mean_out,
-                        double *std_out, cudaStream_t st) {
+                        double *std_out, double *scores_out, cudaStream_t st) {
     std::vector<int64_t> host(4 * (size_t)G + 3, 0);       // off, coff, tile_off [G+1], c [G]: one copy
     int64_t *off = host.data(), *coff = off + (G + 1), *tile = coff + (G + 1);
     for (int g = 0; g < G; ++g) {
@@ -270,7 +219,8 @@ int launch_cohort_batch(const float *fea, const float *Phi, int64_t N, int R, co
     const int la = launch_speaker_stats_batch(fea, Phi, spk, N, R, G, d_off, d_c, M, w.a, nullptr, nullptr, st);
     const int lc = launch_speaker_stats_batch(cohort_fea, Phi, w.cspk, N_c, R, G, d_coff, d_c, (int64_t)G * C, w.co,
                                               nullptr, nullptr, st);
-    const int ls = launch_cohort_scores_batch(w.a, w.co, Phi, G, d_off, d_tile, d_c, tile[G], C, R, w.scores, st);
+    const int ls = launch_cohort_scores_batch(w.a, w.co, Phi, G, d_off, d_tile, d_c, tile[G], C, R, w.scores,
+                                              scores_out, st);
     if (lr < 0 || la < 0 || lc < 0 || ls < 0) return -1;
     cohort_topk_kernel<<<(unsigned)M, kTopThreads, 0, st>>>(w.scores, C, std::min(top_k, C), mean_out, std_out);
     return cudaGetLastError() == cudaSuccess ? lr + la + lc + ls + 1 : -1;

@@ -1,19 +1,19 @@
-// Enrolment against known speakers (DESIGN.md section 5.16).  The archive's speakers (section 5.15's table) and the
-// enrolled speakers get the statistics n, F, b and e of vbx_link (its span and statistics kernels, through
-// launch_speaker_stats), every archive speaker s is scored against every enrolled speaker e with section 5.15's LLR,
-// and each recording's speakers are assigned one-to-one to enrolled speakers or to "unknown":
-//   enroll_score_kernel   llr [M, E], 32 x 32 tiles of the rectangle; per pair the operations of vbx_link's score_tile
-//                         in the same order, so llr[s][e] is bit-identical to -dist[s][e] of vbx_link on the same speakers
-//   enroll_assign_kernel  per recording b with K_b speakers the minimum-cost assignment of the K_b x (E + K_b) matrix
-//                         C[k][e] = threshold - llr[k][e] (e < E), C[k][E + j] = 0 ("unknown" columns), by shortest
-//                         augmenting paths (Jonker-Volgenant, the method of scipy's linear_sum_assignment): one
-//                         Dijkstra per row over the columns; a persistent grid, one recording per CTA at a time
-// With cohort statistics (vbx_enroll_norm, section 5.17) vbx_cohort.cu's norm_scores_kernel turns llr into S in place
-// between the two.  launch_cohort_scores runs enroll_score_kernel against a cohort for vbx_cohort_stats.
-// Batched (vbx_enroll_batch, section 5.19): G problems (e.g. the settings of a sweep) share fea, Phi and the enrolled
-// set; each has its own speakers, c_g and column statistics (vbx_link's statistics kernels over all problems at once),
-// enroll_score_kernel decodes its flat tile index into (problem, tile), and enroll_assign_kernel takes n_thr thresholds
-// from the device, one output plane each.  vbx_enroll is the G = 1 case with null problem arrays.
+// Enrolment against known speakers (DESIGN.md sections 5.16, 5.19).  vbx_enroll_batch runs G problems (e.g. the
+// settings of a sweep; one archive is the batch of one) that share fea, Phi and the enrolled set; each has its own
+// speakers, c_g and column statistics.  The archive's speakers (section 5.15's table) and the enrolled speakers get
+// the statistics n, F, b and e of vbx_link_batch (its span and statistics kernels over all problems at once, through
+// launch_speaker_stats_batch), every archive speaker s is scored against every enrolled speaker e with section 5.15's
+// LLR, and each recording's speakers are assigned one-to-one to enrolled speakers or to "unknown":
+//   enroll_score_kernel   llr [M, E], 32 x 32 tiles of every problem's rectangle, the flat tile index decoded into
+//                         (problem, tile); per pair the operations of vbx_link's score_tile in the same order, so
+//                         llr[s][e] is bit-identical to -dist[s][e] of vbx_link_batch on the same speakers
+//   enroll_assign_kernel  per recording b with K_b speakers and threshold h the minimum-cost assignment of the
+//                         K_b x (E + K_b) matrix C[k][e] = threshold_h - llr[k][e] (e < E), C[k][E + j] = 0 ("unknown"
+//                         columns), by shortest augmenting paths (Jonker-Volgenant, the method of scipy's
+//                         linear_sum_assignment): one Dijkstra per row over the columns; a persistent grid, one
+//                         (threshold, recording) item per CTA at a time, one output plane per threshold
+// With cohort statistics (section 5.17) vbx_cohort.cu's norm_scores_kernel turns llr into S in place between the two.
+// launch_cohort_scores_batch runs enroll_score_kernel against a cohort for vbx_cohort_stats_batch.
 #include <algorithm>
 #include <climits>
 #include <cstring>
@@ -56,56 +56,35 @@ __host__ __device__ Slice slice_at(uint8_t *base, int64_t ncm, int64_t km, size_
     return s;
 }
 
+// The archive speakers of all problems [M], the enrolled speakers once per problem [G E] with their index [G, N_e],
+// llr [M, E], the problem arrays (off, eoff = g E, tile_off [G+1], c [G], thresholds [n_thr], recs [at most M + 1]:
+// the speaker offsets of the recordings that have speakers) and the slices of CTAs that take n_thr x (recordings with
+// speakers) items
 struct EnrollWs {
-    SpeakerStats a, en;      // archive speakers [M], enrolled speakers [E]
-    double *llr;             // [M, E]
-    int64_t *recs;           // [n_busy + 1]: speaker offsets of the recordings that have speakers
+    SpeakerStats a, en;
+    int32_t *espk;
+    double *llr;
+    int64_t *arrays;
     uint8_t *slices;         // ctas x slice_bytes
     size_t slice_bytes;
     int64_t ctas;
 };
 
-EnrollWs enroll_layout(uint8_t *ws, int64_t M, int64_t E, int64_t max_k, int sms, size_t *total) {
+EnrollWs enroll_layout(uint8_t *ws, int64_t G, int64_t M, int64_t E, int64_t N_e, int64_t max_k, int64_t n_thr, int sms,
+                       size_t *total) {
     EnrollWs w;
-    size_t o = 0;
-    auto take = [&](size_t bytes) { uint8_t *p = ws ? ws + o : nullptr; o += al(bytes); return p; };
-    w.a = take_stats(take, M);
-    w.en = take_stats(take, E);
-    w.llr = reinterpret_cast<double *>(take((size_t)M * E * 8));
-    w.recs = reinterpret_cast<int64_t *>(take((M + 1) * 8));
-    slice_at(nullptr, E + max_k, max_k, &w.slice_bytes);
-    w.ctas = std::min<int64_t>((int64_t)kAssignCtasPerSm * std::max(sms, 1), std::max<int64_t>(M, 1));
-    w.slices = take(w.slice_bytes * w.ctas);
-    if (total) *total = o;
-    return w;
-}
-
-// vbx_enroll_batch (section 5.19): the archive speakers of all problems [M], the enrolled speakers once per problem
-// [G E] with their index [G, N_e], llr [M, E], the problem arrays (off, eoff = g E, tile_off [G+1], c [G], thresholds
-// [n_thr], recs [at most M + 1]) and the slices of CTAs that take n_thr x (recordings with speakers) items
-struct EnrollBatchWs {
-    EnrollWs w;
-    int32_t *espk;
-    int64_t *arrays;
-};
-
-EnrollBatchWs enroll_batch_layout(uint8_t *ws, int64_t G, int64_t M, int64_t E, int64_t N_e, int64_t max_k,
-                                  int64_t n_thr, int sms, size_t *total) {
-    EnrollBatchWs b;
-    EnrollWs &w = b.w;
     size_t o = 0;
     auto take = [&](size_t bytes) { uint8_t *p = ws ? ws + o : nullptr; o += al(bytes); return p; };
     w.a = take_stats(take, M);
     w.en = take_stats(take, G * E);
-    b.espk = reinterpret_cast<int32_t *>(take((size_t)G * N_e * 4));
+    w.espk = reinterpret_cast<int32_t *>(take((size_t)G * N_e * 4));
     w.llr = reinterpret_cast<double *>(take((size_t)M * E * 8));
-    b.arrays = reinterpret_cast<int64_t *>(take((size_t)(4 * G + 3 + n_thr + M + 1) * 8));
-    w.recs = nullptr;
+    w.arrays = reinterpret_cast<int64_t *>(take((size_t)(4 * G + 3 + n_thr + M + 1) * 8));
     slice_at(nullptr, E + max_k, max_k, &w.slice_bytes);
     w.ctas = std::min<int64_t>((int64_t)kAssignCtasPerSm * std::max(sms, 1), std::max<int64_t>(M * n_thr, 1));
     w.slices = take(w.slice_bytes * w.ctas);
     if (total) *total = o;
-    return b;
+    return w;
 }
 
 __global__ void repeat_index_kernel(const int32_t *__restrict__ src, int64_t n, int64_t total,
@@ -114,48 +93,37 @@ __global__ void repeat_index_kernel(const int32_t *__restrict__ src, int64_t n, 
         dst[i] = src[i % n];
 }
 
-// The problems of one enroll_score_kernel launch.  G = 1 with null arrays: M rows against E columns with c = c0
-// (vbx_enroll, vbx_cohort_stats).  Batched (section 5.19): problem g's rows are off[g] .. off[g+1]-1 of the row
-// statistics and of llr, its columns g E .. g E + E - 1 of the column statistics (whose b and e depend on c_g), and its
-// tiles tile_off[g] .. tile_off[g+1]-1 of the flat tile index.
+// The problems of one enroll_score_kernel launch: problem g's rows are off[g] .. off[g+1]-1 of the row statistics and
+// of llr, its columns g E .. g E + E - 1 of the column statistics (whose b and e depend on c_g), and its tiles
+// tile_off[g] .. tile_off[g+1]-1 of the flat tile index.
 struct ScoreProblems {
     int G;
     const int64_t *off, *tile_off;
     const double *c;
 };
-constexpr ScoreProblems kOneProblem{1, nullptr, nullptr, nullptr};
 
 // Tile (bi, bj) of 32 archive speakers (rows) x 32 enrolled speakers (columns): 256 threads, 4 pairs each (rows ty,
 // ty + 8, ..), features in chunks of 32 through shared memory; every operation as in vbx_link's score_tile.  The flat
 // tile index runs over the rectangles of all problems (decoded as link_score_kernel does), so the grid stays
-// one-dimensional and capped for any G, M_g and E.  kMany = false (one problem, pr unused) is the code of the
-// single-problem entries; kMany = true decodes the problems.
-template <bool kMany>
+// one-dimensional and capped for any G, M_g and E.
 __global__ void __launch_bounds__(256) enroll_score_kernel(SpeakerStats A0, SpeakerStats En0, const float *__restrict__ Phi,
-                                                           int64_t M0, int64_t E, int R, double c0, double *__restrict__ llr0,
+                                                           int64_t E, int R, double *__restrict__ llr0,
                                                            double *__restrict__ llr_out0, ScoreProblems pr) {
     __shared__ double a[32][33], bt[32][33], ph[32];
-    const int64_t tiles_e = (E + 31) / 32, n_tiles = kMany ? pr.tile_off[pr.G] : ((M0 + 31) / 32) * tiles_e;
+    const int64_t tiles_e = (E + 31) / 32, n_tiles = pr.tile_off[pr.G];
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
     for (int64_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const int g = find_problem(pr.tile_off, pr.G, t);
+        const int64_t base = pr.off[g], col = (int64_t)g * E, M = pr.off[g + 1] - base, lt = t - pr.tile_off[g];
+        const double c = pr.c[g];
         SpeakerStats A = A0, En = En0;
-        int64_t M = M0, lt = t;
-        double c = c0, *llr = llr0, *llr_out = llr_out0;
-        if (kMany) {
-            const int g = find_problem(pr.tile_off, pr.G, t);
-            const int64_t base = pr.off[g], col = (int64_t)g * E;
-            M = pr.off[g + 1] - base;
-            lt = t - pr.tile_off[g];
-            c = pr.c[g];
-            A.n += base;
-            A.e += base;
-            A.b += base * kMaxR;
-            En.n += col;
-            En.e += col;
-            En.b += col * kMaxR;
-            llr += base * E;
-            if (llr_out) llr_out += base * E;
-        }
+        A.n += base;
+        A.e += base;
+        A.b += base * kMaxR;
+        En.n += col;
+        En.e += col;
+        En.b += col * kMaxR;
+        double *llr = llr0 + base * E, *llr_out = llr_out0 ? llr_out0 + base * E : nullptr;
         const int64_t i0 = (lt / tiles_e) * 32, j0 = (lt % tiles_e) * 32;
         const int64_t j = j0 + tx;
         const double nj = j < E ? En.n[j] : 0.0;
@@ -220,29 +188,24 @@ __device__ __forceinline__ void take_min(double &bv, int64_t &bj, double ov, int
 // updated and the path augmented as scipy's rectangular_lsap does.  A step that reaches no column (non-finite costs)
 // leaves the row unassigned.  Outputs per speaker: its enrolled index or -1, and the LLR of its pair, or for an
 // unknown speaker its largest LLR.
-// Work items: one problem (kMany = false): one per recording of recs at the threshold theta0.  Batched (section 5.19): the
-// recordings with speakers of every problem are one list recs (the problems' speakers are packed one after the other,
-// so their offsets run on), and item (h, rec) assigns recording rec at thresholds[h] into plane h of the outputs
-// (assign_out + h plane, best_out + h plane): n_thr x n_recs items over the persistent grid, so the slices stay
-// CTAs x (E + max_k) and the LLR block is computed once for every threshold.  The body is written once (assign_items);
-// enroll_assign_kernel (kMany = false: thetas, n_thr and plane unused) runs it for the single-problem entries and
-// enroll_assign_batch_kernel (kMany = true, bounded for the kAssignCtasPerSm CTAs per SM it is launched with, which
-// keeps its larger state in registers) for vbx_enroll_batch.
-template <bool kMany>
-__device__ __forceinline__ void assign_items(const double *__restrict__ llr, const int64_t *__restrict__ recs,
-                                             int64_t n_recs, int64_t E, double theta0, uint8_t *slices,
-                                             size_t slice_bytes, int64_t max_k, int32_t *__restrict__ assign_all,
-                                             double *__restrict__ best_all, const double *__restrict__ thetas,
-                                             int64_t n_thr, int64_t plane) {
+// Work items: the recordings with speakers of every problem are one list recs (the problems' speakers are packed one
+// after the other, so their offsets run on), and item (h, rec) assigns recording rec at thresholds[h] into plane h of
+// the outputs (assign_out + h plane, best_out + h plane): n_thr x n_recs items over the persistent grid, so the slices
+// stay CTAs x (E + max_k) and the LLR block is computed once for every threshold.  Bounded for the kAssignCtasPerSm
+// CTAs per SM it is launched with, which keeps its state in registers.
+__global__ void __launch_bounds__(kAssignThreads, kAssignCtasPerSm) enroll_assign_kernel(
+    const double *__restrict__ llr, const int64_t *__restrict__ recs, int64_t n_recs, int64_t E, uint8_t *slices,
+    size_t slice_bytes, int64_t max_k, int32_t *__restrict__ assign_all, double *__restrict__ best_all,
+    const double *__restrict__ thetas, int64_t n_thr, int64_t plane) {
     __shared__ double wv[kAssignWarps];
     __shared__ int64_t wj[kAssignWarps];
     __shared__ double s_min;
     __shared__ int64_t s_i, s_sink;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const Slice sl = slice_at(slices + (size_t)blockIdx.x * slice_bytes, E + max_k, max_k, nullptr);
-    for (int64_t item = blockIdx.x; item < (kMany ? n_recs * n_thr : n_recs); item += gridDim.x) {
-        const int64_t h = kMany ? item / n_recs : 0, rec = item - h * n_recs;
-        const double theta = kMany ? thetas[h] : theta0;
+    for (int64_t item = blockIdx.x; item < n_recs * n_thr; item += gridDim.x) {
+        const int64_t h = item / n_recs, rec = item - h * n_recs;
+        const double theta = thetas[h];
         const int64_t s0 = recs[rec], K = recs[rec + 1] - s0, nc = E + K;
         for (int64_t j = tid; j < nc; j += kAssignThreads) {
             sl.v[j] = 0.0;
@@ -344,7 +307,7 @@ __device__ __forceinline__ void assign_items(const double *__restrict__ llr, con
                 for (int o = 16; o; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
             }
             if (lane == 0) {
-                const int64_t o = (kMany ? (item / n_recs) * plane : 0) + s0 + k;   // threshold h's plane
+                const int64_t o = h * plane + s0 + k;         // threshold h's plane
                 assign_all[o] = named ? (int32_t)col : -1;
                 best_all[o] = m;
             }
@@ -353,92 +316,17 @@ __device__ __forceinline__ void assign_items(const double *__restrict__ llr, con
     }
 }
 
-__global__ void __launch_bounds__(kAssignThreads) enroll_assign_kernel(const double *__restrict__ llr,
-                                                                      const int64_t *__restrict__ recs, int64_t n_recs,
-                                                                      int64_t E, double theta, uint8_t *slices,
-                                                                      size_t slice_bytes, int64_t max_k,
-                                                                      int32_t *__restrict__ assign_out,
-                                                                      double *__restrict__ best_out) {
-    assign_items<false>(llr, recs, n_recs, E, theta, slices, slice_bytes, max_k, assign_out, best_out, nullptr, 1, 0);
-}
-
-__global__ void __launch_bounds__(kAssignThreads, kAssignCtasPerSm) enroll_assign_batch_kernel(
-    const double *__restrict__ llr, const int64_t *__restrict__ recs, int64_t n_recs, int64_t E, uint8_t *slices,
-    size_t slice_bytes, int64_t max_k, int32_t *__restrict__ assign_out, double *__restrict__ best_out,
-    const double *__restrict__ thetas, int64_t n_thr, int64_t plane) {
-    assign_items<true>(llr, recs, n_recs, E, 0.0, slices, slice_bytes, max_k, assign_out, best_out, thetas, n_thr, plane);
-}
-
 }  // namespace
-
-size_t enroll_workspace_bytes(int64_t M, int64_t E, int64_t max_k, int sms) {
-    size_t total = 0;
-    enroll_layout(nullptr, M, E, max_k, sms, &total);
-    return total;
-}
-
-int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
-                  const int64_t *rec_off_host, int n_rec, const float *enroll_fea, int64_t N_e, const int32_t *enroll_spk,
-                  int64_t E, double c, double threshold, void *workspace, int sms, int32_t *assign_out,
-                  double *best_llr_out, double *llr_out, double *n_out, double *F_out, double *n_enroll_out,
-                  double *F_enroll_out, cudaStream_t st, const double *mean, const double *std,
-                  const double *enroll_mean, const double *enroll_std) {
-    std::vector<int64_t> busy(1, 0);                  // speaker offsets of the recordings that have speakers
-    int64_t max_k = 0;
-    for (int b = 0; b < n_rec; ++b) {
-        const int64_t k = rec_off_host[b + 1] - rec_off_host[b];
-        if (k > 0) busy.push_back(rec_off_host[b + 1]);
-        max_k = std::max(max_k, k);
-    }
-    const EnrollWs w = enroll_layout(reinterpret_cast<uint8_t *>(workspace), M, E, max_k, sms, nullptr);
-    const int64_t n_busy = (int64_t)busy.size() - 1;
-    int launches = 0;
-    if (n_busy > 0 &&   // pageable source: staged before the call returns, no wait on the stream
-        cudaMemcpyAsync(w.recs, busy.data(), busy.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st) != cudaSuccess)
-        return -1;
-    const int la = launch_speaker_stats(fea, Phi, spk, N, R, M, c, w.a, n_out, F_out, st);
-    const int le = launch_speaker_stats(enroll_fea, Phi, enroll_spk, N_e, R, E, c, w.en, n_enroll_out, F_enroll_out, st);
-    if (la < 0 || le < 0) return -1;
-    launches += la + le;
-    if (M > 0) {
-        const int64_t n_tiles = ((M + 31) / 32) * ((E + 31) / 32);
-        enroll_score_kernel<false><<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(w.a, w.en, Phi, M, E, R, c,
-                                                                                             w.llr, mean ? nullptr : llr_out,
-                                                                                             kOneProblem);
-        ++launches;
-        if (mean) {                                   // normalised scores (section 5.17): assigned and written as llr
-            const int ln = launch_norm_scores(w.llr, M, E, mean, std, enroll_mean, enroll_std, false, 0.0, llr_out, st);
-            if (ln < 0) return -1;
-            launches += ln;
-        }
-    }
-    if (n_busy > 0) {
-        enroll_assign_kernel<<<(unsigned)std::min<int64_t>(n_busy, w.ctas), kAssignThreads, 0, st>>>(
-            w.llr, w.recs, n_busy, E, threshold, w.slices, w.slice_bytes, max_k, assign_out, best_llr_out);
-        ++launches;
-    }
-    return cudaGetLastError() == cudaSuccess ? launches : -1;
-}
-
-int launch_cohort_scores(const SpeakerStats &a, const SpeakerStats &co, const float *Phi, int64_t M, int64_t C, int R,
-                         double c, double *llr, double *llr_out, cudaStream_t st) {
-    if (M == 0) return 0;
-    const int64_t n_tiles = ((M + 31) / 32) * ((C + 31) / 32);
-    enroll_score_kernel<false><<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(a, co, Phi, M, C, R,
-                                                                                                c, llr, llr_out,
-                                                                                                kOneProblem);
-    return cudaGetLastError() == cudaSuccess ? 1 : -1;
-}
 
 int64_t rect_tiles(int64_t M, int64_t C) { return ((M + 31) / 32) * ((C + 31) / 32); }
 
 int launch_cohort_scores_batch(const SpeakerStats &a, const SpeakerStats &co, const float *Phi, int G,
                                const int64_t *off, const int64_t *tile_off, const double *c, int64_t n_tiles, int64_t C,
-                               int R, double *llr, cudaStream_t st) {
+                               int R, double *llr, double *llr_out, cudaStream_t st) {
     if (n_tiles == 0) return 0;
     const ScoreProblems p{G, off, tile_off, c};
-    enroll_score_kernel<true><<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(a, co, Phi, 0, C, R, 0.0,
-                                                                                               llr, nullptr, p);
+    enroll_score_kernel<<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(a, co, Phi, C, R, llr,
+                                                                                         llr_out, p);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -454,7 +342,7 @@ size_t enroll_batch_workspace_bytes(int G, const int64_t *M_host, int64_t E, int
     int64_t M = 0;
     for (int g = 0; g < G; ++g) M += M_host[g];
     size_t total = 0;
-    enroll_batch_layout(nullptr, G, M, E, N_e, max_k, n_thr, sms, &total);
+    enroll_layout(nullptr, G, M, E, N_e, max_k, n_thr, sms, &total);
     return total;
 }
 
@@ -491,36 +379,34 @@ int launch_enroll_batch(const float *fea, const float *Phi, int64_t N, int R, co
         }
     }
     const int64_t M = off[G], n_busy = (int64_t)(host.size() - recs_at) - 1;
-    const EnrollBatchWs b = enroll_batch_layout(reinterpret_cast<uint8_t *>(workspace), G, M, E, N_e, max_k, n_thr,
-                                                sms, nullptr);
-    const EnrollWs &w = b.w;
-    if (cudaMemcpyAsync(b.arrays, host.data(), host.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st) !=
+    const EnrollWs w = enroll_layout(reinterpret_cast<uint8_t *>(workspace), G, M, E, N_e, max_k, n_thr, sms, nullptr);
+    if (cudaMemcpyAsync(w.arrays, host.data(), host.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st) !=
         cudaSuccess)
         return -1;
-    const int64_t *d_off = b.arrays, *d_eoff = d_off + (G + 1), *d_tile = d_eoff + (G + 1);
+    const int64_t *d_off = w.arrays, *d_eoff = d_off + (G + 1), *d_tile = d_eoff + (G + 1);
     const double *d_c = reinterpret_cast<const double *>(d_tile + (G + 1)), *d_thr = d_c + G;
-    const int64_t *d_recs = b.arrays + recs_at;
-    const int lr = launch_repeat_index(enroll_spk, N_e, G, b.espk, st);
+    const int64_t *d_recs = w.arrays + recs_at;
+    const int lr = launch_repeat_index(enroll_spk, N_e, G, w.espk, st);
     const int la = launch_speaker_stats_batch(fea, Phi, spk, N, R, G, d_off, d_c, M, w.a, n_out, F_out, st);
-    const int le = launch_speaker_stats_batch(enroll_fea, Phi, b.espk, N_e, R, G, d_eoff, d_c, (int64_t)G * E, w.en,
+    const int le = launch_speaker_stats_batch(enroll_fea, Phi, w.espk, N_e, R, G, d_eoff, d_c, (int64_t)G * E, w.en,
                                               n_enroll_out, F_enroll_out, st);
     if (lr < 0 || la < 0 || le < 0) return -1;
     int launches = lr + la + le;
     if (M > 0) {
         const ScoreProblems p{G, d_off, d_tile, d_c};
-        enroll_score_kernel<true><<<(unsigned)std::min<int64_t>(tile[G], kScoreGrid), 256, 0, st>>>(
-            w.a, w.en, Phi, 0, E, R, 0.0, w.llr, mean ? nullptr : llr_out, p);
+        enroll_score_kernel<<<(unsigned)std::min<int64_t>(tile[G], kScoreGrid), 256, 0, st>>>(
+            w.a, w.en, Phi, E, R, w.llr, mean ? nullptr : llr_out, p);
         ++launches;
         if (mean) {                                   // normalised scores, each problem with its own statistics
             const NormProblems q{G, d_off, nullptr, nullptr};
             const int ln = launch_norm_scores(w.llr, M, E, mean, std, enroll_mean, enroll_std, false, 0.0, llr_out, st,
-                                              &q);
+                                              q);
             if (ln < 0) return -1;
             launches += ln;
         }
     }
     if (n_busy > 0) {
-        enroll_assign_batch_kernel<<<(unsigned)std::min<int64_t>(n_busy * n_thr, w.ctas), kAssignThreads, 0, st>>>(
+        enroll_assign_kernel<<<(unsigned)std::min<int64_t>(n_busy * n_thr, w.ctas), kAssignThreads, 0, st>>>(
             w.llr, d_recs, n_busy, E, w.slices, w.slice_bytes, max_k, assign_out, best_llr_out, d_thr, n_thr, M);
         ++launches;
     }

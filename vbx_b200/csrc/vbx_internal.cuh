@@ -278,25 +278,19 @@ int launch_ahc(const Plan &pl, const std::vector<int64_t> &d_off, const void *x,
 // laid out as vbx_ahc's, and its Z rows start at row offsets[b] of Z_out
 size_t linkage_workspace_bytes(int64_t T);
 void launch_linkage(const int64_t *offsets, const int64_t *d_off, int n, void *ws, double *Z_out, cudaStream_t st);
-// speaker linking across recordings (vbx_link.cu)
-size_t link_workspace_bytes(int64_t M);
-int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
-                int64_t M, double c, void *workspace, double *n_out, double *F_out, double *dist_out, double *Z_out,
-                cudaStream_t st, const double *mean = nullptr, const double *std = nullptr);
-// G linking problems in one set of launches (vbx_link_batch): M_host [G] speakers and c_host [G] = Fa_g / Fb_g on the
-// HOST; lk_off (when not null) gets the byte offsets [G+1] of the problems' linkage regions
+// speaker linking across recordings (vbx_link.cu): G problems in one set of launches (vbx_link_batch), M_host [G]
+// speakers and c_host [G] = Fa_g / Fb_g on the HOST; lk_off (when not null) gets the byte offsets [G+1] of the
+// problems' linkage regions.  mean, std [sum M] (DEVICE, both or neither): normalised distances
 size_t link_batch_workspace_bytes(int G, const int64_t *M_host, std::vector<int64_t> *lk_off = nullptr);
 int launch_link_batch(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
                       int G, const int64_t *M_host, const double *c_host, void *workspace, double *n_out,
-                      double *F_out, double *dist_out, double *Z_out, cudaStream_t st, const double *mean = nullptr,
-                      const double *std = nullptr);
-// vbx_link's span and statistics kernels over M speakers into caller-owned DEVICE arrays (n, e [M], b [M, kMaxR]
-// float64; first, last [M] and offs [4] int64 scratch): n_s, F_s, b_s and e_s exactly as vbx_link computes them.
-// Returns the number of launches, -1 on a launch error.
+                      double *F_out, double *dist_out, double *Z_out, cudaStream_t st, const double *mean,
+                      const double *std);
+// Caller-owned DEVICE arrays for the statistics of vbx_link_batch's span and statistics kernels: n, e [M],
+// b [M, kMaxR] float64; first, last [M] int64 scratch.
 struct SpeakerStats {
     double *n, *e, *b;
     long long *first, *last;
-    int64_t *offs;
 };
 // The statistics of n speakers carved from a workspace by take(bytes) (host), as the enrolment and cohort layouts hold them
 template <class Take>
@@ -307,13 +301,12 @@ SpeakerStats take_stats(Take &take, int64_t n) {
     s.b = reinterpret_cast<double *>(take(n * kMaxR * 8));
     s.first = reinterpret_cast<long long *>(take(n * 8));
     s.last = reinterpret_cast<long long *>(take(n * 8));
-    s.offs = reinterpret_cast<int64_t *>(take(4 * 8));
+    take(4 * 8);             // unused; kept so that the published batched workspace sizes stay the same
     return s;
 }
-int launch_speaker_stats(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, int64_t M, double c,
-                         const SpeakerStats &s, double *n_out, double *F_out, cudaStream_t st);
-// The same over G problems as vbx_link_batch runs them: spk [G,N] (row g: local speakers of problem g), off [G+1] and
-// c [G] DEVICE; s holds M = off[G] speakers.  Problem g's statistics are bit-identical to launch_speaker_stats on it alone.
+// n_s, F_s, b_s and e_s of G problems into s as vbx_link_batch computes them: spk [G,N] (row g: local speakers of
+// problem g), off [G+1] and c [G] DEVICE; s holds M = off[G] speakers.  Problem g's statistics do not depend on the
+// other problems.  Returns the number of launches, -1 on a launch error.
 int launch_speaker_stats_batch(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, int G,
                                const int64_t *off, const double *c, int64_t M, const SpeakerStats &s, double *n_out,
                                double *F_out, cudaStream_t st);
@@ -326,23 +319,13 @@ struct NormProblems {
     const int64_t *off, *blk, *x_bytes;
 };
 // enrolment against known speakers (vbx_enroll.cu)
-size_t enroll_workspace_bytes(int64_t M, int64_t E, int64_t max_k, int sms);
-int launch_enroll(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
-                  const int64_t *rec_off_host, int n_rec, const float *enroll_fea, int64_t N_e, const int32_t *enroll_spk,
-                  int64_t E, double c, double threshold, void *workspace, int sms, int32_t *assign_out,
-                  double *best_llr_out, double *llr_out, double *n_out, double *F_out, double *n_enroll_out,
-                  double *F_enroll_out, cudaStream_t st, const double *mean = nullptr, const double *std = nullptr,
-                  const double *enroll_mean = nullptr, const double *enroll_std = nullptr);
-// enroll_score_kernel over M scored speakers and C cohort speakers whose statistics are already in a and co: llr [M, C]
-// (and llr_out when not null), bit-identical to vbx_enroll's llr against the same speakers.  Returns 1, 0 for M == 0.
-int launch_cohort_scores(const SpeakerStats &a, const SpeakerStats &co, const float *Phi, int64_t M, int64_t C, int R,
-                         double c, double *llr, double *llr_out, cudaStream_t st);
-// The same over G problems: rows off[g] .. off[g+1]-1 of a against columns g C .. g C + C - 1 of co with c[g], flat
-// tiles tile_off [G+1] (every array DEVICE; n_tiles = tile_off[G] on the host).  Problem g's rows of llr [off[G], C]
-// are bit-identical to launch_cohort_scores on it alone.
+// enroll_score_kernel over G problems whose statistics are already in a and co: rows off[g] .. off[g+1]-1 of a against
+// columns g C .. g C + C - 1 of co with c[g], flat tiles tile_off [G+1] (every array DEVICE; n_tiles = tile_off[G] on
+// the host) into llr [off[G], C] (and llr_out when not null), bit-identical to vbx_enroll_batch's llr against the same
+// speakers.  Returns 1, 0 for n_tiles == 0.
 int launch_cohort_scores_batch(const SpeakerStats &a, const SpeakerStats &co, const float *Phi, int G,
                                const int64_t *off, const int64_t *tile_off, const double *c, int64_t n_tiles, int64_t C,
-                               int R, double *llr, cudaStream_t st);
+                               int R, double *llr, double *llr_out, cudaStream_t st);
 // score tiles of an M x C rectangle (host)
 int64_t rect_tiles(int64_t M, int64_t C);
 // dst [G, n] = G copies of src [n] (DEVICE)
@@ -357,22 +340,18 @@ int launch_enroll_batch(const float *fea, const float *Phi, int64_t N, int R, co
                         double *best_llr_out, double *llr_out, double *n_out, double *F_out, double *n_enroll_out,
                         double *F_enroll_out, cudaStream_t st, const double *mean, const double *std,
                         const double *enroll_mean, const double *enroll_std);
-// score normalisation against a cohort (vbx_cohort.cu)
-size_t cohort_workspace_bytes(int64_t M, int64_t C);
-int launch_cohort(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int64_t M,
-                  const float *cohort_fea, int64_t N_c, const int32_t *cohort_spk, int64_t C, double c, int64_t top_k,
-                  void *workspace, double *mean_out, double *std_out, double *scores_out, cudaStream_t st);
-// G problems against one cohort (vbx_cohort_stats_batch): M_host [G], c_host [G] HOST
+// score normalisation against a cohort (vbx_cohort.cu): G problems against one cohort (vbx_cohort_stats_batch),
+// M_host [G], c_host [G] HOST; scores_out [sum M, C] optional
 size_t cohort_batch_workspace_bytes(int G, const int64_t *M_host, int64_t C, int64_t N_c);
 int launch_cohort_batch(const float *fea, const float *Phi, int64_t N, int R, const int32_t *spk, int G,
                         const int64_t *M_host, const float *cohort_fea, int64_t N_c, const int32_t *cohort_spk,
                         int64_t C, const double *c_host, int64_t top_k, void *workspace, double *mean_out,
-                        double *std_out, cudaStream_t st);
-// x [rows, cols] of LLRs (link: of distances -LLR, diagonal and `skip` entries kept) replaced by the normalised scores;
-// q: several problems (NormProblems), null for one
+                        double *std_out, double *scores_out, cudaStream_t st);
+// x [rows, cols] of LLRs (link: of distances -LLR, diagonal and `skip` entries kept) replaced by the normalised scores
+// of the problems q
 int launch_norm_scores(double *x, int64_t rows, int64_t cols, const double *mean_r, const double *std_r,
                        const double *mean_c, const double *std_c, bool link, double skip, double *copy_out,
-                       cudaStream_t st, const NormProblems *q = nullptr);
+                       cudaStream_t st, const NormProblems &q);
 // wgmma projection (vbx_project_tc.cu)
 size_t tc_scratch_floats();
 int launch_project_wgmma(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,

@@ -9,15 +9,14 @@
 //   link_span_kernel    first / last x-vector of every speaker (integer atomics: order-free)
 //   link_stats_kernel   n_s, F_s (float64, fixed order), b_s and e_s; one CTA per speaker
 //   link_score_kernel   the M x M distances, 32 x 32 tiles of the upper triangle, each written twice
-//   norm_scores_kernel  (vbx_cohort.cu) only with cohort statistics (vbx_link_norm): d = -S in place, section 5.17
-//   ahc_linkage_kernel  (vbx_ahc.cu) unchanged, over the matrix as one "recording" of M items
-// Batched (vbx_link_batch, section 5.18): G independent problems over one fea / Phi, each with its own speaker index
-// [G, N], speaker_rec slice and c_g.  Their speakers are packed by the offsets off [G+1]; the statistics kernels run one
-// CTA per (problem, speaker), the score kernel's flat tile index runs over the upper-triangle tiles of all problems, and
-// one linkage launch has one CTA per problem.  vbx_link is the G = 1 case of the same kernels (LinkProblems with null
-// arrays), so a problem's results do not depend on the others.  vbx_link_batch_norm (section 5.19) adds
-// norm_scores_kernel over every problem's block, as vbx_link_norm does for one; vbx_enroll_batch and
-// vbx_cohort_stats_batch take the batched statistics through launch_speaker_stats_batch.
+//   norm_scores_kernel  (vbx_cohort.cu) only with cohort statistics (mean, std): d = -S in place, section 5.17
+//   ahc_linkage_kernel  (vbx_ahc.cu) unchanged, over each problem's matrix as one "recording" of M_g items
+// vbx_link_batch (sections 5.18, 5.19) runs G independent problems over one fea / Phi, each with its own speaker index
+// [G, N], speaker_rec slice and c_g; one archive is the batch of one.  The problems' speakers are packed by the
+// offsets off [G+1]; the statistics kernels run one CTA per (problem, speaker), the score kernel's flat tile index runs
+// over the upper-triangle tiles of all problems, norm_scores_kernel over every problem's block, and one linkage launch
+// has one CTA per problem, so a problem's results do not depend on the others.  vbx_enroll_batch and
+// vbx_cohort_stats_batch take the statistics through launch_speaker_stats_batch.
 #include <algorithm>
 #include <climits>
 #include <cstring>
@@ -38,12 +37,11 @@ struct LinkWs {
     uint8_t *lk;             // the linkage regions (carve() in vbx_ahc.cu), each D [M_g,M_g] first
     double *n, *e, *b;       // [M], [M], [M,kMaxR]  (M: the speakers of all problems)
     long long *first, *last; // [M]
-    int64_t *offs;           // the problem arrays of LinkProblems (G = 1: {0, M} and {0, 0}, the linkage's offsets and
-                             // workspace offsets)
+    int64_t *offs;           // the problem arrays of LinkProblems
 };
 
-// The problems of one call.  G = 1 with null arrays: one problem of M speakers with c = c0 (vbx_link, and the statistics
-// of vbx_enroll / vbx_cohort_stats); the kernels then read no problem arrays.
+// The problems of one call (the statistics of vbx_enroll_batch / vbx_cohort_stats_batch leave lk_off, tile_off and
+// dist_off null: they launch no score kernel).
 struct LinkProblems {
     int G;
     int64_t M, N;            // speakers of all problems; x-vectors (speaker index [G, N])
@@ -52,14 +50,13 @@ struct LinkProblems {
     const int64_t *tile_off; // [G+1] first flat score tile of each problem
     const int64_t *dist_off; // [G+1] first element of each problem's distances in dist_out
     const double *c;         // [G] Fa_g / Fb_g
-    double c0;
 };
 
 size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
 
 size_t problem_array_bytes(int64_t G) { return (size_t)(5 * G + 4) * 8; }   // off, lk_off, tile_off, dist_off, c
 
-__host__ __device__ int64_t score_tiles(int64_t M) {
+int64_t score_tiles(int64_t M) {
     const int64_t tiles = (M + 31) / 32;
     return tiles * (tiles + 1) / 2;
 }
@@ -92,12 +89,6 @@ __global__ void link_init_kernel(LinkWs w, LinkProblems p) {
         w.first[i] = LLONG_MAX;
         w.last[i] = -1;
     }
-    if (i == 0 && !p.off) {
-        w.offs[0] = 0;
-        w.offs[1] = p.M;
-        w.offs[2] = 0;
-        w.offs[3] = 0;
-    }
 }
 
 // One thread per (problem, x-vector); speaker[g, t] is a local index of problem g.
@@ -105,13 +96,7 @@ __global__ void link_span_kernel(LinkWs w, LinkProblems p, const int32_t *__rest
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (int64_t)p.G * p.N) return;
     const int s = spk[i];
-    int64_t t = i, base = 0, M = p.M;
-    if (p.off) {
-        const int64_t g = i / p.N;
-        t = i - g * p.N;
-        base = p.off[g];
-        M = p.off[g + 1] - base;
-    }
+    const int64_t g = i / p.N, t = i - g * p.N, base = p.off[g], M = p.off[g + 1] - base;
     if (s < 0 || s >= M) return;
     atomicMin(&w.first[base + s], (long long)t);
     atomicMax(&w.last[base + s], (long long)t);
@@ -129,14 +114,10 @@ __global__ void __launch_bounds__(kStatsThreads) link_stats_kernel(LinkWs w, Lin
     __shared__ double cnt[kStatsPhases];
     __shared__ double red[kStatsThreads / 32];
     const int s = blockIdx.x;
-    int ls = s;
-    double c = p.c0;
-    if (p.off) {
-        const int g = find_problem(p.off, p.G, s);
-        ls = s - (int)p.off[g];
-        spk += (int64_t)g * p.N;
-        c = p.c[g];
-    }
+    const int g = find_problem(p.off, p.G, s);
+    const int ls = s - (int)p.off[g];
+    const double c = p.c[g];
+    spk += (int64_t)g * p.N;
     const int k = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long f = w.first[s], l = w.last[s];
     double acc[kMaxR / 32] = {0, 0, 0, 0};
@@ -260,40 +241,26 @@ __device__ __forceinline__ void score_tile(const LinkWs &w, const float *__restr
 __global__ void __launch_bounds__(256) link_score_kernel(LinkWs w, LinkProblems p, const float *__restrict__ Phi,
                                                          const int32_t *__restrict__ spk_rec, int R,
                                                          double *__restrict__ dist_out) {
-    const int64_t all = p.tile_off ? p.tile_off[p.G] : score_tiles(p.M);
-    for (int64_t t = blockIdx.x; t < all; t += gridDim.x) {
+    for (int64_t t = blockIdx.x; t < p.tile_off[p.G]; t += gridDim.x) {
+        const int g = find_problem(p.tile_off, p.G, t);
+        const int64_t base = p.off[g], M = p.off[g + 1] - base, lt = t - p.tile_off[g];
         LinkWs wg = w;
-        int64_t M = p.M, lt = t, base = 0;
-        double c = p.c0, *dist = dist_out;
-        if (p.tile_off) {
-            const int g = find_problem(p.tile_off, p.G, t);
-            base = p.off[g];
-            M = p.off[g + 1] - base;
-            lt = t - p.tile_off[g];
-            c = p.c[g];
-            wg.lk += p.lk_off[g];
-            wg.n += base;
-            wg.e += base;
-            wg.b += base * kMaxR;
-            if (dist) dist += p.dist_off[g];
-        }
+        wg.lk += p.lk_off[g];
+        wg.n += base;
+        wg.e += base;
+        wg.b += base * kMaxR;
+        double *dist = dist_out ? dist_out + p.dist_off[g] : nullptr;
         const int64_t tiles = (M + 31) / 32;
         const double tt = 2.0 * (double)tiles + 1.0;
         auto row0 = [tiles](int64_t b) { return b * tiles - b * (b - 1) / 2; };   // first tile of row b
         int64_t bi = (int64_t)((tt - sqrt(tt * tt - 8.0 * (double)lt)) / 2.0);   // row0 inverted, then rounding corrected
         while (bi > 0 && row0(bi) > lt) --bi;
         while (bi + 1 < tiles && row0(bi + 1) <= lt) ++bi;
-        score_tile(wg, Phi, spk_rec + base, M, R, c, dist, bi, bi + (lt - row0(bi)));
+        score_tile(wg, Phi, spk_rec + base, M, R, p.c[g], dist, bi, bi + (lt - row0(bi)));
     }
 }
 
 }  // namespace
-
-size_t link_workspace_bytes(int64_t M) {
-    size_t total = 0;
-    link_layout(nullptr, al(linkage_workspace_bytes(M)), M, 1, &total);
-    return total;
-}
 
 size_t link_batch_workspace_bytes(int G, const int64_t *M_host, std::vector<int64_t> *lk_off) {
     size_t lk = 0, total = 0;
@@ -311,10 +278,10 @@ size_t link_batch_workspace_bytes(int G, const int64_t *M_host, std::vector<int6
 
 namespace {
 
-// The statistics (and, with Z_out or dist_out, the distances) of the problems p over the workspace w.
+// The statistics (and, with n_tiles > 0 score tiles, the distances) of the problems p over the workspace w.
 int launch_problems(const LinkWs &w, const LinkProblems &p, int64_t n_tiles, const float *fea, const float *Phi,
                     const int32_t *spk, int R, const int32_t *spk_rec, double *n_out, double *F_out, double *dist_out,
-                    bool score, cudaStream_t st) {
+                    cudaStream_t st) {
     int launches = 2;
     link_init_kernel<<<(unsigned)((p.M + 255) / 256), 256, 0, st>>>(w, p);
     if (p.N > 0) {
@@ -322,7 +289,7 @@ int launch_problems(const LinkWs &w, const LinkProblems &p, int64_t n_tiles, con
         ++launches;
     }
     link_stats_kernel<<<(unsigned)p.M, kStatsThreads, 0, st>>>(w, p, fea, Phi, spk, R, n_out, F_out);
-    if (score && n_tiles > 0) {
+    if (n_tiles > 0) {
         link_score_kernel<<<(unsigned)std::min<int64_t>(n_tiles, kScoreGrid), 256, 0, st>>>(w, p, Phi, spk_rec, R,
                                                                                            dist_out);
         ++launches;
@@ -330,38 +297,7 @@ int launch_problems(const LinkWs &w, const LinkProblems &p, int64_t n_tiles, con
     return launches;
 }
 
-LinkProblems single(int64_t M, int64_t N, double c) {
-    LinkProblems p;
-    p.G = 1;
-    p.M = M;
-    p.N = N;
-    p.off = p.lk_off = p.tile_off = p.dist_off = nullptr;
-    p.c = nullptr;
-    p.c0 = c;
-    return p;
-}
-
 }  // namespace
-
-int launch_link(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
-                int64_t M, double c, void *workspace, double *n_out, double *F_out, double *dist_out, double *Z_out,
-                cudaStream_t st, const double *mean, const double *std) {
-    if (M == 0) return 0;
-    const LinkWs w = link_layout(reinterpret_cast<uint8_t *>(workspace), al(linkage_workspace_bytes(M)), M, 1, nullptr);
-    int launches = launch_problems(w, single(M, N, c), score_tiles(M), fea, Phi, spk, R, spk_rec, n_out, F_out,
-                                   mean ? nullptr : dist_out, true, st);
-    if (mean) {                                       // normalised distances (section 5.17): dist_out gets those
-        const int ln = launch_norm_scores(reinterpret_cast<double *>(w.lk), M, M, mean, std, mean, std, true, kBig,
-                                          dist_out, st);
-        if (ln < 0) return -1;
-        launches += ln;
-    }
-    if (M >= 2) {
-        launch_linkage(w.offs, w.offs + 2, 1, w.lk, Z_out, st);
-        ++launches;
-    }
-    return cudaGetLastError() == cudaSuccess ? launches : -1;
-}
 
 int launch_link_batch(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, const int32_t *spk_rec,
                       int G, const int64_t *M_host, const double *c_host, void *workspace, double *n_out,
@@ -395,13 +331,12 @@ int launch_link_batch(const float *fea, const float *Phi, const int32_t *spk, in
     p.tile_off = w.offs + 2 * (G + 1);
     p.dist_off = w.offs + 3 * (G + 1);
     p.c = reinterpret_cast<const double *>(w.offs + 4 * (G + 1));
-    p.c0 = 0.0;
     int launches = launch_problems(w, p, tile[G], fea, Phi, spk, R, spk_rec, n_out, F_out, mean ? nullptr : dist_out,
-                                   true, st);
-    if (mean) {                                       // vbx_link_batch_norm: each problem's block as vbx_link_norm's
+                                   st);
+    if (mean) {                                       // normalised distances (section 5.17): dist_out gets those
         const NormProblems q{G, p.off, p.dist_off, p.lk_off};
         const int ln = launch_norm_scores(reinterpret_cast<double *>(w.lk), dist[G], 1, mean, std, mean, std, true,
-                                          kBig, dist_out, st, &q);
+                                          kBig, dist_out, st, q);
         if (ln < 0) return -1;
         launches += ln;
     }
@@ -409,22 +344,6 @@ int launch_link_batch(const float *fea, const float *Phi, const int32_t *spk, in
         launch_linkage(p.off, p.lk_off, G, w.lk, Z_out, st);
         ++launches;
     }
-    return cudaGetLastError() == cudaSuccess ? launches : -1;
-}
-
-int launch_speaker_stats(const float *fea, const float *Phi, const int32_t *spk, int64_t N, int R, int64_t M, double c,
-                         const SpeakerStats &s, double *n_out, double *F_out, cudaStream_t st) {
-    if (M == 0) return 0;
-    LinkWs w;
-    w.lk = nullptr;
-    w.n = s.n;
-    w.e = s.e;
-    w.b = s.b;
-    w.first = s.first;
-    w.last = s.last;
-    w.offs = s.offs;
-    const int launches = launch_problems(w, single(M, N, c), 0, fea, Phi, spk, R, nullptr, n_out, F_out, nullptr, false,
-                                         st);
     return cudaGetLastError() == cudaSuccess ? launches : -1;
 }
 
@@ -439,7 +358,7 @@ int launch_speaker_stats_batch(const float *fea, const float *Phi, const int32_t
     w.b = s.b;
     w.first = s.first;
     w.last = s.last;
-    w.offs = s.offs;
+    w.offs = nullptr;
     LinkProblems p;
     p.G = G;
     p.M = M;
@@ -447,8 +366,7 @@ int launch_speaker_stats_batch(const float *fea, const float *Phi, const int32_t
     p.off = off;
     p.lk_off = p.tile_off = p.dist_off = nullptr;
     p.c = c;
-    p.c0 = 0.0;
-    const int launches = launch_problems(w, p, 0, fea, Phi, spk, R, nullptr, n_out, F_out, nullptr, false, st);
+    const int launches = launch_problems(w, p, 0, fea, Phi, spk, R, nullptr, n_out, F_out, nullptr, st);
     return cudaGetLastError() == cudaSuccess ? launches : -1;
 }
 

@@ -2,16 +2,16 @@
 
 Each recording's VB-HMM numbers its speakers 1..K.  Enrolment names them: every archive speaker (section 5.15's table)
 is scored against every enrolled speaker with section 5.15's same-speaker LLR, and each recording's speakers are
-assigned one-to-one to enrolled speakers, or to "unknown", by a minimum-cost assignment on the device (vbx_enroll).  A
-speaker takes an enrolled name only where its LLR reaches the threshold, two speakers of one recording never share a
-name, and the sum of LLR - threshold over the named speakers is the largest possible.
+assigned one-to-one to enrolled speakers, or to "unknown", by a minimum-cost assignment on the device
+(vbx_enroll_batch).  A speaker takes an enrolled name only where its LLR reaches the threshold, two speakers of one
+recording never share a name, and the sum of LLR - threshold over the named speakers is the largest possible.
 """
 import ctypes
 from collections import namedtuple
 
 import numpy as np
 
-from .link import speaker_index, speaker_table
+from .link import speaker_table, table_index
 
 UNKNOWN = 'unknown-'       # prefix of the names of speakers that match no enrolled speaker (reserved)
 MAX_THRESHOLD = 1e15
@@ -54,17 +54,14 @@ def check_enrolment(enroll, dim):
 def enroll_speakers(fea, Phi, offsets, labels, enroll_fea, enroll_speaker, Fa, Fb, threshold, device=None, llr=False,
                     max_bytes=2 ** 31, norm=None):
     """Statistics, LLRs and the per-recording assignment of every archive speaker against the enrolled speakers on the
-    device (vbx_enroll).  fea [N,R], Phi [R]: the features the VB-HMM ran with, packed by recording at offsets [B+1];
-    labels: each recording's final first labels.  enroll_fea [N_e,R]: the enrolled x-vectors through the same front
-    end; enroll_speaker [N_e]: their speaker in [0, E), every speaker with at least one x-vector.  Archives whose M x E
-    LLR block exceeds max_bytes are split into chunks of whole recordings, one vbx_enroll call each (the results are
-    the same bits).  norm: None, or (mean [M], std [M], enroll_mean [E], enroll_std [E]) of the archive and enrolled
-    speakers' cohort scores (cohort.cohort_stats): the assignment then runs on the normalised scores S of DESIGN.md
-    section 5.17 with the threshold on S (vbx_enroll_norm), and best_llr and llr hold S.
+    device (vbx_enroll_batch on a batch of one).  fea [N,R], Phi [R]: the features the VB-HMM ran with, packed by
+    recording at offsets [B+1]; labels: each recording's final first labels.  enroll_fea [N_e,R]: the enrolled
+    x-vectors through the same front end; enroll_speaker [N_e]: their speaker in [0, E), every speaker with at least one
+    x-vector.  Archives whose M x E LLR block exceeds max_bytes are split into chunks of whole recordings, one
+    enroll_many call each (the results are the same bits).  norm: None, or (mean [M], std [M], enroll_mean [E],
+    enroll_std [E]) of the archive and enrolled speakers' cohort scores (cohort.cohort_stats): the assignment then runs
+    on the normalised scores S of DESIGN.md section 5.17 with the threshold on S, and best_llr and llr hold S.
     Returns EnrollResult (numpy, speaker_table order), with llr [M,E] when llr=True."""
-    import torch
-    from . import _lib
-    from ._lib import VbxError
     t = check_threshold(threshold)
     offsets = np.asarray(offsets, dtype=np.int64)
     espk = np.asarray(enroll_speaker, dtype=np.int64).reshape(-1)
@@ -75,21 +72,13 @@ def enroll_speakers(fea, Phi, offsets, labels, enroll_fea, enroll_speaker, Fa, F
         raise ValueError('every enrolled speaker 0 .. E-1 needs at least one x-vector')
     table = speaker_table(labels)
     M, B = len(table.rec), len(labels)
-    if not torch.cuda.is_available():
-        raise VbxError('enroll_speakers(): no CUDA device - vbx_b200 has no CPU fallback')
-    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
-    if dev.index is None:
-        dev = torch.device('cuda', torch.cuda.current_device())
-    fea = torch.as_tensor(fea).to(dev, torch.float32).contiguous()
-    Phi = torch.as_tensor(Phi).to(dev, torch.float32).contiguous()
-    efea = torch.as_tensor(enroll_fea).to(dev, torch.float32).contiguous()
-    N, R = int(fea.shape[0]), int(fea.shape[1])
-    if int(offsets[-1]) != N or len(offsets) != B + 1:
+    if int(offsets[-1]) != int(fea.shape[0]) or len(offsets) != B + 1:
         raise ValueError('offsets must hold one more entry than labels and end at the number of x-vectors')
-    if tuple(efea.shape) != (len(espk), R):
-        raise ValueError(f'enroll_fea must be [{len(espk)}, {R}], got {tuple(efea.shape)}')
+    if norm is not None:
+        norm = [np.asarray(a, dtype=np.float64) for a in norm]
+        if [a.shape for a in norm] != [(M,), (M,), (E,), (E,)]:
+            raise ValueError(f'norm must hold mean and std of the {M} archive and the {E} enrolled speakers')
     first = np.searchsorted(table.rec, np.arange(B + 1)).astype(np.int64)     # each recording's first speaker
-    spk = speaker_index(offsets, labels)[0]
     # chunks of whole recordings with at most max_bytes of LLRs (a recording alone may exceed it)
     chunks, b0 = [], 0
     for b in range(B):
@@ -97,57 +86,15 @@ def enroll_speakers(fea, Phi, offsets, labels, enroll_fea, enroll_speaker, Fa, F
             chunks.append((b0, b))
             b0 = b
     chunks.append((b0, B))
-    k_max = int(np.diff(first).max()) if B else 0
-    m_max = max(int(first[b1] - first[a]) for a, b1 in chunks)
-    lib = _lib.load()
-    h = ctypes.c_void_p()
-    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
-        raise VbxError('vbx_create failed: no usable sm_90 device')
-    at = lambda x, off=0: ctypes.c_void_p(x.data_ptr() + off * x.element_size()) if x is not None else None
-    try:
-        need = ctypes.c_size_t()
-        if lib.vbx_enroll_workspace_bytes(h, m_max, E, k_max, ctypes.byref(need)) != 0:
-            raise VbxError(f'vbx_enroll_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
-        with torch.cuda.device(dev):
-            ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=dev)
-            espk_d = torch.from_numpy(espk.astype(np.int32)).to(dev)
-            assign = torch.empty(M, dtype=torch.int32, device=dev)
-            best = torch.empty(M, dtype=torch.float64, device=dev)
-            n = torch.empty(M, dtype=torch.float64, device=dev)
-            F = torch.empty((M, R), dtype=torch.float64, device=dev)
-            n_e = torch.empty(E, dtype=torch.float64, device=dev)
-            F_e = torch.empty((E, R), dtype=torch.float64, device=dev)
-            L = torch.empty((M, E), dtype=torch.float64, device=dev) if llr else None
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            if norm is not None:
-                stats = [torch.as_tensor(np.asarray(a, dtype=np.float64)).to(dev).contiguous() for a in norm]
-                if [tuple(s.shape) for s in stats] != [(M,), (M,), (E,), (E,)]:
-                    raise ValueError(f'norm must hold mean and std of the {M} archive and the {E} enrolled speakers')
-            keep = []
-            for ci, (a, z) in enumerate(chunks):
-                s0, x0, x1 = int(first[a]), int(offsets[a]), int(offsets[z])
-                sp = spk[x0:x1]
-                spk_d = torch.from_numpy(np.where(sp >= 0, sp - s0, -1).astype(np.int32)).to(dev)
-                rec_off = np.ascontiguousarray(first[a:z + 1] - s0, dtype=np.int64)
-                keep.append(spk_d)
-                args = (h, at(fea, x0 * R), at(Phi), x1 - x0, R, at(spk_d), int(first[z]) - s0,
-                        rec_off.ctypes.data_as(ctypes.c_void_p), z - a, at(efea), len(espk), at(espk_d), E,
-                        float(Fa), float(Fb), t, at(ws), ws.numel(), at(assign, s0), at(best, s0),
-                        at(L, s0 * E), at(n, s0), at(F, s0 * R), at(n_e) if ci == 0 else None,
-                        at(F_e) if ci == 0 else None)
-                if norm is None:
-                    rc = lib.vbx_enroll(*args, stream)
-                else:
-                    rc = lib.vbx_enroll_norm(*args, at(stats[0], s0), at(stats[1], s0), at(stats[2]), at(stats[3]),
-                                             stream)
-                if rc != 0:
-                    raise VbxError(f'vbx_enroll failed ({rc}): {lib.vbx_last_error(h).decode()}')
-            out = EnrollResult(table, assign.cpu().numpy().astype(np.int64), best.cpu().numpy(), n.cpu().numpy(),
-                               F.cpu().numpy(), n_e.cpu().numpy(), F_e.cpu().numpy(),
-                               L.cpu().numpy() if llr else None)
-    finally:
-        lib.vbx_destroy(h)
-    return out
+    parts = []
+    for a, z in chunks:
+        s0, s1, x0 = int(first[a]), int(first[z]), int(offsets[a])
+        nm = None if norm is None else [(norm[0][s0:s1], norm[1][s0:s1], norm[2], norm[3])]
+        parts += enroll_many(fea[x0:int(offsets[z])], Phi, offsets[a:z + 1] - x0, [labels[a:z]], enroll_fea, espk,
+                             Fa, Fb, [t], device=device, llr=llr, norm=nm)
+    cat = lambda f: np.concatenate([f(r) for r in parts])
+    return EnrollResult(table, cat(lambda r: r.assign[0]), cat(lambda r: r.best_llr[0]), cat(lambda r: r.n),
+                        cat(lambda r: r.F), parts[0].n_enroll, parts[0].F_enroll, cat(lambda r: r.llr) if llr else None)
 
 
 def check_thresholds(thresholds):
@@ -234,7 +181,7 @@ def enroll_many(fea, Phi, offsets, labels_per_problem, enroll_fea, enroll_speake
                 M_h = np.ascontiguousarray(Ms[idx])
                 tot, Gb = int(M_h.sum()), len(idx)
                 ws = torch.empty(max(ws_bytes(idx), 1), dtype=torch.uint8, device=dev)
-                spk = np.stack([speaker_index(offsets, labels_per_problem[g])[0] for g in idx]).astype(np.int32)
+                spk = np.stack([table_index(offsets, labels_per_problem[g], tables[g]) for g in idx]).astype(np.int32)
                 spk_d = torch.from_numpy(spk).to(dev)
                 rec_off = np.ascontiguousarray(np.stack([firsts[g] for g in idx]))
                 fa, fb = np.ascontiguousarray(Fa[idx]), np.ascontiguousarray(Fb[idx])

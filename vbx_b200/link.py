@@ -41,8 +41,13 @@ def check_threshold(threshold):
 def speaker_index(offsets, labels):
     """(speaker [N] int64, M): the speaker_table index of every x-vector (-1 where its label is negative) of the
     recordings packed at offsets [B+1] with first labels `labels`."""
-    offsets = np.asarray(offsets, dtype=np.int64)
     table = speaker_table(labels)
+    return table_index(offsets, labels, table), len(table.rec)
+
+
+def table_index(offsets, labels, table):
+    """speaker_index's speaker [N] with table = speaker_table(labels) already at hand."""
+    offsets = np.asarray(offsets, dtype=np.int64)
     if len(offsets) != len(labels) + 1:
         raise ValueError('offsets must hold one more entry than labels')
     spk = np.full(int(offsets[-1]), -1, dtype=np.int64)
@@ -53,72 +58,19 @@ def speaker_index(offsets, labels):
             raise ValueError(f'recording {b}: {len(l)} labels for {offsets[b + 1] - offsets[b]} x-vectors')
         own = table.label[first[b]:first[b + 1]]
         spk[offsets[b]:offsets[b + 1]] = np.where(l >= 0, first[b] + np.searchsorted(own, l), -1)
-    return spk, len(table.rec)
+    return spk
 
 
 def link_speakers(fea, Phi, offsets, labels, Fa, Fb, device=None, dist=False, norm=None):
-    """Statistics, pairwise scores and average linkage of every speaker of an archive on the device (vbx_link).
-    fea [N,R] and Phi [R]: the features the VB-HMM ran with (CUDA tensors or arrays, float32), packed by recording at
-    offsets [B+1]; labels: the final first labels of each recording; Fa, Fb: the VB-HMM's scalars.
+    """Statistics, pairwise scores and average linkage of every speaker of an archive on the device (vbx_link_batch on a
+    batch of one).  fea [N,R] and Phi [R]: the features the VB-HMM ran with (CUDA tensors or arrays, float32), packed
+    by recording at offsets [B+1]; labels: the final first labels of each recording; Fa, Fb: the VB-HMM's scalars.
     norm: None, or (mean [M], std [M]) of the speakers' cohort scores (cohort.cohort_stats over the same speakers):
-    the distances are then -S, the normalised scores of DESIGN.md section 5.17 (vbx_link_norm).
+    the distances are then -S, the normalised scores of DESIGN.md section 5.17.
     Returns (table, n [M], F [M,R], Z [M-1,4]) as numpy float64 (speaker_table order), and dist [M,M] with dist=True.
     ValueError when the archive has more speakers than the linkage kernel indexes."""
-    import torch
-    from . import _lib
-    from ._lib import VbxError
-    offsets = np.asarray(offsets, dtype=np.int64)
-    table = speaker_table(labels)
-    M = len(table.rec)
-    if M > _lib.LINK_MAX_SPEAKERS:
-        raise ValueError(f'{M} speakers to link: at most {_lib.LINK_MAX_SPEAKERS} are supported (the workspace would '
-                         f'need more than {8 * M * M} bytes)')
-    if not torch.cuda.is_available():
-        raise VbxError('link_speakers(): no CUDA device - vbx_b200 has no CPU fallback')
-    dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
-    if dev.index is None:
-        dev = torch.device('cuda', torch.cuda.current_device())
-    fea = torch.as_tensor(fea).to(dev, torch.float32).contiguous()
-    Phi = torch.as_tensor(Phi).to(dev, torch.float32).contiguous()
-    N, R = int(fea.shape[0]), int(fea.shape[1])
-    if int(offsets[-1]) != N or len(offsets) != len(labels) + 1:
-        raise ValueError('offsets must hold one more entry than labels and end at the number of x-vectors')
-    spk = speaker_index(offsets, labels)[0].astype(np.int32)
-    lib = _lib.load()
-    h = ctypes.c_void_p()
-    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
-        raise VbxError('vbx_create failed: no usable sm_90 device')
-    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
-    try:
-        need = ctypes.c_size_t()
-        if lib.vbx_link_workspace_bytes(h, M, ctypes.byref(need)) != 0:
-            raise VbxError(f'vbx_link_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
-        with torch.cuda.device(dev):
-            ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=dev)
-            spk_d = torch.from_numpy(spk).to(dev)
-            rec_d = torch.from_numpy(table.rec.astype(np.int32)).to(dev)
-            n = torch.empty(M, dtype=torch.float64, device=dev)
-            F = torch.empty((M, R), dtype=torch.float64, device=dev)
-            D = torch.empty((M, M), dtype=torch.float64, device=dev) if dist else None
-            Z = torch.empty((max(M - 1, 0), 4), dtype=torch.float64, device=dev)
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            if norm is None:
-                rc = lib.vbx_link(h, p(fea), p(Phi), N, R, p(spk_d), M, p(rec_d), float(Fa), float(Fb), p(ws),
-                                  ws.numel(), p(n), p(F), p(D), p(Z), stream)
-            else:
-                mean, std = (torch.as_tensor(np.asarray(a, dtype=np.float64)).to(dev).contiguous() for a in norm)
-                if mean.shape != (M,) or std.shape != (M,):
-                    raise ValueError(f'norm must hold mean and std of the {M} speakers')
-                rc = lib.vbx_link_norm(h, p(fea), p(Phi), N, R, p(spk_d), M, p(rec_d), float(Fa), float(Fb), p(ws),
-                                       ws.numel(), p(n), p(F), p(D), p(Z), p(mean), p(std), stream)
-            if rc != 0:
-                raise VbxError(f'vbx_link failed ({rc}): {lib.vbx_last_error(h).decode()}')
-            out = (table, n.cpu().numpy(), F.cpu().numpy(), Z.cpu().numpy())
-            if dist:
-                out += (D.cpu().numpy(),)
-    finally:
-        lib.vbx_destroy(h)
-    return out
+    return link_many(fea, Phi, offsets, [labels], Fa, Fb, device=device, dist=dist,
+                     norm=None if norm is None else [norm])[0]
 
 
 def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_bytes=None, dist=False, norm=None):
@@ -126,9 +78,9 @@ def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_by
     section 5.18), e.g. the final labels of every setting of a sweep.  fea, Phi, offsets: as for link_speakers;
     labels_per_problem: G lists of first labels per recording; Fa, Fb: numbers or G values, problem g's scalars.
     The problems are packed in order into launches whose workspaces stay within max_bytes (None: one launch), each
-    problem sized by vbx_link_workspace_bytes (sweep.pack: a problem larger than max_bytes on its own raises ValueError).
-    norm: None, or per problem (mean [M_g], std [M_g]) of its speakers' cohort scores (cohort.cohort_stats_many): the
-    distances are then -S as link_speakers(norm=) computes them (vbx_link_batch_norm, DESIGN.md section 5.19).
+    problem sized by vbx_link_batch_workspace_bytes on it alone (sweep.pack: a problem larger than max_bytes on its own
+    raises ValueError).  norm: None, or per problem (mean [M_g], std [M_g]) of its speakers' cohort scores
+    (cohort.cohort_stats_many): the distances are then -S (DESIGN.md sections 5.17, 5.19).
     Returns one (table, n, F, Z) per problem (with dist=True also dist [M,M]), bit-identical to link_speakers on that
     problem alone (with the same norm)."""
     import torch
@@ -142,7 +94,8 @@ def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_by
     Ms = [len(t.rec) for t in tables]
     for g, M in enumerate(Ms):
         if M > _lib.LINK_MAX_SPEAKERS:
-            raise ValueError(f'problem {g}: {M} speakers to link: at most {_lib.LINK_MAX_SPEAKERS} are supported')
+            raise ValueError(f'problem {g}: {M} speakers to link: at most {_lib.LINK_MAX_SPEAKERS} are supported (the '
+                             f'workspace would need more than {8 * M * M} bytes)')
     if not torch.cuda.is_available():
         raise VbxError('link_many(): no CUDA device - vbx_b200 has no CPU fallback')
     dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
@@ -165,13 +118,14 @@ def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_by
     p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
     out = [None] * G
     try:
-        sizes = []
-        for M in Ms:
+        def ws_bytes(M_h):
             need = ctypes.c_size_t()
-            if lib.vbx_link_workspace_bytes(h, M, ctypes.byref(need)) != 0:
-                raise VbxError(f'vbx_link_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
-            sizes.append(int(need.value))
-        batches = [list(range(G))] if max_bytes is None else pack(sizes, max_bytes)
+            if lib.vbx_link_batch_workspace_bytes(h, len(M_h), M_h.ctypes.data_as(ctypes.c_void_p),
+                                                  ctypes.byref(need)) != 0:
+                raise VbxError(f'vbx_link_batch_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
+            return int(need.value)
+        batches = [list(range(G))] if max_bytes is None else \
+            pack([ws_bytes(np.array([M], dtype=np.int64)) for M in Ms], max_bytes)
         with torch.cuda.device(dev):
             stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             for idx in batches:
@@ -179,28 +133,22 @@ def link_many(fea, Phi, offsets, labels_per_problem, Fa, Fb, device=None, max_by
                     continue
                 M_h = np.array([Ms[g] for g in idx], dtype=np.int64)
                 tot = int(M_h.sum())
-                spk = np.stack([speaker_index(offsets, labels_per_problem[g])[0] for g in idx]).astype(np.int32)
+                spk = np.stack([table_index(offsets, labels_per_problem[g], tables[g]) for g in idx]).astype(np.int32)
                 rec = np.concatenate([tables[g].rec for g in idx]).astype(np.int32)
                 fa, fb = np.ascontiguousarray(Fa[idx]), np.ascontiguousarray(Fb[idx])
-                need = ctypes.c_size_t()
-                if lib.vbx_link_batch_workspace_bytes(h, len(idx), M_h.ctypes.data_as(ctypes.c_void_p),
-                                                      ctypes.byref(need)) != 0:
-                    raise VbxError(f'vbx_link_batch_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
-                ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=dev)
+                ws = torch.empty(max(ws_bytes(M_h), 1), dtype=torch.uint8, device=dev)
                 spk_d = torch.from_numpy(spk).to(dev)
                 rec_d = torch.from_numpy(rec).to(dev)
                 n = torch.empty(tot, dtype=torch.float64, device=dev)
                 F = torch.empty((tot, R), dtype=torch.float64, device=dev)
                 D = torch.empty(int((M_h * M_h).sum()), dtype=torch.float64, device=dev) if dist else None
                 Z = torch.empty((tot, 4), dtype=torch.float64, device=dev)
-                args = (h, p(fea), p(Phi), N, R, len(idx), p(spk_d), M_h.ctypes.data_as(ctypes.c_void_p), p(rec_d),
-                        fa.ctypes.data_as(ctypes.c_void_p), fb.ctypes.data_as(ctypes.c_void_p), p(ws), ws.numel(), p(n),
-                        p(F), p(D), p(Z))
-                if norm is None:
-                    rc = lib.vbx_link_batch(*args, stream)
-                else:
+                mean = std = None
+                if norm is not None:
                     mean, std = (torch.from_numpy(np.concatenate([norm[g][k] for g in idx])).to(dev) for k in (0, 1))
-                    rc = lib.vbx_link_batch_norm(*args, p(mean), p(std), stream)
+                rc = lib.vbx_link_batch(h, p(fea), p(Phi), N, R, len(idx), p(spk_d), M_h.ctypes.data_as(ctypes.c_void_p),
+                                        p(rec_d), fa.ctypes.data_as(ctypes.c_void_p), fb.ctypes.data_as(ctypes.c_void_p),
+                                        p(ws), ws.numel(), p(n), p(F), p(D), p(Z), p(mean), p(std), stream)
                 if rc != 0:
                     raise VbxError(f'vbx_link_batch failed ({rc}): {lib.vbx_last_error(h).decode()}')
                 n, F, Z = n.cpu().numpy(), F.cpu().numpy(), Z.cpu().numpy()
