@@ -77,7 +77,9 @@ const char *vbx_last_error(vbx_handle_t h);
  * any failure to capture, launches the kernels directly.  Off while "timing" is on.
  * Tuning knobs: "fb_states_per_lane" (0 = auto, 1, 2, 4; at S = 64 values below 2 and at S = 128 values below 4 are
  * raised to those, since a recording's lane group must fit in a warp), "fb_classic" (forward-backward sweep: 0 = one-step
- * look-ahead recurrences, 1 = normalise-every-frame), "projection" (0 = auto, 1 = FFMA tiles,
+ * look-ahead recurrences, 1 = normalise-every-frame), "fb_ring" (look-ahead sweep fed from shared-memory rings by bulk
+ * copies that recomputes the forward variables from checkpoints instead of parking them in gamma: 1 = default, used when
+ * no recording of the plan exceeds 2048 frames; 0 = register bursts; results are bit-identical), "projection" (0 = auto, 1 = FFMA tiles,
  * 2 = wgmma 3xTF32), "gemm" (in-loop contractions: 0 = tensor cores in split-precision 3xTF32, 1 = FFMA),
  * "timing" (0/1, see vbx_get_timings).  Unknown names return VBX_ERR_ARG. */
 int vbx_set_option(vbx_handle_t h, const char *name, int32_t value);

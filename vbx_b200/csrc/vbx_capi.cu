@@ -25,6 +25,7 @@ struct vbx_handle_s {
     void *plan_mem = nullptr;  // one device allocation backing all plan arrays
     int opt_fb_spl = 0;
     int opt_fb_classic = 0;  // 1 = the normalise-every-frame sweep, 0 = one-step look-ahead
+    int opt_fb_ring = 1;     // look-ahead sweep fed from shared-memory rings (1) or from register bursts (0)
     int opt_projection = 0;
     int opt_timing = 0;
     int opt_gemm = 0;  // 0 = mma.sync 3xTF32, 1 = FFMA
@@ -260,6 +261,10 @@ int vbx_set_option(vbx_handle_t h, const char *name, int32_t value) {
     }
     if (!strcmp(name, "fb_classic")) {
         h->opt_fb_classic = value ? 1 : 0;
+        return VBX_OK;
+    }
+    if (!strcmp(name, "fb_ring")) {
+        h->opt_fb_ring = value ? 1 : 0;
         return VBX_OK;
     }
     if (!strcmp(name, "gemm")) {
@@ -684,7 +689,7 @@ static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *
             {
                 cudaStream_t fs = fb_hi ? h->hi_stream : st;
                 Timed t(h, fs, VBX_K_FWDBWD);
-                rc = counted(h, vbx::launch_forward_backward(pl, h->ws, rp, gamma_io, pi_io, n_states, Li_out, n_iters_out, flags_out, it, h->opt_fb_spl, h->opt_fb_classic, fs), "forward_backward");
+                rc = counted(h, vbx::launch_forward_backward(pl, h->ws, rp, gamma_io, pi_io, n_states, Li_out, n_iters_out, flags_out, it, h->opt_fb_spl, h->opt_fb_classic, h->opt_fb_ring, fs), "forward_backward");
             }
             if (fb_hi) {
                 cudaEventRecord(h->ev_join, h->hi_stream);

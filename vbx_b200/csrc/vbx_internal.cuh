@@ -182,6 +182,38 @@ __device__ __forceinline__ void st_vec<4>(float *p, const float *v) {
     *reinterpret_cast<float4 *>(p) = make_float4(v[0], v[1], v[2], v[3]);
 }
 
+// mbarrier and bulk-copy (cp.async.bulk) primitives of the shared-memory pipelines (vbx_project_tc.cu, vbx_kernels.cu)
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+// raise the expected transaction bytes of the current phase without arriving
+__device__ __forceinline__ void mbar_add_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "WAIT_%=:\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+        "@p bra DONE_%=;\n\t"
+        "bra WAIT_%=;\n\t"
+        "DONE_%=:\n\t}" ::"r"(bar),
+        "r"(parity)
+        : "memory");
+}
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
+                 "l"(src), "r"(bytes), "r"(bar)
+                 : "memory");
+}
+
 // The problem g whose range [pref[g], pref[g+1]) holds x, for non-decreasing pref with pref[0] = 0 <= x < pref[G]:
 // the largest g with pref[g] <= x (never an empty problem's, whose range is empty).  The batched speaker kernels
 // (vbx_link_batch, vbx_enroll_batch, vbx_cohort_stats_batch) decode their flat indices with it.
@@ -214,7 +246,7 @@ int launch_loglik(const Plan &pl, const Workspace &ws, const float *rho, const f
                   cudaStream_t st);
 int launch_forward_backward(const Plan &pl, const Workspace &ws, const RunParams &rp, float *gamma, float *pi,
                             const int32_t *n_states, double *Li, int32_t *n_iters, int32_t *flags, int iter,
-                            int spl, int classic, cudaStream_t st);
+                            int spl, int classic, int ring, cudaStream_t st);
 int launch_elbo_trace(const Plan &pl, const double *Li, int max_iters, double *out, cudaStream_t st);
 // forward and backward sweeps on separate warps + combine pass, any recording length (vbx_fb_split.cu)
 int launch_forward_backward_split(const Plan &pl, const Workspace &ws, const RunParams &rp, float *gamma, float *pi,

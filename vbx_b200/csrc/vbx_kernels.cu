@@ -1281,16 +1281,450 @@ __global__ void __launch_bounds__(128) forward_backward_la_kernel(Plan pl, Works
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// The look-ahead sweep above, fed from shared-memory rings instead of register bursts, and without parking every forward
+// variable in HBM.
+//
+// The sweep is bound by HBM bandwidth (332 B per frame against ~12 flop per state for the kernel above).  Two changes:
+// * Every warp owns a ring of kStages stages in shared memory; lane 0 of each recording group fills a stage with
+//   cp.async.bulk copies of its recording's contiguous row ranges (completing on the stage's mbarrier by transaction
+//   bytes), kStages - 1 stages ahead of the steps that read it, so the prefetch depth no longer depends on registers.
+// * The forward sweep stores a_t only for t = T-1 (it is gamma_{T-1}).  At the first frame of every backward stage it
+//   stores the recurrence state instead (y, Y, q, c, r_s, r_{s+1}: three gamma rows of that stage), and the backward
+//   sweep recomputes the stage's F forward variables from it with the forward sweep's own operations (fwd_step), from
+//   the p rows it reads anyway.  Per frame that drops the write and the read of a_t (128 B) for ~20 B of checkpoints.
+// Stage u holds
+//   forward:  p rows of frames 2 + u FF ... 2 + u FF + FF - 1 (the `pn` operands of steps u FF ...),
+//   backward: p rows of frames lo .. lo+F-1 (lo = T-1-(u+1)F, the steps ii = u F ... handle t = T-2-ii, so step u F + i
+//             reads row F-1-i), the three checkpoint rows (lo >= 1), and 1/sigma as a 16-byte-aligned window.
+// A stage is refilled by its own warp after a __syncwarp (every lane has read it), so the ring needs only full barriers.
+// The arithmetic is that of forward_backward_la_kernel, step for step, and N_s / the re-entry sums go to float64 every
+// F = PB steps as there: outputs are bit-identical.  Frames outside [0, T) are not copied; the steps that would read
+// them (the one-step look-ahead past the last frame, the inactive steps of shorter recordings) only feed state that no
+// active step uses, exactly like the clamped loads of the register version.
+// Checkpoints and 1/sigma are written by generic stores in the forward sweep and read by the async proxy in the backward
+// sweep: every lane fences (fence.proxy.async.global) before the warp issues the first backward copy.
+// ------------------------------------------------------------------------------------------------
+// The look-ahead forward recurrence of forward_backward_la_kernel as one step on an explicit state, shared by the ring
+// sweep's forward pass and its recomputation of the forward variables in the backward pass (same operations, same
+// bits).  State entering the step of frame s: y = y_{s-1}, Yc = Y_{s-1}, q = q_{s-1}, c = c_s, rn = r_s, rs1 = r_{s+1}.
+template <int SPL>
+struct FwdState {
+    float y[SPL];
+    float Yc, q, c, rn, rs1;
+};
+// frame 0 (VBx/VBx.py:164): the state entering frame 1 and a_0
+template <int SPL, int LPR>
+__device__ __forceinline__ void fwd_init(FwdState<SPL> &st, const Vec<SPL> &p0, const Vec<SPL> &p1, const float *pi,
+                                         const float *w, const int l, const bool live, const int ns, float *an) {
+    float loc = 0.f, locq = 0.f, locc = 0.f;
+#pragma unroll
+    for (int k = 0; k < SPL; ++k) {
+        const int s = l * SPL + k;
+        st.y[k] = (live && s < ns) ? p0.v[k] * (pi[k] + VBX_EPS_TR) : 0.f;
+        loc += st.y[k];
+        locq = fmaf(p1.v[k], st.y[k], locq);
+        locc = fmaf(p1.v[k], w[k], locc);
+    }
+    st.Yc = group_sum<LPR>(loc);     // Y_0 = sigma_0
+    st.q = group_sum<LPR>(locq);     // q_0 = p_1 . y_0
+    st.c = group_sum<LPR>(locc);     // c_1 = p_1 . w
+    st.rn = 1.f;                     // r_1
+    st.rs1 = rcp_fast(st.Yc);        // 1/sigma_0 (becomes r_2)
+#pragma unroll
+    for (int k = 0; k < SPL; ++k) an[k] = st.y[k] * st.rs1;
+}
+// frame s from ps = p_s and pn = p_{s+1}: writes a_s to an, returns 1/sigma_s
+template <int SPL, int LPR>
+__device__ __forceinline__ float fwd_step(FwdState<SPL> &st, const Vec<SPL> &ps, const Vec<SPL> &pn, const float *w,
+                                          const float P, float *an) {
+    float ys[SPL], locq = 0.f, locc = 0.f;
+#pragma unroll
+    for (int k = 0; k < SPL; ++k) {
+        ys[k] = (st.rn * ps.v[k]) * fmaf(P, st.y[k], w[k] * st.Yc);
+        locq = fmaf(pn.v[k], ys[k], locq);
+        locc = fmaf(pn.v[k], w[k], locc);
+    }
+    const float qn = group_sum<LPR>(locq);              // consumed by the NEXT step
+    const float cn = group_sum<LPR>(locc);
+    const float Ys = st.rn * fmaf(P, st.q, st.c * st.Yc);   // Y_s = sum_i y_s,i
+    const float inv = rcp_fast(Ys);
+    const float rsig = st.rn * st.Yc * inv;             // 1 / sigma_s
+#pragma unroll
+    for (int k = 0; k < SPL; ++k) {
+        an[k] = ys[k] * inv;
+        st.y[k] = ys[k];
+    }
+    st.Yc = Ys;
+    st.q = qn;
+    st.c = cn;
+    st.rn = st.rs1;
+    st.rs1 = rsig;
+    return rsig;
+}
+
+template <int S_PAD, int SPL>
+struct FbRing {
+    static constexpr int LPR = S_PAD / SPL, RPW = 32 / LPR;
+    static constexpr int F = (SPL == 4) ? 5 : (SPL == 2 ? 10 : 16);   // backward steps per stage (= PB of the kernel above)
+    static constexpr int FF = 2 * F;                                     // forward steps per stage (p rows only)
+    static constexpr int RW = (F + 6 + 3) / 4 * 4;                       // 1/sigma window: F frames widened to 16-byte bounds
+    static constexpr int GROUP = 2 * F * S_PAD + RW;                     // floats per recording group and stage
+    static constexpr int STAGE = RPW * GROUP;
+    static constexpr int kStages = 3;
+    static constexpr int kSmemBytes = 128 + 4 * kStages * STAGE * 4;    // barriers, then the rings of the 4 warps
+};
+
+template <int S_PAD, int SPL>
+__global__ void __launch_bounds__(128) forward_backward_ring_kernel(Plan pl, Workspace ws, RunParams rp, float *gamma,
+                                                                    float *pi_io, const int32_t *__restrict__ n_states) {
+    using G = FbRing<S_PAD, SPL>;
+    constexpr int LPR = G::LPR, RPW = G::RPW, F = G::F, FF = G::FF, NST = G::kStages;
+    extern __shared__ __align__(128) unsigned char fb_ring_smem[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int warp_global = blockIdx.x * 4 + warp;
+    const int g = lane / LPR, l = lane % LPR;
+    const int slot = warp_global * RPW + g;
+    int rec = -1;
+    if (slot < pl.n_rec) rec = pl.order[slot];
+    const bool live = rec >= 0 && ws.active[rec] != 0 && pl.lrec_nchunks[rec] == 0;
+    int64_t f0 = 0;
+    int T = 0;
+    if (live) {
+        f0 = pl.offsets[rec];
+        T = (int)(pl.offsets[rec + 1] - f0);
+    }
+    int Tmax = T, Tmin = live ? T : 0x7fffffff;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        Tmax = max(Tmax, __shfl_xor_sync(0xffffffffu, Tmax, off));
+        Tmin = min(Tmin, __shfl_xor_sync(0xffffffffu, Tmin, off));
+    }
+    if (Tmax == 0) return;  // warp-uniform: no live recording in this warp
+    const int Tlast = max(T - 1, 0);
+    const int ns = live ? (n_states ? n_states[rec] : S_PAD) : 0;
+    const float P = rec >= 0 ? ws.hp[rec].loopP : 0.f, Q = 1.f - P;
+
+    float pi[SPL], w[SPL];
+#pragma unroll
+    for (int k = 0; k < SPL; ++k) {
+        const int s = l * SPL + k;
+        const bool sl = live && s < ns;
+        pi[k] = sl ? pi_io[(int64_t)rec * S_PAD + s] : 0.f;
+        w[k] = sl ? fmaf(Q, pi[k], VBX_EPS_TR) : 0.f;   // VBx/VBx.py:98,159
+    }
+    const float *pp = ws.p + f0 * S_PAD + l * SPL;
+    float *ga = live ? gamma + f0 * S_PAD + l * SPL : ws.scratch + l * SPL;
+    float *rs = live ? ws.rsigma + f0 : ws.scratch + kMaxS;
+    const int64_t gstr = live ? S_PAD : 0;
+    const int rstr = live ? 1 : 0;
+
+    // ---------------- the warp's ring ----------------
+    const uint32_t bar0 = smem_u32(fb_ring_smem) + warp * NST * 8;
+    float *ring = reinterpret_cast<float *>(fb_ring_smem + 128) + warp * NST * G::STAGE;
+    if (lane == 0) {
+#pragma unroll
+        for (int i = 0; i < NST; ++i) mbar_init(bar0 + 8 * i, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+    const bool issuer = live && l == 0;
+    const float *prec = ws.p + f0 * S_PAD;   // the recording's rows, for the copies
+    const float *grec = gamma + f0 * S_PAD;
+    const int nf = (Tmax - 1 + FF - 1) / FF, nb = (Tmax - 1 + F - 1) / F;   // stages of each sweep
+    // stage x of the ring (forward stages 0 .. nf-1, then backward stages nf ..) lives in slot x % NST
+    auto stage_of = [&](const int x) { return ring + (x % NST) * G::STAGE + g * G::GROUP; };
+    auto bar_of = [&](const int x) { return bar0 + 8 * (x % NST); };
+    auto issue_fwd = [&](const int u) {
+        __syncwarp();   // every lane has read the stage this slot held
+        const uint32_t bar = bar_of(u);
+        if (issuer) {
+            const int lo = 2 + u * FF, n = min(FF, T - lo);
+            if (n > 0) {
+                const uint32_t bytes = (uint32_t)n * S_PAD * 4;
+                mbar_add_tx(bar, bytes);
+                bulk_g2s(smem_u32(stage_of(u)), prec + (int64_t)lo * S_PAD, bytes, bar);
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar);
+    };
+    // first float of the 1/sigma window of backward stage u, relative to the recording's frame 0
+    auto rwin = [&](const int u) { return ((f0 + max(T - 1 - (u + 1) * F, 0)) & ~(int64_t)3) - f0; };
+    auto issue_bwd = [&](const int u) {
+        __syncwarp();
+        const uint32_t bar = bar_of(nf + u);
+        if (issuer) {
+            const int hi = T - 2 - u * F, lo = hi - F + 1, lc = max(lo, 0);
+            if (hi >= lc) {
+                const uint32_t rb = (uint32_t)(hi - lc + 1) * S_PAD * 4, cb = lo >= 1 ? 3 * S_PAD * 4 : 0;
+                const int64_t a0 = rwin(u), a1 = ((f0 + hi + 1 + 3) & ~(int64_t)3) - f0;
+                const uint32_t wb = (uint32_t)(a1 - a0) * 4;
+                float *dst = stage_of(nf + u);
+                mbar_add_tx(bar, rb + cb + wb);
+                bulk_g2s(smem_u32(dst + (lc - lo) * S_PAD), prec + (int64_t)lc * S_PAD, rb, bar);
+                if (cb) bulk_g2s(smem_u32(dst + F * S_PAD), grec + (int64_t)lo * S_PAD, cb, bar);   // checkpoint rows
+                bulk_g2s(smem_u32(dst + 2 * F * S_PAD), ws.rsigma + f0 + a0, wb, bar);
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar);
+    };
+
+    // ---------------- forward sweep, VBx/VBx.py:164,167-168 ----------------
+    float alast[SPL];                       // forward variable of the recording's last frame
+    {
+        FwdState<SPL> fs;
+        {
+            const Vec<SPL> p0 = ldg_vec<SPL>(pp);
+            const Vec<SPL> p1 = ldg_vec<SPL>(pp + (int64_t)min(1, Tlast) * S_PAD);
+            for (int u = 0; u < min(NST - 1, nf); ++u) issue_fwd(u);
+            fwd_init<SPL, LPR>(fs, p0, p1, pi, w, l, live, ns, alast);
+            st_vec<SPL>(ga, alast);
+            if (l == 0) rs[0] = fs.rs1;
+        }
+        // step j handles frame s = j + 1 with ps = p_s and pn = p_{s+1}.  Only a_{T-1} is stored (it is gamma_{T-1});
+        // at the first frame of every backward stage that does not reach frame 0 (s = T-1-kF, k >= 1) the state
+        // entering the step is stored in that stage's first three gamma rows, where the backward sweep recomputes the
+        // stage's forward variables from it (they are overwritten with gamma only after that).
+        auto fstep = [&](const int j, const Vec<SPL> &ps, const Vec<SPL> &pn, const bool check) {
+            const int s = j + 1, kb = T - 1 - s;   // frames after s
+            if (kb >= F && kb % F == 0) {
+                sto_vec<SPL>(ga + s * gstr, fs.y);
+                if (l == 0) {
+                    const float sc[4] = {fs.Yc, fs.q, fs.c, fs.rn};
+                    sto_vec<4>(ga + (s + 1) * gstr, sc);
+                    sto_vec<1>(ga + (s + 2) * gstr, &fs.rs1);
+                }
+            }
+            float an[SPL];
+            const float rsig = fwd_step<SPL, LPR>(fs, ps, pn, w, P, an);
+            const bool act = !check || s < T;
+#pragma unroll
+            for (int k = 0; k < SPL; ++k) alast[k] = act ? an[k] : alast[k];
+            if (act) {
+                if (s == T - 1) sto_vec<SPL>(ga + s * gstr, an);
+                if (l == 0) rs[s * rstr] = rsig;
+            }
+        };
+        Vec<SPL> ps = ldg_vec<SPL>(pp + (int64_t)min(1, Tlast) * S_PAD);   // row of frame 1
+        // The stage is read into registers before its first store: the volatile stores keep their order against every
+        // memory access, so a shared-memory load placed at its use would add its latency to every step.
+        auto fstage = [&](const int u, const float *sp, const bool check) {
+            Vec<SPL> buf[FF];
+#pragma unroll
+            for (int i = 0; i < FF; ++i) buf[i] = ld_vec<SPL>(sp + i * S_PAD);
+            if (u + NST - 1 < nf) issue_fwd(u + NST - 1);   // overlaps the shared-memory reads above
+#pragma unroll
+            for (int i = 0; i < FF; ++i) {
+                fstep(u * FF + i, ps, buf[i], check);
+                ps = buf[i];
+            }
+        };
+        for (int u = 0; u < nf; ++u) {
+            mbar_wait(bar_of(u), (u / NST) & 1);
+            const float *sp = stage_of(u) + l * SPL;
+            if ((u + 1) * FF <= Tmin - 1)
+                fstage(u, sp, false);
+            else
+                fstage(u, sp, true);
+        }
+    }
+    // rsigma written by lane l==0 of each group is read by the whole group below; the checkpoints and rsigma are read
+    // by the bulk copies (async proxy) of the backward stages
+    asm volatile("fence.proxy.async.global;" ::: "memory");
+    __syncwarp();
+
+    // ---------------- backward sweep, VBx/VBx.py:165,170-171,174 + eq. (24) statistics ----------------
+    for (int u = 0; u < min(NST - 1, nb); ++u) issue_bwd(u);
+    float g0[SPL], occf[SPL], entf[SPL];
+    double enter[SPL], occ[SPL];
+#pragma unroll
+    for (int k = 0; k < SPL; ++k) {
+        g0[k] = alast[k];        // gamma_{T-1} = forward variable (already stored)
+        occ[k] = (double)alast[k];
+        enter[k] = 0.0;
+        occf[k] = 0.f;
+        entf[k] = 0.f;
+    }
+    {
+        // state entering step ii: b = b_{t+1}, dprev = d_{t+1}, e = e_{t+1}, kap = kappa_{t+1}, f = f_{t+1}
+        // (b_{T-1} = 1 = P * 0 + 1, i.e. v_{T-1} = 0, d_{T-1} = 1, e_{T-1} = 0)
+        float b[SPL], kap[SPL];
+        float dprev = 1.f, e = 0.f, f;
+        {
+            const Vec<SPL> pl1 = ldo_vec<SPL>(pp + (int64_t)Tlast * S_PAD);
+            const float rl1 = ldo_vec<1>(rs + Tlast * rstr).v[0];
+            float locf = 0.f;
+#pragma unroll
+            for (int k = 0; k < SPL; ++k) {
+                b[k] = 1.f;
+                kap[k] = pl1.v[k] * rl1;
+                locf = fmaf(w[k], kap[k], locf);
+            }
+            f = group_sum<LPR>(locf);
+        }
+        // step ii, frame t = T-2-ii: a = a_t, pt = p_t, rt = 1/sigma_t
+        auto bstep = [&](const int ii, const Vec<SPL> &a, const Vec<SPL> &pt, const float rt, const bool check) {
+            const int t = T - 2 - ii;
+            float v[SPL], kapn[SPL], loce = 0.f, locf = 0.f;
+#pragma unroll
+            for (int k = 0; k < SPL; ++k) {
+                v[k] = kap[k] * b[k];                               // v_t = p_{t+1} b_{t+1} / sigma_{t+1}
+                kapn[k] = pt.v[k] * rt;                              // kappa_t
+                const float wk = w[k] * kapn[k];
+                loce = fmaf(wk, v[k], loce);
+                locf += wk;
+            }
+            const float en = group_sum<LPR>(loce);                   // e_t, consumed by the NEXT step
+            const float fn = group_sum<LPR>(locf);                   // f_t
+            const float d = fmaf(P, e, dprev * f);                   // d_t = w . v_t
+            float gn[SPL], bn[SPL], gs = 0.f;
+#pragma unroll
+            for (int k = 0; k < SPL; ++k) {
+                bn[k] = fmaf(P, v[k], d);
+                gn[k] = a.v[k] * bn[k];
+                gs += gn[k];
+            }
+            {   // rows of gamma sum to one (removes the common-mode rounding drift)
+                const float sc = rcp_fast(group_sum<LPR>(gs));
+#pragma unroll
+                for (int k = 0; k < SPL; ++k) gn[k] *= sc;
+            }
+            if (!check) {
+#pragma unroll
+                for (int k = 0; k < SPL; ++k) {
+                    g0[k] = gn[k];
+                    occf[k] += gn[k];
+                    entf[k] += v[k];
+                }
+                sto_vec<SPL>(ga + t * gstr, gn);
+            } else {
+                const bool act = t >= 0;
+#pragma unroll
+                for (int k = 0; k < SPL; ++k) {
+                    g0[k] = act ? gn[k] : g0[k];
+                    occf[k] += act ? gn[k] : 0.f;
+                    entf[k] += act ? v[k] : 0.f;
+                }
+                if (act) sto_vec<SPL>(ga + t * gstr, gn);
+            }
+#pragma unroll
+            for (int k = 0; k < SPL; ++k) {
+                b[k] = bn[k];
+                kap[k] = kapn[k];
+            }
+            dprev = d;
+            e = en;
+            f = fn;
+        };
+        // stage u covers frames lo .. lo+F-1 (lo = T-1-(u+1)F); st: the group's part of the stage.  The forward
+        // variables of those frames are recomputed, with the forward sweep's own operations, from the checkpoint
+        // (lo >= 1) or from frame 0 (lo < 1, where frames below 1 leave the state alone and frame 0 is a_0).
+        // rb: window index of 1/sigma of the stage's first step (clamped: only inactive steps leave the window).
+        auto bstage = [&](const int u, const float *st, const int rb, const bool check) {
+            const float *sp = st + l * SPL, *sr = st + 2 * F * S_PAD;
+            const int lo = T - 1 - (u + 1) * F, z = min(max(-lo, 0), F - 1);
+            Vec<SPL> pr[F];         // p_{lo+i}; read before the first store, as in the forward stages
+            float rt[F];
+#pragma unroll
+            for (int i = 0; i < F; ++i) {
+                pr[i] = ld_vec<SPL>(sp + i * S_PAD);
+                rt[i] = sr[max(rb - i, 0)];
+            }
+            FwdState<SPL> fs, f1;
+            {
+                const Vec<SPL> cy = ld_vec<SPL>(sp + F * S_PAD);
+                const Vec<4> c4 = ld_vec<4>(st + (F + 1) * S_PAD);
+                const float crs = st[(F + 2) * S_PAD];
+                const Vec<SPL> q0 = ld_vec<SPL>(sp + z * S_PAD), q1 = ld_vec<SPL>(sp + min(z + 1, F - 1) * S_PAD);
+                if (u + NST - 1 < nb) issue_bwd(u + NST - 1);
+                float a0[SPL];
+                fwd_init<SPL, LPR>(f1, q0, q1, pi, w, l, live, ns, a0);
+                const bool ck = lo >= 1;
+#pragma unroll
+                for (int k = 0; k < SPL; ++k) {
+                    fs.y[k] = ck ? cy.v[k] : f1.y[k];
+                    f1.y[k] = a0[k];            // f1.y now holds a_0
+                }
+                fs.Yc = ck ? c4.v[0] : f1.Yc;
+                fs.q = ck ? c4.v[1] : f1.q;
+                fs.c = ck ? c4.v[2] : f1.c;
+                fs.rn = ck ? c4.v[3] : f1.rn;
+                fs.rs1 = ck ? crs : f1.rs1;
+            }
+            Vec<SPL> a[F];
+#pragma unroll
+            for (int i = 0; i < F; ++i) {
+                const int s = lo + i;
+                FwdState<SPL> nx = fs;
+                fwd_step<SPL, LPR>(nx, pr[i], pr[min(i + 1, F - 1)], w, P, a[i].v);
+                if (s >= 1) fs = nx;
+#pragma unroll
+                for (int k = 0; k < SPL; ++k) a[i].v[k] = s == 0 ? f1.y[k] : a[i].v[k];
+            }
+#pragma unroll
+            for (int i = 0; i < F; ++i) bstep(u * F + i, a[F - 1 - i], pr[F - 1 - i], rt[i], check);
+#pragma unroll
+            for (int k = 0; k < SPL; ++k) {
+                occ[k] += (double)occf[k];
+                enter[k] += (double)entf[k];
+                occf[k] = 0.f;
+                entf[k] = 0.f;
+            }
+        };
+        for (int u = 0; u < nb; ++u) {
+            mbar_wait(bar_of(nf + u), ((nf + u) / NST) & 1);
+            const float *st = stage_of(nf + u);
+            const int rb = (int)min((int64_t)(T - 2 - u * F) - rwin(u), (int64_t)(G::RW - 1));
+            if ((u + 1) * F <= Tmin - 1)
+                bstage(u, st, rb, false);
+            else
+                bstage(u, st, rb, true);
+        }
+    }
+
+    // ---------------- tail: eq. (24), VBx/VBx.py:101-104 ----------------
+    double pn[SPL];
+    float loc = 0.f;
+#pragma unroll
+    for (int k = 0; k < SPL; ++k) {
+        pn[k] = (double)g0[k] + (double)Q * (double)pi[k] * enter[k];
+        loc += (float)pn[k];
+    }
+    const float tot = group_sum<LPR>(loc);
+    if (live) {
+#pragma unroll
+        for (int k = 0; k < SPL; ++k) {
+            const int s = l * SPL + k;
+            pi_io[(int64_t)rec * S_PAD + s] = (float)(pn[k] / (double)tot);
+            ws.occ[(int64_t)rec * S_PAD + s] = (float)occ[k];
+        }
+    }
+}
+
+// Longest recording of a plan that takes the ring sweep.  On batches with recordings up to 3000 frames (bench.py c3) an
+// earlier form of the ring sweep (forward variables parked in gamma) was faster alone but made the two-stream step
+// slower; the ring sweep has not been measured on such batches since, so they keep the register-burst sweep.
+constexpr int64_t kRingMaxT = 2048;
+
 template <int S_PAD, int SPL>
 static int launch_fb_t(const Plan &pl, const Workspace &ws, const RunParams &rp, float *gamma, float *pi,
-                       const int32_t *n_states, bool classic, cudaStream_t st) {
+                       const int32_t *n_states, bool classic, bool ring, cudaStream_t st) {
     constexpr int RPW = 32 / (S_PAD / SPL);
     const int warps = (pl.n_rec + RPW - 1) / RPW;
     const int blocks = (warps + 3) / 4;
-    if (classic)
+    if (classic) {
         forward_backward_kernel<S_PAD, SPL><<<blocks, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);
-    else
+    } else if (ring && pl.max_T <= kRingMaxT && (reinterpret_cast<uintptr_t>(gamma) & 15) == 0) {   // 16-byte rows for the copies
+        constexpr int smem = FbRing<S_PAD, SPL>::kSmemBytes;
+        if (cudaFuncSetAttribute(forward_backward_ring_kernel<S_PAD, SPL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 smem) != cudaSuccess)
+            return -1;
+        forward_backward_ring_kernel<S_PAD, SPL><<<blocks, 128, smem, st>>>(pl, ws, rp, gamma, pi, n_states);
+    } else {
         forward_backward_la_kernel<S_PAD, SPL><<<blocks, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);
+    }
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
@@ -1396,7 +1830,7 @@ int launch_elbo_trace(const Plan &pl, const double *Li, int max_iters, double *o
 
 int launch_forward_backward(const Plan &pl, const Workspace &ws, const RunParams &rp, float *gamma, float *pi,
                             const int32_t *n_states, double *Li, int32_t *n_iters, int32_t *flags, int iter,
-                            int spl, int classic, cudaStream_t st) {
+                            int spl, int classic, int ring, cudaStream_t st) {
     if (pl.n_rec == 0) return 0;
     if (pl.split) {
         const int rs = launch_forward_backward_split(pl, ws, rp, gamma, pi, n_states, spl, st);
@@ -1405,7 +1839,7 @@ int launch_forward_backward(const Plan &pl, const Workspace &ws, const RunParams
         return cudaGetLastError() == cudaSuccess ? rs + 1 : -1;
     }
     int rc = -1;
-#define VBX_FB(S_, L_) rc = launch_fb_t<S_, L_>(pl, ws, rp, gamma, pi, n_states, classic != 0, st)
+#define VBX_FB(S_, L_) rc = launch_fb_t<S_, L_>(pl, ws, rp, gamma, pi, n_states, classic != 0, ring != 0, st)
     const int S = pl.S;
     if (spl == 0) spl = (S >= 16) ? 2 : 1;
     if (S == 64 && spl < 2) spl = 2;
