@@ -94,7 +94,11 @@ int vbx_bind_workspace(vbx_handle_t h, void *workspace, size_t bytes);
 
 /* VBx/VBx.py:87-89:  rho = fea * sqrt(Phi)  and the per-frame constant G (kept as one float64 sum per
  * recording inside the workspace, since G is state independent and only shifts the ELBO).
- * fea [N,R], Phi [R], rho_out [N,R] (may alias fea). */
+ * fea [N,R], Phi [R], rho_out [N,R] (may alias fea).
+ * Alignment: the kernels access rho and gamma arrays (and fea, Phi, X, V) with 16-byte vectors, so vbx_prepare_scale,
+ * vbx_prepare_project, vbx_run, vbx_run_per_recording, vbx_hard_labels and vbx_hard_labels_keep return VBX_ERR_ARG,
+ * before anything is launched, for any of those device pointers that is not 16-byte aligned (a view that starts
+ * inside an allocation, for example). */
 int vbx_prepare_scale(vbx_handle_t h, const float *fea, const float *Phi, float *rho_out, void *stream);
 
 /* The caller-side projection folded with the scale (VBx/vbhmm.py:129,153 composed with VBx/VBx.py:88-89,

@@ -6,8 +6,10 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <numeric>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/vbx_b200.h"
@@ -76,6 +78,15 @@ int cuda_fail(vbx_handle_t h, cudaError_t e, const char *what) {
     return fail(h, VBX_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
 }
 size_t align_up(size_t v, size_t a = 256) { return (v + a - 1) / a * a; }
+
+// The kernels read and write these arrays with 16-byte vector accesses (float4 rows, the sweeps' bulk copies): a pointer
+// off that grid must be refused before anything is launched.  Null pointers are left to the null checks.
+int misaligned16(vbx_handle_t h, const std::string &who, std::initializer_list<std::pair<const void *, const char *>> arrays) {
+    for (const auto &a : arrays)
+        if (reinterpret_cast<uintptr_t>(a.first) & 15)
+            return fail(h, VBX_ERR_ARG, who + ": " + a.second + " must be 16-byte aligned");
+    return VBX_OK;
+}
 
 // NVTX range around an entry point (visible in nsys / ncu --nvtx timelines; no cost without a tool attached)
 struct Range {
@@ -535,6 +546,7 @@ int vbx_prepare_scale(vbx_handle_t h, const float *fea, const float *Phi, float 
     DeviceGuard guard(h->device);
     if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     if (h->plan.n_frames && (!fea || !Phi || !rho_out)) return fail(h, VBX_ERR_ARG, "vbx_prepare_scale: null pointer");
+    if ((rc = misaligned16(h, "vbx_prepare_scale", {{fea, "fea"}, {Phi, "Phi"}, {rho_out, "rho_out"}}))) return rc;
     {
         Timed t(h, (cudaStream_t)stream, VBX_K_PREPARE);
         rc = counted(h, vbx::launch_prepare_scale(h->plan, h->ws, fea, Phi, rho_out, (cudaStream_t)stream), "prepare_scale");
@@ -553,6 +565,7 @@ int vbx_prepare_project(vbx_handle_t h, const float *X, int32_t D, const float *
     if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     if (h->plan.n_frames && (!X || !V || !Phi || !rho_out)) return fail(h, VBX_ERR_ARG, "vbx_prepare_project: null pointer");
     if (D < 32 || (D & 31)) return fail(h, VBX_ERR_ARG, "vbx_prepare_project: D must be a multiple of 32");
+    if ((rc = misaligned16(h, "vbx_prepare_project", {{X, "X"}, {V, "V"}, {rho_out, "rho_out"}}))) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     bool done = false, fused_g = false;
     Timed *tp = new Timed(h, st, VBX_K_PROJECT);
@@ -637,6 +650,7 @@ static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *
     if (pl.n_rec == 0) return VBX_OK;
     if (!Li_out || !n_iters_out || !flags_out || !pi_io) return fail(h, VBX_ERR_ARG, w + ": null output pointer");
     if (pl.n_frames && (!rho || !Phi || !gamma_io)) return fail(h, VBX_ERR_ARG, w + ": null pointer");
+    if ((rc = misaligned16(h, w, {{rho, "rho"}, {gamma_io, "gamma_io"}}))) return rc;
     vbx::RunParams rp;
     rp.epsilon = epsilon;
     rp.max_iters = max_iters;
@@ -789,6 +803,7 @@ int vbx_hard_labels(vbx_handle_t h, const float *gamma, const int32_t *n_states,
     if (!h) return VBX_ERR_ARG;
     if (!h->planned || h->f64_only) return fail(h, VBX_ERR_STATE, "vbx_hard_labels: call vbx_plan first");
     if (h->plan.n_frames && (!gamma || !first_out)) return fail(h, VBX_ERR_ARG, "vbx_hard_labels: null pointer");
+    if (const int rc = misaligned16(h, "vbx_hard_labels", {{gamma, "gamma"}})) return rc;
     DeviceGuard guard(h->device);
     return counted(h, vbx::launch_hard_labels(h->plan, gamma, n_states, first_out, second_out, (cudaStream_t)stream), "hard_labels");
 }
@@ -800,6 +815,7 @@ int vbx_hard_labels_keep(vbx_handle_t h, const float *gamma, const int32_t *n_st
     if (h->plan.n_rec == 0) return VBX_OK;
     if (!keep || !mass_out || (h->plan.n_frames && (!gamma || !first_out)))
         return fail(h, VBX_ERR_ARG, "vbx_hard_labels_keep: null pointer");
+    if (const int rc = misaligned16(h, "vbx_hard_labels_keep", {{gamma, "gamma"}})) return rc;
     DeviceGuard guard(h->device);
     // keep lives on the device: read it back once to refuse counts below 1 (the labels leave the device next anyway)
     std::vector<int32_t> kh(h->plan.n_rec);

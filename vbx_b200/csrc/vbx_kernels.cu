@@ -1716,7 +1716,7 @@ static int launch_fb_t(const Plan &pl, const Workspace &ws, const RunParams &rp,
     const int blocks = (warps + 3) / 4;
     if (classic) {
         forward_backward_kernel<S_PAD, SPL><<<blocks, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);
-    } else if (ring && pl.max_T <= kRingMaxT && (reinterpret_cast<uintptr_t>(gamma) & 15) == 0) {   // 16-byte rows for the copies
+    } else if (ring && pl.max_T <= kRingMaxT) {   // gamma is 16-byte aligned (checked by the C entries): rows for the copies
         constexpr int smem = FbRing<S_PAD, SPL>::kSmemBytes;
         if (cudaFuncSetAttribute(forward_backward_ring_kernel<S_PAD, SPL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  smem) != cudaSuccess)
