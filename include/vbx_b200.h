@@ -154,6 +154,27 @@ int vbx_run_per_recording(vbx_handle_t h, const float *rho, const float *Phi, fl
                           int32_t max_iters, double epsilon, float *alpha_io, float *invL_io, int32_t warm_start,
                           double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream);
 
+/* vbx_run_per_recording with a Gaussian prior on each state's speaker latent (DESIGN.md section 5.23): state s of
+ * recording b starts from the posterior of y ~ N(0, I) given prior_n[b,s] x-vectors whose feature sum is prior_F[b,s,:]
+ * (the fea units of vbx_prepare_scale, NOT rho: the kernels multiply by sqrt(Phi) themselves), for example the float64
+ * statistics n_enroll / F_enroll of an enrolled speaker (vbx_enroll_batch).  With c = Fa[b] / Fb[b]:
+ *   lambda0 = 1 + c n_e Phi      mu0 = c sqrt(Phi) F_e / lambda0
+ *   invL = 1 / (1 + c (N_s + n_e) Phi)      alpha = c invL (rho^T gamma_s + sqrt(Phi) F_e)
+ *   ELBO regulariser  Fb/2 sum_{s,r} [log(lambda0 invL) - lambda0 invL - lambda0 (alpha - mu0)^2 + 1]
+ * which is the ELBO of the recording with those x-vectors appended as frames held on state s, minus a constant.  The
+ * log-likelihoods, the forward-backward, pi and the stop rule are vbx_run's; warm_start reads alpha_io / invL_io as
+ * given and puts the prior into the regulariser.  prior_n [n_rec,S] and prior_F [n_rec,S,R] are float64 DEVICE arrays
+ * (S, R of the plan; columns s >= n_states[b] are not read); null arrays return VBX_ERR_ARG.  Their values are read on
+ * the device and not validated (n_e >= 0 and finite values are the caller's to check).  A recording whose prior is
+ * all zero gets bit-identical results to vbx_run_per_recording (gamma, pi, Li, n_iters, flags, alpha, invL), whatever
+ * the other recordings' priors.  Stream ordered, no allocation, no host synchronisation.  Option
+ * "graph": the two prior POINTERS are part of a call's identity, and a replay reads their contents as it runs. */
+int vbx_run_prior(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io, float *pi_io,
+                  const int32_t *n_states, const double *Fa, const double *Fb, const double *loop_prob,
+                  int32_t max_iters, double epsilon, float *alpha_io, float *invL_io, int32_t warm_start,
+                  double *Li_out, int32_t *n_iters_out, int32_t *flags_out, const double *prior_n,
+                  const double *prior_F, void *stream);
+
 /* AHC initialisation, VBx/vbhmm.py:131-146, for every recording of the planned batch, in float64 like the reference:
  *   cosine similarity of the recording's rows of x (VBx/diarization_lib.py:190-213; x [N,dim], float32 or float64),
  *   thr_out[b] = twoGMMcalib_lin(similarities)[0] (VBx/diarization_lib.py:13-31, 20 iterations),
@@ -330,6 +351,14 @@ int vbx_run_f64(vbx_handle_t h, void *workspace, size_t workspace_bytes, const d
                 double *gamma_io, double *pi_io, const int32_t *n_states, double Fa, double Fb, double loop_prob,
                 int32_t max_iters, double epsilon, double *alpha_io, double *invL_io, int32_t warm_start,
                 double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream);
+/* vbx_run_f64 with the enrolment prior of vbx_run_prior (same formulas, all in float64, with the scalar Fa / Fb):
+ * prior_n [n_rec,S], prior_F [n_rec,S,R] float64 DEVICE arrays of this plan's S and R; null arrays return VBX_ERR_ARG.
+ * An all-zero prior gives bit-identical results to vbx_run_f64. */
+int vbx_run_f64_prior(vbx_handle_t h, void *workspace, size_t workspace_bytes, const double *fea, const double *Phi,
+                      double *gamma_io, double *pi_io, const int32_t *n_states, double Fa, double Fb, double loop_prob,
+                      int32_t max_iters, double epsilon, double *alpha_io, double *invL_io, int32_t warm_start,
+                      double *Li_out, int32_t *n_iters_out, int32_t *flags_out, const double *prior_n,
+                      const double *prior_F, void *stream);
 
 /* The module-level forward_backward(lls, tr, ip) of the reference (VBx/VBx.py:146-175) for an arbitrary transition
  * matrix, float64, log domain, dense S x S log-sum-exp per frame as the reference computes it (the EM loop itself never

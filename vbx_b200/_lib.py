@@ -16,7 +16,7 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_score', 'vbx_score_overlap', 'vbx_score_jer', 'vbx_link_batch_workspace_bytes', 'vbx_link_batch',
            'vbx_enroll_batch_workspace_bytes', 'vbx_enroll_batch', 'vbx_cohort_stats_batch_workspace_bytes',
            'vbx_cohort_stats_batch', 'vbx_init_turns', 'vbx_combine_workspace_bytes', 'vbx_combine',
-           'vbx_init_random']
+           'vbx_init_random', 'vbx_run_prior', 'vbx_run_f64_prior']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
@@ -80,12 +80,17 @@ def load():
     lib.vbx_run.argtypes = [vp, vp, vp, vp, vp, vp, dbl, dbl, dbl, i32, dbl, vp, vp, i32, vp, vp, vp, vp]
     lib.vbx_run_per_recording.restype = ctypes.c_int
     lib.vbx_run_per_recording.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, dbl, vp, vp, i32, vp, vp, vp, vp]
+    lib.vbx_run_prior.restype = ctypes.c_int
+    lib.vbx_run_prior.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, dbl, vp, vp, i32, vp, vp, vp, vp, vp, vp]
     lib.vbx_launch_count.restype = i64
     lib.vbx_launch_count.argtypes = [vp]
     lib.vbx_f64_workspace_bytes.restype = ctypes.c_int
     lib.vbx_f64_workspace_bytes.argtypes = [vp, ctypes.POINTER(ctypes.c_size_t)]
     lib.vbx_run_f64.restype = ctypes.c_int
     lib.vbx_run_f64.argtypes = [vp, vp, ctypes.c_size_t, vp, vp, vp, vp, vp, dbl, dbl, dbl, i32, dbl, vp, vp, i32, vp, vp, vp, vp]
+    lib.vbx_run_f64_prior.restype = ctypes.c_int
+    lib.vbx_run_f64_prior.argtypes = [vp, vp, ctypes.c_size_t, vp, vp, vp, vp, vp, dbl, dbl, dbl, i32, dbl, vp, vp, i32, vp, vp,
+                                      vp, vp, vp, vp]
     lib.vbx_forward_backward.restype = ctypes.c_int
     lib.vbx_forward_backward.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp]
     lib.vbx_attach_comm.restype = ctypes.c_int

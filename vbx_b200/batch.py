@@ -294,13 +294,13 @@ class VbxBatch:
                     flags=torch.empty(self.B, dtype=torch.int32, device=dev))
 
     # ---- VBx/VBx.py:91-125 ----------------------------------------------------------------
-    def _hyper(self, Fa, Fb, loopProb):
-        """None when Fa, Fb and loopProb are all numbers, else the three as float64 CUDA tensors [B] (numbers broadcast),
-        checked on the host: the library reads per-recording values on the device and cannot validate them, so the
-        check copies them to the host and a per-recording run() waits for the device's current stream.  A broadcast
-        number keeps its tensor between calls (stable pointers: option 'graph' can replay the run)."""
+    def _hyper(self, Fa, Fb, loopProb, arrays=False):
+        """None when Fa, Fb and loopProb are all numbers (and not `arrays`), else the three as float64 CUDA tensors [B]
+        (numbers broadcast), checked on the host: the library reads per-recording values on the device and cannot
+        validate them, so the check copies them to the host and a per-recording run() waits for the device's current
+        stream.  A broadcast number keeps its tensor between calls (stable pointers: option 'graph' can replay the run)."""
         vals = dict(Fa=Fa, Fb=Fb, loopProb=loopProb)
-        if not any(isinstance(v, torch.Tensor) for v in vals.values()):
+        if not arrays and not any(isinstance(v, torch.Tensor) for v in vals.values()):
             return None
         out = []
         for name, v in vals.items():
@@ -326,17 +326,21 @@ class VbxBatch:
         return Fa_t, Fb_t, lp_t
 
     def run(self, gamma, pi, Fa=1.0, Fb=1.0, loopProb=0.9, maxIters=10, epsilon=1e-4,
-            alpha=None, invL=None, warm_start=False, return_model=False, buffers=None):
+            alpha=None, invL=None, warm_start=False, return_model=False, buffers=None, prior=None):
         """gamma [N,S] and pi [B,S] float32 CUDA tensors, updated IN PLACE (padded columns must be 0).
         Fa, Fb, loopProb: numbers for the whole batch, or any of them a float64 CUDA tensor [B] of per-recording values
         (vbx_run_per_recording; numbers are then broadcast).  A recording gets bit-identical results either way.  The
         per-recording values are validated on the host, so such a call synchronises with the current stream.
+        prior: None, or (n [B,S], F [B,S,R]) float64 CUDA tensors, the enrolment prior of each state (vbx_run_prior,
+        DESIGN.md section 5.23): n_e x-vectors with feature sum F_e in fea units.  Checked on the host (synchronises).
         Returns dict(gamma, pi, Li [B,maxIters] float64 (NaN padded), n_iters [B], flags [B][, alpha, invL]).
         buffers: optional dict(Li, n_iters, flags) of preallocated output tensors (see `output_buffers`)."""
         if self.rho is None:
             raise VbxError('call prepare_scale() or prepare_project() first')
         self._f32(gamma, (self.N, self.S), 'gamma')
         self._f32(pi, (self.B, self.S), 'pi')
+        if prior is not None:
+            prior = check_prior(prior, self.B, self.S, self.R, self.device)
         dev = self.device
         if return_model or warm_start:
             if alpha is None:
@@ -352,8 +356,14 @@ class VbxBatch:
             Li = torch.empty((self.B, max(int(maxIters), 1)), dtype=torch.float64, device=dev)
             n_iters = torch.empty(self.B, dtype=torch.int32, device=dev)
             flags = torch.empty(self.B, dtype=torch.int32, device=dev)
-        hyper = self._hyper(Fa, Fb, loopProb)
-        if hyper is None:
+        hyper = self._hyper(Fa, Fb, loopProb, arrays=prior is not None)
+        if prior is not None:
+            self._check(self.lib.vbx_run_prior(
+                self._h, _ptr(self.rho), _ptr(self.Phi), _ptr(gamma), _ptr(pi), _ptr(self.n_states),
+                *(_ptr(t) for t in hyper), int(maxIters), float(epsilon),
+                _ptr(alpha), _ptr(invL), int(bool(warm_start)), _ptr(Li), _ptr(n_iters), _ptr(flags),
+                _ptr(prior[0]), _ptr(prior[1]), self._stream()))
+        elif hyper is None:
             self._check(self.lib.vbx_run(
                 self._h, _ptr(self.rho), _ptr(self.Phi), _ptr(gamma), _ptr(pi), _ptr(self.n_states),
                 float(Fa), float(Fb), float(loopProb), int(maxIters), float(epsilon),
@@ -371,14 +381,37 @@ class VbxBatch:
         return out
 
 
+def check_prior(prior, B, S, R, device):
+    """The enrolment prior of run() / run_f64() checked on the host (ValueError): a pair (n [B,S], F [B,S,R]) of float64
+    tensors on `device`, finite, n >= 0.  Returns the pair contiguous."""
+    if not (isinstance(prior, (tuple, list)) and len(prior) == 2):
+        raise ValueError('prior must be a pair (n [B,S], F [B,S,R]) of float64 CUDA tensors')
+    out = []
+    for t, shape, name in ((prior[0], (B, S), 'prior n'), (prior[1], (B, S, R), 'prior F')):
+        if not (isinstance(t, torch.Tensor) and t.dtype == torch.float64 and t.device == torch.device(device)
+                and tuple(t.shape) == shape):
+            got = f'{t.dtype} {tuple(t.shape)} on {t.device}' if isinstance(t, torch.Tensor) else type(t).__name__
+            raise ValueError(f'{name}: expected a float64 tensor of shape {shape} on {device}, got {got}')
+        out.append(t.contiguous())
+    n, F = out
+    if not (bool(torch.isfinite(n).all()) and bool(torch.isfinite(F).all())):
+        raise ValueError('prior n and F must be finite')
+    if bool((n < 0).any()):
+        raise ValueError('prior n (enrolment x-vector counts) must be >= 0')
+    return n, F
+
+
 def run_f64(vb, fea, Phi, gamma, pi, Fa=1.0, Fb=1.0, loopProb=0.9, maxIters=10, epsilon=1e-4, alpha=None, invL=None,
-            warm_start=False, return_model=False):
+            warm_start=False, return_model=False, prior=None):
     """Float64 evaluation of the EM loop on the planned batch `vb` (VbxBatch(..., allocate=False) is enough).
-    fea [N,R], Phi [R], gamma [N,S], pi [B,S] float64 CUDA tensors (gamma, pi updated in place)."""
+    fea [N,R], Phi [R], gamma [N,S], pi [B,S] float64 CUDA tensors (gamma, pi updated in place).  prior: None, or
+    (n [B,S], F [B,S,R]) float64 CUDA tensors, the enrolment prior of VbxBatch.run (vbx_run_f64_prior)."""
     dev = vb.device
     for t, shape, name in ((fea, (vb.N, vb.R), 'fea'), (Phi, (vb.R,), 'Phi'), (gamma, (vb.N, vb.S), 'gamma'), (pi, (vb.B, vb.S), 'pi')):
         if not (t.is_cuda and t.dtype == torch.float64 and t.is_contiguous() and tuple(t.shape) == shape):
             raise ValueError(f'{name}: expected a contiguous float64 CUDA tensor of shape {shape}')
+    if prior is not None:
+        prior = check_prior(prior, vb.B, vb.S, vb.R, dev)
     need = ctypes.c_size_t()
     vb._check(vb.lib.vbx_f64_workspace_bytes(vb._h, ctypes.byref(need)))
     ws = torch.empty(int(need.value), dtype=torch.uint8, device=dev)
@@ -390,9 +423,13 @@ def run_f64(vb, fea, Phi, gamma, pi, Fa=1.0, Fb=1.0, loopProb=0.9, maxIters=10, 
     Li = torch.empty((vb.B, max(int(maxIters), 1)), dtype=torch.float64, device=dev)
     n_iters = torch.empty(vb.B, dtype=torch.int32, device=dev)
     flags = torch.empty(vb.B, dtype=torch.int32, device=dev)
-    vb._check(vb.lib.vbx_run_f64(vb._h, _ptr(ws), ws.numel(), _ptr(fea), _ptr(Phi), _ptr(gamma), _ptr(pi), _ptr(vb.n_states),
-                                 float(Fa), float(Fb), float(loopProb), int(maxIters), float(epsilon), _ptr(alpha), _ptr(invL),
-                                 int(bool(warm_start)), _ptr(Li), _ptr(n_iters), _ptr(flags), vb._stream()))
+    args = (vb._h, _ptr(ws), ws.numel(), _ptr(fea), _ptr(Phi), _ptr(gamma), _ptr(pi), _ptr(vb.n_states), float(Fa), float(Fb),
+            float(loopProb), int(maxIters), float(epsilon), _ptr(alpha), _ptr(invL), int(bool(warm_start)), _ptr(Li),
+            _ptr(n_iters), _ptr(flags))
+    if prior is None:
+        vb._check(vb.lib.vbx_run_f64(*args, vb._stream()))
+    else:
+        vb._check(vb.lib.vbx_run_f64_prior(*args, _ptr(prior[0]), _ptr(prior[1]), vb._stream()))
     torch.cuda.current_stream(dev).synchronize()     # ws is released when this function returns
     out = dict(gamma=gamma, pi=pi, Li=Li[:, :int(maxIters)], n_iters=n_iters, flags=flags)
     if return_model or warm_start:

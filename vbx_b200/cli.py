@@ -23,7 +23,9 @@ With --enroll-ark FILE --enroll-utt2spk FILE --enroll-threshold X (all three or 
 enrolled speakers of the ark (DESIGN.md section 5.16): a speaker whose log-likelihood ratio against an enrolled speaker
 reaches X takes that speaker's name, one name per speaker within a recording; the others are written as
 unknown-<recording>-<label>, or with --link-threshold linked among themselves and written as unknown-<id>.  With
---output-2nd the second-label RTTMs use the same names.
+--output-2nd the second-label RTTMs use the same names.  With --enroll-prior as well (and --init AHC+VB, no speaker
+counts) the enrolled speakers take part in the VB-HMM (DESIGN.md section 5.23): AHC clusters are assigned to them the
+same way, and an assigned cluster's state starts from that speaker's x-vectors as its speaker prior.
 
 With --cohort-ark FILE --cohort-utt2spk FILE (both or neither; needs --link-threshold or the enrolment options) the
 linking and enrolment scores are normalised against the cohort speakers of the ark (DESIGN.md section 5.17), speakers
@@ -137,6 +139,9 @@ def build_parser():
     ap.add_argument('--enroll-utt2spk', default=None, help='the speaker of each x-vector of --enroll-ark (utt2spk)')
     ap.add_argument('--enroll-threshold', default=None, type=float,
                     help='least log-likelihood ratio at which a speaker takes an enrolled name')
+    ap.add_argument('--enroll-prior', action='store_true',
+                    help='with the enrolment options and --init AHC+VB: AHC clusters assigned to enrolled speakers start '
+                         'the VB-HMM from those speakers\' x-vectors as their speaker prior')
     ap.add_argument('--cohort-ark', default=None,
                     help='x-vectors of cohort speakers (Kaldi ark), none of them in the archive, to normalise the '
                          'linking and enrolment scores by')
@@ -159,6 +164,13 @@ def main(argv=None):
     coh = [args.cohort_ark, args.cohort_utt2spk]
     if any(v is not None for v in coh) and any(v is None for v in coh):
         ap.error('--cohort-ark and --cohort-utt2spk go together')
+    if args.enroll_prior:
+        if args.enroll_ark is None:
+            ap.error('--enroll-prior needs --enroll-ark, --enroll-utt2spk and --enroll-threshold')
+        if args.init != 'AHC+VB':
+            ap.error('--enroll-prior needs --init AHC+VB')
+        if args.num_speakers is not None or args.min_speakers is not None or args.max_speakers is not None:
+            ap.error('--enroll-prior does not combine with --num-speakers / --min-speakers / --max-speakers')
     if args.cohort_top is not None and args.cohort_ark is None:
         ap.error('--cohort-top needs --cohort-ark and --cohort-utt2spk')
     if args.cohort_ark is not None and args.link_threshold is None and args.enroll_ark is None:
@@ -190,7 +202,7 @@ def main(argv=None):
                         num_speakers=args.num_speakers, min_speakers=args.min_speakers, max_speakers=args.max_speakers,
                         link_threshold=args.link_threshold, enroll=enroll, enroll_threshold=args.enroll_threshold,
                         init_rttm=args.init_rttm, init_states=args.init_states, restarts=args.restarts, seed=args.seed,
-                        **norm_kw)
+                        enroll_prior=args.enroll_prior, **norm_kw)
     linked = args.link_threshold is not None
     named_init = args.init == 'RTTM+VB' and enroll is None and not linked
     os.makedirs(args.out_rttm_dir, exist_ok=True)                           # VBx/vbhmm.py:170

@@ -634,7 +634,8 @@ int vbx_prepare_xvectors(vbx_handle_t h, const float *x_raw, int32_t Dx, const f
 static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *rho, const float *Phi, float *gamma_io, float *pi_io,
                     const int32_t *n_states, double Fa, double Fb, double loop_prob, const double *Fa_v, const double *Fb_v,
                     const double *loopP_v, int32_t max_iters, double epsilon, float *alpha_io, float *invL_io,
-                    int32_t warm_start, double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream) {
+                    int32_t warm_start, double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream,
+                    const double *prior_n = nullptr, const double *prior_F = nullptr) {
     Range nvtx_range(who);
     const std::string w(who);
     int rc = check_ready(h, who);
@@ -688,7 +689,8 @@ static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *
             if (rc) return rc;
             {
                 Timed t(h, st, VBX_K_SPEAKER_MODEL);
-                rc = counted(h, vbx::launch_speaker_model(pl, h->ws, Phi, n_states, alpha_io, invL_io, given, st), "speaker_model");
+                rc = counted(h, vbx::launch_speaker_model(pl, h->ws, Phi, n_states, alpha_io, invL_io, given, st, prior_n,
+                                                          prior_F), "speaker_model");
             }
             if (rc) return rc;
             {
@@ -714,7 +716,7 @@ static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *
         if (rp.hybrid && it > 0) {   // one float64 iteration for the recordings in the finishing phase (none at it == 0)
             Timed t(h, st, VBX_K_EXACT64);
             rc = counted(h, vbx::launch_exact64_round(pl, h->ws, rp, rho, Phi, gamma_io, pi_io, n_states, alpha_io, invL_io, Li_out,
-                                                      n_iters_out, flags_out, st), "exact64");
+                                                      n_iters_out, flags_out, st, prior_n, prior_F), "exact64");
             if (rc) return rc;
         }
     }
@@ -732,7 +734,7 @@ static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *
     for (const void *p : {(const void *)rho, (const void *)Phi, (const void *)gamma_io, (const void *)pi_io, (const void *)n_states,
                           (const void *)alpha_io, (const void *)invL_io, (const void *)Li_out, (const void *)n_iters_out,
                           (const void *)flags_out, (const void *)h->ws.p, (const void *)Fa_v, (const void *)Fb_v,
-                          (const void *)loopP_v})
+                          (const void *)loopP_v, (const void *)prior_n, (const void *)prior_F})
         mix((uint64_t)(uintptr_t)p);
     mix(bits(Fa)); mix(bits(Fb)); mix(bits(loop_prob)); mix(bits(epsilon)); mix((uint64_t)max_iters); mix((uint64_t)warm_start);
     if (key == 0) key = 1;
@@ -796,6 +798,17 @@ int vbx_run_per_recording(vbx_handle_t h, const float *rho, const float *Phi, fl
                           double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream) {
     return run_impl(h, "vbx_run_per_recording", true, rho, Phi, gamma_io, pi_io, n_states, 0.0, 1.0, 0.0, Fa, Fb, loop_prob, max_iters,
                     epsilon, alpha_io, invL_io, warm_start, Li_out, n_iters_out, flags_out, stream);
+}
+
+int vbx_run_prior(vbx_handle_t h, const float *rho, const float *Phi, float *gamma_io, float *pi_io,
+                  const int32_t *n_states, const double *Fa, const double *Fb, const double *loop_prob,
+                  int32_t max_iters, double epsilon, float *alpha_io, float *invL_io, int32_t warm_start,
+                  double *Li_out, int32_t *n_iters_out, int32_t *flags_out, const double *prior_n,
+                  const double *prior_F, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    if (!prior_n || !prior_F) return fail(h, VBX_ERR_ARG, "vbx_run_prior: prior_n and prior_F must be device arrays");
+    return run_impl(h, "vbx_run_prior", true, rho, Phi, gamma_io, pi_io, n_states, 0.0, 1.0, 0.0, Fa, Fb, loop_prob, max_iters,
+                    epsilon, alpha_io, invL_io, warm_start, Li_out, n_iters_out, flags_out, stream, prior_n, prior_F);
 }
 
 int vbx_hard_labels(vbx_handle_t h, const float *gamma, const int32_t *n_states, int32_t *first_out,
@@ -1093,11 +1106,13 @@ int vbx_f64_workspace_bytes(vbx_handle_t h, size_t *bytes_out) {
     return VBX_OK;
 }
 
-int vbx_run_f64(vbx_handle_t h, void *workspace, size_t workspace_bytes, const double *fea, const double *Phi,
-                double *gamma_io, double *pi_io, const int32_t *n_states, double Fa, double Fb, double loop_prob,
-                int32_t max_iters, double epsilon, double *alpha_io, double *invL_io, int32_t warm_start,
-                double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream) {
-    if (!h) return VBX_ERR_ARG;
+}  // extern "C"
+
+static int run_f64_impl(vbx_handle_t h, void *workspace, size_t workspace_bytes, const double *fea, const double *Phi,
+                        double *gamma_io, double *pi_io, const int32_t *n_states, double Fa, double Fb, double loop_prob,
+                        int32_t max_iters, double epsilon, double *alpha_io, double *invL_io, int32_t warm_start,
+                        double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream,
+                        const double *prior_n = nullptr, const double *prior_F = nullptr) {
     Range nvtx_range("vbx_run_f64");
     if (!h->planned) return fail(h, VBX_ERR_STATE, "vbx_run_f64: call vbx_plan first");
     DeviceGuard guard(h->device);
@@ -1110,8 +1125,31 @@ int vbx_run_f64(vbx_handle_t h, void *workspace, size_t workspace_bytes, const d
         return fail(h, VBX_ERR_ARG, "vbx_run_f64: null pointer");
     if (warm_start && (!alpha_io || !invL_io)) return fail(h, VBX_ERR_ARG, "vbx_run_f64: warm_start needs alpha_io and invL_io");
     return counted(h, vbx::launch_run_f64(pl, workspace, fea, Phi, gamma_io, pi_io, n_states, Fa, Fb, loop_prob, max_iters, epsilon,
-                                          alpha_io, invL_io, warm_start, Li_out, n_iters_out, flags_out, (cudaStream_t)stream),
+                                          alpha_io, invL_io, warm_start, Li_out, n_iters_out, flags_out, (cudaStream_t)stream,
+                                          prior_n, prior_F),
                    "run_f64");
+}
+
+extern "C" {
+
+int vbx_run_f64(vbx_handle_t h, void *workspace, size_t workspace_bytes, const double *fea, const double *Phi,
+                double *gamma_io, double *pi_io, const int32_t *n_states, double Fa, double Fb, double loop_prob,
+                int32_t max_iters, double epsilon, double *alpha_io, double *invL_io, int32_t warm_start,
+                double *Li_out, int32_t *n_iters_out, int32_t *flags_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    return run_f64_impl(h, workspace, workspace_bytes, fea, Phi, gamma_io, pi_io, n_states, Fa, Fb, loop_prob, max_iters,
+                        epsilon, alpha_io, invL_io, warm_start, Li_out, n_iters_out, flags_out, stream);
+}
+
+int vbx_run_f64_prior(vbx_handle_t h, void *workspace, size_t workspace_bytes, const double *fea, const double *Phi,
+                      double *gamma_io, double *pi_io, const int32_t *n_states, double Fa, double Fb, double loop_prob,
+                      int32_t max_iters, double epsilon, double *alpha_io, double *invL_io, int32_t warm_start,
+                      double *Li_out, int32_t *n_iters_out, int32_t *flags_out, const double *prior_n,
+                      const double *prior_F, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    if (!prior_n || !prior_F) return fail(h, VBX_ERR_ARG, "vbx_run_f64_prior: prior_n and prior_F must be device arrays");
+    return run_f64_impl(h, workspace, workspace_bytes, fea, Phi, gamma_io, pi_io, n_states, Fa, Fb, loop_prob, max_iters,
+                        epsilon, alpha_io, invL_io, warm_start, Li_out, n_iters_out, flags_out, stream, prior_n, prior_F);
 }
 
 int vbx_forward_backward(vbx_handle_t h, const double *lls, const double *tr, const double *ip, int32_t T, int32_t S,

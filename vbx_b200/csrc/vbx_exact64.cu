@@ -206,6 +206,67 @@ __global__ void __launch_bounds__(128) speaker64_kernel(Plan pl, Workspace ws, R
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// enrolment prior (DESIGN.md section 5.23) around the unchanged speaker64_kernel.  prior_stats64 adds n_e to the
+// first M-tile's N_s and sqrt(Phi) F_e to its gamma^T rho, so that speaker64_kernel's tile sums give invL and alpha of
+// the prior; prior_reg64 then adds the prior's terms of the regulariser to reg64.  Both leave every value as it is
+// where the prior is zero: a recording without a prior gets the bits of a run without one.
+// ---------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) prior_stats64_kernel(Plan pl, Workspace ws, const float *__restrict__ Phi,
+                                                            const int32_t *__restrict__ n_states,
+                                                            const double *__restrict__ prior_n,
+                                                            const double *__restrict__ prior_F) {
+    const int rec = blockIdx.x;
+    if (!ws.active64[rec]) return;
+    const int t = pl.mtile_begin[rec];
+    if (t == pl.mtile_begin[rec + 1]) return;
+    const int S = pl.S, R = pl.R, r = threadIdx.x;
+    const int ns = n_states ? n_states[rec] : S;
+    const double sphi = r < R ? sqrt((double)Phi[r]) : 0.0;
+    for (int s = 0; s < ns; ++s) {
+        const double ne = prior_n[(int64_t)rec * S + s];
+        if (r == 0 && ne != 0.0) ws.occp64[(int64_t)t * S + s] += ne;
+        if (r < R) {
+            const double Fe = prior_F[((int64_t)rec * S + s) * R + r];
+            if (Fe != 0.0) ws.partial64[((int64_t)t * S + s) * R + r] += sphi * Fe;
+        }
+    }
+}
+
+// reg64 += Fb/2 sum_{s,r} [log lambda0 - (lambda0 - 1)(invL + d^2) + mu0 (alpha + d)], d = alpha - mu0: the KL divergence
+// to N(mu0, 1/lambda0) minus the one to N(0, I) that speaker64_kernel wrote
+__global__ void __launch_bounds__(128) prior_reg64_kernel(Plan pl, Workspace ws, const float *__restrict__ Phi,
+                                                          const int32_t *__restrict__ n_states,
+                                                          const double *__restrict__ prior_n,
+                                                          const double *__restrict__ prior_F) {
+    __shared__ double sh[4];
+    const int rec = blockIdx.x;
+    if (!ws.active64[rec]) return;
+    const int S = pl.S, R = pl.R, r = threadIdx.x, lane = r & 31, warp = r >> 5;
+    const bool live = r < R;
+    const int ns = n_states ? n_states[rec] : S;
+    const double phi = live ? (double)Phi[r] : 0.0, c = ws.hp[rec].dFaFb;
+    const int t_lo = pl.mtile_begin[rec], t_hi = pl.mtile_begin[rec + 1];
+    double cor = 0.0;
+    for (int s = 0; s < ns && live; ++s) {
+        const int64_t o = ((int64_t)rec * S + s) * R + r;
+        const double ne = prior_n[(int64_t)rec * S + s], Fe = prior_F[o];
+        if (ne == 0.0 && Fe == 0.0) continue;
+        double Ns = 0.0;   // N_s + n_e, as speaker64_kernel summed it
+        for (int t = t_lo; t < t_hi; ++t) Ns += ws.occp64[(int64_t)t * S + s];
+        const double iL = 1.0 / (1.0 + c * Ns * phi), a = ws.alpha64[o];
+        const double lam0 = 1.0 + c * ne * phi, mu0 = c * sqrt(phi) * Fe / lam0, d = a - mu0;
+        cor += log(lam0) - (lam0 - 1.0) * (iL + d * d) + mu0 * (a + d);
+    }
+    cor = gsum<32>(cor);
+    if (lane == 0) sh[warp] = cor;
+    __syncthreads();
+    if (r == 0) {
+        const double tot = (sh[0] + sh[1]) + (sh[2] + sh[3]);
+        if (tot != 0.0) ws.reg64[rec] += 0.5 * ws.hp[rec].dFb * tot;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // log-likelihoods in float64.  One CTA per M-tile, processed in blocks of 64 frames: rho block transposed in
 // shared memory, alpha [r][s] in shared memory, warp = (state quarter, frame half), lane = frame.  S = 128: blocks of 32
 // frames and warp = state eighth (the 64-frame layout would need 225 KB of shared memory).
@@ -514,7 +575,8 @@ int launch_snapshot(const Plan &pl, const Workspace &ws, const float *gamma, con
 template <int S_PAD>
 static int launch_exact64_t(const Plan &pl, const Workspace &ws, const RunParams &rp, const float *rho, const float *Phi,
                             float *gamma, float *pi, const int32_t *n_states, float *alpha_io, float *invL_io, double *Li,
-                            int32_t *n_iters, int32_t *flags, cudaStream_t st) {
+                            int32_t *n_iters, int32_t *flags, cudaStream_t st, const double *prior_n,
+                            const double *prior_F) {
     constexpr int SPL = S_PAD > kMaxS ? 4 : (S_PAD >= 16 ? 2 : 1);
     constexpr int RPW = 32 / (S_PAD / SPL);
     constexpr int FB = x64::loglik64_frames<S_PAD>();
@@ -529,20 +591,24 @@ static int launch_exact64_t(const Plan &pl, const Workspace &ws, const RunParams
     }
     x64::restore64_kernel<<<pl.n_mtiles, 256, 0, st>>>(pl, ws, gamma, n_iters);
     x64::mstep64_kernel<S_PAD><<<pl.n_mtiles, 256, sm_m, st>>>(pl, ws, rho, gamma);
+    if (prior_n) x64::prior_stats64_kernel<<<pl.n_rec, 128, 0, st>>>(pl, ws, Phi, n_states, prior_n, prior_F);
     x64::speaker64_kernel<<<pl.n_rec, 128, 0, st>>>(pl, ws, rp, Phi, n_states, alpha_io, invL_io);
+    if (prior_n) x64::prior_reg64_kernel<<<pl.n_rec, 128, 0, st>>>(pl, ws, Phi, n_states, prior_n, prior_F);
     x64::loglik64_kernel<S_PAD><<<pl.n_mtiles, 256, sm_l, st>>>(pl, ws, rp, rho);
     const int warps = (pl.n_rec + RPW - 1) / RPW;
     x64::fb64_kernel<S_PAD, SPL><<<(warps + 3) / 4, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);
     x64::elbo64_kernel<<<pl.n_rec, 128, 0, st>>>(pl, ws, rp, Li, n_iters, flags);
-    return cudaGetLastError() == cudaSuccess ? 6 : -1;
+    return cudaGetLastError() == cudaSuccess ? (prior_n ? 8 : 6) : -1;
 }
 
 // One float64 iteration for every recording in the finishing phase (ws.active64).
 int launch_exact64_round(const Plan &pl, const Workspace &ws, const RunParams &rp, const float *rho, const float *Phi,
                          float *gamma, float *pi, const int32_t *n_states, float *alpha_io, float *invL_io, double *Li,
-                         int32_t *n_iters, int32_t *flags, cudaStream_t st) {
+                         int32_t *n_iters, int32_t *flags, cudaStream_t st, const double *prior_n,
+                         const double *prior_F) {
     if (pl.n_rec == 0 || pl.n_mtiles == 0) return 0;
-#define VBX_X64(S_) return launch_exact64_t<S_>(pl, ws, rp, rho, Phi, gamma, pi, n_states, alpha_io, invL_io, Li, n_iters, flags, st)
+#define VBX_X64(S_) return launch_exact64_t<S_>(pl, ws, rp, rho, Phi, gamma, pi, n_states, alpha_io, invL_io, Li, n_iters, flags, st, \
+                                                prior_n, prior_F)
     switch (pl.S) {
         case 4: VBX_X64(4);
         case 8: VBX_X64(8);

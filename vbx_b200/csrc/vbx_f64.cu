@@ -70,8 +70,11 @@ __global__ void __launch_bounds__(128) prep_kernel(Plan pl, Buffers b, const dou
 }
 
 // M-step for one (recording, speaker): invL, alpha over r (threads stride the features)      VBx/VBx.py:95-96
-__global__ void __launch_bounds__(128) mstep_kernel(Plan pl, Buffers b, const double *__restrict__ gamma,
-                                                    const double *__restrict__ Phi, const int32_t *n_states, double FaFb) {
+// PRIOR (here and in bias_body): the enrolment prior of prior_n [B,S], prior_F [B,S,R] (DESIGN.md section 5.23)
+template <bool PRIOR>
+__device__ __forceinline__ void mstep_body(const Plan &pl, const Buffers &b, const double *__restrict__ gamma,
+                                           const double *__restrict__ Phi, const int32_t *n_states, double FaFb,
+                                           const double *__restrict__ prior_n, const double *__restrict__ prior_F) {
     const int rec = blockIdx.x / pl.S, s = blockIdx.x % pl.S;
     if (!b.active[rec]) return;
     const int R = pl.R, S = pl.S;
@@ -91,15 +94,33 @@ __global__ void __launch_bounds__(128) mstep_kernel(Plan pl, Buffers b, const do
             Ns += g;
             gr += g * b.rho[(f0 + t) * R + r];
         }
+        if constexpr (PRIOR) {
+            Ns += prior_n[(int64_t)rec * S + s];
+            gr += sqrt(Phi[r]) * prior_F[o];
+        }
         const double iL = 1.0 / (1.0 + FaFb * Ns * Phi[r]);
         b.invL[o] = iL;
         b.alpha[o] = FaFb * iL * gr;
     }
 }
 
+__global__ void __launch_bounds__(128) mstep_kernel(Plan pl, Buffers b, const double *__restrict__ gamma,
+                                                    const double *__restrict__ Phi, const int32_t *n_states, double FaFb) {
+    mstep_body<false>(pl, b, gamma, Phi, n_states, FaFb, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(128) mstep_prior_kernel(Plan pl, Buffers b, const double *__restrict__ gamma,
+                                                          const double *__restrict__ Phi, const int32_t *n_states,
+                                                          double FaFb, const double *__restrict__ prior_n,
+                                                          const double *__restrict__ prior_F) {
+    mstep_body<true>(pl, b, gamma, Phi, n_states, FaFb, prior_n, prior_F);
+}
+
 // per-speaker bias of eq. (23) and the ELBO regulariser of eq. (25)           VBx/VBx.py:97,100
-__global__ void __launch_bounds__(128) bias_kernel(Plan pl, Buffers b, const double *__restrict__ Phi,
-                                                   const int32_t *n_states, double Fb) {
+template <bool PRIOR>
+__device__ __forceinline__ void bias_body(const Plan &pl, const Buffers &b, const double *__restrict__ Phi,
+                                          const int32_t *n_states, double Fb, double FaFb,
+                                          const double *__restrict__ prior_n, const double *__restrict__ prior_F) {
     __shared__ double sh[4];
     const int rec = blockIdx.x;
     if (!b.active[rec]) return;
@@ -114,6 +135,15 @@ __global__ void __launch_bounds__(128) bias_kernel(Plan pl, Buffers b, const dou
                 const double iL = b.invL[o], a = b.alpha[o];
                 c += (iL + a * a) * Phi[r];
                 reg += log(iL) - iL - a * a + 1.0;
+                if constexpr (PRIOR) {   // log(lambda0 iL) - lambda0 iL - lambda0 (a - mu0)^2 + 1: the terms of
+                    // speaker_model_body, each with a factor lambda0 - 1 or mu0 (exactly 0 without a prior)
+                    const double ne = prior_n[(int64_t)rec * S + s], Fe = prior_F[o];
+                    if (ne != 0.0 || Fe != 0.0) {
+                        const double lam0 = 1.0 + FaFb * ne * Phi[r];
+                        const double mu0 = FaFb * sqrt(Phi[r]) * Fe / lam0, d = a - mu0;
+                        reg += log(lam0) - (lam0 - 1.0) * (iL + d * d) + mu0 * (a + d);
+                    }
+                }
             }
         }
         c = block_sum(c, sh);
@@ -121,6 +151,18 @@ __global__ void __launch_bounds__(128) bias_kernel(Plan pl, Buffers b, const dou
     }
     reg = block_sum(reg, sh);
     if (threadIdx.x == 0) b.reg[rec] = 0.5 * Fb * reg;
+}
+
+__global__ void __launch_bounds__(128) bias_kernel(Plan pl, Buffers b, const double *__restrict__ Phi,
+                                                   const int32_t *n_states, double Fb) {
+    bias_body<false>(pl, b, Phi, n_states, Fb, 0.0, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(128) bias_prior_kernel(Plan pl, Buffers b, const double *__restrict__ Phi,
+                                                         const int32_t *n_states, double Fb, double FaFb,
+                                                         const double *__restrict__ prior_n,
+                                                         const double *__restrict__ prior_F) {
+    bias_body<true>(pl, b, Phi, n_states, Fb, FaFb, prior_n, prior_F);
 }
 
 // log-likelihoods, row max, exp: one thread per frame                          VBx/VBx.py:97
@@ -351,7 +393,7 @@ size_t f64_workspace_bytes(const Plan &pl) {
 int launch_run_f64(const Plan &pl, void *workspace, const double *fea, const double *Phi, double *gamma, double *pi,
                    const int32_t *n_states, double Fa, double Fb, double loopP, int max_iters, double epsilon,
                    double *alpha_io, double *invL_io, int warm, double *Li, int32_t *n_iters, int32_t *flags,
-                   cudaStream_t st) {
+                   cudaStream_t st, const double *prior_n, const double *prior_F) {
     if (pl.n_rec == 0) return 0;
     const size_t N = (size_t)pl.n_frames, S = (size_t)pl.S, R = (size_t)pl.R, B = (size_t)pl.n_rec;
     f64::Buffers b;
@@ -386,10 +428,16 @@ int launch_run_f64(const Plan &pl, void *workspace, const double *fea, const dou
     }
     for (int it = 0; it < max_iters; ++it) {
         if (!(it == 0 && warm)) {
-            f64::mstep_kernel<<<pl.n_rec * pl.S, 128, 0, st>>>(pl, b, gamma, Phi, n_states, Fa / Fb);
+            if (prior_n)
+                f64::mstep_prior_kernel<<<pl.n_rec * pl.S, 128, 0, st>>>(pl, b, gamma, Phi, n_states, Fa / Fb, prior_n, prior_F);
+            else
+                f64::mstep_kernel<<<pl.n_rec * pl.S, 128, 0, st>>>(pl, b, gamma, Phi, n_states, Fa / Fb);
             ++launches;
         }
-        f64::bias_kernel<<<pl.n_rec, 128, 0, st>>>(pl, b, Phi, n_states, Fb);
+        if (prior_n)
+            f64::bias_prior_kernel<<<pl.n_rec, 128, 0, st>>>(pl, b, Phi, n_states, Fb, Fa / Fb, prior_n, prior_F);
+        else
+            f64::bias_kernel<<<pl.n_rec, 128, 0, st>>>(pl, b, Phi, n_states, Fb);
         if (fblocks) f64::loglik_kernel<<<fblocks, 128, 0, st>>>(pl, b, Fa);
         if (pl.S <= 64)
             f64::fb_kernel_small<<<pl.n_rec, 32, 0, st>>>(pl, b, gamma, pi, n_states, Fa, loopP, epsilon, Li, n_iters, flags, it, max_iters);

@@ -239,9 +239,10 @@ int launch_run_init(const Plan &pl, const Workspace &ws, const float *gamma, con
                     int32_t *n_iters, int32_t *flags, int max_iters, double Fa, double Fb, double loopP,
                     const double *Fa_v, const double *Fb_v, const double *loopP_v, cudaStream_t st);
 int launch_mstep_partial(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, cudaStream_t st);
+// prior_n [n_rec,S], prior_F [n_rec,S,R] (DEVICE, both or neither): the enrolment prior of DESIGN.md section 5.23
 int launch_speaker_model(const Plan &pl, const Workspace &ws, const float *Phi,
                          const int32_t *n_states, float *alpha_io, float *invL_io, bool from_given,
-                         cudaStream_t st);
+                         cudaStream_t st, const double *prior_n = nullptr, const double *prior_F = nullptr);
 int launch_loglik(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                   cudaStream_t st);
 int launch_forward_backward(const Plan &pl, const Workspace &ws, const RunParams &rp, float *gamma, float *pi,
@@ -262,13 +263,14 @@ int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, con
 int launch_snapshot(const Plan &pl, const Workspace &ws, const float *gamma, const float *pi, int iter, cudaStream_t st);
 int launch_exact64_round(const Plan &pl, const Workspace &ws, const RunParams &rp, const float *rho, const float *Phi,
                          float *gamma, float *pi, const int32_t *n_states, float *alpha_io, float *invL_io, double *Li,
-                         int32_t *n_iters, int32_t *flags, cudaStream_t st);
+                         int32_t *n_iters, int32_t *flags, cudaStream_t st, const double *prior_n = nullptr,
+                         const double *prior_F = nullptr);
 // float64 "exact" path (vbx_f64.cu)
 size_t f64_workspace_bytes(const Plan &pl);
 int launch_run_f64(const Plan &pl, void *workspace, const double *fea, const double *Phi, double *gamma, double *pi,
                    const int32_t *n_states, double Fa, double Fb, double loopP, int max_iters, double epsilon,
                    double *alpha_io, double *invL_io, int warm, double *Li, int32_t *n_iters, int32_t *flags,
-                   cudaStream_t st);
+                   cudaStream_t st, const double *prior_n = nullptr, const double *prior_F = nullptr);
 int launch_hard_labels(const Plan &pl, const float *gamma, const int32_t *n_states, int32_t *first, int32_t *second,
                        cudaStream_t st);
 // labels over the keep[b] states of largest posterior mass (vbx_count.cu)

@@ -427,11 +427,16 @@ int launch_mstep_partial(const Plan &pl, const Workspace &ws, const float *rho, 
 // speaker model: invL, alpha (eqs 17,16; VBx/VBx.py:95-96), the per-speaker bias of eq. (23)
 // (VBx/VBx.py:97) and the per-speaker parts of the ELBO regulariser of eq. (25) (VBx/VBx.py:100).  One CTA per
 // recording, four 128-thread warp-groups each taking every 4th speaker, thread = r.  Sums over tiles run in tile order in float64 (deterministic).
+// PRIOR (DESIGN.md section 5.23): state s of recording rec starts from the Gaussian prior of prior_n [n_rec,S]
+// enrolment x-vectors with feature sum prior_F [n_rec,S,R] instead of N(0, I): n_e joins N_s and sqrt(Phi) F_e joins
+// gamma^T rho before invL and alpha, and the regulariser becomes the KL divergence to N(mu0, 1/lambda0).  Its prior
+// terms are a float64 correction to the float32 terms, exactly 0 for n_e = 0 and F_e = 0.
 // ------------------------------------------------------------------------------------------------
-template <int S8, bool R128>
-__global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace ws, const float *__restrict__ Phi,
-                                                            const int32_t *__restrict__ n_states, float *alpha_io,
-                                                            float *invL_io, int from_given) {
+template <int S8, bool R128, bool PRIOR>
+__device__ __forceinline__ void speaker_model_body(const Plan &pl, const Workspace &ws, const float *__restrict__ Phi,
+                                                   const int32_t *__restrict__ n_states, float *alpha_io, float *invL_io,
+                                                   int from_given, const double *__restrict__ prior_n,
+                                                   const double *__restrict__ prior_F) {
     // one CTA per recording; four 128-thread warp-groups, each takes every 4th speaker, thread = r
     const int S = pl.S, R = pl.R;
     constexpr int NT = S8 / 8, NSP = S8 / 4;   // speakers per warp-group
@@ -467,13 +472,18 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
         const bool dead = s >= ns;   // dead (or padding) column: never wins, never contributes
         float invL = 1.f, alpha = 0.f, Av = 0.f;
         float c = 0.f, reg = 0.f;
+        double cor = 0.0;   // PRIOR only
         if (live && !dead) {
             if (from_given) {
                 alpha = alpha_io[o];
                 invL = invL_io[o];
             } else {
-                const double gr = grs[k];
-                const float Ns = ws.occ[(int64_t)rec * S + s];
+                double gr = grs[k];
+                float Ns = ws.occ[(int64_t)rec * S + s];
+                if constexpr (PRIOR) {
+                    gr += sqrt((double)phi) * prior_F[o];
+                    Ns = (float)((double)Ns + prior_n[(int64_t)rec * S + s]);
+                }
                 invL = 1.f / (1.f + FaFb * Ns * phi);
                 alpha = (float)((double)(FaFb * invL) * gr);
             }
@@ -481,6 +491,17 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
             const float a2 = alpha * alpha;
             reg = logf(invL) - invL - a2 + 1.f;
             c = (invL + a2) * phi;
+            // log(lambda0 invL) - lambda0 invL - lambda0 (alpha - mu0)^2 + 1 minus reg, in float64, written so that every
+            // term has a factor lambda0 - 1 or mu0 (exactly 0 without a prior, whatever the compiler contracts)
+            if constexpr (PRIOR) {
+                const double ne = prior_n[(int64_t)rec * S + s], Fe = prior_F[o];
+                if (ne != 0.0 || Fe != 0.0) {
+                    const double lam0 = 1.0 + ws.hp[rec].dFaFb * ne * (double)phi;
+                    const double mu0 = ws.hp[rec].dFaFb * sqrt((double)phi) * Fe / lam0;
+                    const double a = alpha, d = a - mu0;
+                    cor = log(lam0) - (lam0 - 1.0) * ((double)invL + d * d) + mu0 * (a + d);
+                }
+            }
         }
         if (live && s < S) {
             ws.A[o] = Av;
@@ -492,9 +513,10 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
         sAv[s * kMaxR + r] = Av;                          // columns >= R hold 0
         c = group_sum<32>(c);                             // 32 terms in float, the rest in float64
         reg = group_sum<32>(reg);
+        if constexpr (PRIOR) cor = warp_sum_d(cor);
         if (lane == 0) {
             cpart[s][warp] = (double)c;
-            rpart[s][warp] = (double)reg;
+            rpart[s][warp] = PRIOR ? (double)reg + cor : (double)reg;
         }
     }
     }
@@ -523,23 +545,51 @@ __global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace w
     }
 }
 
+template <int S8, bool R128>
+__global__ void __launch_bounds__(512) speaker_model_kernel(Plan pl, Workspace ws, const float *__restrict__ Phi,
+                                                            const int32_t *__restrict__ n_states, float *alpha_io,
+                                                            float *invL_io, int from_given) {
+    speaker_model_body<S8, R128, false>(pl, ws, Phi, n_states, alpha_io, invL_io, from_given, nullptr, nullptr);
+}
+
+template <int S8, bool R128>
+__global__ void __launch_bounds__(512) speaker_model_prior_kernel(Plan pl, Workspace ws, const float *__restrict__ Phi,
+                                                                  const int32_t *__restrict__ n_states, float *alpha_io,
+                                                                  float *invL_io, int from_given,
+                                                                  const double *__restrict__ prior_n,
+                                                                  const double *__restrict__ prior_F) {
+    speaker_model_body<S8, R128, true>(pl, ws, Phi, n_states, alpha_io, invL_io, from_given, prior_n, prior_F);
+}
+
 int launch_speaker_model(const Plan &pl, const Workspace &ws, const float *Phi,
                          const int32_t *n_states, float *alpha_io, float *invL_io, bool from_given,
-                         cudaStream_t st) {
+                         cudaStream_t st, const double *prior_n, const double *prior_F) {
     if (pl.n_rec == 0) return 0;
     const int S8 = pl.S > 8 ? pl.S : 8;
     const size_t smem = (size_t)S8 * kMaxR * sizeof(float);
     const int fg = from_given ? 1 : 0;
+    const bool prior = prior_n != nullptr;
     if (S8 == kMaxSWide) {   // 64 KB of staged Fa*alpha: above the default dynamic shared-memory limit
-        static bool configured = false;
-        if (!configured) {
+        static bool configured = false, configured_prior = false;
+        if (!prior && !configured) {
             if (cudaFuncSetAttribute(speaker_model_kernel<kMaxSWide, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
                 cudaFuncSetAttribute(speaker_model_kernel<kMaxSWide, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
                 return -1;
             configured = true;
         }
+        if (prior && !configured_prior) {
+            if (cudaFuncSetAttribute(speaker_model_prior_kernel<kMaxSWide, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
+                cudaFuncSetAttribute(speaker_model_prior_kernel<kMaxSWide, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+                return -1;
+            configured_prior = true;
+        }
     }
-#define VBX_SM(S8_, R_) speaker_model_kernel<S8_, R_><<<pl.n_rec, 512, smem, st>>>(pl, ws, Phi, n_states, alpha_io, invL_io, fg)
+#define VBX_SM(S8_, R_)                                                                                                     \
+    if (prior)                                                                                                              \
+        speaker_model_prior_kernel<S8_, R_><<<pl.n_rec, 512, smem, st>>>(pl, ws, Phi, n_states, alpha_io, invL_io, fg,      \
+                                                                         prior_n, prior_F);                                 \
+    else                                                                                                                    \
+        speaker_model_kernel<S8_, R_><<<pl.n_rec, 512, smem, st>>>(pl, ws, Phi, n_states, alpha_io, invL_io, fg)
     if (pl.R == 128) {
         switch (S8) {
             case 8: VBX_SM(8, true); break;

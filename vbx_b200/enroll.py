@@ -236,6 +236,47 @@ def enroll_names(table, assign, best_llr, enrolled_names, recording_names, label
     return names, llrs
 
 
+def prior_states(result, enrolled_names, n_states):
+    """The enrolment prior of the VB-HMM's states (DESIGN.md section 5.23) from an assignment of each recording's AHC
+    clusters (enroll_speakers over the AHC labels: cluster l of recording b is state l).  n_states: the state count of
+    every recording.  Returns (prior, prior_speakers): prior[b] is None when no cluster of recording b was assigned,
+    else (n [n_states[b]], F [n_states[b], R]) float64 with the assigned enrolled speaker's n_enroll, F_enroll in the
+    row of its state and zeros elsewhere; prior_speakers[b] = {state: enrolled name}."""
+    R = np.asarray(result.F_enroll).shape[1]
+    prior = [None] * len(n_states)
+    named = [{} for _ in n_states]
+    for b, l, a in zip(result.table.rec.tolist(), result.table.label.tolist(), np.asarray(result.assign).tolist()):
+        if a < 0:
+            continue
+        if prior[b] is None:
+            prior[b] = (np.zeros(int(n_states[b])), np.zeros((int(n_states[b]), R)))
+        prior[b][0][l] = result.n_enroll[a]
+        prior[b][1][l] = result.F_enroll[a]
+        named[b][l] = enrolled_names[a]
+    return prior, named
+
+
+def carry_assignment(result, labels):
+    """The assignment of an enroll_speakers result over the AHC labels carried to the final labels of the VB-HMM that
+    started from them (every final label is one of the AHC clusters, its state).  Returns (table, assign, best) over
+    link.speaker_table(labels), for enroll_names."""
+    row = {(b, l): i for i, (b, l) in enumerate(zip(result.table.rec.tolist(), result.table.label.tolist()))}
+    table = speaker_table(labels)
+    idx = np.array([row[(b, l)] for b, l in zip(table.rec.tolist(), table.label.tolist())], dtype=np.int64)
+    return table, np.asarray(result.assign)[idx], np.asarray(result.best_llr)[idx]
+
+
+def name_prior_states(names, prior_speakers):
+    """The names of enroll_names with every state that carried an enrolment prior (prior_states' prior_speakers) named
+    by its enrolled speaker, also where it survived the VB-HMM as a second label only.  Changes names in place and
+    returns it."""
+    for nm, pr in zip(names, prior_speakers):
+        for l, name in pr.items():
+            if l in nm:
+                nm[l] = name
+    return names
+
+
 def mask_named(labels, names):
     """An int label array with the labels of enrolled (not unknown-) speakers set to -1 (None stays None)."""
     if labels is None:

@@ -146,11 +146,16 @@ class PartitionedBatch:
     def output_buffers(self, maxIters):
         return None               # the parts allocate their own outputs
 
-    def run(self, gamma, pi, alpha=None, invL=None, buffers=None, **kw):
+    def run(self, gamma, pi, alpha=None, invL=None, buffers=None, prior=None, **kw):
         main = torch.cuda.current_stream(self.device)
+        if prior is not None:      # checked whole, so that a bad prior is refused before any part launches
+            from .batch import check_prior
+            prior = check_prior(prior, self.B, self.S, self.R, self.device)
 
         def one(c, fs, rs):
             extra = {}
+            if prior is not None:
+                extra['prior'] = (prior[0][rs], prior[1][rs])
             if alpha is not None:
                 extra['alpha'] = alpha[rs]
             if invL is not None:

@@ -171,7 +171,7 @@ def keep_labels(gamma, keep):
 
 
 def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None, turns=None, random=None, elbo=False,
-             **run_kw):
+             prior=None, **run_kw):
     """The VB-HMM step (VBx/vbhmm.py:150-162) for the recordings of one state tier, packed: fea [N,R] float32, labels [N]
     AHC labels (device); turns: None, or a resegment.TurnPack of the recordings, which then start from their init
     RTTM's turns instead (vbx_init_turns, DESIGN.md section 5.20; labels is not read).  f64: the float64 kernels
@@ -182,7 +182,8 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None
     the tier), and each tuple gains the unconstrained speaker count and 'vb' or 'mass'.  random: None, or (keys, seeds),
     one integer each per recording: the recordings then start from vbx_init_random's draws (DESIGN.md section 5.22;
     labels is not read).  elbo: every tuple also ends with the recording's final ELBO Li[b, n_iters[b] - 1] (NaN
-    without iterations)."""
+    without iterations).  prior: None, or per recording None or its states' enrolment prior (n [ns], F [ns, R])
+    (enroll.prior_states, DESIGN.md section 5.23); the batch then runs with it, zeros for the other states."""
     from .batch import VbxBatch, run_f64
     offs = np.concatenate([[0], np.cumsum(lens)])
     dt = torch.float64 if f64 else torch.float32
@@ -199,6 +200,12 @@ def _vb_tier(lens, ns, fea, Phi, labels, f64, smoothing, dev, make=None, hi=None
         for b in range(vb.B):          # VBx/vbhmm.py:150-152: qinit = softmax(onehot * smoothing)
             g[offs[b]:offs[b + 1], :ns[b]] = soft_init(labels[offs[b]:offs[b + 1]], int(ns[b]), float(sm[b]), dtype=dt)
             p[b, :ns[b]] = 1.0 / ns[b]
+    if prior is not None and any(x is not None for x in prior):
+        n_h, F_h = np.zeros((vb.B, vb.S)), np.zeros((vb.B, vb.S, vb.R))
+        for b, x in enumerate(prior):
+            if x is not None:
+                n_h[b, :len(x[0])], F_h[b, :len(x[0])] = x
+        run_kw = dict(run_kw, prior=(torch.from_numpy(n_h).to(dev), torch.from_numpy(F_h).to(dev)))
     if f64:
         res = run_f64(vb, fea.double().contiguous(), Phi.double().contiguous(), g, p, **run_kw)   # VBx/vbhmm.py:154-158
         top2 = [hard_labels(g[offs[b]:offs[b + 1], :ns[b]], second=True) for b in range(vb.B)]   # VBx/vbhmm.py:160-162
@@ -244,7 +251,7 @@ def _tier(n_states):
 
 
 def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, make, split, turns=None, random=None,
-              **run_kw):
+              prior=None, **run_kw):
     """Everything after AHC (VBx/vbhmm.py:147-162 and the speaker-count rules of DESIGN.md section 5.14) for the entries
     (k, b): setting k of `hyper`, a list of (Fa, Fb, loopP, smoothing), on recording b.  labels[k]: setting k's AHC
     labels per recording; labels_d[k]: their concatenation on the device (used by init='AHC+VB' only).  fea [N,R] float32
@@ -263,7 +270,8 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
     restart r of (k, b), with random = random_init.RandomStart: random.n_states states each, every batch started by one
     vbx_init_random launch (key random.keys[b], seed random.seed + r); each (k, b) then keeps the restart of largest
     final ELBO (random_init.best_restart) before the count rules, and its tuple ends with (restart, [final ELBO of every
-    restart]).  Returns {(k, b): (labels, labels2nd or None, iterations, flags[, n_speakers_vb, count_rule])}, the last
+    restart]).  prior: None, or per recording None or the enrolment prior of its AHC states (enroll.prior_states,
+    DESIGN.md section 5.23; init='AHC+VB' without bounds only).  Returns {(k, b): (labels, labels2nd or None, iterations, flags[, n_speakers_vb, count_rule])}, the last
     two under bounds."""
     from . import ahc as _ahc
     B = len(lens)
@@ -313,6 +321,8 @@ def _vb_stage(hyper, labels, labels_d, Zs, lens, fea, Phi, bounds, init, dev, ma
                 Fa, Fb, loopP = (torch.tensor([hyper[e[0]][i] for e in group], dtype=torch.float64, device=dev)
                                  for i in range(3))
                 smoothing = [hyper[e[0]][3] for e in group]
+            if prior is not None:
+                init_kw = dict(init_kw, prior=[prior[b] for b in recs])
             sub = _vb_tier(lens[recs], np.array([ns[e] for e in group], dtype=np.int32), g_fea, Phi, g_labels, f64,
                            smoothing, dev, make=make, hi=None if hi is None else hi[recs],
                            Fa=Fa, Fb=Fb, loopProb=loopP, **init_kw, **run_kw)
@@ -508,7 +518,7 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
                   max_iters=40, epsilon=1e-6, device=None, chain='auto', output_2nd=False, overlaps=None,
                   num_speakers=None, min_speakers=None, max_speakers=None, link_threshold=None, enroll=None,
                   enroll_threshold=None, cohort=None, cohort_top=200, init_rttm=None, init_states=None, restarts=None,
-                  seed=None):
+                  seed=None, enroll_prior=False):
     """Every recording of an archive in one call on the device - the body of the loop VBx/vbhmm.py:120-179 for all
     recordings at once: x-vector transform + PLDA projection (vbx_prepare_xvectors) and AHC initialisation (vbx_ahc) as
     one batch, then the VB-HMM with the reference's stop rule (vbx_run) and hard labels (vbx_hard_labels) as one batch
@@ -563,11 +573,20 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
     largest cohort scores), so link_threshold and enroll_threshold are on S; needs link_threshold or enroll.  Each item
     then also has score_norm = {'top_k': min(cohort_top, C), 'cohort_speakers': C}, and with enroll speaker_score
     ({label: the normalised score that decided the name}) in place of speaker_llr.
+    enroll_prior: with enroll and init='AHC+VB' (no count bounds), the enrolled speakers take part in the VB-HMM
+    (DESIGN.md section 5.23): each recording's AHC clusters are assigned to enrolled speakers as its final speakers
+    would be (enroll.enroll_speakers at enroll_threshold, on the normalised score with a cohort), and the state of an
+    assigned cluster starts from the enrolled speaker's x-vectors as its speaker prior (VbxBatch.run(prior=)).  Such a
+    state is named by that speaker (also where it survives as a second label only), every other as without
+    enroll_prior; speaker_llr (speaker_score) holds the cluster's value from that assignment for a prior state and the
+    post-hoc value for every other.  Each item then also has prior_speakers ({state: enrolled name}).  Without any
+    assignment the VB-HMM runs exactly as without enroll_prior.
     Returns {name: dict(rttm, labels, labels2nd or None, n_speakers, iterations[, rttm_overlap, overlap_seconds]
     [, count_rule, n_speakers_vb, count][, global_speakers, rttm_linked][, speaker_names, speaker_llr or speaker_score,
-    rttm_named][, score_norm][, init_speakers, rttm_init])}."""
+    rttm_named][, prior_speakers][, score_norm][, init_speakers, rttm_init])}."""
     random = _check_init(init, overlaps is not None, init_rttm, init_states, restarts, seed)
     bounds = count_bounds(list(recordings), num_speakers, min_speakers, max_speakers)
+    check_enroll_prior(enroll_prior, enroll is not None, init, bounds is not None)
     if link_threshold is not None:
         from .link import check_threshold
         check_threshold(link_threshold)
@@ -612,24 +631,50 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
         from .random_init import name_key
         random = random._replace(keys=[name_key(n) for n in names])
     from .batch import VbxBatch
+    side = lambda sets: _side_features(sets, recordings, names, transform, plda, lda_dim, chain, dev, fea, Phi)
+    enrolled_fea = cohort_fea = matched = prior = prior_speakers = None
+    if enroll_prior:                   # the AHC clusters assigned to enrolled speakers, section 5.23
+        from . import enroll as _enroll
+        enrolled_fea = side(enrolled)
+        norm_ahc = None
+        if cohort_set is not None:
+            cohort_fea = side(cohort_set)
+            norm_ahc = _cohort_norm(cohort_fea, cohort_top, enrolled, enrolled_fea, names, fea, Phi, offs, ahc_labels,
+                                    Fa, Fb, dev)
+        matched = _enroll.enroll_speakers(fea, Phi, offs, ahc_labels, *enrolled_fea, Fa, Fb, enroll_threshold, dev,
+                                          norm=_enroll_norm(norm_ahc))
+        prior, prior_speakers = _enroll.prior_states(matched, [k for k, _ in enrolled],
+                                                     [int(l.max()) + 1 if len(l) else 1 for l in ahc_labels])
+        if all(x is None for x in prior):
+            prior = None
     res = _vb_stage([(Fa, Fb, loopP, smoothing)], [ahc_labels], labels_d, Zs, lens, fea, Phi, bounds, init, dev,
-                    VbxBatch, None, turns=turns, random=random, maxIters=max_iters, epsilon=epsilon)
+                    VbxBatch, None, turns=turns, random=random, prior=prior, maxIters=max_iters, epsilon=epsilon)
     res = [res[(0, b)] for b in range(len(names))]
     labels1, labels2 = [r[0] for r in res], [r[1] for r in res]
     out = {}
     maps = None
-    side = lambda sets: _side_features(sets, recordings, names, transform, plda, lda_dim, chain, dev, fea, Phi)
-    enrolled_fea = side(enrolled) if enrolled is not None else None
+    if enrolled is not None and enrolled_fea is None:
+        enrolled_fea = side(enrolled)
     norm = None
     if cohort_set is not None:
-        norm = _cohort_norm(side(cohort_set), cohort_top, enrolled, enrolled_fea, names, fea, Phi, offs, labels1, Fa,
-                            Fb, dev)
+        norm = _cohort_norm(side(cohort_set) if cohort_fea is None else cohort_fea, cohort_top, enrolled, enrolled_fea,
+                            names, fea, Phi, offs, labels1, Fa, Fb, dev)
     if link_threshold is not None:
         from . import link as _link
         table, _, _, Z = _link.link_speakers(fea, Phi, offs, labels1, Fa, Fb, dev,
                                              norm=None if norm is None else norm['archive'][:2])
         maps = _link.link_cut(Z, table, link_threshold, labels2)
-    if enrolled is not None:
+    if matched is not None:
+        # prior states keep the assignment that attached the prior and its cluster-level value; every other speaker
+        # reports the value post-hoc enrolment gives it
+        table, assign, best = _enroll.carry_assignment(matched, labels1)
+        post = _enroll.enroll_speakers(fea, Phi, offs, labels1, *enrolled_fea, Fa, Fb, enroll_threshold, dev,
+                                       norm=_enroll_norm(norm))
+        best = np.where(assign >= 0, best, post.best_llr)
+        spk_names, spk_llr = _name_archive(table, assign, best, [k for k, _ in enrolled], link_threshold, names, dev,
+                                           fea, Phi, offs, labels1, labels2, Fa, Fb, norm)
+        _enroll.name_prior_states(spk_names, prior_speakers)
+    elif enrolled is not None:
         spk_names, spk_llr = _enroll_archive(enrolled, enrolled_fea, enroll_threshold, link_threshold, names, dev, fea,
                                              Phi, offs, labels1, labels2, Fa, Fb, norm)
     for b, n in enumerate(names):
@@ -647,6 +692,8 @@ def diarize_batch(recordings, transform, plda, Fa, Fb, loopP, lda_dim=128, thres
             out[n].update(speaker_names=spk_names[b], rttm_named=named_lines(n, recordings[n][1], labels1[b], labels2[b],
                                                                              spk_names[b], ovl))
             out[n]['speaker_llr' if norm is None else 'speaker_score'] = spk_llr[b]
+        if prior_speakers is not None:
+            out[n]['prior_speakers'] = prior_speakers[b]
         if norm is not None:
             out[n]['score_norm'] = {'top_k': norm['K'], 'cohort_speakers': norm['C']}
         if turns is not None:
@@ -718,12 +765,26 @@ def _enroll_archive(enrolled, enrolled_fea, threshold, link_threshold, names, de
     link_threshold).  norm: None or _cohort_norm's statistics (section 5.17): both steps then run on the normalised
     scores.  Returns per recording ({label: name}, {label: llr or normalised score})."""
     from . import enroll as _enroll
-    from . import link as _link
     fea_e, spk_e = enrolled_fea
-    en = None if norm is None else tuple(norm['archive'][:2]) + tuple(norm['enrolled'][:2])
-    res = _enroll.enroll_speakers(fea, Phi, offs, labels1, fea_e, spk_e, Fa, Fb, threshold, dev, norm=en)
-    enrolled_names = [k for k, _ in enrolled]
-    spk_names, spk_llr = _enroll.enroll_names(res.table, res.assign, res.best_llr, enrolled_names, names, labels2)
+    res = _enroll.enroll_speakers(fea, Phi, offs, labels1, fea_e, spk_e, Fa, Fb, threshold, dev, norm=_enroll_norm(norm))
+    return _name_archive(res.table, res.assign, res.best_llr, [k for k, _ in enrolled], link_threshold, names, dev, fea,
+                         Phi, offs, labels1, labels2, Fa, Fb, norm)
+
+
+def _enroll_norm(norm):
+    """The norm= argument of enroll.enroll_speakers from _cohort_norm's statistics (None: plain LLRs)."""
+    return None if norm is None else tuple(norm['archive'][:2]) + tuple(norm['enrolled'][:2])
+
+
+def _name_archive(table, assign, best, enrolled_names, link_threshold, names, dev, fea, Phi, offs, labels1, labels2,
+                  Fa, Fb, norm=None):
+    """The names of section 5.16 from an assignment (table, assign, best) over the final first labels labels1: the
+    enrolled name or an unknown one, the unknown speakers linked among themselves with link_threshold (on the
+    normalised scores with _cohort_norm's statistics norm over labels1).  Returns per recording ({label: name},
+    {label: llr or normalised score})."""
+    from . import enroll as _enroll
+    from . import link as _link
+    spk_names, spk_llr = _enroll.enroll_names(table, assign, best, enrolled_names, names, labels2)
     if link_threshold is not None:
         l1 = [_enroll.mask_named(l, m) for l, m in zip(labels1, spk_names)]
         l2 = [_enroll.mask_named(l, m) for l, m in zip(labels2, spk_names)]
@@ -734,11 +795,24 @@ def _enroll_archive(enrolled, enrolled_fea, threshold, link_threshold, names, de
             t2 = _link.speaker_table(l1)
             idx = np.array([row[(b, l)] for b, l in zip(t2.rec.tolist(), t2.label.tolist())], dtype=np.int64)
             sub = (st.mean[idx], st.std[idx])
-        table, _, _, Z = _link.link_speakers(fea, Phi, offs, l1, Fa, Fb, dev, norm=sub)
-        lk = _link.link_cut(Z, table, link_threshold, l2)
-        spk_names, spk_llr = _enroll.enroll_names(res.table, res.assign, res.best_llr, enrolled_names, names, labels2,
-                                                  link=lk)
+        lt, _, _, Z = _link.link_speakers(fea, Phi, offs, l1, Fa, Fb, dev, norm=sub)
+        lk = _link.link_cut(Z, lt, link_threshold, l2)
+        spk_names, spk_llr = _enroll.enroll_names(table, assign, best, enrolled_names, names, labels2, link=lk)
     return spk_names, spk_llr
+
+
+def check_enroll_prior(enroll_prior, enroll, init, bounds):
+    """ValueError unless enroll_prior comes with enrolled speakers (enroll true), init='AHC+VB' and no speaker-count
+    bounds (bounds true): the prior is attached to AHC clusters, and rule 3 of the bounds would re-run from another
+    cut."""
+    if not enroll_prior:
+        return
+    if not enroll:
+        raise ValueError('enroll_prior attaches enrolled speakers to the VB-HMM: it needs enroll')
+    if init != 'AHC+VB':
+        raise ValueError(f"enroll_prior attaches enrolled speakers to AHC clusters: it needs init='AHC+VB', not {init!r}")
+    if bounds:
+        raise ValueError('enroll_prior does not combine with num_speakers / min_speakers / max_speakers')
 
 
 def rttm_name_lines(recording, starts, ends, names):
