@@ -512,6 +512,26 @@ int vbx_combine(vbx_handle_t h, int32_t n_rec, const int64_t *offsets, int64_t N
                 int32_t *labels2_out, int32_t *order_out, double *weights_out, int64_t *D_out, int32_t *map_out,
                 int32_t *n_global_out, int32_t *flags_out, int64_t *O_out, int64_t *L_out, void *stream);
 
+/* Class statistics for training the x-vector transform and the PLDA (DESIGN.md section 5.24).  Needs a handle, no plan.
+ *   X [N, D] float32 DEVICE, contiguous, 16-byte aligned base (may be NULL when N = 0); rows packed by class, D in
+ *     1 .. 1024
+ *   offsets [K+1] int64 HOST: class i is rows offsets[i] .. offsets[i+1] - 1; from 0 to N, not decreasing; empty
+ *     classes are allowed (mean row 0, no contribution)
+ * Outputs (DEVICE, float64):
+ *   means_out [K, D]     m_i = the float64 mean of class i's rows
+ *   scatter_out [D, D]   sum over rows r of (x_r - m_class(r)) (x_r - m_class(r))^T; both triangles, mirror images bit
+ *                        for bit
+ * Rows are centred by their float64 class mean before the products, which accumulate on the FP64 tensor cores (DMMA)
+ * over the tiles on or above the diagonal only.  Partial tiles of row splits (their number a function of N and D) are
+ * summed in a fixed order without atomics: a call is bit-identical from run to run and independent of what the
+ * workspace held.  workspace: vbx_class_scatter_workspace_bytes(N, D, K) bytes, 256-byte aligned: about 8 K + 4 N bytes
+ * plus 32 KB per (split, tile pair), at most about 36 MB of partial tiles.  Stream ordered, no allocation, no host
+ * synchronisation beyond the one copy of offsets from pageable host memory.  VBX_ERR_ARG: null pointers, D outside
+ * 1 .. 1024, K < 1, N < 0, offsets not from 0 to N or decreasing, a misaligned X or workspace, a short workspace. */
+int vbx_class_scatter_workspace_bytes(vbx_handle_t h, int64_t N, int32_t D, int32_t K, size_t *bytes_out);
+int vbx_class_scatter(vbx_handle_t h, const float *X, int64_t N, int32_t D, int32_t K, const int64_t *offsets,
+                      void *workspace, size_t workspace_bytes, double *means_out, double *scatter_out, void *stream);
+
 /* Number of kernels launched by this handle since creation (bench.py reports it as gpu_launches). */
 int64_t vbx_launch_count(vbx_handle_t h);
 

@@ -1291,6 +1291,45 @@ int vbx_combine(vbx_handle_t h, int32_t n_rec, const int64_t *offsets, int64_t N
                    "combine");
 }
 
+static int check_scatter_sizes(vbx_handle_t h, const std::string &who, int64_t N, int32_t D, int32_t K) {
+    if (N < 0 || K < 1) return fail(h, VBX_ERR_ARG, who + ": N must be >= 0 and K >= 1");
+    if (D < 1 || D > 1024) return fail(h, VBX_ERR_ARG, who + ": D must lie in [1, 1024]");
+    return VBX_OK;
+}
+
+int vbx_class_scatter_workspace_bytes(vbx_handle_t h, int64_t N, int32_t D, int32_t K, size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    const int rc = check_scatter_sizes(h, "vbx_class_scatter_workspace_bytes", N, D, K);
+    if (rc != VBX_OK) return rc;
+    *bytes_out = vbx::class_scatter_workspace_bytes(N, D, K);
+    return VBX_OK;
+}
+
+int vbx_class_scatter(vbx_handle_t h, const float *X, int64_t N, int32_t D, int32_t K, const int64_t *offsets,
+                      void *workspace, size_t workspace_bytes, double *means_out, double *scatter_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_class_scatter");
+    const std::string who("vbx_class_scatter");
+    const int rc = check_scatter_sizes(h, who, N, D, K);
+    if (rc != VBX_OK) return rc;
+    if ((N > 0 && !X) || !offsets || !workspace || !means_out || !scatter_out)
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    if (misaligned16(h, who, {{X, "X"}}) != VBX_OK) return VBX_ERR_ARG;
+    if (offsets[0] != 0 || offsets[K] != N) return fail(h, VBX_ERR_ARG, who + ": offsets must run from 0 to N");
+    for (int32_t i = 0; i < K; ++i)
+        if (offsets[i + 1] < offsets[i])
+            return fail(h, VBX_ERR_ARG, who + ": offsets decrease at class " + std::to_string(i));
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
+        return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
+    if (workspace_bytes < vbx::class_scatter_workspace_bytes(N, D, K))
+        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_class_scatter_workspace_bytes()");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_class_scatter(X, N, D, K, offsets, workspace, means_out, scatter_out,
+                                                (cudaStream_t)stream),
+                   "class_scatter");
+}
+
 int vbx_attach_comm(vbx_handle_t h, void *nccl_comm, int32_t n_ranks, const char *libnccl_path) {
     if (!h) return VBX_ERR_ARG;
     if (!nccl_comm) {   // detach

@@ -394,5 +394,9 @@ int launch_xvector_chain_wgmma(const Plan &pl, float *tc_scratch, const float *x
                                const float *mean2, const float *plda_mu, const float *plda_tr, const float *psi,
                                float *x_norm, float *rho, float *gframe, cudaStream_t st, std::string *err);
 int launch_gsum_from_frames(const Plan &pl, const Workspace &ws, const float *gframe, cudaStream_t st);
+// class means and within-class scatter on the FP64 tensor cores (vbx_train.cu, vbx_class_scatter); offsets_host [K+1]
+size_t class_scatter_workspace_bytes(int64_t N, int D, int64_t K);
+int launch_class_scatter(const float *X, int64_t N, int D, int64_t K, const int64_t *offsets_host, void *workspace,
+                         double *means_out, double *scatter_out, cudaStream_t st);
 
 }  // namespace vbx
