@@ -532,6 +532,51 @@ int vbx_class_scatter_workspace_bytes(vbx_handle_t h, int64_t N, int32_t D, int3
 int vbx_class_scatter(vbx_handle_t h, const float *X, int64_t N, int32_t D, int32_t K, const int64_t *offsets,
                       void *workspace, size_t workspace_bytes, double *means_out, double *scatter_out, void *stream);
 
+/* Streaming diarization (DESIGN.md section 5.25): live streams diarized block by block, each stream's speakers carried
+ * into the VB-HMM as priors.  Needs a handle, no plan.  The state of every stream lives in DEVICE memory that the
+ * caller owns, one row per slot:
+ *   ctx_fea [slots, C, R] float32, ctx_lab [slots, C] int32   a ring of the stream's last min(C, count) projected
+ *                                                             x-vectors and their final labels; x-vector g (0-based,
+ *                                                             in push order) sits at position g mod C
+ *   count [slots] int64                                       x-vectors pushed so far
+ *   K [slots] int32                                           speakers so far (labels 0 .. K-1)
+ *   n_hist [slots, S_max] float64, F_hist [slots, S_max, R]   per speaker, the number and the feature sum of the
+ *     float64                                                 x-vectors that have left the ring, summed in time order
+ * A fresh slot is all zero.  A push delivers blocks of h >= 1 new x-vectors to n streams with DISTINCT slots; all the
+ * per-stream arrays below are DEVICE arrays in push order:
+ *   slot [n] int32                  the stream's slot
+ *   blk_off [n+1] int64             its block is rows blk_off[i] .. blk_off[i+1]-1 of blk_fea [*, R] float32 (projected)
+ *   win_off [n+1] int64             its window is rows win_off[i] .. win_off[i+1]-1, min(C, count) + h of them
+ *   blk_lab [*] int32, n_clusters [n] int32   the block's clusters 0 .. c-1 and c, with K + c <= S_max and K + c <= S
+ *                                   (c = 0 when K = S_max: the block rows then start uniform over the K states)
+ * These contents are read on the device and not validated.
+ * vbx_stream_window writes, at the tier's S (the window plan's padded state count):
+ *   fea_out [Nw, R] float32         [context rows, oldest first; block rows]
+ *   gamma_out [Nw, S] float32       softmax(smoothing * onehot(label)) over the K + c states, 0 in the other columns;
+ *                                   a context row's label is its final label, block row t's is K + blk_lab[t]; evaluated
+ *                                   in float64 and rounded once
+ *   pi_out [n, S] float32           1 / (K + c) in the first K + c columns, 0 in the others
+ *   n_states_out [n] int32          K + c
+ *   prior_n_out [n, S], prior_F_out [n, S, R] float64   n_hist, F_hist for the states k < K, 0 for the others
+ * vbx_stream_commit takes first [Nw] int32, the window's first labels (vbx_hard_labels on the window plan), and writes
+ * labels_out [*] int32, the block's final labels on blk_off: a block row on a state k < K is speaker k, and the fresh
+ * states that hold block rows become speakers K, K+1, ... in order of their first row.  It then adds the rows that
+ * leave the ring (the oldest first) to n_hist / F_hist, one sequential float64 sum per (slot, state, feature) without
+ * atomics, writes the block into the ring and advances count and K.  Context rows are never relabelled.  A stream's
+ * results are bit-identical from run to run, whatever the outputs held before and whatever else the push carries.
+ * Stream ordered, no allocation, no host synchronisation.  VBX_ERR_ARG: a null pointer, n < 0, C < 0, R outside
+ * 1 .. 128, S_max or S outside 1 .. 128. */
+int vbx_stream_window(vbx_handle_t h, int32_t n, int32_t C, int32_t R, int32_t S_max, int32_t S, const int32_t *slot,
+                      const int64_t *blk_off, const int64_t *win_off, const int32_t *blk_lab, const int32_t *n_clusters,
+                      const float *blk_fea, double smoothing, const float *ctx_fea, const int32_t *ctx_lab,
+                      const int64_t *count, const int32_t *K, const double *n_hist, const double *F_hist, float *fea_out,
+                      float *gamma_out, float *pi_out, int32_t *n_states_out, double *prior_n_out, double *prior_F_out,
+                      void *stream);
+int vbx_stream_commit(vbx_handle_t h, int32_t n, int32_t C, int32_t R, int32_t S_max, const int32_t *slot,
+                      const int64_t *blk_off, const int64_t *win_off, const float *blk_fea, const int32_t *first,
+                      float *ctx_fea, int32_t *ctx_lab, int64_t *count, int32_t *K, double *n_hist, double *F_hist,
+                      int32_t *labels_out, void *stream);
+
 /* Number of kernels launched by this handle since creation (bench.py reports it as gpu_launches). */
 int64_t vbx_launch_count(vbx_handle_t h);
 

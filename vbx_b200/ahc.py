@@ -62,6 +62,13 @@ def ahc_batch(vb, x, threshold=-0.015, workspace=None):
     """AHC labels for every recording of the planned batch `vb` (VbxBatch).  x: [N,dim] float32 or float64 CUDA tensor
     of transformed x-vectors (the output of VBx/vbhmm.py:129).  Returns (labels, thr, Z): a list of int arrays
     (0-based cluster ids, VBx/vbhmm.py:145-146), the calibrated thresholds [B] and the linkage matrices (list)."""
+    th, Zs = linkage_batch(vb, x, workspace)
+    return cut(Zs, th, vb.lengths, threshold), th, Zs
+
+
+def linkage_batch(vb, x, workspace=None):
+    """The device half of ahc_batch: vbx_ahc on every recording of `vb`, its outputs copied to the host.  Returns (the
+    calibrated thresholds [B], the linkage matrices (list)); cut() turns them into labels."""
     if not (isinstance(x, torch.Tensor) and x.is_cuda and x.is_contiguous() and x.dim() == 2 and x.shape[0] == vb.N
             and x.dtype in (torch.float32, torch.float64)):
         raise ValueError('x: expected a contiguous float32/float64 CUDA tensor of shape [N, dim]')
@@ -77,7 +84,7 @@ def ahc_batch(vb, x, threshold=-0.015, workspace=None):
     Zh, th = Z.cpu().numpy(), thr.cpu().numpy()       # 32 B per x-vector leave the device
     Zs = [Zh[int(vb.offsets[b]):int(vb.offsets[b + 1]) - 1] if vb.offsets[b + 1] > vb.offsets[b] else Zh[0:0]
           for b in range(vb.B)]
-    return cut(Zs, th, vb.lengths, threshold), th, Zs
+    return th, Zs
 
 
 def cut(Zs, th, lengths, threshold):

@@ -380,6 +380,146 @@ class VbxBatch:
             out.update(alpha=alpha, invL=invL)
         return out
 
+    # ---- streaming diarization, DESIGN.md section 5.25 ----------------------------------------------------------------
+    def _stream_args(self, state, slots, blk_fea, blk_off):
+        """The per-stream arrays of a push on this batch's plan (the window plan: recording b is stream slots[b]'s
+        window), checked on the host: slots distinct and in range, blk_fea [*, R] float32 finite, blk_off [B+1] with
+        blocks of >= 1 rows, every window length min(C, count) + h.  Returns (slot, blk_off, win_off) CUDA tensors."""
+        if not isinstance(state, StreamState) or state.device != self.device or state.R != self.R:
+            raise ValueError(f'state: expected a StreamState with R = {self.R} on {self.device}')
+        sl = np.asarray(slots, dtype=np.int64).reshape(-1)
+        if len(sl) != self.B or len(np.unique(sl)) != self.B or (self.B and (sl.min() < 0 or sl.max() >= state.slots)):
+            raise ValueError(f'slots: expected {self.B} distinct slots in [0, {state.slots})')
+        bo = np.asarray(blk_off, dtype=np.int64).reshape(-1)
+        if len(bo) != self.B + 1 or bo[0] != 0 or np.any(np.diff(bo) < 1):
+            raise ValueError(f'blk_off: expected {self.B + 1} increasing offsets from 0, one block of >= 1 rows per stream')
+        if not (isinstance(blk_fea, torch.Tensor) and blk_fea.is_cuda and blk_fea.device == self.device
+                and blk_fea.dtype == torch.float32 and blk_fea.is_contiguous() and tuple(blk_fea.shape) == (int(bo[-1]), self.R)):
+            raise ValueError(f'blk_fea: expected a contiguous float32 tensor of shape ({int(bo[-1])}, {self.R}) on {self.device}')
+        if not bool(torch.isfinite(blk_fea).all()):
+            raise ValueError('blk_fea must be finite')
+        slot_d = torch.from_numpy(sl.astype(np.int32)).to(self.device)
+        count = state.count[slot_d.long()].cpu().numpy()
+        if not np.array_equal(self.lengths, np.minimum(count, state.C) + np.diff(bo)):
+            raise ValueError('the plan\'s lengths must be min(C, count) + h for every stream (the window of the push)')
+        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.int64)).to(self.device)
+        return slot_d, dev(bo), dev(self.offsets)
+
+    def _stream_out(self, out, specs):
+        """Caller-owned outputs of the stream entries, checked (contiguous tensors of the given (shape, dtype) on this
+        batch's device); out None allocates them."""
+        if out is None:
+            return [torch.empty(shape, dtype=dt, device=self.device) for shape, dt in specs]
+        if len(out) != len(specs):
+            raise ValueError(f'out: expected {len(specs)} tensors')
+        for t, (shape, dt) in zip(out, specs):
+            if not (isinstance(t, torch.Tensor) and t.device == self.device and t.dtype == dt and t.is_contiguous()
+                    and tuple(t.shape) == tuple(shape)):
+                raise ValueError(f'out: expected a contiguous {dt} tensor of shape {tuple(shape)} on {self.device}')
+        return list(out)
+
+    def _timed(self, events, call):
+        """call() with the CUDA events pair `events` (None: no timing) recorded right around it on the current stream,
+        so that their interval holds the kernel and not the host checks before it."""
+        if events is not None:
+            events[0].record()
+        self._check(call())
+        if events is not None:
+            events[1].record()
+
+    def stream_window(self, state, slots, blk_fea, blk_off, blk_lab, n_clusters, smoothing, out=None, events=None):
+        """The window of a push on this batch's plan (vbx_stream_window): stream slots[b] (a StreamState slot) takes the
+        block rows blk_off[b] .. blk_off[b+1]-1 of blk_fea [*, R] float32 (projected x-vectors) with its block AHC
+        labels blk_lab (int32 CUDA [*], 0 .. c-1) and c = n_clusters[b] (host ints; K + c <= min(S, S_max), c = 0 only
+        when K = S_max).  Everything is checked on the host first (synchronises).  Returns (fea [N,R] float32,
+        gamma0 [N,S], pi0 [B,S] float32, n_states int32 [B], (prior_n [B,S], prior_F [B,S,R]) float64): the inputs of
+        prepare_scale and run(prior=).  out: None, or those six tensors to write into; events: None, or two CUDA events
+        recorded right before and after the kernel (a measurement aid)."""
+        slot_d, bo_d, wo_d = self._stream_args(state, slots, blk_fea, blk_off)
+        c = np.asarray(n_clusters, dtype=np.int64).reshape(-1)
+        sm = float(smoothing)
+        if not np.isfinite(sm):
+            raise ValueError('smoothing must be finite')
+        if len(c) != self.B or np.any(c < 0):
+            raise ValueError(f'n_clusters: expected {self.B} counts >= 0')
+        K = state.K[slot_d.long()].cpu().numpy().astype(np.int64)
+        if np.any(K + c > min(self.S, state.S_max)) or np.any((c == 0) & (K != state.S_max)):
+            raise ValueError(f'n_clusters: K + c must lie in [1, {min(self.S, state.S_max)}], and c = 0 only at S_max speakers')
+        if not (isinstance(blk_lab, torch.Tensor) and blk_lab.device == self.device and blk_lab.dtype == torch.int32
+                and tuple(blk_lab.shape) == (int(blk_fea.shape[0]),)):
+            raise ValueError(f'blk_lab: expected an int32 tensor of shape ({int(blk_fea.shape[0])},) on {self.device}')
+        blk_lab = blk_lab.contiguous()
+        c_d = torch.from_numpy(c.astype(np.int32)).to(self.device)
+        per_row = torch.repeat_interleave(c_d, torch.diff(bo_d))
+        if bool(((per_row > 0) & ((blk_lab < 0) | (blk_lab >= per_row))).any()):
+            raise ValueError('blk_lab: every label must lie in [0, c) of its stream (not read where c = 0)')
+        f32, f64 = torch.float32, torch.float64
+        fea, gamma, pi, ns, pn, pF = self._stream_out(out, [((self.N, self.R), f32), ((self.N, self.S), f32),
+                                                            ((self.B, self.S), f32), ((self.B,), torch.int32),
+                                                            ((self.B, self.S), f64), ((self.B, self.S, self.R), f64)])
+        self._timed(events, lambda: self.lib.vbx_stream_window(
+            self._h, self.B, state.C, self.R, state.S_max, self.S, _ptr(slot_d), _ptr(bo_d), _ptr(wo_d), _ptr(blk_lab),
+            _ptr(c_d), _ptr(blk_fea), sm, _ptr(state.ctx_fea), _ptr(state.ctx_lab), _ptr(state.count), _ptr(state.K),
+            _ptr(state.n_hist), _ptr(state.F_hist), _ptr(fea), _ptr(gamma), _ptr(pi), _ptr(ns), _ptr(pn), _ptr(pF),
+            self._stream()))
+        return fea, gamma, pi, ns, (pn, pF)
+
+    def stream_commit(self, state, slots, blk_fea, blk_off, first, out=None, events=None):
+        """Fold a push's result into the streams' state (vbx_stream_commit): first (int32 CUDA [N]) holds the window's
+        first labels, as hard_labels leaves them; slots, blk_fea and blk_off as for stream_window.  Checked on the host
+        first (synchronises).  Returns the blocks' final labels, int32 CUDA [blk_off[-1]] (written into out, when given);
+        state is updated in place.  events: as for stream_window."""
+        slot_d, bo_d, wo_d = self._stream_args(state, slots, blk_fea, blk_off)
+        if not (isinstance(first, torch.Tensor) and first.device == self.device and first.dtype == torch.int32
+                and tuple(first.shape) == (self.N,)):
+            raise ValueError(f'first: expected an int32 tensor of shape ({self.N},) on {self.device}')
+        first = first.contiguous()
+        if self.N and bool(((first < 0) | (first >= min(self.S, state.S_max))).any()):
+            raise ValueError(f'first: every label must lie in [0, {min(self.S, state.S_max)})')
+        labels, = self._stream_out(None if out is None else [out], [((int(blk_fea.shape[0]),), torch.int32)])
+        self._timed(events, lambda: self.lib.vbx_stream_commit(
+            self._h, self.B, state.C, self.R, state.S_max, _ptr(slot_d), _ptr(bo_d), _ptr(wo_d), _ptr(blk_fea),
+            _ptr(first), _ptr(state.ctx_fea), _ptr(state.ctx_lab), _ptr(state.count), _ptr(state.K), _ptr(state.n_hist),
+            _ptr(state.F_hist), _ptr(labels), self._stream()))
+        return labels
+
+
+class StreamState:
+    """The device-resident state of `slots` live streams (include/vbx_b200.h vbx_stream_window, DESIGN.md section
+    5.25): a ring of the last C projected x-vectors of each stream and their final labels, its x-vector count, its
+    speaker count K and the float64 history statistics n_hist [slots, S_max], F_hist [slots, S_max, R] of the x-vectors
+    that have left the ring.  Every slot starts empty."""
+
+    def __init__(self, slots, C, R, S_max, device):
+        self.C, self.R, self.S_max = int(C), int(R), int(S_max)
+        self.device = torch.device(device)
+        self.slots = 0
+        self.ctx_fea = torch.zeros((0, max(self.C, 1), self.R), dtype=torch.float32, device=self.device)
+        self.ctx_lab = torch.zeros((0, max(self.C, 1)), dtype=torch.int32, device=self.device)
+        self.count = torch.zeros(0, dtype=torch.int64, device=self.device)
+        self.K = torch.zeros(0, dtype=torch.int32, device=self.device)
+        self.n_hist = torch.zeros((0, self.S_max), dtype=torch.float64, device=self.device)
+        self.F_hist = torch.zeros((0, self.S_max, self.R), dtype=torch.float64, device=self.device)
+        self.grow(slots)
+
+    _FIELDS = ('ctx_fea', 'ctx_lab', 'count', 'K', 'n_hist', 'F_hist')
+
+    def grow(self, slots):
+        """At least `slots` slots, the existing ones kept (a larger allocation and one copy per array)."""
+        if slots <= self.slots:
+            return
+        for name in self._FIELDS:
+            old = getattr(self, name)
+            new = torch.zeros((int(slots),) + tuple(old.shape[1:]), dtype=old.dtype, device=self.device)
+            new[:self.slots] = old
+            setattr(self, name, new)
+        self.slots = int(slots)
+
+    def reset(self, slot):
+        """Empty slot `slot` for a new stream."""
+        for name in self._FIELDS:
+            getattr(self, name)[int(slot)].zero_()
+
 
 def check_prior(prior, B, S, R, device):
     """The enrolment prior of run() / run_f64() checked on the host (ValueError): a pair (n [B,S], F [B,S,R]) of float64

@@ -1330,6 +1330,57 @@ int vbx_class_scatter(vbx_handle_t h, const float *X, int64_t N, int32_t D, int3
                    "class_scatter");
 }
 
+static int check_stream_sizes(vbx_handle_t h, const std::string &who, int32_t n, int32_t C, int32_t R, int32_t S_max,
+                              int32_t S) {
+    if (n < 0 || C < 0) return fail(h, VBX_ERR_ARG, who + ": n and C must be >= 0");
+    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, who + ": R must lie in [1, 128]");
+    if (S_max < 1 || S_max > 128 || S < 1 || S > 128) return fail(h, VBX_ERR_ARG, who + ": S_max and S must lie in [1, 128]");
+    return VBX_OK;
+}
+
+int vbx_stream_window(vbx_handle_t h, int32_t n, int32_t C, int32_t R, int32_t S_max, int32_t S, const int32_t *slot,
+                      const int64_t *blk_off, const int64_t *win_off, const int32_t *blk_lab, const int32_t *n_clusters,
+                      const float *blk_fea, double smoothing, const float *ctx_fea, const int32_t *ctx_lab,
+                      const int64_t *count, const int32_t *K, const double *n_hist, const double *F_hist, float *fea_out,
+                      float *gamma_out, float *pi_out, int32_t *n_states_out, double *prior_n_out, double *prior_F_out,
+                      void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_stream_window");
+    const std::string who("vbx_stream_window");
+    const int rc = check_stream_sizes(h, who, n, C, R, S_max, S);
+    if (rc != VBX_OK) return rc;
+    if (!std::isfinite(smoothing)) return fail(h, VBX_ERR_ARG, who + ": smoothing must be finite");
+    if (n > 0 && (!slot || !blk_off || !win_off || !blk_lab || !n_clusters || !blk_fea || (C > 0 && (!ctx_fea || !ctx_lab)) ||
+                  !count || !K || !n_hist || !F_hist || !fea_out || !gamma_out || !pi_out || !n_states_out ||
+                  !prior_n_out || !prior_F_out))
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_stream_window(n, C, R, S_max, S, slot, blk_off, win_off, blk_lab, n_clusters, blk_fea,
+                                                smoothing, ctx_fea, ctx_lab, count, K, n_hist, F_hist, fea_out, gamma_out,
+                                                pi_out, n_states_out, prior_n_out, prior_F_out, (cudaStream_t)stream),
+                   "stream_window");
+}
+
+int vbx_stream_commit(vbx_handle_t h, int32_t n, int32_t C, int32_t R, int32_t S_max, const int32_t *slot,
+                      const int64_t *blk_off, const int64_t *win_off, const float *blk_fea, const int32_t *first,
+                      float *ctx_fea, int32_t *ctx_lab, int64_t *count, int32_t *K, double *n_hist, double *F_hist,
+                      int32_t *labels_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_stream_commit");
+    const std::string who("vbx_stream_commit");
+    const int rc = check_stream_sizes(h, who, n, C, R, S_max, S_max);
+    if (rc != VBX_OK) return rc;
+    if (n > 0 && (!slot || !blk_off || !win_off || !blk_fea || !first || (C > 0 && (!ctx_fea || !ctx_lab)) || !count ||
+                  !K || !n_hist || !F_hist || !labels_out))
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_stream_commit(n, C, R, S_max, slot, blk_off, win_off, blk_fea, first, ctx_fea, ctx_lab,
+                                                count, K, n_hist, F_hist, labels_out, (cudaStream_t)stream),
+                   "stream_commit");
+}
+
 int vbx_attach_comm(vbx_handle_t h, void *nccl_comm, int32_t n_ranks, const char *libnccl_path) {
     if (!h) return VBX_ERR_ARG;
     if (!nccl_comm) {   // detach

@@ -398,5 +398,16 @@ int launch_gsum_from_frames(const Plan &pl, const Workspace &ws, const float *gf
 size_t class_scatter_workspace_bytes(int64_t N, int D, int64_t K);
 int launch_class_scatter(const float *X, int64_t N, int D, int64_t K, const int64_t *offsets_host, void *workspace,
                          double *means_out, double *scatter_out, cudaStream_t st);
+// streaming diarization: a push's window from the streams' state, and its result folded back (vbx_stream.cu)
+int launch_stream_window(int n, int C, int R, int S_max, int S, const int32_t *slot, const int64_t *blk_off,
+                         const int64_t *win_off, const int32_t *blk_lab, const int32_t *n_clusters, const float *blk_fea,
+                         double smoothing, const float *ctx_fea, const int32_t *ctx_lab, const int64_t *count,
+                         const int32_t *K, const double *n_hist, const double *F_hist, float *fea_out, float *gamma_out,
+                         float *pi_out, int32_t *n_states_out, double *prior_n_out, double *prior_F_out,
+                         cudaStream_t st);
+int launch_stream_commit(int n, int C, int R, int S_max, const int32_t *slot, const int64_t *blk_off,
+                         const int64_t *win_off, const float *blk_fea, const int32_t *first, float *ctx_fea,
+                         int32_t *ctx_lab, int64_t *count, int32_t *K, double *n_hist, double *F_hist,
+                         int32_t *labels_out, cudaStream_t st);
 
 }  // namespace vbx
