@@ -590,7 +590,8 @@ enum vbx_kernel_class {
     VBX_K_LOGLIK = 5,        /* log_p_ + row softmax       VBx/VBx.py:97    */
     VBX_K_FWDBWD = 6,        /* forward-backward, pi, ELBO VBx/VBx.py:98-105 */
     VBX_K_EXACT64 = 7,       /* snapshot + float64 finishing phase (stop rule at float64 resolution) */
-    VBX_N_KERNEL_CLASSES = 8
+    VBX_K_EM_CONTRACT = 8,   /* M-step + speaker model + log_p_ in one cluster kernel (large batches) */
+    VBX_N_KERNEL_CLASSES = 9
 };
 /* With option "timing" = 1 every kernel class is bracketed by CUDA events on the launching stream.
  * Fills ms_out[VBX_N_KERNEL_CLASSES] / count_out[...] with the accumulated device time and launch counts

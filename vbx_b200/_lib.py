@@ -23,7 +23,7 @@ FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
 COMBINE_BAD_LABEL, COMBINE_TOO_MANY_LABELS = 1, 2                  # vbx_combine flags
 LINK_MAX_SPEAKERS = 1 << 29                                        # VBX_LINK_MAX_SPEAKERS
-KERNEL_CLASSES = ['project', 'prepare', 'run_init', 'mstep_partial', 'speaker_model', 'loglik', 'forward_backward', 'exact64']
+KERNEL_CLASSES = ['project', 'prepare', 'run_init', 'mstep_partial', 'speaker_model', 'loglik', 'forward_backward', 'exact64', 'em_contract']
 
 
 class VbxError(RuntimeError):

@@ -7,7 +7,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libvbx_b200.so')
 SOURCES = ['vbx_kernels.cu', 'vbx_mma_kernels.cu', 'vbx_long_kernels.cu', 'vbx_fb_split.cu', 'vbx_project_tc.cu', 'vbx_f64.cu', 'vbx_exact64.cu', 'vbx_fb_dense.cu', 'vbx_ahc.cu',
            'vbx_score.cu', 'vbx_count.cu', 'vbx_link.cu', 'vbx_enroll.cu', 'vbx_cohort.cu', 'vbx_init.cu', 'vbx_combine.cu',
-           'vbx_train.cu', 'vbx_stream.cu', 'vbx_capi.cu']
+           'vbx_train.cu', 'vbx_stream.cu', 'vbx_em_contract.cu', 'vbx_capi.cu']
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 NVCC_FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17', '-Xcompiler', '-fPIC', '-Xptxas', '-v']
 

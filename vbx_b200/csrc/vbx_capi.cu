@@ -426,6 +426,7 @@ int vbx_plan(vbx_handle_t h, const int64_t *offsets_host, int32_t n_rec, int32_t
     pl.S = S;
     pl.exact = h->opt_exact_stop;
     pl.split = split ? 1 : 0;
+    pl.em_cluster = vbx::em_contract_cluster(S, R, maxT, split);
     pl.n_frames = n_rec ? offsets_host[n_rec] : 0;
     pl.n_ltiles = (int32_t)lrec.size();
     pl.n_mtiles = (int32_t)mrec.size();
@@ -681,23 +682,30 @@ static int run_impl(vbx_handle_t h, const char *who, bool per_rec, const float *
                 rc = counted(h, vbx::launch_snapshot(pl, h->ws, gamma_io, pi_io, it, st), "snapshot");
                 if (rc) return rc;
             }
-            if (!given) {
-                Timed t(h, st, VBX_K_MSTEP);
-                rc = counted(h, h->opt_gemm ? vbx::launch_mstep_partial(pl, h->ws, rho, gamma_io, st)
-                                            : vbx::launch_mstep_mma(pl, h->ws, rho, gamma_io, st), "mstep_partial");
+            if (pl.em_cluster && !h->opt_gemm && !given && !prior_n) {
+                Timed t(h, st, VBX_K_EM_CONTRACT);
+                rc = counted(h, vbx::launch_em_contract(pl, h->ws, rho, gamma_io, Phi, n_states, alpha_io, invL_io, st),
+                             "em_contract");
+                if (rc) return rc;
+            } else {   // the three kernels: split plans, S > 16, T > 1024, warm starts and priors
+                if (!given) {
+                    Timed t(h, st, VBX_K_MSTEP);
+                    rc = counted(h, h->opt_gemm ? vbx::launch_mstep_partial(pl, h->ws, rho, gamma_io, st)
+                                                : vbx::launch_mstep_mma(pl, h->ws, rho, gamma_io, st), "mstep_partial");
+                }
+                if (rc) return rc;
+                {
+                    Timed t(h, st, VBX_K_SPEAKER_MODEL);
+                    rc = counted(h, vbx::launch_speaker_model(pl, h->ws, Phi, n_states, alpha_io, invL_io, given, st, prior_n,
+                                                              prior_F), "speaker_model");
+                }
+                if (rc) return rc;
+                {
+                    Timed t(h, st, VBX_K_LOGLIK);
+                    rc = counted(h, h->opt_gemm ? vbx::launch_loglik(pl, h->ws, rho, pi_io, n_states, st) : vbx::launch_loglik_mma(pl, h->ws, rho, pi_io, n_states, st), "loglik");
+                }
+                if (rc) return rc;
             }
-            if (rc) return rc;
-            {
-                Timed t(h, st, VBX_K_SPEAKER_MODEL);
-                rc = counted(h, vbx::launch_speaker_model(pl, h->ws, Phi, n_states, alpha_io, invL_io, given, st, prior_n,
-                                                          prior_F), "speaker_model");
-            }
-            if (rc) return rc;
-            {
-                Timed t(h, st, VBX_K_LOGLIK);
-                rc = counted(h, h->opt_gemm ? vbx::launch_loglik(pl, h->ws, rho, pi_io, n_states, st) : vbx::launch_loglik_mma(pl, h->ws, rho, pi_io, n_states, st), "loglik");
-            }
-            if (rc) return rc;
             if (fb_hi) {   // the sweep on the high-priority side stream, ordered after the log-likelihoods and before the next M-step
                 cudaEventRecord(h->ev_fork, st);
                 cudaStreamWaitEvent(h->hi_stream, h->ev_fork, 0);

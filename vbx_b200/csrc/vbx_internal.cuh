@@ -26,6 +26,8 @@ struct Plan {
     int32_t n_rec = 0, R = 0, S = 0;
     int32_t exact = 0;                  // 1 = the workspace holds the buffers of the float64 finishing phase
     int32_t split = 0;                  // 1 = forward and backward sweeps on separate warps + combine pass (vbx_fb_split.cu)
+    int32_t em_cluster = 0;             // > 0: cluster size of em_contract_kernel, which then runs the iteration's
+                                        // M-step, speaker model and log-likelihood (vbx_em_contract.cu); 0 = three kernels
     int64_t n_frames = 0;
     int32_t n_ltiles = 0, n_mtiles = 0;
     int64_t max_T = 0;
@@ -214,6 +216,29 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
                  : "memory");
 }
 
+// mma.sync.m16n8k8 TF32 and the hi/lo split of the "3xTF32" contractions (vbx_mma_kernels.cu, vbx_em_contract.cu)
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t b0, const uint32_t b1) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// x = hi + lo.  hi = x rounded to nearest TF32 (add half an ulp of the 13 dropped bits, then clear them: ties
+// away from zero, i.e. cvt.rna.tf32.f32, on the integer pipe); lo = x - hi is exact and is handed to the tensor
+// core as is (it keeps lo's top 19 bits), so |x - hi - lo'| <= 2^-22 |x| with errors of either sign.
+// The rounding is a volatile asm so that the compiler keeps each split next to the mma that consumes it (volatile
+// asms are not reordered among themselves); hoisting all splits of a tile up front doubles the register footprint.
+__device__ __forceinline__ void split_tf32(const float x, uint32_t &hi, uint32_t &lo) {
+    asm volatile("{\n\t.reg .b32 t;\n\tadd.u32 t, %1, 0x1000;\n\tand.b32 %0, t, 0xffffe000;\n\t}" : "=r"(hi) : "r"(__float_as_uint(x)));
+    lo = (__float_as_uint(x - __uint_as_float(hi)) + 0x1000u) & 0xffffe000u;
+}
+template <int LANES>
+__device__ __forceinline__ float group_sum(float v) {
+#pragma unroll
+    for (int off = LANES / 2; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    return v;
+}
+
 // The problem g whose range [pref[g], pref[g+1]) holds x, for non-decreasing pref with pref[0] = 0 <= x < pref[G]:
 // the largest g with pref[g] <= x (never an empty problem's, whose range is empty).  The batched speaker kernels
 // (vbx_link_batch, vbx_enroll_batch, vbx_cohort_stats_batch) decode their flat indices with it.
@@ -259,6 +284,11 @@ int launch_forward_backward_long(const Plan &pl, const Workspace &ws, const RunP
 int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, cudaStream_t st);
 int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                       cudaStream_t st);
+// M-step, speaker model and log-likelihood in one cluster kernel (vbx_em_contract.cu): the cluster size for a plan of
+// these dimensions (0 = not available: split plans, S > 16, R != 128, max_T > 1024, or no cluster fits on the device)
+int em_contract_cluster(int S, int R, int64_t max_T, bool split);
+int launch_em_contract(const Plan &pl, const Workspace &ws, const float *rho, const float *gamma, const float *Phi,
+                       const int32_t *n_states, float *alpha_io, float *invL_io, cudaStream_t st);
 // float64 finishing phase of vbx_run (vbx_exact64.cu)
 int launch_snapshot(const Plan &pl, const Workspace &ws, const float *gamma, const float *pi, int iter, cudaStream_t st);
 int launch_exact64_round(const Plan &pl, const Workspace &ws, const RunParams &rp, const float *rho, const float *Phi,

@@ -29,12 +29,6 @@ __device__ __forceinline__ void cp_async_wait_all() {
 }
 
 template <int LANES>
-__device__ __forceinline__ float group_sum(float v) {
-#pragma unroll
-    for (int off = LANES / 2; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-    return v;
-}
-template <int LANES>
 __device__ __forceinline__ float group_max(float v) {
 #pragma unroll
     for (int off = LANES / 2; off > 0; off >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, off));

@@ -17,21 +17,6 @@
 
 namespace vbx {
 
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], const uint32_t b0, const uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-// x = hi + lo.  hi = x rounded to nearest TF32 (add half an ulp of the 13 dropped bits, then clear them: ties
-// away from zero, i.e. cvt.rna.tf32.f32, on the integer pipe); lo = x - hi is exact and is handed to the tensor
-// core as is (it keeps lo's top 19 bits), so |x - hi - lo'| <= 2^-22 |x| with errors of either sign.
-// The rounding is a volatile asm so that the compiler keeps each split next to the mma that consumes it (volatile
-// asms are not reordered among themselves); hoisting all splits of a tile up front doubles the register footprint.
-__device__ __forceinline__ void split_tf32(const float x, uint32_t &hi, uint32_t &lo) {
-    asm volatile("{\n\t.reg .b32 t;\n\tadd.u32 t, %1, 0x1000;\n\tand.b32 %0, t, 0xffffe000;\n\t}" : "=r"(hi) : "r"(__float_as_uint(x)));
-    lo = (__float_as_uint(x - __uint_as_float(hi)) + 0x1000u) & 0xffffe000u;
-}
 __device__ __forceinline__ void cp_async16_(void *smem, const void *gmem) {
     unsigned s = static_cast<unsigned>(__cvta_generic_to_shared(smem));
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
