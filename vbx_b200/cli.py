@@ -38,6 +38,13 @@ RTTM, each x-vector started from the speakers' shares of its segment.  The writt
 (with --output-2nd the second-label RTTMs too) unless linking or enrolment name the speakers.  --threshold is still
 required, as by the reference's parser, and is used only by the AHC that the count bounds' rule 3 needs.
 
+With --adapt [--recentre] [--adapt-within-scale W --adapt-between-scale B --adapt-mean-scale S] the PLDA is first
+adapted to the archive's own x-vectors (DESIGN.md section 5.26, vbx_b200/adapt.py: the variance the archive shows
+beyond the model's, added to the within- and between-speaker covariances at W (0.3) and B (0.7), the mean moved to the
+archive's), with --recentre after the transform's centring means are re-estimated on the archive; everything then runs
+as without, enrolled and cohort x-vectors through the adapted front end.  python -m vbx_b200.train --adapt-plda writes
+the same model to files.
+
 With --init RANDOM+VB --init-states N [--restarts R] [--seed S] the VB-HMM starts from random flat-Dirichlet
 responsibilities over N states instead of AHC (DESIGN.md section 5.22), R starts per recording side by side (default 1),
 restart r drawn with seed S + r (default 0); each recording keeps the restart of largest final ELBO.  No AHC runs unless
@@ -108,6 +115,48 @@ def check_random_options(ap, args):
         ap.error('--seed must lie in [0, 2**64)')
 
 
+def add_adapt_scales(ap, prefix):
+    """--<prefix>within-scale / between-scale / mean-scale (adapt.SCALES; default None: not given)."""
+    for k, v in (('within', 0.3), ('between', 0.7), ('mean', 1.0)):
+        ap.add_argument(f'--{prefix}{k}-scale', default=None, type=float,
+                        help=f'PLDA adaptation: scale of the excess variance added to the {k}-class covariance '
+                             f'(default {v})' if k != 'mean' else
+                             f'PLDA adaptation: weight of the mean shift in the archive\'s covariance (default {v})')
+
+
+def adapt_scales(ap, args, prefix, enabled, what):
+    """The given adaptation scales {within_scale, ...} of add_adapt_scales' options: usage errors (exit 2) for scales
+    without `enabled` (named `what`) and for negative or non-finite ones."""
+    from . import adapt
+    scales = {f'{k}_scale': getattr(args, f'{prefix}{k}_scale') for k in ('within', 'between', 'mean')}
+    scales = {k: v for k, v in scales.items() if v is not None}
+    if scales and not enabled:
+        ap.error(f'the adaptation scales need {what}')
+    try:
+        adapt.check_scales(**scales)
+    except ValueError as e:
+        ap.error(str(e))
+    return scales
+
+
+def add_adapt_options(ap):
+    """--adapt / --recentre / --adapt-within-scale / --adapt-between-scale / --adapt-mean-scale."""
+    ap.add_argument('--adapt', action='store_true',
+                    help='adapt the PLDA to the archive\'s own x-vectors before diarizing it (DESIGN.md section 5.26)')
+    ap.add_argument('--recentre', action='store_true',
+                    help='with --adapt: re-estimate the transform\'s centring means on the archive first')
+    add_adapt_scales(ap, 'adapt-')
+
+
+def check_adapt_options(ap, args):
+    """Usage errors (exit 2) of the --adapt options: --recentre or scales without --adapt, negative or non-finite
+    scales.  Returns the given scales (adapt.adapt_backend's keywords), or None without --adapt."""
+    scales = adapt_scales(ap, args, 'adapt_', args.adapt, '--adapt')
+    if args.recentre and not args.adapt:
+        ap.error('--recentre needs --adapt')
+    return scales if args.adapt else None
+
+
 def build_parser():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     # option names, types and defaults of VBx/vbhmm.py:55-102
@@ -151,6 +200,7 @@ def build_parser():
     ap.add_argument('--init-rttm', default=None,
                     help='with --init RTTM+VB: the diarization (RTTM file or directory of *.rttm) the VB-HMM starts from')
     add_random_options(ap)
+    add_adapt_options(ap)
     return ap
 
 
@@ -180,6 +230,7 @@ def main(argv=None):
     if (args.init == 'RTTM+VB') != (args.init_rttm is not None):
         ap.error('--init RTTM+VB and --init-rttm go together')
     check_random_options(ap, args)
+    scales = check_adapt_options(ap, args)
     from . import formats
     from .pipeline import diarize_batch, linked_lines, named_lines
     from .score import read_overlaps
@@ -196,6 +247,11 @@ def main(argv=None):
         seg_names, times = segs[name]
         assert np.all(np.array(seg_names) == np.array(keys))               # VBx/vbhmm.py:166
         recs[name] = (x, times)
+    if scales is not None:      # section 5.26: the back end adapted to this archive, then everything as without
+        from .adapt import adapt_backend
+        (mean1, mean2, lda), plda, _ = adapt_backend(recs, (mean1, mean2, lda), plda, lda_dim=args.lda_dim,
+                                                     chain=args.chain, device=args.device, recentre=args.recentre,
+                                                     **scales)
     out = diarize_batch(recs, (mean1, mean2, lda), plda, Fa=args.Fa, Fb=args.Fb, loopP=args.loopP, lda_dim=args.lda_dim,
                         threshold=args.threshold, smoothing=args.init_smoothing, init=args.init, chain=args.chain,
                         device=args.device, output_2nd=args.output_2nd, overlaps=overlaps,

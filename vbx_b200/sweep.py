@@ -46,6 +46,8 @@ With --combine N (the N best settings of ranking['full']; needs --ref-rttm) or -
 combined into one by label mapping and weighted voting (DESIGN.md section 5.21): OUT/combined/<recording>.rttm, and
 summary.json gains combined = {hypotheses, recordings: {name: order, weights, speakers}[, der][, jer]}, scored under
 the same protocols.  Every other key of summary.json is as without --combine.
+With --adapt [--recentre] [--adapt-within-scale ...] the back end is adapted to the archive once (DESIGN.md section
+5.26), as cli --adapt adapts it, and every setting runs with the adapted model.
 """
 import argparse
 import itertools
@@ -676,9 +678,10 @@ def build_parser():
     ap.add_argument('--cohort-utt2spk', default=None, help='the speaker of each x-vector of --cohort-ark (utt2spk)')
     ap.add_argument('--cohort-top', default=200, type=int,
                     help="how many of each speaker's largest cohort scores set its mean and spread (default 200)")
-    from .cli import add_count_options, add_random_options
+    from .cli import add_adapt_options, add_count_options, add_random_options
     add_count_options(ap, allow_oracle=True)
     add_random_options(ap)
+    add_adapt_options(ap)
     return ap
 
 
@@ -691,8 +694,9 @@ def main(argv=None):
         ap.error('--cohort-ark and --cohort-utt2spk go together')
     if (args.init == 'RTTM+VB') != (args.init_rttm is not None):
         ap.error('--init RTTM+VB and --init-rttm go together')
-    from .cli import check_random_options
+    from .cli import check_adapt_options, check_random_options
     check_random_options(ap, args)
+    scales = check_adapt_options(ap, args)
     if isinstance(args.combine, int) and args.ref_rttm is None:
         ap.error('--combine N takes the N best settings by DER: it needs --ref-rttm (or --combine all)')
     from . import formats
@@ -704,6 +708,10 @@ def main(argv=None):
         seg_names, times = segs[name]
         assert np.all(np.array(seg_names) == np.array(keys))
         recs[name] = (x, times)
+    if scales is not None:      # adapted once; every setting runs with the adapted model
+        from .adapt import adapt_backend
+        transform, plda, _ = adapt_backend(recs, transform, plda, lda_dim=args.lda_dim, chain=args.chain,
+                                           device=args.device, recentre=args.recentre, **scales)
     from .score import read_overlaps
     overlaps = read_overlaps(args.overlap_rttm) if args.overlap_rttm is not None else None
     grid = dict(Fa=args.Fa, Fb=args.Fb, loopP=args.loopP, threshold=args.threshold, smoothing=args.init_smoothing)

@@ -6,6 +6,17 @@ extractor, or a back end fitted to one's own domain, can be diarized without Kal
 
 and then `python -m vbx_b200.cli --xvec-transform model/transform.npz --plda-file model/plda --lda-dim d ...`.
 
+Three more modes fit the PLDA alone, in the space of a given transform (DESIGN.md section 5.26), and write the same
+three files (the given transform, or its re-centred form, as transform.npz):
+
+    python -m vbx_b200.train --xvec-transform T --xvec-ark-file train.ark --utt2spk train.utt2spk --out-dir model
+    python -m vbx_b200.train --xvec-transform T ... --interpolate-with PLDA --alpha A --out-dir model
+    python -m vbx_b200.train --xvec-transform T --adapt-plda PLDA --xvec-ark-file archive.ark [--recentre] --out-dir model
+
+the first trains the PLDA on labelled x-vectors through T, the second also interpolates it with PLDA (alpha times the
+trained one), the third adapts PLDA to the unlabelled ark, read by recording as the command line reads it
+(vbx_b200/adapt.py).
+
 The model, all float64 (classes with fewer than min_per_speaker x-vectors dropped first; K classes, N x-vectors):
   transform  mean1 = mean of x; y = l2_norm(x - mean1); S_W, S_B the within- and between-class scatters of y over N;
              lda [Dx, d] the generalised eigenvectors of S_B v = lambda S_W v of the d largest lambda, descending,
@@ -140,9 +151,23 @@ def _sync(dev):
     return time.perf_counter()
 
 
-def check_training_set(xvectors, lda_dim, em_iters, min_per_speaker):
-    """The refusals of DESIGN.md section 5.24 on the host.  Returns (names kept, arrays kept, speakers dropped,
-    x-vectors dropped, Dx)."""
+def check_transform(transform, Dx=None):
+    """(mean1 [Dx], mean2 [d], lda [Dx, d]) as float64 arrays, checked for shapes and finite values (ValueError naming
+    them); Dx: the x-vectors' dimension, when known."""
+    mean1, mean2, lda = (np.asarray(a, dtype=np.float64) for a in transform)
+    if lda.ndim != 2 or mean1.shape != (lda.shape[0],) or mean2.shape != (lda.shape[1],):
+        raise ValueError(f'inconsistent x-vector transform: mean1 {mean1.shape}, mean2 {mean2.shape}, lda {lda.shape}')
+    if Dx is not None and lda.shape[0] != Dx:
+        raise ValueError(f'the x-vector transform takes Dx = {lda.shape[0]}, the x-vectors have Dx = {Dx}')
+    if not all(np.all(np.isfinite(a)) for a in (mean1, mean2, lda)):
+        raise ValueError('the x-vector transform holds non-finite values')
+    return mean1, mean2, lda
+
+
+def check_training_set(xvectors, lda_dim, em_iters, min_per_speaker, fixed=False):
+    """The refusals of DESIGN.md section 5.24 on the host; fixed: the transform is given, so lda_dim is its d and only
+    the PLDA's within-class scatter (N - K >= d) constrains the set.  Returns (names kept, arrays kept, speakers
+    dropped, x-vectors dropped, Dx)."""
     for what, v, lo in (('min_per_speaker', min_per_speaker, 1), ('lda_dim', lda_dim, 1), ('em_iters', em_iters, 0)):
         if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < lo:
             raise ValueError(f'{what} must be an integer >= {lo}, got {v!r}')
@@ -169,6 +194,11 @@ def check_training_set(xvectors, lda_dim, em_iters, min_per_speaker):
         raise ValueError(f'{K} speaker(s) with at least {min_per_speaker} x-vectors; training needs at least 2')
     if not 1 <= Dx <= MAX_DIM:
         raise ValueError(f'x-vector dimension {Dx} outside 1 .. {MAX_DIM}')
+    if fixed:
+        if N - K < lda_dim:
+            raise ValueError(f'N - K = {N} - {K} = {N - K} is below d = {lda_dim}: the PLDA\'s within-class scatter would '
+                             f'be singular')
+        return names, arrays, drop_spk, drop_x, Dx
     if lda_dim > Dx or lda_dim > K - 1:
         raise ValueError(f'lda_dim = {lda_dim} exceeds Dx = {Dx} or K - 1 = {K - 1} (the rank of the between-class '
                          f'scatter with K = {K} speakers)')
@@ -177,14 +207,30 @@ def check_training_set(xvectors, lda_dim, em_iters, min_per_speaker):
     return names, arrays, drop_spk, drop_x, Dx
 
 
-def train_backend(xvectors, lda_dim=128, em_iters=10, min_per_speaker=2, device=None):
+def plda_from_covariances(mu, W, B):
+    """The Kaldi form (mean, transform, psi) of the two-covariance PLDA (mu, W, B): W = L L^T, L^-1 B L^-T = U diag(psi)
+    U^T with psi descending, transform = U^T L^-1 with each row's largest-magnitude entry positive, mean = mu.  psi is
+    clipped at 0: B is positive semi-definite, and where it is singular (a PLDA trained in a fixed transform's space
+    on fewer speakers than dimensions) its zero eigenvalues come out as rounding errors of either sign."""
+    _, _, psi, T = joint_diagonalise(W, B)
+    return np.asarray(mu, dtype=np.float64), _positive_largest(T, 1), np.maximum(psi, 0.0)
+
+
+def train_backend(xvectors, lda_dim=128, em_iters=10, min_per_speaker=2, device=None, transform=None):
     """Fit the x-vector transform and the PLDA (the definition in this module's docstring) to {speaker: x [n, Dx]}
     (e.g. formats.read_enrolment).  Returns (transform, plda, report): transform = (mean1, mean2, lda) and plda =
     (mean, transform, psi), float64 numpy, the tuples diarize_batch, sweep_batch and the command line take; report a
     dict of N, K, dropped speakers and x-vectors, Dx, d, the LDA eigenvalues, psi, the objective trace and the seconds
-    of each stage."""
+    of each stage.  transform: None, or a given (mean1, mean2, lda): the LDA stage is skipped, lda_dim is lda's width
+    and the PLDA is fitted in that transform's space (returned unchanged, the report without LDA eigenvalues)."""
     from scipy.linalg import eigh
-    _, arrays, drop_spk, drop_x, Dx = check_training_set(xvectors, lda_dim, em_iters, min_per_speaker)
+    fixed = transform is not None
+    if fixed:
+        transform = check_transform(transform)
+        lda_dim = int(transform[2].shape[1])
+    _, arrays, drop_spk, drop_x, Dx = check_training_set(xvectors, lda_dim, em_iters, min_per_speaker, fixed)
+    if fixed:
+        check_transform(transform, Dx)
     dev = _device(device)
     t = {}
     t0 = _sync(dev)
@@ -196,22 +242,28 @@ def train_backend(xvectors, lda_dim=128, em_iters=10, min_per_speaker=2, device=
     t1 = _sync(dev)
     t['upload'] = t1 - t0
 
-    mean1 = x.mean(0)
+    mean1 = x.mean(0) if not fixed else torch.from_numpy(transform[0]).to(dev)
     y = pipeline.l2_norm_rows(x - mean1[None, :]).float()
     del x
-    my, Sw = class_stats(y, off, dev)
-    mu_y = (n @ my) / N
-    dm = my - mu_y[None, :]
-    Sb = (dm.T * n[None, :]) @ dm / N
-    t2 = _sync(dev)
-    t['lda_stats'] = t2 - t1
-    lam, V = eigh(Sb.cpu().numpy(), Sw.cpu().numpy() / N)
-    lam, lda = lam[::-1][:d].copy(), _positive_largest(V[:, ::-1][:, :d].copy(), 0)
-    t3 = time.perf_counter()
-    t['lda_eig'] = t3 - t2
+    lam = None
+    if fixed:
+        lda, mean2 = transform[2], torch.from_numpy(transform[1]).to(dev)
+        lda_d = torch.from_numpy(lda).to(dev)
+        t3 = _sync(dev)
+    else:
+        my, Sw = class_stats(y, off, dev)
+        mu_y = (n @ my) / N
+        dm = my - mu_y[None, :]
+        Sb = (dm.T * n[None, :]) @ dm / N
+        t2 = _sync(dev)
+        t['lda_stats'] = t2 - t1
+        lam, V = eigh(Sb.cpu().numpy(), Sw.cpu().numpy() / N)
+        lam, lda = lam[::-1][:d].copy(), _positive_largest(V[:, ::-1][:, :d].copy(), 0)
+        t3 = time.perf_counter()
+        t['lda_eig'] = t3 - t2
+        lda_d = torch.from_numpy(lda).to(dev)
+        mean2 = mu_y @ lda_d
 
-    lda_d = torch.from_numpy(lda).to(dev)
-    mean2 = mu_y @ lda_d
     z = pipeline.l2_norm_rows(y.double() @ lda_d - mean2[None, :]).float()
     del y
     mz, S = class_stats(z, off, dev)
@@ -221,14 +273,15 @@ def train_backend(xvectors, lda_dim=128, em_iters=10, min_per_speaker=2, device=
     t4 = _sync(dev)
     t['plda_stats'] = t4 - t3
     W, B, trace = plda_em(Mc, n, S.cpu().numpy(), N, em_iters)
-    _, _, psi, T = joint_diagonalise(W, B)
-    tr = _positive_largest(T, 1)
+    plda = plda_from_covariances(mu.cpu().numpy(), W, B)
     t['plda_em'] = time.perf_counter() - t4
     transform = (mean1.cpu().numpy(), mean2.cpu().numpy(), lda)
-    plda = (mu.cpu().numpy(), tr, psi)
     report = dict(N=N, K=K, speakers_dropped=drop_spk, xvectors_dropped=drop_x, min_per_speaker=min_per_speaker,
-                  Dx=Dx, lda_dim=d, em_iters=em_iters, lda_eigenvalues=lam.tolist(), psi=psi.tolist(),
-                  objective=trace, seconds=t)
+                  Dx=Dx, lda_dim=d, em_iters=em_iters, psi=plda[2].tolist(), objective=trace, seconds=t)
+    if fixed:
+        report['transform'] = 'given'
+    else:
+        report['lda_eigenvalues'] = lam.tolist()
     return transform, plda, report
 
 
@@ -296,6 +349,7 @@ def write_backend(out_dir, transform, plda, report, binary=True):
 
 
 def build_parser():
+    from .cli import add_adapt_scales
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument('--xvec-ark-file', required=True, help='Kaldi ark of the training x-vectors')
     ap.add_argument('--utt2spk', default=None, help='speaker of every x-vector of the ark')
@@ -311,12 +365,61 @@ def build_parser():
                     help='with --ref-rttm: an RTTM name is the same speaker in every recording')
     ap.add_argument('--text-plda', action='store_true', help='write the PLDA as Kaldi text instead of binary')
     ap.add_argument('--device', default=None, help='CUDA device (default: the current one)')
+    ap.add_argument('--xvec-transform', default=None,
+                    help='a fixed x-vector transform (transform.h5 or .npz): train or adapt the PLDA in its space only')
+    ap.add_argument('--interpolate-with', default=None,
+                    help='with --xvec-transform and labels: a PLDA (Kaldi file) in that transform\'s space to '
+                         'interpolate the trained PLDA with')
+    ap.add_argument('--alpha', default=None, type=float,
+                    help='with --interpolate-with: the weight of the trained PLDA, in [0, 1]')
+    ap.add_argument('--adapt-plda', default=None,
+                    help='with --xvec-transform and no labels: the PLDA (Kaldi file) to adapt to the ark')
+    ap.add_argument('--chain', default='auto', choices=['auto', 'tcgen05', 'float64'],
+                    help='with --adapt-plda: the front end the diarization will use (as the command line\'s --chain)')
+    add_adapt_scales(ap, '')
+    ap.add_argument('--recentre', action='store_true',
+                    help='with --adapt-plda: re-estimate the transform\'s centring means on the ark first')
     return ap
 
 
 def main(argv=None):
+    from . import adapt
+    from .cli import adapt_scales
     ap = build_parser()
     args = ap.parse_args(argv)
+    adapting = args.adapt_plda is not None
+    scales = adapt_scales(ap, args, '', adapting, '--adapt-plda')
+    if args.recentre and not adapting:
+        ap.error('--recentre needs --adapt-plda')
+    if (adapting or args.interpolate_with is not None) and args.xvec_transform is None:
+        ap.error('--adapt-plda and --interpolate-with need --xvec-transform: the PLDAs must share a transform')
+    if adapting and args.interpolate_with is not None:
+        ap.error('--adapt-plda and --interpolate-with are separate modes')
+    if (args.interpolate_with is None) != (args.alpha is None):
+        ap.error('--interpolate-with and --alpha go together')
+    if args.alpha is not None:
+        try:
+            adapt.check_alpha(args.alpha)
+        except ValueError as e:
+            ap.error(str(e))
+    if args.chain != 'auto' and not adapting:
+        ap.error('--chain is an option of --adapt-plda')
+    if adapting:
+        if args.utt2spk is not None or args.ref_rttm is not None or args.segments_file is not None:
+            ap.error('--adapt-plda adapts to an unlabelled ark: no --utt2spk, --ref-rttm or --segments-file')
+        if args.speakers_across_recordings or args.min_share is not None:
+            ap.error('--min-share and --speakers-across-recordings need --ref-rttm')
+        transform = formats.read_xvec_transform(args.xvec_transform)
+        plda = formats.read_kaldi_plda(args.adapt_plda)
+        recs = {name: (x, None) for name, (_, x) in formats.read_xvectors_by_recording(args.xvec_ark_file).items()}
+        transform, plda, report = adapt.adapt_backend(recs, transform, plda, lda_dim=args.lda_dim, chain=args.chain,
+                                                      device=args.device, recentre=args.recentre, **scales)
+        report = dict(report, xvec_transform=args.xvec_transform, adapted_plda=args.adapt_plda)
+        paths = write_backend(args.out_dir, transform, plda, report, binary=not args.text_plda)
+        print(f'adapted {args.adapt_plda} to N = {report["N"]} x-vectors: |delta| = {report["delta_norm"]:.4g}, '
+              f'{report["inflated"]} of {len(report["eigenvalues"])} directions inflated'
+              f'{", transform re-centred" if args.recentre else ""}; wrote {", ".join(paths)}')
+        return 0
     if (args.utt2spk is None) == (args.ref_rttm is None):
         ap.error('give exactly one of --utt2spk and --ref-rttm')
     if (args.ref_rttm is None) != (args.segments_file is None):
@@ -335,13 +438,27 @@ def main(argv=None):
                 raise ValueError(f'recording {name!r}: the segments file does not list the ark keys in ark order')
             recs[name] = (x, segs[name][1])
         xvectors, extra = speakers_from_rttm(recs, args.ref_rttm, min_share, args.speakers_across_recordings)
-    transform, plda, report = train_backend(xvectors, args.lda_dim, args.em_iters, args.min_per_speaker, args.device)
+    given = None if args.xvec_transform is None else formats.read_xvec_transform(args.xvec_transform)
+    other = None
+    if args.interpolate_with is not None:
+        other = formats.read_kaldi_plda(args.interpolate_with)
+        adapt.check_plda(other)
+        adapt.check_compatible(given, other)
+    transform, plda, report = train_backend(xvectors, args.lda_dim, args.em_iters, args.min_per_speaker, args.device,
+                                            transform=given)
     if extra:
         report['rttm'] = dict(extra, min_share=min_share, across_recordings=args.speakers_across_recordings)
+    if given is not None:
+        report['xvec_transform'] = args.xvec_transform
+    if other is not None:
+        plda = adapt.interpolate_plda(plda, other, args.alpha)
+        report.update(interpolated_with=args.interpolate_with, alpha=args.alpha, psi=plda[2].tolist())
     paths = write_backend(args.out_dir, transform, plda, report, binary=not args.text_plda)
     print(f'trained on N = {report["N"]} x-vectors of K = {report["K"]} speakers ({report["speakers_dropped"]} speakers, '
           f'{report["xvectors_dropped"]} x-vectors dropped), Dx = {report["Dx"]}, d = {report["lda_dim"]}, objective '
-          f'{report["objective"][0]:.4f} -> {report["objective"][-1]:.4f}; wrote {", ".join(paths)}')
+          f'{report["objective"][0]:.4f} -> {report["objective"][-1]:.4f}'
+          f'{f", interpolated with {args.interpolate_with} at alpha = {args.alpha:g}" if other is not None else ""}; '
+          f'wrote {", ".join(paths)}')
     return 0
 
 
