@@ -18,7 +18,8 @@
  *    recording b is n_states[b] <= S (columns >= n_states[b] hold zeros).
  *  - calls are asynchronous on `stream` (a cudaStream_t passed as void*); there is no host
  *    synchronisation inside vbx_prepare_* / vbx_run.  One handle per (device, stream); a handle must
- *    not be used from two threads at once.
+ *    not be used from two threads at once.  Handles on different devices may be used in one process,
+ *    each from its own thread.
  *  - arithmetic is float32 on the device with float64 accumulation of the ELBO scalars; the reference
  *    is float64 numpy (parity: SURVEY.md section 8c, tests/test_parity_gpu.py).
  */

@@ -7,6 +7,8 @@
 #include <cstdio>
 #include <cstring>
 #include <initializer_list>
+#include <map>
+#include <mutex>
 #include <numeric>
 #include <string>
 #include <utility>
@@ -14,6 +16,19 @@
 
 #include "../../include/vbx_b200.h"
 #include "vbx_internal.cuh"
+
+bool vbx::allow_dynamic_smem(const void *kernel, int bytes) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) return false;
+    static std::mutex mu;
+    static std::map<std::pair<const void *, int>, int> allowed;   // (kernel, device) -> bytes set
+    std::lock_guard<std::mutex> lock(mu);
+    int &have = allowed[{kernel, dev}];
+    if (have >= bytes) return true;
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess) return false;
+    have = bytes;
+    return true;
+}
 
 struct vbx_handle_s {
     int device = 0;
@@ -826,6 +841,7 @@ int vbx_hard_labels(vbx_handle_t h, const float *gamma, const int32_t *n_states,
     if (h->plan.n_frames && (!gamma || !first_out)) return fail(h, VBX_ERR_ARG, "vbx_hard_labels: null pointer");
     if (const int rc = misaligned16(h, "vbx_hard_labels", {{gamma, "gamma"}})) return rc;
     DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     return counted(h, vbx::launch_hard_labels(h->plan, gamma, n_states, first_out, second_out, (cudaStream_t)stream), "hard_labels");
 }
 
@@ -838,6 +854,7 @@ int vbx_hard_labels_keep(vbx_handle_t h, const float *gamma, const int32_t *n_st
         return fail(h, VBX_ERR_ARG, "vbx_hard_labels_keep: null pointer");
     if (const int rc = misaligned16(h, "vbx_hard_labels_keep", {{gamma, "gamma"}})) return rc;
     DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     // keep lives on the device: read it back once to refuse counts below 1 (the labels leave the device next anyway)
     std::vector<int32_t> kh(h->plan.n_rec);
     cudaError_t e = cudaMemcpyAsync(kh.data(), keep, kh.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, (cudaStream_t)stream);
@@ -919,6 +936,7 @@ int vbx_ahc(vbx_handle_t h, const void *x, int32_t x_is_f64, int32_t dim, void *
     if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0) return fail(h, VBX_ERR_ARG, "vbx_ahc: workspace must be 256-byte aligned");
     if (workspace_bytes < h->ahc_need) return fail(h, VBX_ERR_ARG, "vbx_ahc: workspace smaller than vbx_ahc_workspace_bytes()");
     DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
     std::string why;
     int n = vbx::launch_ahc(h->plan, h->ahc_d_off, x, x_is_f64, dim, workspace, workspace_bytes, Z_out, thr_out,
                             (cudaStream_t)stream, &why);

@@ -379,19 +379,6 @@ __global__ void __launch_bounds__(kThreads) combine_vote_kernel(
     labels2_out[t] = n >= 2.0 ? g2 : -1;
 }
 
-bool g_configured[2][64] = {};                       // cudaFuncSetAttribute is per device: [overlap, map][device]
-
-bool configure(int which, const void *kernel, size_t bytes) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return false;
-    if (!g_configured[which][dev]) {
-        if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess)
-            return false;
-        g_configured[which][dev] = true;
-    }
-    return true;
-}
-
 }  // namespace
 
 size_t combine_workspace_bytes(int64_t n_rec, int K, int max_labels) {
@@ -413,8 +400,8 @@ int launch_combine(int64_t n_rec, const int64_t *offsets, int64_t N, const int64
         return -1;
     const int64_t cells = (int64_t)max_labels * max_labels;
     const int shared_block = cells <= kSmemCells;
-    if (!configure(0, reinterpret_cast<const void *>(combine_overlap_kernel), kSmemCells * 8) ||
-        !configure(1, reinterpret_cast<const void *>(combine_map_kernel), sizeof(WarpLsap) * kWarps))
+    if (!allow_dynamic_smem(combine_overlap_kernel, (int)(kSmemCells * 8)) ||
+        !allow_dynamic_smem(combine_map_kernel, (int)(sizeof(WarpLsap) * kWarps)))
         return -1;
     combine_overlap_kernel<<<(unsigned)(n_rec * (n_pairs(K) + K)), kThreads, shared_block ? cells * 8 : 0, st>>>(
         offsets, lo, hi, N, K, labels, labels2, w.n_labels, max_labels, shared_block, O, L, flags_out);

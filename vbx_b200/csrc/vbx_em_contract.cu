@@ -17,8 +17,6 @@
 #include <cooperative_groups.h>
 #include <math_constants.h>
 
-#include <mutex>
-
 #include "vbx_internal.cuh"
 
 namespace cg = cooperative_groups;
@@ -362,34 +360,19 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(128, 3)
     }
 }
 
-// Per device: the kernel's shared-memory attribute is set, and one cluster fits (1), or not (0); -1 = not yet asked.
-// Called by vbx_plan on the plan's device.
+// CL when the kernel may have its shared memory on the current device and one cluster fits there, else 0 (the three
+// kernels run instead; a refusal is not an error).  Called by vbx_plan on the plan's device.
 template <int S_PAD, int CL>
 static int em_contract_cluster_t() {
-    constexpr int kMaxDevices = 64;
-    static std::mutex mu;
-    static int ok[kMaxDevices];
-    static bool init = false;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return (void)cudaGetLastError(), 0;
-    std::lock_guard<std::mutex> lock(mu);
-    if (!init) {
-        for (int &v : ok) v = -1;
-        init = true;
-    }
-    if (ok[dev] < 0) {
-        ok[dev] = 0;
-        if (cudaFuncSetAttribute(em_contract_kernel<S_PAD, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
-            return (void)cudaGetLastError(), 0;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(CL);
-        cfg.blockDim = dim3(128);
-        cfg.dynamicSmemBytes = kSmemBytes;
-        int n = 0;
-        if (cudaOccupancyMaxActiveClusters(&n, em_contract_kernel<S_PAD, CL>, &cfg) != cudaSuccess) return (void)cudaGetLastError(), 0;
-        ok[dev] = n >= 1;
-    }
-    return ok[dev] ? CL : 0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(CL);
+    cfg.blockDim = dim3(128);
+    cfg.dynamicSmemBytes = kSmemBytes;
+    int n = 0;
+    if (!allow_dynamic_smem(em_contract_kernel<S_PAD, CL>, kSmemBytes) ||
+        cudaOccupancyMaxActiveClusters(&n, em_contract_kernel<S_PAD, CL>, &cfg) != cudaSuccess)
+        return (void)cudaGetLastError(), 0;
+    return n >= 1 ? CL : 0;
 }
 
 int em_contract_cluster(int S, int R, int64_t max_T, bool split) {

@@ -582,13 +582,8 @@ static int launch_exact64_t(const Plan &pl, const Workspace &ws, const RunParams
     constexpr int FB = x64::loglik64_frames<S_PAD>();
     const size_t sm_m = S_PAD > kMaxS ? 0 : (size_t)S_PAD * kMaxR * sizeof(double);   // S = 128: no parity reduction
     const size_t sm_l = (size_t)(kMaxR * S_PAD + FB * S_PAD) * sizeof(double) + (size_t)kMaxR * (FB + 1) * sizeof(float);
-    static bool configured = false;
-    if (!configured) {
-        if (cudaFuncSetAttribute(x64::mstep64_kernel<S_PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_m) != cudaSuccess ||
-            cudaFuncSetAttribute(x64::loglik64_kernel<S_PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_l) != cudaSuccess)
-            return -1;
-        configured = true;
-    }
+    if (!allow_dynamic_smem(x64::mstep64_kernel<S_PAD>, (int)sm_m) || !allow_dynamic_smem(x64::loglik64_kernel<S_PAD>, (int)sm_l))
+        return -1;
     x64::restore64_kernel<<<pl.n_mtiles, 256, 0, st>>>(pl, ws, gamma, n_iters);
     x64::mstep64_kernel<S_PAD><<<pl.n_mtiles, 256, sm_m, st>>>(pl, ws, rho, gamma);
     if (prior_n) x64::prior_stats64_kernel<<<pl.n_rec, 128, 0, st>>>(pl, ws, Phi, n_states, prior_n, prior_F);

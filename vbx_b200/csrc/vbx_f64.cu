@@ -419,11 +419,7 @@ int launch_run_f64(const Plan &pl, void *workspace, const double *fea, const dou
     const int fblocks = (int)((pl.n_frames + 127) / 128);
     const size_t fb_smem = (size_t)7 * pl.S * sizeof(double);     // per-state vectors of the sweep
     if (fb_smem > 48 * 1024) {
-        static bool configured = false;
-        if (!configured) {
-            if (cudaFuncSetAttribute(f64::fb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return -1;
-            configured = true;
-        }
+        if (!allow_dynamic_smem(f64::fb_kernel, 200 * 1024)) return -1;
         if (fb_smem > 200 * 1024) return -1;                      // more than 3600 states
     }
     for (int it = 0; it < max_iters; ++it) {

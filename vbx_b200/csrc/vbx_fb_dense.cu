@@ -96,12 +96,7 @@ int launch_fb_dense(const double *lls, const double *tr, const double *ip, int T
     const size_t small = (size_t)2 * S * sizeof(double);
     const size_t full = small + (size_t)S * (S + 1) * sizeof(double);
     if (full <= 200 * 1024) {
-        static bool configured = false;
-        if (!configured) {
-            if (cudaFuncSetAttribute(fb_dense_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess)
-                return -1;
-            configured = true;
-        }
+        if (!allow_dynamic_smem(fb_dense_kernel<true>, 200 * 1024)) return -1;
         fb_dense_kernel<true><<<1, threads, full, st>>>(lls, tr, ip, T, S, post, tll, lfw, lbw);
     } else {
         fb_dense_kernel<false><<<1, threads, small, st>>>(lls, tr, ip, T, S, post, tll, lfw, lbw);

@@ -446,11 +446,7 @@ int launch_split_t(const Plan &pl, const Workspace &ws, const RunParams &rp, flo
     const int n_warps = (pl.n_rec + RPW - 1) / RPW;
     const int blocks = (2 * n_warps + 3) / 4;
     const size_t smem = (size_t)(FBK * LD + NPART * NCOL) * sizeof(float);
-    static bool configured = false;
-    if (!configured) {
-        if (cudaFuncSetAttribute(fb_combine_kernel<S_PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
-        configured = true;
-    }
+    if (!allow_dynamic_smem(fb_combine_kernel<S_PAD>, (int)smem)) return -1;
     fb_sweeps_kernel<S_PAD, SPL><<<blocks, 128, 0, st>>>(pl, ws, rp, pi, n_states, n_warps);
     fb_combine_kernel<S_PAD><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rp, gamma, pi, n_states);
     fb_split_tail_kernel<S_PAD><<<(pl.n_rec + 3) / 4, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);

@@ -111,6 +111,15 @@ struct RunParams {
 constexpr double kStopNoiseC = 2.0;
 constexpr double kStopGuardMult = 16.0;
 
+// Lets `kernel` launch with up to `bytes` of dynamic shared memory on the current device.  The attribute belongs to the
+// device's context, not to the process, so it is set once per (kernel, device) that has not yet been given `bytes`
+// (thread-safe).  False when the runtime refuses; its error is left for cudaGetLastError.
+bool allow_dynamic_smem(const void *kernel, int bytes);
+template <class... Args>
+bool allow_dynamic_smem(void (*kernel)(Args...), int bytes) {
+    return allow_dynamic_smem(reinterpret_cast<const void *>(kernel), bytes);
+}
+
 #ifdef __CUDACC__
 // small vector load/store helpers shared by the kernel translation units
 template <int N>

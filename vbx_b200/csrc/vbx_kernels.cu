@@ -403,12 +403,7 @@ int launch_mstep_partial(const Plan &pl, const Workspace &ws, const float *rho, 
         case 64: mstep_partial_kernel<64><<<pl.n_mtiles, 256, 0, st>>>(pl, ws, rho, gamma); break;
         case kMaxSWide: {   // 64 KB reduction buffer in dynamic shared memory
             constexpr int smem = kMaxSWide * kMaxR * sizeof(float);
-            static bool configured = false;
-            if (!configured) {
-                if (cudaFuncSetAttribute(mstep_partial_kernel<kMaxSWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-                    return -1;
-                configured = true;
-            }
+            if (!allow_dynamic_smem(mstep_partial_kernel<kMaxSWide>, smem)) return -1;
             mstep_partial_kernel<kMaxSWide><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, gamma);
             break;
         }
@@ -564,19 +559,11 @@ int launch_speaker_model(const Plan &pl, const Workspace &ws, const float *Phi,
     const int fg = from_given ? 1 : 0;
     const bool prior = prior_n != nullptr;
     if (S8 == kMaxSWide) {   // 64 KB of staged Fa*alpha: above the default dynamic shared-memory limit
-        static bool configured = false, configured_prior = false;
-        if (!prior && !configured) {
-            if (cudaFuncSetAttribute(speaker_model_kernel<kMaxSWide, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-                cudaFuncSetAttribute(speaker_model_kernel<kMaxSWide, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-                return -1;
-            configured = true;
-        }
-        if (prior && !configured_prior) {
-            if (cudaFuncSetAttribute(speaker_model_prior_kernel<kMaxSWide, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess ||
-                cudaFuncSetAttribute(speaker_model_prior_kernel<kMaxSWide, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-                return -1;
-            configured_prior = true;
-        }
+        const bool ok = prior ? allow_dynamic_smem(speaker_model_prior_kernel<kMaxSWide, true>, (int)smem) &&
+                                    allow_dynamic_smem(speaker_model_prior_kernel<kMaxSWide, false>, (int)smem)
+                              : allow_dynamic_smem(speaker_model_kernel<kMaxSWide, true>, (int)smem) &&
+                                    allow_dynamic_smem(speaker_model_kernel<kMaxSWide, false>, (int)smem);
+        if (!ok) return -1;
     }
 #define VBX_SM(S8_, R_)                                                                                                     \
     if (prior)                                                                                                              \
@@ -711,13 +698,7 @@ template <int S_PAD>
 static int launch_loglik_t(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                            cudaStream_t st) {
     const size_t smem = loglik_smem(S_PAD, pl.R);
-    static bool configured = false;
-    if (!configured) {
-        if (cudaFuncSetAttribute(loglik_kernel<S_PAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)loglik_smem(S_PAD, kMaxR)) != cudaSuccess)
-            return -1;
-        configured = true;
-    }
+    if (!allow_dynamic_smem(loglik_kernel<S_PAD>, (int)loglik_smem(S_PAD, kMaxR))) return -1;
     loglik_kernel<S_PAD><<<pl.n_ltiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
@@ -1762,9 +1743,7 @@ static int launch_fb_t(const Plan &pl, const Workspace &ws, const RunParams &rp,
         forward_backward_kernel<S_PAD, SPL><<<blocks, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);
     } else if (ring && pl.max_T <= kRingMaxT) {   // gamma is 16-byte aligned (checked by the C entries): rows for the copies
         constexpr int smem = FbRing<S_PAD, SPL>::kSmemBytes;
-        if (cudaFuncSetAttribute(forward_backward_ring_kernel<S_PAD, SPL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 smem) != cudaSuccess)
-            return -1;
+        if (!allow_dynamic_smem(forward_backward_ring_kernel<S_PAD, SPL>, smem)) return -1;
         forward_backward_ring_kernel<S_PAD, SPL><<<blocks, 128, smem, st>>>(pl, ws, rp, gamma, pi, n_states);
     } else {
         forward_backward_la_kernel<S_PAD, SPL><<<blocks, 128, 0, st>>>(pl, ws, rp, gamma, pi, n_states);

@@ -169,12 +169,7 @@ int launch_mstep_mma(const Plan &pl, const Workspace &ws, const float *rho, cons
         case 64: mstep_mma_kernel<64><<<pl.n_mtiles, 128, 0, st>>>(pl, ws, rho, gamma); break;
         case kMaxSWide: {
             constexpr int smem = kMaxSWide * (kMaxR + 4) * sizeof(float);
-            static bool configured = false;
-            if (!configured) {
-                if (cudaFuncSetAttribute(mstep_mma_kernel<kMaxSWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-                    return -1;
-                configured = true;
-            }
+            if (!allow_dynamic_smem(mstep_mma_kernel<kMaxSWide>, smem)) return -1;
             mstep_mma_kernel<kMaxSWide><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, gamma);
             break;
         }
@@ -393,46 +388,20 @@ static size_t loglik_mma_smem(int S_pad, int R) {
 template <int S_PAD>
 static int launch_loglik_mma_t(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,
                                cudaStream_t st) {
-    static bool configured = false;
-    if constexpr (S_PAD > kMaxS) {   // split plans only (vbx_plan): the c_t variants, 8 warps per CTA
-        if (!configured) {
-            const int big = (int)loglik_mma_smem(S_PAD, kMaxR);
-            if (cudaFuncSetAttribute(loglik_mma_kernel<S_PAD, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-                cudaFuncSetAttribute(loglik_mma_kernel<S_PAD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess)
-                return -1;
-            configured = true;
-        }
-        if (!pl.split) return -1;
-        const size_t smem = loglik_mma_smem(S_PAD, pl.R);
-        if (pl.R == 128)
-            loglik_mma_kernel<S_PAD, true, true><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, pi, n_states);
-        else
-            loglik_mma_kernel<S_PAD, false, true><<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, pi, n_states);
-        return cudaGetLastError() == cudaSuccess ? 1 : -1;
-    } else {
-    if (!configured) {
-        const int big = (int)loglik_mma_smem(S_PAD, kMaxR);
-        if (cudaFuncSetAttribute(loglik_mma_kernel<S_PAD, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-            cudaFuncSetAttribute(loglik_mma_kernel<S_PAD, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-            cudaFuncSetAttribute(loglik_mma_kernel<S_PAD, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess ||
-            cudaFuncSetAttribute(loglik_mma_kernel<S_PAD, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, big) != cudaSuccess)
-            return -1;
-        configured = true;
-    }
+    const int big = (int)loglik_mma_smem(S_PAD, kMaxR);
     const size_t smem = loglik_mma_smem(S_PAD, pl.R);
-    if (pl.split) {
-        if (pl.R == 128)
-            loglik_mma_kernel<S_PAD, true, true><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
-        else
-            loglik_mma_kernel<S_PAD, false, true><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
+    if constexpr (S_PAD > kMaxS) {   // split plans only (vbx_plan): the c_t variants, 8 warps per CTA
+        if (!pl.split) return -1;
+        auto kernel = pl.R == 128 ? loglik_mma_kernel<S_PAD, true, true> : loglik_mma_kernel<S_PAD, false, true>;
+        if (!allow_dynamic_smem(kernel, big)) return -1;
+        kernel<<<pl.n_mtiles, 256, smem, st>>>(pl, ws, rho, pi, n_states);
     } else {
-        if (pl.R == 128)
-            loglik_mma_kernel<S_PAD, true, false><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
-        else
-            loglik_mma_kernel<S_PAD, false, false><<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
+        auto kernel = pl.split ? (pl.R == 128 ? loglik_mma_kernel<S_PAD, true, true> : loglik_mma_kernel<S_PAD, false, true>)
+                               : (pl.R == 128 ? loglik_mma_kernel<S_PAD, true, false> : loglik_mma_kernel<S_PAD, false, false>);
+        if (!allow_dynamic_smem(kernel, big)) return -1;
+        kernel<<<pl.n_mtiles, 128, smem, st>>>(pl, ws, rho, pi, n_states);
     }
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
-    }
 }
 
 int launch_loglik_mma(const Plan &pl, const Workspace &ws, const float *rho, const float *pi, const int32_t *n_states,

@@ -343,9 +343,6 @@ __global__ void build_plda_v_kernel(const float *__restrict__ tr, const float *_
     }
 }
 
-// cudaFuncSetAttribute is per device; everything else the launches need comes from the caller's workspace
-bool g_configured[64][3][2] = {};
-
 using EncodeTiledFn = CUresult (*)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                    const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -399,20 +396,12 @@ int launch_gemm_tc(float *vimg, int64_t N, const float *X, int D, const float *V
                    const float *a_off, const float *e_off, cudaStream_t st, std::string *err) {
     CUtensorMap xmap;
     if (!encode_x_map(&xmap, X, N, D, err)) return -1;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64) {
-        if (err) *err = "device index out of range";
+    if (!allow_dynamic_smem(project_wgmma_kernel<MODE, NS>, Pipe<NS>::kSmemBytes)) {
+        if (err) *err = "the device refused the wgmma projection's shared-memory size";
         return -1;
     }
-    if (!g_configured[dev][MODE][NS - 2]) {
-        if (cudaFuncSetAttribute(project_wgmma_kernel<MODE, NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Pipe<NS>::kSmemBytes) !=
-            cudaSuccess) {
-            if (err) *err = "cudaFuncSetAttribute(smem) failed";
-            return -1;
-        }
-        g_configured[dev][MODE][NS - 2] = true;
-    }
+    int dev = 0;
+    cudaGetDevice(&dev);
     int sms = 0;
     if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms < 1) {
         if (err) *err = "cudaDeviceGetAttribute(multiprocessor count) failed";

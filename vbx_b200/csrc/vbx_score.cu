@@ -227,9 +227,6 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(
     }
 }
 
-// cudaFuncSetAttribute is per device and per instantiation: [kSecond + 2 kLabelTime][device]
-bool g_score_configured[4][64] = {};
-
 }  // namespace
 
 int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const int64_t *sys_hi, const int64_t *sys_join_hi,
@@ -242,7 +239,6 @@ int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const
                  cudaStream_t st) {
     if (n_entries == 0) return 0;
     const bool second = labels2 != nullptr, label_time = T_out != nullptr;
-    const int variant = (int)second + 2 * (int)label_time;
     auto kernel = label_time ? (second ? score_kernel<true, true> : score_kernel<false, true>)
                              : (second ? score_kernel<true, false> : score_kernel<false, false>);
     const int64_t smem_cells = max_cells < kScoreSmemCells ? max_cells : kScoreSmemCells;
@@ -250,16 +246,7 @@ int launch_score(int n_rec, const int64_t *sys_off, const int64_t *sys_lo, const
     const int64_t smem_words = smem_cells + (label_time ? kScoreSmemLabels : 0);
     const int64_t max_words = kScoreSmemCells + (label_time ? kScoreSmemLabels : 0);
     const size_t smem = (size_t)smem_words * sizeof(unsigned long long);
-    if (smem > 48 * 1024) {
-        int dev = 0;
-        if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return -1;
-        if (!g_score_configured[variant][dev]) {
-            if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)(max_words * sizeof(unsigned long long))) != cudaSuccess)
-                return -1;
-            g_score_configured[variant][dev] = true;
-        }
-    }
+    if (smem > 48 * 1024 && !allow_dynamic_smem(kernel, (int)(max_words * sizeof(unsigned long long)))) return -1;
     kernel<<<n_entries, kScoreThreads, smem, st>>>(n_rec, sys_off, sys_lo, sys_hi, sys_join_hi, reg_off, reg_lo, reg_hi, reg_mask,
                                                    reg_ovl, n_ref, entry_rec, label_off, labels, labels2, n_labels, o_off,
                                                    max_cells, smem_cells, covered_out, fa_out, O_out, flags_out, t_off, T_out);
