@@ -339,6 +339,54 @@ int vbx_cohort_stats_batch(vbx_handle_t h, const float *fea, const float *Phi, i
                            void *workspace, size_t workspace_bytes, double *mean_out, double *std_out,
                            double *scores_out, void *stream);
 
+/* Speaker-verification trials (DESIGN.md section 5.27).  Each needs a handle, no plan; stream ordered, no allocation,
+ * no host synchronisation; small scalars go to the device in one copy from pageable host memory.
+ *
+ * vbx_verify_score: T trials, each an enrolment item against a test item.  The enrolment side is enroll_fea [N_e,R]
+ * float32 with enroll_item [N_e] int32 in [0, M_e) (-1: none), the test side test_fea [N_t,R] with test_item [N_t] in
+ * [0, M_t), Phi [R] (all DEVICE: x-vectors through the front end, R <= 128; every item should own an x-vector).  Each
+ * item gets vbx_link_batch's statistics n, F, b, e with c = Fa / Fb (Fa, Fb finite and > 0); pack each item's x-vectors
+ * together, as for vbx_link_batch (spread-out items cost up to M N reads).  Trial t = (trial_enroll[t], trial_test[t])
+ * (DEVICE int32) writes score_out [T] (DEVICE float64) in trial order:
+ *   LLR(i, j) of vbx_link_batch, bit-identical to vbx_enroll_batch's and vbx_cohort_stats_batch's score of the pair
+ *   (enrolment item as the row) and to the swapped trial's score with the sides swapped,
+ * or with enroll_mean, enroll_std [M_e] and test_mean, test_std [M_t] (DEVICE, all four or none: cohort statistics
+ * from vbx_cohort_stats_batch, every std finite and > 0) the AS-norm score
+ *   S = 1/2 [ (LLR - enroll_mean[i]) / enroll_std[i] + (LLR - test_mean[j]) / test_std[j] ].
+ * A trial whose index lies outside its side scores NaN.  workspace: vbx_verify_score_workspace_bytes(M_e, M_t) bytes,
+ * 256-byte aligned: about 1.1 KB per item.  VBX_ERR_ARG: M_e, M_t, N_e or N_t < 1, T < 0, R outside 1 .. 128, a bad
+ * Fa or Fb, some but not all of the four statistics, null pointers, a misaligned or short workspace.
+ *
+ * vbx_verify_metrics: the error rates of T >= 1 scores [T] (DEVICE float64) with is_target [T] (DEVICE uint8, nonzero =
+ * target trial) at n_op operating points p_target [n_op] (HOST, each in (0, 1)) with costs c_miss, c_fa (finite, > 0).
+ * Candidate thresholds are the distinct scores (-0.0 and +0.0 one value) and +inf; at threshold t a trial is accepted
+ * when score >= t, P_miss(t) = #targets below t / N_tar and P_fa(t) = #nontargets at or above t / N_non (exact counts,
+ * one float64 division each).  Outputs (DEVICE):
+ *   counts_out [3] int64      N_tar, N_non and the number of non-finite scores (the metrics are meaningless then)
+ *   eer_out [1]               with k the first candidate where P_miss >= P_fa, a and b = P_miss - P_fa at k - 1 and k:
+ *                             P_fa(k-1) + a / (a - b) (P_fa(k) - P_fa(k-1))
+ *   min_dcf_out [n_op]        min over the candidates of (c_miss p P_miss + c_fa (1-p) P_fa) / min(c_miss p, c_fa (1-p))
+ *   threshold_out [n_op]      the lowest candidate attaining it
+ *   act_dcf_out [n_op]        the same cost at the Bayes threshold log(c_fa (1-p) / (c_miss p)), score >= it accepted
+ *   cllr_out [1]              1 / (2 ln 2) [mean over targets of softplus(-s) + mean over nontargets of softplus(s)]
+ * The metrics need N_tar, N_non >= 1 (NaN otherwise).  The sort is cub::DeviceRadixSort; every reduction runs in a
+ * fixed order without floating-point atomics, so a call is bit-identical from run to run and for any order of the trials.
+ * workspace: vbx_verify_metrics_workspace_bytes(T, n_op) bytes (the sort's temporary storage included; sized for the
+ * handle's device), 256-byte aligned: about 34 T bytes plus the sort's.  VBX_ERR_ARG: T < 1, n_op outside 1 ..
+ * VBX_VERIFY_MAX_OPS, a p_target outside (0, 1), bad costs, null pointers, a misaligned or short workspace. */
+#define VBX_VERIFY_MAX_OPS 64
+int vbx_verify_score_workspace_bytes(vbx_handle_t h, int32_t M_e, int32_t M_t, size_t *bytes_out);
+int vbx_verify_score(vbx_handle_t h, const float *enroll_fea, int64_t N_e, const int32_t *enroll_item, int32_t M_e,
+                     const float *test_fea, int64_t N_t, const int32_t *test_item, int32_t M_t, int32_t R,
+                     const float *Phi, double Fa, double Fb, const int32_t *trial_enroll, const int32_t *trial_test,
+                     int64_t T, const double *enroll_mean, const double *enroll_std, const double *test_mean,
+                     const double *test_std, void *workspace, size_t workspace_bytes, double *score_out, void *stream);
+int vbx_verify_metrics_workspace_bytes(vbx_handle_t h, int64_t T, int32_t n_op, size_t *bytes_out);
+int vbx_verify_metrics(vbx_handle_t h, const double *scores, const uint8_t *is_target, int64_t T, int32_t n_op,
+                       const double *p_target, double c_miss, double c_fa, void *workspace, size_t workspace_bytes,
+                       int64_t *counts_out, double *eer_out, double *cllr_out, double *min_dcf_out,
+                       double *threshold_out, double *act_dcf_out, void *stream);
+
 /* Float64 evaluation of the same EM loop ("exact" mode for the one-recording-per-call use of VBx/vbhmm.py:154-158,
  * where the reference stops on an ELBO improvement < 1e-6, VBx/vbhmm.py:157 -- below float32 resolution).
  * All arrays float64: fea [N,R] (the reference's X, VBx/VBx.py:30), Phi [R], gamma_io [N,S], pi_io [n_rec,S],

@@ -17,7 +17,8 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_enroll_batch_workspace_bytes', 'vbx_enroll_batch', 'vbx_cohort_stats_batch_workspace_bytes',
            'vbx_cohort_stats_batch', 'vbx_init_turns', 'vbx_combine_workspace_bytes', 'vbx_combine',
            'vbx_init_random', 'vbx_run_prior', 'vbx_run_f64_prior', 'vbx_class_scatter_workspace_bytes',
-           'vbx_class_scatter', 'vbx_stream_window', 'vbx_stream_commit']
+           'vbx_class_scatter', 'vbx_stream_window', 'vbx_stream_commit', 'vbx_verify_score_workspace_bytes',
+           'vbx_verify_score', 'vbx_verify_metrics_workspace_bytes', 'vbx_verify_metrics']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
@@ -141,6 +142,16 @@ def load():
                                       vp, vp, vp, vp, vp, vp]
     lib.vbx_stream_commit.restype = ctypes.c_int
     lib.vbx_stream_commit.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.vbx_verify_score_workspace_bytes.restype = ctypes.c_int
+    lib.vbx_verify_score_workspace_bytes.argtypes = [vp, i32, i32, ctypes.POINTER(ctypes.c_size_t)]
+    lib.vbx_verify_score.restype = ctypes.c_int
+    lib.vbx_verify_score.argtypes = [vp, vp, i64, vp, i32, vp, i64, vp, i32, i32, vp, dbl, dbl, vp, vp, i64, vp, vp, vp,
+                                     vp, vp, ctypes.c_size_t, vp, vp]
+    lib.vbx_verify_metrics_workspace_bytes.restype = ctypes.c_int
+    lib.vbx_verify_metrics_workspace_bytes.argtypes = [vp, i64, i32, ctypes.POINTER(ctypes.c_size_t)]
+    lib.vbx_verify_metrics.restype = ctypes.c_int
+    lib.vbx_verify_metrics.argtypes = [vp, vp, vp, i64, i32, vp, dbl, dbl, vp, ctypes.c_size_t, vp, vp, vp, vp, vp, vp,
+                                       vp]
     lib.vbx_get_timings.restype = ctypes.c_int
     lib.vbx_get_timings.argtypes = [vp, ctypes.POINTER(dbl), ctypes.POINTER(i64), i32]
     _lib = lib

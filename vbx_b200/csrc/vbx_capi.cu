@@ -1125,6 +1125,94 @@ int vbx_cohort_stats_batch(vbx_handle_t h, const float *fea, const float *Phi, i
                    "cohort_batch");
 }
 
+int vbx_verify_score_workspace_bytes(vbx_handle_t h, int32_t M_e, int32_t M_t, size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    if (M_e < 1 || M_t < 1) return fail(h, VBX_ERR_ARG, "vbx_verify_score_workspace_bytes: need M_e, M_t >= 1");
+    *bytes_out = vbx::verify_score_workspace_bytes(M_e, M_t);
+    return VBX_OK;
+}
+
+int vbx_verify_score(vbx_handle_t h, const float *enroll_fea, int64_t N_e, const int32_t *enroll_item, int32_t M_e,
+                     const float *test_fea, int64_t N_t, const int32_t *test_item, int32_t M_t, int32_t R,
+                     const float *Phi, double Fa, double Fb, const int32_t *trial_enroll, const int32_t *trial_test,
+                     int64_t T, const double *enroll_mean, const double *enroll_std, const double *test_mean,
+                     const double *test_std, void *workspace, size_t workspace_bytes, double *score_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_verify_score");
+    const std::string who("vbx_verify_score");
+    if (M_e < 1 || M_t < 1 || N_e < 1 || N_t < 1 || T < 0)
+        return fail(h, VBX_ERR_ARG, who + ": need M_e, M_t, N_e, N_t >= 1 and T >= 0");
+    if (R < 1 || R > vbx::kMaxR) return fail(h, VBX_ERR_ARG, who + ": R must lie in [1, 128]");
+    if (!(std::isfinite(Fa) && Fa > 0.0 && std::isfinite(Fb) && Fb > 0.0))
+        return fail(h, VBX_ERR_ARG, who + ": Fa and Fb must be finite and > 0");
+    const double c = Fa / Fb;
+    if (!(c > 0.0) || c == INFINITY) return fail(h, VBX_ERR_ARG, who + ": Fa / Fb must be finite and > 0");
+    const int n_norm = !!enroll_mean + !!enroll_std + !!test_mean + !!test_std;
+    if (n_norm != 0 && n_norm != 4)
+        return fail(h, VBX_ERR_ARG, who + ": give all four of enroll_mean, enroll_std, test_mean and test_std, or none");
+    if (!enroll_fea || !enroll_item || !test_fea || !test_item || !Phi || !workspace ||
+        (T > 0 && (!trial_enroll || !trial_test || !score_out)))
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
+        return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
+    if (workspace_bytes < vbx::verify_score_workspace_bytes(M_e, M_t))
+        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_verify_score_workspace_bytes()");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_verify_score(enroll_fea, N_e, enroll_item, M_e, test_fea, N_t, test_item, M_t, R, Phi,
+                                               c, trial_enroll, trial_test, T, enroll_mean, enroll_std, test_mean,
+                                               test_std, workspace, score_out, (cudaStream_t)stream),
+                   "verify_score");
+}
+
+int vbx_verify_metrics_workspace_bytes(vbx_handle_t h, int64_t T, int32_t n_op, size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    if (T < 1 || n_op < 1 || n_op > VBX_VERIFY_MAX_OPS)
+        return fail(h, VBX_ERR_ARG, "vbx_verify_metrics_workspace_bytes: need T >= 1 and n_op in [1, VBX_VERIFY_MAX_OPS]");
+    DeviceGuard guard(h->device);         // the sort's temporary storage is sized for the handle's device
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    *bytes_out = vbx::verify_metrics_workspace_bytes(T, n_op);
+    return VBX_OK;
+}
+
+int vbx_verify_metrics(vbx_handle_t h, const double *scores, const uint8_t *is_target, int64_t T, int32_t n_op,
+                       const double *p_target, double c_miss, double c_fa, void *workspace, size_t workspace_bytes,
+                       int64_t *counts_out, double *eer_out, double *cllr_out, double *min_dcf_out,
+                       double *threshold_out, double *act_dcf_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_verify_metrics");
+    const std::string who("vbx_verify_metrics");
+    if (T < 1 || n_op < 1 || n_op > VBX_VERIFY_MAX_OPS)
+        return fail(h, VBX_ERR_ARG, who + ": need T >= 1 and n_op in [1, VBX_VERIFY_MAX_OPS]");
+    if (!(std::isfinite(c_miss) && c_miss > 0.0 && std::isfinite(c_fa) && c_fa > 0.0))
+        return fail(h, VBX_ERR_ARG, who + ": c_miss and c_fa must be finite and > 0");
+    if (!scores || !is_target || !p_target || !workspace || !counts_out || !eer_out || !cllr_out || !min_dcf_out ||
+        !threshold_out || !act_dcf_out)
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    std::vector<double> ops(4 * (size_t)n_op);
+    for (int32_t o = 0; o < n_op; ++o) {
+        const double p = p_target[o];
+        if (!(p > 0.0 && p < 1.0))
+            return fail(h, VBX_ERR_ARG, who + ": p_target[" + std::to_string(o) + "] must lie in (0, 1)");
+        ops[4 * o] = c_miss * p;
+        ops[4 * o + 1] = c_fa * (1.0 - p);
+        ops[4 * o + 2] = std::min(ops[4 * o], ops[4 * o + 1]);
+        ops[4 * o + 3] = std::log(ops[4 * o + 1] / ops[4 * o]);
+        if (!(ops[4 * o + 2] > 0.0) || !std::isfinite(ops[4 * o + 3]))
+            return fail(h, VBX_ERR_ARG, who + ": the costs of p_target[" + std::to_string(o) + "] are out of range");
+    }
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
+        return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    if (workspace_bytes < vbx::verify_metrics_workspace_bytes(T, n_op))
+        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_verify_metrics_workspace_bytes()");
+    return counted(h, vbx::launch_verify_metrics(scores, is_target, T, ops.data(), n_op, workspace,
+                                                 reinterpret_cast<long long *>(counts_out), eer_out, cllr_out,
+                                                 min_dcf_out, threshold_out, act_dcf_out, (cudaStream_t)stream),
+                   "verify_metrics");
+}
+
 int vbx_f64_workspace_bytes(vbx_handle_t h, size_t *bytes_out) {
     if (!h || !bytes_out) return VBX_ERR_ARG;
     if (!h->planned) return fail(h, VBX_ERR_STATE, "vbx_f64_workspace_bytes: call vbx_plan first");

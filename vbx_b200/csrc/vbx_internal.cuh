@@ -425,6 +425,19 @@ int launch_cohort_batch(const float *fea, const float *Phi, int64_t N, int R, co
 int launch_norm_scores(double *x, int64_t rows, int64_t cols, const double *mean_r, const double *std_r,
                        const double *mean_c, const double *std_c, bool link, double skip, double *copy_out,
                        cudaStream_t st, const NormProblems &q);
+// speaker-verification trials (vbx_verify.cu): statistics of both sides, the trial scores (mean_e .. std_t all DEVICE,
+// all four or none: AS-norm), and the error rates of a scored list; ops_host [n_op, 4] = C_miss p, C_fa (1 - p), their
+// min and the Bayes threshold of every operating point (HOST)
+size_t verify_score_workspace_bytes(int64_t M_e, int64_t M_t);
+int launch_verify_score(const float *enroll_fea, int64_t N_e, const int32_t *enroll_item, int64_t M_e,
+                        const float *test_fea, int64_t N_t, const int32_t *test_item, int64_t M_t, int R,
+                        const float *Phi, double c, const int32_t *ti, const int32_t *tj, int64_t T,
+                        const double *mean_e, const double *std_e, const double *mean_t, const double *std_t,
+                        void *workspace, double *score_out, cudaStream_t st);
+size_t verify_metrics_workspace_bytes(int64_t T, int n_op);
+int launch_verify_metrics(const double *scores, const uint8_t *is_target, int64_t T, const double *ops_host, int n_op,
+                          void *workspace, long long *counts_out, double *eer_out, double *cllr_out,
+                          double *min_dcf_out, double *threshold_out, double *act_dcf_out, cudaStream_t st);
 // wgmma projection (vbx_project_tc.cu)
 size_t tc_scratch_floats();
 int launch_project_wgmma(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,

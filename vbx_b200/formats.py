@@ -252,6 +252,37 @@ def read_enrolment(ark, utt2spk):
     return {k: np.stack(v) for k, v in out.items()}
 
 
+def read_trials(path, enrol_items=None, test_items=None):
+    """Kaldi trial list, one 'enrol-id test-id [target|nontarget]' line per trial; blank lines skipped, duplicates kept.
+    Returns (enrol ids, test ids, is_target bool array or None when every line has two columns).  ValueError: lines of
+    both two and three columns, another column count, a label word other than target / nontarget, an empty list, and
+    with enrol_items / test_items (the ids of each side) an id that is not an item of its side."""
+    known = [None if v is None else set(v) for v in (enrol_items, test_items)]
+    enrol, test, lab, ncols = [], [], [], set()
+    with open(path) as f:
+        for n, line in enumerate(f, 1):
+            p = line.split()
+            if not p:
+                continue
+            if len(p) not in (2, 3):
+                raise ValueError(f'{path}:{n}: expected "enrol-id test-id [target|nontarget]", got {line.strip()!r}')
+            ncols.add(len(p))
+            if len(ncols) > 1:
+                raise ValueError(f'{path}:{n}: lines of two and of three columns mixed')
+            if len(p) == 3:
+                if p[2] not in ('target', 'nontarget'):
+                    raise ValueError(f'{path}:{n}: the label {p[2]!r} is neither target nor nontarget')
+                lab.append(p[2] == 'target')
+            for k, side in ((0, 'enrolment'), (1, 'test')):
+                if known[k] is not None and p[k] not in known[k]:
+                    raise ValueError(f'{path}:{n}: {p[k]!r} is not an item of the {side} side')
+            enrol.append(p[0])
+            test.append(p[1])
+    if not enrol:
+        raise ValueError(f'{path}: no trials')
+    return enrol, test, (np.array(lab, dtype=bool) if ncols == {3} else None)
+
+
 def read_speaker_counts(path):
     """Two-column 'recording count' file -> {recording: int}.  Blank lines and lines starting with '#' are skipped."""
     out = {}
