@@ -1,12 +1,14 @@
 """Device time of the fused EM contraction alone (em_contract_kernel, vbx_em_contract.cu), against the HBM bytes its shapes
 must move, on the headline shape: 4096 recordings x 1000 frames, S = 16, R = 128, 10 iterations (one launch each).
+--frames / --recordings time other shapes: recordings of at most 512 frames take clusters of 4 CTAs instead of 8 (e.g.
+--frames 500 --recordings 8192).
 
 bytes per launch:  rho read once (4 R), gamma read (4 S), p and rowmax written (4 S + 4) per frame, plus alpha and invL
                    written (2 x 4 S R) per recording
 Kernel times come from torch.profiler (CUDA activity) over --runs calls of vbx_run after a warm-up; the achieved bandwidth
 is those bytes over the kernel's device time, also as a fraction of 3.35 TB/s (H100 SXM data sheet).
 
-    python tools/bench_em_contract.py [--runs 5] [--out result.json]
+    python tools/bench_em_contract.py [--runs 5] [--frames 1000] [--recordings 4096] [--out result.json]
 """
 import argparse
 import json
@@ -24,14 +26,19 @@ from vbx_b200 import synth  # noqa: E402
 from vbx_b200.batch import VbxBatch  # noqa: E402
 
 HBM = 3.35e12
-B, T, R, S, ITERS = 4096, 1000, 128, 16, 10
+R, S, ITERS = 128, 16, 10
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--runs', type=int, default=5)
+    ap.add_argument('--frames', type=int, default=1000, help='frames per recording (at most 1024)')
+    ap.add_argument('--recordings', type=int, default=4096, help='a multiple of 8')
     ap.add_argument('--out', default=None)
     a = ap.parse_args()
+    B, T = a.recordings, a.frames
+    if not 0 < T <= 1024 or B <= 0 or B % 8:
+        raise SystemExit('--frames must be 1 .. 1024 and --recordings a positive multiple of 8')
     if not torch.cuda.is_available():
         raise SystemExit('bench_em_contract.py needs a CUDA device')
     dev = torch.device('cuda:0')

@@ -52,18 +52,17 @@ __device__ __forceinline__ void st_async(uint32_t addr, float v, uint32_t bar) {
 // statement, so that both compute the same invL, alpha, bias and regulariser bit for bit (tests/test_em_contract_gpu.py
 // holds them to it).  speaker_model_body keeps its own copy: calling this from it changes the register allocation and so
 // the machine code of the speaker-model kernels.  A change to either copy must be made to both.  The thread is column r
-// of state s, its warp r / 32; gr = sum over the recording's M-tiles of gamma^T rho in tile order (float64).  Returns
-// Fa * alpha and the values alpha_io / invL_io take (all 0 in dead columns); the warp's sums of the bias and regulariser
-// terms go to cpart[s][warp] / rpart[s][warp].
-__device__ __forceinline__ float speaker_state(const Workspace &ws, int rec, int S, int s, int r, int ns, float phi, float Fa,
-                                               float FaFb, double gr, float &alpha_out, float &invL_out,
-                                               double (*cpart)[4], double (*rpart)[4]) {
+// of state s, its warp r / 32; Ns = ws.occ of the state, read by the caller (only for live states); gr = sum over the
+// recording's M-tiles of gamma^T rho in tile order (float64).  Returns Fa * alpha and the values alpha_io / invL_io take
+// (all 0 in dead columns); the warp's sums of the bias and regulariser terms go to cpart[s][warp] / rpart[s][warp].
+__device__ __forceinline__ float speaker_state(int s, int r, int ns, float Ns, float phi, float Fa, float FaFb, double gr,
+                                               float &alpha_out, float &invL_out, double (*cpart)[4],
+                                               double (*rpart)[4]) {
     const int warp = r >> 5, lane = r & 31;
     const bool dead = s >= ns;   // dead (or padding) column: never wins, never contributes
     float invL = 1.f, alpha = 0.f, Av = 0.f;
     float c = 0.f, reg = 0.f;
     if (!dead) {
-        const float Ns = ws.occ[(int64_t)rec * S + s];
         invL = 1.f / (1.f + FaFb * Ns * phi);
         alpha = (float)((double)(FaFb * invL) * gr);
         Av = Fa * alpha;
@@ -81,12 +80,12 @@ __device__ __forceinline__ float speaker_state(const Workspace &ws, int rec, int
     }
     return Av;
 }
-// bias (returned) and regulariser (regp) of state s from the four warps' sums of speaker_state
-__device__ __forceinline__ float speaker_bias(const Workspace &ws, int rec, int s, int ns, double (*cpart)[4],
-                                              double (*rpart)[4], double &regp) {
+// bias (returned) and regulariser (regp) of state s from the four warps' sums of speaker_state; dFa = ws.hp[rec].dFa
+__device__ __forceinline__ float speaker_bias(double dFa, int s, int ns, double (*cpart)[4], double (*rpart)[4],
+                                              double &regp) {
     const bool dead = s >= ns;
     regp = dead ? 0.0 : (rpart[s][0] + rpart[s][1]) + (rpart[s][2] + rpart[s][3]);
-    return dead ? CUDART_INF_F : (float)(ws.hp[rec].dFa * 0.5 * ((cpart[s][0] + cpart[s][1]) + (cpart[s][2] + cpart[s][3])));
+    return dead ? CUDART_INF_F : (float)(dFa * 0.5 * ((cpart[s][0] + cpart[s][1]) + (cpart[s][2] + cpart[s][3])));
 }
 }  // namespace
 
@@ -123,6 +122,19 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(128, 3)
     const int nchunks = (len + kRows - 1) / kRows;
     const int nmine = nchunks > fs ? (nchunks - fs + kSlots - 1) / kSlots : 0;   // held chunks c = fs + 4i, i < nmine
     const int nmt = (nmine + 1) >> 1;                                            // m-tiles of 16 held rows
+    // The speaker model's inputs from global memory, read while rho is loading.  Read behind the cluster barrier, as
+    // they were, they put up to three dependent L2 round trips between the M-step and the log-likelihood (the
+    // occupancies wait for n_states, the bias for a read behind a CTA barrier), and that path holds the CTA's rho slice.
+    const int ns = n_states ? n_states[rec] : S_PAD;
+    const float phi = Phi[tid];
+    const float Fa = ws.hp[rec].Fa, FaFb = ws.hp[rec].FaFb;
+    const double dFa = ws.hp[rec].dFa;
+    float Ns[NOWN];
+#pragma unroll
+    for (int k = 0; k < NOWN; ++k) {
+        const int s = rank + CL * k;
+        Ns[k] = s < ns ? ws.occ[(int64_t)rec * S_PAD + s] : 0.f;
+    }
 
     // ---- load: held chunk i on mbarrier i / 4; rows past the end of the recording (up to the last m-tile) are zero ----
     if (tid == 0) {
@@ -202,11 +214,22 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(128, 3)
     // ---- speaker model of the owned states s = rank + CL k; thread = r ----
     // The global stores of the speaker model wait until the slot sums are no longer needed: a cluster barrier's release
     // would otherwise wait for them to drain.
-    const int ns = n_states ? n_states[rec] : S_PAD;
     float avs[NOWN], alphas[NOWN], invLs[NOWN];
     {
-        const float phi = Phi[tid];
-        const float Fa = ws.hp[rec].Fa, FaFb = ws.hp[rec].FaFb;
+        // Every slot accumulator the thread needs, from every CTA of the cluster, is read before any is summed, so that
+        // the distributed-shared-memory reads are in flight together.  Read per state, each state's reads would wait
+        // behind the previous state's stores to cpart and rpart (the compiler cannot tell the two memories apart).
+        // Tiles past the recording's end are read but not summed.
+        constexpr int MT = CL / kSlots;   // M-tiles of the cluster
+        float red_v[NOWN][MT][kSlots];
+#pragma unroll
+        for (int k = 0; k < NOWN; ++k) {
+            const int s = min(rank + CL * k, S8 - 1);
+#pragma unroll
+            for (int t = 0; t < MT; ++t)
+#pragma unroll
+                for (int k2 = 0; k2 < kSlots; ++k2) red_v[k][t][k2] = cluster.map_shared_rank(&red[s][tid], kSlots * t + k2)[0];
+        }
 #pragma unroll
         for (int k = 0; k < NOWN; ++k) {
             const int s = rank + CL * k;
@@ -214,20 +237,23 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(128, 3)
             if (s < S8) {
                 double gr = 0.0;
                 if (s < ns)
-                    for (int t = 0; t < ntiles; ++t) {
-                        float v = cluster.map_shared_rank(&red[s][tid], kSlots * t)[0];
 #pragma unroll
-                        for (int k2 = 1; k2 < kSlots; ++k2) v += cluster.map_shared_rank(&red[s][tid], kSlots * t + k2)[0];
-                        gr += (double)v;
+                    for (int t = 0; t < MT; ++t) {
+                        if (t < ntiles) {
+                            float v = red_v[k][t][0];
+#pragma unroll
+                            for (int k2 = 1; k2 < kSlots; ++k2) v += red_v[k][t][k2];
+                            gr += (double)v;
+                        }
                     }
-                avs[k] = speaker_state(ws, rec, S_PAD, s, tid, ns, phi, Fa, FaFb, gr, alphas[k], invLs[k], cpart, rpart);
+                avs[k] = speaker_state(s, tid, ns, Ns[k], phi, Fa, FaFb, gr, alphas[k], invLs[k], cpart, rpart);
             }
         }
     }
     __syncthreads();
     float own_bias = 0.f;
     double own_regp = 0.0;
-    if (tid < NOWN && rank + CL * tid < S_PAD) own_bias = speaker_bias(ws, rec, rank + CL * tid, ns, cpart, rpart, own_regp);
+    if (tid < NOWN && rank + CL * tid < S_PAD) own_bias = speaker_bias(dFa, rank + CL * tid, ns, cpart, rpart, own_regp);
     cluster.sync();   // every peer has read the slot sums: their space takes Fa*alpha and the bias
     {
         // column r of state s  ->  fragment element ((i KS + j) 32 + 4 gs + fq) 2 + e of loglik_mma's R = 128 permutation
