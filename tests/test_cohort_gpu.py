@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from oracle import enroll_oracle, link_oracle, norm_oracle
+from test_link_gpu import SPEAKER_WIDTHS, width_phi
 from vbx_b200 import cohort, enroll, link, pipeline
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden')
@@ -19,8 +20,8 @@ THRESHOLDS = (-1e6, -20.0, -2.0, 0.0, 1.0, 5.0, 1e6)
 
 def _ragged(seed, R, R_live, C, counts=(3, 0, 128, 1, 17, 0, 2, 40, 150)):
     """A seeded archive (recordings without x-vectors, 1 .. 150 speakers per recording with gaps in the label values, a
-    speaker with one x-vector, features >= R_live padded with zeros) and C cohort speakers packed by speaker, drawn
-    around the same pool of centres."""
+    speaker with one x-vector, features >= R_live padded with zeros, Phi from width_phi at the SPEAKER_WIDTHS) and C
+    cohort speakers packed by speaker, drawn around the same pool of centres."""
     rng = np.random.default_rng(seed)
     centres = rng.standard_normal((40, R_live)) * 2.0
     lens, labels, feas = [], [], []
@@ -41,7 +42,7 @@ def _ragged(seed, R, R_live, C, counts=(3, 0, 128, 1, 17, 0, 2, 40, 150)):
         f[:, :R_live] = who[np.searchsorted(vals, lab)] + rng.standard_normal((len(lab), R_live))
         feas.append(f)
     Phi = np.zeros(R, dtype=np.float32)
-    Phi[:R_live] = np.sort(rng.uniform(0.2, 6.0, R_live))[::-1]
+    Phi[:R_live] = width_phi(rng, R) if R in SPEAKER_WIDTHS else np.sort(rng.uniform(0.2, 6.0, R_live))[::-1]
     offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
     cspk = np.repeat(np.arange(C), rng.integers(1, 7, C))
     cfea = np.zeros((len(cspk), R), dtype=np.float32)
@@ -59,8 +60,9 @@ def _oracle(fea, Phi, offs, labels, cfea, cspk):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('C', [2, 33, 1000])
-@pytest.mark.parametrize('R,R_live', [(128, 128), (16, 13), (8, 1)])
+@pytest.mark.parametrize('R,R_live,C', [(R, R_live, C) for C in (2, 33, 1000)
+                                        for R, R_live in ((128, 128), (16, 13), (8, 1))]
+                         + [(R, R, 33) for R in SPEAKER_WIDTHS])
 def test_stats_equal_the_oracle(R, R_live, C):
     fea, Phi, offs, labels, cfea, cspk = _ragged(R + C, R, R_live, C)
     table, n, F, L0 = _oracle(fea, Phi, offs, labels, cfea, cspk)
@@ -133,7 +135,7 @@ def _partition(table, maps):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('R,R_live', [(128, 128), (16, 13)])
+@pytest.mark.parametrize('R,R_live', [(128, 128), (16, 13)] + [(R, R) for R in SPEAKER_WIDTHS])
 def test_normalised_link_distances(R, R_live):
     fea, Phi, offs, labels, cfea, cspk = _ragged(7 + R, R, R_live, 60, counts=(3, 0, 128, 1, 17, 0, 2, 40))
     table, n, F, L0 = _oracle(fea, Phi, offs, labels, cfea, cspk)

@@ -11,8 +11,9 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import enroll_oracle, link_oracle
-from vbx_b200 import enroll, link, pipeline, score
+from oracle import enroll_oracle, link_oracle, norm_oracle
+from test_link_gpu import SPEAKER_WIDTHS, width_phi
+from vbx_b200 import cohort, enroll, link, pipeline, score
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden')
 C = 0.3 / 17
@@ -21,8 +22,8 @@ THRESHOLDS = (-1e6, -50.0, 0.0, 20.0, 1e6)
 
 def _ragged(seed, R, R_live, E, counts=(3, 0, 128, 1, 17, 0, 2, 40, 150)):
     """A seeded archive (recordings without x-vectors, 1 .. 150 speakers per recording with gaps in the label values, a
-    speaker with one x-vector, features >= R_live padded with zeros) and E enrolled speakers, packed by speaker, drawn
-    around the same pool of centres."""
+    speaker with one x-vector, features >= R_live padded with zeros, Phi from width_phi at the SPEAKER_WIDTHS) and E
+    enrolled speakers, packed by speaker, drawn around the same pool of centres."""
     rng = np.random.default_rng(seed)
     centres = rng.standard_normal((40, R_live)) * 2.0
     lens, labels, feas = [], [], []
@@ -43,7 +44,7 @@ def _ragged(seed, R, R_live, E, counts=(3, 0, 128, 1, 17, 0, 2, 40, 150)):
         f[:, :R_live] = who[np.searchsorted(vals, lab)] + rng.standard_normal((len(lab), R_live))
         feas.append(f)
     Phi = np.zeros(R, dtype=np.float32)
-    Phi[:R_live] = np.sort(rng.uniform(0.2, 6.0, R_live))[::-1]
+    Phi[:R_live] = width_phi(rng, R) if R in SPEAKER_WIDTHS else np.sort(rng.uniform(0.2, 6.0, R_live))[::-1]
     offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
     espk = np.repeat(np.arange(E), rng.integers(1, 7, E))
     efea = np.zeros((len(espk), R), dtype=np.float32)
@@ -64,8 +65,9 @@ def _oracle(fea, Phi, offs, labels, efea, espk):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('E', [1, 7, 300])
-@pytest.mark.parametrize('R,R_live', [(128, 128), (16, 13), (8, 1)])
+@pytest.mark.parametrize('R,R_live,E', [(R, R_live, E) for E in (1, 7, 300)
+                                        for R, R_live in ((128, 128), (16, 13), (8, 1))]
+                         + [(R, R, 33) for R in SPEAKER_WIDTHS])            # E = 33: a tail tile of one column
 def test_device_equals_the_oracle(R, R_live, E):
     fea, Phi, offs, labels, efea, espk = _ragged(R + E, R, R_live, E)
     table, n0, F0, ne0, Fe0, L0, rec_off = _oracle(fea, Phi, offs, labels, efea, espk)
@@ -97,11 +99,9 @@ def test_device_equals_the_oracle(R, R_live, E):
             assert not named.any()
 
 
-@pytest.mark.gpu
-def test_llr_is_bit_identical_to_vbx_link():
+def _llr_is_minus_link(fea, Phi, offs, labels, efea, espk):
     """The enrolled speakers appended to the archive as one-speaker recordings: vbx_link's distances between archive and
-    enrolled speakers are exactly -llr."""
-    fea, Phi, offs, labels, efea, espk = _ragged(5, 16, 13, 9)
+    enrolled speakers are exactly -llr.  Returns the enrolment result."""
     res = enroll.enroll_speakers(fea, Phi, offs, labels, efea, espk, 0.3, 17.0, 0.0, llr=True)
     cnt = np.bincount(espk)
     ext_labels = labels + [np.zeros(k, dtype=np.int64) for k in cnt]
@@ -110,6 +110,58 @@ def test_llr_is_bit_identical_to_vbx_link():
     M = len(res.table.rec)
     assert len(table.rec) == M + len(cnt)
     assert np.array_equal(res.llr, -D[:M, M:])
+    return res
+
+
+@pytest.mark.gpu
+def test_llr_is_bit_identical_to_vbx_link():
+    _llr_is_minus_link(*_ragged(5, 16, 13, 9))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('R', SPEAKER_WIDTHS)
+def test_llr_is_bit_identical_to_vbx_link_and_the_cohort_scores(R):
+    """At every width: enrolment llr = -link distance, and the enrolled speakers taken as a cohort score exactly llr."""
+    fea, Phi, offs, labels, efea, espk = _ragged(R, R, R, 9)
+    res = _llr_is_minus_link(fea, Phi, offs, labels, efea, espk)
+    st = cohort.cohort_stats(fea, Phi, offs, labels, efea, espk, 0.3, 17.0, top_k=2, scores=True)
+    assert np.array_equal(st.scores, res.llr)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('E', [31, 32, 33])
+@pytest.mark.parametrize('M', [32, 33, 64, 65])
+def test_tile_edges_at_width_100(M, E):
+    """R = 100 (a partial last chunk that ends in a partial log group) at the 32-speaker tile edges: an archive of
+    exactly M speakers (M - 24 of them in one recording) linked, enrolled against E speakers and scored against them as
+    a cohort of C = E, each against the oracle."""
+    R = 100
+    fea, Phi, offs, labels, efea, espk = _ragged(100 * M + E, R, R, E, counts=(3, 0, M - 24, 1, 17, 0, 2, 1))
+    table, n0, F0, ne0, Fe0, L0, rec_off = _oracle(fea, Phi, offs, labels, efea, espk)
+    assert len(table.rec) == M and len(ne0) == E
+    t, n, F, Z, D = link.link_speakers(fea, Phi, offs, labels, 0.3, 17.0, dist=True)
+    assert np.array_equal(n, n0)
+    np.testing.assert_allclose(F, F0, rtol=1e-12, atol=1e-12 * np.abs(F0).max())
+    D0 = link_oracle.distances(n0, F0, Phi, C, table.rec)
+    big = D0 == link.BIG
+    assert np.array_equal(D == link.BIG, big) and np.array_equal(D, D.T)
+    scale = np.abs(D0[~big]).max()
+    np.testing.assert_allclose(D[~big], D0[~big], rtol=1e-12, atol=1e-12 * scale)
+    Zs = link_oracle.link(D0)
+    low = Zs[:, 2] < 1e15
+    assert np.array_equal(Z[:, 2] < 1e15, low)
+    np.testing.assert_allclose(Z[low], Zs[low], rtol=1e-12, atol=1e-12 * scale)
+    scale = np.abs(L0).max()
+    for th in THRESHOLDS:
+        res = enroll.enroll_speakers(fea, Phi, offs, labels, efea, espk, 0.3, 17.0, th, llr=True)
+        np.testing.assert_allclose(res.llr, L0, rtol=1e-12, atol=1e-12 * scale)
+        want, obj = enroll_oracle.assign(L0, rec_off, th)
+        assert np.array_equal(res.assign, want), th
+    st = cohort.cohort_stats(fea, Phi, offs, labels, efea, espk, 0.3, 17.0, top_k=17, scores=True)
+    np.testing.assert_allclose(st.scores, L0, rtol=1e-12, atol=1e-12 * scale)
+    mu0, sd0 = norm_oracle.top_stats(L0, 17)
+    np.testing.assert_allclose(st.mean, mu0, rtol=1e-12, atol=1e-12 * scale)
+    np.testing.assert_allclose(st.std, sd0, rtol=1e-12, atol=1e-12 * scale)
 
 
 @pytest.mark.gpu

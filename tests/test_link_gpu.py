@@ -15,11 +15,23 @@ from vbx_b200 import link, pipeline, score
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden')
 C = 0.3 / 17
+# Feature widths of the speaker-pair scores (score_tile, enroll_score_kernel and verify_score_kernel stage 32-feature
+# chunks and take one log per group of 8 denominators): a single partial group (1, 3, 7), one group and one feature
+# (9), whole groups inside a chunk (24), both sides of the 32-, 64- and 96-feature chunk edges, and a partial last chunk
+# that ends in a partial group (100, 127).  Every feature is live (width_phi).
+SPEAKER_WIDTHS = [1, 3, 7, 9, 24, 31, 33, 40, 63, 65, 96, 100, 127]
+
+
+def width_phi(rng, R):
+    """Phi [R] of a SPEAKER_WIDTHS case: every feature live, log-uniform over four decades (1e-2 .. 1e2), descending, so
+    that every feature's term shows in the LLR at 1e-12."""
+    return np.sort(10.0 ** rng.uniform(-2.0, 2.0, R))[::-1].astype(np.float32)
 
 
 def _ragged(seed, R, R_live):
     """A seeded archive: recordings without x-vectors, 1 .. 128 speakers per recording with gaps in the label values, a
-    speaker with one x-vector, features drawn around a pool of centres; features >= R_live padded with zeros."""
+    speaker with one x-vector, features drawn around a pool of centres; features >= R_live padded with zeros, Phi from
+    width_phi at the SPEAKER_WIDTHS."""
     rng = np.random.default_rng(seed)
     centres = rng.standard_normal((40, R_live)) * 2.0
     counts = [3, 0, 128, 1, 17, 0, 2, 40]
@@ -41,7 +53,7 @@ def _ragged(seed, R, R_live):
         f[:, :R_live] = who[np.searchsorted(vals, lab)] + rng.standard_normal((len(lab), R_live))
         feas.append(f)
     Phi = np.zeros(R, dtype=np.float32)
-    Phi[:R_live] = np.sort(rng.uniform(0.2, 6.0, R_live))[::-1]
+    Phi[:R_live] = width_phi(rng, R) if R in SPEAKER_WIDTHS else np.sort(rng.uniform(0.2, 6.0, R_live))[::-1]
     offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
     return np.concatenate(feas), Phi, offs, labels
 
@@ -64,8 +76,9 @@ def _partition(table, maps):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('R,R_live', [(128, 128), (16, 13), (8, 1)])
-@pytest.mark.parametrize('seed', [0, 1])
+@pytest.mark.parametrize('seed,R,R_live', [(seed, R, R_live) for seed in (0, 1)
+                                            for R, R_live in ((128, 128), (16, 13), (8, 1))]
+                         + [(R, R, R) for R in SPEAKER_WIDTHS])
 def test_device_equals_the_oracle(R, R_live, seed):
     fea, Phi, offs, labels = _ragged(seed, R, R_live)
     table, n, F, Z, D = link.link_speakers(torch.from_numpy(fea).cuda(), torch.from_numpy(Phi).cuda(), offs, labels,
@@ -131,6 +144,66 @@ def test_bit_identical_and_permutation_invariant():
         pc = _partition(c[0], link.link_cut(c[3], c[0], t))
         assert sorted(sorted((b, l) for b, l in g) for g in pa) == \
             sorted(sorted((perm[b], l) for b, l in g) for g in pc), t
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('R', [100, 128])
+@pytest.mark.parametrize('c', [1e30, 1e36, 1e40])
+def test_large_c_does_not_overflow_the_log_groups(R, c):
+    """Fa = 1, Fb = 1 / c: any finite positive Fa and Fb are accepted, and from c of about 1e36 on a product of 8
+    denominators 1 + c (n_i + n_j) Phi_r exceeds DBL_MAX although each is below 1e44.  Zero features make every b 0, so
+    an LLR is its log part alone (no cancellation in the oracle either).  The link distances, enrolment, cohort and
+    verification LLRs equal the oracle to 1e-12 of the sum of their |log| terms, and are one another bit for bit."""
+    from oracle import verify_oracle
+    from vbx_b200 import cohort, enroll, verify
+    Fa, Fb = 1.0, 1.0 / c
+    cc = Fa / Fb                                              # the c of the kernels
+    rng = np.random.default_rng(R + int(np.log10(c)))
+    Phi = np.sort(10.0 ** rng.uniform(np.log10(0.5), np.log10(40.0), R))[::-1].astype(np.float32)
+    n_a = [1, 50, 3, 17, 50, 8, 2, 40, 5, 50, 11, 29]         # two speakers per recording
+    labels = [np.repeat([0, 1], n_a[k:k + 2]) for k in range(0, len(n_a), 2)]
+    offs = np.concatenate([[0], np.cumsum([len(l) for l in labels])]).astype(np.int64)
+    fea = np.zeros((int(offs[-1]), R), dtype=np.float32)
+    n_e = [1, 50, 4, 30, 2, 50, 9, 15, 50]
+    espk = np.repeat(np.arange(len(n_e)), n_e)
+    efea = np.zeros((len(espk), R), dtype=np.float32)
+    M, E = len(n_a), len(n_e)
+    # the oracle over the archive's speakers and then the enrolled ones
+    n = np.array(n_a + n_e, dtype=np.float64)
+    L0 = link_oracle.llr(n, np.zeros((M + E, R)), Phi, cc)
+    ph = Phi.astype(np.float64)
+    logs = np.log(1.0 + cc * n[:, None] * ph[None, :]).sum(1)
+    pair = np.array([[np.log(1.0 + cc * (a + b) * ph).sum() for b in n] for a in n])
+    scale = pair + logs[:, None] + logs[None, :]              # sum over r of |log L_su| + |log L_s| + |log L_u|
+    groups = np.log(1.0 + cc * (n[:, None, None] + n[None, :, None]) * ph[None, None, :])
+    groups = np.add.reduceat(groups, np.arange(0, R, 8), axis=2)
+    assert ((groups > np.log(np.finfo(np.float64).max)).any()) == (c > 1e33)   # the edge is reached from 1e36 on
+    assert np.isfinite(L0).all() and (1.0 + cc * 100 * ph.max()) < 1e300
+
+    def check(got, want, sc):
+        assert np.isfinite(got).all()
+        assert (np.abs(got - want) <= 1e-12 * np.abs(want) + 1e-12 * sc).all(), np.abs(got - want).max()
+
+    table, nd, _, _, D = link.link_speakers(fea, Phi, offs, labels, Fa, Fb, dist=True)
+    assert np.array_equal(nd, n[:M])
+    cross = table.rec[:, None] != table.rec[None, :]
+    assert np.array_equal(D == link.BIG, ~cross & ~np.eye(M, dtype=bool))
+    check(D[cross], -L0[:M, :M][cross], scale[:M, :M][cross])
+    res = enroll.enroll_speakers(fea, Phi, offs, labels, efea, espk, Fa, Fb, 0.0, llr=True)
+    check(res.llr, L0[:M, M:], scale[:M, M:])
+    st = cohort.cohort_stats(fea, Phi, offs, labels, efea, espk, Fa, Fb, top_k=2, scores=True)
+    spk, _ = link.speaker_index(offs, labels)
+    ii, jj = np.meshgrid(np.arange(M), np.arange(E), indexing='ij')
+    tr = np.stack([ii.ravel(), jj.ravel()], 1)
+    v = verify.score_trials(fea, spk, efea, espk, Phi, tr, Fa=Fa, Fb=Fb)
+    ne_v, Fe_v = verify_oracle.statistics(fea, spk, M)
+    nt_v, Ft_v = verify_oracle.statistics(efea, espk, E)
+    check(v, verify_oracle.llr_trials(ne_v, Fe_v, nt_v, Ft_v, ph, cc, tr[:, 0], tr[:, 1]), scale[:M, M:].ravel())
+    # the chain: verify = cohort = enrol = -link (the enrolled speakers appended as one-speaker recordings)
+    ext = labels + [np.zeros(k, dtype=np.int64) for k in n_e]
+    ext_offs = np.concatenate([offs, offs[-1] + np.cumsum(n_e)])
+    D2 = link.link_speakers(np.concatenate([fea, efea]), Phi, ext_offs, ext, Fa, Fb, dist=True)[4]
+    assert v.tobytes() == st.scores.tobytes() == res.llr.tobytes() == (-D2[:M, M:]).tobytes()
 
 
 def test_too_many_speakers_is_a_value_error(monkeypatch):

@@ -13,6 +13,7 @@ import pytest
 import torch
 
 from oracle import enroll_oracle
+from test_link_gpu import SPEAKER_WIDTHS, width_phi
 from vbx_b200 import _lib, cohort, enroll, formats, link, pipeline, score, sweep, synth
 
 pytestmark = pytest.mark.gpu
@@ -24,9 +25,10 @@ THETAS = [-1e6, -50.0, 0.0, 20.0, 1e6]
 def _archive(seed, R, E, counts=((3, 0, 150, 1, 17, 0, 2), (0, 0, 0, 0, 0, 0, 0), (5, 2, 0, 40, 1, 1, 9), (1,) * 7)):
     """Seeded features of 7 recordings (one without x-vectors) and one problem per entry of counts (speakers per
     recording; a problem without speakers, a recording with 150), label values with gaps and x-vectors without a
-    speaker; E enrolled speakers around the same centres, enrolled speakers 0 and 1 with identical x-vectors."""
+    speaker; E enrolled speakers around the same centres, enrolled speakers 0 and 1 with identical x-vectors.  The last
+    3 features are padded, except at the SPEAKER_WIDTHS: there every feature is live, with Phi from width_phi."""
     rng = np.random.default_rng(seed)
-    R_live = max(R - 3, 1)
+    R_live = R if R in SPEAKER_WIDTHS else max(R - 3, 1)
     centres = rng.standard_normal((40, R_live)) * 2.0
     lens = [max(2 * k, 6) if k else 0 for k in np.max(np.array(counts), 0)]
     lens[5] = 0
@@ -35,7 +37,7 @@ def _archive(seed, R, E, counts=((3, 0, 150, 1, 17, 0, 2), (0, 0, 0, 0, 0, 0, 0)
     fea = np.zeros((N, R), np.float32)
     fea[:, :R_live] = centres[rng.integers(0, 40, N)] + rng.standard_normal((N, R_live))
     Phi = np.zeros(R, np.float32)
-    Phi[:R_live] = np.sort(rng.uniform(0.2, 6.0, R_live))[::-1]
+    Phi[:R_live] = width_phi(rng, R) if R in SPEAKER_WIDTHS else np.sort(rng.uniform(0.2, 6.0, R_live))[::-1]
     problems = []
     for ks in counts:
         labels = []
@@ -111,7 +113,7 @@ def _norms(fea, Phi, offs, problems, efea, espk, Fa, Fb, rng):
     return out, cfea, cspk
 
 
-@pytest.mark.parametrize('R, E', [(8, 1), (16, 7), (128, 300), (16, 300), (128, 7)])
+@pytest.mark.parametrize('R, E', [(8, 1), (16, 7), (128, 300), (16, 300), (128, 7)] + [(R, 33) for R in SPEAKER_WIDTHS])
 @pytest.mark.parametrize('normalised', [False, True])
 def test_enroll_many_is_enroll_speakers_problem_by_problem(R, E, normalised):
     fea, Phi, offs, problems, efea, espk, Fa, Fb = _archive(R * 1000 + E, R, E)

@@ -11,6 +11,7 @@ import pytest
 import torch
 
 from oracle import link_oracle
+from test_link_gpu import SPEAKER_WIDTHS, width_phi
 from vbx_b200 import _lib, formats, link, pipeline, score, sweep, synth
 
 pytestmark = pytest.mark.gpu
@@ -20,13 +21,15 @@ MS = [0, 1, 2, 33, 128, 700]
 
 
 def _problems(seed, R):
-    """One archive of 20 recordings and a problem per M in MS, each with its own labels (value gaps, -1 entries)."""
+    """One archive of 20 recordings and a problem per M in MS, each with its own labels (value gaps, -1 entries); Phi
+    from width_phi at the SPEAKER_WIDTHS."""
     rng = np.random.default_rng(seed)
     lens = rng.integers(40, 80, 20)
     lens[3] = 0
     centres = rng.standard_normal((60, R)) * 2.0
     fea = (centres[rng.integers(0, 60, int(lens.sum()))] + rng.standard_normal((int(lens.sum()), R))).astype(np.float32)
-    Phi = np.sort(rng.uniform(0.2, 6.0, R))[::-1].astype(np.float32).copy()
+    Phi = (width_phi(rng, R) if R in SPEAKER_WIDTHS
+           else np.sort(rng.uniform(0.2, 6.0, R))[::-1].astype(np.float32).copy())
     offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
     problems = []
     for M in MS:
@@ -59,7 +62,7 @@ def _partition(table, maps):
     return sorted(map(sorted, g.values()))
 
 
-@pytest.mark.parametrize('R', [8, 16, 128])
+@pytest.mark.parametrize('R', [8, 16, 128] + SPEAKER_WIDTHS)
 def test_link_many_is_link_speakers_problem_by_problem(R):
     fea, Phi, offs, problems, Fa, Fb = _problems(R, R)
     fea_d, Phi_d = torch.from_numpy(fea).to(DEV), torch.from_numpy(Phi).to(DEV)

@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from oracle import verify_oracle as O
+from test_link_gpu import SPEAKER_WIDTHS, width_phi
 from vbx_b200 import _lib, cohort, formats, pipeline, train, verify
 
 DEV = 'cuda:0'
@@ -27,8 +28,9 @@ def side(M, R, Phi, rng, multi, centres=None):
 
 
 def problem(R, multi, seed, M_e=40, M_t=60, T=2500):
+    """Seeded sides and trials; Phi from width_phi at the SPEAKER_WIDTHS."""
     rng = np.random.default_rng(seed)
-    Phi = np.sort(rng.uniform(0.2, 8.0, R))[::-1].astype(np.float32)
+    Phi = width_phi(rng, R) if R in SPEAKER_WIDTHS else np.sort(rng.uniform(0.2, 8.0, R))[::-1].astype(np.float32)
     fe, ie = side(M_e, R, Phi, rng, multi)
     ft, it = side(M_t, R, Phi, rng, multi)
     tr = np.stack([rng.integers(0, M_e, T), rng.integers(0, M_t, T)], 1)
@@ -48,7 +50,7 @@ def close(got, want, tol=1e-12):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('R', [8, 16, 128])
+@pytest.mark.parametrize('R', [8, 16, 128] + SPEAKER_WIDTHS)
 @pytest.mark.parametrize('c', [1.0, 0.3 / 17])
 @pytest.mark.parametrize('multi', [False, True])
 def test_scores_match_the_oracle(R, c, multi):
@@ -59,7 +61,8 @@ def test_scores_match_the_oracle(R, c, multi):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('R, multi', [(16, True), (128, False), (128, True)])
+@pytest.mark.parametrize('R, multi', [(16, True), (128, False), (128, True)]
+                         + [(R, k % 2 == 0) for k, R in enumerate(SPEAKER_WIDTHS)])
 def test_scores_are_the_cohort_scores_bit_for_bit(R, multi):
     Fa, Fb = 0.3, 17.0
     fe, ie, ft, it, Phi, _ = problem(R, multi, 7 * R)
@@ -74,11 +77,12 @@ def test_scores_are_the_cohort_scores_bit_for_bit(R, multi):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('multi', [False, True])
-def test_as_norm_matches_the_oracle(multi):
-    fe, ie, ft, it, Phi, tr = problem(128, multi, 31)
+@pytest.mark.parametrize('R, multi', [pytest.param(128, m, id=str(m)) for m in (False, True)]
+                         + [(R, k % 2 == 1) for k, R in enumerate(SPEAKER_WIDTHS)])
+def test_as_norm_matches_the_oracle(R, multi):
+    fe, ie, ft, it, Phi, tr = problem(R, multi, 31 if R == 128 else R)
     rng = np.random.default_rng(5)
-    fc, ic = side(300, 128, Phi, rng, True)
+    fc, ic = side(300, R, Phi, rng, True)
     norm = verify.trial_norm(fe, ie, ft, it, Phi, fc, ic, 0.3, 17.0, top_k=50, device=DEV)
     got = verify.score_trials(fe, ie, ft, it, Phi, tr, Fa=0.3, Fb=17.0, norm=norm, device=DEV)
     want = O.as_norm(oracle_llr(fe, ie, ft, it, Phi, tr, 0.3 / 17.0), *norm, tr[:, 0], tr[:, 1])
@@ -303,4 +307,16 @@ def test_command_line_takes_trains_output(tmp_path):
                         os.path.join(mdir, 'transform.npz'), '--plda-file', os.path.join(mdir, 'plda'), '--lda-dim',
                         str(d), '--device', DEV, '--scores-out', out]) == 0
     v = np.array([float(l.split()[2]) for l in open(out)])
-    assert len(v) == 10 * (len(e_names) - 10) and np.isfinite(v).all()
+    assert len(v) == 10 * (len(e_names) - 10)
+    # the float64 oracle on the trained model's projection of the same x-vectors (both sides read from one ark)
+    names, x, item = verify.read_items(e_ark)
+    transform = formats.read_xvec_transform(os.path.join(mdir, 'transform.npz'))
+    pl = formats.read_kaldi_plda(os.path.join(mdir, 'plda'))
+    x_all = np.concatenate([x, x])
+    chain = pipeline._resolve_chain('auto', transform, pl, d, Dx)
+    front, _, fea, Phi = pipeline._project(x_all, [len(x_all)], transform, pl, d, chain, torch.device(DEV))
+    front.close()
+    fea, Phi = fea.cpu().numpy(), Phi.cpu().numpy()
+    assert fea.shape == (2 * len(x), d)
+    tr = np.array([[names.index(a), names.index(b)] for a in e_names[:10] for b in e_names[10:]])
+    close(v, oracle_llr(fea[:len(x)], item, fea[len(x):], item, Phi, tr, 1.0))

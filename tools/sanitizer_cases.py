@@ -3,7 +3,8 @@ D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings w
 6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels (also under a speaker-count bound),
 the dense forward_backward(), the ELBO trace, DER / JER scoring, speaker linking across recordings (one problem and
 batched), enrolment
-against known speakers and score normalisation against a cohort (one problem and batched).
+against known speakers and score normalisation against a cohort (one problem and batched, and at R = 100), and
+verification trials with AS-norm and the error rates.
 
     compute-sanitizer --tool memcheck --error-exitcode 3 python tools/sanitizer_cases.py
 """
@@ -155,6 +156,34 @@ for eb_norm in (None, [a[:2] + b[:2] for a, b in zip(eb_st, eb_en)]):
 eb_link = link.link_many(e_fea, l_phi, e_offs, eb_labels, eb_fa, eb_fb, dev, dist=True, norm=[a[:2] for a in eb_st])
 torch.cuda.synchronize()
 print('cohort batch ok', float(eb_st[2].std.min()), float(eb_en[2].std.min()), float(eb_link[2][3][:, 2].min()))
+
+# the speaker-pair scores at R = 100 (a partial last chunk ending in a partial log group): linking, enrolment with
+# E = 33 and cohort statistics with C = 33 (tail tiles), the speakers of the archive above
+w_fea = torch.randn((sum(e_lens), 100), device=dev)
+w_phi = torch.rand(100, device=dev) + 0.01
+w_offs = np.concatenate([[0], np.cumsum(e_lens)])
+w_x = torch.randn((70, 100), device=dev)
+w_spk = np.concatenate([np.arange(33), gl.integers(0, 33, 37)])
+w_link = link.link_speakers(w_fea, w_phi, w_offs, e_labels, 0.3, 17.0, dev, dist=True)
+w_enr = enroll.enroll_speakers(w_fea, w_phi, w_offs, e_labels, w_x, w_spk, 0.3, 17.0, 0.0, dev, llr=True)
+w_st = cohort.cohort_stats(w_fea, w_phi, w_offs, e_labels, w_x, w_spk, 0.3, 17.0, top_k=10, device=dev, scores=True)
+torch.cuda.synchronize()
+print('R=100 link, enroll, cohort ok', len(w_link[0].rec), int((w_enr.assign >= 0).sum()), float(w_st.std.min()))
+
+# verification trials (vbx_verify_score, vbx_verify_metrics): single and multi-x-vector items at R = 100, trials whose
+# count is not a multiple of 32 (a warp with idle lanes), AS-norm against a cohort, and the error rates with ties
+from vbx_b200 import verify  # noqa: E402
+v_e, v_t = w_x[:40].cpu().numpy(), w_fea[:500].cpu().numpy()
+v_ie, v_it = np.arange(40) % 17, gl.integers(0, 61, 500)
+v_it[:61] = np.arange(61)
+v_phi = w_phi.cpu().numpy()
+v_tr = np.stack([gl.integers(0, 17, 1001), gl.integers(0, 61, 1001)], 1)
+v_norm = verify.trial_norm(v_e, v_ie, v_t, v_it, v_phi, w_x.cpu().numpy(), w_spk, 0.3, 17.0, top_k=20, device=dev)
+v_s = verify.score_trials(v_e, v_ie, v_t, v_it, v_phi, v_tr, Fa=0.3, Fb=17.0, norm=v_norm, device=dev)
+v_y = v_tr[:, 0] == v_tr[:, 1] % 17
+v_m = verify.error_rates(np.round(v_s, 1), v_y, (0.01, 0.5), device=dev)
+torch.cuda.synchronize()
+print('verify ok', float(v_s.min()), v_m['eer'], v_m['cllr'])
 
 # wgmma projection at the smallest and largest D, one frame and one frame past a full wave of tiles
 sms = torch.cuda.get_device_properties(0).multi_processor_count

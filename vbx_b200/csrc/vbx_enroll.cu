@@ -15,6 +15,7 @@
 // With cohort statistics (section 5.17) vbx_cohort.cu's norm_scores_kernel turns llr into S in place between the two.
 // launch_cohort_scores_batch runs enroll_score_kernel against a cohort for vbx_cohort_stats_batch.
 #include <algorithm>
+#include <cfloat>
 #include <climits>
 #include <cstring>
 #include <vector>
@@ -25,13 +26,36 @@ namespace vbx {
 
 namespace {
 
-constexpr int kLogGroup = 8;                // as vbx_link: log of a product of 8 denominators
+constexpr int kLogGroup = 8;                // as vbx_link: log of a product of 8 denominators, overflowed_log_sum
 constexpr int64_t kScoreGrid = 1 << 20;     // CTAs of enroll_score_kernel at most; beyond that they stride over the tiles
 constexpr int kAssignThreads = 256;
 constexpr int kAssignWarps = kAssignThreads / 32;
 constexpr int kAssignCtasPerSm = 2;
 
 __host__ __device__ size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// As vbx_link: the log term sum_r log(fma(cm, Phi_r, 1)) of a pair whose sum of group logs came out +inf: some product of
+// kLogGroup denominators overflowed (each denominator is finite, but any finite positive Fa / Fb is accepted, so c can
+// be large).  The same groups in the same order, each multiply that would overflow first flushing the product so far
+// into the sum; a group that did not overflow gives the same log as in the scoring loop.  Out of line and reached only
+// from that case, so the loop's registers and instructions stay those of plain groups.
+__device__ __noinline__ double overflowed_log_sum(double cm, const float *__restrict__ Phi, int R) {
+    double lg = 0.0, prod = 1.0;
+    for (int r = 0; r < R; ++r) {
+        const double den = fma(cm, (double)Phi[r], 1.0), pd = prod * den;
+        if (pd > DBL_MAX) {
+            lg += log(prod);
+            prod = den;
+        } else {
+            prod = pd;
+        }
+        if ((r % kLogGroup) == kLogGroup - 1 || r == R - 1) {
+            lg += log(prod);
+            prod = 1.0;
+        }
+    }
+    return lg;
+}
 
 // one CTA's column and row state in the workspace: columns nc = E + K_b <= E + max_k, rows K_b <= max_k
 struct Slice {
@@ -160,6 +184,9 @@ __global__ void __launch_bounds__(256) enroll_score_kernel(SpeakerStats A0, Spea
             }
             __syncthreads();                          // also keeps the next tile's loads behind this tile's reads
         }
+#pragma unroll
+        for (int u = 0; u < 4; ++u)
+            if (lg[u] > DBL_MAX) lg[u] = overflowed_log_sum(cm[u], Phi, R);
         if (j >= E) continue;
         const double ej = En.e[j];
 #pragma unroll

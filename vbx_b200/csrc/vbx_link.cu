@@ -18,6 +18,7 @@
 // has one CTA per problem, so a problem's results do not depend on the others.  vbx_enroll_batch and
 // vbx_cohort_stats_batch take the statistics through launch_speaker_stats_batch.
 #include <algorithm>
+#include <cfloat>
 #include <climits>
 #include <cstring>
 
@@ -30,7 +31,7 @@ namespace {
 constexpr double kBig = 1.0e30;            // cannot-link distance: finite (scipy and the linkage stop at non-finite ones)
 constexpr int kStatsThreads = 256;
 constexpr int kStatsPhases = kStatsThreads / 32;   // x-vector t = first + k, first + k + 8, ... makes phase k
-constexpr int kLogGroup = 8;               // log of a product of 8 denominators: each is 1 + c n Phi, so no overflow
+constexpr int kLogGroup = 8;               // log of a product of 8 denominators (overflowed_log_sum where one overflows)
 constexpr int64_t kScoreGrid = 1 << 20;    // CTAs of link_score_kernel at most; beyond that they stride over the tiles
 
 struct LinkWs {
@@ -53,6 +54,29 @@ struct LinkProblems {
 };
 
 size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// The log term sum_r log(fma(cm, Phi_r, 1)) of a pair whose sum of group logs came out +inf: some product of
+// kLogGroup denominators overflowed (each denominator is finite, but any finite positive Fa / Fb is accepted, so c can
+// be large).  The same groups in the same order, each multiply that would overflow first flushing the product so far
+// into the sum; a group that did not overflow gives the same log as in the scoring loop.  Out of line and reached only
+// from that case, so the loop's registers and instructions stay those of plain groups.
+__device__ __noinline__ double overflowed_log_sum(double cm, const float *__restrict__ Phi, int R) {
+    double lg = 0.0, prod = 1.0;
+    for (int r = 0; r < R; ++r) {
+        const double den = fma(cm, (double)Phi[r], 1.0), pd = prod * den;
+        if (pd > DBL_MAX) {
+            lg += log(prod);
+            prod = den;
+        } else {
+            prod = pd;
+        }
+        if ((r % kLogGroup) == kLogGroup - 1 || r == R - 1) {
+            lg += log(prod);
+            prod = 1.0;
+        }
+    }
+    return lg;
+}
 
 size_t problem_array_bytes(int64_t G) { return (size_t)(5 * G + 4) * 8; }   // off, lk_off, tile_off, dist_off, c
 
@@ -207,6 +231,9 @@ __device__ __forceinline__ void score_tile(const LinkWs &w, const float *__restr
         }
         __syncthreads();
     }
+#pragma unroll
+    for (int u = 0; u < 4; ++u)
+        if (lg[u] > DBL_MAX) lg[u] = overflowed_log_sum(cm[u], Phi, R);
     double *D = reinterpret_cast<double *>(w.lk);
     const int rj = j < M ? spk_rec[j] : -1;
     const double ej = j < M ? w.e[j] : 0.0;

@@ -26,6 +26,7 @@
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
+#include <cfloat>
 #include <cmath>
 #include <cstring>
 #include <vector>
@@ -36,7 +37,7 @@ namespace vbx {
 
 namespace {
 
-constexpr int kLogGroup = 8;                // as vbx_link: log of a product of 8 denominators
+constexpr int kLogGroup = 8;                // as vbx_link: log of a product of 8 denominators, overflowed_log_sum
 constexpr int kScoreWarps = 2;              // warps per CTA of verify_score_kernel (33.8 KB of staging)
 constexpr int64_t kScoreGrid = 1 << 20;     // CTAs of verify_score_kernel at most; beyond that they stride
 constexpr int kSweepThreads = 256;
@@ -45,6 +46,29 @@ constexpr int kCllrThreads = 256;
 constexpr int kCllrCtas = 256;              // the fixed partition of the Cllr sums
 
 __host__ __device__ size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// As vbx_link: the log term sum_r log(fma(cm, Phi_r, 1)) of a pair whose sum of group logs came out +inf: some product of
+// kLogGroup denominators overflowed (each denominator is finite, but any finite positive Fa / Fb is accepted, so c can
+// be large).  The same groups in the same order, each multiply that would overflow first flushing the product so far
+// into the sum; a group that did not overflow gives the same log as in the scoring loop.  Out of line and reached only
+// from that case, so the loop's registers and instructions stay those of plain groups.
+__device__ __noinline__ double overflowed_log_sum(double cm, const float *__restrict__ Phi, int R) {
+    double lg = 0.0, prod = 1.0;
+    for (int r = 0; r < R; ++r) {
+        const double den = fma(cm, (double)Phi[r], 1.0), pd = prod * den;
+        if (pd > DBL_MAX) {
+            lg += log(prod);
+            prod = den;
+        } else {
+            prod = pd;
+        }
+        if ((r % kLogGroup) == kLogGroup - 1 || r == R - 1) {
+            lg += log(prod);
+            prod = 1.0;
+        }
+    }
+    return lg;
+}
 
 // ---------------------------------------------------------------------------------------------------------------- scores
 
@@ -67,8 +91,8 @@ VerifyScoreWs score_layout(uint8_t *ws, int64_t M_e, int64_t M_t, size_t *total)
 // Warp w of the grid takes trials 32 w .. 32 w + 31, lane l trial 32 w + l.  Per chunk of 32 features the warp loads
 // the b rows of its 32 enrolment and 32 test items (row v: lane = feature, 256 contiguous bytes) into its own shared
 // tiles, then each lane runs over the chunk for its trial with score_tile's operations: den = fma(cm, Phi_r, 1),
-// x = b_i + b_j, q += x x / den, prod *= den and lg += log(prod) after every kLogGroup features and the last.  A trial
-// whose index lies outside its side loads nothing and writes NaN.
+// x = b_i + b_j, q += x x / den, prod *= den and lg += log(prod) after every kLogGroup features and the last (an lg of
+// +inf recomputed by overflowed_log_sum).  A trial whose index lies outside its side loads nothing and writes NaN.
 __global__ void __launch_bounds__(kScoreWarps * 32) verify_score_kernel(
     SpeakerStats En, SpeakerStats Te, int64_t M_e, int64_t M_t, const float *__restrict__ Phi, int R, double c,
     const int32_t *__restrict__ ti, const int32_t *__restrict__ tj, int64_t T, const double *__restrict__ mean_e,
@@ -107,6 +131,7 @@ __global__ void __launch_bounds__(kScoreWarps * 32) verify_score_kernel(
             }
             __syncwarp();                             // the next chunk rewrites the tiles
         }
+        if (lg > DBL_MAX) lg = overflowed_log_sum(cm, Phi, R);
         if (t >= T) continue;
         double s = NAN;
         if (ok) {
