@@ -387,6 +387,25 @@ int vbx_verify_metrics(vbx_handle_t h, const double *scores, const uint8_t *is_t
                        int64_t *counts_out, double *eer_out, double *cllr_out, double *min_dcf_out,
                        double *threshold_out, double *act_dcf_out, void *stream);
 
+/* vbx_verify_calibrate (DESIGN.md section 5.28): the linear calibration llr = a s + b of T >= 1 scores [T] (DEVICE
+ * float64) with is_target [T] (DEVICE uint8, nonzero = target trial) at the prior in (0, 1): (a, b) minimise the
+ * prior-weighted logistic cost
+ *   C(a, b) = prior / N_tar sum_tar softplus(-z) + (1 - prior) / N_non sum_non softplus(z),  z = a s + b + logit(prior),
+ * by Newton's method with step halving from (0, 0) on the device (at most 64 passes; once the predicted decrease is
+ * <= 2^-52 C one last full step is taken and the fit ends), and min_cllr is the Cllr of the optimal monotone (PAV) transform of the scores at prior 1/2, from the
+ * upper hull of the ROC points of the distinct scores (exact integer arithmetic).  Outputs (DEVICE):
+ *   info_out [5] int64    status (0 fitted, 1 separable classes or a missing class: no finite minimiser, the fit is not
+ *                         run, 2 non-finite scores, 3 the pass limit reached), passes, N_tar, N_non, hull vertices
+ *   out [4] float64       a, b, cllr_prior = C(a, b) / ln 2 (NaN for status 1 and 2), min_cllr (NaN for status 2)
+ * Every sum runs in an order fixed by the sorted scores, so a call is bit-identical from run to run and for any order of
+ * the trials.  Stream ordered, no allocation, no host synchronisation; a fixed number of launches.  workspace:
+ * vbx_verify_calibrate_workspace_bytes(T) bytes (the sort's temporary storage included; sized for the handle's device),
+ * 256-byte aligned: about 42 T bytes plus the sort's.  VBX_ERR_ARG: T < 1, a prior outside (0, 1), null pointers, a
+ * misaligned or short workspace. */
+int vbx_verify_calibrate_workspace_bytes(vbx_handle_t h, int64_t T, size_t *bytes_out);
+int vbx_verify_calibrate(vbx_handle_t h, const double *scores, const uint8_t *is_target, int64_t T, double prior,
+                         void *workspace, size_t workspace_bytes, int64_t *info_out, double *out, void *stream);
+
 /* Float64 evaluation of the same EM loop ("exact" mode for the one-recording-per-call use of VBx/vbhmm.py:154-158,
  * where the reference stops on an ELBO improvement < 1e-6, VBx/vbhmm.py:157 -- below float32 resolution).
  * All arrays float64: fea [N,R] (the reference's X, VBx/VBx.py:30), Phi [R], gamma_io [N,S], pi_io [n_rec,S],

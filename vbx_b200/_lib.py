@@ -18,7 +18,8 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_cohort_stats_batch', 'vbx_init_turns', 'vbx_combine_workspace_bytes', 'vbx_combine',
            'vbx_init_random', 'vbx_run_prior', 'vbx_run_f64_prior', 'vbx_class_scatter_workspace_bytes',
            'vbx_class_scatter', 'vbx_stream_window', 'vbx_stream_commit', 'vbx_verify_score_workspace_bytes',
-           'vbx_verify_score', 'vbx_verify_metrics_workspace_bytes', 'vbx_verify_metrics']
+           'vbx_verify_score', 'vbx_verify_metrics_workspace_bytes', 'vbx_verify_metrics',
+           'vbx_verify_calibrate_workspace_bytes', 'vbx_verify_calibrate']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
@@ -152,6 +153,10 @@ def load():
     lib.vbx_verify_metrics.restype = ctypes.c_int
     lib.vbx_verify_metrics.argtypes = [vp, vp, vp, i64, i32, vp, dbl, dbl, vp, ctypes.c_size_t, vp, vp, vp, vp, vp, vp,
                                        vp]
+    lib.vbx_verify_calibrate_workspace_bytes.restype = ctypes.c_int
+    lib.vbx_verify_calibrate_workspace_bytes.argtypes = [vp, i64, ctypes.POINTER(ctypes.c_size_t)]
+    lib.vbx_verify_calibrate.restype = ctypes.c_int
+    lib.vbx_verify_calibrate.argtypes = [vp, vp, vp, i64, dbl, vp, ctypes.c_size_t, vp, vp, vp]
     lib.vbx_get_timings.restype = ctypes.c_int
     lib.vbx_get_timings.argtypes = [vp, ctypes.POINTER(dbl), ctypes.POINTER(i64), i32]
     _lib = lib

@@ -32,6 +32,11 @@ linking and enrolment scores are normalised against the cohort speakers of the a
 known to be none of the archive's: each score is standardised by the mean and spread of both speakers' --cohort-top
 (default 200) largest cohort scores, and --link-threshold and --enroll-threshold are on that normalised score.
 
+With --calibration FILE (a file of python -m vbx_b200.verify --calibrate-out, fitted with this run's model files, Fa,
+Fb, --lda-dim and cohort; DESIGN.md section 5.28) --link-threshold and --enroll-threshold are calibrated LLRs, and
+--enroll-threshold may be omitted (default 0: likelihood ratio >= 1).  They are mapped to raw thresholds (t - b) / a
+before diarizing, which decides exactly as thresholding a s + b.  Not with --adapt.
+
 With --init RTTM+VB --init-rttm PATH (an RTTM file or directory holding every recording of the archive) the VB-HMM
 resegments an existing diarization instead of starting from AHC (DESIGN.md section 5.20): one state per speaker of the
 RTTM, each x-vector started from the speakers' shares of its segment.  The written RTTMs keep the input's speaker names
@@ -187,7 +192,9 @@ def build_parser():
     ap.add_argument('--enroll-ark', default=None, help='x-vectors of known speakers (Kaldi ark) to name speakers by')
     ap.add_argument('--enroll-utt2spk', default=None, help='the speaker of each x-vector of --enroll-ark (utt2spk)')
     ap.add_argument('--enroll-threshold', default=None, type=float,
-                    help='least log-likelihood ratio at which a speaker takes an enrolled name')
+                    help='least log-likelihood ratio at which a speaker takes an enrolled name (with --calibration a '
+                         'calibrated LLR, default 0: likelihood ratio >= 1; for a prior P of an enrolled match, '
+                         'log((1 - P) / P))')
     ap.add_argument('--enroll-prior', action='store_true',
                     help='with the enrolment options and --init AHC+VB: AHC clusters assigned to enrolled speakers start '
                          'the VB-HMM from those speakers\' x-vectors as their speaker prior')
@@ -199,16 +206,47 @@ def build_parser():
                     help='how many of each speaker\'s largest cohort scores set its mean and spread (default 200)')
     ap.add_argument('--init-rttm', default=None,
                     help='with --init RTTM+VB: the diarization (RTTM file or directory of *.rttm) the VB-HMM starts from')
+    ap.add_argument('--calibration', default=None,
+                    help='a calibration file of python -m vbx_b200.verify --calibrate-out (DESIGN.md section 5.28): '
+                         '--link-threshold and --enroll-threshold are calibrated LLRs')
     add_random_options(ap)
     add_adapt_options(ap)
     return ap
+
+
+def calibrated_thresholds(ap, args):
+    """With --calibration: the raw --link-threshold and --enroll-threshold of the calibrated ones given (an omitted
+    --enroll-threshold is 0) by verify.raw_threshold.  The map a s + b is affine with a > 0, so average linkage,
+    the one-to-one enrolment assignment and AS-norm's S decide on a s + b >= t exactly as on s >= (t - b) / a.  Usage
+    errors (exit 2): no linking or enrolment, --adapt (the model changes at run time), a file that does not fit this
+    run's score kind (with or without a cohort), Fa, Fb, --lda-dim, --cohort-top or model files."""
+    from . import verify
+    if args.enroll_threshold is not None and args.enroll_ark is None:
+        ap.error('--enroll-threshold needs --enroll-ark and --enroll-utt2spk')
+    if args.link_threshold is None and args.enroll_ark is None:
+        ap.error('--calibration needs --link-threshold or the enrolment options')
+    if args.adapt:
+        ap.error('--calibration does not combine with --adapt: the adapted model is not the one it was fitted for')
+    try:
+        cal = verify.read_calibration(args.calibration)
+        why = verify.calibration_mismatch(cal, 'llr' if args.cohort_ark is None else 'as-norm', args.Fa, args.Fb,
+                                          args.lda_dim, 200 if args.cohort_top is None else args.cohort_top,
+                                          args.xvec_transform, args.plda_file)
+        if why is not None:
+            ap.error(f'--calibration: {why}')
+        link = None if args.link_threshold is None else verify.raw_threshold(cal, args.link_threshold)
+        enroll = None if args.enroll_ark is None else \
+            verify.raw_threshold(cal, 0.0 if args.enroll_threshold is None else args.enroll_threshold)
+    except (OSError, ValueError) as e:
+        ap.error(f'--calibration: {e}')
+    return link, enroll
 
 
 def main(argv=None):
     ap = build_parser()
     args = ap.parse_args(argv)
     assert 0 <= args.loopP <= 1, f'Expecting loopP between 0 and 1, got {args.loopP} instead.'     # VBx/vbhmm.py:103
-    enr = [args.enroll_ark, args.enroll_utt2spk, args.enroll_threshold]
+    enr = [args.enroll_ark, args.enroll_utt2spk] + ([args.enroll_threshold] if args.calibration is None else [])
     if any(v is not None for v in enr) and any(v is None for v in enr):
         ap.error('--enroll-ark, --enroll-utt2spk and --enroll-threshold go together')
     coh = [args.cohort_ark, args.cohort_utt2spk]
@@ -231,6 +269,8 @@ def main(argv=None):
         ap.error('--init RTTM+VB and --init-rttm go together')
     check_random_options(ap, args)
     scales = check_adapt_options(ap, args)
+    if args.calibration is not None:
+        args.link_threshold, args.enroll_threshold = calibrated_thresholds(ap, args)
     from . import formats
     from .pipeline import diarize_batch, linked_lines, named_lines
     from .score import read_overlaps

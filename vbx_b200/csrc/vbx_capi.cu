@@ -1213,6 +1213,36 @@ int vbx_verify_metrics(vbx_handle_t h, const double *scores, const uint8_t *is_t
                    "verify_metrics");
 }
 
+int vbx_verify_calibrate_workspace_bytes(vbx_handle_t h, int64_t T, size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    if (T < 1) return fail(h, VBX_ERR_ARG, "vbx_verify_calibrate_workspace_bytes: need T >= 1");
+    DeviceGuard guard(h->device);         // the sort's temporary storage is sized for the handle's device
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    *bytes_out = vbx::verify_calibrate_workspace_bytes(T);
+    return VBX_OK;
+}
+
+int vbx_verify_calibrate(vbx_handle_t h, const double *scores, const uint8_t *is_target, int64_t T, double prior,
+                         void *workspace, size_t workspace_bytes, int64_t *info_out, double *out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_verify_calibrate");
+    const std::string who("vbx_verify_calibrate");
+    if (T < 1) return fail(h, VBX_ERR_ARG, who + ": need T >= 1");
+    if (!(prior > 0.0 && prior < 1.0)) return fail(h, VBX_ERR_ARG, who + ": prior must lie in (0, 1)");
+    if (!std::isfinite(std::log(prior / (1.0 - prior))))
+        return fail(h, VBX_ERR_ARG, who + ": the log odds of prior are out of range");
+    if (!scores || !is_target || !workspace || !info_out || !out) return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
+        return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    if (workspace_bytes < vbx::verify_calibrate_workspace_bytes(T))
+        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_verify_calibrate_workspace_bytes()");
+    return counted(h, vbx::launch_verify_calibrate(scores, is_target, T, prior, workspace,
+                                                   reinterpret_cast<long long *>(info_out), out, (cudaStream_t)stream),
+                   "verify_calibrate");
+}
+
 int vbx_f64_workspace_bytes(vbx_handle_t h, size_t *bytes_out) {
     if (!h || !bytes_out) return VBX_ERR_ARG;
     if (!h->planned) return fail(h, VBX_ERR_STATE, "vbx_f64_workspace_bytes: call vbx_plan first");

@@ -438,6 +438,11 @@ size_t verify_metrics_workspace_bytes(int64_t T, int n_op);
 int launch_verify_metrics(const double *scores, const uint8_t *is_target, int64_t T, const double *ops_host, int n_op,
                           void *workspace, long long *counts_out, double *eer_out, double *cllr_out,
                           double *min_dcf_out, double *threshold_out, double *act_dcf_out, cudaStream_t st);
+// the calibration of a scored list (vbx_verify.cu, section 5.28): info_out [5] status, passes, N_tar, N_non, hull vertices;
+// out [4] a, b, cllr_prior, min_cllr (both DEVICE)
+size_t verify_calibrate_workspace_bytes(int64_t T);
+int launch_verify_calibrate(const double *scores, const uint8_t *is_target, int64_t T, double prior, void *workspace,
+                            long long *info_out, double *out, cudaStream_t st);
 // wgmma projection (vbx_project_tc.cu)
 size_t tc_scratch_floats();
 int launch_project_wgmma(const Plan &pl, float *tc_scratch, const float *X, int D, const float *V, const float *Phi, float *rho,

@@ -21,6 +21,18 @@
 //                         butterfly, warps in order)
 //   verify_final_kernel   one thread: the partials reduced, EER by linear interpolation, minDCF and its threshold, actDCF at
 //                         the Bayes threshold by binary search, Cllr
+// The calibration of a scored list (DESIGN.md section 5.28) starts from the same sort (sort_trials) and runs
+//   calibrate_split_kernel     the sorted scores by rank within their class (targets, then nontargets)
+//   calibrate_init_kernel      one thread: counts, the status (non-finite, separable), the Newton start (0, 0)
+//   calibrate_eval_kernel      the prior-weighted logistic cost, gradient and Hessian sums at the trial point on a fixed
+//                              grid (as verify_cllr_kernel)
+//   calibrate_update_kernel    the partials summed, then one thread: Newton with step halving; after convergence both kernels return at once, so
+//                              the host launches a fixed number of passes
+//   calibrate_hull_*_kernel    the upper ROC hull of the candidate thresholds: per-thread monotone chains of fixed chunks
+//                              of sorted positions, then log2(chunks) levels merging neighbouring chains (128-bit cross
+//                              products: exact)
+//   calibrate_segments_kernel  the minCllr terms of the hull segments on a fixed grid, in hull order
+//   calibrate_final_kernel     one thread: the outputs
 // Everything a call computes depends on the scores and labels alone (not on their order, the grid or earlier calls).
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -163,17 +175,23 @@ struct SweepPart {
     long long lo, hi;        // slot 1 + o: its lowest position; slot 0: last failing / first passing candidate
 };
 
-struct VerifyMetricsWs {
+// The sorted list both entry points start from: (key, label) pairs ascending, the targets before each sorted position and
+// the number of non-finite scores
+struct SortedTrials {
     unsigned long long *key_in, *key;
     uint8_t *lab_in, *lab;
     long long *tar;          // [T] targets before each sorted position
+    unsigned long long *nonfinite;
+    void *cub_tmp;
+    size_t cub_bytes;
+};
+
+struct VerifyMetricsWs {
+    SortedTrials p;
     double *terms;           // [T] Cllr terms: targets at their class rank, nontargets at N_tar + their class rank
     SweepPart *part;         // [(n_op + 1), kSweepGrid]
     double *cllr_part;       // [2, kCllrCtas]
-    unsigned long long *nonfinite;
     double *ops;             // [n_op, 4]: C_miss p, C_fa (1 - p), their min, the Bayes threshold
-    void *cub_tmp;
-    size_t cub_bytes;
 };
 
 size_t cub_temp_bytes(int64_t T) {
@@ -188,18 +206,18 @@ VerifyMetricsWs metrics_layout(uint8_t *ws, int64_t T, int n_op, size_t cub_byte
     VerifyMetricsWs w;
     size_t o = 0;
     auto take = [&](size_t bytes) { uint8_t *p = ws ? ws + o : nullptr; o += al(bytes); return p; };
-    w.key_in = reinterpret_cast<unsigned long long *>(take((size_t)T * 8));
-    w.key = reinterpret_cast<unsigned long long *>(take((size_t)T * 8));
-    w.lab_in = take((size_t)T);
-    w.lab = take((size_t)T);
-    w.tar = reinterpret_cast<long long *>(take((size_t)T * 8));
+    w.p.key_in = reinterpret_cast<unsigned long long *>(take((size_t)T * 8));
+    w.p.key = reinterpret_cast<unsigned long long *>(take((size_t)T * 8));
+    w.p.lab_in = take((size_t)T);
+    w.p.lab = take((size_t)T);
+    w.p.tar = reinterpret_cast<long long *>(take((size_t)T * 8));
     w.terms = reinterpret_cast<double *>(take((size_t)T * 8));
     w.part = reinterpret_cast<SweepPart *>(take((size_t)(n_op + 1) * kSweepGrid * sizeof(SweepPart)));
     w.cllr_part = reinterpret_cast<double *>(take(2 * kCllrCtas * 8));
-    w.nonfinite = reinterpret_cast<unsigned long long *>(take(8));
+    w.p.nonfinite = reinterpret_cast<unsigned long long *>(take(8));
     w.ops = reinterpret_cast<double *>(take((size_t)n_op * 4 * 8));
-    w.cub_tmp = take(cub_bytes);
-    w.cub_bytes = cub_bytes;
+    w.p.cub_tmp = take(cub_bytes);
+    w.p.cub_bytes = cub_bytes;
     if (total) *total = o;
     return w;
 }
@@ -406,6 +424,329 @@ __global__ void verify_final_kernel(const unsigned long long *__restrict__ key, 
     *cllr_out = (st / (double)cnt.n_tar + sn / (double)cnt.n_non) / (2.0 * log(2.0));
 }
 
+// ----------------------------------------------------------------------------------------------------------- calibration
+
+constexpr int kCalThreads = 256;
+constexpr int kCalCtas = 256;               // the fixed partition of the Newton sums and the minCllr sum
+constexpr int kCalMaxPasses = 64;           // Newton passes (evaluation + update) the host launches
+constexpr int kHullChunk = 256;             // sorted positions per thread at the first hull level
+constexpr int kCalSums = 6;                 // per class: softplus, r s, r, h s^2, h s, h
+
+struct CalState {
+    long long done, status, passes, have;   // status 0 converged, 1 separable, 2 non-finite, 3 pass limit
+    long long polish;                       // the trial point is the last, full Newton step
+    double a, b, C, ga, gb, haa, hab, hbb;  // the accepted point, its cost, gradient and Hessian
+    double da, db, t, ta, tb;               // the Newton direction, the step and the trial point
+};
+
+struct HullPoint {
+    long long x, y;                         // nontargets and targets at or above a candidate threshold
+};
+
+struct VerifyCalWs {
+    SortedTrials p;
+    double *split;           // [T] sorted scores by class rank: targets [0, N_tar), nontargets [N_tar, T)
+    HullPoint *hull;         // [T + 1] each chunk's chain from its first slot
+    long long *hlen;         // [n_chunks] the chain length of the chunk that starts a chain
+    double *eval_part;       // [2, kCalSums, kCalCtas]
+    double *seg_part;        // [kCalCtas]
+    CalState *state;
+};
+
+__host__ __device__ int64_t hull_chunks(int64_t T) { return (T + 1 + kHullChunk - 1) / kHullChunk; }
+
+int hull_levels(int64_t T) {
+    int l = 0;
+    while ((int64_t(1) << l) < hull_chunks(T)) ++l;
+    return l;
+}
+
+VerifyCalWs calibrate_layout(uint8_t *ws, int64_t T, size_t cub_bytes, size_t *total) {
+    VerifyCalWs w;
+    size_t o = 0;
+    auto take = [&](size_t bytes) { uint8_t *p = ws ? ws + o : nullptr; o += al(bytes); return p; };
+    w.p.key_in = reinterpret_cast<unsigned long long *>(take((size_t)T * 8));
+    w.p.key = reinterpret_cast<unsigned long long *>(take((size_t)T * 8));
+    w.p.lab_in = take((size_t)T);
+    w.p.lab = take((size_t)T);
+    w.p.tar = reinterpret_cast<long long *>(take((size_t)T * 8));
+    w.p.nonfinite = reinterpret_cast<unsigned long long *>(take(8));
+    w.split = reinterpret_cast<double *>(take((size_t)T * 8));
+    w.hull = reinterpret_cast<HullPoint *>(take((size_t)(T + 1) * sizeof(HullPoint)));
+    w.hlen = reinterpret_cast<long long *>(take((size_t)hull_chunks(T) * 8));
+    w.eval_part = reinterpret_cast<double *>(take(2 * kCalSums * kCalCtas * 8));
+    w.seg_part = reinterpret_cast<double *>(take(kCalCtas * 8));
+    w.state = reinterpret_cast<CalState *>(take(sizeof(CalState)));
+    w.p.cub_tmp = take(cub_bytes);
+    w.p.cub_bytes = cub_bytes;
+    if (total) *total = o;
+    return w;
+}
+
+// Every sorted score at its rank within its class (verify_sweep_kernel's indexing of the Cllr terms), so that the sums
+// below run in an order the trials' order does not change.
+__global__ void calibrate_split_kernel(const unsigned long long *__restrict__ key, const uint8_t *__restrict__ lab,
+                                       const long long *__restrict__ tar, int64_t T, double *__restrict__ split) {
+    const Counts cnt = class_counts(tar, lab, T);
+    for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < T; s += (int64_t)gridDim.x * blockDim.x) {
+        const long long tb = tar[s];
+        split[lab[s] ? tb : cnt.n_tar + (s - tb)] = key_score(key[s]);
+    }
+}
+
+// One thread: the counts, the status of the list (non-finite scores, then separable classes: a finite minimiser exists
+// exactly when min_tar < max_non and min_non < max_tar) and the start of the Newton state machine at (0, 0).
+__global__ void calibrate_init_kernel(const uint8_t *__restrict__ lab, const long long *__restrict__ tar, int64_t T,
+                                      const double *__restrict__ split, const unsigned long long *__restrict__ nonfinite,
+                                      CalState *__restrict__ state) {
+    const Counts cnt = class_counts(tar, lab, T);
+    CalState z{};
+    if (*nonfinite) z.status = 2;
+    else if (cnt.n_tar == 0 || cnt.n_non == 0) z.status = 1;
+    else if (!(split[0] < split[T - 1] && split[cnt.n_tar] < split[cnt.n_tar - 1])) z.status = 1;
+    z.done = z.status != 0;
+    *state = z;
+}
+
+// (sum over the CTA of each of the kCalSums values): the butterfly and the warps in order of cllr_block_sum
+__device__ __forceinline__ void cal_block_sums(double (&v)[kCalSums]) {
+    __shared__ double red[kCalSums][kCalThreads / 32];
+    for (int q = 0; q < kCalSums; ++q)
+        for (int o = 16; o; o >>= 1) v[q] += __shfl_xor_sync(0xffffffffu, v[q], o);
+    if ((threadIdx.x & 31) == 0)
+        for (int q = 0; q < kCalSums; ++q) red[q][threadIdx.x >> 5] = v[q];
+    __syncthreads();
+    for (int q = 0; q < kCalSums; ++q) {
+        double t = 0.0;
+        for (int w = 0; w < kCalThreads / 32; ++w) t += red[q][w];
+        v[q] = t;
+    }
+    __syncthreads();
+}
+
+// grid (kCalCtas, 2): y = 0 the targets, y = 1 the nontargets, thread k of the grid summing class ranks k,
+// k + kCalCtas x kCalThreads, ... in order.  At the trial point z = a s + b + logit(prior), e = exp(-|z|):
+//   target     softplus(-z),  r = sigma(z) - 1 = -sigma(-z)
+//   nontarget  softplus(z),   r = sigma(z)
+// and h = sigma(z) sigma(-z) = e / (1 + e)^2 for both; the sums of softplus, r s, r, h s^2, h s and h.
+__global__ void __launch_bounds__(kCalThreads) calibrate_eval_kernel(const double *__restrict__ split,
+                                                                      const uint8_t *__restrict__ lab,
+                                                                      const long long *__restrict__ tar, int64_t T,
+                                                                      double logit_prior,
+                                                                      const CalState *__restrict__ state,
+                                                                      double *__restrict__ eval_part) {
+    if (state->done) return;
+    const Counts cnt = class_counts(tar, lab, T);
+    const bool target = blockIdx.y == 0;
+    const int64_t base = target ? 0 : cnt.n_tar, n = target ? cnt.n_tar : cnt.n_non;
+    const double a = state->ta, b = state->tb;
+    double v[kCalSums] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int64_t k = (int64_t)blockIdx.x * kCalThreads + threadIdx.x; k < n; k += (int64_t)kCalCtas * kCalThreads) {
+        const double s = split[base + k];
+        const double z = __dadd_rn(__dadd_rn(__dmul_rn(a, s), b), logit_prior);
+        const double e = exp(-fabs(z)), l1 = log1p(e), op = __dadd_rn(1.0, e);
+        const double hi = __ddiv_rn(1.0, op), lo = __ddiv_rn(e, op);     // sigma(|z|), sigma(-|z|)
+        const double pz = z >= 0.0 ? hi : lo, pmz = z >= 0.0 ? lo : hi;   // sigma(z), sigma(-z)
+        const double sp = __dadd_rn(fmax(target ? -z : z, 0.0), l1);
+        const double r = target ? -pmz : pz;
+        const double h = __dmul_rn(hi, lo);
+        v[0] += sp;
+        v[1] += __dmul_rn(r, s);
+        v[2] += r;
+        v[3] += __dmul_rn(__dmul_rn(h, s), s);
+        v[4] += __dmul_rn(h, s);
+        v[5] += h;
+    }
+    cal_block_sums(v);
+    if (threadIdx.x == 0)
+        for (int q = 0; q < kCalSums; ++q) eval_part[(blockIdx.y * kCalSums + q) * kCalCtas + blockIdx.x] = v[q];
+}
+
+// 2 kCalSums warps sum the partials, one per class and quantity, in a fixed order; then one thread: the cost, gradient and Hessian at the trial point weighted by prior / N_tar
+// and (1 - prior) / N_non, then one step of the state machine.  The first evaluation, or one whose cost did not
+// increase, is accepted: d = -H^-1 g, and the trial point is the accepted one plus d.  A cost that increased halves the
+// step.  Once the predicted decrease -g.d / 2 <= 2^-52 C the cost cannot tell the points apart any more, although the
+// point can still be off by about sqrt(2^-52) of its scale: that last full step is taken without the test (a pass of
+// its own, which ends the fit), bringing the point to the precision of the gradient.  The pass limit ends the fit with
+// status 3.
+__global__ void __launch_bounds__(2 * kCalSums * 32) calibrate_update_kernel(const uint8_t *__restrict__ lab,
+                                                                              const long long *__restrict__ tar,
+                                                                              int64_t T, double prior,
+                                                                              const double *__restrict__ eval_part,
+                                                                              CalState *__restrict__ state) {
+    __shared__ double sum[2][kCalSums];
+    if (state->done) return;
+    {   // warp (class, quantity): lane l sums partials l, l + 32, ... in order, then a fixed butterfly
+        const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+        const double *p = eval_part + (int64_t)w * kCalCtas;
+        double t = 0.0;
+        for (int b = lane; b < kCalCtas; b += 32) t += p[b];
+        for (int o = 16; o; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+        if (lane == 0) sum[w / kCalSums][w % kCalSums] = t;
+    }
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    CalState S = *state;
+    const Counts cnt = class_counts(tar, lab, T);
+    const double wt = __ddiv_rn(prior, (double)cnt.n_tar), wn = __ddiv_rn(1.0 - prior, (double)cnt.n_non);
+    double f[kCalSums];
+    for (int q = 0; q < kCalSums; ++q) f[q] = __dadd_rn(__dmul_rn(wt, sum[0][q]), __dmul_rn(wn, sum[1][q]));
+    S.passes += 1;
+    if (S.polish) {                                   // differences in C are below its rounding here: no test
+        S.a = S.ta;
+        S.b = S.tb;
+        S.C = f[0];
+        S.done = 1;
+    } else if (!S.have || f[0] <= S.C) {
+        S.have = 1;
+        S.a = S.ta;
+        S.b = S.tb;
+        S.C = f[0];
+        S.ga = f[1];
+        S.gb = f[2];
+        S.haa = f[3];
+        S.hab = f[4];
+        S.hbb = f[5];
+        const double det = __dsub_rn(__dmul_rn(S.haa, S.hbb), __dmul_rn(S.hab, S.hab));
+        S.da = -__ddiv_rn(__dsub_rn(__dmul_rn(S.hbb, S.ga), __dmul_rn(S.hab, S.gb)), det);
+        S.db = -__ddiv_rn(__dsub_rn(__dmul_rn(S.haa, S.gb), __dmul_rn(S.hab, S.ga)), det);
+        const double dec = -0.5 * __dadd_rn(__dmul_rn(S.ga, S.da), __dmul_rn(S.gb, S.db));
+        if (!isfinite(dec)) {
+            S.done = 1;
+            S.status = 3;
+        } else {
+            S.polish = dec <= 0x1p-52 * S.C;
+            S.t = 1.0;
+            S.ta = __dadd_rn(S.a, S.da);
+            S.tb = __dadd_rn(S.b, S.db);
+        }
+    } else {
+        S.t *= 0.5;
+        S.ta = __dadd_rn(S.a, __dmul_rn(S.t, S.da));
+        S.tb = __dadd_rn(S.b, __dmul_rn(S.t, S.db));
+    }
+    if (!S.done && S.passes == kCalMaxPasses) {
+        S.done = 1;
+        S.status = 3;
+    }
+    *state = S;
+}
+
+// The ROC point of sorted position s (a candidate): nontargets and targets at or above its score
+__device__ __forceinline__ HullPoint roc_point(const long long *tar, const Counts &cnt, int64_t T, int64_t s) {
+    long long miss, fa;
+    cnt.at(tar, T, s, miss, fa);
+    return HullPoint{fa, cnt.n_tar - miss};
+}
+
+// Positions run from (N_non, N_tar) at s = 0 to (0, 0) at s = T.  o, a, b in that order: b is kept after a when the
+// turn o -> a -> b is strictly convex, (a - o) x (b - o) > 0; the products are exact in 128 bits.
+__device__ __forceinline__ bool strict_turn(const HullPoint &o, const HullPoint &a, const HullPoint &b) {
+    const __int128 c = (__int128)(a.x - o.x) * (b.y - o.y) - (__int128)(a.y - o.y) * (b.x - o.x);
+    return c > 0;
+}
+
+// Monotone chain step: pop while the last two vertices and p do not turn strictly, then push p.
+__device__ __forceinline__ void chain_push(HullPoint *__restrict__ h, long long &n, const HullPoint &p) {
+    while (n >= 2 && !strict_turn(h[n - 2], h[n - 1], p)) --n;
+    h[n++] = p;
+}
+
+// Level 0: thread i the chain of the candidates among positions [i kHullChunk, (i + 1) kHullChunk) n [0, T], from the
+// chunk's first slot of hull; an empty chain when the chunk has no candidate.
+__global__ void calibrate_hull_chunk_kernel(const unsigned long long *__restrict__ key, const uint8_t *__restrict__ lab,
+                                            const long long *__restrict__ tar, int64_t T, HullPoint *__restrict__ hull,
+                                            long long *__restrict__ hlen) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= hull_chunks(T)) return;
+    const Counts cnt = class_counts(tar, lab, T);
+    const int64_t s0 = i * kHullChunk, s1 = min(s0 + kHullChunk, T + 1);
+    HullPoint *h = hull + s0;
+    long long n = 0;
+    for (int64_t s = s0; s < s1; ++s)
+        if (is_candidate(key, T, s)) chain_push(h, n, roc_point(tar, cnt, T, s));
+    hlen[i] = n;
+}
+
+// Level l >= 1: thread j merges the chain starting at chunk 2j 2^(l-1) with the one at (2j + 1) 2^(l-1): the second's
+// vertices pushed in order onto the first (a vertex of the hull of the union is a vertex of one of the two chains).  The
+// result is written in place from the first chain's slot; a write never passes the vertex of the second being read.
+__global__ void calibrate_hull_merge_kernel(int64_t T, int level, HullPoint *__restrict__ hull,
+                                            long long *__restrict__ hlen) {
+    const int64_t n_chunks = hull_chunks(T), half = int64_t(1) << (level - 1);
+    const int64_t c0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 2 * half, c1 = c0 + half;
+    if (c1 >= n_chunks) return;
+    HullPoint *h = hull + c0 * kHullChunk;
+    const HullPoint *g = hull + c1 * kHullChunk;
+    long long n = hlen[c0];
+    const long long m = hlen[c1];
+    for (long long k = 0; k < m; ++k) chain_push(h, n, g[k]);
+    hlen[c0] = n;
+}
+
+// The minCllr term of hull segment k (dx nontargets, dy targets), 0 for a zero count:
+//   dy / N_tar log1p(dx N_tar / (dy N_non)) + dx / N_non log1p(dy N_non / (dx N_tar))
+__device__ __forceinline__ double segment_term(const HullPoint &p, const HullPoint &q, const Counts &cnt) {
+    const double dx = (double)(p.x - q.x), dy = (double)(p.y - q.y);
+    if (dx == 0.0 || dy == 0.0) return 0.0;
+    const double nt = (double)cnt.n_tar, nn = (double)cnt.n_non;
+    const double u = __ddiv_rn(__dmul_rn(dx, nt), __dmul_rn(dy, nn)), v = __ddiv_rn(__dmul_rn(dy, nn), __dmul_rn(dx, nt));
+    return __dadd_rn(__dmul_rn(__ddiv_rn(dy, nt), log1p(u)), __dmul_rn(__ddiv_rn(dx, nn), log1p(v)));
+}
+
+// grid kCalCtas: thread k of the grid sums segments k, k + kCalCtas x kCalThreads, ... of the hull in order
+__global__ void __launch_bounds__(kCalThreads) calibrate_segments_kernel(const uint8_t *__restrict__ lab,
+                                                                          const long long *__restrict__ tar, int64_t T,
+                                                                          const HullPoint *__restrict__ hull,
+                                                                          const long long *__restrict__ hlen,
+                                                                          double *__restrict__ seg_part) {
+    const Counts cnt = class_counts(tar, lab, T);
+    const long long n = hlen[0];
+    double v = 0.0;
+    for (int64_t k = (int64_t)blockIdx.x * kCalThreads + threadIdx.x; k + 1 < n; k += (int64_t)kCalCtas * kCalThreads)
+        v += segment_term(hull[k], hull[k + 1], cnt);
+    v = cllr_block_sum(v);
+    if (threadIdx.x == 0) seg_part[blockIdx.x] = v;
+}
+
+// One thread: info [status, passes, N_tar, N_non, hull vertices], out [a, b, cllr_prior, min_cllr]; a, b and cllr_prior
+// are NaN unless the fit ran (status 0 or 3), min_cllr is NaN for non-finite scores.
+__global__ void calibrate_final_kernel(const uint8_t *__restrict__ lab, const long long *__restrict__ tar, int64_t T,
+                                       const CalState *__restrict__ state, const long long *__restrict__ hlen,
+                                       const double *__restrict__ seg_part, long long *__restrict__ info,
+                                       double *__restrict__ out) {
+    const Counts cnt = class_counts(tar, lab, T);
+    const CalState S = *state;
+    info[0] = S.status;
+    info[1] = S.passes;
+    info[2] = cnt.n_tar;
+    info[3] = cnt.n_non;
+    info[4] = hlen[0];
+    const bool fit = S.status == 0 || S.status == 3;
+    out[0] = fit ? S.a : NAN;
+    out[1] = fit ? S.b : NAN;
+    out[2] = fit ? S.C / log(2.0) : NAN;
+    double m = 0.0;
+    for (int b = 0; b < kCalCtas; ++b) m += seg_part[b];
+    out[3] = S.status == 2 ? NAN : m / (2.0 * log(2.0));
+}
+
+// The front half of vbx_verify_metrics and vbx_verify_calibrate: the non-finite count cleared, keys and labels, the
+// radix sort and the target scan.  4 launches (the sort's and the scan's kernels counted as one each), -1 on an error.
+int sort_trials(const double *scores, const uint8_t *is_target, int64_t T, const SortedTrials &w, cudaStream_t st) {
+    if (cudaMemsetAsync(w.nonfinite, 0, 8, st) != cudaSuccess) return -1;
+    const unsigned grid = (unsigned)std::min<int64_t>((T + 255) / 256, 4096);
+    verify_keys_kernel<<<grid, 256, 0, st>>>(scores, is_target, T, w.key_in, w.lab_in, w.nonfinite);
+    size_t bytes = w.cub_bytes;
+    if (cub::DeviceRadixSort::SortPairs(w.cub_tmp, bytes, w.key_in, w.key, w.lab_in, w.lab, T, 0, 64, st) !=
+        cudaSuccess)
+        return -1;
+    verify_tar_kernel<<<grid, 256, 0, st>>>(w.lab, T, w.tar);
+    bytes = w.cub_bytes;
+    if (cub::DeviceScan::ExclusiveSum(w.cub_tmp, bytes, w.tar, T, st) != cudaSuccess) return -1;
+    return 4;
+}
+
 }  // namespace
 
 size_t verify_score_workspace_bytes(int64_t M_e, int64_t M_t) {
@@ -436,6 +777,42 @@ int launch_verify_score(const float *enroll_fea, int64_t N_e, const int32_t *enr
     return cudaGetLastError() == cudaSuccess ? le + lt + 1 : -1;
 }
 
+size_t verify_calibrate_workspace_bytes(int64_t T) {
+    size_t total = 0;
+    calibrate_layout(nullptr, T, cub_temp_bytes(T), &total);
+    return total;
+}
+
+int launch_verify_calibrate(const double *scores, const uint8_t *is_target, int64_t T, double prior, void *workspace,
+                            long long *info_out, double *out, cudaStream_t st) {
+    const VerifyCalWs w = calibrate_layout(reinterpret_cast<uint8_t *>(workspace), T, cub_temp_bytes(T), nullptr);
+    int launches = sort_trials(scores, is_target, T, w.p, st);
+    if (launches < 0) return -1;
+    const SortedTrials &p = w.p;
+    const unsigned grid = (unsigned)std::min<int64_t>((T + 255) / 256, 4096);
+    calibrate_split_kernel<<<grid, 256, 0, st>>>(p.key, p.lab, p.tar, T, w.split);
+    calibrate_init_kernel<<<1, 1, 0, st>>>(p.lab, p.tar, T, w.split, p.nonfinite, w.state);
+    const double logit_prior = std::log(prior / (1.0 - prior));
+    for (int k = 0; k < kCalMaxPasses; ++k) {
+        calibrate_eval_kernel<<<dim3(kCalCtas, 2), kCalThreads, 0, st>>>(w.split, p.lab, p.tar, T, logit_prior, w.state,
+                                                                        w.eval_part);
+        calibrate_update_kernel<<<1, 2 * kCalSums * 32, 0, st>>>(p.lab, p.tar, T, prior, w.eval_part, w.state);
+    }
+    const int64_t n_chunks = hull_chunks(T);
+    calibrate_hull_chunk_kernel<<<(unsigned)((n_chunks + 127) / 128), 128, 0, st>>>(p.key, p.lab, p.tar, T, w.hull,
+                                                                                     w.hlen);
+    const int levels = hull_levels(T);
+    for (int l = 1; l <= levels; ++l) {
+        const int64_t pairs = (n_chunks + (int64_t(2) << (l - 1)) - 1) / (int64_t(2) << (l - 1));
+        calibrate_hull_merge_kernel<<<(unsigned)((pairs + 127) / 128), 128, 0, st>>>(T, l, w.hull, w.hlen);
+    }
+    calibrate_segments_kernel<<<kCalCtas, kCalThreads, 0, st>>>(p.lab, p.tar, T, w.hull, w.hlen, w.seg_part);
+    calibrate_final_kernel<<<1, 1, 0, st>>>(p.lab, p.tar, T, w.state, w.hlen, w.seg_part, info_out, out);
+    // the sort prefix, split, init, the Newton passes, the hull levels, segments, final
+    launches += 2 + 2 * kCalMaxPasses + 1 + levels + 2;
+    return cudaGetLastError() == cudaSuccess ? launches : -1;
+}
+
 size_t verify_metrics_workspace_bytes(int64_t T, int n_op) {
     size_t total = 0;
     metrics_layout(nullptr, T, n_op, cub_temp_bytes(T), &total);
@@ -446,22 +823,14 @@ int launch_verify_metrics(const double *scores, const uint8_t *is_target, int64_
                           void *workspace, long long *counts_out, double *eer_out, double *cllr_out,
                           double *min_dcf_out, double *threshold_out, double *act_dcf_out, cudaStream_t st) {
     const VerifyMetricsWs w = metrics_layout(reinterpret_cast<uint8_t *>(workspace), T, n_op, cub_temp_bytes(T), nullptr);
-    if (cudaMemsetAsync(w.nonfinite, 0, 8, st) != cudaSuccess) return -1;
     if (cudaMemcpyAsync(w.ops, ops_host, (size_t)n_op * 4 * sizeof(double), cudaMemcpyHostToDevice, st) != cudaSuccess)
         return -1;
-    const unsigned grid = (unsigned)std::min<int64_t>((T + 255) / 256, 4096);
-    verify_keys_kernel<<<grid, 256, 0, st>>>(scores, is_target, T, w.key_in, w.lab_in, w.nonfinite);
-    size_t bytes = w.cub_bytes;
-    if (cub::DeviceRadixSort::SortPairs(w.cub_tmp, bytes, w.key_in, w.key, w.lab_in, w.lab, T, 0, 64, st) !=
-        cudaSuccess)
-        return -1;
-    verify_tar_kernel<<<grid, 256, 0, st>>>(w.lab, T, w.tar);
-    bytes = w.cub_bytes;
-    if (cub::DeviceScan::ExclusiveSum(w.cub_tmp, bytes, w.tar, T, st) != cudaSuccess) return -1;
+    if (sort_trials(scores, is_target, T, w.p, st) < 0) return -1;
+    const SortedTrials &p = w.p;
     const int gx = (int)std::min<int64_t>((T + kSweepThreads) / kSweepThreads, kSweepGrid);   // T + 1 positions
-    verify_sweep_kernel<<<dim3(gx, n_op + 1), kSweepThreads, 0, st>>>(w.key, w.lab, w.tar, T, w.ops, w.terms, w.part);
-    verify_cllr_kernel<<<dim3(kCllrCtas, 2), kCllrThreads, 0, st>>>(w.terms, w.lab, w.tar, T, w.cllr_part);
-    verify_final_kernel<<<1, 1, 0, st>>>(w.key, w.lab, w.tar, T, w.ops, n_op, w.part, gx, w.cllr_part, w.nonfinite,
+    verify_sweep_kernel<<<dim3(gx, n_op + 1), kSweepThreads, 0, st>>>(p.key, p.lab, p.tar, T, w.ops, w.terms, w.part);
+    verify_cllr_kernel<<<dim3(kCllrCtas, 2), kCllrThreads, 0, st>>>(w.terms, p.lab, p.tar, T, w.cllr_part);
+    verify_final_kernel<<<1, 1, 0, st>>>(p.key, p.lab, p.tar, T, w.ops, n_op, w.part, gx, w.cllr_part, p.nonfinite,
                                           counts_out, eer_out, cllr_out, min_dcf_out, threshold_out, act_dcf_out);
     // keys, sort (its kernels counted as one), labels, scan (counted as one), sweep, Cllr, final
     return cudaGetLastError() == cudaSuccess ? 7 : -1;

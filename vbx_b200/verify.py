@@ -32,6 +32,13 @@ score >= t / N_non, exact integer counts and one float64 division each.
        reported next to it.
 Defaults p = 0.01, C_miss = C_fa = 1.  The metrics need at least one target and one nontarget trial.
 
+Calibration (DESIGN.md section 5.28).  --calibrate-out FILE fits llr = a s + b to the labelled list by prior-weighted
+logistic regression (--calibration-prior, default 0.5) on the device (vbx_verify_calibrate), writes it with the score
+kind, Fa, Fb, --lda-dim, --cohort-top and the SHA-256 of the model files, and reports minCllr and the metrics of the
+calibrated scores on the same list (self-calibrated: an optimistic figure).  --calibration FILE scores a s + b instead
+of s; the file must match this run's kind, Fa, Fb, --lda-dim, --cohort-top and model files.  python -m vbx_b200.cli
+--calibration FILE states --link-threshold and --enroll-threshold as calibrated LLRs.
+
 Statistics and scores run in vbx_verify_score, the metrics in vbx_verify_metrics (sort, scans and fixed-order
 reductions on the device: bit-identical from run to run and for any order of the trials).
 """
@@ -214,6 +221,165 @@ def error_rates(scores, labels, p_targets=(DEFAULT_P_TARGET,), c_miss=1.0, c_fa=
                 act_dcf=res[2 + 2 * n_op:].tolist())
 
 
+CALIBRATION_VERSION = 1
+CALIBRATION_KEYS = ('version', 'a', 'b', 'prior', 'score_kind', 'Fa', 'Fb', 'lda_dim', 'cohort_top',
+                    'xvec_transform_sha256', 'plda_file_sha256', 'n_target', 'n_nontarget')
+SEPARABLE, NONFINITE, NOT_CONVERGED = 1, 2, 3       # vbx_verify_calibrate statuses
+
+
+def calibrate(scores, labels, prior=0.5, device=None):
+    """The linear calibration llr = a s + b of scored trials on the device (vbx_verify_calibrate, DESIGN.md section
+    5.28): (a, b) minimise the prior-weighted logistic cost, cllr_prior = C(a, b) / ln 2 (at prior 0.5 the Cllr of
+    a s + b), min_cllr the Cllr of the optimal monotone transform of the scores (PAV; at prior 0.5).  Returns dict(a, b,
+    prior, cllr_prior, min_cllr, passes, n_target, n_nontarget, hull_vertices).  ValueError before any device work: an
+    empty list, labels of another length, no target or no nontarget trial, a prior outside (0, 1); after the device
+    pass: separable classes or non-finite scores.  VbxError: the fit did not converge."""
+    import torch
+    from . import _lib
+    from ._lib import VbxError
+    prior = float(prior)
+    if not 0.0 < prior < 1.0:
+        raise ValueError(f'prior must lie in (0, 1), got {prior!r}')
+    lab = np.asarray(labels).reshape(-1)
+    T = int(scores.shape[0]) if hasattr(scores, 'shape') else len(scores)
+    if T == 0:
+        raise ValueError('no trials')
+    if len(lab) != T:
+        raise ValueError(f'{len(lab)} labels for {T} scores')
+    lab = lab.astype(bool)
+    n_tar = int(lab.sum())
+    if n_tar == 0 or n_tar == T:
+        raise ValueError(f'a calibration needs target and nontarget trials, got {n_tar} targets of {T}')
+    dev = _device(device)
+    lib = _lib.load()
+    h = ctypes.c_void_p()
+    if lib.vbx_create(dev.index, ctypes.byref(h)) != 0:
+        raise VbxError('vbx_create failed: no usable sm_90 device')
+    p = lambda t: ctypes.c_void_p(t.data_ptr())
+    try:
+        need = ctypes.c_size_t()
+        if lib.vbx_verify_calibrate_workspace_bytes(h, T, ctypes.byref(need)) != 0:
+            raise VbxError(f'vbx_verify_calibrate_workspace_bytes failed: {lib.vbx_last_error(h).decode()}')
+        with torch.cuda.device(dev):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            s = torch.as_tensor(scores).to(dev, torch.float64).contiguous().reshape(-1)
+            y = torch.from_numpy(lab.astype(np.uint8)).to(dev)
+            ws = torch.empty(int(need.value), dtype=torch.uint8, device=dev)
+            info = torch.empty(5, dtype=torch.int64, device=dev)
+            res = torch.empty(4, dtype=torch.float64, device=dev)
+            rc = lib.vbx_verify_calibrate(h, p(s), p(y), T, prior, p(ws), ws.numel(), p(info), p(res), stream)
+            if rc != 0:
+                raise VbxError(f'vbx_verify_calibrate failed ({rc}): {lib.vbx_last_error(h).decode()}')
+            info, res = info.cpu().numpy(), res.cpu().numpy()
+    finally:
+        lib.vbx_destroy(h)
+    status = int(info[0])
+    if status == NONFINITE:
+        raise ValueError('non-finite score(s): a calibration needs finite scores')
+    if status == SEPARABLE:
+        s = np.asarray(scores.detach().cpu().numpy() if hasattr(scores, 'detach') else scores, dtype=np.float64)
+        s = s.reshape(-1)
+        how = 'at or above' if s[lab].min() >= s[~lab].max() else 'at or below'
+        raise ValueError(f'the classes are separable: every target trial scores {how} every nontarget trial, so the '
+                         f'logistic regression has no finite minimiser (minCllr {float(res[3]):.6g})')
+    if status == NOT_CONVERGED:
+        raise VbxError(f'vbx_verify_calibrate: the fit did not converge in {int(info[1])} passes')
+    return dict(a=float(res[0]), b=float(res[1]), prior=prior, cllr_prior=float(res[2]), min_cllr=float(res[3]),
+                passes=int(info[1]), n_target=int(info[2]), n_nontarget=int(info[3]), hull_vertices=int(info[4]))
+
+
+def file_sha256(path):
+    """The SHA-256 of a file's bytes, hex."""
+    import hashlib
+    d = hashlib.sha256()
+    with open(path, 'rb') as f:
+        for chunk in iter(lambda: f.read(1 << 20), b''):
+            d.update(chunk)
+    return d.hexdigest()
+
+
+def write_calibration(path, fit, score_kind, Fa, Fb, lda_dim, cohort_top, xvec_transform, plda_file):
+    """Write a calibration file (JSON): calibrate's a, b, prior and trial counts, and what the scores it was fitted on
+    depend on: the score kind ('llr' / 'as-norm'), Fa, Fb, lda_dim, cohort_top (as-norm only, else None) and the
+    SHA-256 of the x-vector transform and PLDA files."""
+    if score_kind not in ('llr', 'as-norm'):
+        raise ValueError(f'score_kind must be llr or as-norm, got {score_kind!r}')
+    doc = dict(version=CALIBRATION_VERSION, a=float(fit['a']), b=float(fit['b']), prior=float(fit['prior']),
+               score_kind=score_kind, Fa=float(Fa), Fb=float(Fb), lda_dim=int(lda_dim),
+               cohort_top=None if score_kind == 'llr' else int(cohort_top),
+               xvec_transform_sha256=file_sha256(xvec_transform), plda_file_sha256=file_sha256(plda_file),
+               n_target=int(fit['n_target']), n_nontarget=int(fit['n_nontarget']))
+    with open(path, 'w') as f:
+        json.dump(doc, f, indent=1)
+        f.write('\n')
+    return doc
+
+
+def read_calibration(path):
+    """A calibration file as a dict, checked: ValueError for an unknown version, a missing key, a non-finite number, a
+    prior outside (0, 1), an unknown score kind, a cohort_top that does not fit the kind, bad counts or hashes."""
+    with open(path) as f:
+        try:
+            doc = json.load(f)
+        except json.JSONDecodeError as e:
+            raise ValueError(f'{path}: not a calibration file ({e})')
+    if not isinstance(doc, dict):
+        raise ValueError(f'{path}: not a calibration file')
+    if doc.get('version') != CALIBRATION_VERSION:
+        raise ValueError(f'{path}: calibration format version {doc.get("version")!r}, this reader knows '
+                         f'{CALIBRATION_VERSION}')
+    missing = [k for k in CALIBRATION_KEYS if k not in doc]
+    if missing:
+        raise ValueError(f'{path}: missing {", ".join(missing)}')
+    for k in ('a', 'b', 'prior', 'Fa', 'Fb'):
+        v = doc[k]
+        if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+            raise ValueError(f'{path}: {k} must be a finite number, got {v!r}')
+        doc[k] = float(v)
+    if not 0.0 < doc['prior'] < 1.0:
+        raise ValueError(f'{path}: prior must lie in (0, 1), got {doc["prior"]!r}')
+    if not (doc['Fa'] > 0 and doc['Fb'] > 0):
+        raise ValueError(f'{path}: Fa and Fb must be > 0')
+    if doc['score_kind'] not in ('llr', 'as-norm'):
+        raise ValueError(f'{path}: score_kind must be llr or as-norm, got {doc["score_kind"]!r}')
+    for k in ('lda_dim', 'n_target', 'n_nontarget'):
+        if isinstance(doc[k], bool) or not isinstance(doc[k], int) or doc[k] < 1:
+            raise ValueError(f'{path}: {k} must be an integer >= 1, got {doc[k]!r}')
+    top = doc['cohort_top']
+    if doc['score_kind'] == 'llr' and top is not None:
+        raise ValueError(f'{path}: cohort_top is for as-norm scores only')
+    if doc['score_kind'] == 'as-norm' and (isinstance(top, bool) or not isinstance(top, int) or top < 2):
+        raise ValueError(f'{path}: as-norm scores need an integer cohort_top >= 2, got {top!r}')
+    for k in ('xvec_transform_sha256', 'plda_file_sha256'):
+        v = doc[k]
+        if not (isinstance(v, str) and len(v) == 64 and all(c in '0123456789abcdef' for c in v)):
+            raise ValueError(f'{path}: {k} must be a SHA-256 in hex')
+    return doc
+
+
+def raw_threshold(cal, t):
+    """The raw score threshold (t - b) / a in float64 of a calibrated LLR threshold t: a calibrated score a s + b is
+    >= t exactly where s >= (t - b) / a, up to the rounding of this division.  ValueError when a <= 0 (the
+    calibration does not keep the scores' order)."""
+    a, b = float(cal['a']), float(cal['b'])
+    if not a > 0.0:
+        raise ValueError(f'the calibration\'s slope a = {a!r} is not positive: a threshold cannot be carried over')
+    return (float(t) - b) / a
+
+
+def calibration_mismatch(cal, score_kind, Fa, Fb, lda_dim, cohort_top, xvec_transform, plda_file):
+    """The first way in which a calibration does not fit a run's scores, as a message, or None."""
+    want = dict(score_kind=score_kind, Fa=float(Fa), Fb=float(Fb), lda_dim=int(lda_dim),
+                cohort_top=None if score_kind == 'llr' else int(cohort_top))
+    for k, v in want.items():
+        if cal[k] != v:
+            return f'the calibration was fitted with {k} {cal[k]!r}, this run has {v!r}'
+    for k, path in (('xvec_transform_sha256', xvec_transform), ('plda_file_sha256', plda_file)):
+        if cal[k] != file_sha256(path):
+            return f'the calibration was fitted with another {k[:-7].replace("_", "-")} ({path} differs)'
+    return None
+
+
 def trial_norm(enroll_fea, enroll_item, test_fea, test_item, Phi, cohort_fea, cohort_speaker, Fa=1.0, Fb=1.0,
                top_k=None, device=None):
     """The norm= of score_trials: each side's items' top-K cohort statistics (cohort.cohort_stats with offsets None and
@@ -279,6 +445,13 @@ def build_parser():
     ap.add_argument('--c-fa', type=float, default=1.0, help='cost of a false alarm (default 1)')
     ap.add_argument('--scores-out', default=None, help='write "enrol test score" lines in trial order')
     ap.add_argument('--json', default=None, help='write the metrics, score kind, counts and timings as JSON')
+    ap.add_argument('--calibrate-out', default=None,
+                    help='fit the calibration llr = a s + b to the labelled trials (DESIGN.md section 5.28) and write '
+                         'it to this file; the metrics of the calibrated scores on the same list are reported too')
+    ap.add_argument('--calibration-prior', type=float, default=None,
+                    help='with --calibrate-out: the prior of the logistic regression (default 0.5)')
+    ap.add_argument('--calibration', default=None,
+                    help='a calibration file of --calibrate-out: score a s + b for the metrics and --scores-out')
     return ap
 
 
@@ -292,6 +465,13 @@ def check_args(ap, args):
         ap.error('--cohort-top must be >= 2')
     if args.lda_dim < 1:
         ap.error('--lda-dim must be >= 1')
+    if args.calibrate_out is not None and args.calibration is not None:
+        ap.error('--calibrate-out and --calibration do not combine: fit on one list, apply to another')
+    if args.calibration_prior is not None:
+        if args.calibrate_out is None:
+            ap.error('--calibration-prior needs --calibrate-out')
+        if not 0.0 < args.calibration_prior < 1.0:
+            ap.error('--calibration-prior must lie in (0, 1)')
     for name in ('Fa', 'Fb', 'c_miss', 'c_fa'):
         v = getattr(args, name)
         if not (math.isfinite(v) and v > 0):
@@ -306,11 +486,24 @@ def main(argv=None):
     ap = build_parser()
     args = ap.parse_args(argv)
     ps = check_args(ap, args)
+    cal = None
+    if args.calibration is not None:
+        try:
+            cal = read_calibration(args.calibration)
+            why = calibration_mismatch(cal, 'llr' if args.cohort_ark is None else 'as-norm', args.Fa, args.Fb,
+                                       args.lda_dim, 200 if args.cohort_top is None else args.cohort_top,
+                                       args.xvec_transform, args.plda_file)
+        except (OSError, ValueError) as e:
+            ap.error(f'--calibration: {e}')
+        if why is not None:
+            ap.error(f'--calibration: {why}')
     from . import formats, pipeline
     t0 = time.perf_counter()
     en, xe, ie = read_items(args.enroll_ark, args.enroll_utt2spk)
     tn, xt, it = read_items(args.test_ark, args.test_utt2spk)
     e_ids, t_ids, labels = formats.read_trials(args.trials, en, tn)
+    if args.calibrate_out is not None and labels is None:
+        ap.error('--calibrate-out needs a labelled trial list')
     ei, ti = {n: k for k, n in enumerate(en)}, {n: k for k, n in enumerate(tn)}
     trials = np.stack([np.array([ei[n] for n in e_ids], dtype=np.int64), np.array([ti[n] for n in t_ids], dtype=np.int64)], 1)
     cohort = formats.read_enrolment(args.cohort_ark, args.cohort_utt2spk) if args.cohort_ark is not None else None
@@ -341,10 +534,19 @@ def main(argv=None):
     scores = score_trials(fe, ie, ft, it, Phi, trials, Fa=args.Fa, Fb=args.Fb, norm=norm, device=dev)
     t4 = time.perf_counter()
     kind = 'llr' if norm is None else 'as-norm'
+    if cal is not None:
+        scores = cal['a'] * scores + cal['b']
     metrics = None
     if labels is not None:
         metrics = error_rates(scores, labels, ps, args.c_miss, args.c_fa, device=dev)
     t5 = time.perf_counter()
+    fit = fit_metrics = None
+    if args.calibrate_out is not None:
+        fit = calibrate(scores, labels, 0.5 if args.calibration_prior is None else args.calibration_prior, device=dev)
+        write_calibration(args.calibrate_out, fit, kind, args.Fa, args.Fb, args.lda_dim,
+                          200 if args.cohort_top is None else args.cohort_top, args.xvec_transform, args.plda_file)
+        fit_metrics = error_rates(fit['a'] * scores + fit['b'], labels, ps, args.c_miss, args.c_fa, device=dev)
+    t6 = time.perf_counter()
     if args.scores_out is not None:
         with open(args.scores_out, 'w') as f:
             f.write(''.join(f'{a} {b} {float(s)!r}\n' for a, b, s in zip(e_ids, t_ids, scores.tolist())))
@@ -361,6 +563,16 @@ def main(argv=None):
             doc.update(eer=metrics['eer'], cllr=metrics['cllr'],
                        operating_points=[dict(p_target=p, min_dcf=m, threshold=th, act_dcf=a) for p, m, th, a in
                                          zip(ps, metrics['min_dcf'], metrics['threshold'], metrics['act_dcf'])])
+        if cal is not None:
+            doc.update(calibration_applied=dict(file=args.calibration, a=cal['a'], b=cal['b'], prior=cal['prior']))
+        if fit is not None:
+            doc['timings_s']['calibrate'] = t6 - t5
+            doc.update(min_cllr=fit['min_cllr'], calibration=dict(
+                a=fit['a'], b=fit['b'], prior=fit['prior'], cllr_prior=fit['cllr_prior'], passes=fit['passes'],
+                hull_vertices=fit['hull_vertices'], self_calibrated=True, eer=fit_metrics['eer'],
+                cllr=fit_metrics['cllr'],
+                operating_points=[dict(p_target=p, min_dcf=m, threshold=th, act_dcf=a) for p, m, th, a in
+                                  zip(ps, fit_metrics['min_dcf'], fit_metrics['threshold'], fit_metrics['act_dcf'])]))
         with open(args.json, 'w') as f:
             json.dump(doc, f, indent=1)
     if metrics is None:
@@ -370,6 +582,10 @@ def main(argv=None):
                         zip(ps, metrics['min_dcf'], metrics['threshold'], metrics['act_dcf']))
         print(f'verify: {len(scores)} trials ({n_tar} target), {kind}: EER {100 * metrics["eer"]:.3f} %, {ops}, '
               f'Cllr ({kind}) {metrics["cllr"]:.4f}')
+    if fit is not None:
+        print(f'verify: calibration a {fit["a"]:.6g}, b {fit["b"]:.6g} at prior {fit["prior"]:g} written to '
+              f'{args.calibrate_out}: minCllr {fit["min_cllr"]:.4f}, Cllr of the calibrated scores (self-calibrated) '
+              f'{fit_metrics["cllr"]:.4f}')
     return 0
 
 
