@@ -15,10 +15,10 @@ from vbx_b200 import link, pipeline, score
 
 GOLD = os.path.join(os.path.dirname(__file__), 'golden')
 C = 0.3 / 17
-# Feature widths of the speaker-pair scores (score_tile, enroll_score_kernel and verify_score_kernel stage 32-feature
-# chunks and take one log per group of 8 denominators): a single partial group (1, 3, 7), one group and one feature
-# (9), whole groups inside a chunk (24), both sides of the 32-, 64- and 96-feature chunk edges, and a partial last chunk
-# that ends in a partial group (100, 127).  Every feature is live (width_phi).
+# Feature widths of the speaker-pair scores (the link and enrolment tiles and verify_score_kernel stage 32-feature
+# chunks, and llr_step takes one log per group of 8 denominators): a single partial group (1, 3, 7), one group and one
+# feature (9), whole groups inside a chunk (24), both sides of the 32-, 64- and 96-feature chunk edges, and a partial
+# last chunk that ends in a partial group (100, 127).  Every feature is live (width_phi).
 SPEAKER_WIDTHS = [1, 3, 7, 9, 24, 31, 33, 40, 63, 65, 96, 100, 127]
 
 

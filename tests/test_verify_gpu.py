@@ -1,6 +1,7 @@
 """Speaker-verification trials on the GPU (DESIGN.md section 5.27): trial scores against the float64 oracle and bit for
-bit against the cohort scores of the same pairs, AS-norm, the error rates bit for bit against the oracle, the refusals
-of the Python layer and of the C ABI, and the command line end to end."""
+bit against the cohort scores of the same pairs, AS-norm against the oracle and bit for bit against the normalised
+enrolment scores, the error rates bit for bit against the oracle, the refusals of the Python layer and of the C ABI,
+and the command line end to end."""
 import ctypes
 import json
 import os
@@ -11,7 +12,7 @@ import torch
 
 from oracle import verify_oracle as O
 from test_link_gpu import SPEAKER_WIDTHS, width_phi
-from vbx_b200 import _lib, cohort, formats, pipeline, train, verify
+from vbx_b200 import _lib, cohort, enroll, formats, pipeline, train, verify
 
 DEV = 'cuda:0'
 GOLD = os.path.join(os.path.dirname(__file__), 'golden')
@@ -74,6 +75,23 @@ def test_scores_are_the_cohort_scores_bit_for_bit(R, multi):
     assert got.tobytes() == L.ravel().tobytes()
     swapped = verify.score_trials(ft, it, fe, ie, Phi, tr[:, ::-1], Fa=Fa, Fb=Fb, device=DEV)
     assert swapped.tobytes() == got.tobytes()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('R, multi', [(16, True), (128, False), (128, True)]
+                         + [(R, k % 2 == 0) for k, R in enumerate(SPEAKER_WIDTHS)])
+def test_as_norm_is_the_normalised_enrolment_score_bit_for_bit(R, multi):
+    """Enrolment items as the speakers of one recording, test items as the enrolled speakers: every trial's AS-norm
+    score is the normalised enrolment score of the same pair."""
+    Fa, Fb = 0.3, 17.0
+    fe, ie, ft, it, Phi, _ = problem(R, multi, 7 * R)
+    fc, ic = side(300, R, Phi, np.random.default_rng(5), True)
+    norm = verify.trial_norm(fe, ie, ft, it, Phi, fc, ic, Fa, Fb, top_k=50, device=DEV)
+    S = enroll.enroll_speakers(fe, Phi, [0, len(ie)], [ie], ft, it, Fa, Fb, 0.0, device=DEV, llr=True, norm=norm).llr
+    ii, jj = np.meshgrid(np.arange(S.shape[0]), np.arange(S.shape[1]), indexing='ij')
+    tr = np.stack([ii.ravel(), jj.ravel()], 1)
+    got = verify.score_trials(fe, ie, ft, it, Phi, tr, Fa=Fa, Fb=Fb, norm=norm, device=DEV)
+    assert got.tobytes() == S.ravel().tobytes()
 
 
 @pytest.mark.gpu

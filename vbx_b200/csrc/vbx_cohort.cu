@@ -25,19 +25,6 @@ constexpr int kTopThreads = 256;
 constexpr int kTopWarps = kTopThreads / 32;
 constexpr int64_t kNormGrid = 1 << 20;     // CTAs of norm_scores_kernel at most; beyond that they stride
 
-__host__ __device__ size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
-
-// Doubles ordered as their keys are ordered (as unsigned integers): negative values bit-inverted, the others with the
-// sign bit set.  -0.0 sorts just below +0.0; equal values have equal keys.
-__device__ __forceinline__ unsigned long long order_key(double v) {
-    const unsigned long long u = (unsigned long long)__double_as_longlong(v);
-    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
-}
-
-__device__ __forceinline__ double key_value(unsigned long long k) {
-    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
-}
-
 // Sum over the CTA: a fixed butterfly in every warp, then the warps in order (the same bits on every run).
 __device__ __forceinline__ double block_sum(double v, double *red) {
     for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -136,7 +123,7 @@ __global__ void __launch_bounds__(256) norm_scores_kernel(double *__restrict__ x
         double d = *xt;
         if (!link || (i != j && d != skip)) {
             const double l = link ? -d : d;
-            const double s = 0.5 * ((l - mr[ri]) / sr[ri] + (l - mc[cj]) / sc[cj]);
+            const double s = as_norm(l, mr, sr, ri, mc, sc, cj);
             d = link ? -s : s;
             *xt = d;
         }

@@ -32,7 +32,6 @@ constexpr int kWarps = kThreads / 32;
 constexpr int kCols = 384;                       // kMaxGlobal + kMaxLabels "unmatched" columns, rounded up to 32
 constexpr int64_t kSmemCells = 64 * 128;         // 64 KB of int64, the shared block of score_kernel
 
-__host__ __device__ inline size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
 __host__ __device__ inline int64_t n_pairs(int K) { return (int64_t)K * (K - 1) / 2; }
 __host__ __device__ inline int pair_index(int a, int b, int K) { return a * (2 * K - a - 1) / 2 + (b - a - 1); }   // a < b
 __host__ __device__ inline int global_stride(int K, int ML) { return K * ML < kMaxGlobal ? K * ML : kMaxGlobal; }

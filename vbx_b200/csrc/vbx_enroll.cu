@@ -5,8 +5,8 @@
 // launch_speaker_stats_batch), every archive speaker s is scored against every enrolled speaker e with section 5.15's
 // LLR, and each recording's speakers are assigned one-to-one to enrolled speakers or to "unknown":
 //   enroll_score_kernel   llr [M, E], 32 x 32 tiles of every problem's rectangle, the flat tile index decoded into
-//                         (problem, tile); per pair the operations of vbx_link's score_tile in the same order, so
-//                         llr[s][e] is bit-identical to -dist[s][e] of vbx_link_batch on the same speakers
+//                         (problem, tile); llr[s][e] is bit-identical to -dist[s][e] of vbx_link_batch on the same
+//                         speakers (both score through tile_llr_sums and pair_llr)
 //   enroll_assign_kernel  per recording b with K_b speakers and threshold h the minimum-cost assignment of the
 //                         K_b x (E + K_b) matrix C[k][e] = threshold_h - llr[k][e] (e < E), C[k][E + j] = 0 ("unknown"
 //                         columns), by shortest augmenting paths (Jonker-Volgenant, the method of scipy's
@@ -26,36 +26,10 @@ namespace vbx {
 
 namespace {
 
-constexpr int kLogGroup = 8;                // as vbx_link: log of a product of 8 denominators, overflowed_log_sum
 constexpr int64_t kScoreGrid = 1 << 20;     // CTAs of enroll_score_kernel at most; beyond that they stride over the tiles
 constexpr int kAssignThreads = 256;
 constexpr int kAssignWarps = kAssignThreads / 32;
 constexpr int kAssignCtasPerSm = 2;
-
-__host__ __device__ size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
-
-// As vbx_link: the log term sum_r log(fma(cm, Phi_r, 1)) of a pair whose sum of group logs came out +inf: some product of
-// kLogGroup denominators overflowed (each denominator is finite, but any finite positive Fa / Fb is accepted, so c can
-// be large).  The same groups in the same order, each multiply that would overflow first flushing the product so far
-// into the sum; a group that did not overflow gives the same log as in the scoring loop.  Out of line and reached only
-// from that case, so the loop's registers and instructions stay those of plain groups.
-__device__ __noinline__ double overflowed_log_sum(double cm, const float *__restrict__ Phi, int R) {
-    double lg = 0.0, prod = 1.0;
-    for (int r = 0; r < R; ++r) {
-        const double den = fma(cm, (double)Phi[r], 1.0), pd = prod * den;
-        if (pd > DBL_MAX) {
-            lg += log(prod);
-            prod = den;
-        } else {
-            prod = pd;
-        }
-        if ((r % kLogGroup) == kLogGroup - 1 || r == R - 1) {
-            lg += log(prod);
-            prod = 1.0;
-        }
-    }
-    return lg;
-}
 
 // one CTA's column and row state in the workspace: columns nc = E + K_b <= E + max_k, rows K_b <= max_k
 struct Slice {
@@ -126,10 +100,9 @@ struct ScoreProblems {
     const double *c;
 };
 
-// Tile (bi, bj) of 32 archive speakers (rows) x 32 enrolled speakers (columns): 256 threads, 4 pairs each (rows ty,
-// ty + 8, ..), features in chunks of 32 through shared memory; every operation as in vbx_link's score_tile.  The flat
-// tile index runs over the rectangles of all problems (decoded as link_score_kernel does), so the grid stays
-// one-dimensional and capped for any G, M_g and E.
+// Tile (bi, bj) of 32 archive speakers (rows) x 32 enrolled speakers (columns) (tile_llr_sums).  The flat tile index
+// runs over the rectangles of all problems (decoded as link_score_kernel does), so the grid stays one-dimensional and
+// capped for any G, M_g and E.
 __global__ void __launch_bounds__(256) enroll_score_kernel(SpeakerStats A0, SpeakerStats En0, const float *__restrict__ Phi,
                                                            int64_t E, int R, double *__restrict__ llr0,
                                                            double *__restrict__ llr_out0, ScoreProblems pr) {
@@ -157,43 +130,15 @@ __global__ void __launch_bounds__(256) enroll_score_kernel(SpeakerStats A0, Spea
             const int64_t i = i0 + ty + 8 * u;
             cm[u] = c * ((i < M ? A.n[i] : 0.0) + nj);
         }
-        for (int r0 = 0; r0 < R; r0 += 32) {
-            for (int v = ty; v < 32; v += 8) {
-                const int r = r0 + tx;
-                a[v][tx] = (i0 + v < M && r < R) ? A.b[(i0 + v) * kMaxR + r] : 0.0;
-                bt[v][tx] = (j0 + v < E && r < R) ? En.b[(j0 + v) * kMaxR + r] : 0.0;
-            }
-            if (ty == 0) ph[tx] = r0 + tx < R ? (double)Phi[r0 + tx] : 0.0;
-            __syncthreads();
-            const int len = min(32, R - r0);
-            for (int k = 0; k < len; ++k) {
-                const double bj_k = bt[tx][k], p = ph[k];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const double den = fma(cm[u], p, 1.0), x = a[ty + 8 * u][k] + bj_k;
-                    q[u] += x * x / den;
-                    prod[u] *= den;
-                }
-                if (((r0 + k) % kLogGroup) == kLogGroup - 1 || r0 + k == R - 1) {
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        lg[u] += log(prod[u]);
-                        prod[u] = 1.0;
-                    }
-                }
-            }
-            __syncthreads();                          // also keeps the next tile's loads behind this tile's reads
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-            if (lg[u] > DBL_MAX) lg[u] = overflowed_log_sum(cm[u], Phi, R);
+        tile_llr_sums(a, bt, ph, A.b, M, En.b, E, Phi, R, i0, j0, cm, q, lg, prod);
+        llr_finish<4>(lg, cm, Phi, R);
         if (j >= E) continue;
         const double ej = En.e[j];
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
             const int64_t i = i0 + ty + 8 * u;
             if (i >= M) continue;
-            const double l = (A.n[i] == 0.0 || nj == 0.0) ? 0.0 : 0.5 * ((q[u] - lg[u]) - (A.e[i] + ej));
+            const double l = pair_llr(q[u], lg[u], A.n[i], nj, A.e[i], ej);
             llr[i * E + j] = l;
             if (llr_out) llr_out[i * E + j] = l;
         }

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cfloat>
 #include <string>
 #include <vector>
 
@@ -20,6 +21,9 @@ constexpr int kMaxS = 64;
 // (vbx_fb_split.cu).  Buffers sized by kMaxS keep their size for S <= 64; the S = 128 instantiations size theirs by S.
 constexpr int kMaxSWide = 128;
 constexpr int kTcMaxD = 2048;  // largest raw dimension of the tensor-core front end (bounds its scratch in the workspace)
+
+// v rounded up to 256 bytes: the alignment of every region the workspace layouts carve
+__host__ __device__ inline size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
 
 // Device-resident description of a planned batch (arrays owned by the handle).
 struct Plan {
@@ -259,6 +263,119 @@ __device__ __forceinline__ int find_problem(const int64_t *__restrict__ pref, in
         else hi = mid;
     }
     return lo;
+}
+
+// Doubles ordered as their keys are ordered (as unsigned integers): negative values bit-inverted, the others with the
+// sign bit set.  -0.0 sorts just below +0.0; equal values have equal keys.
+__device__ __forceinline__ unsigned long long order_key(double v) {
+    const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+
+__device__ __forceinline__ double key_value(unsigned long long k) {
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+
+// The same-speaker LLR of two speakers i, j (DESIGN.md section 5.15) with the statistics n, e, b of vbx_link_batch and
+// c = Fa / Fb: cm = c (n_i + n_j), and over the features r = 0 .. R-1 in order
+//   den = fma(cm, Phi_r, 1),  x = b_i,r + b_j,r,  q += x x / den,  prod *= den,
+// with lg += log(prod) (and prod = 1) after every kLogGroup-th feature and after the last, then
+//   LLR = 1/2 ((q - lg) - (e_i + e_j)),  0 when either speaker has no x-vectors.
+// The link, enrolment, cohort and verification kernels all score with llr_step, llr_finish and pair_llr, so they give
+// the same bits for the same pair whatever the order in which their staging delivers the operands.
+constexpr int kLogGroup = 8;
+
+// The log term sum_r log(fma(cm, Phi_r, 1)) of a pair whose sum of group logs came out +inf: some product of kLogGroup
+// denominators overflowed (each denominator is finite, but any finite positive Fa / Fb is accepted, so c can be large).
+// The same groups in the same order, each multiply that would overflow first flushing the product so far into the sum;
+// a group that did not overflow gives the same log as llr_step.  Out of line and reached only from that case, so the
+// scoring loops' registers and instructions stay those of plain groups.
+static __device__ __noinline__ double overflowed_log_sum(double cm, const float *__restrict__ Phi, int R) {
+    double lg = 0.0, prod = 1.0;
+    for (int r = 0; r < R; ++r) {
+        const double den = fma(cm, (double)Phi[r], 1.0), pd = prod * den;
+        if (pd > DBL_MAX) {
+            lg += log(prod);
+            prod = den;
+        } else {
+            prod = pd;
+        }
+        if ((r % kLogGroup) == kLogGroup - 1 || r == R - 1) {
+            lg += log(prod);
+            prod = 1.0;
+        }
+    }
+    return lg;
+}
+
+// Feature r (of R) of U pairs at once, with p = Phi_r and x(u) = b_i,r + b_j,r of pair u.  The group test is one branch
+// for all U pairs.
+template <int U, class X>
+__device__ __forceinline__ void llr_step(double *q, double *lg, double *prod, const double *cm, double p, X x, int r,
+                                         int R) {
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+        const double den = fma(cm[u], p, 1.0), xu = x(u);
+        q[u] += xu * xu / den;
+        prod[u] *= den;
+    }
+    if ((r % kLogGroup) == kLogGroup - 1 || r == R - 1) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+            lg[u] += log(prod[u]);
+            prod[u] = 1.0;
+        }
+    }
+}
+
+// After the last feature: a sum of group logs of +inf is recomputed by overflowed_log_sum.
+template <int U>
+__device__ __forceinline__ void llr_finish(double *lg, const double *cm, const float *__restrict__ Phi, int R) {
+#pragma unroll
+    for (int u = 0; u < U; ++u)
+        if (lg[u] > DBL_MAX) lg[u] = overflowed_log_sum(cm[u], Phi, R);
+}
+
+// The feature sums of a 32 x 32 tile of pairs for link_score_kernel and enroll_score_kernel: 256 threads, thread
+// (tx, ty) = (threadIdx.x & 31, threadIdx.x >> 5) taking the 4 pairs (row i0 + ty + 8u, column j0 + tx), u = 0 .. 3.
+// The b rows of the 32 rows (bi [M_i, kMaxR]) and the 32 columns (bj [M_j, kMaxR]) and Phi pass through the kernel's
+// shared arrays a, bt and ph in chunks of 32 features; rows and columns past M_i, M_j read as 0.  q, lg and prod are
+// the pairs' accumulators.
+__device__ __forceinline__ void tile_llr_sums(double (&a)[32][33], double (&bt)[32][33], double (&ph)[32],
+                                              const double *bi, int64_t M_i, const double *bj, int64_t M_j,
+                                              const float *__restrict__ Phi, int R, int64_t i0, int64_t j0,
+                                              const double (&cm)[4], double (&q)[4], double (&lg)[4],
+                                              double (&prod)[4]) {
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    for (int r0 = 0; r0 < R; r0 += 32) {
+        for (int v = ty; v < 32; v += 8) {
+            const int r = r0 + tx;
+            a[v][tx] = (i0 + v < M_i && r < R) ? bi[(i0 + v) * kMaxR + r] : 0.0;
+            bt[v][tx] = (j0 + v < M_j && r < R) ? bj[(j0 + v) * kMaxR + r] : 0.0;
+        }
+        if (ty == 0) ph[tx] = r0 + tx < R ? (double)Phi[r0 + tx] : 0.0;
+        __syncthreads();
+        const int len = min(32, R - r0);
+        for (int k = 0; k < len; ++k) {
+            const double bj_k = bt[tx][k];
+            llr_step<4>(q, lg, prod, cm, ph[k], [&](int u) { return a[ty + 8 * u][k] + bj_k; }, r0 + k, R);
+        }
+        __syncthreads();                              // also keeps the next tile's loads behind this tile's reads
+    }
+}
+
+// e_i and e_j are read only for two non-empty speakers.  half = -0.5 gives link's distance -LLR, the same bits as
+// -pair_llr but +0.0 for an empty speaker.
+__device__ __forceinline__ double pair_llr(double q, double lg, double n_i, double n_j, const double &e_i,
+                                           const double &e_j, double half = 0.5) {
+    return (n_i == 0.0 || n_j == 0.0) ? 0.0 : half * ((q - lg) - (e_i + e_j));
+}
+
+// The AS-norm score of an LLR l between i and j, with the cohort means and standard deviations mean_i[i], std_i[i] and
+// mean_j[j], std_j[j] (section 5.17).  The sum commutes, so (i, j) and (j, i) give the same number.
+__device__ __forceinline__ double as_norm(double l, const double *mean_i, const double *std_i, int64_t i,
+                                          const double *mean_j, const double *std_j, int64_t j) {
+    return 0.5 * ((l - mean_i[i]) / std_i[i] + (l - mean_j[j]) / std_j[j]);
 }
 
 #endif  // __CUDACC__

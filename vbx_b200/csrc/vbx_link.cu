@@ -31,13 +31,11 @@ namespace {
 constexpr double kBig = 1.0e30;            // cannot-link distance: finite (scipy and the linkage stop at non-finite ones)
 constexpr int kStatsThreads = 256;
 constexpr int kStatsPhases = kStatsThreads / 32;   // x-vector t = first + k, first + k + 8, ... makes phase k
-constexpr int kLogGroup = 8;               // log of a product of 8 denominators (overflowed_log_sum where one overflows)
 constexpr int64_t kScoreGrid = 1 << 20;    // CTAs of link_score_kernel at most; beyond that they stride over the tiles
 
 struct LinkWs {
     uint8_t *lk;             // the linkage regions (carve() in vbx_ahc.cu), each D [M_g,M_g] first
-    double *n, *e, *b;       // [M], [M], [M,kMaxR]  (M: the speakers of all problems)
-    long long *first, *last; // [M]
+    SpeakerStats s;          // M: the speakers of all problems
     int64_t *offs;           // the problem arrays of LinkProblems
 };
 
@@ -53,31 +51,6 @@ struct LinkProblems {
     const double *c;         // [G] Fa_g / Fb_g
 };
 
-size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
-
-// The log term sum_r log(fma(cm, Phi_r, 1)) of a pair whose sum of group logs came out +inf: some product of
-// kLogGroup denominators overflowed (each denominator is finite, but any finite positive Fa / Fb is accepted, so c can
-// be large).  The same groups in the same order, each multiply that would overflow first flushing the product so far
-// into the sum; a group that did not overflow gives the same log as in the scoring loop.  Out of line and reached only
-// from that case, so the loop's registers and instructions stay those of plain groups.
-__device__ __noinline__ double overflowed_log_sum(double cm, const float *__restrict__ Phi, int R) {
-    double lg = 0.0, prod = 1.0;
-    for (int r = 0; r < R; ++r) {
-        const double den = fma(cm, (double)Phi[r], 1.0), pd = prod * den;
-        if (pd > DBL_MAX) {
-            lg += log(prod);
-            prod = den;
-        } else {
-            prod = pd;
-        }
-        if ((r % kLogGroup) == kLogGroup - 1 || r == R - 1) {
-            lg += log(prod);
-            prod = 1.0;
-        }
-    }
-    return lg;
-}
-
 size_t problem_array_bytes(int64_t G) { return (size_t)(5 * G + 4) * 8; }   // off, lk_off, tile_off, dist_off, c
 
 int64_t score_tiles(int64_t M) {
@@ -91,15 +64,15 @@ LinkWs link_layout(uint8_t *ws, size_t lk_bytes, int64_t M, int64_t G, size_t *t
     size_t o = 0;
     w.lk = ws;
     o += lk_bytes;
-    w.n = reinterpret_cast<double *>(ws + o);
+    w.s.n = reinterpret_cast<double *>(ws + o);
     o += al((size_t)M * 8);
-    w.e = reinterpret_cast<double *>(ws + o);
+    w.s.e = reinterpret_cast<double *>(ws + o);
     o += al((size_t)M * 8);
-    w.b = reinterpret_cast<double *>(ws + o);
+    w.s.b = reinterpret_cast<double *>(ws + o);
     o += al((size_t)M * kMaxR * 8);
-    w.first = reinterpret_cast<long long *>(ws + o);
+    w.s.first = reinterpret_cast<long long *>(ws + o);
     o += al((size_t)M * 8);
-    w.last = reinterpret_cast<long long *>(ws + o);
+    w.s.last = reinterpret_cast<long long *>(ws + o);
     o += al((size_t)M * 8);
     w.offs = reinterpret_cast<int64_t *>(ws + o);
     o += al(problem_array_bytes(G));
@@ -110,8 +83,8 @@ LinkWs link_layout(uint8_t *ws, size_t lk_bytes, int64_t M, int64_t G, size_t *t
 __global__ void link_init_kernel(LinkWs w, LinkProblems p) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < p.M) {
-        w.first[i] = LLONG_MAX;
-        w.last[i] = -1;
+        w.s.first[i] = LLONG_MAX;
+        w.s.last[i] = -1;
     }
 }
 
@@ -122,8 +95,8 @@ __global__ void link_span_kernel(LinkWs w, LinkProblems p, const int32_t *__rest
     const int s = spk[i];
     const int64_t g = i / p.N, t = i - g * p.N, base = p.off[g], M = p.off[g + 1] - base;
     if (s < 0 || s >= M) return;
-    atomicMin(&w.first[base + s], (long long)t);
-    atomicMax(&w.last[base + s], (long long)t);
+    atomicMin(&w.s.first[base + s], (long long)t);
+    atomicMax(&w.s.last[base + s], (long long)t);
 }
 
 // One CTA per speaker over its span first .. last.  Warp k sums phase k of the span sequentially (lane = feature,
@@ -143,7 +116,7 @@ __global__ void __launch_bounds__(kStatsThreads) link_stats_kernel(LinkWs w, Lin
     const double c = p.c[g];
     spk += (int64_t)g * p.N;
     const int k = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long long f = w.first[s], l = w.last[s];
+    const long long f = w.s.first[s], l = w.s.last[s];
     double acc[kMaxR / 32] = {0, 0, 0, 0};
     double m = 0.0;
     if (l >= 0) {
@@ -168,7 +141,7 @@ __global__ void __launch_bounds__(kStatsThreads) link_stats_kernel(LinkWs w, Lin
         for (int q = 0; q < kStatsPhases; ++q) F += part[q][r];
         const double ph = (double)Phi[r];
         const double L = 1.0 + c * n * ph, b = c * sqrt(ph) * F;
-        w.b[(int64_t)s * kMaxR + r] = b;
+        w.s.b[(int64_t)s * kMaxR + r] = b;
         if (F_out) F_out[(int64_t)s * R + r] = F;
         e += b * b / L - log(L);
     }
@@ -178,17 +151,16 @@ __global__ void __launch_bounds__(kStatsThreads) link_stats_kernel(LinkWs w, Lin
     if (threadIdx.x == 0) {
         double tot = 0.0;
         for (int q = 0; q < kStatsThreads / 32; ++q) tot += red[q];
-        w.e[s] = tot;
-        w.n[s] = n;
+        w.s.e[s] = tot;
+        w.s.n[s] = n;
         if (n_out) n_out[s] = n;
     }
 }
 
-// Tile (bi, bj), bj >= bi, of 32 x 32 speaker pairs: 256 threads, 4 pairs each (rows ty, ty + 8, ..), features in chunks
-// of 32 through shared memory.  Every pair sums its features in order r = 0 .. R-1 with operands that commute, so
-// d[i][j] and d[j][i] are the same number; the tile is written row-wise and, through shared memory, column-wise.  The
-// tiles of the upper triangle are numbered row by row (row bi holds tiles - bi of them) and the CTAs stride over them,
-// so the grid stays one-dimensional and within its limit for every M.
+// Tile (bi, bj), bj >= bi, of 32 x 32 speaker pairs (tile_llr_sums).  Every pair sums its features in order
+// r = 0 .. R-1 with operands that commute, so d[i][j] and d[j][i] are the same number; the tile is written row-wise
+// and, through shared memory, column-wise.  The tiles of the upper triangle are numbered row by row (row bi holds
+// tiles - bi of them) and the CTAs stride over them, so the grid stays one-dimensional and within its limit for any M.
 __device__ __forceinline__ void score_tile(const LinkWs &w, const float *__restrict__ Phi,
                                            const int32_t *__restrict__ spk_rec, int64_t M, int R, double c,
                                            double *__restrict__ dist_out, int64_t bi, int64_t bj) {
@@ -197,46 +169,18 @@ __device__ __forceinline__ void score_tile(const LinkWs &w, const float *__restr
     const int64_t i0 = (int64_t)bi * 32, j0 = (int64_t)bj * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
     const int64_t j = j0 + tx;
-    const double nj = j < M ? w.n[j] : 0.0;
+    const double nj = j < M ? w.s.n[j] : 0.0;
     double cm[4], q[4] = {0, 0, 0, 0}, lg[4] = {0, 0, 0, 0}, prod[4] = {1, 1, 1, 1};
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
         const int64_t i = i0 + ty + 8 * u;
-        cm[u] = c * ((i < M ? w.n[i] : 0.0) + nj);
+        cm[u] = c * ((i < M ? w.s.n[i] : 0.0) + nj);
     }
-    for (int r0 = 0; r0 < R; r0 += 32) {
-        for (int v = ty; v < 32; v += 8) {
-            const int r = r0 + tx;
-            a[v][tx] = (i0 + v < M && r < R) ? w.b[(i0 + v) * kMaxR + r] : 0.0;
-            bt[v][tx] = (j0 + v < M && r < R) ? w.b[(j0 + v) * kMaxR + r] : 0.0;
-        }
-        if (ty == 0) ph[tx] = r0 + tx < R ? (double)Phi[r0 + tx] : 0.0;
-        __syncthreads();
-        const int len = min(32, R - r0);
-        for (int k = 0; k < len; ++k) {
-            const double bj_k = bt[tx][k], p = ph[k];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const double den = fma(cm[u], p, 1.0), x = a[ty + 8 * u][k] + bj_k;
-                q[u] += x * x / den;
-                prod[u] *= den;
-            }
-            if (((r0 + k) % kLogGroup) == kLogGroup - 1 || r0 + k == R - 1) {
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    lg[u] += log(prod[u]);
-                    prod[u] = 1.0;
-                }
-            }
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int u = 0; u < 4; ++u)
-        if (lg[u] > DBL_MAX) lg[u] = overflowed_log_sum(cm[u], Phi, R);
+    tile_llr_sums(a, bt, ph, w.s.b, M, w.s.b, M, Phi, R, i0, j0, cm, q, lg, prod);
+    llr_finish<4>(lg, cm, Phi, R);
     double *D = reinterpret_cast<double *>(w.lk);
     const int rj = j < M ? spk_rec[j] : -1;
-    const double ej = j < M ? w.e[j] : 0.0;
+    const double ej = j < M ? w.s.e[j] : 0.0;
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
         const int64_t i = i0 + ty + 8 * u;
@@ -244,8 +188,7 @@ __device__ __forceinline__ void score_tile(const LinkWs &w, const float *__restr
         double d;
         if (i == j) d = 0.0;
         else if (spk_rec[i] == rj) d = kBig;
-        else if (w.n[i] == 0.0 || nj == 0.0) d = 0.0;
-        else d = -0.5 * ((q[u] - lg[u]) - (w.e[i] + ej));
+        else d = pair_llr(q[u], lg[u], w.s.n[i], nj, w.s.e[i], ej, -0.5);
         tile[ty + 8 * u][tx] = d;
         D[i * M + j] = d;
         if (dist_out) dist_out[i * M + j] = d;
@@ -273,9 +216,9 @@ __global__ void __launch_bounds__(256) link_score_kernel(LinkWs w, LinkProblems 
         const int64_t base = p.off[g], M = p.off[g + 1] - base, lt = t - p.tile_off[g];
         LinkWs wg = w;
         wg.lk += p.lk_off[g];
-        wg.n += base;
-        wg.e += base;
-        wg.b += base * kMaxR;
+        wg.s.n += base;
+        wg.s.e += base;
+        wg.s.b += base * kMaxR;
         double *dist = dist_out ? dist_out + p.dist_off[g] : nullptr;
         const int64_t tiles = (M + 31) / 32;
         const double tt = 2.0 * (double)tiles + 1.0;
@@ -378,14 +321,7 @@ int launch_speaker_stats_batch(const float *fea, const float *Phi, const int32_t
                                const int64_t *off, const double *c, int64_t M, const SpeakerStats &s, double *n_out,
                                double *F_out, cudaStream_t st) {
     if (M == 0) return 0;
-    LinkWs w;
-    w.lk = nullptr;
-    w.n = s.n;
-    w.e = s.e;
-    w.b = s.b;
-    w.first = s.first;
-    w.last = s.last;
-    w.offs = nullptr;
+    const LinkWs w{nullptr, s, nullptr};
     LinkProblems p;
     p.G = G;
     p.M = M;

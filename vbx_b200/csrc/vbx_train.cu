@@ -29,8 +29,6 @@ constexpr int kPitch = kTile + 8;         // doubles per shared row: the 8 x 4 f
 constexpr int kThreads = 128;             // 4 warps, 2 x 2 of 32 x 32 outputs
 constexpr int kTargetCtas = 1024;         // tile pairs x splits aimed at (several waves on 132 SMs)
 
-__host__ __device__ size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
-
 int64_t tile_count(int D) { return (D + kTile - 1) / kTile; }
 int64_t pair_count(int D) { const int64_t T = tile_count(D); return T * (T + 1) / 2; }
 

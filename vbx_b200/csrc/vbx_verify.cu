@@ -2,10 +2,10 @@
 // a test item (a speaker's x-vectors, or one x-vector); both sides get the statistics n, F, b, e of section 5.15 through
 // launch_speaker_stats_batch (one problem per side, c = Fa / Fb), and
 //   verify_score_kernel   one warp per 32 trials (i, j): the b rows of the two sides staged through shared memory in
-//                         32-feature chunks with coalesced loads, each lane summing its own trial in order r = 0 .. R-1
-//                         with vbx_link's score_tile operations in the same order, so a trial's LLR is bit-identical to
-//                         the enrolment and cohort LLR of the same pair; with cohort statistics the AS-norm score S of
-//                         norm_scores_kernel's expression (enrolment item = row, test item = column)
+//                         32-feature chunks with coalesced loads, each lane summing its own trial with llr_step and
+//                         pair_llr, so a trial's LLR is bit-identical to the enrolment and cohort LLR of the same pair;
+//                         with cohort statistics norm_scores_kernel's AS-norm score (as_norm; enrolment item = row,
+//                         test item = column)
 // The error rates of a scored list (target / nontarget labels) run on the device in a fixed order, without atomics on
 // floating-point values:
 //   verify_keys_kernel    order-preserving 64-bit keys (-0.0 folded into +0.0), labels as 0 / 1, non-finite scores
@@ -49,38 +49,12 @@ namespace vbx {
 
 namespace {
 
-constexpr int kLogGroup = 8;                // as vbx_link: log of a product of 8 denominators, overflowed_log_sum
 constexpr int kScoreWarps = 2;              // warps per CTA of verify_score_kernel (33.8 KB of staging)
 constexpr int64_t kScoreGrid = 1 << 20;     // CTAs of verify_score_kernel at most; beyond that they stride
 constexpr int kSweepThreads = 256;
 constexpr int kSweepGrid = 1024;            // CTAs per slot of verify_sweep_kernel at most
 constexpr int kCllrThreads = 256;
 constexpr int kCllrCtas = 256;              // the fixed partition of the Cllr sums
-
-__host__ __device__ size_t al(size_t v) { return (v + 255) & ~(size_t)255; }
-
-// As vbx_link: the log term sum_r log(fma(cm, Phi_r, 1)) of a pair whose sum of group logs came out +inf: some product of
-// kLogGroup denominators overflowed (each denominator is finite, but any finite positive Fa / Fb is accepted, so c can
-// be large).  The same groups in the same order, each multiply that would overflow first flushing the product so far
-// into the sum; a group that did not overflow gives the same log as in the scoring loop.  Out of line and reached only
-// from that case, so the loop's registers and instructions stay those of plain groups.
-__device__ __noinline__ double overflowed_log_sum(double cm, const float *__restrict__ Phi, int R) {
-    double lg = 0.0, prod = 1.0;
-    for (int r = 0; r < R; ++r) {
-        const double den = fma(cm, (double)Phi[r], 1.0), pd = prod * den;
-        if (pd > DBL_MAX) {
-            lg += log(prod);
-            prod = den;
-        } else {
-            prod = pd;
-        }
-        if ((r % kLogGroup) == kLogGroup - 1 || r == R - 1) {
-            lg += log(prod);
-            prod = 1.0;
-        }
-    }
-    return lg;
-}
 
 // ---------------------------------------------------------------------------------------------------------------- scores
 
@@ -102,9 +76,8 @@ VerifyScoreWs score_layout(uint8_t *ws, int64_t M_e, int64_t M_t, size_t *total)
 
 // Warp w of the grid takes trials 32 w .. 32 w + 31, lane l trial 32 w + l.  Per chunk of 32 features the warp loads
 // the b rows of its 32 enrolment and 32 test items (row v: lane = feature, 256 contiguous bytes) into its own shared
-// tiles, then each lane runs over the chunk for its trial with score_tile's operations: den = fma(cm, Phi_r, 1),
-// x = b_i + b_j, q += x x / den, prod *= den and lg += log(prod) after every kLogGroup features and the last (an lg of
-// +inf recomputed by overflowed_log_sum).  A trial whose index lies outside its side loads nothing and writes NaN.
+// tiles, then each lane runs llr_step over the chunk for its trial.  A trial whose index lies outside its side loads
+// nothing and writes NaN.
 __global__ void __launch_bounds__(kScoreWarps * 32) verify_score_kernel(
     SpeakerStats En, SpeakerStats Te, int64_t M_e, int64_t M_t, const float *__restrict__ Phi, int R, double c,
     const int32_t *__restrict__ ti, const int32_t *__restrict__ tj, int64_t T, const double *__restrict__ mean_e,
@@ -131,41 +104,23 @@ __global__ void __launch_bounds__(kScoreWarps * 32) verify_score_kernel(
             ph[wl][lane] = r < R ? (double)Phi[r] : 0.0;
             __syncwarp();
             const int len = min(32, R - r0);
-            for (int k = 0; k < len; ++k) {
-                const double p = ph[wl][k];
-                const double den = fma(cm, p, 1.0), x = a[wl][lane][k] + bt[wl][lane][k];
-                q += x * x / den;
-                prod *= den;
-                if (((r0 + k) % kLogGroup) == kLogGroup - 1 || r0 + k == R - 1) {
-                    lg += log(prod);
-                    prod = 1.0;
-                }
-            }
+            for (int k = 0; k < len; ++k)
+                llr_step<1>(&q, &lg, &prod, &cm, ph[wl][k], [&](int) { return a[wl][lane][k] + bt[wl][lane][k]; },
+                            r0 + k, R);
             __syncwarp();                             // the next chunk rewrites the tiles
         }
-        if (lg > DBL_MAX) lg = overflowed_log_sum(cm, Phi, R);
+        llr_finish<1>(&lg, &cm, Phi, R);
         if (t >= T) continue;
         double s = NAN;
         if (ok) {
-            const double l = (ni == 0.0 || nj == 0.0) ? 0.0 : 0.5 * ((q - lg) - (En.e[i] + Te.e[j]));
-            s = mean_e ? 0.5 * ((l - mean_e[i]) / std_e[i] + (l - mean_t[j]) / std_t[j]) : l;
+            const double l = pair_llr(q, lg, ni, nj, En.e[i], Te.e[j]);
+            s = mean_e ? as_norm(l, mean_e, std_e, i, mean_t, std_t, j) : l;
         }
         score_out[t] = s;
     }
 }
 
 // ------------------------------------------------------------------------------------------------------------- metrics
-
-// Doubles ordered as their keys are ordered (as unsigned integers): negative values bit-inverted, the others with the
-// sign bit set (vbx_cohort's order_key), after -0.0 is folded into +0.0 so that the two are one value.
-__device__ __forceinline__ unsigned long long score_key(double v) {
-    const unsigned long long u = (unsigned long long)__double_as_longlong(v == 0.0 ? 0.0 : v);
-    return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
-}
-
-__device__ __forceinline__ double key_score(unsigned long long k) {
-    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
-}
 
 // log(1 + exp(x)) as max(x, 0) + log1p(exp(-|x|))
 __device__ __forceinline__ double softplus(double x) { return __dadd_rn(fmax(x, 0.0), log1p(exp(-fabs(x)))); }
@@ -229,7 +184,7 @@ __global__ void verify_keys_kernel(const double *__restrict__ scores, const uint
     for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < T; t += (int64_t)gridDim.x * blockDim.x) {
         const double v = scores[t];
         bad += isfinite(v) ? 0u : 1u;
-        key[t] = score_key(v);
+        key[t] = order_key(v == 0.0 ? 0.0 : v);   // -0.0 and +0.0: one value
         lab[t] = is_target[t] ? 1 : 0;
     }
     for (int o = 16; o; o >>= 1) bad += __shfl_xor_sync(0xffffffffu, bad, o);
@@ -317,7 +272,7 @@ __global__ void __launch_bounds__(kSweepThreads) verify_sweep_kernel(const unsig
     SweepPart p{INFINITY, eer ? -1ll : (long long)LLONG_MAX, (long long)T};
     for (int64_t s = (int64_t)blockIdx.x * kSweepThreads + threadIdx.x; s <= T; s += (int64_t)gridDim.x * kSweepThreads) {
         if (eer && s < T) {                           // the Cllr term of this trial at its rank within its class
-            const double v = key_score(key[s]);
+            const double v = key_value(key[s]);
             const long long tb = tar[s];
             if (lab[s]) terms[tb] = softplus(-v);
             else terms[cnt.n_tar + (s - tb)] = softplus(v);
@@ -377,7 +332,7 @@ __global__ void verify_final_kernel(const unsigned long long *__restrict__ key, 
     counts_out[0] = cnt.n_tar;
     counts_out[1] = cnt.n_non;
     counts_out[2] = (long long)*nonfinite;
-    auto value = [&](long long s) { return s < T ? key_score(key[s]) : (double)INFINITY; };
+    auto value = [&](long long s) { return s < T ? key_value(key[s]) : (double)INFINITY; };
     // EER: the segment between the last candidate with P_miss < P_fa and the first with P_miss >= P_fa
     long long lo = -1, hi = T;
     for (int b = 0; b < grid_x; ++b) {
@@ -409,7 +364,7 @@ __global__ void verify_final_kernel(const unsigned long long *__restrict__ key, 
         long long l = 0, r = T;
         while (l < r) {
             const long long m = l + (r - l) / 2;
-            if (key_score(key[m]) < theta) l = m + 1;
+            if (key_value(key[m]) < theta) l = m + 1;
             else r = m;
         }
         long long miss, fa;
@@ -490,7 +445,7 @@ __global__ void calibrate_split_kernel(const unsigned long long *__restrict__ ke
     const Counts cnt = class_counts(tar, lab, T);
     for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < T; s += (int64_t)gridDim.x * blockDim.x) {
         const long long tb = tar[s];
-        split[lab[s] ? tb : cnt.n_tar + (s - tb)] = key_score(key[s]);
+        split[lab[s] ? tb : cnt.n_tar + (s - tb)] = key_value(key[s]);
     }
 }
 
