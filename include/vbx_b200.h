@@ -645,6 +645,37 @@ int vbx_stream_commit(vbx_handle_t h, int32_t n, int32_t C, int32_t R, int32_t S
                       float *ctx_fea, int32_t *ctx_lab, int64_t *count, int32_t *K, double *n_hist, double *F_hist,
                       int32_t *labels_out, void *stream);
 
+/* Enrolled speakers in streams (DESIGN.md section 5.29), called after a push's vbx_stream_commit.  The enrolment state
+ * is one more DEVICE array the caller owns beside the stream state: named [slots, S_max] int32, the enrolled speaker
+ * (0 .. E-1) each stream speaker is named by, or -1 (a fresh slot is all -1).  The enrolled speakers' statistics
+ * n_enroll [E], F_enroll [E, R] float64 (DEVICE) are vbx_enroll_batch's n_enroll_out / F_enroll_out.  The candidates
+ * are HOST arrays: n streams with distinct slot [n] in [0, slots), each with cand_off[i+1] - cand_off[i] >= 1 distinct
+ * speakers cand_k [M] in [0, S_max) (M = cand_off[n]), packed in stream order; they should be the stream's unnamed
+ * speakers (named = -1, k < K) that hold rows of the push (not validated: read on the device).  For every candidate:
+ *   n = n_hist[k] + ring rows labelled k, F = F_hist[k] + those rows (oldest first, one sequential float64 sum), and
+ *   b, e of vbx_link_batch with c = Fa / Fb; the LLR against every enrolled speaker (section 5.15's score, the kernel of
+ *   vbx_enroll_batch: bit-identical to its llr for the same statistics); -inf for the enrolled speakers the stream
+ *   has already named a speaker by; then each stream's candidates are assigned one-to-one as vbx_enroll_batch assigns
+ *   a recording's speakers at `threshold`.
+ * Outputs (DEVICE): assign_out [M] int32 the enrolled index or -1; best_llr_out [M] the assigned pair's LLR, or for an
+ * unassigned candidate its largest LLR over the enrolled speakers the stream has not claimed (-inf when it claimed
+ * them all); optional (null: not written) llr_out [M, E] the LLRs before the claimed ones are masked, n_out [M],
+ * F_out [M, R].  Then named[slot, k] = assign for every assigned candidate and, with prior = 1, n_hist[slot, k] +=
+ * n_enroll[a], F_hist[slot, k] += F_enroll[a].  A stream's results do not depend on the rest of the batch.
+ * workspace: vbx_stream_enroll_workspace_bytes(n, M, E, max_k) bytes, max_k >= the largest candidate count of a
+ * stream, 256-byte aligned.  Stream ordered, no allocation, no host synchronisation beyond one copy of the candidate
+ * lists from pageable host memory.  VBX_ERR_ARG: a null pointer, sizes as vbx_stream_commit's, slots < n, E < 1,
+ * |threshold| > 1e15, Fa / Fb not finite and >= 0, prior not 0 / 1, candidate lists as above violated, a misaligned or
+ * short workspace. */
+int vbx_stream_enroll_workspace_bytes(vbx_handle_t h, int32_t n, int64_t M, int64_t E, int32_t max_k,
+                                      size_t *bytes_out);
+int vbx_stream_enroll(vbx_handle_t h, int32_t n, int32_t slots, int32_t C, int32_t R, int32_t S_max,
+                      const int32_t *slot, const int64_t *cand_off, const int32_t *cand_k, const float *Phi, double Fa,
+                      double Fb, const float *ctx_fea, const int32_t *ctx_lab, const int64_t *count, double *n_hist,
+                      double *F_hist, int32_t *named, const double *n_enroll, const double *F_enroll, int64_t E,
+                      double threshold, int32_t prior, void *workspace, size_t workspace_bytes, int32_t *assign_out,
+                      double *best_llr_out, double *llr_out, double *n_out, double *F_out, void *stream);
+
 /* Number of kernels launched by this handle since creation (bench.py reports it as gpu_launches). */
 int64_t vbx_launch_count(vbx_handle_t h);
 

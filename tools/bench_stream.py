@@ -16,6 +16,20 @@
 The card's name, power limit and maximum SM clock are read in the same run.  Prints one JSON line; --out also writes it.
 
     python tools/bench_stream.py --out profiles/h100_stream.json
+
+With --enroll-speakers E1,E2,... it measures enrolled speakers in streams (DESIGN.md section 5.29) instead:
+3. Speed, per E: the streams of 1. (--streams, C = 240, 10 s pushes) run by two StreamDiarizers fed the same blocks,
+   one with E enrolled speakers (20 x-vectors each; the first min(E, 200) are the pool speakers the streams draw from,
+   the rest speakers no stream has), threshold 0, and one without; after the warm-up pushes the two alternate which
+   pushes first.  Per push the wall time of each (medians), the naming step's interval (timing['enroll']), the
+   candidates it scored and their LLR pairs (candidates x E), and a byte model of the statistics kernel.  One more push
+   runs under torch.profiler for the device time of each new kernel.
+4. Quality: the archive of the enrolment tests (8 recordings, 10 pool speakers, 20 held-out x-vectors of each enrolled)
+   streamed with 5 and 10 s blocks (C = 240), with and without enroll_prior, scored by name (collar 0.25) against the
+   reference, beside offline diarize_batch(enroll=[, enroll_prior]) at the same threshold; and the share of stream
+   speakers named at their first push.
+
+    python tools/bench_stream.py --streams 4096 --enroll-speakers 100,1000 --out profiles/h100_stream_enroll.json
 """
 import argparse
 import json
@@ -139,16 +153,160 @@ def quality(x_ref, transform, plda, kw, dev):
     return out
 
 
+ENROLL_KERNELS = ('stream_enroll_stats_kernel', 'enroll_score_kernel', 'stream_enroll_mask_kernel',
+                  'enroll_assign_kernel', 'stream_enroll_apply_kernel')
+
+
+def enrolled_speakers(src, E, dim, seed):
+    """E enrolled speakers of 20 x-vectors: the first min(E, 200) around the pool centres of src, the rest around new
+    centres no stream draws from."""
+    rng = np.random.default_rng(seed)
+    extra = src.mean + 2.0 * src.sd * rng.standard_normal((max(E - len(src.centres), 0), dim))
+    centres = np.concatenate([src.centres, extra.astype(np.float32)])[:E]
+    return {f'e{j:04d}': c + 0.5 * src.sd * rng.standard_normal((20, dim)) for j, c in enumerate(centres)}
+
+
+def stats_bytes(timing, C, R, E):
+    """Bytes stream_enroll_stats_kernel moves at most in one push: per stream with candidates the ring's labels and
+    every ring row (C (R + 1) 4; only the candidates' rows are read), per candidate its history read and its b, e, n
+    written ((R + 1) 8 each way), per enrolled speaker n_e, F_e read and b, e, n written."""
+    return timing['enroll_streams'] * C * (R + 1) * 4 + timing['enroll_candidates'] * (R + 1) * 16 + E * (R + 1) * 16
+
+
+def enroll_speed(n, E, pushes, x_ref, transform, plda, kw, dev):
+    src = Streams(x_ref, n, seed=n)
+    enr = enrolled_speakers(src, E, x_ref.shape[1], seed=E)
+    mk = lambda **e: StreamDiarizer(transform, plda, kw['Fa'], kw['Fb'], kw['loopP'], smoothing=kw['smoothing'],
+                                    context=240, device=dev, **e)
+    sd_e, sd_0 = mk(enroll=enr, enroll_threshold=0.0), mk()
+    for _ in range(240 // H + 1):
+        blk = src.block()
+        sd_e.push(blk)
+        sd_0.push(blk)
+    sd_e.timing = []
+    walls = {'with': [], 'without': []}
+    for i in range(pushes):
+        blk = src.block()
+        for which in (('with', 'without') if i % 2 == 0 else ('without', 'with')):
+            sd = sd_e if which == 'with' else sd_0
+            t0 = time.perf_counter()
+            sd.push(blk)
+            walls[which].append(time.perf_counter() - t0)
+    T = sd_e.timing
+    blk = src.block()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        sd_e.push(blk)
+        torch.cuda.synchronize(dev)
+    dev_us = {}
+    for ev in prof.key_averages():
+        for k in ENROLL_KERNELS:
+            if k in ev.key:
+                dev_us[k] = dev_us.get(k, 0.0) + ev.device_time_total
+    med = lambda v: float(np.median(v))
+    cand = med([t['enroll_candidates'] for t in T])
+    sb = med([stats_bytes(t, 240, sd_e.R, E) for t in T])
+    stats_ms = dev_us.get('stream_enroll_stats_kernel', float('nan')) * 1e-3
+    named = [len(st.names) for st in sd_e.streams.values()]
+    return dict(streams=n, enrolled=E, block_xvectors=H, context=240, pushes_timed=pushes,
+                wall_ms_with=round(med(walls['with']) * 1e3, 2), wall_ms_without=round(med(walls['without']) * 1e3, 2),
+                wall_ms_added=round((med(walls['with']) - med(walls['without'])) * 1e3, 2),
+                enroll_step_ms=round(med([t['enroll'] for t in T]) * 1e3, 3),
+                candidates_per_push=cand, streams_with_candidates=med([t['enroll_streams'] for t in T]),
+                llr_pairs_per_push=int(cand * E),
+                kernel_ms_profiled_push={k: round(v * 1e-3, 4) for k, v in dev_us.items()},
+                stats_bytes_bound=int(sb), stats_kernel_GBps_bound=round(sb / (stats_ms * 1e-3) / 1e9, 1),
+                named_speakers_mean=round(float(np.mean(named)), 2))
+
+
+def sessions(x_es, seed=13, n_rec=8, pool=10):
+    """The multi-session archive of the enrolment tests: pool speakers at 2 sd around ES2005a's mean x-vector, 2 .. 5
+    per recording with sticky turns, reference rows naming them p<index>, and 20 held-out x-vectors of each."""
+    rng = np.random.default_rng(seed)
+    sd = x_es.std(0)
+    centres = x_es.mean(0) + 2.0 * sd * rng.standard_normal((pool, x_es.shape[1]))
+    recs, rows = {}, []
+    for r in range(n_rec):
+        T = int(rng.integers(300, 601))
+        who = rng.choice(pool, 2 + r % 4, replace=False)
+        spk = np.zeros(T, dtype=np.int64)
+        for t in range(1, T):
+            spk[t] = spk[t - 1] if rng.random() < 0.97 else rng.integers(len(who))
+        x = centres[who[spk]] + 0.5 * sd * rng.standard_normal((T, x_es.shape[1]))
+        seg = np.stack([np.arange(T) * 0.24, np.arange(T) * 0.24 + 1.5], 1)
+        name = f'ses{r:02d}'
+        recs[name] = (x, seg)
+        rows += [(name, round(t * 0.24, 2), 0.24, f'p{k}') for t, k in enumerate(who[spk])]
+    held = {f'p{k}': centres[k] + 0.5 * sd * rng.standard_normal((20, x_es.shape[1])) for k in range(pool)}
+    return recs, rows, held
+
+
+def enroll_quality(x_ref, transform, plda, kw, dev, threshold=0.0):
+    recs, rows, held = sessions(x_ref)
+    opts = dict(threshold=-0.015, max_iters=40, epsilon=1e-6)
+    turns = lambda lines: [(l.split()[1], float(l.split()[3]), float(l.split()[4]), l.split()[7]) for l in lines]
+    der = lambda sys_rows: round(100 * score.score_rttm(rows, sys_rows, 0.25, False, by_name=True)[1]['by_name']['der'], 2)
+    out = dict(threshold=threshold, offline=[], streamed=[])
+    for prior in (False, True):
+        off = pipeline.diarize_batch(recs, transform, plda, kw['Fa'], kw['Fb'], kw['loopP'], smoothing=kw['smoothing'],
+                                     init='AHC+VB', enroll=held, enroll_threshold=threshold, enroll_prior=prior, **opts)
+        out['offline'].append(dict(enroll_prior=prior,
+                                   der_by_name=der([r for n in recs for r in turns(off[n]['rttm_named'])])))
+    for B in (5.0, 10.0):
+        for prior in (False, True):
+            sd = StreamDiarizer(transform, plda, kw['Fa'], kw['Fb'], kw['loopP'], smoothing=kw['smoothing'], context=240,
+                                device=dev, enroll=held, enroll_threshold=threshold, enroll_prior=prior, **opts)
+            first, at_first = {}, 0
+            for push in block_schedule(recs, B):
+                if not push:
+                    continue
+                got = sd.push({n: (recs[n][0][r], recs[n][1][r]) for n, r in push.items()})
+                for n, res in got.items():
+                    for k in np.unique(res['labels']).tolist():
+                        if (n, k) not in first:
+                            first[(n, k)] = True
+                            at_first += k in res['named']
+            named = sum(len(st.names) for st in sd.streams.values())
+            out['streamed'].append(dict(block_seconds=B, enroll_prior=prior,
+                                        der_by_name=der([r for n in recs for r in turns(sd.rttm(n))]),
+                                        speakers=len(first), named=named, named_at_first_push=at_first,
+                                        share_named_at_first_push=round(at_first / max(len(first), 1), 4)))
+    return out
+
+
+def enroll_main(args, x_ref, transform, plda, kw, dev):
+    runs = []
+    for n in (int(v) for v in args.streams.split(',')):
+        for E in (int(v) for v in args.enroll_speakers.split(',')):
+            runs.append(enroll_speed(n, E, args.pushes, x_ref, transform, plda, kw, dev))
+            print(json.dumps(runs[-1]), file=sys.stderr)
+            torch.cuda.empty_cache()
+    q = enroll_quality(x_ref, transform, plda, kw, dev)
+    print(json.dumps(q), file=sys.stderr)
+    smi = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'],
+                         capture_output=True, text=True).stdout.strip().splitlines()
+    line = dict(gpu=smi[0] if smi else torch.cuda.get_device_name(0), speed=runs, quality=q)
+    s = json.dumps(line)
+    print(s)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, 'w') as f:
+            f.write(s + '\n')
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--streams', default='1024,4096')
     ap.add_argument('--pushes', type=int, default=10)
+    ap.add_argument('--enroll-speakers', default=None,
+                    help='E1,E2,...: measure enrolled speakers in streams (DESIGN.md section 5.29) instead')
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit('bench_stream.py needs a CUDA device')
     dev = torch.device('cuda:0')
     x_ref, transform, plda, kw = model()
+    if args.enroll_speakers is not None:
+        return enroll_main(args, x_ref, transform, plda, kw, dev)
     runs = []
     for n in (int(v) for v in args.streams.split(',')):
         runs.append(speed(n, args.pushes, x_ref, transform, plda, kw, dev))

@@ -19,7 +19,8 @@ EXPORTS = ['vbx_version', 'vbx_padded_states', 'vbx_padded_states_wide', 'vbx_cr
            'vbx_init_random', 'vbx_run_prior', 'vbx_run_f64_prior', 'vbx_class_scatter_workspace_bytes',
            'vbx_class_scatter', 'vbx_stream_window', 'vbx_stream_commit', 'vbx_verify_score_workspace_bytes',
            'vbx_verify_score', 'vbx_verify_metrics_workspace_bytes', 'vbx_verify_metrics',
-           'vbx_verify_calibrate_workspace_bytes', 'vbx_verify_calibrate']
+           'vbx_verify_calibrate_workspace_bytes', 'vbx_verify_calibrate', 'vbx_stream_enroll_workspace_bytes',
+           'vbx_stream_enroll']
 
 FLAG_NONFINITE, FLAG_ELBO_DECREASED, FLAG_CONVERGED = 1, 2, 4
 SCORE_BAD_LABEL, SCORE_BAD_REGION, SCORE_BAD_RECORDING = 1, 2, 4      # vbx_score / vbx_score_overlap / vbx_score_jer flags
@@ -143,6 +144,11 @@ def load():
                                       vp, vp, vp, vp, vp, vp]
     lib.vbx_stream_commit.restype = ctypes.c_int
     lib.vbx_stream_commit.argtypes = [vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.vbx_stream_enroll_workspace_bytes.restype = ctypes.c_int
+    lib.vbx_stream_enroll_workspace_bytes.argtypes = [vp, i32, i64, i64, i32, ctypes.POINTER(ctypes.c_size_t)]
+    lib.vbx_stream_enroll.restype = ctypes.c_int
+    lib.vbx_stream_enroll.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, vp, dbl, dbl, vp, vp, vp, vp, vp, vp, vp,
+                                      vp, i64, dbl, i32, vp, ctypes.c_size_t, vp, vp, vp, vp, vp, vp]
     lib.vbx_verify_score_workspace_bytes.restype = ctypes.c_int
     lib.vbx_verify_score_workspace_bytes.argtypes = [vp, i32, i32, ctypes.POINTER(ctypes.c_size_t)]
     lib.vbx_verify_score.restype = ctypes.c_int

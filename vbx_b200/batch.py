@@ -521,6 +521,127 @@ class StreamState:
             getattr(self, name)[int(slot)].zero_()
 
 
+class StreamEnrolment:
+    """Enrolled speakers of the streams of a StreamState (include/vbx_b200.h vbx_stream_enroll, DESIGN.md section 5.29):
+    named [slots, S_max] int32, the enrolled speaker each stream speaker is named by or -1, kept the size of the state's
+    slots by grow() and reset(); and the enrolled speakers' statistics n_enroll [E], F_enroll [E, R] float64 on the
+    state's device (vbx_enroll_batch's n_enroll / F_enroll)."""
+
+    def __init__(self, state, n_enroll, F_enroll):
+        if not isinstance(state, StreamState):
+            raise ValueError('state: expected a StreamState')
+        self.device, self.S_max, self.R = state.device, state.S_max, state.R
+        self.n_enroll = torch.as_tensor(n_enroll, dtype=torch.float64).to(self.device).contiguous()
+        self.F_enroll = torch.as_tensor(F_enroll, dtype=torch.float64).to(self.device).contiguous()
+        self.E = int(self.n_enroll.shape[0]) if self.n_enroll.ndim == 1 else 0
+        if self.E < 1 or tuple(self.F_enroll.shape) != (self.E, self.R):
+            raise ValueError(f'n_enroll [E] and F_enroll [E, {self.R}] with E >= 1 expected')
+        if not (bool(torch.isfinite(self.n_enroll).all()) and bool(torch.isfinite(self.F_enroll).all())
+                and bool((self.n_enroll > 0).all())):
+            raise ValueError('n_enroll must be > 0 and n_enroll, F_enroll finite')
+        self.named = torch.full((0, self.S_max), -1, dtype=torch.int32, device=self.device)
+        self.slots = 0
+        self.grow(state.slots)
+        self.lib = _lib.load()
+        self._h = ctypes.c_void_p()
+        if self.lib.vbx_create(self.device.index, ctypes.byref(self._h)) != 0:
+            raise VbxError('vbx_create failed: no usable sm_90 device')
+
+    def grow(self, slots):
+        """At least `slots` slots, the existing ones kept; new slots unnamed."""
+        if slots <= self.slots:
+            return
+        new = torch.full((int(slots), self.S_max), -1, dtype=torch.int32, device=self.device)
+        new[:self.slots] = self.named
+        self.named, self.slots = new, int(slots)
+
+    def reset(self, slot):
+        """Slot `slot` unnamed, for a new stream."""
+        self.named[int(slot)] = -1
+
+    def close(self):
+        if getattr(self, '_h', None) is not None and self._h.value:
+            self.lib.vbx_destroy(self._h)
+            self._h = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _check(self, rc, what):
+        if rc != 0:
+            msg = self.lib.vbx_last_error(self._h)
+            raise VbxError(f'{what} failed ({rc}): {msg.decode() if msg else "?"}')
+
+    def assign(self, state, slots, candidates, Phi, Fa, Fb, threshold, prior=False, detail=False, out=None):
+        """Name candidates of the streams in `slots` (vbx_stream_enroll): candidates[i] lists the speakers of stream
+        slots[i] to score, each unnamed and below the stream's K (every stream with at least one; distinct speakers).
+        Phi [R] float32 CUDA; Fa, Fb, threshold as vbx_enroll_batch takes them; prior: add the enrolled statistics of
+        every assigned candidate to its history.  Everything is checked on the host first (synchronises).  Returns
+        (assign int32 [M], best_llr, llr [M, E], n [M], F [M, R] float64) CUDA tensors in the packed candidate order,
+        llr, n and F None unless detail; out: None, or those five tensors to write into (implies detail).  named and,
+        with prior, state.n_hist / F_hist are updated."""
+        from .enroll import check_threshold
+        if not (isinstance(state, StreamState) and state.device == self.device and state.S_max == self.S_max
+                and state.R == self.R and state.slots == self.slots):
+            raise ValueError('state: expected the StreamState this enrolment state was made for, grown alike')
+        sl = np.asarray(slots, dtype=np.int64).reshape(-1)
+        n = len(sl)
+        if len(candidates) != n:
+            raise ValueError(f'candidates: expected one list per stream, {n} of them')
+        if len(np.unique(sl)) != n or (n and (sl.min() < 0 or sl.max() >= state.slots)):
+            raise ValueError(f'slots: expected distinct slots in [0, {state.slots})')
+        cand = [np.asarray(c, dtype=np.int64).reshape(-1) for c in candidates]
+        if any(len(c) == 0 or len(np.unique(c)) != len(c) for c in cand):
+            raise ValueError('candidates: every stream needs at least one candidate, all distinct')
+        t = check_threshold(threshold)
+        c = float(Fa) / float(Fb) if float(Fb) != 0 else float('inf')
+        if not (np.isfinite(c) and c >= 0):
+            raise ValueError('Fa / Fb must be finite and >= 0')
+        if not (isinstance(Phi, torch.Tensor) and Phi.device == self.device and Phi.dtype == torch.float32
+                and tuple(Phi.shape) == (self.R,)):
+            raise ValueError(f'Phi: expected a float32 tensor of shape ({self.R},) on {self.device}')
+        Phi = Phi.contiguous()
+        if n:
+            idx = torch.from_numpy(sl).to(self.device)
+            both = torch.cat([state.K[idx, None], self.named[idx]], 1).cpu().numpy()     # one read-back
+            K, named = both[:, 0], both[:, 1:]
+            for i, cl in enumerate(cand):
+                if cl.min() < 0 or cl.max() >= K[i] or np.any(named[i][cl] >= 0):
+                    raise ValueError(f'candidates of slot {int(sl[i])}: every speaker must be unnamed and lie in '
+                                     f'[0, {int(K[i])})')
+        off = np.concatenate([[0], np.cumsum([len(c) for c in cand])]).astype(np.int64)
+        M = int(off[-1])
+        f64 = torch.float64
+        specs = [((M,), torch.int32), ((M,), f64), ((M, self.E), f64), ((M,), f64), ((M, self.R), f64)]
+        if out is None:
+            out = [torch.empty(shape, dtype=dt, device=self.device) if detail or j < 2 else None
+                   for j, (shape, dt) in enumerate(specs)]
+        elif len(out) != 5 or any(not (isinstance(o, torch.Tensor) and o.device == self.device and o.dtype == dt
+                                       and o.is_contiguous() and tuple(o.shape) == shape) for o, (shape, dt) in zip(out, specs)):
+            raise ValueError('out: expected five contiguous tensors (assign, best_llr, llr, n, F) of the packed shapes')
+        if n == 0:
+            return tuple(out)
+        slot_h = np.ascontiguousarray(sl, dtype=np.int32)
+        k_h = np.ascontiguousarray(np.concatenate(cand), dtype=np.int32)
+        v = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+        need = ctypes.c_size_t()
+        max_k = int(np.diff(off).max())
+        self._check(self.lib.vbx_stream_enroll_workspace_bytes(self._h, n, M, self.E, max_k, ctypes.byref(need)),
+                    'vbx_stream_enroll_workspace_bytes')
+        with torch.cuda.device(self.device):
+            ws = torch.empty(max(int(need.value), 1), dtype=torch.uint8, device=self.device)
+            stream = ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+            self._check(self.lib.vbx_stream_enroll(
+                self._h, n, state.slots, state.C, self.R, self.S_max, v(slot_h), v(off), v(k_h), _ptr(Phi), float(Fa),
+                float(Fb), _ptr(state.ctx_fea), _ptr(state.ctx_lab), _ptr(state.count), _ptr(state.n_hist),
+                _ptr(state.F_hist), _ptr(self.named), _ptr(self.n_enroll), _ptr(self.F_enroll), self.E, t, int(bool(prior)),
+                _ptr(ws), ws.numel(), *map(_ptr, out), stream), 'vbx_stream_enroll')
+        return tuple(out)
+
+
 def check_prior(prior, B, S, R, device):
     """The enrolment prior of run() / run_f64() checked on the host (ValueError): a pair (n [B,S], F [B,S,R]) of float64
     tensors on `device`, finite, n >= 0.  Returns the pair contiguous."""

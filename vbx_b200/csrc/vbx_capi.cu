@@ -1525,6 +1525,81 @@ int vbx_stream_commit(vbx_handle_t h, int32_t n, int32_t C, int32_t R, int32_t S
                    "stream_commit");
 }
 
+// The candidate lists of vbx_stream_enroll: n streams with distinct slots in [0, slots), cand_off from 0 with 1 .. S_max
+// candidates per stream, each a distinct speaker in [0, S_max).  *max_k gets the largest candidate count.
+static int check_stream_candidates(vbx_handle_t h, const std::string &who, int32_t n, int32_t slots, int32_t S_max,
+                                   const int32_t *slot, const int64_t *cand_off, const int32_t *cand_k, int64_t *max_k) {
+    *max_k = 0;
+    if (n == 0) return VBX_OK;
+    if (!slot || !cand_off || !cand_k) return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    if (cand_off[0] != 0) return fail(h, VBX_ERR_ARG, who + ": cand_off[0] must be 0");
+    std::vector<uint8_t> seen_slot((size_t)slots, 0);
+    std::vector<uint8_t> seen_k((size_t)S_max, 0);
+    for (int32_t i = 0; i < n; ++i) {
+        if (slot[i] < 0 || slot[i] >= slots || seen_slot[slot[i]])
+            return fail(h, VBX_ERR_ARG, who + ": slots must be distinct and lie in [0, slots)");
+        seen_slot[slot[i]] = 1;
+        const int64_t k = cand_off[i + 1] - cand_off[i];
+        if (k < 1 || k > S_max)
+            return fail(h, VBX_ERR_ARG, who + ": every stream needs 1 .. S_max candidates (cand_off)");
+        *max_k = std::max(*max_k, k);
+        std::fill(seen_k.begin(), seen_k.end(), 0);
+        for (int64_t m = cand_off[i]; m < cand_off[i + 1]; ++m) {
+            if (cand_k[m] < 0 || cand_k[m] >= S_max || seen_k[cand_k[m]])
+                return fail(h, VBX_ERR_ARG, who + ": a stream's candidates must be distinct speakers in [0, S_max)");
+            seen_k[cand_k[m]] = 1;
+        }
+    }
+    return VBX_OK;
+}
+
+int vbx_stream_enroll_workspace_bytes(vbx_handle_t h, int32_t n, int64_t M, int64_t E, int32_t max_k,
+                                      size_t *bytes_out) {
+    if (!h || !bytes_out) return VBX_ERR_ARG;
+    if (n < 0 || M < n || E < 1 || max_k < 0 || max_k > 128 || (int64_t)max_k * n < M)
+        return fail(h, VBX_ERR_ARG, "vbx_stream_enroll_workspace_bytes: need 0 <= n <= M <= n max_k, E >= 1 and "
+                                    "max_k in [0, 128]");
+    *bytes_out = vbx::stream_enroll_workspace_bytes(n, M, E, max_k, h->sms);
+    return VBX_OK;
+}
+
+int vbx_stream_enroll(vbx_handle_t h, int32_t n, int32_t slots, int32_t C, int32_t R, int32_t S_max,
+                      const int32_t *slot, const int64_t *cand_off, const int32_t *cand_k, const float *Phi, double Fa,
+                      double Fb, const float *ctx_fea, const int32_t *ctx_lab, const int64_t *count, double *n_hist,
+                      double *F_hist, int32_t *named, const double *n_enroll, const double *F_enroll, int64_t E,
+                      double threshold, int32_t prior, void *workspace, size_t workspace_bytes, int32_t *assign_out,
+                      double *best_llr_out, double *llr_out, double *n_out, double *F_out, void *stream) {
+    if (!h) return VBX_ERR_ARG;
+    Range nvtx_range("vbx_stream_enroll");
+    const std::string who("vbx_stream_enroll");
+    int rc = check_stream_sizes(h, who, n, C, R, S_max, S_max);
+    if (rc != VBX_OK) return rc;
+    if (slots < n) return fail(h, VBX_ERR_ARG, who + ": slots < n");
+    if (E < 1) return fail(h, VBX_ERR_ARG, who + ": E must be >= 1");
+    if (prior != 0 && prior != 1) return fail(h, VBX_ERR_ARG, who + ": prior must be 0 or 1");
+    if (!(std::fabs(threshold) <= 1e15)) return fail(h, VBX_ERR_ARG, who + ": |threshold| must be <= 1e15");
+    const double c = Fa / Fb;
+    if (!(c >= 0.0) || c == INFINITY) return fail(h, VBX_ERR_ARG, who + ": Fa / Fb must be finite and >= 0");
+    int64_t max_k = 0;
+    rc = check_stream_candidates(h, who, n, slots, S_max, slot, cand_off, cand_k, &max_k);
+    if (rc != VBX_OK) return rc;
+    if (n == 0) return VBX_OK;
+    if (!Phi || (C > 0 && (!ctx_fea || !ctx_lab)) || !count || !n_hist || !F_hist || !named || !n_enroll ||
+        !F_enroll || !workspace || !assign_out || !best_llr_out)
+        return fail(h, VBX_ERR_ARG, who + ": null pointer");
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255) != 0)
+        return fail(h, VBX_ERR_ARG, who + ": workspace must be 256-byte aligned");
+    if (workspace_bytes < vbx::stream_enroll_workspace_bytes(n, cand_off[n], E, max_k, h->sms))
+        return fail(h, VBX_ERR_ARG, who + ": workspace smaller than vbx_stream_enroll_workspace_bytes()");
+    DeviceGuard guard(h->device);
+    if (guard.err != cudaSuccess) return cuda_fail(h, guard.err, "cudaSetDevice");
+    return counted(h, vbx::launch_stream_enroll(n, C, R, S_max, slot, cand_off, cand_k, Phi, c, ctx_fea, ctx_lab, count,
+                                                n_hist, F_hist, named, n_enroll, F_enroll, E, threshold, prior,
+                                                workspace, h->sms, assign_out, best_llr_out, llr_out, n_out, F_out,
+                                                (cudaStream_t)stream),
+                   "stream_enroll");
+}
+
 int vbx_attach_comm(vbx_handle_t h, void *nccl_comm, int32_t n_ranks, const char *libnccl_path) {
     if (!h) return VBX_ERR_ARG;
     if (!nccl_comm) {   // detach

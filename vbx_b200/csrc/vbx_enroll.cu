@@ -302,6 +302,25 @@ int launch_cohort_scores_batch(const SpeakerStats &a, const SpeakerStats &co, co
     return cudaGetLastError() == cudaSuccess ? 1 : -1;
 }
 
+size_t enroll_assign_workspace_bytes(int64_t E, int64_t max_k, int64_t n_recs, int sms) {
+    size_t slice = 0;
+    slice_at(nullptr, E + max_k, max_k, &slice);
+    return slice * (size_t)std::min<int64_t>((int64_t)kAssignCtasPerSm * std::max(sms, 1), std::max<int64_t>(n_recs, 1));
+}
+
+int launch_enroll_assign(const double *llr, const int64_t *recs, int64_t n_recs, int64_t E, int64_t max_k,
+                         const double *threshold, void *slices, int sms, int32_t *assign_out, double *best_llr_out,
+                         cudaStream_t st) {
+    if (n_recs == 0) return 0;
+    size_t slice = 0;
+    slice_at(nullptr, E + max_k, max_k, &slice);
+    const int64_t ctas = std::min<int64_t>((int64_t)kAssignCtasPerSm * std::max(sms, 1), n_recs);
+    enroll_assign_kernel<<<(unsigned)ctas, kAssignThreads, 0, st>>>(llr, recs, n_recs, E,
+                                                                    reinterpret_cast<uint8_t *>(slices), slice, max_k,
+                                                                    assign_out, best_llr_out, threshold, 1, 0);
+    return cudaGetLastError() == cudaSuccess ? 1 : -1;
+}
+
 int launch_repeat_index(const int32_t *src, int64_t n, int G, int32_t *dst, cudaStream_t st) {
     const int64_t total = (int64_t)G * n;
     if (total == 0) return 0;

@@ -364,6 +364,15 @@ __device__ __forceinline__ void tile_llr_sums(double (&a)[32][33], double (&bt)[
     }
 }
 
+// Feature r of a speaker's statistics (section 5.15): with n x-vectors and feature sum F_r, L_r = 1 + c n Phi_r and
+// b_r = c sqrt(Phi_r) F_r; speaker_e_term is feature r's term b_r^2 / L_r - log L_r of e.  link_stats_kernel and the
+// stream enrolment's statistics both take b and e from here.
+__device__ __forceinline__ void speaker_L_b(double c, double n, double ph, double F, double &L, double &b) {
+    L = 1.0 + c * n * ph;
+    b = c * sqrt(ph) * F;
+}
+__device__ __forceinline__ double speaker_e_term(double L, double b) { return b * b / L - log(L); }
+
 // e_i and e_j are read only for two non-empty speakers.  half = -0.5 gives link's distance -LLR, the same bits as
 // -pair_llr but +0.0 for an empty speaker.
 __device__ __forceinline__ double pair_llr(double q, double lg, double n_i, double n_j, const double &e_i,
@@ -516,6 +525,13 @@ struct NormProblems {
 int launch_cohort_scores_batch(const SpeakerStats &a, const SpeakerStats &co, const float *Phi, int G,
                                const int64_t *off, const int64_t *tile_off, const double *c, int64_t n_tiles, int64_t C,
                                int R, double *llr, double *llr_out, cudaStream_t st);
+// enroll_assign_kernel at one threshold (DEVICE [1]) over n_recs items whose speakers are rows recs[i] .. recs[i+1]-1
+// of llr [*, E] (recs DEVICE [n_recs + 1], at most max_k speakers each); slices: enroll_assign_workspace_bytes bytes.
+// Returns 1, 0 for n_recs == 0.
+size_t enroll_assign_workspace_bytes(int64_t E, int64_t max_k, int64_t n_recs, int sms);
+int launch_enroll_assign(const double *llr, const int64_t *recs, int64_t n_recs, int64_t E, int64_t max_k,
+                         const double *threshold, void *slices, int sms, int32_t *assign_out, double *best_llr_out,
+                         cudaStream_t st);
 // score tiles of an M x C rectangle (host)
 int64_t rect_tiles(int64_t M, int64_t C);
 // dst [G, n] = G copies of src [n] (DEVICE)
@@ -583,5 +599,13 @@ int launch_stream_commit(int n, int C, int R, int S_max, const int32_t *slot, co
                          const int64_t *win_off, const float *blk_fea, const int32_t *first, float *ctx_fea,
                          int32_t *ctx_lab, int64_t *count, int32_t *K, double *n_hist, double *F_hist,
                          int32_t *labels_out, cudaStream_t st);
+// enrolled speakers in streams (vbx_stream.cu, section 5.29): slot_host [n], cand_off_host [n+1], cand_k_host [M] HOST
+size_t stream_enroll_workspace_bytes(int n, int64_t M, int64_t E, int64_t max_k, int sms);
+int launch_stream_enroll(int n, int C, int R, int S_max, const int32_t *slot_host, const int64_t *cand_off_host,
+                         const int32_t *cand_k_host, const float *Phi, double c, const float *ctx_fea,
+                         const int32_t *ctx_lab, const int64_t *count, double *n_hist, double *F_hist, int32_t *named,
+                         const double *n_enroll, const double *F_enroll, int64_t E, double threshold, int prior,
+                         void *workspace, int sms, int32_t *assign_out, double *best_llr_out, double *llr_out,
+                         double *n_out, double *F_out, cudaStream_t st);
 
 }  // namespace vbx

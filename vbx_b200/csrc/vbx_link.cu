@@ -139,11 +139,11 @@ __global__ void __launch_bounds__(kStatsThreads) link_stats_kernel(LinkWs w, Lin
     for (int r = threadIdx.x; r < R; r += kStatsThreads) {
         double F = 0.0;
         for (int q = 0; q < kStatsPhases; ++q) F += part[q][r];
-        const double ph = (double)Phi[r];
-        const double L = 1.0 + c * n * ph, b = c * sqrt(ph) * F;
+        double L, b;
+        speaker_L_b(c, n, (double)Phi[r], F, L, b);
         w.s.b[(int64_t)s * kMaxR + r] = b;
         if (F_out) F_out[(int64_t)s * R + r] = F;
-        e += b * b / L - log(L);
+        e += speaker_e_term(L, b);
     }
     for (int o = 16; o; o >>= 1) e += __shfl_xor_sync(0xffffffffu, e, o);   // fixed butterfly, then warps in order
     if (lane == 0) red[k] = e;
