@@ -1,5 +1,5 @@
 """Representative runs for compute-sanitizer (memcheck / racecheck / synccheck / initcheck): wgmma projection at
-D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule), state counts
+D = 32 ... 2048 and x-vector chain (Dx = 256, 512), batches holding recordings without frames, fused and split forward-backward, chunked scan, the float64 finishing phase (stop rule, also with the enrolment prior at S = 4 and 128), state counts
 6..128 (both contraction modes at S = 128), per-recording state masks, AHC, hard labels (also under a speaker-count bound),
 the dense forward_backward(), the ELBO trace, DER / JER scoring, speaker linking across recordings (one problem and
 batched), enrolment
@@ -72,6 +72,38 @@ for gm in (0, 1):
     run([513, 512, 1, 2, 300], 128, 2, ns=[128, 100, 65, 3, 1], gemm=gm, tag=f'S=128 masks gemm={gm}')
     run([4100, 0, 300], 100, 2, D=256, gemm=gm, tag=f'S=128 long + empty gemm={gm}')
     run([300, 120, 64], 100, 30, eps=1e-5, gemm=gm, tag=f'S=128 stop rule, float64 finish gemm={gm}')
+# the float64 finishing round with the enrolment prior at S = 4 and S = 128: empty recordings, T = 1 and 65 (a partial
+# 64-frame block), 513 (a partial M-tile); states 0 and 2 enrolled from the recording's own frames, recording 1 without a
+# prior.  epsilon is placed from a float32-only run (epsilon = -inf) so that recording 3 hands over at iteration 1: its
+# Li[0] is then redone in float64 and differs from the float32 value.
+for S_, fb_ in ((4, 2), (100, 1)):
+    p_lens = [0, 513, 1, 65, 0, 300]
+    p_vb = VbxBatch(p_lens, 128, S_, device=dev, fb_split=fb_)
+    p_d = synth.make_batch([t for t in p_lens if t], R=128, S=S_, seed=5, dtype=np.float32)
+    p_off = np.concatenate([[0], np.cumsum(p_lens)])
+    p_n = np.zeros((len(p_lens), p_vb.S))
+    p_F = np.zeros((len(p_lens), p_vb.S, 128))
+    for b in (2, 3, 5):
+        fb = p_d['fea'][p_off[b]:p_off[b + 1]].astype(np.float64)
+        p_n[b, 0], p_n[b, 2] = 40.0, 3.0
+        p_F[b, 0], p_F[b, 2] = 40.0 * fb.mean(0), fb[:1].sum(0) * 3.0
+    p_prior = (torch.from_numpy(p_n).to(dev), torch.from_numpy(p_F).to(dev))
+    p_vb.prepare_scale(torch.from_numpy(p_d['fea']).to(dev), torch.from_numpy(p_d['Phi']).to(dev))
+
+    def p_run(eps):
+        g = torch.zeros((p_vb.N, p_vb.S), device=dev)
+        g[:, :S_] = torch.from_numpy(p_d['gamma0']).to(dev)
+        p = torch.zeros((len(p_lens), p_vb.S), device=dev)
+        p[:, :S_] = 1.0 / S_
+        o = p_vb.run(g, p, Fa=0.3, Fb=17.0, loopProb=0.99, maxIters=30, epsilon=eps, return_model=True, prior=p_prior)
+        return o['Li'].cpu().numpy(), o['n_iters'].cpu().numpy()
+
+    li32, _ = p_run(-float('inf'))
+    p_eps = float(li32[3, 1] - li32[3, 0] - 4.0 * 2.0 ** -24 * abs(li32[3, 1]))      # d_1 - 2 nb_1
+    li, n_it = p_run(p_eps)
+    p_vb.close()
+    assert li[3, 0] != li32[3, 0], 'recording 3 did not reach the float64 finishing round'
+    print('float64 finish with prior ok', S_, n_it.tolist())
 # per-recording Fa / Fb / loopP on every schedule, with the float64 finish
 run([300, 45, 1, 129, 600], 16, 30, fb_split=1, eps=1e-5, per_rec=True, tag='per-recording split')
 run([300, 45, 1, 129, 600], 16, 30, fb_split=2, eps=1e-5, per_rec=True, tag='per-recording fused')

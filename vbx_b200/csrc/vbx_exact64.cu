@@ -7,9 +7,11 @@
 // SWITCHES: iterations k-1 and k are discarded, the state that entered iteration k-1 is restored (gamma and pi are
 // snapshotted at the start of every float32 iteration, two deep), and the remaining iterations -- beginning with
 // k-1, so that the test of iteration k already compares two float64 values -- are evaluated by the kernels of this
-// file: every quantity in float64 (inputs: the float32 rho and the float32-stored gamma, both exact in float64),
-// with the reference's test on exact ELBO values.  A switched recording lags one round behind the others.  gamma is stored in float32 between iterations (the output
-// precision); that perturbs the ELBO by < 1e-9 near the fixed point, three orders below epsilon.
+// file: every quantity in float64 (inputs: the float32 rho and the float32-stored gamma and pi, exact in float64),
+// with the reference's test on exact ELBO values.  A switched recording lags one round behind the others.  Two values
+// are stored in float32: gamma between iterations (the output precision) and the normalised forward variables, which
+// fb64 parks in gamma for the backward sweep (their rounding reaches gamma and pi); pi stays float64 across rounds.  That
+// perturbs the ELBO steps by < 1e-9 near the fixed point, three orders below epsilon.
 // Each kernel handles only recordings with ws.active64 != 0; a round of these launches costs a few microseconds
 // when no recording is in this phase.
 //
